@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Headline benchmark: MLP training throughput (samples/s, whole job) on the reference's
 default workload - MLP 784-128-127-126-125-124-123-10, 4 micro-batches, SGD lr 0.006
-(BASELINE.md section 2) - data parallel over N B200s.
+(BASELINE.md section 2) - data parallel over N H100s.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
 
 * ``value``  : device-timed (CUDA events on the engine's stream, barrier + synchronize on
                both sides, MAX over ranks) with every step's inputs copied from a
@@ -14,6 +14,14 @@ default workload - MLP 784-128-127-126-125-124-123-10, 4 micro-batches, SGD lr 0
                global batch = 128 x N.  ``--scaling strong`` keeps the global batch at 128.
 * ``--impl reference`` runs the unmodified reference (NumPy on the host CPUs, mpi4py shim)
                on the same config; N ranks = N processes.
+* ``--dump-outputs DIR``: after the timed steps, what the last step left for its caller - the
+               loss (``loss.npy``, float64) and the updated weight arena of the stage
+               (``weights_stage<k>.npy``, float32, biases included; a fixed seeded sample with its positions
+               in ``weights_stage<k>_idx.npy`` when the arenas exceed 64 MB in all) - so that two builds can
+               be compared output for output.  Inputs and initial weights are seeded: the same arguments
+               give the same inputs on every run.
+* ``--steps K`` sets the steps of one timed block; every measurement (device-timed, e2e, and the
+               informational tf32 run) times ``--repeats`` blocks of K steps and reports the median block.
 """
 from __future__ import annotations
 
@@ -34,7 +42,7 @@ LR = 0.006
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=200, help="steps per timed block (each measurement times --repeats blocks)")
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", choices=["ours", "reference"], default="ours")
     ap.add_argument("--scaling", choices=["weak", "strong"], default="weak")
@@ -55,7 +63,39 @@ def parse():
     ap.add_argument("--repeats", type=int, default=5, help="the K-step block is timed this many times; the MEDIAN block is reported")
     ap.add_argument("--no-exposed", action="store_true", help="skip the compute-only twin run that yields comm.exposed_ms_per_step")
     ap.add_argument("--ref-threads", type=int, default=0, help="reference arm: BLAS threads per rank (0 = calibrate over a sweep)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last step's loss and the updated weights as DIR/<name>.npy after the timed steps")
     return ap.parse_args()
+
+
+DUMP_LIMIT_BYTES = 64 << 20          # all --dump-outputs files together
+
+
+def dump_outputs(out_dir, trainer, loss, grid, limit_bytes=DUMP_LIMIT_BYTES):
+    """The last timed step's results as a caller receives them: its loss (last pipeline stage) and the weights it
+    updated (one file per pipeline stage, written by replica 0).  The files of all stages stay within ``limit_bytes``:
+    a stage whose weight arena does not fit its share is written as a fixed sample - positions drawn with a seeded
+    generator from the arena size alone (``weights_stage<k>_idx.npy``, int64) and the weights there
+    (``weights_stage<k>.npy``) - so two builds sample the same positions."""
+    import numpy as np
+    import torch
+
+    if grid.replica != 0:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    stage = trainer.pp_comm.Get_rank()
+    weights = trainer.model.arena.weights.detach().reshape(-1)
+    budget = (limit_bytes - 4096 * (2 * grid.pp + 1)) // grid.pp     # this stage's share, less the .npy headers
+    if weights.numel() * 4 <= budget:
+        np.save(os.path.join(out_dir, f"weights_stage{stage}.npy"), weights.float().cpu().numpy())
+    else:
+        n_sample = budget // 12                                         # float32 value + int64 position each
+        idx = np.unique(np.random.default_rng(1234).integers(0, weights.numel(), size=n_sample, dtype=np.int64))
+        picked = weights[torch.from_numpy(idx).to(weights.device)].float().cpu().numpy()
+        np.save(os.path.join(out_dir, f"weights_stage{stage}_idx.npy"), idx)
+        np.save(os.path.join(out_dir, f"weights_stage{stage}.npy"), picked)
+    if trainer.is_last:
+        np.save(os.path.join(out_dir, "loss.npy"), np.array([loss], dtype=np.float64))
 
 
 def relaunch_under_torchrun(args):
@@ -87,7 +127,7 @@ def run_reference(args):
     import run_reference as rr
 
     if not rr.reference_available():
-        print(json.dumps({"impl": "reference", "unavailable": "baseline/_ref not installed (pip --target baseline/_ref /root/reference)"}))
+        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref not installed (python oracle/build_reference.py <ShallowSpeed checkout>)"}))
         return
     rank = int(os.environ.get("RANK", "0"))
     gbs = global_batch(args)
@@ -237,6 +277,8 @@ def run_ours(args):
         e2e_samples = timed_blocks(e2e_step, args.steps, args.repeats, stream)
         losses.append(trainer.flush())
     sampler[0] = None
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, trainer, losses[-1], grid)
     ms_dev, dev_blocks = reduce_blocks(dev_samples)
     ms_e2e, e2e_blocks = reduce_blocks(e2e_samples)
     clocks = clk.summary()
@@ -306,9 +348,8 @@ def run_ours(args):
             "impl": "ours", "metric": "MLP training samples/sec (whole job)", "value": value, "unit": "samples/s",
             "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_dev / args.steps,
             "higher_is_better": True, "scaling": args.scaling, "vs_baseline": None,
-            "dtype": ("fp32 (storage + accumulate fp32; products on tcgen05 as 3xTF32 = lo*hi + hi*lo + hi*hi; measured error vs an fp64 "
-                      "oracle at K=784: 6.4e-6 with the default chain-kernel instantiation, 8.5e-7 with SSB_CHAIN_ACC=1, "
-                      "cuBLAS fp32 2.9e-7 - profiles/precision_r2.md)"
+            "dtype": ("fp32 (storage + accumulate fp32; tensor-core products as 3xTF32 = lo*hi + hi*lo + hi*hi, "
+                      "each 32-wide k-block summed in fp32)"
                       if args.precision == "fp32" else "tf32 (fp32 storage + accumulate, single-pass tf32 products)"),
             "data": "synthetic MNIST-shaped, random-init weights",
             "e2e": {"value": e2e, "unit": "samples/s", "ms_per_step": ms_e2e / args.steps, "h2d_bytes_per_step": h2d,
@@ -327,7 +368,7 @@ def run_ours(args):
                        "pp_transport": (trainer.worker.pp_transport if args.pp > 1 else "none"), "cuda_graph": (not args.no_graph) and not eng.comm_timing_enabled(),
                        "kernels_per_step": kps, "graph_nodes": int(eng.graph_nodes()),
                        "l2": f"inputs cycle through a pool of {pool} distinct batches ({pool * h2d / 1e6:.0f} MB"
-                             + (" > 126 MB L2)" if pool * h2d > 126e6 else ")")
+                             + (" > 50 MB L2)" if pool * h2d > 50e6 else ")")
                              + f"; weights of this stage: {trainer.model.arena.weights.numel() * 4 / 1e6:.1f} MB"
                              + (" (legitimately L2-resident across steps)" if trainer.model.arena.weights.numel() * 4 < 20e6 else " (larger than L2: streamed from HBM every step)"),
                        "uses_chain_kernel": bool(eng.uses_chain()) if hasattr(eng, "uses_chain") else None,

@@ -1,4 +1,4 @@
-// Python bindings (torch extension) for the sm_100a kernels and the native runtime.
+// Python bindings (torch extension) for the sm_90a kernels and the native runtime.
 #include <torch/extension.h>
 #include <pybind11/stl.h>
 #include <sstream>
@@ -28,33 +28,13 @@ static void cuda_ok(cudaError_t e, const char* what) {
 }
 static cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 
-// y[rows, out] = relu?(x @ W^T + b)
-static ssb::GemmLo make_lo(const c10::optional<Tensor>& a, const c10::optional<Tensor>& b, const c10::optional<Tensor>& out) {
-    ssb::GemmLo lo;
-    if (a.has_value() && b.has_value()) {
-        lo.A = a->data_ptr<float>();
-        lo.B = b->data_ptr<float>();
-        lo.out = out.has_value() ? out->data_ptr<float>() : nullptr;
-    }
-    return lo;
-}
-
-static void split_lo(const Tensor& x, Tensor& lo) {
-    TORCH_CHECK(x.is_cuda() && lo.is_cuda() && x.scalar_type() == torch::kFloat32 && lo.scalar_type() == torch::kFloat32);
-    TORCH_CHECK(x.storage().nbytes() > 0 && x.numel() == lo.numel());
-    c10::cuda::CUDAGuard guard(x.device());
-    // operates on the padded storage of 2-D views (same strides for x and lo)
-    const int64_t n = x.dim() == 2 ? x.size(0) * x.stride(0) : x.numel();
-    cuda_ok(ssb::launch_split_lo(x.data_ptr<float>(), lo.data_ptr<float>(), n, cur_stream()), "split_lo");
-}
-
 // k_splits: 0 / 1 = plain kernel, -1 = let the planner decide, k >= 2 = force k (must not leave a split empty).
 // The workspace and the tile counters are torch tensors owned by the caller's scope (stream-ordered reuse).
 static void enable_splitk(ssb::GemmPlan& plan, int64_t k_splits, const Tensor& like, Tensor& ws, Tensor& counters) {
     if (k_splits == 0 || k_splits == 1) return;
     int splits = (int)k_splits;
     if (k_splits < 0) {
-        int dev = 0, sms = 148;
+        int dev = 0, sms = 132;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         splits = ssb::gemm_splitk_choice(plan, sms);
@@ -67,9 +47,9 @@ static void enable_splitk(ssb::GemmPlan& plan, int64_t k_splits, const Tensor& l
     TORCH_CHECK(err == nullptr, "split-K: ", err ? err : "");
 }
 
+// y[rows, out] = relu?(x @ W^T + b); split: 3xTF32 (fp32-equivalent) products
 static void linear_fwd(const Tensor& x, const Tensor& W, const c10::optional<Tensor>& bias, int64_t bias_stride,
-                       bool relu, Tensor& y, const c10::optional<Tensor>& W_lo, const c10::optional<Tensor>& x_lo,
-                       const c10::optional<Tensor>& y_lo, int64_t k_splits) {
+                       bool relu, Tensor& y, bool split, int64_t k_splits) {
     check_mat(x, "x"); check_mat(W, "W"); check_mat(y, "y");
     const int rows = x.size(0), in = x.size(1), out = W.size(0);
     TORCH_CHECK(W.size(1) == in && y.size(0) == rows && y.size(1) == out, "linear_fwd: shape mismatch");
@@ -77,8 +57,7 @@ static void linear_fwd(const Tensor& x, const Tensor& W, const c10::optional<Ten
     ssb::GemmPlan plan;
     const char* err = ssb::gemm_plan_fwd(&plan, W.data_ptr<float>(), ld_of(W), x.data_ptr<float>(), ld_of(x),
                                          y.data_ptr<float>(), ld_of(y), rows, in, out,
-                                         bias.has_value() ? bias->data_ptr<float>() : nullptr, (int)bias_stride, relu,
-                                         make_lo(W_lo, x_lo, y_lo));
+                                         bias.has_value() ? bias->data_ptr<float>() : nullptr, (int)bias_stride, relu, split);
     TORCH_CHECK(err == nullptr, "linear_fwd: ", err ? err : "");
     Tensor ws, counters;
     enable_splitk(plan, k_splits, x, ws, counters);
@@ -87,8 +66,7 @@ static void linear_fwd(const Tensor& x, const Tensor& W, const c10::optional<Ten
 
 // dx[rows, in] = (dz @ W) * (mask > 0)
 static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<Tensor>& mask, Tensor& dx,
-                         const c10::optional<Tensor>& W_lo, const c10::optional<Tensor>& dz_lo, const c10::optional<Tensor>& dx_lo,
-                         int64_t k_splits) {
+                         bool split, int64_t k_splits) {
     check_mat(dz, "dz"); check_mat(W, "W"); check_mat(dx, "dx");
     const int rows = dz.size(0), out = dz.size(1), in = W.size(1);
     TORCH_CHECK(W.size(0) == out && dx.size(0) == rows && dx.size(1) == in, "linear_dgrad: shape mismatch");
@@ -98,7 +76,7 @@ static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<
     const char* err = ssb::gemm_plan_dgrad(&plan, W.data_ptr<float>(), ld_of(W), dz.data_ptr<float>(), ld_of(dz),
                                            dx.data_ptr<float>(), ld_of(dx), rows, in, out,
                                            mask.has_value() ? mask->data_ptr<float>() : nullptr,
-                                           mask.has_value() ? ld_of(*mask) : 0, make_lo(W_lo, dz_lo, dx_lo));
+                                           mask.has_value() ? ld_of(*mask) : 0, split);
     TORCH_CHECK(err == nullptr, "linear_dgrad: ", err ? err : "");
     Tensor ws, counters;
     enable_splitk(plan, k_splits, dz, ws, counters);
@@ -108,7 +86,7 @@ static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<
 // G[out, in] (+)= dz^T @ x ; db[out] (+)= colsum(dz) ; optionally W -= lr * (G + ...)
 static void linear_wgrad(const Tensor& dz, const Tensor& x, Tensor& G, bool accumulate, const c10::optional<Tensor>& db,
                          int64_t db_stride, const c10::optional<Tensor>& W, double lr, bool fuse_sgd,
-                         const c10::optional<Tensor>& dz_lo, const c10::optional<Tensor>& x_lo) {
+                         bool split) {
     check_mat(dz, "dz"); check_mat(x, "x"); check_mat(G, "G");
     const int rows = dz.size(0), out = dz.size(1), in = x.size(1);
     TORCH_CHECK(x.size(0) == rows && G.size(0) == out && G.size(1) == in, "linear_wgrad: shape mismatch");
@@ -118,7 +96,7 @@ static void linear_wgrad(const Tensor& dz, const Tensor& x, Tensor& G, bool accu
                                            G.data_ptr<float>(), ld_of(G), rows, in, out, accumulate,
                                            db.has_value() ? db->data_ptr<float>() : nullptr, (int)db_stride,
                                            W.has_value() ? W->data_ptr<float>() : nullptr,
-                                           W.has_value() ? ld_of(*W) : 0, (float)lr, fuse_sgd, make_lo(dz_lo, x_lo, c10::nullopt));
+                                           W.has_value() ? ld_of(*W) : 0, (float)lr, fuse_sgd, split);
     TORCH_CHECK(err == nullptr, "linear_wgrad: ", err ? err : "");
     cuda_ok(ssb::gemm_launch(plan, cur_stream()), "linear_wgrad launch");
 }
@@ -173,16 +151,13 @@ static void argmax_correct(const Tensor& pred, const Tensor& target, Tensor& cor
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-    m.doc() = "shallowspeed_b200 native module: sm_100a kernels + C++ pipeline runtime";
-    m.def("split_lo", &split_lo);
+    m.doc() = "shallowspeed_b200 native module: sm_90a kernels + C++ pipeline runtime";
     m.def("linear_fwd", &linear_fwd, py::arg("x"), py::arg("W"), py::arg("bias"), py::arg("bias_stride"), py::arg("relu"),
-          py::arg("y"), py::arg("W_lo") = py::none(), py::arg("x_lo") = py::none(), py::arg("y_lo") = py::none(),
-          py::arg("k_splits") = 0);
+          py::arg("y"), py::arg("split") = false, py::arg("k_splits") = 0);
     m.def("linear_dgrad", &linear_dgrad, py::arg("dz"), py::arg("W"), py::arg("mask"), py::arg("dx"),
-          py::arg("W_lo") = py::none(), py::arg("dz_lo") = py::none(), py::arg("dx_lo") = py::none(), py::arg("k_splits") = 0);
+          py::arg("split") = false, py::arg("k_splits") = 0);
     m.def("linear_wgrad", &linear_wgrad, py::arg("dz"), py::arg("x"), py::arg("G"), py::arg("accumulate"), py::arg("db"),
-          py::arg("db_stride"), py::arg("W"), py::arg("lr"), py::arg("fuse_sgd"), py::arg("dz_lo") = py::none(),
-          py::arg("x_lo") = py::none());
+          py::arg("db_stride"), py::arg("W"), py::arg("lr"), py::arg("fuse_sgd"), py::arg("split") = false);
     m.def("loss_head", &loss_head);
     m.def("softmax_grad", &softmax_grad);
     m.def("relu_mask_", &relu_mask_);
@@ -207,13 +182,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         ssb::dp_layer_geometry(in, out, dp, &block_n, &tm, &tn, &slots, &slot_floats, one_shot ? 1 : 0);
         return std::make_tuple(block_n, tm, tn, slots, slot_floats);
     });
-    // host-only planning logic, callable without a GPU (tests/test_splitk_planning.py):
+    // host-only planning logic, callable without a GPU (tests/test_planning.py):
     // (k_splits chosen, k-blocks per split, error string of enable() with dummy buffers or "")
     m.def("splitk_plan", [](int m_total, int n_rows, int k_total, int num_sms, int force) {
         ssb::GemmPlan plan{};
         plan.mode = ssb::GEMM_FWD;
         plan.p.m_total = m_total; plan.p.n_total = n_rows; plan.p.k_total = k_total;
-        plan.p.block_n = n_rows >= 256 ? 256 : (n_rows + 15) / 16 * 16;
+        plan.p.block_n = n_rows >= 64 ? 64 : (n_rows + 15) / 16 * 16;   // as gemm_plan_fwd
         plan.grid = dim3((m_total + 127) / 128, (n_rows + plan.p.block_n - 1) / plan.p.block_n, 1);
         int splits = force > 0 ? force : ssb::gemm_splitk_choice(plan, num_sms);
         const int num_kb = (k_total + 31) / 32;

@@ -1,7 +1,7 @@
 // Latency-optimal fused data-parallel path for narrow layers (the reference's workload): ONE kernel for the whole
 // stage does, per [128 x 32] weight tile,
 //
-//     dW tile = dZ^T X                       tcgen05.mma (3xTF32 or TF32), accumulator in TMEM
+//     dW tile = dZ^T X                       mma.sync (3xTF32 or TF32), accumulator in registers
 //  A) every row of the partial goes to the replica that OWNS the row        (reduce-scatter hop, NVLink)
 //  B) the owner sums the dp partials in rank order, applies SGD              (bit-identical everywhere: computed once)
 //  C) and sends the NEW WEIGHTS of its rows to every replica                 (all-gather hop, NVLink)
@@ -16,7 +16,7 @@
 // one grid, co-resident by construction: tiles + chain CTAs <= #SMs).  Each CTA's TMA producer waits on the chain
 // kernel's per-layer device counter (dz[l] final and W_l no longer read by dgrad), so the communication of layer l
 // overlaps the backward pass of layers l-1 .. 1 - the reference's overlap structure
-// (/root/reference/shallowspeed/pipe.py:302-327, 389-400), tile by tile instead of layer by layer.
+// (shallowspeed/pipe.py:302-327, 389-400 of the reference), tile by tile instead of layer by layer.
 //
 // Deadlock freedom: phase A never waits; phase B waits only for phase-A lines; phase C only for phase-B lines; every
 // CTA of every rank is resident; all spins are bounded (trap instead of hanging the GPU).
@@ -29,7 +29,7 @@
 
 namespace ssb {
 
-static constexpr int kThreads = 192;                   // warp 0 TMA, warp 1 MMA, warps 2..5 epilogue / protocol
+static constexpr int kThreads = 160;                   // warp 0 TMA, warps 1..4 MMA + epilogue / protocol
 static constexpr uint32_t kBlockM = 128;
 static constexpr uint32_t kBlockK = 32;
 static constexpr uint32_t kABytes = kBlockM * 128;     // dZ^T tile of one k-block: 4 MN-major panels
@@ -77,37 +77,23 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
     const DpLLEntry& e = entries[blockIdx.x];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int num_kb = (e.k_total + (int)kBlockK - 1) / (int)kBlockK;
-    const uint32_t half_bytes = kABytes + kBBytes;
-    const uint32_t stage_bytes = e.split ? 2u * half_bytes : half_bytes;
+    const uint32_t stage_bytes = kABytes + kBBytes;
     const uint32_t own_off = p.stages * stage_bytes;                       // tile staging [128 rows][kOwnLd] floats
     const uint32_t own_bytes = kBlockM * kOwnLd * 4u;
     const uint32_t bar_base = smem_base + own_off + own_bytes;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
-    const uint32_t tmem_full_bar = bar_base + 8u * (2 * p.stages);
-    const uint32_t tmem_slot = tmem_full_bar + 8u;
-    volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + own_off + own_bytes + 8u * (2 * p.stages + 1));
-    const uint32_t tmem_cols = e.split ? 64u : 32u;
-    const uint32_t small_off = e.split ? 32u : 0u;           // second accumulator for the small 3xTF32 cross terms (ptx.cuh)
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&e.tmA);
         tma_prefetch_desc(&e.tmB);
         for (int s = 0; s < p.stages; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 5);          // MMA commit + the 4 epilogue warps (bias-gradient reduction)
+            mbar_init(empty_bar(s), 4);          // one arrive per math warp
         }
-        mbar_init(tmem_full_bar, 1);
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, tmem_cols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
 
     if (warp == 0) {
         // ------------------------------------------------------------ TMA producer (converged warp, elected lane issues)
@@ -126,95 +112,47 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
 #pragma unroll
                 for (int i = 0; i < 4; ++i) tma_load_2d(a_dst + i * kPanelBytes, &e.tmA, full_bar(s), e.m0 + 32 * i, k0);
                 tma_load_2d(b_dst, &e.tmB, full_bar(s), e.n0, k0);
-                if (e.split) {
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) tma_load_2d(a_dst + half_bytes + i * kPanelBytes, &e.tmAlo, full_bar(s), e.m0 + 32 * i, k0);
-                    tma_load_2d(b_dst + half_bytes, &e.tmBlo, full_bar(s), e.n0, k0);
-                }
-            }
-            __syncwarp();
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------ MMA issuer
-        const uint32_t idesc = umma_idesc_tf32(kBlockM, 32u, 1u, 1u);
-        const uint32_t mn_hi = umma_desc_hi(512u, 1u);
-        for (int kb = 0; kb < num_kb; ++kb) {
-            const int s = kb % p.stages;
-            mbar_wait(full_bar(s), (kb / p.stages) & 1);
-            tc_fence_after();
-            const uint32_t a_src = smem_base + s * stage_bytes, b_src = a_src + kABytes;
-            const uint32_t a_lo = umma_desc_lo(a_src, kPanelBytes), b_lo = umma_desc_lo(b_src, kPanelBytes);
-            if (elect_one()) {
-                if (e.split) {
-                    const uint32_t al = a_lo + (half_bytes >> 4), bl = b_lo + (half_bytes >> 4);
-#pragma unroll
-                    for (int k4 = 0; k4 < 4; ++k4) {
-                        const uint32_t first = (kb | k4) != 0 ? 1u : 0u;
-                        umma_tf32(tmem_base + small_off, umma_desc_pack(al + k4 * 64u, mn_hi), umma_desc_pack(b_lo + k4 * 64u, mn_hi), idesc, first);
-                        umma_tf32(tmem_base + small_off, umma_desc_pack(a_lo + k4 * 64u, mn_hi), umma_desc_pack(bl + k4 * 64u, mn_hi), idesc, 1u);
-                        umma_tf32(tmem_base, umma_desc_pack(a_lo + k4 * 64u, mn_hi), umma_desc_pack(b_lo + k4 * 64u, mn_hi), idesc, first);
-                    }
-                } else {
-#pragma unroll
-                    for (int k4 = 0; k4 < 4; ++k4)
-                        umma_tf32(tmem_base, umma_desc_pack(a_lo + k4 * 64u, mn_hi), umma_desc_pack(b_lo + k4 * 64u, mn_hi), idesc, (kb | k4) != 0 ? 1u : 0u);
-                }
-                umma_commit(empty_bar(s));
-                if (kb == num_kb - 1) umma_commit(tmem_full_bar);
             }
             __syncwarp();
         }
     } else {
-        // ------------------------------------------------------------ epilogue warps: GEMM drain + the LL protocol
+        // ------------------------------------------------------------ math warps: the GEMM + the LL protocol
         const uint32_t epoch = *reinterpret_cast<const volatile uint32_t*>(p.epoch_ptr);
         const uint32_t parity = epoch & 1u;
         const int q = warp & 3;
-        const int m_local = q * 32 + lane;                       // row of the tile = TMEM lane
-        const int etid = (warp - 2) * 32 + lane;                 // 0..127
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
+        const int m_local = q * 32 + lane;                       // row of the tile owned by this thread after the GEMM
+        const int etid = (warp - 1) * 32 + lane;                 // 0..127
         constexpr int rpo = (int)kBlockM / DP;                   // rows per owner
         const int lpr = e.has_bias ? 17 : 16;                    // lines per row (line 16 = bias gradient / new bias)
         const int rows_valid = min((int)kBlockM, e.m_total - e.m0);
         float* own = reinterpret_cast<float*>(smem_gen + own_off);
 
         LLDBG(0);                                                // CTA resident, waiting for operands
-        // bias gradient of my row: column sum of dZ over the local rows, read from the staged A panels
+        // this warp's 32 rows of the tile, and the bias gradient of my row: column sum of dZ over the local rows, read
+        // from the staged A panels
+        float acc[2][4][4];
+        warp_acc_zero(acc);
         float dbsum = 0.f;
         for (int kb = 0; kb < num_kb; ++kb) {
             const int s = kb % p.stages;
             mbar_wait(full_bar(s), (kb / p.stages) & 1);
+            const uint32_t a_src = smem_base + s * stage_bytes;
+            if (e.split) warp_mma_kblock<4, true, true, true>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, 4, lane);
+            else warp_mma_kblock<4, true, true, false>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, 4, lane);
             if (e.has_bias) {
-                const uint32_t panel = smem_base + s * stage_bytes + q * kPanelBytes;
 #pragma unroll 8
-                for (int r = 0; r < 32; ++r) {
-                    const uint32_t addr = panel + r * 128u + ((((uint32_t)lane >> 3) ^ (r & 3u)) << 5) + ((lane & 7u) << 2);
-                    float v;
-                    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
-                    dbsum += v;
-                }
+                for (int r = 0; r < 32; ++r) dbsum += lds_f32(a_src + operand_off<true>((uint32_t)m_local, (uint32_t)r));
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(empty_bar(s));
         }
         LLDBG(1);                                                // all operand tiles landed (gate open + TMA)
-        mbar_wait(tmem_full_bar, 0);
-        tc_fence_after();
         LLDBG(2);                                                // accumulator complete
-        float v[32];
-        {
-            float a[16], b[16];
-            tmem_ld16_acc(taddr, small_off, a);
-            tmem_ld16_acc(taddr + 16, small_off, b);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) { v[j] = a[j]; v[16 + j] = b[j]; }
-        }
-        tc_fence_before();
 
         // ---------------- phase A: every row of the partial goes to the owner of that row.  The tile is staged in shared
         // memory first so that consecutive lanes write consecutive 16-byte lines: a replica's slice [rpo rows][lpr lines]
         // is contiguous in its landing zone, i.e. every warp store is one 512-byte run on the wire.
-#pragma unroll
-        for (int j = 0; j < 32; ++j) own[m_local * kOwnLd + j] = v[j];
+        warp_acc_to_rows(acc, own + q * 32 * kOwnLd, kOwnLd, 4, lane);
         own[m_local * kOwnLd + 32] = dbsum;
         asm volatile("bar.sync 1, 128;" ::: "memory");
         {
@@ -287,11 +225,6 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
                         const int n = e.n0 + 2 * j;
                         if (n < e.n_total) { w0 = wv0[u] - p.lr * s0; wrow[n] = w0; }
                         if (n + 1 < e.n_total) { w1 = wv1[u] - p.lr * s1; wrow[n + 1] = w1; }
-                        if (p.W_lo != nullptr) {               // lo twins of the new weights ride along (no arena-wide split kernel)
-                            float* lrow = p.W_lo + e.w_offset + (int64_t)(e.m0 + row) * e.ldw;
-                            if (n < e.n_total) lrow[n] = tf32_lo(w0);
-                            if (n + 1 < e.n_total) lrow[n + 1] = tf32_lo(w1);
-                        }
                     } else {
                         w0 = wv0[u] - p.lr * s0;                 // bias lives in column `in` of the block
                         wrow[e.n_total] = w0;
@@ -332,11 +265,6 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
                         const int n = e.n0 + 2 * jv[u];
                         if (n < e.n_total) wrow[n] = __uint_as_float(x.x);
                         if (n + 1 < e.n_total) wrow[n + 1] = __uint_as_float(x.z);
-                        if (p.W_lo != nullptr) {
-                            float* lrow = p.W_lo + e.w_offset + (int64_t)(e.m0 + rowv[u]) * e.ldw;
-                            if (n < e.n_total) lrow[n] = tf32_lo(__uint_as_float(x.x));
-                            if (n + 1 < e.n_total) lrow[n + 1] = tf32_lo(__uint_as_float(x.z));
-                        }
                     } else {
                         wrow[e.n_total] = __uint_as_float(x.x);
                     }
@@ -344,11 +272,6 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
             }
         }
         LLDBG(5);                                                // all replicas' rows written locally
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, tmem_cols);
     }
 }
 
@@ -367,22 +290,17 @@ const char* dp_ll_plan(DpLLPlan* plan, const DpLLLayer* layers, int n_layers, in
     bool split = false;
     for (int l = 0; l < n_layers; ++l) {
         const DpLLLayer& ly = layers[l];
-        CUtensorMap tmA, tmB, tmAlo, tmBlo;
+        CUtensorMap tmA, tmB;
         if (const char* err = make_tmap_mn(&tmA, ly.dZ, ly.out, rows, ly.lddz)) return err;
         if (const char* err = make_tmap_mn(&tmB, ly.X, ly.in, rows, ly.ldx)) return err;
-        tmAlo = tmA; tmBlo = tmB;
-        const bool sp = ly.dZ_lo != nullptr && ly.X_lo != nullptr;
-        if (sp) {
-            if (const char* err = make_tmap_mn(&tmAlo, ly.dZ_lo, ly.out, rows, ly.lddz)) return err;
-            if (const char* err = make_tmap_mn(&tmBlo, ly.X_lo, ly.in, rows, ly.ldx)) return err;
-        }
+        const bool sp = ly.split != 0;                              // 3xTF32: the kernel derives the lo parts from the tiles
         split = split || sp;
         const int tm = (ly.out + (int)kBlockM - 1) / (int)kBlockM, tn = (ly.in + 31) / 32;
         for (int mt = 0; mt < tm; ++mt)
             for (int nt = 0; nt < tn; ++nt) {
                 DpLLEntry e;
                 memset(&e, 0, sizeof(e));
-                e.tmA = tmA; e.tmB = tmB; e.tmAlo = tmAlo; e.tmBlo = tmBlo;
+                e.tmA = tmA; e.tmB = tmB;
                 e.m0 = mt * (int)kBlockM; e.n0 = nt * 32;
                 e.m_total = ly.out; e.n_total = ly.in; e.k_total = rows;
                 e.split = sp ? 1 : 0;
@@ -395,12 +313,12 @@ const char* dp_ll_plan(DpLLPlan* plan, const DpLLLayer* layers, int n_layers, in
     }
     if (tile != base.n_tiles) return "dp_ll_plan: tile count does not match the landing zones of the DpContext";
     const int num_kb = (rows + (int)kBlockK - 1) / (int)kBlockK;
-    const int stage_bytes = (int)(kABytes + kBBytes) * (split ? 2 : 1);
+    const int stage_bytes = (int)(kABytes + kBBytes);
     int stages = (190 * 1024) / stage_bytes;
     stages = std::min(stages, std::max(num_kb, 2));
     stages = std::min(stages, 8);
     plan->p.stages = stages;
-    plan->smem_bytes = stages * stage_bytes + (int)kBlockM * kOwnLd * 4 + 1024 + 8 * (2 * stages + 2) + 16;
+    plan->smem_bytes = stages * stage_bytes + (int)kBlockM * kOwnLd * 4 + 1024 + 8 * (2 * stages) + 16;
     DpLLEntry* dev = nullptr;
     if (cudaMalloc(&dev, host.size() * sizeof(DpLLEntry)) != cudaSuccess) return "dp_ll_plan: cudaMalloc failed";
     if (cudaMemcpy(dev, host.data(), host.size() * sizeof(DpLLEntry), cudaMemcpyHostToDevice) != cudaSuccess) {

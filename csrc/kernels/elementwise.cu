@@ -44,7 +44,7 @@ __global__ void __launch_bounds__(256) loss_head_kernel(const float* __restrict_
                                                         float* __restrict__ probs, int ldp,
                                                         float* __restrict__ dlogits, int ldd,
                                                         float* __restrict__ loss_out, int rows_total, int cols, float inv_batch,
-                                                        int rows_per_block, float* __restrict__ dlogits_lo) {
+                                                        int rows_per_block) {
     // one CTA per micro-batch: the global-max / loss contract is per micro-batch
     __shared__ float scratch[32];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
@@ -54,7 +54,6 @@ __global__ void __launch_bounds__(256) loss_head_kernel(const float* __restrict_
     if (aux != nullptr) aux += (size_t)row0 * lda;
     if (probs != nullptr) probs += (size_t)row0 * ldp;
     if (dlogits != nullptr) dlogits += (size_t)row0 * ldd;
-    if (dlogits_lo != nullptr) dlogits_lo += (size_t)row0 * ldd;
     if (loss_out != nullptr) loss_out += blockIdx.x;
 
     float mx = -FLT_MAX;
@@ -87,7 +86,6 @@ __global__ void __launch_bounds__(256) loss_head_kernel(const float* __restrict_
                 const float up = (MODE == 1) ? (-2.f * (aux[(size_t)r * lda + c] - pc) * inv_batch) : aux[(size_t)r * lda + c];
                 const float dzv = pc * up - pc * gsum;
                 dlogits[(size_t)r * ldd + c] = dzv;
-                if (dlogits_lo != nullptr) dlogits_lo[(size_t)r * ldd + c] = tf32_lo(dzv);
             }
         }
     }
@@ -99,39 +97,36 @@ __global__ void __launch_bounds__(256) loss_head_kernel(const float* __restrict_
 
 cudaError_t launch_loss_head(const float* logits, int ldl, const float* target, int ldt, float* probs, int ldp,
                              float* dlogits, int ldd, float* loss_out, int rows, int cols, float inv_batch,
-                             cudaStream_t stream, int rows_per_mubatch, float* dlogits_lo) {
+                             cudaStream_t stream, int rows_per_mubatch) {
     const int rpb = rows_per_mubatch > 0 ? rows_per_mubatch : rows;
     const int blocks = (rows + rpb - 1) / rpb;
     if (target != nullptr)
-        loss_head_kernel<1><<<blocks, 256, 0, stream>>>(logits, ldl, target, ldt, probs, ldp, dlogits, ldd, loss_out, rows, cols, inv_batch, rpb, dlogits_lo);
+        loss_head_kernel<1><<<blocks, 256, 0, stream>>>(logits, ldl, target, ldt, probs, ldp, dlogits, ldd, loss_out, rows, cols, inv_batch, rpb);
     else
-        loss_head_kernel<0><<<blocks, 256, 0, stream>>>(logits, ldl, nullptr, 0, probs, ldp, nullptr, 0, nullptr, rows, cols, 0.f, rpb, nullptr);
+        loss_head_kernel<0><<<blocks, 256, 0, stream>>>(logits, ldl, nullptr, 0, probs, ldp, nullptr, 0, nullptr, rows, cols, 0.f, rpb);
     return cudaGetLastError();
 }
 
 cudaError_t launch_softmax_grad(const float* logits, int ldl, const float* upstream, int ldu, float* dlogits, int ldd,
                                 int rows, int cols, cudaStream_t stream) {
-    loss_head_kernel<2><<<1, 256, 0, stream>>>(logits, ldl, upstream, ldu, nullptr, 0, dlogits, ldd, nullptr, rows, cols, 0.f, rows, nullptr);
+    loss_head_kernel<2><<<1, 256, 0, stream>>>(logits, ldl, upstream, ldu, nullptr, 0, dlogits, ldd, nullptr, rows, cols, 0.f, rows);
     return cudaGetLastError();
 }
 
 // ---------------------------------------------------------------- elementwise
-__global__ void relu_mask_kernel(float* __restrict__ g, int ldg, const float* __restrict__ y, int ldy, int rows, int cols,
-                                 float* __restrict__ g_lo) {
+__global__ void relu_mask_kernel(float* __restrict__ g, int ldg, const float* __restrict__ y, int ldy, int rows, int cols) {
     const long total = (long)rows * cols;
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
         const int r = (int)(i / cols), c = (int)(i % cols);
-        float v = g[(size_t)r * ldg + c];
-        if (!(y[(size_t)r * ldy + c] > 0.f)) { v = 0.f; g[(size_t)r * ldg + c] = 0.f; }
-        if (g_lo != nullptr) g_lo[(size_t)r * ldg + c] = tf32_lo(v);
+        if (!(y[(size_t)r * ldy + c] > 0.f)) g[(size_t)r * ldg + c] = 0.f;
     }
 }
-cudaError_t launch_relu_mask(float* g, int ldg, const float* y, int ldy, int rows, int cols, cudaStream_t stream, float* g_lo) {
+cudaError_t launch_relu_mask(float* g, int ldg, const float* y, int ldy, int rows, int cols, cudaStream_t stream) {
     const long total = (long)rows * cols;
     int blocks = (int)((total + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     if (blocks < 1) blocks = 1;
-    relu_mask_kernel<<<blocks, 256, 0, stream>>>(g, ldg, y, ldy, rows, cols, g_lo);
+    relu_mask_kernel<<<blocks, 256, 0, stream>>>(g, ldg, y, ldy, rows, cols);
     return cudaGetLastError();
 }
 
@@ -140,7 +135,7 @@ __global__ void relu_fwd_kernel(const float* __restrict__ x, float* __restrict__
 }
 cudaError_t launch_relu_fwd(const float* x, float* y, long n, cudaStream_t stream) {
     int blocks = (int)((n + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     if (blocks < 1) blocks = 1;
     relu_fwd_kernel<<<blocks, 256, 0, stream>>>(x, y, n);
     return cudaGetLastError();
@@ -151,31 +146,9 @@ __global__ void axpby_kernel(const float* __restrict__ x, const float* __restric
 }
 cudaError_t launch_axpby(const float* x, const float* t, float* y, float a, float b, long n, cudaStream_t stream) {
     int blocks = (int)((n + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     if (blocks < 1) blocks = 1;
     axpby_kernel<<<blocks, 256, 0, stream>>>(x, t, y, a, b, n);
-    return cudaGetLastError();
-}
-
-__global__ void split_lo_kernel(const float4* __restrict__ x, float4* __restrict__ lo, long n4) {
-    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
-        const float4 v = x[i];
-        lo[i] = make_float4(tf32_lo(v.x), tf32_lo(v.y), tf32_lo(v.z), tf32_lo(v.w));
-    }
-}
-__global__ void split_lo_tail_kernel(const float* x, float* lo, long start, long n) {
-    const long i = start + blockIdx.x * (long)blockDim.x + threadIdx.x;
-    if (i < n) lo[i] = tf32_lo(x[i]);
-}
-cudaError_t launch_split_lo(const float* x, float* lo, long n, cudaStream_t stream) {
-    const bool aligned = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(lo)) & 15) == 0;
-    const long n4 = aligned ? n / 4 : 0;
-    if (n4 > 0) {
-        long blocks = (n4 + 255) / 256;
-        if (blocks > 148 * 8) blocks = 148 * 8;
-        split_lo_kernel<<<(int)blocks, 256, 0, stream>>>(reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(lo), n4);
-    }
-    if (n4 * 4 < n) split_lo_tail_kernel<<<(int)((n - n4 * 4 + 255) / 256), 256, 0, stream>>>(x, lo, n4 * 4, n);
     return cudaGetLastError();
 }
 
@@ -199,7 +172,7 @@ cudaError_t launch_sgd(float* w, const float* g, float lr, long n, cudaStream_t 
     const long n4 = aligned ? n / 4 : 0;
     if (n4 > 0) {
         long blocks = (n4 + 255) / 256;
-        if (blocks > 148 * 8) blocks = 148 * 8;
+        if (blocks > 132 * 8) blocks = 132 * 8;
         sgd_kernel<<<(int)blocks, 256, 0, stream>>>(reinterpret_cast<float4*>(w), reinterpret_cast<const float4*>(g), lr, n4);
     }
     const long done = n4 * 4;

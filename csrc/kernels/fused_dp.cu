@@ -1,8 +1,8 @@
-// THE fused data-parallel path (SURVEY.md K3 + C3 + K6, BASELINE.json north star):
+// THE fused data-parallel path (SURVEY.md K3 + C3 + K6):
 //
-//     dW tile = dZ^T X   (tcgen05, accumulator in TMEM)
-//       -> pushed straight from TMEM/registers into the OWNER replica's staging memory over
-//          NVLink (P2P st.global), tile by tile while the next tile's MMA runs
+//     dW tile = dZ^T X   (mma.sync TF32 / 3xTF32, accumulator in registers)
+//       -> pushed from a shared-memory staging tile into the OWNER replica's staging memory over
+//          NVLink (P2P st.global), tile by tile while the next tile's operands stream in
 //       -> the owner sums the DP partials in fixed rank order (bitwise deterministic, and
 //          bit-identical on every replica because only the owner computes the result)
 //       -> W_tile -= lr * sum, and the NEW WEIGHTS are written to every replica's W (P2P)
@@ -24,7 +24,8 @@
 
 namespace ssb {
 
-static constexpr int kThreads = 192;
+static constexpr int kThreads = 160;                   // warp 0 TMA, warps 1..4 MMA + push / reduce
+static constexpr int kMaxBlockN = 64;                  // a math warp holds a 32 x block_n fp32 accumulator in registers
 static constexpr uint32_t kBlockM = 128;
 static constexpr uint32_t kBlockK = 32;
 static constexpr uint32_t kABytes = kBlockM * 128;
@@ -165,7 +166,6 @@ __device__ __forceinline__ void dp_wait_tile_done(const DpPeers& peers, const Dp
 // =============================================================================================
 __global__ void __launch_bounds__(kThreads, 1)
 fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                      const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo,
                       const DpLayerParams p, const DpPeers peers) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
@@ -185,40 +185,22 @@ fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     const int cta = p.helpers > 1 ? blockIdx.x / p.helpers : blockIdx.x;      // tile-group index
     const int n_cta = p.helpers > 1 ? gridDim.x / p.helpers : gridDim.x;
     const uint32_t b_bytes = p.block_n * 128u;
-    const uint32_t half_bytes = kABytes + b_bytes;
-    const uint32_t stage_bytes = p.split ? 2u * half_bytes : half_bytes;
+    const uint32_t stage_bytes = kABytes + b_bytes;
     const uint32_t tile_bytes_k = kBlockM * ((uint32_t)p.block_n * 4u + 16u);
     const uint32_t bar_base = smem_base + p.stages * stage_bytes + tile_bytes_k;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
-    const uint32_t tmem_full_bar = bar_base + 8u * (2 * p.stages);
-    const uint32_t tmem_empty_bar = tmem_full_bar + 8u;
-    const uint32_t tmem_slot = tmem_empty_bar + 8u;
-    volatile uint32_t* tmem_slot_gen =
-        reinterpret_cast<volatile uint32_t*>(smem_gen + p.stages * stage_bytes + tile_bytes_k + 8u * (2 * p.stages + 2));
-    uint32_t tmem_cols = 32;
-    while (tmem_cols < (uint32_t)p.block_n * (p.split ? 2u : 1u)) tmem_cols <<= 1;
-    const uint32_t small_off = p.split ? (uint32_t)p.block_n : 0u;   // second accumulator for the small 3xTF32 cross terms (ptx.cuh)
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < p.stages; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 5);          // MMA commit + the 4 epilogue warps (bias-gradient reduction)
+            mbar_init(empty_bar(s), 4);          // one arrive per math warp
         }
-        mbar_init(tmem_full_bar, 1);
-        mbar_init(tmem_empty_bar, 4);            // one arrive per epilogue warp
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, tmem_cols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
     const uint32_t epoch = *reinterpret_cast<const volatile uint32_t*>(p.epoch_ptr);
 
     if (warp == 0) {
@@ -238,50 +220,6 @@ fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                         for (int i = 0; i < 4; ++i) tma_load_2d(a_dst + i * kPanelBytes, &tmA, full_bar(s), m0 + 32 * i, k0);
                         for (int j = 0; j < p.block_n / 32; ++j)
                             tma_load_2d(b_dst + j * kPanelBytes, &tmB, full_bar(s), n0 + 32 * j, k0);
-                        if (p.split) {
-#pragma unroll
-                            for (int i = 0; i < 4; ++i)
-                                tma_load_2d(a_dst + half_bytes + i * kPanelBytes, &tmAlo, full_bar(s), m0 + 32 * i, k0);
-                            for (int j = 0; j < p.block_n / 32; ++j)
-                                tma_load_2d(b_dst + half_bytes + j * kPanelBytes, &tmBlo, full_bar(s), n0 + 32 * j, k0);
-                        }
-                    }
-                    __syncwarp();
-                }
-            }
-        }
-    } else if (warp == 1) {
-        {
-            const uint32_t idesc = umma_idesc_tf32(kBlockM, p.block_n, 1u, 1u);
-            const uint32_t mn_hi = umma_desc_hi(512u, 1u);
-            int it = 0, tile_i = 0;
-            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++tile_i) {
-                mbar_wait(tmem_empty_bar, (tile_i & 1) ^ 1);      // epilogue drained the accumulator
-                tc_fence_after();
-                for (int kb = 0; kb < num_kb; ++kb, ++it) {
-                    const int s = it % p.stages;
-                    const uint32_t ph = (it / p.stages) & 1;
-                    mbar_wait(full_bar(s), ph);
-                    tc_fence_after();
-                    const uint32_t a_src = smem_base + s * stage_bytes, b_src = a_src + kABytes;
-                    const uint32_t a_lo = umma_desc_lo(a_src, kPanelBytes), b_lo = umma_desc_lo(b_src, kPanelBytes);
-                    if (elect_one()) {
-                        if (p.split) {
-                            const uint32_t al = a_lo + (half_bytes >> 4), bl = b_lo + (half_bytes >> 4);
-#pragma unroll
-                            for (int k4 = 0; k4 < 4; ++k4) {
-                                const uint32_t first = (kb | k4) != 0 ? 1u : 0u;
-                                umma_tf32(tmem_base + small_off, umma_desc_pack(al + k4 * 64u, mn_hi), umma_desc_pack(b_lo + k4 * 64u, mn_hi), idesc, first);
-                                umma_tf32(tmem_base + small_off, umma_desc_pack(a_lo + k4 * 64u, mn_hi), umma_desc_pack(bl + k4 * 64u, mn_hi), idesc, 1u);
-                                umma_tf32(tmem_base, umma_desc_pack(a_lo + k4 * 64u, mn_hi), umma_desc_pack(b_lo + k4 * 64u, mn_hi), idesc, first);
-                            }
-                        } else
-#pragma unroll
-                        for (int k4 = 0; k4 < 4; ++k4)
-                            umma_tf32(tmem_base, umma_desc_pack(a_lo + k4 * 64u, mn_hi), umma_desc_pack(b_lo + k4 * 64u, mn_hi), idesc,
-                                      (kb | k4) != 0 ? 1u : 0u);
-                        umma_commit(empty_bar(s));
-                        if (kb == num_kb - 1) umma_commit(tmem_full_bar);
                     }
                     __syncwarp();
                 }
@@ -290,55 +228,42 @@ fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     } else {
         const int q = warp & 3;
         const int m_local = q * 32 + lane;
-        const int etid = (warp - 2) * 32 + lane;                 // 0..127 among the epilogue threads
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
+        const int etid = (warp - 1) * 32 + lane;                 // 0..127 among the math threads
+        const int nt = p.block_n / 8;
         // ---------------- phase A: compute every tile, push the partial to its owner
         const bool batch_flags = (num_tiles > (int)gridDim.x) && p.helpers <= 1;   // more than one tile per CTA
         if (etid == 0) DPDBG(0);
         int it = 0, tile_i = 0;
         for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++tile_i) {
             const TileCoord tc = tile_coord(p, t);
+            float acc[2][kMaxBlockN / 8][4];
+            warp_acc_zero(acc);
             float dbsum = 0.f;
             for (int kb = 0; kb < num_kb; ++kb, ++it) {
                 const int s = it % p.stages;
                 const uint32_t ph = (it / p.stages) & 1;
                 mbar_wait(full_bar(s), ph);
+                const uint32_t a_src = smem_base + s * stage_bytes;
+                if (p.split) warp_mma_kblock<kMaxBlockN / 8, true, true, true>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, nt, lane);
+                else warp_mma_kblock<kMaxBlockN / 8, true, true, false>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, nt, lane);
                 if (tc.nt == 0) {
-                    const uint32_t panel = smem_base + s * stage_bytes + q * kPanelBytes;
 #pragma unroll 8
-                    for (int r = 0; r < 32; ++r) {
-                        const uint32_t addr = panel + r * 128u + ((((uint32_t)lane >> 3) ^ (r & 3u)) << 5) + ((lane & 7u) << 2);
-                        float v;
-                        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
-                        dbsum += v;
-                    }
+                    for (int r = 0; r < 32; ++r) dbsum += lds_f32(a_src + operand_off<true>((uint32_t)m_local, (uint32_t)r));
                 }
                 __syncwarp();
                 if (lane == 0) mbar_arrive(empty_bar(s));
             }
-            mbar_wait(tmem_full_bar, tile_i & 1);
-            tc_fence_after();
             if (etid == 0 && tile_i == 0) DPDBG(1);
             const int n_dst = p.one_shot ? p.dp : 1;
-            // TMEM (thread = row) -> padded smem tile -> row-contiguous 512-byte warp stores: each P2P store
+            // registers -> padded smem tile (one row per thread) -> row-contiguous 512-byte warp stores: each P2P store
             // instruction carries one full contiguous row segment over NVLink instead of 32 scattered 16-byte pieces
             const uint32_t pitch = (uint32_t)p.block_n * 4u + 16u;
             uint8_t* tile = smem_gen + p.stages * stage_bytes;
-            for (int c = 0; c < p.block_n; c += 16) {
-                float v[16];
-                tmem_ld16_acc(taddr + c, small_off, v);
-#pragma unroll
-                for (int g4 = 0; g4 < 4; ++g4)
-                    *reinterpret_cast<float4*>(tile + (size_t)m_local * pitch + (size_t)(c + 4 * g4) * 4) =
-                        make_float4(v[4 * g4], v[4 * g4 + 1], v[4 * g4 + 2], v[4 * g4 + 3]);
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tmem_empty_bar);           // accumulator drained: the next tile's MMA may start
+            warp_acc_to_rows(acc, reinterpret_cast<float*>(tile) + q * 32 * (int)(pitch / 4u), (int)(pitch / 4u), nt, lane);
+            if (p.bulk_push) fence_proxy_async_smem();            // every writer, before the barrier: rows are read by the TMA engine
             asm volatile("bar.sync 1, 128;" ::: "memory");
             if (p.bulk_push) {
-                // one TMA bulk copy per row and destination, issued by the thread that wrote the row
-                fence_proxy_async_smem();
+                // one TMA bulk copy per row and destination (the row's writers fenced before the barrier above)
                 for (int d = 0; d < n_dst; ++d) {
                     const int dst_rank = p.one_shot ? d : tc.owner;
                     float* dst = stage_slot(peers, p, dst_rank, p.rank, tc.slot, epoch);
@@ -349,7 +274,7 @@ fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 tma_store_wait_all();
                 asm volatile("fence.proxy.async;" ::: "memory");
             } else {
-                const int ew = warp - 2;                          // 0..3
+                const int ew = warp - 1;                          // 0..3
                 const int f4_per_row = p.block_n / 4;
                 for (int d = 0; d < n_dst; ++d) {
                     const int dst_rank = p.one_shot ? d : tc.owner;
@@ -417,11 +342,6 @@ fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
             }
         }
     }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, tmem_cols);
-    }
 }
 
 // =============================================================================================
@@ -487,7 +407,7 @@ const char* make_tmap_mn(CUtensorMap* map, const float* base, int inner, int out
 
 void dp_layer_geometry(int in, int out, int dp, int* block_n, int* n_tiles_m, int* n_tiles_n, int64_t* slots, int64_t* slot_floats_out,
                        int one_shot) {
-    *block_n = in >= 128 ? 128 : (in + 31) / 32 * 32;
+    *block_n = in >= kMaxBlockN ? kMaxBlockN : (in + 31) / 32 * 32;
     // latency-bound one-shot layers: narrow tiles => 4x more CTAs share the push and the reduce
     if (one_shot && !getenv("SSB_DP_WIDE_TILES")) *block_n = 32;
     *n_tiles_m = (out + (int)kBlockM - 1) / (int)kBlockM;
@@ -498,7 +418,7 @@ void dp_layer_geometry(int in, int out, int dp, int* block_n, int* n_tiles_m, in
 }
 
 const char* fused_dp_plan(FusedDpPlan* plan, const float* dZ, int lddz, const float* X, int ldx, int rows, const DpLayerParams& lp,
-                          const DpPeers& peers, int max_ctas, const float* dZ_lo, const float* X_lo) {
+                          const DpPeers& peers, int max_ctas, bool split) {
     *plan = FusedDpPlan{};
     plan->p = lp;
     plan->peers = peers;
@@ -507,22 +427,16 @@ const char* fused_dp_plan(FusedDpPlan* plan, const float* dZ, int lddz, const fl
     if (dZ != nullptr) {
         if (const char* e = make_tmap_mn(&plan->tmA, dZ, p.m_total, rows, lddz)) return e;
         if (const char* e = make_tmap_mn(&plan->tmB, X, p.n_total, rows, ldx)) return e;
-        plan->tmAlo = plan->tmA; plan->tmBlo = plan->tmB;
-        p.split = 0;
-        if (dZ_lo != nullptr && X_lo != nullptr) {
-            p.split = 1;
-            if (const char* e = make_tmap_mn(&plan->tmAlo, dZ_lo, p.m_total, rows, lddz)) return e;
-            if (const char* e = make_tmap_mn(&plan->tmBlo, X_lo, p.n_total, rows, ldx)) return e;
-        }
+        p.split = split ? 1 : 0;                  // 3xTF32: the kernel derives the lo parts from the tiles
     }
     const int num_kb = (rows + (int)kBlockK - 1) / (int)kBlockK;
-    const int stage_bytes = ((int)kABytes + p.block_n * 128) * (p.split ? 2 : 1);
+    const int stage_bytes = (int)kABytes + p.block_n * 128;
     const int tile_bytes = (int)kBlockM * (p.block_n * 4 + 16);   // padded transpose tile for coalesced P2P stores
     int stages = (200 * 1024 - tile_bytes) / stage_bytes;
     if (stages > 6) stages = 6;
     if (stages > std::max(num_kb, 2)) stages = std::max(num_kb, 2);
     p.stages = stages;
-    plan->smem_bytes = stages * stage_bytes + tile_bytes + 1024 + 8 * (2 * stages + 3) + 16;
+    plan->smem_bytes = stages * stage_bytes + tile_bytes + 1024 + 8 * (2 * stages) + 16;
     const int tiles = p.n_tiles_m * p.n_tiles_n;
     plan->grid = tiles < max_ctas ? tiles : max_ctas;
     // small one-shot layers: spend idle SMs on the reduce (helper CTAs split the tile rows)
@@ -541,7 +455,7 @@ cudaError_t launch_fused_wgrad_dp(const FusedDpPlan& plan, cudaStream_t stream) 
         if (e != cudaSuccess) return e;
         configured = true;
     }
-    fused_wgrad_dp_kernel<<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmAlo, plan.tmBlo, plan.p, plan.peers);
+    fused_wgrad_dp_kernel<<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.p, plan.peers);
     return cudaGetLastError();
 }
 cudaError_t fused_dp_configure() {

@@ -1,4 +1,4 @@
-// Host-side launch API of the hand-written sm_100a kernels (no torch dependency, so the
+// Host-side launch API of the hand-written sm_90a kernels (no torch dependency, so the
 // .cu files compile stand-alone with nvcc and the C++ runtime can call them directly).
 #pragma once
 #include <cstdint>
@@ -11,8 +11,8 @@ namespace ssb {
 enum GemmMode : int { GEMM_FWD = 0, GEMM_DGRAD = 1, GEMM_WGRAD = 2 };
 
 // One description for the three Linear GEMMs.  Every GEMM is issued "swapped": the
-// FEATURE dimension sits on the tcgen05 M axis (128 TMEM lanes) and the skinny dimension
-// (micro-batch rows: 4..256) on the N axis, so a 4-row micro-batch costs an N=16 MMA
+// FEATURE dimension sits on the M axis of the 128-row tile and the skinny dimension
+// (micro-batch rows: 4..256) on the N axis, so a 4-row micro-batch costs an N=16 tile
 // instead of a 128-row tile that is 97 % padding.
 //
 //   FWD   D[m=out, n=row] = sum_k W[m,k]  * X[n,k]      A=W   (K-major)  B=X  (K-major)
@@ -20,7 +20,7 @@ enum GemmMode : int { GEMM_FWD = 0, GEMM_DGRAD = 1, GEMM_WGRAD = 2 };
 //   WGRAD D[m=out, n=in ] = sum_k dZ[k,m] * X[k,n]      A=dZ  (MN-major) B=X  (MN-major)
 struct GemmParams {
     int m_total, n_total, k_total;
-    int block_n;        // UMMA N: multiple of 16 (32 when B is MN-major), <= 256
+    int block_n;        // tile N: multiple of 16 (32 when B is MN-major), <= 64
     int stages;         // smem pipeline depth
     // FWD / DGRAD epilogue: out[n * ldo + m]
     float* out;
@@ -42,11 +42,8 @@ struct GemmParams {
     int ldw;
     float lr;
     int fuse_sgd;
-    int acc_split;      // 3xTF32: small cross terms in their own accumulator + rotating main accumulators (ptx.cuh); 0 = one accumulator
-    // fp32-equivalent mode (3xTF32): both operands come with a `lo` twin (x - trunc_tf32(x)); FWD/DGRAD
-    // also emit the lo twin of their output so the next GEMM can consume it
+    // fp32-equivalent mode (3xTF32 products, the operands' lo parts x - trunc_tf32(x) derived in the kernel)
     int split;
-    float* out_lo;
     // split-K (FWD / DGRAD, see gemm_plan_enable_splitk): blockIdx.z owns a k-range, partial tiles go through
     // `partial` [tile][split][block_n][128], the last arriver at tile_counter[tile] reduces + runs the epilogue
     int k_splits;                 // 0 / 1 = off
@@ -56,7 +53,6 @@ struct GemmParams {
 
 struct GemmPlan {          // a fully prepared launch (tensor maps are 128 B each)
     CUtensorMap tmA, tmB, tmC;   // C: WGRAD output tile (G, or W when the SGD update is fused)
-    CUtensorMap tmAlo, tmBlo;    // lo twins of the operands (split mode)
     GemmParams p;
     int mode;
     dim3 grid;
@@ -68,19 +64,15 @@ struct GemmPlan {          // a fully prepared launch (tensor maps are 128 B eac
 //   FWD:   W[out, in] (ldw), X[rows, in] (ldx)            -> Y[rows, out] (ldy)
 //   DGRAD: W[out, in] (ldw), dZ[rows, out] (lddz)         -> dX[rows, in] (lddx)
 //   WGRAD: dZ[rows, out] (lddz), X[rows, in] (ldx)        -> G[out, in] (ldg)
-// *_lo pointers: nullptr = plain TF32; non-null = 3xTF32 (twins share the layout of their tensor)
-struct GemmLo {
-    const float* A = nullptr;   // lo twin of the first operand  (W for fwd/dgrad, dZ for wgrad)
-    const float* B = nullptr;   // lo twin of the second operand (X for fwd, dZ for dgrad, X for wgrad)
-    float* out = nullptr;       // fwd/dgrad: where to write the lo twin of the output
-};
+// split: false = plain TF32 products; true = 3xTF32 (fp32-equivalent; the kernels derive the operands' lo parts
+// x - trunc_tf32(x) from the staged tiles)
 const char* gemm_plan_fwd(GemmPlan* plan, const float* W, int ldw, const float* X, int ldx, float* Y, int ldy,
-                          int rows, int in, int out, const float* bias, int bias_stride, int relu, GemmLo lo = GemmLo());
+                          int rows, int in, int out, const float* bias, int bias_stride, int relu, bool split = false);
 const char* gemm_plan_dgrad(GemmPlan* plan, const float* W, int ldw, const float* dZ, int lddz, float* dX, int lddx,
-                            int rows, int in, int out, const float* mask, int ldmask, GemmLo lo = GemmLo());
+                            int rows, int in, int out, const float* mask, int ldmask, bool split = false);
 const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const float* X, int ldx, float* G, int ldg,
                             int rows, int in, int out, int accumulate, float* db, int db_stride, float* W, int ldw,
-                            float lr, int fuse_sgd, GemmLo lo = GemmLo());
+                            float lr, int fuse_sgd, bool split = false);
 // Split-K for FWD / DGRAD plans whose output has fewer tiles than the chip has SMs (wide, weight-bound layers):
 // choice() returns the number of k-splits (1 = leave the plan alone); enable() rewires the plan (grid.z, ring
 // depth for two CTAs per SM).  workspace: gemm_splitk_workspace_floats() floats; counters: one zeroed uint per tile.
@@ -90,7 +82,7 @@ const char* gemm_plan_enable_splitk(GemmPlan* plan, int k_splits, float* workspa
 cudaError_t gemm_launch(const GemmPlan& plan, cudaStream_t stream);
 // Grouped launch of several WGRAD plans (different layers) as ONE grid: a device table holds one entry per CTA.
 struct alignas(128) GemmGroupEntry {
-    CUtensorMap tmA, tmB, tmC, tmAlo, tmBlo;
+    CUtensorMap tmA, tmB, tmC;
     GemmParams p;
     int bx, by;                    // tile coordinates of this CTA inside its GEMM
 };
@@ -131,13 +123,13 @@ struct DpLayerParams {
     // one NVLink hop instead of two).  Staging is double-buffered by epoch parity (stage_parity_stride).
     int one_shot;
     int64_t stage_parity_stride;
-    int split;                       // 3xTF32: lo twins of dZ / X are loaded too
+    int split;                       // 3xTF32 products (lo parts derived from the staged dZ / X tiles)
     int helpers;                     // CTAs per tile: CTA 0 computes + pushes, all of them share the reduce rows
     int bulk_push;                   // 1: push tiles with cp.async.bulk (TMA engine), 0: coalesced st.global
     unsigned long long* dbg;         // optional: 8 globaltimer stamps of CTA 0 (phase timeline)
 };
 struct FusedDpPlan {
-    CUtensorMap tmA, tmB, tmAlo, tmBlo;
+    CUtensorMap tmA, tmB;
     DpLayerParams p;
     DpPeers peers;
     int grid;
@@ -147,8 +139,7 @@ void dp_layer_geometry(int in, int out, int dp, int* block_n, int* n_tiles_m, in
                        int64_t* slot_floats, int one_shot);
 // dZ == nullptr: plan for dp_reduce_sgd (no GEMM)
 const char* fused_dp_plan(FusedDpPlan* plan, const float* dZ, int lddz, const float* X, int ldx, int rows,
-                          const DpLayerParams& lp, const DpPeers& peers, int max_ctas, const float* dZ_lo = nullptr,
-                          const float* X_lo = nullptr);
+                          const DpLayerParams& lp, const DpPeers& peers, int max_ctas, bool split = false);
 cudaError_t fused_dp_configure();
 cudaError_t launch_fused_wgrad_dp(const FusedDpPlan& plan, cudaStream_t stream);
 cudaError_t launch_dp_reduce_sgd(const FusedDpPlan& plan, cudaStream_t stream);
@@ -156,7 +147,7 @@ cudaError_t launch_bump_epoch(uint32_t* epoch, cudaStream_t stream);
 
 // ---- LL two-shot fused DP path for narrow layers (csrc/kernels/dp_ll.cu): all layers of a stage in ONE launch
 struct DpLLEntry {               // one CTA = one [128 x 32] tile of one layer's weight gradient
-    CUtensorMap tmA, tmB, tmAlo, tmBlo;   // dZ (MN-major A), X (MN-major B) and their lo twins
+    CUtensorMap tmA, tmB;        // dZ (MN-major A), X (MN-major B)
     int m0, n0;                  // tile origin in (out, in)
     int m_total, n_total, k_total;
     int split, has_bias;
@@ -174,13 +165,13 @@ struct DpLLParams {
     const uint32_t* gate_step;   // steps of the launching engine (gate target = gate_mult * *gate_step)
     int n_tiles, stages;
     float* W;                    // local weight arena
-    float* W_lo;                 // optional: lo twins of the weights (3xTF32), refreshed by whoever stores a weight
     uint4* llA[kMaxDp];          // reduce-scatter landing zones  [parity][src][tile][128 / dp rows][17 lines]
     uint4* llC[kMaxDp];          // all-gather landing zones      [parity][tile][128 rows][17 lines]
     unsigned long long* dbg;     // optional phase timeline: 8 globaltimer stamps per tile (first 28 tiles)
 };
 struct DpLLLayer {
-    const float *dZ, *X, *dZ_lo, *X_lo;
+    const float *dZ, *X;
+    int split;                   // 3xTF32 products
     int lddz, ldx, in, out, ldw;
     int64_t w_offset;
     const uint32_t* gate_flag;
@@ -192,7 +183,6 @@ struct DpLLPlan {
     DpLLEntry* entries_dev;
     int grid, smem_bytes;
 };
-int acc_split_default();   // tc_gemm.cu: SSB_ACC_SPLIT (default 1)
 int dp_ll_tiles(int in, int out);
 size_t dp_ll_zone_lines(int dp, int n_tiles);
 const char* dp_ll_plan(DpLLPlan* plan, const DpLLLayer* layers, int n_layers, int rows, const DpLLParams& base);
@@ -209,11 +199,8 @@ struct ChainLayer {
 struct ChainParams {
     int n_layers;
     ChainLayer layers[kChainMaxLayers];
-    const CUtensorMap* maps;         // device array: [2l] W_l K-major (fwd), [2l+1] W_l MN-major (dgrad), [2L] X;
-                                     // split mode: the same 2L+1 maps for the lo twins follow at [2L+1 ..]
+    const CUtensorMap* maps;         // device array: [2l] W_l K-major (fwd), [2l+1] W_l MN-major (dgrad), [2L] X
     int split;                       // 3xTF32 (fp32-equivalent) products
-    float* act_lo[kChainMaxLayers + 1];   // lo twins written next to act / dz (consumed by the wgrad GEMMs)
-    float* dz_lo[kChainMaxLayers + 1];
     const float* W;                  // weight arena (bias reads)
     float* act[kChainMaxLayers + 1]; // act[0] = stage input, act[l] = output of layer l  ([all rows, ld])
     float* dz[kChainMaxLayers + 1];  // dz[l] = gradient w.r.t. the pre-activation of layer l (dz[0]: stage input grad)
@@ -233,7 +220,7 @@ struct ChainParams {
     //    gradients of the next stage for a backward launch) is final in local memory once *in_flag >= *pp_epoch; the
     //    epilogue warps wait for it and stage the tile into shared memory - weights stream in meanwhile;
     //  * x_from_global: forward launch of a stage > 0: the input tile is read from act[0] by the epilogue warps (after the
-    //    flag) instead of by TMA next to layer 1's weights, its lo twin is written to act_lo[0] on the way;
+    //    flag) instead of by TMA next to layer 1's weights;
     //  * out_peer != nullptr: the tile this launch produces for the neighbour (last forward output / dz[0]) is ALSO stored
     //    into the neighbour's receive slot, then one system fence + *out_flag = epoch; *out_credit >= epoch - 1 (the
     //    neighbour released its slots of the previous step) is awaited first.
@@ -243,10 +230,8 @@ struct ChainParams {
     float* out_peer;
     uint32_t* out_flag;
     const uint32_t* out_credit;
-    int acc_split;                   // 3xTF32: launch the instantiation with separate + rotating accumulators for long reductions (SSB_CHAIN_ACC=1)
-    int sync_debug;                  // SSB_RACECHECK=1: an explicit named barrier among the epilogue warps per layer, so that
-                                     // compute-sanitizer's racecheck (which cannot see tcgen05.commit -> mbarrier ordering) can
-                                     // verify the reuse of the activation ping-pong tiles
+    int sync_debug;                  // SSB_RACECHECK=1: one more named barrier among the math warps per layer (racecheck aid
+                                     // for the reuse of the activation ping-pong tiles)
     uint32_t* ready;                 // optional [n_layers + 1] device counters: every epilogue warp of every CTA adds 1 to
                                      // ready[l] once its part of dz[l] (and everything it wrote before) is globally visible
     unsigned long long* dbg;         // optional timeline buffer (3 roles x 256 globaltimer stamps), CTA 0 only
@@ -258,7 +243,7 @@ struct ChainPlan {
 };
 bool chain_eligible(const ChainLayer* layers, int n_layers, int mb_rows, int out_dim, bool has_loss, bool split = false);
 const char* chain_plan(ChainPlan* plan, const ChainParams& params, const float* x, int ldx, int total_rows, int n_mubatches,
-                       const float* W_lo = nullptr, const float* x_lo = nullptr);
+                       bool split = false);
 bool chain_budget(int mb_rows, bool split, int* kps, int* stages, int* smem_bytes);   // host arithmetic only
 void chain_plan_free(ChainPlan* plan);
 cudaError_t chain_configure();
@@ -269,18 +254,15 @@ cudaError_t chain_launch(const ChainPlan& plan, cudaStream_t stream);
 // grad, 1/batch_size inside) and loss_out[0] = sum((t-p)^2)/batch_size.
 cudaError_t launch_loss_head(const float* logits, int ldl, const float* target, int ldt, float* probs, int ldp,
                              float* dlogits, int ldd, float* loss_out, int rows, int cols, float inv_batch,
-                             cudaStream_t stream, int rows_per_mubatch = 0, float* dlogits_lo = nullptr);   // >0: one CTA per micro-batch, loss_out[mu]
+                             cudaStream_t stream, int rows_per_mubatch = 0);   // >0: one CTA per micro-batch, loss_out[mu]
 // generic softmax backward for the functional API: dz = p*up - p*sum(p*up)
 cudaError_t launch_softmax_grad(const float* logits, int ldl, const float* upstream, int ldu, float* dlogits, int ldd,
                                 int rows, int cols, cudaStream_t stream);
 // g[r, c] = y[r, c] > 0 ? g[r, c] : 0   (stage-boundary ReLU backward)
-cudaError_t launch_relu_mask(float* g, int ldg, const float* y, int ldy, int rows, int cols, cudaStream_t stream,
-                             float* g_lo = nullptr);   // g_lo: recomputed lo twin of the masked gradient
+cudaError_t launch_relu_mask(float* g, int ldg, const float* y, int ldy, int rows, int cols, cudaStream_t stream);
 cudaError_t launch_relu_fwd(const float* x, float* y, long n, cudaStream_t stream);
 // y = a * x + b * t  (mse grad: a=2/B, b=-2/B)
 cudaError_t launch_axpby(const float* x, const float* t, float* y, float a, float b, long n, cudaStream_t stream);
-// lo[i] = x[i] - trunc_tf32(x[i]) over a flat buffer (weights after the update, staged inputs)
-cudaError_t launch_split_lo(const float* x, float* lo, long n, cudaStream_t stream);
 // w -= lr * g over a flat arena
 cudaError_t launch_sgd(float* w, const float* g, float lr, long n, cudaStream_t stream);
 // correct[0] += #rows with argmax(pred) == argmax(target)

@@ -4,14 +4,14 @@
 // single launch:   forward L layers -> loss head -> backward (dgrad) L-1 layers.
 //
 //   * activations never leave the SM between layers: the epilogue writes the layer output
-//     into shared memory directly in the swizzled K-major layout tcgen05.mma wants as the
-//     next layer's B operand (and a copy to global for the weight-gradient GEMMs / pipeline);
+//     into shared memory directly in the swizzled K-major layout the next layer's MMAs read
+//     as their B operand (and a copy to global for the weight-gradient GEMMs / pipeline);
 //   * weights are streamed by a producer thread that runs AHEAD of the math through a deep
 //     TMA ring - weight tiles do not depend on activations, so layer l+1's weights are in
 //     flight while layer l is being computed;
-//   * accumulators live in TMEM; fused epilogues: bias + ReLU (forward), softmax + MSE
-//     gradient + softmax Jacobian (loss head, warp shuffles across the class lanes), ReLU
-//     mask (backward).
+//   * accumulators live in the registers of the warp whose epilogue consumes them (mma.sync
+//     TF32, 3xTF32 for fp32-equivalent products); fused epilogues: bias + ReLU (forward),
+//     softmax + MSE gradient + softmax Jacobian (loss head), ReLU mask (backward).
 //
 // This removes ~14 dependent kernel launches (and their prologues / cold starts) from the
 // critical path of the reference workload; the per-layer kernels in tc_gemm.cu remain the
@@ -23,12 +23,14 @@
 
 namespace ssb {
 
-static constexpr int kThreads = 320;                      // 2 control warps + 8 epilogue warps
+static constexpr int kThreads = 288;                      // 1 producer warp + 8 math / epilogue warps
 static constexpr uint32_t kBlockM = 128;
 static constexpr uint32_t kBlockK = 32;
 static constexpr uint32_t kABytes = kBlockM * 128;
 static constexpr uint32_t kPanelBytes = 32 * 128;
 static constexpr int kScratchLd = 33;                     // odd pitch: conflict-free row-per-lane access
+// columns (micro-batch rows) of one math warp: 16 * ceil(N / 32) <= 64
+static int chain_warp_cols(int n_pad) { return 16 * ((n_pad / 16 + 1) / 2); }
 
 __device__ __forceinline__ float warp_sum_f(float v) {
 #pragma unroll
@@ -55,18 +57,12 @@ __device__ __forceinline__ unsigned long long gtime() {
 }
 #define DBG(role, idx) do { if (p.dbg != nullptr && blockIdx.x == 0 && (idx) < 256) p.dbg[(role) * 256 + (idx)] = gtime(); } while (0)
 
-// SPLIT (3xTF32) is a compile-time switch: the single-pass TF32 instantiation carries none of the lo-twin code.
-// (Round 2 also tried deriving the lo twins of the streamed weight tiles in shared memory instead of loading them - half
-// the L2->SM bytes, bit-identical results - but with only 3 ring slots of 40 KB the extra split stage in the slot cycle
-// cost more than the bytes saved: 92.8 vs 78.7 us/step.  Removed; see profiles/variants_r2.md.)
-// FOLD (pipeline boundaries inside the kernel, see ChainParams) is a compile-time switch as well: merely carrying that code
-// - a prologue, two predicated peer stores per element in the epilogues - cost the single-GPU / data-parallel step 8 us
-// (same-box bisect, profiles/variants_r2.md), so launches without a folded boundary use the instantiation without it.
-// ACC (3xTF32 only): separate + rotating accumulators for long reductions (layer 1, K = 784: error 2.9x cuBLAS fp32 instead
-// of 22x, profiles/precision_r2.md).  Compile-time as well, and OFF by default for this kernel: the same one-call, same-box
-// comparison of build variants showed that carrying that code costs 6 us per step (85.0 vs 79.2 us) whether or not it runs.
-// `SSB_CHAIN_ACC=1` selects the accurate instantiation; the per-layer GEMM kernels (wide layers) always use the scheme.
-template <bool SPLIT, bool FOLD, bool ACC>
+// SPLIT (3xTF32) is a compile-time switch: the single-pass TF32 instantiation carries none of the extra products.
+// FOLD (pipeline boundaries inside the kernel, see ChainParams) is a compile-time switch as well: launches without a
+// folded boundary use the instantiation without its prologue and its predicated peer stores.
+// NTW: n8 tiles of a math warp's accumulator (chain_warp_cols / 8, rounded up to 2, 4 or 8) - sized at compile time
+// so that small micro-batches keep their accumulators in a few registers.
+template <bool SPLIT, bool FOLD, int NTW>
 __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
@@ -75,63 +71,38 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int L = p.n_layers;
-    const int N = p.n_pad;                                   // UMMA N (rows of this micro-batch, padded to 16)
+    const int N = p.n_pad;                                   // tile N (rows of this micro-batch, padded to 16)
     const int row0 = (p.mu_base + (int)blockIdx.x) * p.mb_rows;                 // first global row of this micro-batch
     const uint32_t b_bytes = (uint32_t)N * 128u;             // one 32-feature panel of an activation tile
-    const uint32_t half_stage = (uint32_t)p.kps * (kABytes + b_bytes);    // kps A tiles, then kps X tiles (layer 1)
-    const uint32_t stage_bytes = SPLIT ? 2u * half_stage : half_stage;  // split: lo twins in the second half
+    const uint32_t stage_bytes = (uint32_t)p.kps * (kABytes + b_bytes);   // kps A tiles, then kps X tiles (layer 1)
     const uint32_t stage_b_off = (uint32_t)p.kps * kABytes;
     const uint32_t abuf_bytes = 4u * b_bytes;
-    const uint32_t n_abuf = SPLIT ? 4u : 2u;                            // hi ping-pong (+ lo ping-pong)
-    const uint32_t abuf0 = smem_base + p.stages * stage_bytes;
-    const uint32_t lo_off = 2u * abuf_bytes;                              // lo tile of buffer b sits lo_off behind its hi tile
-    const uint32_t bar_base = abuf0 + n_abuf * abuf_bytes;
+    const uint32_t abuf0 = smem_base + p.stages * stage_bytes;            // activation ping-pong
+    const uint32_t bar_base = abuf0 + 2u * abuf_bytes;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
-    const uint32_t tmem_full_bar = bar_base + 8u * (2 * p.stages);
-    const uint32_t act_ready_bar = tmem_full_bar + 8u;
-    const uint32_t tmem_slot = act_ready_bar + 8u;
-    volatile uint32_t* tmem_slot_gen =
-        reinterpret_cast<volatile uint32_t*>(smem_gen + p.stages * stage_bytes + n_abuf * abuf_bytes + 8u * (2 * p.stages + 2));
-    // 3xTF32: up to 4 rotating main accumulators (long reductions only: layer 1) + one for the small cross terms, see ptx.cuh
-    constexpr int kTmemBudget = 512;
-    constexpr bool acc_split = SPLIT && ACC;
-    const int max_rot = acc_split ? acc_rotation(1 << 20, N, kTmemBudget) : 1;
-    uint32_t tmem_cols = 32;
-    while (tmem_cols < (uint32_t)N * (acc_split ? (uint32_t)max_rot + 1u : 1u)) tmem_cols <<= 1;
-    const uint32_t small_off = acc_split ? (uint32_t)N * (uint32_t)max_rot : 0u;
-    // loss-head transpose scratch [N][kScratchLd] floats, behind the barriers (128 B further)
-    const uint32_t scratch_off = p.stages * stage_bytes + n_abuf * abuf_bytes + 8u * (2 * p.stages + 2) + 128u;
+    // loss-head transpose scratch [N][kScratchLd] floats behind the barriers
+    const uint32_t scratch_off = p.stages * stage_bytes + 2u * abuf_bytes + 8u * (2 * p.stages) + 128u;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < p.stages; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 1);
+            mbar_init(empty_bar(s), 8);                      // one arrive per math warp
         }
-        mbar_init(tmem_full_bar, 1);
-        mbar_init(act_ready_bar, 8);                         // one arrive per epilogue warp
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, tmem_cols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
 
     // number of backward GEMMs: layers L..lo (layer 1's dgrad is skipped on the first stage)
     const int bwd_lo = p.first_stage ? 2 : 1;
-    const int lo_base = 2 * L + 1;                           // index of the first lo-twin tensor map
 
     if (warp == 0) {
         // ============================================================ weight (and X) producer
-        // The whole warp walks the loop (converged); one elect.sync-chosen lane issues, so ptxas can
-        // feed the uniform-datapath instructions (UTMALDG) directly instead of an ELECT/BRA.U.ANY loop.
+        // The whole warp walks the loop (converged); one elect.sync-chosen lane issues.  Weight tiles do not depend on
+        // activations, so the ring runs ahead of the math into the next layer.
         {
             int it = 0;
-            auto acquire = [&](uint32_t bytes) {
+            auto acquire = [&]() {
                 const int s = it % p.stages;
                 mbar_wait(empty_bar(s), ((it / p.stages) & 1) ^ 1);
                 return s;
@@ -142,21 +113,15 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     const bool with_x = (l == 1) && !(FOLD && p.x_from_global);   // folded pipeline input: staged by the epilogue warps
                     for (int kb0 = 0; kb0 < nkb; kb0 += p.kps, ++it) {
                         const int cnt = min(p.kps, nkb - kb0);
-                        const int s = acquire(0);
+                        const int s = acquire();
                         const uint32_t a_dst = smem_base + s * stage_bytes;
                         if (elect_one()) {
                             DBG(0, it);
-                            mbar_arrive_expect_tx(full_bar(s), (uint32_t)cnt * (kABytes + (with_x ? b_bytes : 0u)) * (SPLIT ? 2u : 1u));
+                            mbar_arrive_expect_tx(full_bar(s), (uint32_t)cnt * (kABytes + (with_x ? b_bytes : 0u)));
                             for (int j = 0; j < cnt; ++j) {
                                 tma_load_2d(a_dst + j * kABytes, p.maps + 2 * (l - 1), full_bar(s), (kb0 + j) * kBlockK, 0);
                                 if (with_x)
                                     tma_load_2d(a_dst + stage_b_off + j * b_bytes, p.maps + 2 * L, full_bar(s), (kb0 + j) * kBlockK, row0);
-                                if (SPLIT) {
-                                    tma_load_2d(a_dst + half_stage + j * kABytes, p.maps + lo_base + 2 * (l - 1), full_bar(s), (kb0 + j) * kBlockK, 0);
-                                    if (with_x)
-                                        tma_load_2d(a_dst + half_stage + stage_b_off + j * b_bytes, p.maps + lo_base + 2 * L, full_bar(s),
-                                                    (kb0 + j) * kBlockK, row0);
-                                }
                             }
                         }
                         __syncwarp();
@@ -168,20 +133,16 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     const int nkb = (p.layers[l - 1].out + (int)kBlockK - 1) / (int)kBlockK;
                     for (int kb0 = 0; kb0 < nkb; kb0 += p.kps, ++it) {
                         const int cnt = min(p.kps, nkb - kb0);
-                        const int s = acquire(0);
+                        const int s = acquire();
                         const uint32_t a_dst = smem_base + s * stage_bytes;
                         if (elect_one()) {
                             DBG(0, it);
-                            mbar_arrive_expect_tx(full_bar(s), (uint32_t)cnt * kABytes * (SPLIT ? 2u : 1u));
+                            mbar_arrive_expect_tx(full_bar(s), (uint32_t)cnt * kABytes);
                             for (int j = 0; j < cnt; ++j) {
 #pragma unroll
-                                for (int i = 0; i < 4; ++i) {
+                                for (int i = 0; i < 4; ++i)
                                     tma_load_2d(a_dst + j * kABytes + i * kPanelBytes, p.maps + 2 * (l - 1) + 1, full_bar(s), 32 * i,
                                                 (kb0 + j) * kBlockK);
-                                    if (SPLIT)
-                                        tma_load_2d(a_dst + half_stage + j * kABytes + i * kPanelBytes, p.maps + lo_base + 2 * (l - 1) + 1,
-                                                    full_bar(s), 32 * i, (kb0 + j) * kBlockK);
-                                }
                             }
                         }
                         __syncwarp();
@@ -189,121 +150,48 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 }
             }
         }
-    } else if (warp == 1) {
-        // ============================================================ MMA issuer (converged warp, elected lane issues)
-        {
-            int it = 0, act_waits = 0, gemm_i = 0;
-            const uint32_t idesc_f = umma_idesc_tf32(kBlockM, N, 0u, 0u);
-            const uint32_t idesc_b = umma_idesc_tf32(kBlockM, N, 1u, 0u);
-            const uint32_t k_hi = umma_desc_hi(1024u, 2u), mn_hi = umma_desc_hi(512u, 1u);
-            auto run_gemm = [&](int nkb, bool a_mn, bool b_from_stage, uint32_t bsrc) {
-                if (!b_from_stage) {                          // operand tile written by the epilogue warps; their
-                    mbar_wait(act_ready_bar, (act_waits & 1));   // arrive also means the accumulator was drained
-                    ++act_waits;
-                    tc_fence_after();
-                }
-                if (lane == 0) DBG(1, 3 * gemm_i);
-                // only LONG reductions (layer 1 of the first stage: K = 784) use the extra accumulators; the 128-wide layers
-                // keep one accumulator and the lean epilogue (their error is ~4x cuBLAS fp32 already)
-                const bool acc_l = acc_split && nkb >= 8;
-                const int rot = acc_l ? acc_rotation(nkb, N, kTmemBudget) : 1;
-                uint32_t rot_i = 0u;                          // main accumulator of the current k-block (round robin)
-                for (int kb0 = 0; kb0 < nkb; kb0 += p.kps, ++it) {
-                    const int cnt = min(p.kps, nkb - kb0);
-                    const int s = it % p.stages;
-                    mbar_wait(full_bar(s), (it / p.stages) & 1);
-                    tc_fence_after();
-                    if (kb0 + cnt >= nkb && lane == 0) DBG(1, 3 * gemm_i + 1);
-                    const uint32_t a_src = smem_base + s * stage_bytes;
-                    if (elect_one()) {
-                        uint32_t rot_e = rot_i;               // the elected lane's running copy; every lane advances rot_i below
-                        for (int j = 0; j < cnt; ++j) {
-                            const uint32_t a_j = a_src + j * kABytes;
-                            const uint32_t b_j = b_from_stage ? a_src + stage_b_off + j * b_bytes : bsrc + (kb0 + j) * b_bytes;
-                            const uint32_t a_lo = a_mn ? umma_desc_lo(a_j, kPanelBytes) : umma_desc_lo(a_j, 16u);
-                            const uint32_t b_lo = umma_desc_lo(b_j, 16u);
-                            const uint32_t a_step = a_mn ? 64u : 2u;
-                            const uint32_t ah = a_mn ? mn_hi : k_hi, id = a_mn ? idesc_b : idesc_f;
-                            if (SPLIT) {                           // lo*hi + hi*lo + hi*hi (raw tiles are the hi parts)
-                                const uint32_t al_lo = a_lo + (half_stage >> 4);
-                                const uint32_t bl_lo = b_lo + ((b_from_stage ? half_stage : lo_off) >> 4);
-                                if (!acc_l) {
-                                    // short reduction: one accumulator, nothing but the three MMAs in the issue path (this warp sits
-                                    // on the ring's critical cycle: every extra instruction per k-block shows up 73 times per step)
-#pragma unroll
-                                    for (int k4 = 0; k4 < 4; ++k4) {
-                                        umma_tf32(tmem_base, umma_desc_pack(al_lo + k4 * a_step, ah), umma_desc_pack(b_lo + k4 * 2u, k_hi), id,
-                                                  ((kb0 + j) | k4) != 0 ? 1u : 0u);
-                                        umma_tf32(tmem_base, umma_desc_pack(a_lo + k4 * a_step, ah), umma_desc_pack(bl_lo + k4 * 2u, k_hi), id, 1u);
-                                        umma_tf32(tmem_base, umma_desc_pack(a_lo + k4 * a_step, ah), umma_desc_pack(b_lo + k4 * 2u, k_hi), id, 1u);
-                                    }
-                                } else {
-                                    // long reduction: small cross terms in their own accumulator, hi*hi rotating over `rot` accumulators
-                                    const bool first_kb = (kb0 + j) == 0;
-                                    const uint32_t small_acc = tmem_base + small_off;
-                                    const uint32_t main_acc = tmem_base + rot_e * (uint32_t)N;
-                                    const bool main_fresh = (kb0 + j) < rot;   // first product into this main accumulator
-                                    rot_e = (rot_e + 1u == (uint32_t)rot) ? 0u : rot_e + 1u;
-#pragma unroll
-                                    for (int k4 = 0; k4 < 4; ++k4) {
-                                        umma_tf32(small_acc, umma_desc_pack(al_lo + k4 * a_step, ah), umma_desc_pack(b_lo + k4 * 2u, k_hi), id,
-                                                  (first_kb && k4 == 0) ? 0u : 1u);
-                                        umma_tf32(small_acc, umma_desc_pack(a_lo + k4 * a_step, ah), umma_desc_pack(bl_lo + k4 * 2u, k_hi), id, 1u);
-                                        umma_tf32(main_acc, umma_desc_pack(a_lo + k4 * a_step, ah), umma_desc_pack(b_lo + k4 * 2u, k_hi), id,
-                                                  (main_fresh && k4 == 0) ? 0u : 1u);
-                                    }
-                                }
-                            } else
-#pragma unroll
-                            for (int k4 = 0; k4 < 4; ++k4)
-                                umma_tf32(tmem_base, umma_desc_pack(a_lo + k4 * a_step, ah), umma_desc_pack(b_lo + k4 * 2u, k_hi), id,
-                                          ((kb0 + j) | k4) != 0 ? 1u : 0u);
-                        }
-                        umma_commit(empty_bar(s));
-                        if (kb0 + cnt >= nkb) umma_commit(tmem_full_bar);
-                    }
-                    if (acc_l)
-                        for (int j = 0; j < cnt; ++j) rot_i = (rot_i + 1u == (uint32_t)rot) ? 0u : rot_i + 1u;   // all lanes, off the issue path
-                    __syncwarp();
-                }
-                if (lane == 0) DBG(1, 3 * gemm_i + 2);
-                ++gemm_i;
-            };
-            int buf = 0;                                     // activation buffer the NEXT gemm reads
-            if (p.do_fwd) {
-                for (int l = 1; l <= L; ++l) {
-                    const int nkb = (p.layers[l - 1].in + (int)kBlockK - 1) / (int)kBlockK;
-                    // layer 1 reads X from its ring slots (TMA), or - folded pipeline input - from abuf 1 (staged by the epilogue warps)
-                    const bool x_glob = FOLD && (l == 1) && p.x_from_global;
-                    run_gemm(nkb, false, l == 1 && !x_glob, abuf0 + (x_glob ? 1 : buf) * abuf_bytes);
-                    if (l > 1) buf ^= 1;                     // layer l read buf, wrote buf^1
-                    else buf = 0;                            // layer 1 wrote abuf 0
-                }
-            }
-            if (p.do_bwd) {
-                // the loss head / boundary loader wrote dZ_L into the buffer after the last forward output
-                for (int l = L; l >= bwd_lo; --l) {
-                    const int nkb = (p.layers[l - 1].out + (int)kBlockK - 1) / (int)kBlockK;
-                    run_gemm(nkb, true, false, abuf0 + buf * abuf_bytes);
-                    buf ^= 1;
-                }
-            }
-        }
     } else {
-        // ============================================================ epilogue warps
-        const int q = warp & 3;                              // TMEM lane quarter this warp may access
-        const int half = (warp - 2) >> 2;                    // two warps per quarter: each takes half of the columns
-        const int m = q * 32 + lane;                         // feature handled by this thread (TMEM lane)
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
+        // ============================================================ math + epilogue warps
+        // Warp (q, half) owns output features q*32 .. q*32+31 and micro-batch rows [c_lo, c_hi): it runs the tensor-core
+        // MMAs of exactly the block its epilogue consumes, so accumulators never leave the warp's registers (lane r reads
+        // feature row r through warp_acc_row16).  The activation tile of the next GEMM is written by all 8 warps and
+        // published with one named barrier among them.
+        const int q = warp & 3;
+        const int half = (warp - 1) >> 2;
+        const int m = q * 32 + lane;                         // feature handled by this thread in the epilogue
         // column (= row of the micro-batch) range of this warp, in chunks of 16
         const int n_chunks = N / 16;
         const int c_lo = 16 * ((n_chunks * half) / 2), c_hi = 16 * ((n_chunks * (half + 1)) / 2);
-        int tmem_waits = 0;
+        const int nt = (c_hi - c_lo) / 8;
+        float acc[2][NTW][4];                                // this warp's block of the current layer's product
+        int it = 0, gemm_i = 0;
         int wbuf = 0;                                        // activation buffer the NEXT epilogue writes
-        auto st_tile = [&](uint32_t dst, int n, int feat, float x) {   // operand tile(s) for the next GEMM
-            const uint32_t off = (dst - smem_base) + act_smem_off(n, feat, b_bytes);
-            *reinterpret_cast<float*>(smem_gen + off) = x;
-            if (SPLIT) *reinterpret_cast<float*>(smem_gen + off + lo_off) = tf32_lo(x);
+        // D[features, rows] of one layer: A = weights from the ring (K-major forward, MN-major backward), B = the
+        // activation tile (layer 1: X from the ring slots) -> acc
+        auto run_gemm = [&](int nkb, bool a_mn, bool b_from_stage, uint32_t bsrc) {
+            if (threadIdx.x == 32) DBG(1, 2 * gemm_i);
+            warp_acc_zero(acc);
+            for (int kb0 = 0; kb0 < nkb; kb0 += p.kps, ++it) {
+                const int cnt = min(p.kps, nkb - kb0);
+                const int s = it % p.stages;
+                mbar_wait(full_bar(s), (it / p.stages) & 1);
+                const uint32_t a_src = smem_base + s * stage_bytes;
+                for (int j = 0; j < cnt; ++j) {
+                    const uint32_t a_j = a_src + j * kABytes;
+                    const uint32_t b_j = b_from_stage ? a_src + stage_b_off + j * b_bytes : bsrc + (kb0 + j) * b_bytes;
+                    if (a_mn)
+                        warp_mma_kblock<NTW, true, false, SPLIT>(acc, a_j, (uint32_t)q * 32u, b_j, (uint32_t)c_lo, nt, lane);
+                    else
+                        warp_mma_kblock<NTW, false, false, SPLIT>(acc, a_j, (uint32_t)q * 32u, b_j, (uint32_t)c_lo, nt, lane);
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty_bar(s));
+            }
+            if (threadIdx.x == 32) DBG(1, 2 * gemm_i + 1);
+            ++gemm_i;
+        };
+        auto st_tile = [&](uint32_t dst, int n, int feat, float x) {   // operand tile for the next GEMM
+            *reinterpret_cast<float*>(smem_gen + (dst - smem_base) + act_smem_off(n, feat, b_bytes)) = x;
         };
         // dz[l] (and every global store this warp issued before) is complete: one release-add per warp on ready[l]
         // (consumers: the gated weight-gradient / data-parallel kernels running next to this one)
@@ -312,20 +200,18 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             __syncwarp();
             if (lane == 0) red_add_release_gpu(p.ready + l, 1u);
         };
-        auto publish = [&]() {                               // smem tile complete -> MMA warp may read it
-            if (threadIdx.x == 64) DBG(2, 2 * (tmem_waits - 1) + 1);
-            fence_proxy_async_smem();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(act_ready_bar);
+        auto publish = [&]() {                               // smem tile complete -> every math warp may read it
+            if (threadIdx.x == 32) DBG(2, gemm_i);
+            asm volatile("bar.sync 2, 256;" ::: "memory");
         };
+        int buf = 0;                                         // activation buffer the NEXT gemm reads
         // ---------------- folded pipeline boundaries (see ChainParams): credit of the slots we will write, arrival of
-        // the tile we consume.  One thread spins (bounded), a named barrier among the 8 epilogue warps publishes the result.
+        // the tile we consume.  One thread spins (bounded), a named barrier among the 8 math warps publishes the result.
         uint32_t pp_epoch = 0u;
         if constexpr (FOLD) {
         if (p.in_flag != nullptr || p.out_peer != nullptr) {
             pp_epoch = *reinterpret_cast<const volatile uint32_t*>(p.pp_epoch);
-            if (threadIdx.x == 64) {
+            if (threadIdx.x == 32) {
                 if (p.out_peer != nullptr) wait_flag_ge(p.out_credit, pp_epoch - 1u);
                 if (p.in_flag != nullptr) wait_flag_ge(p.in_flag, pp_epoch);
             }
@@ -333,16 +219,14 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         }
         if (p.do_fwd && p.x_from_global) {
             // stage the input tile [rows x in] (written into act[0] by the previous stage over NVLink) as layer 1's B operand
-            // in abuf 1, and its lo twin for the weight-gradient GEMM of layer 1
+            // in abuf 1
             const int in0 = p.layers[0].in;
             const uint32_t dstx = abuf0 + 1u * abuf_bytes;
             const float* __restrict__ xin = p.act[0] + (int64_t)row0 * p.act_ld[0];
             for (int n = c_lo; n < c_hi; ++n) {
                 float x = 0.f;
-                if (m < in0 && n < p.mb_rows) {
+                if (m < in0 && n < p.mb_rows)
                     asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(x) : "l"(xin + (int64_t)n * p.act_ld[0] + m));
-                    if (SPLIT) p.act_lo[0][(int64_t)(row0 + n) * p.act_ld[0] + m] = tf32_lo(x);
-                }
                 st_tile(dstx, n, m, x);
             }
             publish();
@@ -355,12 +239,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 const float bias = m_ok ? __ldg(p.W + ly.w_off + (int64_t)m * ly.ldw + ly.in) : 0.f;
                 const bool is_logits = (l == L) && p.do_loss;
                 const int nkb_f = (ly.in + (int)kBlockK - 1) / (int)kBlockK;
-                const bool acc_f = acc_split && nkb_f >= 8;   // as the MMA warp chose: extra accumulators for long reductions only
-                mbar_wait(tmem_full_bar, tmem_waits & 1);
-                ++tmem_waits;
-                tc_fence_after();
+                // layer 1 reads X from its ring slots (TMA), or - folded pipeline input - from abuf 1 (staged above)
+                const bool x_glob = FOLD && (l == 1) && p.x_from_global;
+                run_gemm(nkb_f, false, l == 1 && !x_glob, abuf0 + (x_glob ? 1 : buf) * abuf_bytes);
+                if (l > 1) buf ^= 1;                         // layer l read buf, wrote buf^1
+                else buf = 0;                                // layer 1 writes abuf 0
                 if (p.sync_debug) asm volatile("bar.sync 2, 256;" ::: "memory");   // racecheck aid, see kernels.h
-                if (threadIdx.x == 64) DBG(2, 2 * (tmem_waits - 1));
                 const uint32_t dst = abuf0 + wbuf * abuf_bytes;
                 float* __restrict__ gout = p.act[l] + (int64_t)row0 * p.act_ld[l];
                 if (!is_logits) {
@@ -368,9 +252,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     // publish it, and only then drain the global copy (needed later by wgrad / the pipeline)
                     const bool single = (c_hi - c_lo == 16);
                     float keep[16];
-                    for (int c = c_lo; c < c_hi; c += 16) {
+#pragma unroll
+                    for (int ch = 0; ch < NTW / 2; ++ch) {
+                        const int c = c_lo + 16 * ch;
+                        if (c >= c_hi) break;
                         float v[16];
-                        if (acc_f) tmem_ld16_acc(taddr + c, small_off, v, acc_rotation(nkb_f, N, kTmemBudget), (uint32_t)N); else tmem_ld16(taddr + c, v);
+                        warp_acc_row16(acc, ch, v, lane);
 #pragma unroll
                         for (int j = 0; j < 16; ++j) {
                             float x = v[j] + bias;
@@ -381,7 +268,6 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                             if (single) keep[j] = x;
                             else if (m_ok && n < p.mb_rows) {
                                 gout[(int64_t)n * p.act_ld[l] + m] = x;
-                                if (SPLIT) p.act_lo[l][(int64_t)(row0 + n) * p.act_ld[l] + m] = tf32_lo(x);
                                 if constexpr (FOLD) { if (l == L && p.out_peer != nullptr) p.out_peer[(int64_t)n * p.act_ld[l] + m] = x; }
                             }
                         }
@@ -392,31 +278,34 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         for (int j = 0; j < 16; ++j)
                             if (c_lo + j < p.mb_rows) {
                                 gout[(int64_t)(c_lo + j) * p.act_ld[l] + m] = keep[j];
-                                if (SPLIT) p.act_lo[l][(int64_t)(row0 + c_lo + j) * p.act_ld[l] + m] = tf32_lo(keep[j]);
                                 if constexpr (FOLD) { if (l == L && p.out_peer != nullptr) p.out_peer[(int64_t)(c_lo + j) * p.act_ld[l] + m] = keep[j]; }
                             }
                     }
                     wbuf ^= 1;
                     if (l == 1) wbuf = 1;                    // layer 1 wrote abuf 0; layer 2 reads 0, writes 1
                 } else {
-                    // ---------------- loss head on the logits tile (class = TMEM lane, row = TMEM column)
+                    // ---------------- loss head on the logits tile (class = feature lane, row = column)
                     // softmax contract of the reference: shift by the GLOBAL max of the micro-batch, +1e-7.
-                    // Step 1: warp q == 0 (the class lanes) transposes logits (+bias) into a [row][class] scratch
-                    // in smem.  Step 2: each lane owns ROWS, loops over the <= 32 classes in registers - no
-                    // cross-lane reductions except one max and one sum for the whole micro-batch.
+                    // Step 1: the class-lane warps (q == 0, both halves) transpose logits (+bias) into a [row][class]
+                    // scratch in smem.  Step 2: each lane of warp (0, 0) owns ROWS, loops over the <= 32 classes in
+                    // registers - no cross-lane reductions except one max and one sum for the whole micro-batch.
                     const int C = ly.out;
                     float* scratch = reinterpret_cast<float*>(smem_gen + scratch_off);   // [N][kScratchLd]
                     float loss = 0.f;
-                    if (q == 0 && half == 0) {
-                        for (int c = 0; c < N; c += 16) {
+                    if (q == 0) {
+#pragma unroll
+                        for (int ch = 0; ch < NTW / 2; ++ch) {
+                            const int c = c_lo + 16 * ch;
+                            if (c >= c_hi) break;
                             float v[16];
-                            if (acc_f) tmem_ld16_acc(taddr + c, small_off, v, acc_rotation(nkb_f, N, kTmemBudget), (uint32_t)N); else tmem_ld16(taddr + c, v);
-                            if (m < C) {
+                            warp_acc_row16(acc, ch, v, lane);
+                            if (m < C)
 #pragma unroll
                                 for (int j = 0; j < 16; ++j) scratch[(c + j) * kScratchLd + m] = v[j] + bias;
-                            }
                         }
-                        __syncwarp();
+                    }
+                    asm volatile("bar.sync 2, 256;" ::: "memory");
+                    if (q == 0 && half == 0) {
                         float gmax = -3.0e38f;
                         for (int n = lane; n < p.mb_rows; n += 32)
                             for (int k = 0; k < C; ++k) gmax = fmaxf(gmax, scratch[n * kScratchLd + k]);
@@ -456,7 +345,6 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                                             gout[(int64_t)n * p.act_ld[l] + k] = zr[k];
                                             p.probs[(int64_t)(row0 + n) * p.ldp + k] = ev[k];
                                             if (p.dz[l] != nullptr) p.dz[l][(int64_t)(row0 + n) * p.act_ld[l] + k] = dzv;
-                                            if (SPLIT && p.dz_lo[l] != nullptr) p.dz_lo[l][(int64_t)(row0 + n) * p.act_ld[l] + k] = tf32_lo(dzv);
                                         }
                                         if (p.do_bwd) st_tile(dst, n, k, dzv);
                                     }
@@ -480,7 +368,6 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                                         gout[(int64_t)n * p.act_ld[l] + k] = zr[k];
                                         p.probs[(int64_t)(row0 + n) * p.ldp + k] = pr;
                                         if (p.dz[l] != nullptr) p.dz[l][(int64_t)(row0 + n) * p.act_ld[l] + k] = dzv;
-                                        if (SPLIT && p.dz_lo[l] != nullptr) p.dz_lo[l][(int64_t)(row0 + n) * p.act_ld[l] + k] = tf32_lo(dzv);
                                     }
                                     if (p.do_bwd) st_tile(dst, n, k, dzv);
                                 }
@@ -502,7 +389,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         if (FOLD && p.do_fwd && !p.do_bwd && p.out_peer != nullptr) {
             // the stage's output tile is in the next stage's receive slot: one fence, then its arrival flag
             asm volatile("bar.sync 2, 256;" ::: "memory");
-            if (threadIdx.x == 64) {
+            if (threadIdx.x == 32) {
                 __threadfence_system();
                 st_relaxed_sys(p.out_flag, pp_epoch);
             }
@@ -520,7 +407,6 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(x) : "l"(g + (int64_t)n * p.act_ld[L] + m));   // may be peer-written
                     if (ly.relu && !(y[(int64_t)n * p.act_ld[L] + m] > 0.f)) x = 0.f;
                     g[(int64_t)n * p.act_ld[L] + m] = x;     // the wgrad GEMM reads the masked gradient
-                    if (SPLIT) p.dz_lo[L][(int64_t)(row0 + n) * p.act_ld[L] + m] = tf32_lo(x);
                 }
                 st_tile(dst, n, m, x);
             }
@@ -528,13 +414,14 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             wbuf ^= 1;
         }
         if (p.do_bwd) {
+            // the loss head / boundary loader wrote dZ_L into the buffer after the last forward output
             for (int l = L; l >= bwd_lo; --l) {
                 const ChainLayer& ly = p.layers[l - 1];
                 const bool m_ok = m < ly.in;                 // output feature of dgrad = input feature of layer l
                 const bool mask_on = (l >= 2) && p.layers[l - 2].relu;
                 const float* __restrict__ yprev = p.act[l - 1] + (int64_t)row0 * p.act_ld[l - 1];
                 float* __restrict__ gprev = p.dz[l - 1] + (int64_t)row0 * p.act_ld[l - 1];
-                // the masks do not depend on the MMA: fetch them while it runs (N <= 32: all of them)
+                // the masks do not depend on the MMA: fetch them before it runs (N <= 32: all of them)
                 float mk0[16];
                 const bool pre = (c_hi - c_lo == 16);        // N <= 32: one chunk per warp, prefetch its masks
                 if (pre) {
@@ -542,16 +429,20 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     for (int j = 0; j < 16; ++j)
                         mk0[j] = (mask_on && m_ok && c_lo + j < p.mb_rows) ? yprev[(int64_t)(c_lo + j) * p.act_ld[l - 1] + m] : 1.f;
                 }
-                mbar_wait(tmem_full_bar, tmem_waits & 1);
-                ++tmem_waits;
-                tc_fence_after();
+                const int nkb = (ly.out + (int)kBlockK - 1) / (int)kBlockK;
+                run_gemm(nkb, true, false, abuf0 + buf * abuf_bytes);
+                buf ^= 1;
                 if (p.sync_debug) asm volatile("bar.sync 2, 256;" ::: "memory");   // racecheck aid, see kernels.h
-                if (threadIdx.x == 64) DBG(2, 2 * (tmem_waits - 1));
                 const uint32_t dst = abuf0 + wbuf * abuf_bytes;
                 const bool more = (l > bwd_lo);              // another dgrad consumes this tile
                 const bool single = (c_hi - c_lo == 16);
                 float keep[16];
-                for (int c = c_lo; c < c_hi; c += 16) {
+#pragma unroll
+                for (int ch = 0; ch < NTW / 2; ++ch) {
+                    const int c = c_lo + 16 * ch;
+                    if (c >= c_hi) break;
+                    float v[16];
+                    warp_acc_row16(acc, ch, v, lane);
                     float mk[16];
 #pragma unroll
                     for (int j = 0; j < 16; ++j) {
@@ -559,8 +450,6 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         if (pre) mk[j] = mk0[j];
                         else mk[j] = (mask_on && m_ok && n < p.mb_rows) ? yprev[(int64_t)n * p.act_ld[l - 1] + m] : 1.f;
                     }
-                    float v[16];
-                    tmem_ld16(taddr + c, v);   // backward reductions run over <= 128 output features: one accumulator
 #pragma unroll
                     for (int j = 0; j < 16; ++j) {
                         const int n = c + j;
@@ -570,7 +459,6 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         if (single) keep[j] = x;
                         else if (m_ok && n < p.mb_rows) {
                             gprev[(int64_t)n * p.act_ld[l - 1] + m] = x;
-                            if (SPLIT) p.dz_lo[l - 1][(int64_t)(row0 + n) * p.act_ld[l - 1] + m] = tf32_lo(x);
                             if constexpr (FOLD) { if (l == 1 && p.out_peer != nullptr) p.out_peer[(int64_t)n * p.act_ld[0] + m] = x; }
                         }
                     }
@@ -584,7 +472,6 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     for (int j = 0; j < 16; ++j)
                         if (c_lo + j < p.mb_rows) {
                             gprev[(int64_t)(c_lo + j) * p.act_ld[l - 1] + m] = keep[j];
-                            if (SPLIT) p.dz_lo[l - 1][(int64_t)(row0 + c_lo + j) * p.act_ld[l - 1] + m] = tf32_lo(keep[j]);
                             if constexpr (FOLD) { if (l == 1 && p.out_peer != nullptr) p.out_peer[(int64_t)(c_lo + j) * p.act_ld[0] + m] = keep[j]; }
                         }
                 }
@@ -593,18 +480,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             if (FOLD && p.out_peer != nullptr && !p.first_stage) {
                 // dz[0] is in the previous stage's receive slot: one fence, then its arrival flag
                 asm volatile("bar.sync 2, 256;" ::: "memory");
-                if (threadIdx.x == 64) {
+                if (threadIdx.x == 32) {
                     __threadfence_system();
                     st_relaxed_sys(p.out_flag, pp_epoch);
                 }
             }
         }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, tmem_cols);
     }
 }
 
@@ -614,14 +495,17 @@ const char* make_tmap_k(CUtensorMap* map, const float* base, int inner, int oute
 
 // Shared-memory plan of the chain kernel for one micro-batch size: k-panels per ring stage, ring depth, total bytes.
 // Pure host arithmetic (no CUDA calls) so it can be unit-tested without a GPU (tests/test_planning.py).
+// `split` (3xTF32) needs no extra shared memory: the lo parts are derived from the staged tiles.
 bool chain_budget(int mb_rows, bool split, int* kps_out, int* stages_out, int* smem_bytes_out) {
+    (void)split;
+    if (mb_rows < 1 || mb_rows > 128) return false;
     const int n_pad = (mb_rows + 15) / 16 * 16;
     const int abuf_bytes = 4 * n_pad * 128;
-    const int scratch_bytes = n_pad * kScratchLd * 4 + 256;
-    const int budget = 222 * 1024 - (split ? 4 : 2) * abuf_bytes - scratch_bytes;
+    const int scratch_bytes = n_pad * kScratchLd * 4 + 256;   // loss head
+    const int budget = 222 * 1024 - 2 * abuf_bytes - scratch_bytes;
     int kps = 4, stage_bytes = 0, stages = 0;
     for (; kps >= 1; kps >>= 1) {            // biggest stage (fewest waits/commits) that still double-buffers
-        stage_bytes = kps * ((int)kABytes + n_pad * 128) * (split ? 2 : 1);
+        stage_bytes = kps * ((int)kABytes + n_pad * 128);
         stages = budget / stage_bytes;
         if (stages >= 2) break;
     }
@@ -629,7 +513,7 @@ bool chain_budget(int mb_rows, bool split, int* kps_out, int* stages_out, int* s
     if (stages > 8) stages = 8;
     *kps_out = kps;
     *stages_out = stages;
-    *smem_bytes_out = stages * stage_bytes + (split ? 4 : 2) * abuf_bytes + 1024 + 8 * (2 * stages + 3) + 16 + scratch_bytes;
+    *smem_bytes_out = stages * stage_bytes + 2 * abuf_bytes + 1024 + 8 * (2 * stages) + 128 + scratch_bytes;
     return true;
 }
 
@@ -650,29 +534,23 @@ bool chain_eligible(const ChainLayer* layers, int n_layers, int mb_rows, int out
 }
 
 const char* chain_plan(ChainPlan* plan, const ChainParams& params, const float* x, int ldx, int total_rows, int n_mubatches,
-                       const float* W_lo, const float* x_lo) {
+                       bool split) {
     *plan = ChainPlan{};
     ChainParams& p = plan->p;
     p = params;
     const int L = p.n_layers;
     p.n_pad = (p.mb_rows + 15) / 16 * 16;
-    p.split = (W_lo != nullptr) ? 1 : 0;
-    const int nmaps = 2 * L + 1;
-    const int halves = p.split ? 2 : 1;
-    std::vector<CUtensorMap> host(nmaps * halves);
-    for (int half = 0; half < halves; ++half) {
-        const float* Wb = half ? W_lo : p.W;
-        const float* xb = half ? x_lo : x;
-        for (int l = 0; l < L; ++l) {
-            const ChainLayer& ly = p.layers[l];
-            if (const char* e = make_tmap_k(&host[half * nmaps + 2 * l], Wb + ly.w_off, ly.in, ly.out, ly.ldw, kBlockM)) return e;
-            if (const char* e = make_tmap_mn(&host[half * nmaps + 2 * l + 1], Wb + ly.w_off, ly.in, ly.out, ly.ldw)) return e;
-        }
-        if (xb != nullptr) {
-            if (const char* e = make_tmap_k(&host[half * nmaps + 2 * L], xb, p.layers[0].in, total_rows, ldx, p.n_pad)) return e;
-        } else {
-            host[half * nmaps + 2 * L] = host[half * nmaps];
-        }
+    p.split = split ? 1 : 0;                      // 3xTF32: the kernel derives the lo parts of its operands from the staged tiles
+    std::vector<CUtensorMap> host(2 * L + 1);
+    for (int l = 0; l < L; ++l) {
+        const ChainLayer& ly = p.layers[l];
+        if (const char* e = make_tmap_k(&host[2 * l], p.W + ly.w_off, ly.in, ly.out, ly.ldw, kBlockM)) return e;
+        if (const char* e = make_tmap_mn(&host[2 * l + 1], p.W + ly.w_off, ly.in, ly.out, ly.ldw)) return e;
+    }
+    if (x != nullptr) {
+        if (const char* e = make_tmap_k(&host[2 * L], x, p.layers[0].in, total_rows, ldx, p.n_pad)) return e;
+    } else {
+        host[2 * L] = host[0];
     }
     CUtensorMap* dev = nullptr;
     if (cudaMalloc(&dev, host.size() * sizeof(CUtensorMap)) != cudaSuccess) return "chain_plan: cudaMalloc failed";
@@ -694,34 +572,42 @@ void chain_plan_free(ChainPlan* plan) {
     plan->maps_dev = nullptr;
 }
 
-template <bool SPLIT, bool FOLD, bool ACC>
-static cudaError_t chain_configure_one() {
-    return cudaFuncSetAttribute(mlp_chain_kernel<SPLIT, FOLD, ACC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+template <int NTW>
+static cudaError_t chain_configure_ntw() {
+    cudaError_t e;
+    const int smem = 227 * 1024;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, true, NTW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    return cudaFuncSetAttribute(mlp_chain_kernel<true, true, NTW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
 }
 
 cudaError_t chain_configure() {
     cudaError_t e;
-    if ((e = chain_configure_one<false, false, false>()) != cudaSuccess) return e;
-    if ((e = chain_configure_one<false, true, false>()) != cudaSuccess) return e;
-    if ((e = chain_configure_one<true, false, false>()) != cudaSuccess) return e;
-    if ((e = chain_configure_one<true, true, false>()) != cudaSuccess) return e;
-    if ((e = chain_configure_one<true, false, true>()) != cudaSuccess) return e;
-    return chain_configure_one<true, true, true>();
+    if ((e = chain_configure_ntw<2>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<4>()) != cudaSuccess) return e;
+    return chain_configure_ntw<8>();
+}
+
+template <int NTW>
+static void chain_launch_ntw(const ChainPlan& plan, bool fold, cudaStream_t stream) {
+    const ChainParams& p = plan.p;
+#define SSB_CHAIN_LAUNCH(S, F) mlp_chain_kernel<S, F, NTW><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(p)
+    if (!p.split) {
+        if (fold) SSB_CHAIN_LAUNCH(false, true); else SSB_CHAIN_LAUNCH(false, false);
+    } else {
+        if (fold) SSB_CHAIN_LAUNCH(true, true); else SSB_CHAIN_LAUNCH(true, false);
+    }
+#undef SSB_CHAIN_LAUNCH
 }
 
 cudaError_t chain_launch(const ChainPlan& plan, cudaStream_t stream) {
     const ChainParams& p = plan.p;
     const bool fold = p.in_flag != nullptr || p.out_peer != nullptr || p.x_from_global != 0;
-    const bool acc = p.split && p.acc_split != 0;
-#define SSB_CHAIN_LAUNCH(S, F, A) mlp_chain_kernel<S, F, A><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(p)
-    if (!p.split) {
-        if (fold) SSB_CHAIN_LAUNCH(false, true, false); else SSB_CHAIN_LAUNCH(false, false, false);
-    } else if (!acc) {
-        if (fold) SSB_CHAIN_LAUNCH(true, true, false); else SSB_CHAIN_LAUNCH(true, false, false);
-    } else {
-        if (fold) SSB_CHAIN_LAUNCH(true, true, true); else SSB_CHAIN_LAUNCH(true, false, true);
-    }
-#undef SSB_CHAIN_LAUNCH
+    const int cols = chain_warp_cols(p.n_pad);
+    if (cols <= 16) chain_launch_ntw<2>(plan, fold, stream);
+    else if (cols <= 32) chain_launch_ntw<4>(plan, fold, stream);
+    else chain_launch_ntw<8>(plan, fold, stream);
     return cudaGetLastError();
 }
 

@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05
-// (alloc / mma / commit / ld / fences) and system-scope flag ops for peer-memory
-// protocols.  Nothing here is generic CUDA C++ - this file only compiles for sm_100a.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), warp-level TF32
+// tensor-core tiles fed from swizzled shared memory, and system-scope flag ops for peer-memory
+// protocols.  Nothing here is generic CUDA C++ - this file only compiles for sm_90a.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -91,160 +91,144 @@ __device__ __forceinline__ void bulk_copy_s2g(void* gdst, uint32_t smem_src, uin
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-// make generic-proxy smem writes visible to the async proxy (TMA / tcgen05 operand reads)
+// make generic-proxy smem writes visible to the async proxy (TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ------------------------------------------------------------------ tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_slot, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_slot), "r"(ncols)
-                 : "memory");
+// ------------------------------------------------------------------ warp-level TF32 tensor-core tiles
+// Every operand tile in shared memory is made of 128-byte rows (32 fp32) in the TMA SWIZZLE_128B layout: the 16-byte
+// chunk index of an element is XOR-ed with (row & 7), rows 128 B apart, tile base 1024 B aligned.
+//   K-major  tile [mn rows x 32 k]                     : element (mn, k) in row mn
+//   MN-major tile = panels of [32 k-rows x 32 mn] (4 KB): element (mn, k) in row k of panel mn / 32
+__device__ __forceinline__ uint32_t sw128_off(uint32_t row, uint32_t col) {
+    return row * 128u + ((((col >> 2) ^ row) & 7u) << 4) + ((col & 3u) << 2);
 }
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+template <bool MN>
+__device__ __forceinline__ uint32_t operand_off(uint32_t mn, uint32_t k) {
+    return MN ? (mn >> 5) * 4096u + sw128_off(k, mn & 31u) : sw128_off(mn, k);
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// not volatile: the loads may be scheduled across the (register-only) mma.sync; the memory clobber keeps them behind
+// the mbarrier waits that make the tiles valid
+__device__ __forceinline__ float lds_f32(uint32_t addr) {
+    float v;
+    asm("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+    return v;
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], TF32 inputs, FP32 accumulate, one CTA.
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread retired
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-                 : "memory");
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+                 "{%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
+// 3xTF32: x = hi + lo with hi = trunc_tf32(x) (the top 19 bits) and lo = x - hi exact in fp32, so
+// a*b ~= lo_a*hi_b + hi_a*lo_b + hi_a*hi_b  (error ~2^-20 relative).  The hi operand is truncated explicitly, so the
+// split does not depend on how the tensor core treats the low 13 mantissa bits of its inputs.
+__device__ __forceinline__ uint32_t tf32_hi_bits(float x) { return __float_as_uint(x) & 0xFFFFE000u; }
 
-// 3xTF32 keeps TWO accumulators per tile: the hi*hi products go to the main one, the two small cross terms (lo*hi,
-// hi*lo; 2^-11 of the result) to a second one `small_off` columns further.  The tensor core's accumulate step truncates
-// (measured: error grows linearly with the number of accumulate steps, ~0.7 * n * 2^-24 relative), so keeping the small
-// terms out of the main chain cuts the steps that matter by 3x; the two are added here in fp32 (round to nearest).
-// small_off == 0: single accumulator (TF32 mode).
-// two accumulators, both loads in flight before ONE wait (the common 3xTF32 case: one main accumulator + the small one)
-__device__ __forceinline__ void tmem_ld16_pair(uint32_t taddr, uint32_t small_off, float (&v)[16]) {
-    uint32_t r[16], w[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]),
-          "=r"(w[8]), "=r"(w[9]), "=r"(w[10]), "=r"(w[11]), "=r"(w[12]), "=r"(w[13]), "=r"(w[14]), "=r"(w[15])
-        : "r"(taddr + small_off)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// One warp: D[32 x 8*nt] += A[m_base .. m_base+31, one 32-wide k-block] * B[n_base .. n_base+8*nt-1, same k-block]^T,
+// both operands read from swizzled tiles (operand_off).  The k-block's products are summed into a fresh tensor-core
+// accumulator and then added to `acc` with an fp32 add, so the accumulated rounding error grows with the number of
+// 32-wide k-blocks, not with the number of MMA steps.  SPLIT: 3xTF32 products, the lo parts derived from the tile.
+// acc[i][j][r]: m16 tile i, n8 tile j, mma.sync C fragment register r (rows lane/4 (+8), columns 2*(lane%4) (+1)).
+template <int NT, bool A_MN, bool B_MN, bool SPLIT>
+__device__ __forceinline__ void warp_mma_kblock(float (&acc)[2][NT][4], uint32_t a_tile, uint32_t m_base, uint32_t b_tile,
+                                                uint32_t n_base, int nt, int lane) {
+    const uint32_t g = (uint32_t)lane >> 2, t = (uint32_t)lane & 3u;
+    float part[2][NT][4];
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]) + __uint_as_float(w[i]);
-}
-// Long reductions additionally rotate the hi*hi products of successive k-blocks over `n_main` main accumulators
-// (`main_stride` columns apart): each chain is n_main times shorter; the partial sums are added here.
-__device__ __forceinline__ void tmem_ld16_acc(uint32_t taddr, uint32_t small_off, float (&v)[16], int n_main = 1, uint32_t main_stride = 0u) {
-    tmem_ld16(taddr, v);
-    for (int r = 1; r < n_main; ++r) {
-        float w[16];
-        tmem_ld16(taddr + (uint32_t)r * main_stride, w);
+    for (int i = 0; i < 2; ++i)
 #pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] += w[i];
+        for (int j = 0; j < NT; ++j)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) part[i][j][r] = 0.f;
+#pragma unroll
+    for (uint32_t k0 = 0; k0 < 32u; k0 += 8u) {
+        uint32_t ah[2][4], al[2][4];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const uint32_t r0 = m_base + 16u * i + g;
+            const float x[4] = {lds_f32(a_tile + operand_off<A_MN>(r0, k0 + t)), lds_f32(a_tile + operand_off<A_MN>(r0 + 8u, k0 + t)),
+                                lds_f32(a_tile + operand_off<A_MN>(r0, k0 + t + 4u)),
+                                lds_f32(a_tile + operand_off<A_MN>(r0 + 8u, k0 + t + 4u))};
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                ah[i][r] = tf32_hi_bits(x[r]);
+                al[i][r] = __float_as_uint(x[r] - __uint_as_float(ah[i][r]));
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < NT; ++j) {
+            if (j < nt) {
+                const uint32_t n = n_base + 8u * j + g;
+                const float y0 = lds_f32(b_tile + operand_off<B_MN>(n, k0 + t));
+                const float y1 = lds_f32(b_tile + operand_off<B_MN>(n, k0 + t + 4u));
+                const uint32_t bh0 = tf32_hi_bits(y0), bh1 = tf32_hi_bits(y1);
+                const uint32_t bl0 = __float_as_uint(y0 - __uint_as_float(bh0)), bl1 = __float_as_uint(y1 - __uint_as_float(bh1));
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    if (SPLIT) {
+                        mma_tf32(part[i][j], al[i], bh0, bh1);
+                        mma_tf32(part[i][j], ah[i], bl0, bl1);
+                    }
+                    mma_tf32(part[i][j], ah[i], bh0, bh1);
+                }
+            }
+        }
     }
-    if (small_off != 0u) {
-        float w[16];
-        tmem_ld16(taddr + small_off, w);
 #pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] += w[i];
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < NT; ++j)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) acc[i][j][r] += part[i][j][r];
+}
+
+template <int NT>
+__device__ __forceinline__ void warp_acc_zero(float (&acc)[2][NT][4]) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < NT; ++j)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) acc[i][j][r] = 0.f;
+}
+
+// Lane r receives row r of the warp's 32-row block, columns 16*ch .. 16*ch+15, straight from the accumulator fragments
+// (warp shuffles, no shared memory).  Every lane of the warp must call it; ch must be a compile-time constant after
+// unrolling, so that the fragments stay in registers.
+template <int NT>
+__device__ __forceinline__ void warp_acc_row16(const float (&acc)[2][NT][4], int ch, float (&v)[16], int lane) {
+    const int src_g = lane & 7, hi_tile = lane >> 4, hi_row = (lane >> 3) & 1;
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+        const int j = 2 * ch + (c >> 3), src = src_g * 4 + ((c & 7) >> 1), e = c & 1;
+        const float a0 = __shfl_sync(0xffffffffu, acc[0][j][e], src);
+        const float a1 = __shfl_sync(0xffffffffu, acc[0][j][2 + e], src);
+        const float a2 = __shfl_sync(0xffffffffu, acc[1][j][e], src);
+        const float a3 = __shfl_sync(0xffffffffu, acc[1][j][2 + e], src);
+        v[c] = hi_tile ? (hi_row ? a3 : a2) : (hi_row ? a1 : a0);
     }
 }
-// how many main accumulators a reduction over `nkb` k-blocks of a tile with `n_cols` columns uses inside a budget of
-// `budget_cols` TMEM columns (one more accumulator of the same width holds the small terms)
-__host__ __device__ __forceinline__ int acc_rotation(int nkb, int n_cols, int budget_cols) {
-    if (nkb < 8) return 1;
-    int r = budget_cols / n_cols - 1;
-    return r < 1 ? 1 : (r > 4 ? 4 : r);
-}
 
-// ------------------------------------------------------------------ UMMA descriptors
-// Shared-memory matrix descriptor, SWIZZLE_128B (layout_type 2), Blackwell version 1.
-//   K-major  operand tile [rows x 32 fp32]: rows are 128 B apart, 8-row groups 1024 B apart
-//            -> SBO = 1024 B, LBO unused.
-//   MN-major operand tile = panels of [32 k-rows x 32 fp32 (128 B)]: 8-k-row groups are
-//            1024 B apart (SBO), successive 32-wide MN panels are `panel_bytes` apart (LBO).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= static_cast<uint64_t>(1) << 46;   // descriptor version (Blackwell)
-    d |= static_cast<uint64_t>(2) << 61;   // SWIZZLE_128B
-    return d;
-}
-// MN-major 32-bit operands: SWIZZLE_128B_BASE32B (layout type 1): atoms of 4 k-rows x 128 B,
-// XOR on 32-byte chunks.  LBO = distance between 32-wide MN panels, SBO = distance between
-// 4-k-row atoms (512 B when k-rows are contiguous).
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128_32b(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= static_cast<uint64_t>(1) << 46;   // descriptor version (Blackwell)
-    d |= static_cast<uint64_t>(1) << 61;   // SWIZZLE_128B_BASE32B
-    return d;
-}
-// Descriptor = (hi << 32) | lo.  Within one k-block only the start address (lo[13:0]) moves, so the
-// issue loop builds lo/hi once and then steps lo by a constant - the uniform datapath that feeds
-// UTCHMMA is slow (each dependent op ~10+ cycles), so every op removed from the issue loop counts.
-__device__ __forceinline__ uint32_t umma_desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
-    return ((smem_addr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
-}
-__device__ __forceinline__ uint32_t umma_desc_hi(uint32_t sbo_bytes, uint32_t layout_type) {
-    return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14) | (layout_type << 29);
-}
-__device__ __forceinline__ uint64_t umma_desc_pack(uint32_t lo, uint32_t hi) {
-    return (static_cast<uint64_t>(hi) << 32) | lo;
-}
-// Instruction descriptor for kind::tf32, fp32 accumulate, M x N tile.
-__device__ __forceinline__ uint32_t umma_idesc_tf32(uint32_t M, uint32_t N, uint32_t a_mn_major, uint32_t b_mn_major) {
-    return (1u << 4)                 // D format  = F32
-           | (2u << 7)               // A format  = TF32
-           | (2u << 10)              // B format  = TF32
-           | (a_mn_major << 15) | (b_mn_major << 16)
-           | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-// ------------------------------------------------------------------ 3xTF32 operand splitting
-// tcgen05.mma.kind::tf32 TRUNCATES the low 13 mantissa bits of its fp32 operands (measured on
-// B200: 1+2^-11+2^-12 -> 1, 1+2^-10-2^-23 -> 1, sign-symmetric).  So the raw fp32 tile is the exact
-// "hi" operand trunc(x), and lo = x - trunc(x) (exact in fp32) is the only extra tensor needed for
-// an fp32-equivalent product  a*b ~= lo_a*hi_b + hi_a*lo_b + hi_a*hi_b  (error ~2^-20 relative).
-__device__ __forceinline__ float tf32_lo(float x) {
-    return x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
+// Accumulator fragments -> a per-warp row-major scratch [32 rows][ld] (ld odd: conflict-free row-per-lane reads), so that
+// afterwards lane r reads row r of the warp's block: scratch[lane * ld + column].
+template <int NT>
+__device__ __forceinline__ void warp_acc_to_rows(const float (&acc)[2][NT][4], float* scratch, int ld, int nt, int lane) {
+    const int g = lane >> 2, t = lane & 3;
+    __syncwarp();   // the previous readers of the scratch are done
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < NT; ++j) {
+            if (j < nt) {
+                float* r0 = scratch + (16 * i + g) * ld + 8 * j + 2 * t;
+                r0[0] = acc[i][j][0];
+                r0[1] = acc[i][j][1];
+                r0[8 * ld] = acc[i][j][2];
+                r0[8 * ld + 1] = acc[i][j][3];
+            }
+        }
+    __syncwarp();
 }
 
 // ------------------------------------------------------------------ system-scope flags (peer memory)

@@ -1,18 +1,16 @@
-// tcgen05 / TMEM / TMA GEMM family for the Linear layer (SURVEY.md K1, K2, K3, K6, K7).
+// TMA + mbarrier + tensor-core GEMM family for the Linear layer (SURVEY.md K1, K2, K3, K6, K7).
 //
 // One warp-specialised kernel, three instantiations (see GemmMode in kernels.h):
 //   warp 0    : TMA producer  - cp.async.bulk.tensor tiles (SWIZZLE_128B) into a ring of smem stages
-//   warp 1    : MMA issuer    - one thread issues tcgen05.mma.kind::tf32 (fp32 data, fp32 accumulate
-//                               in TMEM); tcgen05.commit releases smem stages / signals the epilogue
-//   warps 2-5 : epilogue      - tcgen05.ld TMEM -> registers, fused bias / ReLU / ReLU-mask /
-//                               grad-accumulate / SGD, coalesced global stores.  During the WGRAD
-//                               main loop these warps also reduce db = colsum(dZ) straight from the
-//                               staged A tiles in shared memory (exact fp32, no extra pass over dZ).
+//   warps 1-4 : math + epilogue - each warp owns 32 rows of the 128-row tile: mma.sync TF32 (fp32 data, fp32
+//                               accumulate in registers, 3xTF32 for fp32-equivalent products) straight from the
+//                               swizzled stages, then fused bias / ReLU / ReLU-mask / grad-accumulate / SGD and
+//                               coalesced global stores.  During the WGRAD main loop these warps also reduce
+//                               db = colsum(dZ) from the staged A tiles (exact fp32, no extra pass over dZ).
 //
 // Operand staging (all tiles are 32 fp32 = 128 B wide, the SWIZZLE_128B span):
-//   K-major  tile: one TMA box [rows x 32 k]           -> 8-row groups 1024 B apart (SBO)
-//   MN-major tile: panels of  [32 k-rows x 32 mn]      -> 4096 B per panel (LBO), 4-k-row atoms 512 B (SBO);
-//                  32-bit MN-major operands require the SWIZZLE_128B_BASE32B flavour (TMA: 128B_ATOM_32B)
+//   K-major  tile: one TMA box [rows x 32 k]                       -> rows 128 B apart
+//   MN-major tile: panels of  [32 k-rows x 32 mn], 4096 B per panel -> k-rows 128 B apart
 // Ragged edges are handled by TMA out-of-bounds zero fill, so no dimension needs padding
 // beyond the 16-byte row pitch rule (the reference model's 127/126/125/123-wide layers).
 #include "kernels.h"
@@ -26,8 +24,9 @@
 
 namespace ssb {
 
-static constexpr int kThreads = 192;
+static constexpr int kThreads = 160;
 static constexpr uint32_t kBlockM = 128;
+static constexpr int kMaxBlockN = 64;                   // a math warp holds a 32 x block_n fp32 accumulator in registers
 static constexpr uint32_t kBlockK = 32;                 // fp32 elements = 128 B
 static constexpr uint32_t kABytes = kBlockM * 128;      // 16 KB per stage
 static constexpr uint32_t kPanelBytes = 32 * 128;       // MN-major panel: 32 k-rows x 128 B
@@ -40,8 +39,7 @@ static constexpr uint32_t kPanelBytes = 32 * 128;       // MN-major panel: 32 k-
 // layers' tiles in ONE launch, tensor maps and parameters read from a device table).
 template <int MODE, bool SPLITK>
 __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
-                                             const CUtensorMap& tmAlo, const CUtensorMap& tmBlo, const GemmParams& p, const int bx,
-                                             const int by, const int bz) {
+                                             const GemmParams& p, const int bx, const int by, const int bz) {
     constexpr bool A_MN = (MODE != GEMM_FWD);
     constexpr bool B_MN = (MODE == GEMM_WGRAD);
 
@@ -60,27 +58,14 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
         kb0 = bz * per;
         num_kb = min(per, num_kb - kb0);
     }
-    const uint32_t b_bytes = p.block_n * 128u;
-    const uint32_t half_bytes = kABytes + b_bytes;              // [A][B]; split mode appends [A_lo][B_lo]
-    const uint32_t stage_bytes = p.split ? 2u * half_bytes : half_bytes;
+    const uint32_t stage_bytes = kABytes + p.block_n * 128u;    // [A][B]
     // WGRAD stages its output tile (block_n/32 swizzled panels of [128 rows x 128 B]) behind the ring
     const uint32_t epi_base = smem_base + p.stages * stage_bytes;
     const uint32_t epi_bytes = (MODE == GEMM_WGRAD) ? (uint32_t)p.block_n * 512u : 0u;
     const uint32_t bar_base = epi_base + epi_bytes;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
-    const uint32_t tmem_full_bar = bar_base + 8u * (2 * p.stages);
-    const uint32_t tmem_slot = tmem_full_bar + 8u;
-    volatile uint32_t* tmem_slot_gen =
-        reinterpret_cast<volatile uint32_t*>(smem_gen + p.stages * stage_bytes + epi_bytes + 8u * (2 * p.stages) + 8u);
-
-    // 3xTF32 accumulators (ptx.cuh): one for the small cross terms; FWD / DGRAD reductions over >= 8 k-blocks rotate the
-    // hi*hi products over up to 4 main accumulators, inside half of the TMEM columns.
-    const bool acc_split = p.split && p.acc_split;
-    const int rot = (acc_split && MODE != GEMM_WGRAD) ? acc_rotation(num_kb, p.block_n, 256) : 1;   // 256 of 512 columns: two CTAs of this kernel may share an SM
-    uint32_t tmem_cols = 32;
-    while (tmem_cols < (uint32_t)p.block_n * (acc_split ? (uint32_t)rot + 1u : 1u)) tmem_cols <<= 1;
-    const uint32_t small_off = acc_split ? (uint32_t)p.block_n * (uint32_t)rot : 0u;
+    volatile uint32_t* flag_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + p.stages * stage_bytes + epi_bytes + 8u * (2 * p.stages));
 
     const bool db_active = (MODE == GEMM_WGRAD) && (p.db != nullptr) && (by == 0);
 
@@ -90,23 +75,15 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
         if (MODE == GEMM_WGRAD) tma_prefetch_desc(&tmC);
         for (int s = 0; s < p.stages; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), db_active ? 5 : 1);   // MMA commit (+ 4 db-reducing warps)
+            mbar_init(empty_bar(s), 4);                   // one arrive per math warp
         }
-        mbar_init(tmem_full_bar, 1);
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, tmem_cols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
 
     if (warp == 0) {
         // ------------------------------------------------------------ TMA producer
-        // converged warp; one elect.sync-chosen lane issues (no ELECT/BRA.U.ANY uniformization loops)
+        // converged warp; one elect.sync-chosen lane issues
         for (int kb = 0; kb < num_kb; ++kb) {
             const int s = kb % p.stages;
             const uint32_t ph = (kb / p.stages) & 1;
@@ -128,119 +105,58 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                     for (int j = 0; j < p.block_n / 32; ++j)
                         tma_load_2d(b_dst + j * kPanelBytes, &tmB, full_bar(s), n0 + 32 * j, k0);
                 }
-                if (p.split) {                                // lo twins: same boxes, second half of the stage
-                    const uint32_t al = a_dst + half_bytes, bl = b_dst + half_bytes;
-                    if (!A_MN) {
-                        tma_load_2d(al, &tmAlo, full_bar(s), k0, m0);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) tma_load_2d(al + i * kPanelBytes, &tmAlo, full_bar(s), m0 + 32 * i, k0);
-                    }
-                    if (!B_MN) {
-                        tma_load_2d(bl, &tmBlo, full_bar(s), k0, n0);
-                    } else {
-                        for (int j = 0; j < p.block_n / 32; ++j)
-                            tma_load_2d(bl + j * kPanelBytes, &tmBlo, full_bar(s), n0 + 32 * j, k0);
-                    }
-                }
             }
             __syncwarp();
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------ MMA issuer (converged warp, elected lane)
-        {
-            const uint32_t idesc = umma_idesc_tf32(kBlockM, p.block_n, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-            const uint32_t a_hi = A_MN ? umma_desc_hi(512u, 1u) : umma_desc_hi(1024u, 2u);
-            const uint32_t b_hi = B_MN ? umma_desc_hi(512u, 1u) : umma_desc_hi(1024u, 2u);
-            uint32_t rot_i = 0u;                          // main accumulator of the current k-block (round robin)
-            for (int kb = 0; kb < num_kb; ++kb) {
-                const int s = kb % p.stages;
-                const uint32_t ph = (kb / p.stages) & 1;
-                mbar_wait(full_bar(s), ph);
-                tc_fence_after();
-                const uint32_t a_src = smem_base + s * stage_bytes;
-                const uint32_t b_src = a_src + kABytes;
-                // descriptors: built once per k-block, stepped by a constant per UMMA_K = 8 slice
-                const uint32_t a_lo = A_MN ? umma_desc_lo(a_src, kPanelBytes) : umma_desc_lo(a_src, 16u);
-                const uint32_t b_lo = B_MN ? umma_desc_lo(b_src, kPanelBytes) : umma_desc_lo(b_src, 16u);
-                constexpr uint32_t a_step = A_MN ? (1024u >> 4) : (32u >> 4);
-                constexpr uint32_t b_step = B_MN ? (1024u >> 4) : (32u >> 4);
-                if (elect_one()) {
-                    if (p.split) {
-                        // fp32-equivalent product: small terms first, then hi*hi (the raw tiles ARE the hi parts)
-                        const uint32_t al_lo = a_lo + (half_bytes >> 4), bl_lo = b_lo + (half_bytes >> 4);
-                        // accumulators of this k-block as plain registers (no modulo in the issue loop: the uniform datapath is slow)
-                        const uint32_t small_acc = tmem_base + small_off;
-                        const uint32_t main_acc = tmem_base + rot_i * (uint32_t)p.block_n;
-                        const bool main_fresh = acc_split && kb < rot;
-#pragma unroll
-                        for (int k4 = 0; k4 < 4; ++k4) {
-                            umma_tf32(small_acc, umma_desc_pack(al_lo + k4 * a_step, a_hi), umma_desc_pack(b_lo + k4 * b_step, b_hi),
-                                      idesc, (kb == 0 && k4 == 0) ? 0u : 1u);
-                            umma_tf32(small_acc, umma_desc_pack(a_lo + k4 * a_step, a_hi), umma_desc_pack(bl_lo + k4 * b_step, b_hi),
-                                      idesc, 1u);
-                            umma_tf32(main_acc, umma_desc_pack(a_lo + k4 * a_step, a_hi), umma_desc_pack(b_lo + k4 * b_step, b_hi),
-                                      idesc, (main_fresh && k4 == 0) ? 0u : 1u);
-                        }
-                    } else
-#pragma unroll
-                    for (int k4 = 0; k4 < 4; ++k4)
-                        umma_tf32(tmem_base, umma_desc_pack(a_lo + k4 * a_step, a_hi), umma_desc_pack(b_lo + k4 * b_step, b_hi), idesc,
-                                  (kb | k4) != 0 ? 1u : 0u);
-                    umma_commit(empty_bar(s));                // smem stage free once these MMAs retire
-                    if (kb == num_kb - 1) umma_commit(tmem_full_bar);   // accumulator complete
-                }
-                rot_i = (rot_i + 1u == (uint32_t)rot) ? 0u : rot_i + 1u;   // every lane keeps the round-robin index (any lane may be elected)
-                __syncwarp();
-            }
-        }
     } else {
-        // ------------------------------------------------------------ epilogue warps
-        const int q = warp & 3;                           // TMEM lane quarter this warp may read
+        // ------------------------------------------------------------ math + epilogue warps
+        // warp w owns the 32 output rows q*32 .. q*32+31 of the tile (all block_n columns): tensor-core MMAs from the
+        // staged tiles into registers, then one row per lane (warp_acc_row16) for the fused epilogue.
+        const int q = warp & 3;
         const int m_local = q * 32 + lane;
         const int m = m0 + m_local;
         const bool m_ok = m < p.m_total;
+        const int nt = p.block_n / 8;
+        constexpr int kChunks = kMaxBlockN / 16;
 
+        float acc[2][kMaxBlockN / 8][4];
+        warp_acc_zero(acc);
         float dbsum = 0.f;
-        if (MODE == GEMM_WGRAD && db_active) {
-            // db[m] = sum over micro-batch rows of dZ[row, m], read from the staged A panels.
-            for (int kb = 0; kb < num_kb; ++kb) {
-                const int s = kb % p.stages;
-                const uint32_t ph = (kb / p.stages) & 1;
-                mbar_wait(full_bar(s), ph);
-                const uint32_t panel = smem_base + s * stage_bytes + q * kPanelBytes;
+        for (int kb = 0; kb < num_kb; ++kb) {
+            const int s = kb % p.stages;
+            const uint32_t ph = (kb / p.stages) & 1;
+            mbar_wait(full_bar(s), ph);
+            const uint32_t a_src = smem_base + s * stage_bytes;
+            if (p.split)
+                warp_mma_kblock<kMaxBlockN / 8, A_MN, B_MN, true>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, nt, lane);
+            else
+                warp_mma_kblock<kMaxBlockN / 8, A_MN, B_MN, false>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, nt, lane);
+            if (MODE == GEMM_WGRAD && db_active) {
+                // db[m] = sum over micro-batch rows of dZ[row, m], read from the staged A panels (exact fp32)
 #pragma unroll 8
-                for (int r = 0; r < 32; ++r) {
-                    // SWIZZLE_128B_ATOM_32B: 32-byte chunk index ^= (row & 3)
-                    const uint32_t addr = panel + r * 128u + ((((uint32_t)lane >> 3) ^ (r & 3u)) << 5) + ((lane & 7u) << 2);
-                    float v;
-                    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
-                    dbsum += v;
-                }
-                __syncwarp();
-                if (lane == 0) mbar_arrive(empty_bar(s));
+                for (int r = 0; r < 32; ++r) dbsum += lds_f32(a_src + operand_off<true>((uint32_t)m_local, (uint32_t)r));
             }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar(s));
         }
-
-        mbar_wait(tmem_full_bar, 0);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
 
         if constexpr (SPLITK) {
             // ---- split-K: publish the raw partial, last arriver reduces (fixed split order) + epilogue
             const int tile = (int)(by * gridDim.x + bx);
             const size_t tile_floats = (size_t)p.block_n * kBlockM;
             float* ws = p.partial + ((size_t)tile * p.k_splits + bz) * tile_floats;
-            for (int c = 0; c < p.block_n; c += 16) {
-                float v[16];
-                tmem_ld16_acc(taddr + c, small_off, v, rot, (uint32_t)p.block_n);
 #pragma unroll
-                for (int j = 0; j < 16; ++j) __stcg(ws + (size_t)(c + j) * kBlockM + m_local, v[j]);   // lanes -> consecutive floats
+            for (int ch = 0; ch < kChunks; ++ch) {
+                if (16 * ch >= p.block_n) break;
+                float v[16];
+                warp_acc_row16(acc, ch, v, lane);
+#pragma unroll
+                for (int j = 0; j < 16; ++j) __stcg(ws + (size_t)(16 * ch + j) * kBlockM + m_local, v[j]);   // lanes -> consecutive floats
             }
             __threadfence();
             asm volatile("bar.sync 1, 128;" ::: "memory");
-            volatile uint32_t* last_flag = tmem_slot_gen + 1;
-            if (warp == 2 && lane == 0) {
+            volatile uint32_t* last_flag = flag_gen;
+            if (warp == 1 && lane == 0) {
                 const unsigned old = atomicAdd(p.tile_counter + tile, 1u);
                 const bool last = (old == (unsigned)p.k_splits - 1u);
                 if (last) p.tile_counter[tile] = 0u;          // re-arm for the next launch (graph replay)
@@ -281,10 +197,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                             x = (mk[j] > 0.f) ? x : 0.f;
                         }
                         const int n = n0 + c + j;
-                        if (n < p.n_total) {
-                            out[(size_t)n * p.ldo + m] = x;
-                            if (p.out_lo != nullptr) p.out_lo[(size_t)n * p.ldo + m] = tf32_lo(x);
-                        }
+                        if (n < p.n_total) out[(size_t)n * p.ldo + m] = x;
                     }
                 }
             }
@@ -293,7 +206,10 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             if (MODE == GEMM_FWD && p.bias != nullptr && m_ok) bias = __ldg(p.bias + (size_t)m * p.bias_stride);
             const float* __restrict__ mask = p.mask;
             float* __restrict__ out = p.out;
-            for (int c = 0; c < p.block_n; c += 16) {
+#pragma unroll
+            for (int ch = 0; ch < kChunks; ++ch) {
+                const int c = 16 * ch;
+                if (c >= p.block_n) break;
                 float mk[16];
                 if (MODE == GEMM_DGRAD && mask != nullptr && m_ok) {
 #pragma unroll
@@ -303,7 +219,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                     }
                 }
                 float v[16];
-                tmem_ld16_acc(taddr + c, small_off, v, rot, (uint32_t)p.block_n);
+                warp_acc_row16(acc, ch, v, lane);
                 if (!m_ok) continue;
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
@@ -318,38 +234,33 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
                     const int n = n0 + c + j;
-                    if (n < p.n_total) {
-                        out[(size_t)n * p.ldo + m] = v[j];     // lanes -> consecutive m: coalesced
-                        if (p.out_lo != nullptr) p.out_lo[(size_t)n * p.ldo + m] = tf32_lo(v[j]);
-                    }
+                    if (n < p.n_total) out[(size_t)n * p.ldo + m] = v[j];     // lanes -> consecutive m: coalesced
                 }
             }
         } else {
-            // WGRAD: TMEM -> registers -> swizzled smem panels -> ONE TMA store (overwrite) or TMA
-            // reduce-add (accumulate, performed in L2) per 32-column panel.  With fuse_sgd the tile is
-            // scaled by -lr and reduce-added straight into W: dW never touches memory, zero_grad and
-            // the optimizer pass disappear.  OOB rows/columns are clipped by the tensor map, so the
-            // bias column (index n_total of the same [out, ld] block) is never touched here.
+            // WGRAD: registers -> swizzled smem panels -> ONE TMA store (overwrite) or TMA reduce-add (accumulate,
+            // performed in L2) per 32-column panel.  With fuse_sgd the tile is scaled by -lr and reduce-added straight into
+            // W: dW never touches memory, zero_grad and the optimizer pass disappear.  OOB rows/columns are clipped by the
+            // tensor map, so the bias column (index n_total of the same [out, ld] block) is never touched here.
             const float scale = p.fuse_sgd ? -p.lr : 1.f;
-            for (int pj = 0; pj < p.block_n / 32; ++pj) {
-                const uint32_t prow = epi_base + pj * (kBlockM * 128u) + (uint32_t)m_local * 128u;
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    float v[16];
-                    tmem_ld16_acc(taddr + pj * 32 + h * 16, small_off, v);
+            for (int ch = 0; ch < kChunks; ++ch) {
+                if (16 * ch >= p.block_n) break;
+                float v[16];
+                warp_acc_row16(acc, ch, v, lane);
+                const uint32_t prow = epi_base + (ch >> 1) * (kBlockM * 128u) + (uint32_t)m_local * 128u;
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        const uint32_t chunk = (uint32_t)(h * 4 + q) ^ ((uint32_t)m_local & 7u);
-                        asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(prow + (chunk << 4)),
-                                     "f"(v[4 * q] * scale), "f"(v[4 * q + 1] * scale), "f"(v[4 * q + 2] * scale),
-                                     "f"(v[4 * q + 3] * scale)
-                                     : "memory");
-                    }
+                for (int q4 = 0; q4 < 4; ++q4) {
+                    const uint32_t chunk = (uint32_t)((ch & 1) * 4 + q4) ^ ((uint32_t)m_local & 7u);
+                    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(prow + (chunk << 4)),
+                                 "f"(v[4 * q4] * scale), "f"(v[4 * q4 + 1] * scale), "f"(v[4 * q4 + 2] * scale),
+                                 "f"(v[4 * q4 + 3] * scale)
+                                 : "memory");
                 }
             }
             fence_proxy_async_smem();
-            asm volatile("bar.sync 1, 128;" ::: "memory");           // the 4 epilogue warps only
-            if (warp == 2 && lane == 0) {
+            asm volatile("bar.sync 1, 128;" ::: "memory");           // the 4 math warps only
+            if (warp == 1 && lane == 0) {
                 const bool add = p.accumulate || p.fuse_sgd;
                 for (int pj = 0; pj < p.block_n / 32; ++pj) {
                     if (n0 + pj * 32 >= p.n_total) break;
@@ -360,10 +271,10 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                 tma_store_commit();
                 tma_store_wait_all();
             }
-            // TMA stores clip the inner dimension at 16-byte granularity (measured on B200: with
-            // in % 4 != 0 the partially valid last chunk is written in full), i.e. the bias slot in
-            // column `in` may just have been overwritten with the (zero) accumulator of an OOB
-            // column.  The bias gradient is therefore written strictly AFTER the tile store retired.
+            // TMA stores clip the inner dimension at 16-byte granularity (with in % 4 != 0 the partially valid last
+            // chunk may be written in full), i.e. the bias slot in column `in` may just have been overwritten with the
+            // (zero) accumulator of an OOB column.  The bias gradient is therefore written strictly AFTER the tile
+            // store retired.
             asm volatile("bar.sync 1, 128;" ::: "memory");
             if (db_active && m_ok) {
                 if (p.fuse_sgd) {
@@ -375,39 +286,26 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                 }
             }
         }
-        tc_fence_before();
-    }
-
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, tmem_cols);
     }
 }
 
 template <int MODE, bool SPLITK = false>
 __global__ void __launch_bounds__(kThreads, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAlo,
-               const __grid_constant__ CUtensorMap tmBlo, const GemmParams p) {
-    tc_gemm_body<MODE, SPLITK>(tmA, tmB, tmC, tmAlo, tmBlo, p, (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z);
+               const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+    tc_gemm_body<MODE, SPLITK>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z);
 }
 
 // ---- grouped weight-gradient launch: the tiles of SEVERAL layers' WGRAD GEMMs in one grid (one table entry per CTA).
 // Removes the fork / join of one graph node per layer from the end of a step: with the zero-copy loss the fp32 training
-// step of a narrow stage is chain kernel -> grouped wgrad (+SGD) -> W_lo refresh (or chain || LL kernel under DP).
+// step of a narrow stage is chain kernel -> grouped wgrad (+SGD) (or chain || LL kernel under DP).
 __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const GemmGroupEntry* __restrict__ entries) {
     const GemmGroupEntry& e = entries[blockIdx.x];
     const GemmParams p = e.p;                      // private copy: the body reads these fields in every loop
-    tc_gemm_body<GEMM_WGRAD, false>(e.tmA, e.tmB, e.tmC, e.tmAlo, e.tmBlo, p, e.bx, e.by, 0);
+    tc_gemm_body<GEMM_WGRAD, false>(e.tmA, e.tmB, e.tmC, p, e.bx, e.by, 0);
 }
 
 // =========================================================================== host side
-// SSB_ACC_SPLIT=0: all three 3xTF32 products into one accumulator (the round-1 behaviour), for A/B measurements
-int acc_split_default() {
-    static const int v = [] { const char* e = getenv("SSB_ACC_SPLIT"); return (e && atoi(e) == 0) ? 0 : 1; }();
-    return v;
-}
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -426,8 +324,7 @@ static EncodeTiledFn get_encode_fn() {
 }
 
 // 2-D fp32 row-major tensor [outer, inner] with pitch ld (floats); box = [box_outer, box_inner=32], SWIZZLE_128B.
-static const char* make_tmap(CUtensorMap* map, const float* base, int inner, int outer, int ld, int box_outer,
-                             bool mn_major = false, bool l2_256 = true) {
+static const char* make_tmap(CUtensorMap* map, const float* base, int inner, int outer, int ld, int box_outer) {
     EncodeTiledFn enc = get_encode_fn();
     if (!enc) return "cuTensorMapEncodeTiled entry point not available";
     if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return "TMA: base address must be 16-byte aligned";
@@ -439,9 +336,7 @@ static const char* make_tmap(CUtensorMap* map, const float* base, int inner, int
     cuuint32_t box[2] = {kBlockK, (cuuint32_t)box_outer};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     // 32-bit MN-major UMMA operands only exist in the "128B swizzle, 32B atom" flavour
-                     mn_major ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled failed";
@@ -449,11 +344,11 @@ static const char* make_tmap(CUtensorMap* map, const float* base, int inner, int
 
 // MN-major operand map ([rows(K) x 32 mn] panels) for other translation units (fused_dp.cu)
 const char* make_tmap_mn(CUtensorMap* map, const float* base, int inner, int outer, int ld) {
-    return make_tmap(map, base, inner, outer, ld, 32, true);
+    return make_tmap(map, base, inner, outer, ld, 32);
 }
 
 const char* make_tmap_k(CUtensorMap* map, const float* base, int inner, int outer, int ld, int box_outer) {
-    return make_tmap(map, base, inner, outer, ld, box_outer, false);
+    return make_tmap(map, base, inner, outer, ld, box_outer);
 }
 
 static int round_up_i(int x, int m) { return (x + m - 1) / m * m; }
@@ -461,81 +356,66 @@ static int round_up_i(int x, int m) { return (x + m - 1) / m * m; }
 static void finish_plan(GemmPlan* plan) {
     GemmParams& p = plan->p;
     const int num_kb = (p.k_total + (int)kBlockK - 1) / (int)kBlockK;
-    const int stage_bytes = ((int)kABytes + p.block_n * 128) * (p.split ? 2 : 1);
+    const int stage_bytes = (int)kABytes + p.block_n * 128;
     const int epi_bytes = plan->mode == GEMM_WGRAD ? p.block_n * 512 : 0;
     int stages = (200 * 1024 - epi_bytes) / stage_bytes;
     if (stages > 6) stages = 6;
     if (stages > num_kb) stages = num_kb;
     if (stages < 1) stages = 1;
     p.stages = stages;
-    plan->smem_bytes = stages * stage_bytes + epi_bytes + 1024 /*align slack*/ + 8 * (2 * stages + 2) + 16;
+    plan->smem_bytes = stages * stage_bytes + epi_bytes + 1024 /*align slack*/ + 8 * (2 * stages) + 16;
     plan->grid = dim3((p.m_total + kBlockM - 1) / kBlockM, (p.n_total + p.block_n - 1) / p.block_n, 1);
 }
 
 const char* gemm_plan_fwd(GemmPlan* plan, const float* W, int ldw, const float* X, int ldx, float* Y, int ldy, int rows,
-                          int in, int out, const float* bias, int bias_stride, int relu, GemmLo lo) {
+                          int in, int out, const float* bias, int bias_stride, int relu, bool split) {
     *plan = GemmPlan{};
     plan->mode = GEMM_FWD;
     GemmParams& p = plan->p;
     p.m_total = out; p.n_total = rows; p.k_total = in;
-    p.block_n = rows >= 256 ? 256 : round_up_i(rows, 16);
+    p.block_n = rows >= kMaxBlockN ? kMaxBlockN : round_up_i(rows, 16);
     p.out = Y; p.ldo = ldy; p.bias = bias; p.bias_stride = bias_stride; p.relu = relu;
     if (const char* e = make_tmap(&plan->tmA, W, in, out, ldw, kBlockM)) return e;
     if (const char* e = make_tmap(&plan->tmB, X, in, rows, ldx, p.block_n)) return e;
     plan->tmC = plan->tmA;
-    plan->tmAlo = plan->tmA; plan->tmBlo = plan->tmB;
-    if (lo.A != nullptr && lo.B != nullptr) {
-        p.split = 1; p.out_lo = lo.out; p.acc_split = acc_split_default();
-        if (const char* e = make_tmap(&plan->tmAlo, lo.A, in, out, ldw, kBlockM)) return e;
-        if (const char* e = make_tmap(&plan->tmBlo, lo.B, in, rows, ldx, p.block_n)) return e;
-    }
+    p.split = split ? 1 : 0;
     finish_plan(plan);
     return nullptr;
 }
 
 const char* gemm_plan_dgrad(GemmPlan* plan, const float* W, int ldw, const float* dZ, int lddz, float* dX, int lddx,
-                            int rows, int in, int out, const float* mask, int ldmask, GemmLo lo) {
+                            int rows, int in, int out, const float* mask, int ldmask, bool split) {
     *plan = GemmPlan{};
     plan->mode = GEMM_DGRAD;
     GemmParams& p = plan->p;
     p.m_total = in; p.n_total = rows; p.k_total = out;
-    p.block_n = rows >= 256 ? 256 : round_up_i(rows, 16);
+    p.block_n = rows >= kMaxBlockN ? kMaxBlockN : round_up_i(rows, 16);
     p.out = dX; p.ldo = lddx; p.mask = mask; p.ldmask = ldmask;
-    if (const char* e = make_tmap(&plan->tmA, W, in, out, ldw, 32, true)) return e;          // MN-major panels [32 k x 32 m]
+    if (const char* e = make_tmap(&plan->tmA, W, in, out, ldw, 32)) return e;          // MN-major panels [32 k x 32 m]
     if (const char* e = make_tmap(&plan->tmB, dZ, out, rows, lddz, p.block_n)) return e;
     plan->tmC = plan->tmA;
-    plan->tmAlo = plan->tmA; plan->tmBlo = plan->tmB;
-    if (lo.A != nullptr && lo.B != nullptr) {
-        p.split = 1; p.out_lo = lo.out; p.acc_split = acc_split_default();
-        if (const char* e = make_tmap(&plan->tmAlo, lo.A, in, out, ldw, 32, true)) return e;
-        if (const char* e = make_tmap(&plan->tmBlo, lo.B, out, rows, lddz, p.block_n)) return e;
-    }
+    p.split = split ? 1 : 0;
     finish_plan(plan);
     return nullptr;
 }
 
 const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const float* X, int ldx, float* G, int ldg,
                             int rows, int in, int out, int accumulate, float* db, int db_stride, float* W, int ldw,
-                            float lr, int fuse_sgd, GemmLo lo) {
+                            float lr, int fuse_sgd, bool split) {
     *plan = GemmPlan{};
     plan->mode = GEMM_WGRAD;
     GemmParams& p = plan->p;
     p.m_total = out; p.n_total = in; p.k_total = rows;
-    p.block_n = in >= 128 ? 128 : round_up_i(in, 32);
+    p.block_n = in >= kMaxBlockN ? kMaxBlockN : round_up_i(in, 32);
     p.G = G; p.ldg = ldg; p.accumulate = accumulate; p.db = db; p.db_stride = db_stride;
     p.W = W; p.ldw = ldw; p.lr = lr; p.fuse_sgd = fuse_sgd;
     if (fuse_sgd && W == nullptr) return "fuse_sgd needs W";
     if (fuse_sgd && accumulate) return "fuse_sgd cannot be combined with accumulate (reduce into G, then run the SGD pass)";
     // output tile map: [out, in] with the block's row pitch; fused SGD targets W itself
     if (const char* e = make_tmap(&plan->tmC, fuse_sgd ? W : G, in, out, fuse_sgd ? ldw : ldg, kBlockM)) return e;
-    if (const char* e = make_tmap(&plan->tmA, dZ, out, rows, lddz, 32, true)) return e;
-    if (const char* e = make_tmap(&plan->tmB, X, in, rows, ldx, 32, true)) return e;
-    plan->tmAlo = plan->tmA; plan->tmBlo = plan->tmB;
-    if (lo.A != nullptr && lo.B != nullptr) {
-        p.split = 1; p.acc_split = acc_split_default();
-        if (const char* e = make_tmap(&plan->tmAlo, lo.A, out, rows, lddz, 32, true)) return e;
-        if (const char* e = make_tmap(&plan->tmBlo, lo.B, in, rows, ldx, 32, true)) return e;
-    }
+    if (const char* e = make_tmap(&plan->tmA, dZ, out, rows, lddz, 32)) return e;
+    if (const char* e = make_tmap(&plan->tmB, X, in, rows, ldx, 32)) return e;
+    p.split = split ? 1 : 0;
     finish_plan(plan);
     return nullptr;
 }
@@ -569,13 +449,13 @@ const char* gemm_plan_enable_splitk(GemmPlan* plan, int k_splits, float* workspa
     if (workspace == nullptr || counters == nullptr) return "split-K needs a workspace and zeroed tile counters";
     p.k_splits = k_splits; p.partial = workspace; p.tile_counter = counters;
     // two CTAs per SM: at most ~100 KB of ring per CTA
-    const int stage_bytes = ((int)kABytes + p.block_n * 128) * (p.split ? 2 : 1);
+    const int stage_bytes = (int)kABytes + p.block_n * 128;
     int stages = (100 * 1024) / stage_bytes;
     if (stages > 6) stages = 6;
     if (stages > per) stages = per;
     if (stages < 2) stages = 2;
     p.stages = stages;
-    plan->smem_bytes = stages * stage_bytes + 1024 + 8 * (2 * stages + 2) + 16;
+    plan->smem_bytes = stages * stage_bytes + 1024 + 8 * (2 * stages) + 16;
     plan->grid.z = k_splits;
     return nullptr;
 }
@@ -594,7 +474,7 @@ const char* gemm_group_plan(GemmGroupPlan* out, const GemmPlan* plans, int n_pla
             for (unsigned bx = 0; bx < g.grid.x; ++bx) {
                 GemmGroupEntry e;
                 memset(&e, 0, sizeof(e));
-                e.tmA = g.tmA; e.tmB = g.tmB; e.tmC = g.tmC; e.tmAlo = g.tmAlo; e.tmBlo = g.tmBlo;
+                e.tmA = g.tmA; e.tmB = g.tmB; e.tmC = g.tmC;
                 e.p = g.p; e.bx = (int)bx; e.by = (int)by;
                 host.push_back(e);
             }
@@ -651,12 +531,12 @@ static cudaError_t launch_mode(const GemmPlan& plan, cudaStream_t stream) {
     }
     if constexpr (MODE != GEMM_WGRAD) {
         if (plan.p.k_splits > 1) {
-            tc_gemm_kernel<MODE, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.tmAlo, plan.tmBlo, plan.p);
+            tc_gemm_kernel<MODE, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
             g_launches.fetch_add(1, std::memory_order_relaxed);
             return cudaGetLastError();
         }
     }
-    tc_gemm_kernel<MODE><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.tmAlo, plan.tmBlo, plan.p);
+    tc_gemm_kernel<MODE><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return cudaGetLastError();
 }

@@ -120,7 +120,7 @@ public:
 
 private:
     static int num_sms() {
-        int dev = 0, sms = 148;
+        int dev = 0, sms = 132;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         return sms;

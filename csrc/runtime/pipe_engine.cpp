@@ -116,23 +116,6 @@ void PipeEngine::alloc_buffers() {
     if (cfg_.training)
         for (int l = 0; l <= L_; ++l) dz_all_[l] = dalloc((size_t)M * mb * act_ld_[l]);
     probs_all_ = dalloc((size_t)M * mb * act_ld_[L_]);
-    act_lo_all_.assign(L_ + 1, nullptr);
-    dz_lo_all_.assign(L_ + 1, nullptr);
-    act_lo_.assign(M, std::vector<float*>(L_ + 1, nullptr));
-    dz_lo_.assign(M, std::vector<float*>(L_ + 1, nullptr));
-    if (cfg_.split) {
-        W_lo_ = dalloc((size_t)arena_numel_);
-        for (int set = 0; set < 2; ++set) x_lo_sets_[set] = dalloc((size_t)M * mb * act_ld_[0]);
-        act_lo_all_[0] = x_lo_sets_[0];
-        for (int l = 1; l <= L_; ++l) act_lo_all_[l] = dalloc((size_t)M * mb * act_ld_[l]);
-        if (cfg_.training)
-            for (int l = 0; l <= L_; ++l) dz_lo_all_[l] = dalloc((size_t)M * mb * act_ld_[l]);
-        for (int mu = 0; mu < M; ++mu)
-            for (int l = 0; l <= L_; ++l) {
-                act_lo_[mu][l] = act_lo_all_[l] + (size_t)mu * mb * act_ld_[l];
-                if (cfg_.training) dz_lo_[mu][l] = dz_lo_all_[l] + (size_t)mu * mb * act_ld_[l];
-            }
-    }
     act_.assign(M, std::vector<float*>(L_ + 1, nullptr));
     dz_.assign(M, std::vector<float*>(L_ + 1, nullptr));
     probs_.assign(M, nullptr);
@@ -152,44 +135,15 @@ void PipeEngine::select_set(int set) {
     y_stage_ = y_stage_sets_[set];
     act_all_[0] = x_stage_;
     for (int mu = 0; mu < cfg_.n_mu; ++mu) act_[mu][0] = act_all_[0] + (size_t)mu * cfg_.mb_rows * act_ld_[0];
-    if (cfg_.split) {
-        act_lo_all_[0] = x_lo_sets_[set];
-        for (int mu = 0; mu < cfg_.n_mu; ++mu) act_lo_[mu][0] = act_lo_all_[0] + (size_t)mu * cfg_.mb_rows * act_ld_[0];
-    }
-}
-
-// lo-twin operand sets for the three GEMMs of layer l (mu < 0: all micro-batches at once)
-GemmLo PipeEngine::lo_fwd(int l, int mu) const {
-    GemmLo g;
-    if (!cfg_.split) return g;
-    g.A = W_lo_ + cfg_.layers[l - 1].offset;
-    g.B = mu < 0 ? act_lo_all_[l - 1] : act_lo_[mu][l - 1];
-    g.out = mu < 0 ? act_lo_all_[l] : act_lo_[mu][l];
-    return g;
-}
-GemmLo PipeEngine::lo_dgrad(int l, int mu) const {
-    GemmLo g;
-    if (!cfg_.split) return g;
-    g.A = W_lo_ + cfg_.layers[l - 1].offset;
-    g.B = mu < 0 ? dz_lo_all_[l] : dz_lo_[mu][l];
-    g.out = mu < 0 ? dz_lo_all_[l - 1] : dz_lo_[mu][l - 1];
-    return g;
-}
-GemmLo PipeEngine::lo_wgrad(int l, int mu) const {
-    GemmLo g;
-    if (!cfg_.split) return g;
-    g.A = mu < 0 ? dz_lo_all_[l] : dz_lo_[mu][l];
-    g.B = mu < 0 ? act_lo_all_[l - 1] : act_lo_[mu][l - 1];
-    return g;
 }
 
 // Opt-in (SSB_SPLITK=1: automatic, SSB_SPLITK=k: force k where legal): give FWD / DGRAD GEMMs of wide layers
-// enough CTAs to saturate HBM (8192 outputs = only 64 tiles on 148 SMs).  Not yet the default: the kernel
+// enough CTAs to saturate HBM (8192 outputs = only 64 tiles on 132 SMs).  Not yet the default: the kernel
 // variant still has to be validated on hardware.
 void PipeEngine::maybe_splitk(GemmPlan& g) {
     const char* env = getenv("SSB_SPLITK");
     if (!env || atoi(env) <= 0 || g.mode == GEMM_WGRAD) return;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     CUDA_CHECK(cudaGetDevice(&dev));
     CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     int splits = gemm_splitk_choice(g, sms);
@@ -251,8 +205,6 @@ int PipeEngine::add_chain(int stream, int mu_base, int n_mu, bool do_fwd, bool d
         cp.act[l] = act_all_[l];
         cp.dz[l] = cfg_.training ? dz_all_[l] : nullptr;
         cp.act_ld[l] = act_ld_[l];
-        cp.act_lo[l] = cfg_.split ? act_lo_all_[l] : nullptr;
-        cp.dz_lo[l] = (cfg_.split && cfg_.training) ? dz_lo_all_[l] : nullptr;
     }
     cp.target = y_stage_; cp.ldt = y_ld_;
     cp.probs = probs_all_; cp.ldp = act_ld_[L_];
@@ -262,7 +214,6 @@ int PipeEngine::add_chain(int stream, int mu_base, int n_mu, bool do_fwd, bool d
     cp.do_fwd = do_fwd; cp.do_loss = do_loss; cp.do_bwd = do_bwd; cp.first_stage = cfg_.is_first;
     cp.dbg = nullptr;
     cp.sync_debug = (getenv("SSB_RACECHECK") && atoi(getenv("SSB_RACECHECK")) > 0) ? 1 : 0;
-    cp.acc_split = (getenv("SSB_CHAIN_ACC") && atoi(getenv("SSB_CHAIN_ACC")) > 0) ? 1 : 0;   // accurate instantiation, see mlp_chain.cu
     if (fold != nullptr && pp_ctx_ != nullptr) {
         cp.in_flag = fold->in_flag; cp.x_from_global = fold->x_from_global ? 1 : 0;
         cp.out_peer = fold->out_peer; cp.out_flag = fold->out_flag; cp.out_credit = fold->out_credit;
@@ -278,8 +229,7 @@ int PipeEngine::add_chain(int stream, int mu_base, int n_mu, bool do_fwd, bool d
         cp.dbg = chain_dbg_;
     }
     ChainPlan plan;
-    const char* err = chain_plan(&plan, cp, act_all_[0], act_ld_[0], cfg_.n_mu * cfg_.mb_rows, n_mu, cfg_.split ? W_lo_ : nullptr,
-                                 cfg_.split ? act_lo_all_[0] : nullptr);
+    const char* err = chain_plan(&plan, cp, act_all_[0], act_ld_[0], cfg_.n_mu * cfg_.mb_rows, n_mu, cfg_.split != 0);
     if (err) throw std::runtime_error(std::string("PipeEngine chain plan: ") + err);
     chain_plans_.push_back(plan);
     Op op;
@@ -328,7 +278,6 @@ void PipeEngine::build(const std::vector<std::tuple<int, int, int>>& instrs) {
         for (int l = 0; l < nl; ++l) { cl[l].in = cfg_.layers[l].in; cl[l].out = cfg_.layers[l].out; }
         chain_ok_ = L_ >= 1 && L_ <= kChainMaxLayers && !getenv("SSB_NO_CHAIN") &&
                     chain_eligible(cl, L_, cfg_.mb_rows, cfg_.out_dim, cfg_.is_last != 0, cfg_.split != 0);
-        w_lo_needed_ = cfg_.split != 0;      // chain kernel and per-layer fwd / dgrad kernels load the weights' lo twins
     }
     if (pp_ctx_) {
         // peer-memory transport: the neighbours write straight into my receive slots, which therefore live in the
@@ -363,11 +312,6 @@ void PipeEngine::plan_per_mubatch() {
     const bool first = cfg_.is_first, last = cfg_.is_last;
     std::vector<bool> started(streams_.size(), false);
     started[0] = true;
-    if (w_lo_needed_ && !cfg_.training) {      // inference: weights are updated by the training engine between calls
-        Op sp;
-        sp.kind = OP_SPLIT; sp.stream = 0; sp.a = W_; sp.b = W_lo_; sp.n = arena_numel_;
-        ops_.push_back(sp);
-    }
     Op begin;
     begin.kind = OP_RECORD; begin.stream = 0; begin.event = new_event();
     ops_.push_back(begin);
@@ -528,11 +472,6 @@ void PipeEngine::plan_per_mubatch() {
                 if (ev_in[mu] >= 0) {
                     emit_wait(s, ev_in[mu]);
                     ev_in[mu] = -1;
-                    if (cfg_.split) {   // activations arrived over NCCL: build their lo twin before the first GEMM reads it
-                        Op sp;
-                        sp.kind = OP_SPLIT; sp.stream = s; sp.a = act_[mu][0]; sp.b = act_lo_[mu][0]; sp.n = (int64_t)mb * act_ld_[0];
-                        ops_.push_back(sp);
-                    }
                 }
                 if (chain_ok_) {
                     // whole stage forward (+ loss head on the last stage) of this micro-batch in one launch
@@ -557,7 +496,7 @@ void PipeEngine::plan_per_mubatch() {
                         const LayerSpec& ls = cfg_.layers[l - 1];
                         GemmPlan g;
                         check(gemm_plan_fwd(&g, Wl(l), ls.ld, act_[mu][l - 1], act_ld_[l - 1], act_[mu][l], act_ld_[l], mb,
-                                            ls.in, ls.out, Wl(l) + ls.in, ls.ld, ls.relu, lo_fwd(l, mu)));
+                                            ls.in, ls.out, Wl(l) + ls.in, ls.ld, ls.relu, cfg_.split != 0));
                         add_gemm(g, s, l, mu);
                     }
                     if (!cfg_.training && last) {
@@ -603,7 +542,7 @@ void PipeEngine::plan_per_mubatch() {
                         GemmPlan g;
                         check(gemm_plan_wgrad(&g, dz_[mu][l], act_ld_[l], act_[mu][l - 1], act_ld_[l - 1], Gl(l), ls.ld, mb,
                                               ls.in, ls.out, first_write[l] ? 0 : 1, Gl(l) + ls.in, ls.ld, nullptr, 0, 0.f, 0,
-                                              lo_wgrad(l, mu)));
+                                              cfg_.split != 0));
                         add_gemm(g, w, l, mu);
                         first_write[l] = false;
                         if (final_bwd && cfg_.dp_mode == 1 && cfg_.dp_size > 1) {
@@ -625,7 +564,6 @@ void PipeEngine::plan_per_mubatch() {
                         lh.c = probs_[mu]; lh.ldc = act_ld_[L_];
                         lh.d = dz_[mu][L_]; lh.ldd = act_ld_[L_];
                         lh.rows = mb; lh.cols = cfg_.out_dim; lh.scalar = 1.0f / (float)cfg_.global_batch; lh.mu = mu;
-                    lh.e = cfg_.split ? dz_lo_[mu][L_] : nullptr;
                         lh.f = loss_zero_copy_ ? loss_target() : nullptr;
                         ops_.push_back(lh);
                     } else if (L_ > 0 && cfg_.layers[L_ - 1].relu) {
@@ -633,7 +571,6 @@ void PipeEngine::plan_per_mubatch() {
                         rm.kind = OP_RELU_MASK; rm.stream = s;
                         rm.a = dz_[mu][L_]; rm.lda = act_ld_[L_]; rm.b = act_[mu][L_]; rm.ldb = act_ld_[L_];
                         rm.rows = mb; rm.cols = cfg_.layers[L_ - 1].out;
-                    rm.e = cfg_.split ? dz_lo_[mu][L_] : nullptr;
                         ops_.push_back(rm);
                     }
                     for (int l = L_; l >= 1; --l) {
@@ -645,7 +582,7 @@ void PipeEngine::plan_per_mubatch() {
                         GemmPlan g;
                         check(gemm_plan_wgrad(&g, dz_[mu][l], act_ld_[l], act_[mu][l - 1], act_ld_[l - 1], Gl(l), ls.ld, mb,
                                               ls.in, ls.out, first_write[l] ? 0 : 1, Gl(l) + ls.in, ls.ld, nullptr, 0, 0.f, 0,
-                                              lo_wgrad(l, mu)));
+                                              cfg_.split != 0));
                         add_gemm(g, w, l, mu);
                         first_write[l] = false;
                         if (final_bwd && cfg_.dp_mode == 1 && cfg_.dp_size > 1) {
@@ -661,7 +598,7 @@ void PipeEngine::plan_per_mubatch() {
                             const float* mask = (l >= 2 && cfg_.layers[l - 2].relu) ? act_[mu][l - 1] : nullptr;
                             GemmPlan g2;
                             check(gemm_plan_dgrad(&g2, Wl(l), ls.ld, dz_[mu][l], act_ld_[l], dz_[mu][l - 1], act_ld_[l - 1], mb, ls.in,
-                                                  ls.out, mask, act_ld_[l - 1], lo_dgrad(l, mu)));
+                                                  ls.out, mask, act_ld_[l - 1], cfg_.split != 0));
                             add_gemm(g2, s, l, mu);
                         }
                     }
@@ -703,7 +640,7 @@ void PipeEngine::plan_per_mubatch() {
                             const LayerSpec& ls = cfg_.layers[l - 1];
                             GemmPlan g;
                             check(gemm_plan_wgrad(&g, dz_all_[l], act_ld_[l], act_all_[l - 1], act_ld_[l - 1], Gl(l), ls.ld, rows_all, ls.in,
-                                                  ls.out, 0, Gl(l) + ls.in, ls.ld, Wl(l), ls.ld, cfg_.lr, 1, lo_wgrad(l, -1)));
+                                                  ls.out, 0, Gl(l) + ls.in, ls.ld, Wl(l), ls.ld, cfg_.lr, 1, cfg_.split != 0));
                             grouped.push_back(g);
                         }
                         GemmGroupPlan gp;
@@ -717,14 +654,12 @@ void PipeEngine::plan_per_mubatch() {
                         for (int l = L_; l >= 1; --l) {
                             const LayerSpec& ls = cfg_.layers[l - 1];
                             DpLLLayer ly{};
-                            ly.dZ = dz_all_[l]; ly.X = act_all_[l - 1];
-                            ly.dZ_lo = cfg_.split ? dz_lo_all_[l] : nullptr; ly.X_lo = cfg_.split ? act_lo_all_[l - 1] : nullptr;
+                            ly.dZ = dz_all_[l]; ly.X = act_all_[l - 1]; ly.split = cfg_.split;
                             ly.lddz = act_ld_[l]; ly.ldx = act_ld_[l - 1]; ly.in = ls.in; ly.out = ls.out; ly.ldw = ls.ld; ly.w_offset = ls.offset;
                             lls.push_back(ly);
                         }
                         DpLLPlan lp;
                         DpLLParams base = dp_ctx_->ll_params();
-                        base.W_lo = cfg_.split ? W_lo_ : nullptr;
                         check(dp_ll_plan(&lp, lls.data(), (int)lls.size(), rows_all, base));
                         ll_plans_.push_back(lp);
                         Op lo;
@@ -764,11 +699,6 @@ void PipeEngine::plan_per_mubatch() {
         cr.b = cfg_.training ? reinterpret_cast<float*>(pp_ctx_->next_dz_credit()) : nullptr;
         ops_.push_back(cr);
     }
-    if (w_lo_needed_ && cfg_.training && !(defer_wgrad && ll_ok)) {   // weights changed: refresh their lo twin (the LL kernel does it itself)
-        Op sp;
-        sp.kind = OP_SPLIT; sp.stream = 0; sp.a = W_; sp.b = W_lo_; sp.n = arena_numel_;
-        ops_.push_back(sp);
-    }
     if (cfg_.training && last && !loss_zero_copy_) {
         Op cp;
         cp.kind = OP_MEMCPY_LOSS; cp.stream = 0; cp.a = loss_host_ + cur_set_ * std::max(cfg_.n_mu, 16);
@@ -779,7 +709,7 @@ void PipeEngine::plan_per_mubatch() {
 // Stage without pipeline communication (pp == 1): micro-batches are independent until the
 // optimizer step, so every layer runs ONCE over all of them (rows = n_mu * mb_rows).  The
 // loss head still runs one CTA per micro-batch (its global-max contract is per micro-batch),
-// the weight gradient accumulates over the micro-batches in TMEM (k-blocks in micro-batch
+// the weight gradient accumulates over the micro-batches in registers (k-blocks in micro-batch
 // order) instead of through memory, and with a single replica the SGD update is fused into
 // the wgrad epilogue (TMA reduce-add of -lr * dW into W): ZeroGrad / OptimizerStep vanish.
 void PipeEngine::build_coalesced() {
@@ -803,11 +733,6 @@ void PipeEngine::build_coalesced() {
     auto use = [&](int s) { if (!started[s]) { emit_wait(s, ev_begin); started[s] = true; } };
     auto sw = [&](int l) { return 1 + n_mu_streams_ + (l % n_w_streams_); };
 
-    if (w_lo_needed_ && !cfg_.training) {      // weights are updated by the training engine between calls
-        Op sp;
-        sp.kind = OP_SPLIT; sp.stream = 0; sp.a = W_; sp.b = W_lo_; sp.n = arena_numel_;
-        ops_.push_back(sp);
-    }
     const bool chain = chain_ok_;
     // Gated launch: the LL data-parallel kernel (dp_ll.cu) is forked at the START of the step next to the chain kernel
     // instead of behind it.  The chain kernel's epilogue warps count up a per-layer device counter when dz[l] is
@@ -842,7 +767,7 @@ void PipeEngine::build_coalesced() {
             const LayerSpec& ls = cfg_.layers[l - 1];
             GemmPlan g;
             check(gemm_plan_fwd(&g, Wl(l), ls.ld, act_all_[l - 1], act_ld_[l - 1], act_all_[l], act_ld_[l], rows, ls.in, ls.out,
-                                Wl(l) + ls.in, ls.ld, ls.relu, lo_fwd(l, -1)));
+                                Wl(l) + ls.in, ls.ld, ls.relu, cfg_.split != 0));
             add_gemm(g, 0, l);
         }
         if (!cfg_.training) {
@@ -862,7 +787,6 @@ void PipeEngine::build_coalesced() {
         lh.a = act_all_[L_]; lh.lda = act_ld_[L_]; lh.b = y_stage_; lh.ldb = y_ld_; lh.c = probs_all_; lh.ldc = act_ld_[L_];
         lh.d = dz_all_[L_]; lh.ldd = act_ld_[L_]; lh.rows = rows; lh.cols = cfg_.out_dim;
         lh.scalar = 1.0f / (float)cfg_.global_batch; lh.mu = 0; lh.n = mb;
-        lh.e = cfg_.split ? dz_lo_all_[L_] : nullptr;
         lh.f = loss_zero_copy_ ? loss_target() : nullptr;
         ops_.push_back(lh);
     }
@@ -892,14 +816,14 @@ void PipeEngine::build_coalesced() {
             const float* mask = cfg_.layers[l - 2].relu ? act_all_[l - 1] : nullptr;
             GemmPlan g;
             check(gemm_plan_dgrad(&g, Wl(l), ls.ld, dz_all_[l], act_ld_[l], dz_all_[l - 1], act_ld_[l - 1], rows, ls.in, ls.out,
-                                  mask, act_ld_[l - 1], lo_dgrad(l, -1)));
+                                  mask, act_ld_[l - 1], cfg_.split != 0));
             add_gemm(g, 0, l);
             ev_dg = emit_record(0);
         }
         if (fused_dp && ll_on) {
             DpLLLayer ly{};
             ly.dZ = dz_all_[l]; ly.X = act_all_[l - 1];
-            ly.dZ_lo = cfg_.split ? dz_lo_all_[l] : nullptr; ly.X_lo = cfg_.split ? act_lo_all_[l - 1] : nullptr;
+            ly.split = cfg_.split;
             ly.lddz = act_ld_[l]; ly.ldx = act_ld_[l - 1]; ly.in = ls.in; ly.out = ls.out; ly.ldw = ls.ld; ly.w_offset = ls.offset;
             if (gate_on_) {
                 // GEMM + reduce-scatter hop start when dz[l] is final; the in-place update of W_l additionally waits until
@@ -931,7 +855,7 @@ void PipeEngine::build_coalesced() {
                 lp.dbg = chain_dbg_ + 3 * 256 + 8 * l;
             }
             check(fused_dp_plan(&fp, dz_all_[l], act_ld_[l], act_all_[l - 1], act_ld_[l - 1], rows, lp, dp_ctx_->peers(), kFusedDpMaxCtas,
-                                cfg_.split ? dz_lo_all_[l] : nullptr, cfg_.split ? act_lo_all_[l - 1] : nullptr));
+                                cfg_.split != 0));
             dp_plans_.push_back(fp);
             Op fo;
             fo.kind = OP_FUSED_DP; fo.stream = sdp; fo.gemm = (int)dp_plans_.size() - 1; fo.layer = l;
@@ -946,7 +870,7 @@ void PipeEngine::build_coalesced() {
         }
         GemmPlan g;
         check(gemm_plan_wgrad(&g, dz_all_[l], act_ld_[l], act_all_[l - 1], act_ld_[l - 1], Gl(l), ls.ld, rows, ls.in, ls.out, 0,
-                              Gl(l) + ls.in, ls.ld, fuse ? Wl(l) : nullptr, ls.ld, cfg_.lr, fuse ? 1 : 0, lo_wgrad(l, -1)));
+                              Gl(l) + ls.in, ls.ld, fuse ? Wl(l) : nullptr, ls.ld, cfg_.lr, fuse ? 1 : 0, cfg_.split != 0));
         if (group_wgrad) {                                  // launched together after the loop
             grouped.push_back(g);
             continue;
@@ -965,7 +889,6 @@ void PipeEngine::build_coalesced() {
         // deepest layer first: its tiles get the lowest block indices, i.e. they are resident first and their gate opens first
         DpLLParams base = dp_ctx_->ll_params();
         base.gate_step = gate_on_ ? gate_step_ : nullptr;
-        base.W_lo = cfg_.split ? W_lo_ : nullptr;          // owner rows and received rows refresh their lo twins
         if (getenv("SSB_CHAIN_TIMELINE")) {
             if (!chain_dbg_) {
                 CUDA_CHECK(cudaMalloc(&chain_dbg_, 4 * 256 * sizeof(unsigned long long)));
@@ -1011,16 +934,6 @@ void PipeEngine::build_coalesced() {
     }
     for (size_t s = 1; s < streams_.size(); ++s)
         if (started[s]) { const int e = emit_record((int)s); emit_wait(0, e); }
-    // lo twins of the updated weights: the LL data-parallel kernel writes them next to the weights it stores; every other
-    // update path (SGD-fused wgrad via TMA reduce-add, NCCL / NVLS / flag-protocol kernels) is followed by the arena-wide
-    // split kernel.  (A read-modify-write wgrad epilogue that wrote W_lo itself was measured 6 us/step SLOWER than TMA
-    // reduce-add + split kernel on the same box - 98.1 vs 92.1 us - and removed.)
-    const bool wlo_in_update = !ll_layers.empty();
-    if (w_lo_needed_ && !wlo_in_update) {
-        Op sp;
-        sp.kind = OP_SPLIT; sp.stream = 0; sp.a = W_; sp.b = W_lo_; sp.n = arena_numel_;
-        ops_.push_back(sp);
-    }
     if (!loss_zero_copy_) {
         Op cp;
         cp.kind = OP_MEMCPY_LOSS; cp.stream = 0; cp.a = loss_host_ + cur_set_ * std::max(cfg_.n_mu, 16);
@@ -1033,7 +946,7 @@ void PipeEngine::finish_build() {
     for (auto& op : ops_sets_[0]) {
         if (op.kind == OP_GEMM || op.kind == OP_LOSS_HEAD || op.kind == OP_SOFTMAX || op.kind == OP_RELU_MASK ||
             op.kind == OP_SGD || op.kind == OP_ARGMAX || op.kind == OP_FUSED_DP || op.kind == OP_DP_REDUCE ||
-            op.kind == OP_BUMP_EPOCH || op.kind == OP_CHAIN || op.kind == OP_SPLIT || op.kind == OP_NVLS_SGD ||
+            op.kind == OP_BUMP_EPOCH || op.kind == OP_CHAIN || op.kind == OP_NVLS_SGD ||
             op.kind == OP_PP_PUSH || op.kind == OP_PP_WAIT || op.kind == OP_PP_CREDIT || op.kind == OP_PP_BUMP ||
             op.kind == OP_WGRAD_GROUP || op.kind == OP_BUMP_STEP || op.kind == OP_DP_LL)
             ++kernels_per_step_;
@@ -1043,11 +956,6 @@ void PipeEngine::finish_build() {
     // kernel attributes are configured up front (never inside a capture); communicators are
     // warmed up by their creator.  No eager pass here: a training step mutates the weights.
     CUDA_CHECK(gemm_configure());
-    if (w_lo_needed_) {                      // first step needs a valid lo twin of the initial weights
-        CUDA_CHECK(launch_split_lo(W_, W_lo_, arena_numel_, streams_[0]));
-        CUDA_CHECK(cudaStreamSynchronize(streams_[0]));
-    }
-    if (cfg_.split && cfg_.is_first) ++kernels_per_step_;   // + the staged-input split issued on the copy stream every step
     if (!chain_plans_.empty()) CUDA_CHECK(chain_configure());
     if (cfg_.dp_mode == 2) CUDA_CHECK(fused_dp_configure());
     if (!ll_plans_.empty()) CUDA_CHECK(dp_ll_configure());
@@ -1079,7 +987,7 @@ void PipeEngine::exec(const Op& op) {
         case OP_WGRAD_GROUP: CUDA_CHECK(gemm_group_launch(group_plans_[op.gemm], st)); break;
         case OP_LOSS_HEAD:
             CUDA_CHECK(launch_loss_head(op.a, op.lda, op.b, op.ldb, op.c, op.ldc, op.d, op.ldd, (op.f ? op.f : loss_dev_) + op.mu, op.rows,
-                                        op.cols, op.scalar, st, (int)op.n, op.e));
+                                        op.cols, op.scalar, st, (int)op.n));
             break;
         case OP_SOFTMAX:
             CUDA_CHECK(launch_loss_head(op.a, op.lda, nullptr, 0, op.b, op.ldb, nullptr, 0, nullptr, op.rows, op.cols, 0.f, st,
@@ -1088,14 +996,13 @@ void PipeEngine::exec(const Op& op) {
         case OP_ARGMAX:
             CUDA_CHECK(launch_argmax_correct(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, correct_dev_, st));
             break;
-        case OP_RELU_MASK: CUDA_CHECK(launch_relu_mask(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, st, op.e)); break;
-        case OP_SPLIT: CUDA_CHECK(launch_split_lo(op.a, op.b, (long)op.n, st)); break;
+        case OP_RELU_MASK: CUDA_CHECK(launch_relu_mask(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, st)); break;
         case OP_SGD: CUDA_CHECK(launch_sgd(op.a, op.b, op.scalar, op.n, st)); break;
         case OP_NVLS_SGD: {
             if (!nvls_ctx_) throw std::runtime_error("PipeEngine: dp_mode nvls needs an NvlsContext");
             if (nvls_ctx_->weights() != W_ || nvls_ctx_->grads() != G_)
                 throw std::runtime_error("PipeEngine: the parameter arena must live in the NVLS allocation");
-            int dev = 0, sms = 148;
+            int dev = 0, sms = 132;
             CUDA_CHECK(cudaGetDevice(&dev));
             CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
             CUDA_CHECK(launch_nvls_reduce_sgd(nvls_ctx_->params(), sms, st));
@@ -1158,7 +1065,6 @@ static const char* op_name(int kind) {
         case OP_PP_WAIT: return "pp_wait";
         case OP_PP_CREDIT: return "pp_credit";
         case OP_CHAIN: return "mlp_chain";
-        case OP_SPLIT: return "split_lo";
         case OP_MEMCPY_LOSS: return "loss_d2h";
         case OP_ARGMAX: return "argmax_correct";
         case OP_WAIT: return "wait_event";
@@ -1247,8 +1153,6 @@ void PipeEngine::stage_inputs(const float* x, const float* y) {
     if (y != nullptr && cfg_.is_last)
         CUDA_CHECK(cudaMemcpy2DAsync(y_stage_sets_[set], (size_t)y_ld_ * 4, y, (size_t)cfg_.out_dim * 4, (size_t)cfg_.out_dim * 4,
                                      rows, kind, copy_stream_));
-    if (cfg_.split && x != nullptr && cfg_.is_first)   // lo twin of the staged inputs, off the critical path
-        CUDA_CHECK(launch_split_lo(x_stage_sets_[set], x_lo_sets_[set], (long)rows * act_ld_[0], copy_stream_));
     CUDA_CHECK(cudaEventRecord(ev_copy_[set], copy_stream_));
     staged_ = true;
 }

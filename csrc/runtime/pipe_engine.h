@@ -2,7 +2,7 @@
 // ONCE into a static plan of kernel launches / NCCL ops on CUDA streams with event
 // dependencies, optionally captured into a CUDA graph, then replays it every step.
 //
-// This is the B200 replacement of the reference's Python `Worker.execute` loop
+// This is the native replacement of the reference's Python `Worker.execute` loop
 // (shallowspeed/pipe.py:434-466), which re-allocates buffers and re-dispatches Python
 // objects for every batch.  Differences that matter for performance:
 //   * persistent, pre-planned buffers + prebuilt TMA tensor maps (zero per-step host work
@@ -43,7 +43,7 @@ struct LayerSpec {
 
 enum OpKind : int {
     OP_GEMM = 0, OP_LOSS_HEAD, OP_SOFTMAX, OP_RELU_MASK, OP_SGD, OP_COMM_GROUP, OP_ALLREDUCE, OP_FUSED_DP,
-    OP_WAIT, OP_RECORD, OP_MEMCPY_LOSS, OP_ARGMAX, OP_DP_REDUCE, OP_BUMP_EPOCH, OP_CHAIN, OP_SPLIT, OP_NVLS_SGD,
+    OP_WAIT, OP_RECORD, OP_MEMCPY_LOSS, OP_ARGMAX, OP_DP_REDUCE, OP_BUMP_EPOCH, OP_CHAIN, OP_NVLS_SGD,
     OP_PP_PUSH, OP_PP_WAIT, OP_PP_CREDIT, OP_PP_BUMP, OP_WGRAD_GROUP, OP_BUMP_STEP, OP_DP_LL
 };
 
@@ -62,7 +62,7 @@ struct Op {
     int layer = -1, mu = -1;
     std::vector<CommItem> comm;
     // generic pointers for the small kernels
-    float *a = nullptr, *b = nullptr, *c = nullptr, *d = nullptr, *e = nullptr;   // e: lo twin of the output (split mode)
+    float *a = nullptr, *b = nullptr, *c = nullptr, *d = nullptr;
     float* f = nullptr;        // loss head: where the loss values go when not the default device scratch
     int lda = 0, ldb = 0, ldc = 0, ldd = 0, rows = 0, cols = 0;
     float scalar = 0.f;
@@ -157,17 +157,9 @@ private:
     std::vector<std::vector<float*>> act_, dz_;  // [mu][l]
     std::vector<float*> probs_;
     std::vector<float*> act_all_, dz_all_;       // [l] contiguous over micro-batches
-    std::vector<float*> act_lo_all_, dz_lo_all_; // lo twins (split mode)
-    std::vector<std::vector<float*>> act_lo_, dz_lo_;
-    float* W_lo_ = nullptr;
     bool gate_on_ = false;           // grouped wgrad forked next to the chain kernel, gated by device counters
     uint32_t* gate_ready_ = nullptr; // [L + 1] per-layer counters written by the chain kernel
     uint32_t* gate_step_ = nullptr;  // steps of THIS engine (bumped in front of the gated kernel)
-    bool w_lo_needed_ = false;       // 3xTF32: the chain kernel and the per-layer fwd / dgrad kernels load the weights' lo twins
-    float* x_lo_sets_[2] = {nullptr, nullptr};
-    GemmLo lo_fwd(int l, int mu) const;
-    GemmLo lo_dgrad(int l, int mu) const;
-    GemmLo lo_wgrad(int l, int mu) const;
     float* probs_all_ = nullptr;
     bool coalesced_ = false;
     float *x_stage_ = nullptr, *y_stage_ = nullptr, *loss_dev_ = nullptr, *loss_host_ = nullptr;

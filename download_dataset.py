@@ -3,7 +3,7 @@
 fetch MNIST-784 from OpenML, scale to [0,1], subtract the global mean, one-hot the labels,
 85/15 split with seed 42, write ``x_{train,val}.parquet`` + ``y_{train,val}.npy``.
 
-The B200 target environment has no network: ``--synthetic`` (or a failed download) writes
+The GPU machines may have no network: ``--synthetic`` (or a failed download) writes
 the deterministic MNIST-shaped synthetic set in the SAME file format instead, so train.py
 and the unmodified reference can both consume it.  Files go to ``data/mnist_784/`` - the
 directory train.py reads (the reference writes to ``../data`` and reads ``data``: a quirk

@@ -22,18 +22,10 @@ prod, mma, epi = t[0:256], t[256:512], t[512:768]
 t0 = min(v for v in t if v > 0)
 rel = lambda v: (v - t0) / 1000.0 if v > 0 else None
 print("producer tile issue times (us):", [round(rel(v), 2) for v in prod if v > 0])
-print("gemm: (start-after-act-wait, last-tile-landed, committed) | epilogue: (tmem_full seen, publish)")
+print("gemm: (start, accumulator complete) of math warp 1 | publish of the tile written after it")
 for g in range(14):
-    a, b, c = mma[3 * g:3 * g + 3]
-    e0, e1 = epi[2 * g:2 * g + 2]
+    a, b = mma[2 * g:2 * g + 2]
+    e = epi[g + 1]
     if a == 0:
         break
-    print(f"gemm {g:2d}: mma {rel(a):7.2f} {rel(b):7.2f} {rel(c):7.2f} | epi {rel(e0) if e0 else -1:7.2f} {rel(e1) if e1 else -1:7.2f}")
-
-print("fine stamps, gemm 2 (fwd layer 3): k-loop (after full wait, after commit) x4 | epilogue (after tmem_ld, after stores) x2")
-g = 2
-print(" mma:", [round(rel(v), 2) if v else None for v in mma[64 + 8 * g:64 + 8 * g + 8]])
-print(" epi:", [round(rel(v), 2) if v else None for v in epi[64 + 8 * g:64 + 8 * g + 4]])
-g = 3
-print(" mma:", [round(rel(v), 2) if v else None for v in mma[64 + 8 * g:64 + 8 * g + 8]])
-print(" epi:", [round(rel(v), 2) if v else None for v in epi[64 + 8 * g:64 + 8 * g + 4]])
+    print(f"gemm {g:2d}: mma {rel(a):7.2f} {rel(b):7.2f} | publish {rel(e) if e else -1:7.2f}")

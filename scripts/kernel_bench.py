@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Per-kernel device timing (CUDA events, warm-up, L2 flush between timed launches or
-back-to-back) of the sm_100a GEMM family on the shapes of the default MLP and of the
+back-to-back) of the sm_90a GEMM family on the shapes of the default MLP and of the
 hidden=8192 stress config.  Prints one JSON line per case with achieved bytes/s and the
-fraction of the measured HBM copy bandwidth (MEASURED_PEAKS.json)."""
+fraction of the HBM bandwidth (measured, from MEASURED_PEAKS.json, else the H100 SXM data sheet)."""
 import argparse
 import json
 import os
@@ -19,7 +19,7 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "_fallback": True}
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "_fallback": True}   # H100 SXM data sheet
 
 
 def time_fn(fn, iters, flush=None):
@@ -51,8 +51,7 @@ def time_rotating(fns, iters):
     """Back-to-back launches cycling through `len(fns)` instances of the same op on DISTINCT operand buffers whose total
     size is several times L2: every launch streams its weights from HBM (the previous launches evicted them) and the lines
     it evicts are CLEAN.  The per-iteration "cold" mode above flushes L2 with a read-modify-write pass, i.e. it leaves up to
-    126 MB of dirty lines whose write-back competes with the timed kernel's reads (pessimistic by up to 1.47x for a 268 MB
-    weight matrix); this mode is what a real step of a model larger than L2 looks like."""
+    50 MB (the H100's L2) of dirty lines whose write-back competes with the timed kernel's reads; this mode is what a real step of a model larger than L2 looks like."""
     for f in fns:
         f()
     torch.cuda.synchronize()
@@ -75,7 +74,7 @@ def main():
     args = ap.parse_args()
     pk = peaks()
     dev = "cuda"
-    flush = torch.zeros(160 * 1024 * 1024 // 4, device=dev)   # 160 MB > 126 MB L2
+    flush = torch.zeros(128 * 1024 * 1024 // 4, device=dev)   # 128 MB > 50 MB L2
     shapes = []
     if args.shapes in ("default", "all"):
         shapes += [(32, 784, 128), (32, 128, 127), (32, 123, 10), (4, 784, 128), (128, 784, 128)]
@@ -84,7 +83,7 @@ def main():
     for rows, k, n in shapes:
         x = torch.randn(rows, k, device=dev)
         ld = (k + 1 + 7) // 8 * 8
-        n_rot = max(1, min(4, int(3 * 126e6 // (n * ld * 4)) + 1)) if n * ld * 4 > 32e6 else 1   # >= 3 x L2 of distinct weights
+        n_rot = max(1, min(4, int(3 * 50e6 // (n * ld * 4)) + 1)) if n * ld * 4 > 16e6 else 1   # >= 3 x L2 of distinct weights
         Wbs = [torch.randn(n, ld, device=dev) for _ in range(n_rot)]
         Gbs = [torch.zeros(n, ld, device=dev) for _ in range(n_rot)]
         Wb, Gb = Wbs[0], Gbs[0]

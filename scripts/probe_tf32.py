@@ -1,4 +1,8 @@
-import sys; sys.path.insert(0, '/root/repo')
+"""What the TF32 GEMM path does to operand bits just past the 10-bit mantissa (both operand positions)."""
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from shallowspeed_b200.ops import cuda as K
 vals = {"1+2^-11+2^-12": 1 + 2**-11 + 2**-12, "1+2^-11 (tie)": 1 + 2**-11, "1+2^-10+2^-11 (tie)": 1 + 2**-10 + 2**-11,

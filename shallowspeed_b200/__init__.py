@@ -1,4 +1,4 @@
-"""shallowspeed_b200 - a Blackwell-native data + pipeline parallel MLP trainer with the
+"""shallowspeed_b200 - an H100-native data + pipeline parallel MLP trainer with the
 capabilities of siboehm/ShallowSpeed (see SURVEY.md / DESIGN.md)."""
 __version__ = "0.1.0"
 

@@ -8,12 +8,12 @@ on ANY layout -> DP == sequential), ``load_micro_batch_input/target(batch_id,
 mubatch_id)`` return contiguous row slices, ``get_num_batches``, ``get_num_mubatches``,
 ``len``.
 
-B200-first additions: there is no network in the target environment, so the dataset can
+GPU-first additions: the GPU machines may have no network, so the dataset can
 be *synthetic* (``synthetic_mnist``: class-conditional prototypes + noise with MNIST's
 shape, split sizes and normalisation - learnable, so accuracy curves still mean
 something); the shard lives either in pinned host memory (end-to-end path: one H2D copy
 per step) or resident in HBM (``device=...``; 59 500 x 784 fp32 = 187 MB, nothing next to
-180 GB); ``write_reference_files`` stores any dataset in the reference's on-disk format
+80 GB); ``write_reference_files`` stores any dataset in the reference's on-disk format
 (x_{split}.parquet + y_{split}.npy) so the unmodified reference can train on identical
 data.
 """

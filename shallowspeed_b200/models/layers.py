@@ -11,7 +11,7 @@ The class skeleton is the reference's on purpose: ``Module`` / ``ReLU`` / ``Soft
 cache keys (``bitmask_{id}`` / ``input_{id}``) and hook loops, because that API surface IS the parity requirement
 (layers.py:31-96, 169-233).  What is new here is everything underneath it:
 
-B200-first differences (design, not translation):
+GPU-first differences (design, not translation):
 
 * storage is ``torch.Tensor``; all parameters of a pipeline stage live in ONE flat
   fp32 arena (``ParamArena``) with a twin arena for gradients.  Each Linear owns an

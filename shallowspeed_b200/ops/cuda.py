@@ -1,4 +1,4 @@
-"""Python face of the hand-written sm_100a kernels (``csrc/kernels``).
+"""Python face of the hand-written sm_90a kernels (``csrc/kernels``).
 
 Every function here launches OUR kernels - there is no torch/cuBLAS fallback: if the
 native module is missing on a GPU box the import fails loudly (the driver checks which
@@ -14,7 +14,7 @@ try:
     from .. import _C  # built in-tree: python setup.py build_ext --inplace
 except ImportError as e:  # pragma: no cover
     raise ImportError(
-        "shallowspeed_b200._C (sm_100a kernels + runtime) is not built. Run "
+        "shallowspeed_b200._C (sm_90a kernels + runtime) is not built. Run "
         "`python setup.py build_ext --inplace` (or __graft_entry__.build())."
     ) from e
 
@@ -57,23 +57,14 @@ def _bias_arg(bias, out_dims):
 
 
 # ------------------------------------------------------------------ GEMMs
-# precision: "tf32" = one tcgen05.mma.kind::tf32 pass (operands truncated to 10 mantissa bits);
-#            "fp32" = 3xTF32: lo twins (x - trunc(x)) of both operands, three MMAs per k-slice, error ~2^-20.
+# precision: "tf32" = one TF32 tensor-core pass (operands truncated to 10 mantissa bits);
+#            "fp32" = 3xTF32: lo parts (x - trunc(x)) of both operands, derived in the kernel, three MMAs per k-slice,
+#            error ~2^-20.
 PRECISION = "fp32"
 
 
 def _split(precision):
     return (precision or PRECISION) in ("fp32", "fp32x3", "3xtf32")
-
-
-def lo_twin(t: torch.Tensor) -> torch.Tensor:
-    """lo = t - trunc_tf32(t), same padded layout as t (t must be tma_ready).  The split kernel writes the whole padded
-    storage (rows x pitch), so the buffer needs no memset: one kernel per twin, not two."""
-    base = torch.empty(t.size(0), t.stride(0), dtype=torch.float32, device=t.device)
-    lo = base[:, : t.size(1)]
-    assert lo.stride(0) == t.stride(0)
-    _C.split_lo(t, lo)
-    return lo
 
 
 def linear_fwd(x, weight, bias=None, relu=False, out=None, precision=None, k_splits=0):
@@ -82,10 +73,7 @@ def linear_fwd(x, weight, bias=None, relu=False, out=None, precision=None, k_spl
     rows, out_dims = x.size(0), weight.size(0)
     y = out if out is not None else empty_padded(rows, out_dims, x.device)
     b, bstride = _bias_arg(bias, out_dims)
-    if _split(precision):
-        _C.linear_fwd(x, weight, b, bstride, bool(relu), y, lo_twin(weight), lo_twin(x), None, int(k_splits))
-    else:
-        _C.linear_fwd(x, weight, b, bstride, bool(relu), y, None, None, None, int(k_splits))
+    _C.linear_fwd(x, weight, b, bstride, bool(relu), y, _split(precision), int(k_splits))
     return y
 
 
@@ -93,10 +81,7 @@ def linear_dgrad(dz, weight, mask=None, out=None, precision=None, k_splits=0):
     dz, weight = as_tma(dz), as_tma(weight)
     dx = out if out is not None else empty_padded(dz.size(0), weight.size(1), dz.device)
     m = None if mask is None else as_tma(mask)
-    if _split(precision):
-        _C.linear_dgrad(dz, weight, m, dx, lo_twin(weight), lo_twin(dz), None, int(k_splits))
-    else:
-        _C.linear_dgrad(dz, weight, m, dx, None, None, None, int(k_splits))
+    _C.linear_dgrad(dz, weight, m, dx, _split(precision), int(k_splits))
     return dx
 
 
@@ -105,10 +90,7 @@ def linear_wgrad(dz, x, grad_w, accumulate=False, grad_b=None, weight=None, lr=0
     ``weight`` (TMA reduce-add of -lr * dW)."""
     dz, x = as_tma(dz), as_tma(x)
     b, bstride = _bias_arg(grad_b, dz.size(1))
-    if _split(precision):
-        _C.linear_wgrad(dz, x, grad_w, bool(accumulate), b, bstride, weight, float(lr), bool(fuse_sgd), lo_twin(dz), lo_twin(x))
-    else:
-        _C.linear_wgrad(dz, x, grad_w, bool(accumulate), b, bstride, weight, float(lr), bool(fuse_sgd), None, None)
+    _C.linear_wgrad(dz, x, grad_w, bool(accumulate), b, bstride, weight, float(lr), bool(fuse_sgd), _split(precision))
     return grad_w
 
 

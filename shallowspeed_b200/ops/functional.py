@@ -2,15 +2,15 @@
 
 Capability parity with the reference's ``shallowspeed/functional.py:4-44``
 (relu, relu_grad, linear, linear_grad, softmax, softmax_grad, mse_loss,
-mse_loss_grad), re-designed for B200:
+mse_loss_grad), re-designed for the GPU:
 
 * tensors are ``torch.Tensor`` (fp32 storage);
-* on a CUDA device every op dispatches to a hand-written sm_100a kernel
-  (``csrc/kernels``: tcgen05/TMEM GEMMs fed by TMA for the three Linear GEMMs,
+* on a CUDA device every op dispatches to a hand-written sm_90a kernel
+  (``csrc/kernels``: tensor-core GEMMs fed by TMA for the three Linear GEMMs,
   a fused loss-head kernel for softmax/MSE) through ``shallowspeed_b200.ops.cuda``;
 * on CPU the same math runs through plain torch ops - this is the numerics
   oracle the GPU tests compare against, and the "plumbing" path that runs
-  without a GPU (BASELINE.json config 1).
+  without a GPU (the sequential CPU configuration).
 
 Numerical contracts kept from the reference (SURVEY.md section 2.2(4)):
 softmax shifts by the *global* max of the whole micro-batch and adds 1e-7 to

@@ -1,7 +1,7 @@
 """Optimizer.  Parity: ``SGD(parameters, lr).step()`` = ``param.data -= lr * param.grad``
 for trainable params (reference ``shallowspeed/optimizer.py:4-13``); stateless.
 
-B200: when all parameters are views into one ``ParamArena`` the update is a single fused
+GPU: when all parameters are views into one ``ParamArena`` the update is a single fused
 pass over the flat buffers (one multi-tensor kernel on CUDA, ``csrc/kernels/elementwise.cu``)
 instead of one axpy per parameter.  On the native engine's fused path the update happens
 inside the wgrad+all-reduce kernel and ``step`` is not called at all.

@@ -10,10 +10,10 @@ VM is backend agnostic.  Three implementations:
 
 * ``SelfComm``    - size-1 communicator (sequential training, no-ops).
 * ``TorchComm``   - a ``torch.distributed`` process group (NCCL over NVLink/NVSwitch on
-                    B200, gloo on CPU).
+                    GPUs, gloo on CPU).
 * ``ThreadComm``  - in-process fabric for fast multi-"rank" tests (threads + queues).
 
-The *hot* DP path on B200 does not go through this file at all: the native engine
+The *hot* DP path on GPUs does not go through this file at all: the native engine
 reduces gradients inside the wgrad kernel over peer memory (``csrc/kernels``).
 """
 from __future__ import annotations

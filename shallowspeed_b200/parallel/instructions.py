@@ -93,7 +93,7 @@ class BackwardGradAcc(MuBatchPipeInstr):
 class BackwardGradAllReduce(MuBatchPipeInstr):
     """Local backward of the LAST-processed micro-batch: every layer's gradient becomes
     final here, so the DP reduction of layer l is started as soon as it is computed and
-    overlaps the backward of layer l-1 (on B200: fused into the wgrad kernel)."""
+    overlaps the backward of layer l-1 (on the GPU: fused into the wgrad kernel)."""
 
     opcode = 8
 

@@ -6,7 +6,7 @@ dataset, optimizer)``, same ``execute(sched, batch_id)``, one method per instruc
 ``input_buffers`` / ``output_buffers`` readable after ``execute`` (train.py reads
 ``output_buffers[0]`` to compute accuracy).
 
-This VM is the portable path (CPU/gloo, debugging, numerics oracle).  On B200 the same
+This VM is the portable path (CPU/gloo, debugging, numerics oracle).  On a GPU the same
 instruction stream is lowered once into a static plan and run by the native executor
 (``parallel.engine`` -> ``csrc/runtime``) on CUDA streams + NCCL p2p + the fused
 in-kernel DP reduction.

@@ -3,7 +3,7 @@
 The reference only prints cumulative wall-clock per epoch (train.py:131-137).  For a
 multi-GPU trainer numbers must be taken on the device (CUDA events on the launching
 stream), reduced as MAX over ranks, and accompanied by the SM clocks seen during the
-timed region (B200_PROFILING.md "Timing hygiene").
+timed region.
 """
 from __future__ import annotations
 
@@ -60,8 +60,8 @@ _QUERY = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,
 
 
 class ClockSampler:
-    """Samples SM clocks / power / throttle reasons while a timed region runs (B200_PROFILING.md "clocks DURING the timed
-    region").  Preferred source: NVML in-process (a thread polling every ``period_ms``; works for regions of a few
+    """Samples SM clocks / power / throttle reasons while a timed region runs (the clocks DURING the timed
+    region, not before or after it).  Preferred source: NVML in-process (a thread polling every ``period_ms``; works for regions of a few
     milliseconds - the driver times 20 steps of ~0.1 ms); fallback: an ``nvidia-smi -lms`` child process, which needs
     ~100 ms to deliver its first line."""
 

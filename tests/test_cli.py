@@ -57,8 +57,8 @@ def test_train_rejects_bad_grids():
     assert r.returncode != 0            # 128 % 3 != 0 / world size mismatch
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(ROOT, "baseline", "_ref", "shallowspeed", "pipe.py")),
-                    reason="reference not installed in baseline/_ref")
+@pytest.mark.skipif(not os.path.exists(os.path.join(ROOT, "oracle", "_ref", "shallowspeed", "pipe.py")),
+                    reason="reference not installed in oracle/_ref (oracle/build_reference.py, run by build())")
 def test_bench_reference_arm_json_contract():
     r = _run(["bench.py", "--impl", "reference", "--steps", "5", "--warmup", "3"])
     assert r.returncode == 0, r.stderr[-2000:]
@@ -114,9 +114,9 @@ def test_tuning_file_ships_with_every_variant_off_and_env_wins(tmp_path, monkeyp
     import shallowspeed_b200 as pkg
 
     cfg = json.load(open(os.path.join(ROOT, "shallowspeed_b200", "tuning.json")))
-    # a switch is flipped only together with its measurement: every enabled one is named in profiles/variants_r2.md
-    notes = open(os.path.join(ROOT, "profiles", "variants_r2.md")).read()
-    assert all(k in notes for k, v in cfg.items() if k.startswith("SSB_") and v), "flip a switch only together with its measurement"
+    # a switch is flipped only together with its documentation: every enabled one is named in DESIGN.md
+    notes = open(os.path.join(ROOT, "DESIGN.md")).read()
+    assert all(k in notes for k, v in cfg.items() if k.startswith("SSB_") and v), "flip a switch only together with its documentation"
     assert pkg.TUNING == {} or all(k in os.environ for k in pkg.TUNING)
     # semantics of the loader, on a scratch copy
     import importlib.util
@@ -137,3 +137,36 @@ def test_tuning_file_ships_with_every_variant_off_and_env_wins(tmp_path, monkeyp
         assert applied == {"SSB_DEMO_ON": "1", "SSB_SPLITK": "2"} and "SSB_DEMO_OFF" not in os.environ
     finally:
         os.environ.pop("SSB_DEMO_ON", None)        # set by the loader itself, not by monkeypatch
+
+
+def test_bench_dump_outputs_stays_within_its_budget(tmp_path):
+    """--dump-outputs writes a small arena in full and a large one as a fixed, seeded sample with its positions, always
+    within the byte budget (64 MB by default; a tiny budget here so the arena is 'large')."""
+    import importlib.util
+    import types
+
+    import numpy as np
+    import torch
+
+    spec = importlib.util.spec_from_file_location("bench_under_test", os.path.join(ROOT, "bench.py"))
+    bench = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(bench)
+    assert bench.DUMP_LIMIT_BYTES == 64 << 20
+    w = torch.arange(200_000, dtype=torch.float32)
+    trainer = types.SimpleNamespace(model=types.SimpleNamespace(arena=types.SimpleNamespace(weights=w)),
+                                    pp_comm=types.SimpleNamespace(Get_rank=lambda: 0), is_last=True)
+    grid = types.SimpleNamespace(replica=0, pp=1)
+
+    full = tmp_path / "full"
+    bench.dump_outputs(str(full), trainer, 0.5, grid)
+    assert sorted(p.name for p in full.iterdir()) == ["loss.npy", "weights_stage0.npy"]
+    assert np.array_equal(np.load(full / "weights_stage0.npy"), w.numpy()) and np.load(full / "loss.npy")[0] == 0.5
+
+    limit = 64 << 10
+    for d in ("a", "b"):
+        bench.dump_outputs(str(tmp_path / d), trainer, 0.5, grid, limit_bytes=limit)
+        assert sum(p.stat().st_size for p in (tmp_path / d).iterdir()) <= limit
+    idx, vals = np.load(tmp_path / "a" / "weights_stage0_idx.npy"), np.load(tmp_path / "a" / "weights_stage0.npy")
+    assert len(idx) > 1000 and np.array_equal(vals, w.numpy()[idx])
+    assert np.array_equal(idx, np.load(tmp_path / "b" / "weights_stage0_idx.npy"))   # same positions on every run
+

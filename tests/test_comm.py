@@ -94,15 +94,18 @@ def test_watchdog_reports_and_aborts_on_timeout(monkeypatch):
     assert w._pp_nccl.aborted
 
 
-def test_fd_passing_over_unix_socket(tmp_path):
+def test_fd_passing_over_unix_socket():
     """NVLS set-up hands the multicast object's POSIX fd to the other replicas with SCM_RIGHTS; check the transport
     with a pipe: what the peers write into the received descriptors arrives at the leader's read end."""
     import os
+    import tempfile
 
     from shallowspeed_b200.parallel import engine as E
 
     r, w = os.pipe()
-    path = str(tmp_path / "fd.sock")
+    # a unix socket path is limited to ~108 bytes, which a deeply nested temporary directory can exceed
+    sock_dir = tempfile.mkdtemp(prefix="ssb_fd_", dir="/tmp")
+    path = os.path.join(sock_dir, "fd.sock")
     srv = E.serve_fd(path, w, 2)
     got = []
 
@@ -122,6 +125,7 @@ def test_fd_passing_over_unix_socket(tmp_path):
     assert sorted(os.read(r, 16)) == [65, 66] and sorted(got) == [0, 1]
     os.close(r)
     assert not os.path.exists(path)
+    os.rmdir(sock_dir)
 
 
 def test_nvls_requires_support_and_is_reported_unavailable_on_cpu():

@@ -32,7 +32,7 @@ def _tiles(sizes):
 def test_tile_counts_of_the_reference_model():
     t = _tiles(SIZES)
     assert t == [25, 4, 4, 4, 4, 4, 4]          # in / 32 tiles per layer (out <= 128: one row of tiles)
-    assert sum(t) == 49                          # + 4 chain CTAs: co-resident on 148 SMs
+    assert sum(t) == 49                          # + 4 chain CTAs: co-resident on 132 SMs
 
 
 @pytest.mark.parametrize("dp", [2, 4, 8])

@@ -1,4 +1,4 @@
-"""Numerics of every hand-written sm_100a kernel against a plain PyTorch fp32 reference
+"""Numerics of every hand-written sm_90a kernel against a plain PyTorch fp32 reference
 of the same op.  TF32 tensor-core math (10-bit mantissa products, fp32 accumulate) =>
 tolerances are relative to the magnitude of the result."""
 import pytest
@@ -156,14 +156,12 @@ def test_module_path_matches_cpu():
 
 
 # ---------------------------------------------------------------------------------------------------------
-# How close to fp32 is the 3xTF32 scheme REALLY?  Same inputs through (a) our tcgen05 kernels in fp32 mode and
-# (b) torch.matmul in true fp32 (TF32 disabled), both measured against an fp64 oracle.  What limits 3xTF32 on tcgen05 is
-# not the operand split (error 2^-21 per product) but the tensor core's accumulate step, which truncates: the error grows
-# linearly with the number of accumulate steps n (~0.7 n 2^-24), where cuBLAS' FFMA chain rounds to nearest (~sqrt(K)).
-# First measurement (one accumulator, n = 3K/8): 4x cuBLAS at K=128, 22x at K=784, 148x at K=8192.  The kernels now keep
-# the small cross terms in their own accumulator and rotate the hi*hi products of long reductions over 4 accumulators
-# (n = K/32), split-K divides n further.  Asserted: within 8x of cuBLAS fp32 for K <= 2048, within 32x at K = 8192 without
-# split-K; the measured numbers are printed (-s) and recorded in profiles/precision_r2.md.
+# How close to fp32 is the 3xTF32 scheme REALLY?  Same inputs through (a) our tensor-core kernels in fp32 mode and
+# (b) torch.matmul in true fp32 (TF32 disabled), both measured against an fp64 oracle.  What limits 3xTF32 is not the
+# operand split (error 2^-21 per product) but the tensor core's accumulate step, whose error grows with the number of
+# accumulate steps, where cuBLAS' FFMA chain rounds to nearest.  The kernels therefore sum each 32-wide k-block in a fresh
+# tensor-core accumulator and add the k-block sums in fp32 (ptx.cuh warp_mma_kblock).  Asserted: within 8x of cuBLAS fp32
+# for K <= 2048, within 32x at K = 8192; the measured numbers are printed (-s).
 # ---------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("rows,k,n", [(32, 784, 128), (128, 784, 128), (32, 128, 127), (32, 123, 10), (128, 2048, 512), (8, 8192, 256)])
 def test_3xtf32_error_next_to_cublas_fp32(rows, k, n):

@@ -155,7 +155,7 @@ def test_dp2_pp4_gpipe(tmp_path):
 
 
 def test_wide_model_dp2_fused(tmp_path):
-    """layers wider than 128: per-layer tcgen05 GEMM kernels (no chain), multi-tile fused wgrad+DP kernels,
+    """layers wider than 128: per-layer tensor-core GEMM kernels (no chain), multi-tile fused wgrad+DP kernels,
     two-shot single-owner protocol on the 4 MB layers"""
     _run(2, 1, "naive", "fused", tmp_path, sizes=WIDE)
 
@@ -166,7 +166,6 @@ def test_wide_model_dp2_pp2_1f1b(tmp_path):
 
 # ---------------------------------------------------------------------------------------------------------
 # NVLS path (--comm nvls): the switch reduces the gradient arena and multicasts the updated weights.
-# Validated on 2 x B200 in round 2 (profiles/raw/session_b_pytest_multi.log).
 # ---------------------------------------------------------------------------------------------------------
 
 
@@ -179,7 +178,7 @@ def test_nvls_reduce_sgd_matches_oracle(dp, pp, sched, coalesce, tmp_path):
 
 # ---------------------------------------------------------------------------------------------------------
 # Peer-memory pipeline transport (--pp-transport peer / SSB_PP_PEER=1): one-sided pushes + epoch flags instead of
-# NCCL send/recv.  Validated on 2 x B200 in round 2.
+# NCCL send/recv.
 # ---------------------------------------------------------------------------------------------------------
 
 

@@ -110,34 +110,25 @@ def test_microbatch_accumulation_equals_full_batch():
         assert torch.allclose(p.grad, q.grad, atol=2e-6)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/shallowspeed"), reason="reference not mounted")
 def test_matches_reference_model_numerics():
-    """Same init, same forward, same gradients as the reference's NumPy model."""
-    import sys
-
-    sys.path.insert(0, "/root/reference")
-    try:
-        from shallowspeed.layers import MLP as RefMLP
-    finally:
-        sys.path.pop(0)
-    import contextlib
-    import io
-
+    """Same init, same forward, same gradients as the original NumPy model (tests/golden/reference_mlp_numerics.npz:
+    its output and a fixed sample of every parameter's initial value and gradient)."""
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_mlp_numerics.npz"))
     sizes = [784, 128, 127, 126, 125, 124, 123, 10]
-    with contextlib.redirect_stdout(io.StringIO()):
-        ref = RefMLP(sizes, 0, 1, 128)
     ours = MLP(sizes, 0, 1, 128)
-    for rp, p in zip(ref.parameters(), ours.parameters()):
-        # under NumPy >= 2 the reference's weights silently become fp64 (SURVEY.md fact 5);
-        # the intended fp32 values agree to 1 ulp
-        assert np.allclose(rp.data.astype(np.float32), p.data.numpy(), atol=1e-7, rtol=0)
+    params = list(ours.parameters())
+    assert len(params) == len(g["counts"])
+    bounds = np.concatenate([[0], np.cumsum(g["counts"])])
+    sample = [slice(bounds[i], bounds[i + 1]) for i in range(len(params))]
+    for i, p in enumerate(params):
+        assert tuple(p.data.shape) == tuple(int(d) for d in g["shapes"][i] if d >= 0)
+        # the original's weights become fp64 under NumPy >= 2; the intended fp32 values agree to 1 ulp
+        assert np.allclose(g["init"][sample[i]], p.data.numpy().reshape(-1)[g["idx"][sample[i]]], atol=1e-7, rtol=0)
     rs = np.random.RandomState(0)
     x = rs.randn(32, 784).astype(np.float32)
     t = np.eye(10, dtype=np.float32)[rs.randint(0, 10, 32)]
-    out_ref = ref.forward(x, 0)
     out = ours.forward(torch.from_numpy(x), 0)
-    assert np.allclose(out_ref, out.numpy(), atol=1e-5)
-    ref.backward(t, 0)
+    assert np.allclose(g["output"], out.numpy(), atol=1e-5)
     ours.backward(torch.from_numpy(t), 0)
-    for rp, p in zip(ref.parameters(), ours.parameters()):
-        assert np.allclose(rp.grad, p.grad.numpy(), atol=1e-5)
+    for i, p in enumerate(params):
+        assert np.allclose(g["grad"][sample[i]], p.grad.numpy().reshape(-1)[g["idx"][sample[i]]], atol=1e-5)

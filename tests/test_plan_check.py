@@ -15,7 +15,7 @@ GOOD = """
 8 record_event stream=6 event=3
 9 wait_event stream=0 event=2
 10 wait_event stream=0 event=3
-11 split_lo stream=0
+11 sgd stream=0
 12 loss_d2h stream=0
 """
 

@@ -22,8 +22,8 @@ def test_planner_never_leaves_a_split_empty_and_keeps_two_ctas_per_sm_in_smem(sm
                 assert grid_z == splits
                 assert (splits - 1) * per < num_kb <= splits * per          # every split owns >= 1 k-block
                 assert per >= 8                                              # enough work to fill the pipeline
-                tiles = ((m + 127) // 128) * ((rows + (256 if rows >= 256 else (rows + 15) // 16 * 16) - 1)
-                                               // (256 if rows >= 256 else (rows + 15) // 16 * 16))
+                bn = 64 if rows >= 64 else (rows + 15) // 16 * 16
+                tiles = ((m + 127) // 128) * ((rows + bn - 1) // bn)
                 assert tiles * 2 <= sms and tiles * splits <= 2 * sms + tiles
                 assert 2 <= stages <= 6 and smem <= 113 * 1024               # two CTAs per SM fit
     assert seen_split > 20
@@ -42,20 +42,19 @@ def test_chain_budget_fits_the_sm_and_keeps_a_double_buffered_ring():
     for split in (False, True):
         for mb in (1, 4, 16, 32, 33, 64, 96, 128):
             ok, kps, stages, smem = _C.chain_budget(mb, split)
-            if not ok:
-                assert split and mb > 48            # only the fp32 twin buffers of big micro-batches do not fit
-                continue
+            assert ok                               # 3xTF32 derives its lo parts in registers: no twin buffers
             assert kps in (1, 2, 4) and 2 <= stages <= 8
-            assert smem <= 227 * 1024               # opt-in dynamic shared memory limit of an sm_100a CTA
+            assert smem <= 227 * 1024               # opt-in dynamic shared memory limit of an sm_90a CTA
     assert _C.chain_budget(32, False)[:3] == (True, 4, 2)      # the flagship config: K=128 per stage, double-buffered
-    assert _C.chain_budget(32, True)[0] and _C.chain_budget(128, False)[0] and not _C.chain_budget(128, True)[0]
+    assert _C.chain_budget(32, True)[:3] == (True, 4, 2)
+    assert not _C.chain_budget(129, False)[0]
 
 
 def test_chain_eligibility_rules():
     ref = [(784, 128), (128, 127), (127, 126), (126, 125), (125, 124), (124, 123), (123, 10)]
     assert _C.chain_eligible(ref, 32, 10, True, False) and _C.chain_eligible(ref, 32, 10, True, True)
     assert _C.chain_eligible(ref, 128, 10, True, False)
-    assert not _C.chain_eligible(ref, 128, 10, True, True)            # falls back to the per-layer kernels
+    assert _C.chain_eligible(ref, 128, 10, True, True)                # fp32 (3xTF32) needs no extra shared memory
     assert not _C.chain_eligible([(784, 256), (256, 10)], 32, 10, True, False)     # wider than one M tile
     assert not _C.chain_eligible([(784, 128), (128, 64)], 32, 64, True, False)     # loss head handles <= 32 classes
     assert _C.chain_eligible([(784, 128), (128, 64)], 32, 64, False, False)        # ... but a middle stage may be 64 wide

@@ -1,9 +1,8 @@
 """Bit-level model of the fp32-equivalent tensor-core scheme (3xTF32), on the CPU.
 
-Hardware fact (probed on B200, scripts/probe_tf32.py): ``tcgen05.mma.kind::tf32`` TRUNCATES its fp32 operands to 10 mantissa
-bits (round toward zero).  So hi(x) = x with the low 13 bits cleared is exactly what the tensor core sees when it is handed
-the raw fp32 tile, lo(x) = x - hi(x) is exactly representable in fp32 and has itself <= 13 significant bits (it survives a
-second truncation with at most a 2^-10 relative loss), and
+The kernels hand the tensor core hi(x) = x with the low 13 mantissa bits cleared (truncation, csrc/kernels/ptx.cuh), so
+lo(x) = x - hi(x) is exactly representable in fp32 and has itself <= 13 significant bits (it survives a second truncation
+to tf32 with at most a 2^-10 relative loss), and
 
         a*b  ~=  lo(a)*hi(b) + hi(a)*lo(b) + hi(a)*hi(b)          (the lo*lo term, ~2^-22 relative, is dropped)
 
@@ -58,7 +57,7 @@ def test_dropped_lo_lo_term_is_the_only_systematic_error():
     b = rng.standard_normal((4096, 8)).astype(np.float32)
     exact_products = a.astype(np.float64) @ b.astype(np.float64)
     lolo = lo(a).astype(np.float64) @ lo(b).astype(np.float64)
-    # the lo twins are truncated once more by the tensor core: that loses at most 2^-10 of a term that is itself 2^-11 small
+    # the lo parts are truncated once more by the tensor core: that loses at most 2^-10 of a term that is itself 2^-11 small
     resid = exact_products - mm_3xtf32(a, b) - lolo
     assert np.abs(lolo).max() < 1e-4 * np.abs(exact_products).max()
     assert np.abs(resid).max() < 4e-6 * np.abs(exact_products).max()

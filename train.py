@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Training driver.  Same CLI as the reference's ``train.py`` (``--dp/--pp/--schedule``,
 train.py:63-76) - plus the knobs the reference hard-codes as module constants
-(train.py:56-59, 98, 107, 111) and the B200 runtime options.
+(train.py:56-59, 98, 107, 111) and the GPU runtime options.
 
 Launch (one process per GPU / per (dp, pp) cell):
 
@@ -85,7 +85,7 @@ def build_parser():
     # runtime
     p.add_argument("--device", choices=["auto", "cpu", "cuda"], default="auto")
     p.add_argument("--engine", choices=["auto", "python", "native"], default="auto",
-                   help="python = portable instruction VM; native = C++ executor + sm_100a kernels")
+                   help="python = portable instruction VM; native = C++ executor + sm_90a kernels")
     p.add_argument("--comm", choices=["fused", "nccl", "nvls"], default="fused",
                    help="native engine DP path: in-kernel reduction over peer memory, or plain NCCL all-reduce (A/B baseline)")
     p.add_argument("--pp-transport", choices=["nccl", "peer"], default=None,

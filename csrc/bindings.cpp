@@ -84,19 +84,29 @@ static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<
 }
 
 // G[out, in] (+)= dz^T @ x ; db[out] (+)= colsum(dz) ; optionally W -= lr * (G + ...)
+// With momentum / weight decay the fused update follows the stateful rule; V is the momentum buffer with W's layout
+// (same row pitch; its column `in` belongs to the bias).
 static void linear_wgrad(const Tensor& dz, const Tensor& x, Tensor& G, bool accumulate, const c10::optional<Tensor>& db,
                          int64_t db_stride, const c10::optional<Tensor>& W, double lr, bool fuse_sgd,
-                         bool split) {
+                         bool split, const c10::optional<Tensor>& V, double momentum, double weight_decay, bool nesterov) {
     check_mat(dz, "dz"); check_mat(x, "x"); check_mat(G, "G");
     const int rows = dz.size(0), out = dz.size(1), in = x.size(1);
     TORCH_CHECK(x.size(0) == rows && G.size(0) == out && G.size(1) == in, "linear_wgrad: shape mismatch");
+    ssb::SgdState opt;
+    opt.momentum = (float)momentum; opt.weight_decay = (float)weight_decay; opt.nesterov = nesterov ? 1 : 0;
+    if (V.has_value()) {
+        check_mat(*V, "V");
+        TORCH_CHECK(W.has_value() && V->size(0) == out && V->size(1) == in && ld_of(*V) == ld_of(*W),
+                    "linear_wgrad: V must have W's shape and row pitch");
+        opt.V = V->data_ptr<float>();
+    }
     c10::cuda::CUDAGuard guard(dz.device());
     ssb::GemmPlan plan;
     const char* err = ssb::gemm_plan_wgrad(&plan, dz.data_ptr<float>(), ld_of(dz), x.data_ptr<float>(), ld_of(x),
                                            G.data_ptr<float>(), ld_of(G), rows, in, out, accumulate,
                                            db.has_value() ? db->data_ptr<float>() : nullptr, (int)db_stride,
                                            W.has_value() ? W->data_ptr<float>() : nullptr,
-                                           W.has_value() ? ld_of(*W) : 0, (float)lr, fuse_sgd, split);
+                                           W.has_value() ? ld_of(*W) : 0, (float)lr, fuse_sgd, split, opt);
     TORCH_CHECK(err == nullptr, "linear_wgrad: ", err ? err : "");
     cuda_ok(ssb::gemm_launch(plan, cur_stream()), "linear_wgrad launch");
 }
@@ -142,6 +152,22 @@ static void sgd_(Tensor& w, const Tensor& g, double lr) {
     c10::cuda::CUDAGuard guard(w.device());
     cuda_ok(ssb::launch_sgd(w.data_ptr<float>(), g.data_ptr<float>(), (float)lr, w.numel(), cur_stream()), "sgd");
 }
+static void sgd_momentum_(Tensor& w, const Tensor& g, const c10::optional<Tensor>& v, double lr, double momentum,
+                          double weight_decay, bool nesterov) {
+    TORCH_CHECK(w.is_contiguous() && g.is_contiguous() && w.numel() == g.numel());
+    TORCH_CHECK(w.scalar_type() == torch::kFloat32 && g.scalar_type() == torch::kFloat32);
+    ssb::SgdState opt;
+    opt.momentum = (float)momentum; opt.weight_decay = (float)weight_decay; opt.nesterov = nesterov ? 1 : 0;
+    if (v.has_value()) {
+        TORCH_CHECK(v->is_contiguous() && v->numel() == w.numel() && v->scalar_type() == torch::kFloat32 && v->is_cuda());
+        opt.V = v->data_ptr<float>();
+    }
+    const char* err = ssb::sgd_state_check(opt);
+    TORCH_CHECK(err == nullptr, "sgd_momentum_: ", err ? err : "");
+    c10::cuda::CUDAGuard guard(w.device());
+    cuda_ok(ssb::launch_sgd_momentum(w.data_ptr<float>(), g.data_ptr<float>(), (float)lr, opt, w.numel(), cur_stream()),
+            "sgd_momentum");
+}
 static void argmax_correct(const Tensor& pred, const Tensor& target, Tensor& correct) {
     check_mat(pred, "pred"); check_mat(target, "target");
     TORCH_CHECK(correct.scalar_type() == torch::kInt32 && correct.is_cuda());
@@ -157,13 +183,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("linear_dgrad", &linear_dgrad, py::arg("dz"), py::arg("W"), py::arg("mask"), py::arg("dx"),
           py::arg("split") = false, py::arg("k_splits") = 0);
     m.def("linear_wgrad", &linear_wgrad, py::arg("dz"), py::arg("x"), py::arg("G"), py::arg("accumulate"), py::arg("db"),
-          py::arg("db_stride"), py::arg("W"), py::arg("lr"), py::arg("fuse_sgd"), py::arg("split") = false);
+          py::arg("db_stride"), py::arg("W"), py::arg("lr"), py::arg("fuse_sgd"), py::arg("split") = false,
+          py::arg("V") = py::none(), py::arg("momentum") = 0.0, py::arg("weight_decay") = 0.0, py::arg("nesterov") = false);
     m.def("loss_head", &loss_head);
     m.def("softmax_grad", &softmax_grad);
     m.def("relu_mask_", &relu_mask_);
     m.def("relu_fwd", &relu_fwd);
     m.def("axpby", &axpby);
     m.def("sgd_", &sgd_);
+    m.def("sgd_momentum_", &sgd_momentum_, py::arg("w"), py::arg("g"), py::arg("v"), py::arg("lr"), py::arg("momentum"),
+          py::arg("weight_decay"), py::arg("nesterov"));
     m.def("argmax_correct", &argmax_correct);
     m.def("gemm_kernel_count", &ssb::gemm_kernel_count);
     m.def("chain_budget", [](int mb_rows, bool split) {
@@ -203,6 +232,18 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         return std::make_tuple(splits, per, (int)plan.grid.z, plan.p.stages, plan.smem_bytes, err);
     });
     // LL data-parallel kernel: host-side geometry (tiles per layer, lines per landing zone), callable without a GPU
+    // owner rank of every parameter element of one layer ([out, in + 1], bias last; -1 = every replica), no GPU needed
+    m.def("dp_owner_map", [](int proto, int in, int out, int ld, int64_t offset, int dp) {
+        torch::Tensor t = torch::empty({out, in + 1}, torch::kInt8);
+        auto a = t.accessor<int8_t, 2>();
+        for (int mm = 0; mm < out; ++mm)
+            for (int nn = 0; nn <= in; ++nn) a[mm][nn] = (int8_t)ssb::dp_element_owner(proto, in, out, ld, offset, dp, mm, nn);
+        return t;
+    });
+    m.attr("DP_PROTO_ALL") = (int)ssb::DP_PROTO_ALL;
+    m.attr("DP_PROTO_LL") = (int)ssb::DP_PROTO_LL;
+    m.attr("DP_PROTO_TWO_SHOT") = (int)ssb::DP_PROTO_TWO_SHOT;
+    m.attr("DP_PROTO_NVLS") = (int)ssb::DP_PROTO_NVLS;
     m.def("dp_ll_tiles", [](int in, int out) { return ssb::dp_ll_tiles(in, out); });
     m.def("dp_ll_zone_lines", [](int dp, int n_tiles) { return (int64_t)ssb::dp_ll_zone_lines(dp, n_tiles); });
     // Exercises the C++ runtime features that break when libstdc++ is linked statically next to torch's dynamic

@@ -67,7 +67,9 @@ __device__ __forceinline__ unsigned long long gtime_ll() {
 // optional phase timeline (SSB_CHAIN_TIMELINE=1): 8 stamps per tile, written by the tile's first epilogue thread
 #define LLDBG(i) do { if (p.dbg != nullptr && etid == 0 && e.tile < 28) p.dbg[8 * e.tile + (i)] = gtime_ll(); } while (0)
 
-template <int DP>
+// STATEFUL: momentum / weight decay in phase B through sgd_direction; the owner of a row keeps its momentum in its LOCAL
+// arena (p.opt.V, loaded with the weights before the first wait) and never sends it.
+template <int DP, bool STATEFUL = false>
 __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntry* __restrict__ entries, const DpLLParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
@@ -185,6 +187,7 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
             for (int i0 = etid; i0 < n_lines; i0 += 128 * kLB) {
                 uint4 ln[kLB][DP];
                 float wv0[kLB], wv1[kLB];
+                float vv0[kLB], vv1[kLB];                // momentum (STATEFUL only)
 #pragma unroll
                 for (int u = 0; u < kLB; ++u) {
                     const int idx = i0 + 128 * u;
@@ -197,6 +200,11 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
                     const int n = j < 16 ? e.n0 + 2 * j : e.n_total;
                     wv0[u] = (j == 16 || n < e.n_total) ? wrow[n] : 0.f;
                     wv1[u] = (j < 16 && n + 1 < e.n_total) ? wrow[n + 1] : 0.f;
+                    if constexpr (STATEFUL) {
+                        const float* vrow = p.opt.V != nullptr ? p.opt.V + (wrow - p.W) : nullptr;
+                        vv0[u] = (vrow != nullptr && (j == 16 || n < e.n_total)) ? vrow[n] : 0.f;
+                        vv1[u] = (vrow != nullptr && j < 16 && n + 1 < e.n_total) ? vrow[n + 1] : 0.f;
+                    }
                 }
 #pragma unroll
                 for (int u = 0; u < kLB; ++u) {
@@ -221,6 +229,22 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
                     const int row = p.rank * rpo + r;            // row inside the tile
                     float* wrow = p.W + e.w_offset + (int64_t)(e.m0 + row) * e.ldw;
                     float w0 = 0.f, w1 = 0.f;
+                    if constexpr (STATEFUL) {                    // s0 / s1 become the step directions
+                        const float mu = p.opt.momentum, wd = p.opt.weight_decay;
+                        const bool nv = p.opt.nesterov != 0;
+                        s0 = sgd_direction<false>(s0, wv0[u], vv0[u], mu, wd, nv);
+                        s1 = sgd_direction<false>(s1, wv1[u], vv1[u], mu, wd, nv);
+                        if (p.opt.V != nullptr) {
+                            float* vrow = p.opt.V + (wrow - p.W);
+                            if (j < 16) {
+                                const int n = e.n0 + 2 * j;
+                                if (n < e.n_total) vrow[n] = vv0[u];
+                                if (n + 1 < e.n_total) vrow[n + 1] = vv1[u];
+                            } else {
+                                vrow[e.n_total] = vv0[u];
+                            }
+                        }
+                    }
                     if (j < 16) {
                         const int n = e.n0 + 2 * j;
                         if (n < e.n_total) { w0 = wv0[u] - p.lr * s0; wrow[n] = w0; }
@@ -339,14 +363,27 @@ cudaError_t dp_ll_configure() {
     cudaError_t err;
     if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
     if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
-    return cudaFuncSetAttribute(dp_ll_wgrad_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
+    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
+    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
+    return cudaFuncSetAttribute(dp_ll_wgrad_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
 }
 
 cudaError_t launch_dp_ll(const DpLLPlan& plan, cudaStream_t stream) {
+    const bool stateful = plan.p.opt.momentum != 0.f || plan.p.opt.weight_decay != 0.f;
     switch (plan.p.dp) {
-        case 2: dp_ll_wgrad_kernel<2><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p); break;
-        case 4: dp_ll_wgrad_kernel<4><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p); break;
-        case 8: dp_ll_wgrad_kernel<8><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p); break;
+        case 2:
+            if (stateful) dp_ll_wgrad_kernel<2, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
+            else dp_ll_wgrad_kernel<2><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
+            break;
+        case 4:
+            if (stateful) dp_ll_wgrad_kernel<4, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
+            else dp_ll_wgrad_kernel<4><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
+            break;
+        case 8:
+            if (stateful) dp_ll_wgrad_kernel<8, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
+            else dp_ll_wgrad_kernel<8><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
+            break;
         default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();

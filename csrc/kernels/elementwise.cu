@@ -180,6 +180,56 @@ cudaError_t launch_sgd(float* w, const float* g, float lr, long n, cudaStream_t 
     return cudaGetLastError();
 }
 
+// flat-arena SGD with the stateful rule (sgd_direction): same float4 body and scalar tail as sgd_kernel, plus the
+// momentum buffer v (nullptr when momentum == 0: weight decay alone keeps no state).
+__device__ __forceinline__ float sgd_momentum_elem(float w, float g, float* v, long i, float lr, float mu, float wd,
+                                                   bool nesterov) {
+    float vi = v != nullptr ? v[i] : 0.f;
+    const float d = sgd_direction<false>(g, w, vi, mu, wd, nesterov);
+    if (v != nullptr) v[i] = vi;
+    return w - lr * d;
+}
+__global__ void __launch_bounds__(256) sgd_momentum_kernel(float4* __restrict__ w, const float4* __restrict__ g,
+                                                           float4* __restrict__ v, float lr, float mu, float wd,
+                                                           int nesterov, long n4) {
+    const long stride = (long)gridDim.x * blockDim.x;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += stride) {
+        float4 a = w[i];
+        const float4 b = g[i];
+        float4 m = v != nullptr ? v[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+        const bool nv = nesterov != 0;
+        a.x -= lr * sgd_direction<false>(b.x, a.x, m.x, mu, wd, nv);
+        a.y -= lr * sgd_direction<false>(b.y, a.y, m.y, mu, wd, nv);
+        a.z -= lr * sgd_direction<false>(b.z, a.z, m.z, mu, wd, nv);
+        a.w -= lr * sgd_direction<false>(b.w, a.w, m.w, mu, wd, nv);
+        if (v != nullptr) v[i] = m;
+        w[i] = a;
+    }
+}
+__global__ void sgd_momentum_tail_kernel(float* w, const float* g, float* v, float lr, float mu, float wd, int nesterov,
+                                         long start, long n) {
+    const long i = start + blockIdx.x * (long)blockDim.x + threadIdx.x;
+    if (i < n) w[i] = sgd_momentum_elem(w[i], g[i], v, i, lr, mu, wd, nesterov != 0);
+}
+cudaError_t launch_sgd_momentum(float* w, const float* g, float lr, const SgdState& opt, long n, cudaStream_t stream) {
+    if (sgd_state_check(opt) != nullptr) return cudaErrorInvalidValue;
+    float* v = opt.V;
+    const bool aligned = ((reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(v)) & 15) == 0;
+    const long n4 = aligned ? n / 4 : 0;
+    if (n4 > 0) {
+        long blocks = (n4 + 255) / 256;
+        if (blocks > 132 * 8) blocks = 132 * 8;
+        sgd_momentum_kernel<<<(int)blocks, 256, 0, stream>>>(reinterpret_cast<float4*>(w), reinterpret_cast<const float4*>(g),
+                                                             reinterpret_cast<float4*>(v), lr, opt.momentum, opt.weight_decay,
+                                                             opt.nesterov, n4);
+    }
+    const long done = n4 * 4;
+    if (done < n)
+        sgd_momentum_tail_kernel<<<(int)((n - done + 255) / 256), 256, 0, stream>>>(w, g, v, lr, opt.momentum, opt.weight_decay,
+                                                                                  opt.nesterov, done, n);
+    return cudaGetLastError();
+}
+
 // one warp per row: argmax(pred) == argmax(target) (first maximum wins, like numpy.argmax)
 __global__ void argmax_correct_kernel(const float* __restrict__ pred, int ldp, const float* __restrict__ target, int ldt,
                                       int rows, int cols, int* correct) {

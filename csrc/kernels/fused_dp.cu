@@ -65,8 +65,19 @@ __device__ __forceinline__ float* stage_slot(const DpPeers& peers, const DpLayer
            (p.one_shot ? (int64_t)(epoch & 1u) * p.stage_parity_stride : 0);
 }
 
+// one element of the stateful rule: reads and writes the local momentum at arena offset `off`
+__device__ __forceinline__ float elem_direction(const DpLayerParams& p, int64_t off, float g, float w) {
+    float v = p.opt.V != nullptr ? p.opt.V[off] : 0.f;
+    const float d = sgd_direction<false>(g, w, v, p.opt.momentum, p.opt.weight_decay, p.opt.nesterov != 0);
+    if (p.opt.V != nullptr) p.opt.V[off] = v;
+    return d;
+}
+
 // ---- phase B: the owner reduces one tile in rank order, applies SGD, publishes the weights
 // Executed by `nthreads` threads (tid in [0, nthreads)), all of which must call it.
+// STATEFUL: momentum / weight decay through sgd_direction; the momentum of the tile lives in the reducing replica's
+// LOCAL arena p.opt.V (the owner's, or every replica's own with one_shot) and is never published.
+template <bool STATEFUL>
 __device__ void dp_owner_reduce_tile(const DpPeers& peers, const DpLayerParams& p, const TileCoord& tc, uint32_t epoch,
                                      int tid, int nthreads, int bar_id, int part = 0, int nparts = 1, bool publish = true) {
     const int me = p.rank;
@@ -123,13 +134,26 @@ __device__ void dp_owner_reduce_tile(const DpPeers& peers, const DpLayerParams& 
             const int64_t woff = p.w_offset + (int64_t)m * p.ldw + n;
             if (vec_ok && n + 3 < p.n_total) {
                 float4 w = wv[u];
+                if constexpr (STATEFUL) {                      // sum becomes the step direction
+                    float4* vp = p.opt.V != nullptr ? reinterpret_cast<float4*>(p.opt.V + woff) : nullptr;
+                    float4 v = vp != nullptr ? *vp : make_float4(0.f, 0.f, 0.f, 0.f);
+                    const float mu = p.opt.momentum, wd = p.opt.weight_decay;
+                    const bool nv = p.opt.nesterov != 0;
+                    sum.x = sgd_direction<false>(sum.x, w.x, v.x, mu, wd, nv);
+                    sum.y = sgd_direction<false>(sum.y, w.y, v.y, mu, wd, nv);
+                    sum.z = sgd_direction<false>(sum.z, w.z, v.z, mu, wd, nv);
+                    sum.w = sgd_direction<false>(sum.w, w.w, v.w, mu, wd, nv);
+                    if (vp != nullptr) *vp = v;
+                }
                 w.x -= p.lr * sum.x; w.y -= p.lr * sum.y; w.z -= p.lr * sum.z; w.w -= p.lr * sum.w;
                 if (n_pub == 1) *reinterpret_cast<float4*>(peers.W[me] + woff) = w;
                 else for (int r2 = 0; r2 < p.dp; ++r2) *reinterpret_cast<float4*>(peers.W[r2] + woff) = w;   // publish to all replicas
             } else {
                 const float sv[4] = {sum.x, sum.y, sum.z, sum.w};
                 for (int e = 0; e < 4 && n + e < p.n_total; ++e) {
-                    const float w = peers.W[me][woff + e] - p.lr * sv[e];
+                    float d = sv[e];
+                    if constexpr (STATEFUL) d = elem_direction(p, woff + e, d, peers.W[me][woff + e]);
+                    const float w = peers.W[me][woff + e] - p.lr * d;
                     if (n_pub == 1) peers.W[me][woff + e] = w;
                     else for (int r2 = 0; r2 < p.dp; ++r2) peers.W[r2][woff + e] = w;
                 }
@@ -144,6 +168,7 @@ __device__ void dp_owner_reduce_tile(const DpPeers& peers, const DpLayerParams& 
             for (int s = 0; s < p.dp; ++s)
                 sum += ld_cg_f(st0 + (int64_t)s * p.stage_src_stride + (int64_t)kBlockM * p.block_n + r);
             const int64_t boff = p.w_offset + (int64_t)m * p.ldw + p.n_total;
+            if constexpr (STATEFUL) sum = elem_direction(p, boff, sum, peers.W[me][boff]);
             const float b = peers.W[me][boff] - p.lr * sum;
             if (n_pub == 1) peers.W[me][boff] = b;
             else for (int r2 = 0; r2 < p.dp; ++r2) peers.W[r2][boff] = b;
@@ -164,6 +189,7 @@ __device__ __forceinline__ void dp_wait_tile_done(const DpPeers& peers, const Dp
 // =============================================================================================
 // Kernel 1: WGRAD GEMM fused with the DP reduction + SGD + weight broadcast (persistent tiles)
 // =============================================================================================
+template <bool STATEFUL = false>
 __global__ void __launch_bounds__(kThreads, 1)
 fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       const DpLayerParams p, const DpPeers peers) {
@@ -179,7 +205,7 @@ fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         // helper CTA (one-shot layers, one tile per CTA group): no GEMM - just its share of the reduce
         const uint32_t epoch_h = *reinterpret_cast<const volatile uint32_t*>(p.epoch_ptr);
         const TileCoord tc = tile_coord(p, blockIdx.x / p.helpers);
-        dp_owner_reduce_tile(peers, p, tc, epoch_h, threadIdx.x, kThreads, 1, blockIdx.x % p.helpers, p.helpers);
+        dp_owner_reduce_tile<STATEFUL>(peers, p, tc, epoch_h, threadIdx.x, kThreads, 1, blockIdx.x % p.helpers, p.helpers);
         return;
     }
     const int cta = p.helpers > 1 ? blockIdx.x / p.helpers : blockIdx.x;      // tile-group index
@@ -319,7 +345,7 @@ fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         for (int t = cta; t < num_tiles; t += n_cta) {
             const TileCoord tc = tile_coord(p, t);
             if (p.one_shot || tc.owner == p.rank)
-                dp_owner_reduce_tile(peers, p, tc, epoch, etid, 128, 1, 0, p.helpers > 1 ? p.helpers : 1, /*publish=*/!batch_flags);
+                dp_owner_reduce_tile<STATEFUL>(peers, p, tc, epoch, etid, 128, 1, 0, p.helpers > 1 ? p.helpers : 1, /*publish=*/!batch_flags);
         }
         if (batch_flags && !p.one_shot) {
             // all owned tiles of this CTA are reduced and their new weights stored into every replica: one fence, all flags
@@ -347,6 +373,7 @@ fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 // =============================================================================================
 // Kernel 2: the same protocol on an already accumulated gradient block G (no GEMM)
 // =============================================================================================
+template <bool STATEFUL = false>
 __global__ void __launch_bounds__(128, 1) dp_reduce_sgd_kernel(const DpLayerParams p, const DpPeers peers) {
     const uint32_t epoch = *reinterpret_cast<const volatile uint32_t*>(p.epoch_ptr);
     const int num_tiles = p.n_tiles_m * p.n_tiles_n;
@@ -390,7 +417,7 @@ __global__ void __launch_bounds__(128, 1) dp_reduce_sgd_kernel(const DpLayerPara
     }
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         const TileCoord tc = tile_coord(p, t);
-        if (p.one_shot || tc.owner == p.rank) dp_owner_reduce_tile(peers, p, tc, epoch, tid, 128, 1);
+        if (p.one_shot || tc.owner == p.rank) dp_owner_reduce_tile<STATEFUL>(peers, p, tc, epoch, tid, 128, 1);
     }
     if (tid == 0 && !p.one_shot) {
         for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
@@ -448,21 +475,45 @@ const char* fused_dp_plan(FusedDpPlan* plan, const float* dZ, int lddz, const fl
     return nullptr;
 }
 
+static bool stateful(const DpLayerParams& p) { return p.opt.momentum != 0.f || p.opt.weight_decay != 0.f; }
+
+int dp_element_owner(int proto, int in, int out, int ld, int64_t offset, int dp, int m, int n) {
+    if (dp <= 1) return -1;
+    switch (proto) {
+        case DP_PROTO_LL: return (m % (int)kBlockM) / ((int)kBlockM / dp);          // rows per owner = 128 / dp (dp_ll.cu)
+        case DP_PROTO_TWO_SHOT: {
+            int block_n = 0, tm = 0, tn = 0;
+            int64_t slots = 0, slot_floats = 0;
+            dp_layer_geometry(in, out, dp, &block_n, &tm, &tn, &slots, &slot_floats, 0);
+            const int t = (m / (int)kBlockM) * tn + (n >= in ? 0 : n / block_n);      // the bias rides with tile column 0
+            return t % dp;
+        }
+        case DP_PROTO_NVLS: return (int)(((offset + (int64_t)m * ld + n) / 4) % dp);
+        default: return -1;
+    }
+}
+
+cudaError_t fused_dp_configure() {
+    cudaError_t e = cudaFuncSetAttribute(fused_wgrad_dp_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(fused_wgrad_dp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+}
 cudaError_t launch_fused_wgrad_dp(const FusedDpPlan& plan, cudaStream_t stream) {
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(fused_wgrad_dp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+        cudaError_t e = fused_dp_configure();
         if (e != cudaSuccess) return e;
         configured = true;
     }
-    fused_wgrad_dp_kernel<<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.p, plan.peers);
+    if (stateful(plan.p))
+        fused_wgrad_dp_kernel<true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.p, plan.peers);
+    else
+        fused_wgrad_dp_kernel<false><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.p, plan.peers);
     return cudaGetLastError();
 }
-cudaError_t fused_dp_configure() {
-    return cudaFuncSetAttribute(fused_wgrad_dp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-}
 cudaError_t launch_dp_reduce_sgd(const FusedDpPlan& plan, cudaStream_t stream) {
-    dp_reduce_sgd_kernel<<<plan.grid, 128, 0, stream>>>(plan.p, plan.peers);
+    if (stateful(plan.p)) dp_reduce_sgd_kernel<true><<<plan.grid, 128, 0, stream>>>(plan.p, plan.peers);
+    else dp_reduce_sgd_kernel<false><<<plan.grid, 128, 0, stream>>>(plan.p, plan.peers);
     return cudaGetLastError();
 }
 cudaError_t launch_bump_epoch(uint32_t* epoch, cudaStream_t stream) {

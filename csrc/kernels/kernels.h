@@ -10,6 +10,20 @@ namespace ssb {
 
 enum GemmMode : int { GEMM_FWD = 0, GEMM_DGRAD = 1, GEMM_WGRAD = 2 };
 
+// Hyper-parameters of the SGD update beyond lr (torch.optim.SGD, dampening 0).  The default is plain SGD, w -= lr * g,
+// which runs the stateless kernels.  V: momentum buffer laid out like the weights it belongs to (nullptr when
+// momentum == 0: weight decay alone needs no state).
+struct SgdState {
+    float* V = nullptr;
+    float momentum = 0.f;
+    float weight_decay = 0.f;
+    int nesterov = 0;
+    bool plain() const { return momentum == 0.f && weight_decay == 0.f; }
+};
+// nullptr if the combination is valid: 0 <= momentum < 1, weight_decay >= 0, nesterov only with momentum, and a
+// buffer exactly when momentum > 0
+const char* sgd_state_check(const SgdState& s);
+
 // One description for the three Linear GEMMs.  Every GEMM is issued "swapped": the
 // FEATURE dimension sits on the M axis of the 128-row tile and the skinny dimension
 // (micro-batch rows: 4..256) on the N axis, so a 4-row micro-batch costs an N=16 tile
@@ -42,6 +56,11 @@ struct GemmParams {
     int ldw;
     float lr;
     int fuse_sgd;
+    // stateful update rule of the fused SGD (see SgdState): V = momentum buffer with W's layout (pitch ldw, nullable
+    // when momentum == 0), read and written per element; W is read as well when weight_decay != 0
+    float* V;
+    float momentum, weight_decay;
+    int nesterov;
     // fp32-equivalent mode (3xTF32 products, the operands' lo parts x - trunc_tf32(x) derived in the kernel)
     int split;
     // split-K (FWD / DGRAD, see gemm_plan_enable_splitk): blockIdx.z owns a k-range, partial tiles go through
@@ -72,7 +91,7 @@ const char* gemm_plan_dgrad(GemmPlan* plan, const float* W, int ldw, const float
                             int rows, int in, int out, const float* mask, int ldmask, bool split = false);
 const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const float* X, int ldx, float* G, int ldg,
                             int rows, int in, int out, int accumulate, float* db, int db_stride, float* W, int ldw,
-                            float lr, int fuse_sgd, bool split = false);
+                            float lr, int fuse_sgd, bool split = false, const SgdState& opt = SgdState{});
 // Split-K for FWD / DGRAD plans whose output has fewer tiles than the chip has SMs (wide, weight-bound layers):
 // choice() returns the number of k-splits (1 = leave the plan alone); enable() rewires the plan (grid.z, ring
 // depth for two CTAs per SM).  workspace: gemm_splitk_workspace_floats() floats; counters: one zeroed uint per tile.
@@ -89,6 +108,7 @@ struct alignas(128) GemmGroupEntry {
 struct GemmGroupPlan {
     GemmGroupEntry* entries_dev;
     int n, smem_bytes, n_gemms;
+    int stateful;                  // the plans use the stateful SGD rule (all of them or none)
 };
 const char* gemm_group_plan(GemmGroupPlan* out, const GemmPlan* plans, int n_plans);
 cudaError_t gemm_group_launch(const GemmGroupPlan& plan, cudaStream_t stream);
@@ -127,6 +147,8 @@ struct DpLayerParams {
     int helpers;                     // CTAs per tile: CTA 0 computes + pushes, all of them share the reduce rows
     int bulk_push;                   // 1: push tiles with cp.async.bulk (TMA engine), 0: coalesced st.global
     unsigned long long* dbg;         // optional: 8 globaltimer stamps of CTA 0 (phase timeline)
+    SgdState opt;                    // update rule; opt.V = this replica's LOCAL momentum arena (the owner's copy is the
+                                     // canonical one: tile t's momentum lives at rank t % dp, every rank's with one_shot)
 };
 struct FusedDpPlan {
     CUtensorMap tmA, tmB;
@@ -135,6 +157,13 @@ struct FusedDpPlan {
     int grid;
     int smem_bytes;
 };
+// Which replica owns (reduces, updates, keeps the momentum of) each parameter element under the DP protocol a layer
+// runs: DP_PROTO_ALL = every replica (single replica, NCCL all-reduce, one-shot fused layers), LL = tile row r at rank
+// r / (128 / dp), TWO_SHOT = tile t at rank t % dp (bias with tile column 0), NVLS = float4 chunk c of the arena at
+// rank c % dp.  Element (m, n) of the layer's [out, ld] block at arena offset `offset`, n <= in (n == in: bias).
+// Returns the rank, or -1 for every replica.  Host only.
+enum DpProto : int { DP_PROTO_ALL = 0, DP_PROTO_LL = 1, DP_PROTO_TWO_SHOT = 2, DP_PROTO_NVLS = 3 };
+int dp_element_owner(int proto, int in, int out, int ld, int64_t offset, int dp, int m, int n);
 void dp_layer_geometry(int in, int out, int dp, int* block_n, int* n_tiles_m, int* n_tiles_n, int64_t* slots,
                        int64_t* slot_floats, int one_shot);
 // dZ == nullptr: plan for dp_reduce_sgd (no GEMM)
@@ -168,6 +197,7 @@ struct DpLLParams {
     uint4* llA[kMaxDp];          // reduce-scatter landing zones  [parity][src][tile][128 / dp rows][17 lines]
     uint4* llC[kMaxDp];          // all-gather landing zones      [parity][tile][128 rows][17 lines]
     unsigned long long* dbg;     // optional phase timeline: 8 globaltimer stamps per tile (first 28 tiles)
+    SgdState opt;                // update rule; opt.V = LOCAL momentum arena, read / written only for the rows this rank owns
 };
 struct DpLLLayer {
     const float *dZ, *X;
@@ -265,6 +295,8 @@ cudaError_t launch_relu_fwd(const float* x, float* y, long n, cudaStream_t strea
 cudaError_t launch_axpby(const float* x, const float* t, float* y, float a, float b, long n, cudaStream_t stream);
 // w -= lr * g over a flat arena
 cudaError_t launch_sgd(float* w, const float* g, float lr, long n, cudaStream_t stream);
+// the same pass with the stateful rule (momentum buffer opt.V over the same n elements, weight decay, Nesterov)
+cudaError_t launch_sgd_momentum(float* w, const float* g, float lr, const SgdState& opt, long n, cudaStream_t stream);
 // correct[0] += #rows with argmax(pred) == argmax(target)
 cudaError_t launch_argmax_correct(const float* pred, int ldp, const float* target, int ldt, int rows, int cols,
                                   int* correct, cudaStream_t stream);

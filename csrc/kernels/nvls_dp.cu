@@ -35,7 +35,9 @@ __device__ __forceinline__ void multimem_red_release_add(uint32_t* mc_addr, uint
     asm volatile("multimem.red.release.sys.global.add.u32 [%0], %1;" ::"l"(mc_addr), "r"(v) : "memory");
 }
 
-template <bool SGD>
+// STATEFUL (SGD only): momentum / weight decay through sgd_direction; the owner of chunk c reads and writes its unicast
+// momentum V[c] (never multicast: no other replica touches chunk c's state).
+template <bool SGD, bool STATEFUL = false>
 __global__ void __launch_bounds__(256) nvls_reduce_kernel(const NvlsParams p) {
     const uint32_t epoch = *p.epoch + 1u;                     // same value on every replica (one bump per launch)
     const uint32_t target = epoch * (uint32_t)p.dp;
@@ -56,7 +58,19 @@ __global__ void __launch_bounds__(256) nvls_reduce_kernel(const NvlsParams p) {
         const float4 g = multimem_ld_reduce_f4(p.G_mc + 4 * c);
         if (SGD) {
             float4 w = *reinterpret_cast<const float4*>(p.W_uc + 4 * c);
-            w.x -= p.lr * g.x; w.y -= p.lr * g.y; w.z -= p.lr * g.z; w.w -= p.lr * g.w;
+            if constexpr (STATEFUL) {
+                float4* vp = p.opt.V != nullptr ? reinterpret_cast<float4*>(p.opt.V + 4 * c) : nullptr;
+                float4 v = vp != nullptr ? *vp : make_float4(0.f, 0.f, 0.f, 0.f);
+                const float mu = p.opt.momentum, wd = p.opt.weight_decay;
+                const bool nv = p.opt.nesterov != 0;
+                w.x -= p.lr * sgd_direction<false>(g.x, w.x, v.x, mu, wd, nv);
+                w.y -= p.lr * sgd_direction<false>(g.y, w.y, v.y, mu, wd, nv);
+                w.z -= p.lr * sgd_direction<false>(g.z, w.z, v.z, mu, wd, nv);
+                w.w -= p.lr * sgd_direction<false>(g.w, w.w, v.w, mu, wd, nv);
+                if (vp != nullptr) *vp = v;
+            } else {
+                w.x -= p.lr * g.x; w.y -= p.lr * g.y; w.z -= p.lr * g.z; w.w -= p.lr * g.w;
+            }
             multimem_st_f4(p.W_mc + 4 * c, w);
         } else {
             multimem_st_f4(p.G_mc + 4 * c, g);
@@ -89,7 +103,10 @@ static int nvls_grid(const NvlsParams& p, int max_ctas) {
 }
 
 cudaError_t launch_nvls_reduce_sgd(const NvlsParams& p, int max_ctas, cudaStream_t stream) {
-    nvls_reduce_kernel<true><<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
+    if (p.opt.momentum != 0.f || p.opt.weight_decay != 0.f)
+        nvls_reduce_kernel<true, true><<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
+    else
+        nvls_reduce_kernel<true><<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
     return cudaGetLastError();
 }
 

@@ -288,4 +288,22 @@ __device__ __forceinline__ float4 ld_nc_f4(const float* p) {
     return v;
 }
 
+// ------------------------------------------------------------------ optimizer update rule
+// torch.optim.SGD with dampening 0, for one element: returns the step direction d (the caller applies w -= lr * d) and
+// updates the momentum buffer v in place.  Every fused update site calls this, so all of them round alike:
+//     g' = g + wd * w ;  v = mu * v + g' ;  d = nesterov ? g' + mu * v : v
+// With mu == 0 the result is d = g' whatever v holds, so a site without a momentum buffer passes v = 0 and skips the
+// store.  The explicitly rounded operations keep the compiler from contracting differently at different sites.
+// PLAIN (no momentum, no weight decay) is today's d = g and compiles to exactly the stateless code.
+template <bool PLAIN>
+__device__ __forceinline__ float sgd_direction(float g, float w, float& v, float mu, float wd, bool nesterov) {
+    if constexpr (PLAIN) {
+        return g;
+    } else {
+        const float gp = __fadd_rn(g, __fmul_rn(wd, w));
+        v = __fadd_rn(__fmul_rn(mu, v), gp);
+        return nesterov ? __fadd_rn(gp, __fmul_rn(mu, v)) : v;
+    }
+}
+
 }  // namespace ssb

@@ -37,7 +37,9 @@ static constexpr uint32_t kPanelBytes = 32 * 128;       // MN-major panel: 32 k-
 // waits for anybody, so the CTAs of a tile need not be co-resident.
 // The body is shared by the one-GEMM-per-launch kernels below and by the grouped weight-gradient kernel (several
 // layers' tiles in ONE launch, tensor maps and parameters read from a device table).
-template <int MODE, bool SPLITK>
+// STATEFUL (WGRAD with fuse_sgd only): the SGD update uses momentum / weight decay (GemmParams::V, ...); the false
+// instantiations are the plain w -= lr * dW code.
+template <int MODE, bool SPLITK, bool STATEFUL = false>
 __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
                                              const GemmParams& p, const int bx, const int by, const int bz) {
     constexpr bool A_MN = (MODE != GEMM_FWD);
@@ -242,12 +244,70 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             // performed in L2) per 32-column panel.  With fuse_sgd the tile is scaled by -lr and reduce-added straight into
             // W: dW never touches memory, zero_grad and the optimizer pass disappear.  OOB rows/columns are clipped by the
             // tensor map, so the bias column (index n_total of the same [out, ld] block) is never touched here.
+            // STATEFUL (fuse_sgd with momentum / weight decay): the tile holds the final dW, so each lane turns its row's
+            // 16 values into the step direction d (sgd_direction) - reading and writing its V entries, and reading W
+            // only with weight decay - before the same -lr scaling and reduce-add.  Columns >= n_total get d = 0 and
+            // are never stored: column n_total is the bias slot, which the bias path below updates.
             const float scale = p.fuse_sgd ? -p.lr : 1.f;
 #pragma unroll
             for (int ch = 0; ch < kChunks; ++ch) {
                 if (16 * ch >= p.block_n) break;
                 float v[16];
                 warp_acc_row16(acc, ch, v, lane);
+                if constexpr (STATEFUL) {
+                    const int nc = n0 + 16 * ch;
+                    const bool has_v = p.V != nullptr, has_wd = p.weight_decay != 0.f;
+                    float vm[16], wv[16];
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) { vm[j] = 0.f; wv[j] = 0.f; }
+                    // all loads in flight before any use; 16-byte accesses where all 4 columns are real (V and W rows
+                    // are 16-byte aligned: TMA-legal pitch, nc a multiple of 16)
+                    if (m_ok) {
+                        const size_t row = (size_t)m * p.ldw + nc;
+#pragma unroll
+                        for (int q4 = 0; q4 < 4; ++q4) {
+                            if (nc + 4 * q4 + 3 < p.n_total) {
+                                if (has_v) {
+                                    const float4 t = *reinterpret_cast<const float4*>(p.V + row + 4 * q4);
+                                    vm[4 * q4] = t.x; vm[4 * q4 + 1] = t.y; vm[4 * q4 + 2] = t.z; vm[4 * q4 + 3] = t.w;
+                                }
+                                if (has_wd) {
+                                    const float4 t = *reinterpret_cast<const float4*>(p.W + row + 4 * q4);
+                                    wv[4 * q4] = t.x; wv[4 * q4 + 1] = t.y; wv[4 * q4 + 2] = t.z; wv[4 * q4 + 3] = t.w;
+                                }
+                            } else {
+#pragma unroll
+                                for (int e = 0; e < 4; ++e) {
+                                    const int j = 4 * q4 + e;
+                                    if (nc + j < p.n_total) {
+                                        if (has_v) vm[j] = p.V[row + j];
+                                        if (has_wd) wv[j] = p.W[row + j];
+                                    }
+                                }
+                            }
+                        }
+                    }
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const bool ok = m_ok && nc + j < p.n_total;
+                        const float d = sgd_direction<false>(v[j], wv[j], vm[j], p.momentum, p.weight_decay, p.nesterov != 0);
+                        v[j] = ok ? d : 0.f;
+                    }
+                    if (m_ok && has_v) {
+                        const size_t row = (size_t)m * p.ldw + nc;
+#pragma unroll
+                        for (int q4 = 0; q4 < 4; ++q4) {
+                            if (nc + 4 * q4 + 3 < p.n_total) {
+                                *reinterpret_cast<float4*>(p.V + row + 4 * q4) =
+                                    make_float4(vm[4 * q4], vm[4 * q4 + 1], vm[4 * q4 + 2], vm[4 * q4 + 3]);
+                            } else {
+#pragma unroll
+                                for (int e = 0; e < 4; ++e)
+                                    if (nc + 4 * q4 + e < p.n_total) p.V[row + 4 * q4 + e] = vm[4 * q4 + e];
+                            }
+                        }
+                    }
+                }
                 const uint32_t prow = epi_base + (ch >> 1) * (kBlockM * 128u) + (uint32_t)m_local * 128u;
 #pragma unroll
                 for (int q4 = 0; q4 < 4; ++q4) {
@@ -278,8 +338,16 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             asm volatile("bar.sync 1, 128;" ::: "memory");
             if (db_active && m_ok) {
                 if (p.fuse_sgd) {
-                    float* bp = p.W + (size_t)m * p.ldw + (p.db - p.G);   // bias lives at the same offset in W
-                    *bp -= p.lr * dbsum;
+                    const size_t boff = (size_t)m * p.ldw + (p.db - p.G);  // bias lives at the same offset in W (and V)
+                    float* bp = p.W + boff;
+                    if constexpr (STATEFUL) {
+                        float vb = p.V != nullptr ? p.V[boff] : 0.f;
+                        const float d = sgd_direction<false>(dbsum, *bp, vb, p.momentum, p.weight_decay, p.nesterov != 0);
+                        if (p.V != nullptr) p.V[boff] = vb;
+                        *bp -= p.lr * d;
+                    } else {
+                        *bp -= p.lr * dbsum;
+                    }
                 } else {
                     float* dbp = p.db + (size_t)m * p.db_stride;
                     *dbp = p.accumulate ? (*dbp + dbsum) : dbsum;
@@ -289,20 +357,21 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
     }
 }
 
-template <int MODE, bool SPLITK = false>
+template <int MODE, bool SPLITK = false, bool STATEFUL = false>
 __global__ void __launch_bounds__(kThreads, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
-    tc_gemm_body<MODE, SPLITK>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z);
+    tc_gemm_body<MODE, SPLITK, STATEFUL>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z);
 }
 
 // ---- grouped weight-gradient launch: the tiles of SEVERAL layers' WGRAD GEMMs in one grid (one table entry per CTA).
 // Removes the fork / join of one graph node per layer from the end of a step: with the zero-copy loss the fp32 training
 // step of a narrow stage is chain kernel -> grouped wgrad (+SGD) (or chain || LL kernel under DP).
+template <bool STATEFUL = false>
 __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const GemmGroupEntry* __restrict__ entries) {
     const GemmGroupEntry& e = entries[blockIdx.x];
     const GemmParams p = e.p;                      // private copy: the body reads these fields in every loop
-    tc_gemm_body<GEMM_WGRAD, false>(e.tmA, e.tmB, e.tmC, p, e.bx, e.by, 0);
+    tc_gemm_body<GEMM_WGRAD, false, STATEFUL>(e.tmA, e.tmB, e.tmC, p, e.bx, e.by, 0);
 }
 
 // =========================================================================== host side
@@ -353,6 +422,16 @@ const char* make_tmap_k(CUtensorMap* map, const float* base, int inner, int oute
 
 static int round_up_i(int x, int m) { return (x + m - 1) / m * m; }
 
+static bool is_stateful(const GemmParams& p) { return p.fuse_sgd && (p.momentum != 0.f || p.weight_decay != 0.f); }
+
+const char* sgd_state_check(const SgdState& s) {
+    if (!(s.momentum >= 0.f && s.momentum < 1.f)) return "momentum must be in [0, 1)";
+    if (!(s.weight_decay >= 0.f)) return "weight_decay must be >= 0";
+    if (s.nesterov && s.momentum == 0.f) return "nesterov needs momentum > 0";
+    if ((s.momentum > 0.f) != (s.V != nullptr)) return "a momentum buffer is needed exactly when momentum > 0";
+    return nullptr;
+}
+
 static void finish_plan(GemmPlan* plan) {
     GemmParams& p = plan->p;
     const int num_kb = (p.k_total + (int)kBlockK - 1) / (int)kBlockK;
@@ -401,7 +480,7 @@ const char* gemm_plan_dgrad(GemmPlan* plan, const float* W, int ldw, const float
 
 const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const float* X, int ldx, float* G, int ldg,
                             int rows, int in, int out, int accumulate, float* db, int db_stride, float* W, int ldw,
-                            float lr, int fuse_sgd, bool split) {
+                            float lr, int fuse_sgd, bool split, const SgdState& opt) {
     *plan = GemmPlan{};
     plan->mode = GEMM_WGRAD;
     GemmParams& p = plan->p;
@@ -411,6 +490,11 @@ const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const flo
     p.W = W; p.ldw = ldw; p.lr = lr; p.fuse_sgd = fuse_sgd;
     if (fuse_sgd && W == nullptr) return "fuse_sgd needs W";
     if (fuse_sgd && accumulate) return "fuse_sgd cannot be combined with accumulate (reduce into G, then run the SGD pass)";
+    if (!opt.plain()) {
+        if (!fuse_sgd) return "momentum / weight decay need fuse_sgd (the update rule runs in the epilogue)";
+        if (const char* e = sgd_state_check(opt)) return e;
+        p.V = opt.V; p.momentum = opt.momentum; p.weight_decay = opt.weight_decay; p.nesterov = opt.nesterov;
+    }
     // output tile map: [out, in] with the block's row pitch; fused SGD targets W itself
     if (const char* e = make_tmap(&plan->tmC, fuse_sgd ? W : G, in, out, fuse_sgd ? ldw : ldg, kBlockM)) return e;
     if (const char* e = make_tmap(&plan->tmA, dZ, out, rows, lddz, 32)) return e;
@@ -465,10 +549,12 @@ const char* gemm_group_plan(GemmGroupPlan* out, const GemmPlan* plans, int n_pla
     if (n_plans < 1) return "gemm_group_plan: no plans";
     std::vector<GemmGroupEntry> host;
     int smem = 0;
+    const bool stateful = is_stateful(plans[0].p);
     for (int i = 0; i < n_plans; ++i) {
         const GemmPlan& g = plans[i];
         if (g.mode != GEMM_WGRAD) return "gemm_group_plan: only weight-gradient GEMMs can be grouped";
         if (g.p.k_splits > 1) return "gemm_group_plan: split-K plans cannot be grouped";
+        if (is_stateful(g.p) != stateful) return "gemm_group_plan: plans mix the plain and the stateful SGD rule";
         if (g.smem_bytes > smem) smem = g.smem_bytes;
         for (unsigned by = 0; by < g.grid.y; ++by)
             for (unsigned bx = 0; bx < g.grid.x; ++bx) {
@@ -486,6 +572,7 @@ const char* gemm_group_plan(GemmGroupPlan* out, const GemmPlan* plans, int n_pla
         return "gemm_group_plan: table upload failed";
     }
     out->entries_dev = dev; out->n = (int)host.size(); out->smem_bytes = smem; out->n_gemms = n_plans;
+    out->stateful = stateful ? 1 : 0;
     return nullptr;
 }
 
@@ -506,7 +593,9 @@ cudaError_t gemm_configure() {
     if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_FWD>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_DGRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_WGRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_WGRAD, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_FWD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_DGRAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     g_configured = true;
@@ -518,7 +607,10 @@ cudaError_t gemm_group_launch(const GemmGroupPlan& plan, cudaStream_t stream) {
         cudaError_t e = gemm_configure();
         if (e != cudaSuccess) return e;
     }
-    tc_wgrad_group_kernel<<<plan.n, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev);
+    if (plan.stateful)
+        tc_wgrad_group_kernel<true><<<plan.n, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev);
+    else
+        tc_wgrad_group_kernel<false><<<plan.n, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev);
     g_launches.fetch_add(plan.n_gemms, std::memory_order_relaxed);
     return cudaGetLastError();
 }
@@ -532,6 +624,12 @@ static cudaError_t launch_mode(const GemmPlan& plan, cudaStream_t stream) {
     if constexpr (MODE != GEMM_WGRAD) {
         if (plan.p.k_splits > 1) {
             tc_gemm_kernel<MODE, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
+            g_launches.fetch_add(1, std::memory_order_relaxed);
+            return cudaGetLastError();
+        }
+    } else {
+        if (is_stateful(plan.p)) {
+            tc_gemm_kernel<MODE, false, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
             g_launches.fetch_add(1, std::memory_order_relaxed);
             return cudaGetLastError();
         }

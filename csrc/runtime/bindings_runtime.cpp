@@ -151,10 +151,14 @@ private:
 class PyEngine {
 public:
     PyEngine(const std::vector<std::tuple<int, int, int, int64_t, int>>& layers, py::dict cfg, torch::Tensor weights,
-             torch::Tensor grads)
-        : weights_(weights), grads_(grads) {
+             torch::Tensor grads, c10::optional<torch::Tensor> momentum)
+        : weights_(weights), grads_(grads), momentum_(momentum) {
         TORCH_CHECK(weights.is_cuda() && grads.is_cuda() && weights.is_contiguous() && grads.is_contiguous());
         TORCH_CHECK(weights.scalar_type() == torch::kFloat32 && grads.scalar_type() == torch::kFloat32);
+        if (momentum.has_value())
+            TORCH_CHECK(momentum->is_cuda() && momentum->is_contiguous() && momentum->scalar_type() == torch::kFloat32 &&
+                            momentum->numel() >= weights.numel() && momentum->device() == weights.device(),
+                        "PipeEngine: the momentum arena must be a contiguous fp32 CUDA buffer covering the weight arena");
         EngineConfig c;
         for (auto& t : layers) c.layers.push_back({std::get<0>(t), std::get<1>(t), std::get<2>(t), std::get<3>(t), std::get<4>(t)});
         auto geti = [&](const char* k, int dflt) { return cfg.contains(k) ? cfg[k].cast<int>() : dflt; };
@@ -166,8 +170,12 @@ public:
         c.dp_size = geti("dp_size", 1); c.dp_rank = geti("dp_rank", 0); c.dp_mode = geti("dp_mode", 0);
         c.in_dim = geti("in_dim", 784); c.out_dim = geti("out_dim", 10);
         c.split = geti("split", 0);
+        c.momentum = cfg.contains("momentum") ? cfg["momentum"].cast<float>() : 0.f;
+        c.weight_decay = cfg.contains("weight_decay") ? cfg["weight_decay"].cast<float>() : 0.f;
+        c.nesterov = geti("nesterov", 0);
         c10::cuda::CUDAGuard guard(weights.device());
-        engine_ = std::make_unique<PipeEngine>(c, weights.data_ptr<float>(), grads.data_ptr<float>(), weights.numel());
+        engine_ = std::make_unique<PipeEngine>(c, weights.data_ptr<float>(), grads.data_ptr<float>(), weights.numel(),
+                                               momentum.has_value() ? momentum->data_ptr<float>() : nullptr);
     }
     void set_pp_comm(std::shared_ptr<NcclComm> c) { pp_ = c; engine_->set_pp_comm(c->get()); }
     void set_dp_comm(std::shared_ptr<NcclComm> c) { dp_ = c; engine_->set_dp_comm(c->get()); }
@@ -231,11 +239,13 @@ public:
     bool coalesced() { return engine_->coalesced(); }
     int64_t main_stream() { return reinterpret_cast<int64_t>(engine_->main_stream()); }
     std::string describe() { return engine_->describe(); }
+    std::vector<int> layer_protocols() { return engine_->layer_protocols(); }
     std::string plan_text(int set) { return engine_->plan_text(set); }
     std::vector<unsigned long long> chain_timeline() { return engine_->chain_timeline(); }
 
 private:
     torch::Tensor weights_, grads_;
+    c10::optional<torch::Tensor> momentum_;   // kept alive: the plan holds raw pointers into it
     std::pair<c10::optional<torch::Tensor>, c10::optional<torch::Tensor>> held_[2];
     unsigned hold_i_ = 0;
     std::shared_ptr<NcclComm> pp_, dp_;
@@ -278,7 +288,9 @@ void bind_runtime(py::module_& m) {
         .def("open_prev", &PyPpContext::open_prev)
         .def("open_next", &PyPpContext::open_next);
     py::class_<PyEngine>(m, "PipeEngine")
-        .def(py::init<const std::vector<std::tuple<int, int, int, int64_t, int>>&, py::dict, torch::Tensor, torch::Tensor>())
+        .def(py::init<const std::vector<std::tuple<int, int, int, int64_t, int>>&, py::dict, torch::Tensor, torch::Tensor,
+                      c10::optional<torch::Tensor>>(),
+             py::arg("layers"), py::arg("cfg"), py::arg("weights"), py::arg("grads"), py::arg("momentum") = py::none())
         .def("set_pp_comm", &PyEngine::set_pp_comm)
         .def("set_dp_comm", &PyEngine::set_dp_comm)
         .def("set_dp_context", &PyEngine::set_dp_context)
@@ -307,6 +319,7 @@ void bind_runtime(py::module_& m) {
         .def("coalesced", &PyEngine::coalesced)
         .def("main_stream", &PyEngine::main_stream)
         .def("describe", &PyEngine::describe)
+        .def("layer_protocols", &PyEngine::layer_protocols)
         .def("plan_text", &PyEngine::plan_text, py::arg("set") = 0)
         .def("chain_timeline", &PyEngine::chain_timeline);
 }

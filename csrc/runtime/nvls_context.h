@@ -21,6 +21,8 @@
 #include <cstdint>
 #include <string>
 
+#include "kernels/kernels.h"
+
 namespace ssb {
 
 struct NvlsParams {
@@ -37,6 +39,7 @@ struct NvlsParams {
     int64_t numel;          // floats to reduce / update (multiple of 4)
     int dp, rank;
     float lr;
+    SgdState opt;           // update rule; opt.V = LOCAL momentum arena (unicast), chunk c's entries live at rank c % dp
 };
 
 class NvlsContext {

@@ -35,8 +35,12 @@ static int round_up(int x, int m) { return (x + m - 1) / m * m; }
 // leave some SMs to the concurrently running dgrad chain; also bounds co-residency needs
 static constexpr int kFusedDpMaxCtas = 120;
 
-PipeEngine::PipeEngine(const EngineConfig& cfg, float* weights, float* grads, int64_t arena_numel)
-    : cfg_(cfg), W_(weights), G_(grads), arena_numel_(arena_numel), L_((int)cfg.layers.size()) {
+PipeEngine::PipeEngine(const EngineConfig& cfg, float* weights, float* grads, int64_t arena_numel, float* momentum)
+    : cfg_(cfg), W_(weights), G_(grads), V_(momentum), arena_numel_(arena_numel), L_((int)cfg.layers.size()) {
+    const SgdState opt = opt_for(0);
+    if (const char* e = sgd_state_check(opt)) throw std::runtime_error(std::string("PipeEngine: ") + e);
+    // who owns which momentum entries: every replica unless a layer's update runs in an owner-based DP reduction
+    layer_proto_.assign(L_, (cfg_.training && cfg_.dp_mode == 3 && cfg_.dp_size > 1) ? DP_PROTO_NVLS : DP_PROTO_ALL);
     n_mu_streams_ = std::max(1, std::min(cfg_.n_mu, 8));   // one stream per micro-batch in flight (GPipe with 8 micro-batches: all 8)
     n_w_streams_ = std::max(1, std::min(L_, 8));        // one stream per layer's wgrad when possible
     if (const char* e = getenv("SSB_MU_STREAMS")) n_mu_streams_ = std::max(1, std::min(atoi(e), std::max(1, cfg_.n_mu)));
@@ -52,6 +56,13 @@ PipeEngine::PipeEngine(const EngineConfig& cfg, float* weights, float* grads, in
         CUDA_CHECK(cudaEventCreateWithFlags(&ev_done_[i], cudaEventDisableTiming));
     }
     alloc_buffers();
+}
+
+SgdState PipeEngine::opt_for(int layer) const {
+    SgdState s;
+    s.momentum = cfg_.momentum; s.weight_decay = cfg_.weight_decay; s.nesterov = cfg_.nesterov;
+    if (V_ != nullptr) s.V = V_ + (layer >= 1 ? cfg_.layers[layer - 1].offset : 0);
+    return s;
 }
 
 PipeEngine::~PipeEngine() {
@@ -615,6 +626,8 @@ void PipeEngine::plan_per_mubatch() {
                     for (auto& pd : pending_dp) {
                         emit_wait(s_dp_, pd.second);
                         DpLayerParams lp = dp_ctx_->layer_params(pd.first - 1);
+                        lp.opt = opt_for(0);
+                        layer_proto_[pd.first - 1] = lp.one_shot ? DP_PROTO_ALL : DP_PROTO_TWO_SHOT;
                         lp.G = Gl(pd.first);
                         FusedDpPlan fp;
                         check(fused_dp_plan(&fp, nullptr, 0, nullptr, 0, mb, lp, dp_ctx_->peers(), kFusedDpMaxCtas));
@@ -640,7 +653,8 @@ void PipeEngine::plan_per_mubatch() {
                             const LayerSpec& ls = cfg_.layers[l - 1];
                             GemmPlan g;
                             check(gemm_plan_wgrad(&g, dz_all_[l], act_ld_[l], act_all_[l - 1], act_ld_[l - 1], Gl(l), ls.ld, rows_all, ls.in,
-                                                  ls.out, 0, Gl(l) + ls.in, ls.ld, Wl(l), ls.ld, cfg_.lr, 1, cfg_.split != 0));
+                                                  ls.out, 0, Gl(l) + ls.in, ls.ld, Wl(l), ls.ld, cfg_.lr, 1, cfg_.split != 0,
+                                                  opt_for(l)));
                             grouped.push_back(g);
                         }
                         GemmGroupPlan gp;
@@ -660,6 +674,8 @@ void PipeEngine::plan_per_mubatch() {
                         }
                         DpLLPlan lp;
                         DpLLParams base = dp_ctx_->ll_params();
+                        base.opt = opt_for(0);
+                        for (int l = 0; l < L_; ++l) layer_proto_[l] = DP_PROTO_LL;
                         check(dp_ll_plan(&lp, lls.data(), (int)lls.size(), rows_all, base));
                         ll_plans_.push_back(lp);
                         Op lo;
@@ -846,6 +862,8 @@ void PipeEngine::build_coalesced() {
             if (ev_dg >= 0) emit_wait(sdp, ev_dg);
             FusedDpPlan fp;
             DpLayerParams lp = dp_ctx_->layer_params(l - 1);
+            lp.opt = opt_for(0);
+            layer_proto_[l - 1] = lp.one_shot ? DP_PROTO_ALL : DP_PROTO_TWO_SHOT;
             if (getenv("SSB_CHAIN_TIMELINE")) {
                 if (!chain_dbg_) {
                     CUDA_CHECK(cudaMalloc(&chain_dbg_, 4 * 256 * sizeof(unsigned long long)));
@@ -870,7 +888,8 @@ void PipeEngine::build_coalesced() {
         }
         GemmPlan g;
         check(gemm_plan_wgrad(&g, dz_all_[l], act_ld_[l], act_all_[l - 1], act_ld_[l - 1], Gl(l), ls.ld, rows, ls.in, ls.out, 0,
-                              Gl(l) + ls.in, ls.ld, fuse ? Wl(l) : nullptr, ls.ld, cfg_.lr, fuse ? 1 : 0, cfg_.split != 0));
+                              Gl(l) + ls.in, ls.ld, fuse ? Wl(l) : nullptr, ls.ld, cfg_.lr, fuse ? 1 : 0, cfg_.split != 0,
+                              fuse ? opt_for(l) : SgdState{}));
         if (group_wgrad) {                                  // launched together after the loop
             grouped.push_back(g);
             continue;
@@ -888,6 +907,8 @@ void PipeEngine::build_coalesced() {
     if (!ll_layers.empty()) {
         // deepest layer first: its tiles get the lowest block indices, i.e. they are resident first and their gate opens first
         DpLLParams base = dp_ctx_->ll_params();
+        base.opt = opt_for(0);
+        for (int l = 0; l < L_; ++l) layer_proto_[l] = DP_PROTO_LL;
         base.gate_step = gate_on_ ? gate_step_ : nullptr;
         if (getenv("SSB_CHAIN_TIMELINE")) {
             if (!chain_dbg_) {
@@ -997,7 +1018,12 @@ void PipeEngine::exec(const Op& op) {
             CUDA_CHECK(launch_argmax_correct(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, correct_dev_, st));
             break;
         case OP_RELU_MASK: CUDA_CHECK(launch_relu_mask(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, st)); break;
-        case OP_SGD: CUDA_CHECK(launch_sgd(op.a, op.b, op.scalar, op.n, st)); break;
+        case OP_SGD: {
+            const SgdState opt = opt_for(0);
+            if (opt.plain()) CUDA_CHECK(launch_sgd(op.a, op.b, op.scalar, op.n, st));
+            else CUDA_CHECK(launch_sgd_momentum(op.a, op.b, op.scalar, opt, op.n, st));
+            break;
+        }
         case OP_NVLS_SGD: {
             if (!nvls_ctx_) throw std::runtime_error("PipeEngine: dp_mode nvls needs an NvlsContext");
             if (nvls_ctx_->weights() != W_ || nvls_ctx_->grads() != G_)
@@ -1005,7 +1031,9 @@ void PipeEngine::exec(const Op& op) {
             int dev = 0, sms = 132;
             CUDA_CHECK(cudaGetDevice(&dev));
             CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-            CUDA_CHECK(launch_nvls_reduce_sgd(nvls_ctx_->params(), sms, st));
+            NvlsParams np = nvls_ctx_->params();
+            np.opt = opt_for(0);
+            CUDA_CHECK(launch_nvls_reduce_sgd(np, sms, st));
             break;
         }
         case OP_ALLREDUCE:
@@ -1260,7 +1288,14 @@ std::string PipeEngine::describe() const {
     std::ostringstream os;
     os << "PipeEngine(stage " << cfg_.stage << "/" << cfg_.n_stages << ", layers=" << L_ << ", mb_rows=" << cfg_.mb_rows
        << ", n_mu=" << cfg_.n_mu << ", ops=" << ops_sets_[0].size() << ", kernels/step=" << kernels_per_step_
-       << ", graph_nodes=" << graph_nodes_ << ", splitk_gemms=" << splitk_gemms_ << ", streams=" << streams_.size() << ", events=" << events_.size() << ")";
+       << ", graph_nodes=" << graph_nodes_ << ", splitk_gemms=" << splitk_gemms_ << ", streams=" << streams_.size() << ", events=" << events_.size();
+    if (cfg_.training) {
+        os << ", update=sgd(lr=" << cfg_.lr;
+        if (cfg_.momentum != 0.f) os << ", momentum=" << cfg_.momentum << (cfg_.nesterov ? ", nesterov" : "");
+        if (cfg_.weight_decay != 0.f) os << ", weight_decay=" << cfg_.weight_decay;
+        os << ")";
+    }
+    os << ")";
     return os.str();
 }
 

@@ -84,11 +84,17 @@ struct EngineConfig {
                             // 3 = NVLS: one kernel reduces the gradient arena in the switch, applies SGD, multicasts W
     int in_dim = 784, out_dim = 10;
     int split = 0;          // 1 = fp32-equivalent tensor-core products (3xTF32), 0 = single-pass TF32
+    // SGD beyond lr (torch.optim.SGD, dampening 0).  All zero = plain SGD and the stateless kernels.  Momentum needs
+    // the engine's momentum arena (same layout as the weights); under the in-kernel DP reductions (dp_mode 2, 3) each
+    // replica updates only the entries it owns (layer_protocols()).
+    float momentum = 0.f, weight_decay = 0.f;
+    int nesterov = 0;
 };
 
 class PipeEngine {
 public:
-    explicit PipeEngine(const EngineConfig& cfg, float* weights, float* grads, int64_t arena_numel);
+    // momentum: flat momentum arena (arena_numel floats, the weights' offsets), nullptr unless cfg.momentum > 0
+    explicit PipeEngine(const EngineConfig& cfg, float* weights, float* grads, int64_t arena_numel, float* momentum = nullptr);
     ~PipeEngine();
 
     // communicators (optional): created by the caller from ncclUniqueIds exchanged over torch.distributed
@@ -130,6 +136,8 @@ public:
     bool uses_chain() const { return chain_ok_; }
     cudaStream_t main_stream() { return streams_[0]; }
     const EngineConfig& config() const { return cfg_; }
+    // per layer: the DpProto under which its update runs (which replica owns which momentum entries)
+    const std::vector<int>& layer_protocols() const { return layer_proto_; }
     std::string describe() const;
     std::string plan_text(int set = 0) const;
     std::vector<unsigned long long> chain_timeline();   // SSB_CHAIN_TIMELINE=1: globaltimer stamps of the chain kernel
@@ -149,8 +157,10 @@ private:
     void exec(const Op& op);
     cudaStream_t stream_of(const Op& op) const;
 
+    SgdState opt_for(int layer) const;   // the update rule for layer l's block (l = 0: the whole arena)
     EngineConfig cfg_;
-    float *W_, *G_;
+    float *W_, *G_, *V_;
+    std::vector<int> layer_proto_;
     int64_t arena_numel_;
     int L_;
     std::vector<int> act_ld_;                    // per layer boundary 0..L

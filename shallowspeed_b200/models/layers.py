@@ -66,6 +66,10 @@ class ParamArena:
         self.numel = max(off, self.BLOCK_ALIGN)
         self.weights = torch.zeros(self.numel, dtype=torch.float32, device=device)
         self.grads = torch.zeros(self.numel, dtype=torch.float32, device=device)
+        # SGD momentum buffer, same offsets and row pitches as ``weights``; allocated by ``enable_momentum`` only, so
+        # plain SGD costs no memory.  Ordinary device memory even when the weights live in memory shared with peers:
+        # only this replica ever reads or writes it.
+        self.momentum: Optional[torch.Tensor] = None
         self._listeners: list[Callable[[], None]] = []
 
     # -- views ---------------------------------------------------------------
@@ -83,7 +87,18 @@ class ParamArena:
         in_dims = self.blocks[i][1]
         return self.block(i, grads)[:, in_dims : in_dims + 1].t()  # [1, out], strides (1, ld)
 
+    def momentum_block(self, i: int) -> torch.Tensor:
+        """The ``[out, ld]`` block *i* of the momentum buffer (bias momentum in column ``in``)."""
+        o, _ = self.blocks[i]
+        return self.momentum[self.offsets[i] : self.offsets[i] + o * self.lds[i]].view(o, self.lds[i])
+
     # -- storage management ----------------------------------------------------
+    def enable_momentum(self):
+        """Allocate the (zeroed) momentum buffer on the weights' device; a no-op when it exists."""
+        if self.momentum is None:
+            self.momentum = torch.zeros(self.numel, dtype=torch.float32, device=self.weights.device)
+        return self.momentum
+
     def on_rebind(self, fn: Callable[[], None]):
         self._listeners.append(fn)
 
@@ -96,6 +111,8 @@ class ParamArena:
             weights[: self.numel].copy_(self.weights)
             grads[: self.numel].copy_(self.grads)
         self.weights, self.grads = weights, grads
+        if self.momentum is not None and self.momentum.device != weights.device:
+            self.momentum = self.momentum.to(weights.device)
         for fn in self._listeners:
             fn()
 

@@ -233,6 +233,13 @@ class NativeWorker:
             self.dp_mode = comm_mode
         # native communicators are shared between the train and the validation worker
         self.lr = optimizer.lr if optimizer is not None else 0.0
+        # the update rule beyond lr (optimizer.SGD); the engine keeps the momentum in the model arena's buffer
+        self.momentum = float(getattr(optimizer, "momentum", 0.0) or 0.0)
+        self.weight_decay = float(getattr(optimizer, "weight_decay", 0.0) or 0.0)
+        self.nesterov = bool(getattr(optimizer, "nesterov", False))
+        if self.momentum > 0.0 and getattr(optimizer, "arena", None) is not model.arena:
+            raise ValueError("NativeWorker: SGD with momentum must be built with arena=model.arena (the engine keeps the "
+                             "momentum in the arena's buffer)")
         self._dp_ctx = None
         self._nvls_ctx = None
         # Engines that share a communicator (train + validation worker on one pipeline group) run on their own
@@ -254,6 +261,7 @@ class NativeWorker:
                     self._dp_nccl = make_nccl_comm(self.dp_comm)
         self._engines = {}
         self._last_engine = None
+        self._train_engine = None      # the training plan whose DP protocols decide who owns which momentum entries
 
     # ------------------------------------------------------------------ plan cache
     def _key(self, sched: Schedule):
@@ -275,7 +283,11 @@ class NativeWorker:
                    dp_size=self.dp_comm.Get_size(), dp_rank=self.dp_comm.Get_rank(),
                    dp_mode=DP_MODE[self.dp_mode] if training else 0, in_dim=m.in_dim, out_dim=m.out_dim,
                    split=1 if self.precision in ("fp32", "fp32x3", "3xtf32") else 0)
-        eng = _C().PipeEngine(specs, cfg, m.arena.weights, m.arena.grads)
+        momentum = None
+        if training and (self.momentum != 0.0 or self.weight_decay != 0.0):
+            cfg.update(momentum=self.momentum, weight_decay=self.weight_decay, nesterov=int(self.nesterov))
+            momentum = m.arena.momentum if self.momentum > 0.0 else None
+        eng = _C().PipeEngine(specs, cfg, m.arena.weights, m.arena.grads, momentum)
         if self._pp_nccl is not None:
             eng.set_pp_comm(self._pp_nccl)
         if self._dp_nccl is not None and training:
@@ -289,6 +301,8 @@ class NativeWorker:
                                                sched.is_first_stage, sched.is_last_stage))
         torch.cuda.synchronize(self.device)
         eng.build([encode(i) for i in flatten(list(sched.steps()))])
+        if training:
+            self._train_engine = eng
         return eng
 
     def engine_for(self, sched: Schedule):
@@ -370,8 +384,62 @@ class NativeWorker:
     def kernels_per_step(self, sched):
         return int(self.engine_for(sched).kernels_per_step())
 
+    # ------------------------------------------------------------------ optimizer state (checkpoints)
+    def optimizer_state(self):
+        """Collective over the DP group: the canonical full momentum arena of this stage (CPU, None without momentum),
+        each entry taken from the replica that owns it, so the result does not depend on the DP transport.  Entries
+        every replica owns come from DP rank 0; the rest of the arena (padding) is zero everywhere."""
+        buf = self.model.arena.momentum
+        if self.momentum == 0.0 or buf is None:
+            return None
+        self.sync_to_model()
+        n = self.model.arena.numel
+        dp, rank = self.dp_comm.Get_size(), self.dp_comm.Get_rank()
+        if dp == 1:
+            return buf[:n].detach().cpu().clone()
+        eng = self._train_engine
+        protos = list(eng.layer_protocols()) if eng is not None else [0] * len(self.model.linears)
+        mine = owned_elements(self.model.arena, self.model.linears, protos, dp, rank, shared_to_rank0=True).to(buf.device)
+        part = torch.where(mine, buf[:n], torch.zeros_like(buf[:n]))
+        import torch.distributed as dist
+
+        dist.all_reduce(part, op=dist.ReduceOp.SUM, group=self.dp_comm.group)   # exactly one non-zero term per entry
+        return part.cpu()
+
+    def load_optimizer_state(self, full):
+        """Restore a buffer returned by ``optimizer_state`` into this replica (every replica loads the full buffer; the
+        entries it does not own are never read)."""
+        if full is None:
+            return
+        buf = self.model.arena.momentum
+        if buf is None or full.numel() != self.model.arena.numel:
+            raise ValueError("optimizer state does not match this model's momentum arena")
+        self.sync_to_model()
+        buf[: full.numel()].copy_(full.to(buf.device))
+        torch.cuda.synchronize(self.device)
+
     def describe(self, sched):
         return self.engine_for(sched).describe()
+
+
+def owned_elements(arena, linears, protocols, dp, rank, shared_to_rank0=False):
+    """Bool mask over ``arena`` (CPU): the parameter elements (weights and bias columns) replica ``rank`` of ``dp``
+    owns when layer i's update runs under ``protocols[i]`` (``_C.DP_PROTO_*``; the rule is ``dp_element_owner`` in
+    ``csrc/kernels/fused_dp.cu``).  Elements every replica owns count for every rank, or only for rank 0 with
+    ``shared_to_rank0``.  Padding belongs to rank 0 only with ``shared_to_rank0``."""
+    C = _C()
+    mask = torch.zeros(arena.numel, dtype=torch.bool)
+    if shared_to_rank0 and rank == 0:
+        mask[:] = True                                     # padding and alignment gaps: zero on every replica
+    for lin, proto in zip(linears, protocols):
+        i = lin.block_index
+        off, ld = int(arena.offsets[i]), int(arena.lds[i])
+        o, k = arena.blocks[i]
+        owners = C.dp_owner_map(int(proto), k, o, ld, off, int(dp))            # [out, in + 1], -1 = every replica
+        shared = owners < 0
+        own = (owners == rank) | (shared if (not shared_to_rank0 or rank == 0) else torch.zeros_like(shared))
+        mask[off:off + o * ld].view(o, ld)[:, : k + 1] = own
+    return mask
 
 
 class Trainer:
@@ -386,7 +454,7 @@ class Trainer:
     def __init__(self, layer_sizes, global_batch_size=128, n_mubatches=4, lr=0.006, schedule="naive",
                  dp_comm=None, pp_comm=None, grid: Optional[ProcessGrid] = None, comm_mode="fused",
                  use_graph=True, device=None, seed_mode="shape", precision="fp32", watchdog_s=None, pp_transport=None,
-                 local_batch_size=None):
+                 local_batch_size=None, momentum=0.0, weight_decay=0.0, nesterov=False):
         from ..models.mlp import MLP
         from ..optimizer import SGD
         from .schedules import SCHEDULE_NAME_TO_CLS
@@ -401,7 +469,8 @@ class Trainer:
         # scale stays 1 / global_batch_size.
         self.local_batch_size = int(local_batch_size) if local_batch_size else global_batch_size // dp
         self.model = MLP(layer_sizes, self.pp_comm.Get_rank(), pp, global_batch_size, seed_mode=seed_mode).to(self.device)
-        self.optimizer = SGD(self.model.parameters(), lr, arena=self.model.arena)
+        self.optimizer = SGD(self.model.parameters(), lr, momentum=momentum, weight_decay=weight_decay, nesterov=nesterov,
+                             arena=self.model.arena)
 
         class _Shape:  # the worker only needs the micro-batch size from the dataset
             mubatch_size = self.local_batch_size // n_mubatches

@@ -75,6 +75,9 @@ def build_parser():
     p.add_argument("--global-batch-size", type=int, default=GLOBAL_BATCH_SIZE)
     p.add_argument("--n-mubatches", type=int, default=N_MUBATCHES)
     p.add_argument("--lr", type=float, default=LEARNING_RATE)
+    p.add_argument("--momentum", type=float, default=0.0, help="SGD momentum (torch.optim.SGD semantics, dampening 0)")
+    p.add_argument("--weight-decay", type=float, default=0.0, help="L2 penalty added to the gradient (biases included)")
+    p.add_argument("--nesterov", action="store_true", help="Nesterov momentum (needs --momentum > 0)")
     p.add_argument("--layer-sizes", type=int, nargs="+", default=None, help="explicit layer widths (default: reference MLP)")
     p.add_argument("--hidden", type=int, default=None, help="with --n-layers: 784 -> hidden x (n-1) -> 10")
     p.add_argument("--n-layers", type=int, default=None)
@@ -163,13 +166,16 @@ def main(args):
     model.to(device)
     model.train()
     hparams = {"lr": float(args.lr), "global_batch_size": int(args.global_batch_size), "seed_mode": str(args.seed_mode),
-               "n_mubatches": int(args.n_mubatches)}
+               "n_mubatches": int(args.n_mubatches), "momentum": float(args.momentum),
+               "weight_decay": float(args.weight_decay), "nesterov": bool(args.nesterov)}
+    # before the resume: the momentum arena it restores is allocated here
+    optimizer = SGD(model.parameters(), lr=args.lr, momentum=args.momentum, weight_decay=args.weight_decay,
+                    nesterov=args.nesterov, arena=model.arena)
     resumed_step = 0
     if args.resume:
         from shallowspeed_b200.utils.checkpoint import load_stage
 
         resumed_step = load_stage(model, args.resume, pp_comm.Get_rank(), args.pp, expect_hparams=hparams)
-    optimizer = SGD(model.parameters(), lr=args.lr, arena=model.arena)
 
     dataset = Dataset(save_dir, global_batch_size=args.global_batch_size,
                       mubatch_size=local_batch_size // args.n_mubatches, validation=False,
@@ -242,8 +248,12 @@ def main(args):
     if args.save:
         from shallowspeed_b200.utils.checkpoint import save_stage
 
+        if engine == "native":
+            momentum = worker.optimizer_state()
+        else:
+            momentum = model.arena.momentum if optimizer.momentum > 0.0 else None
         if dp_comm.Get_rank() == 0:
-            save_stage(model, args.save, pp_comm.Get_rank(), args.pp, step=step, hparams=hparams)
+            save_stage(model, args.save, pp_comm.Get_rank(), args.pp, step=step, hparams=hparams, momentum=momentum)
     logger.close()
     if args.dp * args.pp > 1:
         import torch.distributed as dist

@@ -69,7 +69,9 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
     auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
     volatile uint32_t* flag_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + p.stages * stage_bytes + epi_bytes + 8u * (2 * p.stages));
 
-    const bool db_active = (MODE == GEMM_WGRAD) && (p.db != nullptr) && (by == 0);
+    // the bias gradient is written by the CTA of the LAST column tile: its own tile store is the one that can spill into
+    // the bias column (see the epilogue), so only that CTA can order the two
+    const bool db_active = (MODE == GEMM_WGRAD) && (p.db != nullptr) && (by == (p.n_total - 1) / p.block_n);
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
@@ -334,7 +336,8 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             // TMA stores clip the inner dimension at 16-byte granularity (with in % 4 != 0 the partially valid last
             // chunk may be written in full), i.e. the bias slot in column `in` may just have been overwritten with the
             // (zero) accumulator of an OOB column.  The bias gradient is therefore written strictly AFTER the tile
-            // store retired.
+            // store retired, by this CTA only when it owns the last column tile: a CTA of another column tile could not
+            // order its write against that store, and a plain (non-accumulating) store there would erase it.
             asm volatile("bar.sync 1, 128;" ::: "memory");
             if (db_active && m_ok) {
                 if (p.fuse_sgd) {

@@ -200,6 +200,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         const bool ok = ssb::chain_budget(mb_rows, split, &kps, &stages, &smem);
         return std::make_tuple(ok, kps, stages, smem);
     });
+    m.def("chain_cluster_budget", [](int mb_rows, int cluster, bool split) {
+        int kps = 0, stages = 0, smem = 0;
+        const bool ok = ssb::chain_cluster_budget(mb_rows, cluster, split, &kps, &stages, &smem);
+        return std::make_tuple(ok, kps, stages, smem);
+    });
+    m.def("chain_cluster_size", [](const std::vector<std::pair<int, int>>& in_out, bool do_fwd, bool do_loss, bool do_bwd,
+                                   bool first_stage, bool gated, bool folded) {
+        std::vector<ssb::ChainLayer> ls(in_out.size());
+        for (size_t i = 0; i < in_out.size(); ++i) { ls[i] = ssb::ChainLayer{}; ls[i].in = in_out[i].first; ls[i].out = in_out[i].second; }
+        return ssb::chain_cluster_size(ls.data(), (int)ls.size(), do_fwd, do_loss, do_bwd, first_stage, gated, folded);
+    });
     m.def("chain_eligible", [](const std::vector<std::pair<int, int>>& in_out, int mb_rows, int out_dim, bool has_loss, bool split) {
         std::vector<ssb::ChainLayer> ls(in_out.size());
         for (size_t i = 0; i < in_out.size(); ++i) { ls[i] = ssb::ChainLayer{}; ls[i].in = in_out[i].first; ls[i].out = in_out[i].second; }

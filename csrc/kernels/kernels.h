@@ -242,6 +242,7 @@ struct ChainParams {
     float* loss;                     // [n_mubatches]
     int mb_rows, n_pad, stages;
     int kps;                         // 32-wide k-blocks per pipeline stage (one wait / one commit per stage)
+    int cluster;                     // CTAs per micro-batch (thread-block cluster; 1 = one CTA owns the micro-batch)
     int mu_base;                     // first micro-batch handled by CTA 0 (per-micro-batch launches)
     float inv_batch;
     int do_fwd, do_loss, do_bwd, first_stage;
@@ -270,11 +271,19 @@ struct ChainPlan {
     ChainParams p;
     CUtensorMap* maps_dev;
     int grid, smem_bytes;
+    int cluster;                     // CTAs per micro-batch (grid = micro-batches x cluster)
 };
 bool chain_eligible(const ChainLayer* layers, int n_layers, int mb_rows, int out_dim, bool has_loss, bool split = false);
 const char* chain_plan(ChainPlan* plan, const ChainParams& params, const float* x, int ldx, int total_rows, int n_mubatches,
                        bool split = false);
 bool chain_budget(int mb_rows, bool split, int* kps, int* stages, int* smem_bytes);   // host arithmetic only
+// Cluster plan of one chain launch (host arithmetic only).  chain_cluster_size: CTAs per micro-batch, ceil(w / 32) for the
+// widest tile w the launch writes into shared memory (every forward output, every dgrad output, and dZ_L when a
+// backward-only launch stages it), and 1 for launches gated for a co-resident consumer or with folded pipeline
+// boundaries.  chain_cluster_budget: the shared-memory plan at that size (chain_budget's when cluster == 1).
+int chain_cluster_size(const ChainLayer* layers, int n_layers, bool do_fwd, bool do_loss, bool do_bwd, bool first_stage,
+                       bool gated, bool folded);
+bool chain_cluster_budget(int mb_rows, int cluster, bool split, int* kps, int* stages, int* smem_bytes);
 void chain_plan_free(ChainPlan* plan);
 cudaError_t chain_configure();
 cudaError_t chain_launch(const ChainPlan& plan, cudaStream_t stream);

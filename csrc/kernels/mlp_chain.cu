@@ -16,6 +16,13 @@
 // This removes ~14 dependent kernel launches (and their prologues / cold starts) from the
 // critical path of the reference workload; the per-layer kernels in tc_gemm.cu remain the
 // general path (wide layers) and compute the weight gradients afterwards.
+//
+// Cluster form (CLUSTER, C = ChainParams::cluster CTAs per micro-batch): CTA rank c of the micro-batch's thread-block
+// cluster owns output features [32c, 32c + 32) of every GEMM and streams only that slice of each weight matrix.  Its
+// eight math warps split the k-blocks four ways (warp (q, half) takes the k-blocks kb with kb % 4 == q, for its half of
+// the rows) and add the four partial sums through shared memory in a fixed order.  The 32-feature output is exactly one
+// K-major panel of the next GEMM's B operand: it is written locally and copied into the same offset of every peer
+// (cp.async.bulk shared::cta -> shared::cluster, completion counted on the peer's per-buffer mbarrier).
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -62,8 +69,10 @@ __device__ __forceinline__ unsigned long long gtime() {
 // folded boundary use the instantiation without its prologue and its predicated peer stores.
 // NTW: n8 tiles of a math warp's accumulator (chain_warp_cols / 8, rounded up to 2, 4 or 8) - sized at compile time
 // so that small micro-batches keep their accumulators in a few registers.
-template <bool SPLIT, bool FOLD, int NTW>
+// CLUSTER: the cluster form (see the top of the file); never combined with FOLD.
+template <bool SPLIT, bool FOLD, int NTW, bool CLUSTER>
 __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParams p) {
+    static_assert(!(FOLD && CLUSTER), "folded pipeline launches run one CTA per micro-batch");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t smem_base = (raw + 1023u) & ~1023u;
@@ -72,29 +81,41 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int L = p.n_layers;
     const int N = p.n_pad;                                   // tile N (rows of this micro-batch, padded to 16)
-    const int row0 = (p.mu_base + (int)blockIdx.x) * p.mb_rows;                 // first global row of this micro-batch
+    const int rank = CLUSTER ? (int)cluster_ctarank() : 0;  // feature slice [32 rank, 32 rank + 32) of every GEMM
+    const int mb = CLUSTER ? (int)blockIdx.x / p.cluster : (int)blockIdx.x;   // micro-batch of this CTA (in the launch)
+    const int row0 = (p.mu_base + mb) * p.mb_rows;           // first global row of this micro-batch
+    const uint32_t a_bytes = CLUSTER ? kPanelBytes : kABytes;   // one k-block of the weight operand: 32 or 128 features
     const uint32_t b_bytes = (uint32_t)N * 128u;             // one 32-feature panel of an activation tile
-    const uint32_t stage_bytes = (uint32_t)p.kps * (kABytes + b_bytes);   // kps A tiles, then kps X tiles (layer 1)
-    const uint32_t stage_b_off = (uint32_t)p.kps * kABytes;
+    const uint32_t stage_bytes = (uint32_t)p.kps * (a_bytes + b_bytes);   // kps A tiles, then kps X tiles (layer 1)
+    const uint32_t stage_b_off = (uint32_t)p.kps * a_bytes;
     const uint32_t abuf_bytes = 4u * b_bytes;
     const uint32_t abuf0 = smem_base + p.stages * stage_bytes;            // activation ping-pong
     const uint32_t bar_base = abuf0 + 2u * abuf_bytes;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
-    // loss-head transpose scratch [N][kScratchLd] floats behind the barriers
-    const uint32_t scratch_off = p.stages * stage_bytes + 2u * abuf_bytes + 8u * (2 * p.stages) + 128u;
+    auto recv_bar = [&](int b) { return bar_base + 8u * (2 * p.stages + b); };   // CLUSTER: peer panels of abuf b landed
+    // loss-head transpose scratch [N][kScratchLd] floats behind the barriers (CLUSTER: shared with the k-phase partials)
+    const uint32_t scratch_off = p.stages * stage_bytes + 2u * abuf_bytes + 8u * (2 * p.stages + (CLUSTER ? 2 : 0)) + 128u;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < p.stages; ++s) {
             mbar_init(full_bar(s), 1);
             mbar_init(empty_bar(s), 8);                      // one arrive per math warp
         }
+        if constexpr (CLUSTER) {
+            mbar_init(recv_bar(0), 1);                       // the local arm; the peers' bytes are transaction counts
+            mbar_init(recv_bar(1), 1);
+        }
         fence_barrier_init();
     }
-    __syncthreads();
+    if constexpr (CLUSTER) cluster_sync();                   // the peers' barriers are initialised before any copy targets them
+    else __syncthreads();
 
     // number of backward GEMMs: layers L..lo (layer 1's dgrad is skipped on the first stage)
     const int bwd_lo = p.first_stage ? 2 : 1;
+    // CLUSTER: a CTA whose feature slice starts at or beyond a GEMM's output width has nothing to compute in it (the
+    // 10-class logits on ranks >= 1); producer and math warps skip it alike
+    auto idle = [&](int width) { return CLUSTER && 32 * rank >= width; };
 
     if (warp == 0) {
         // ============================================================ weight (and X) producer
@@ -109,6 +130,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             };
             if (p.do_fwd) {
                 for (int l = 1; l <= L; ++l) {
+                    if (idle(p.layers[l - 1].out)) continue;
                     const int nkb = (p.layers[l - 1].in + (int)kBlockK - 1) / (int)kBlockK;
                     const bool with_x = (l == 1) && !(FOLD && p.x_from_global);   // folded pipeline input: staged by the epilogue warps
                     for (int kb0 = 0; kb0 < nkb; kb0 += p.kps, ++it) {
@@ -117,9 +139,10 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         const uint32_t a_dst = smem_base + s * stage_bytes;
                         if (elect_one()) {
                             DBG(0, it);
-                            mbar_arrive_expect_tx(full_bar(s), (uint32_t)cnt * (kABytes + (with_x ? b_bytes : 0u)));
+                            mbar_arrive_expect_tx(full_bar(s), (uint32_t)cnt * (a_bytes + (with_x ? b_bytes : 0u)));
                             for (int j = 0; j < cnt; ++j) {
-                                tma_load_2d(a_dst + j * kABytes, p.maps + 2 * (l - 1), full_bar(s), (kb0 + j) * kBlockK, 0);
+                                // CLUSTER: the 32 rows of W_l this CTA's features need (32-row box)
+                                tma_load_2d(a_dst + j * a_bytes, p.maps + 2 * (l - 1), full_bar(s), (kb0 + j) * kBlockK, 32 * rank);
                                 if (with_x)
                                     tma_load_2d(a_dst + stage_b_off + j * b_bytes, p.maps + 2 * L, full_bar(s), (kb0 + j) * kBlockK, row0);
                             }
@@ -130,6 +153,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             }
             if (p.do_bwd) {
                 for (int l = L; l >= bwd_lo; --l) {
+                    if (idle(p.layers[l - 1].in)) continue;
                     const int nkb = (p.layers[l - 1].out + (int)kBlockK - 1) / (int)kBlockK;
                     for (int kb0 = 0; kb0 < nkb; kb0 += p.kps, ++it) {
                         const int cnt = min(p.kps, nkb - kb0);
@@ -137,12 +161,17 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         const uint32_t a_dst = smem_base + s * stage_bytes;
                         if (elect_one()) {
                             DBG(0, it);
-                            mbar_arrive_expect_tx(full_bar(s), (uint32_t)cnt * kABytes);
+                            mbar_arrive_expect_tx(full_bar(s), (uint32_t)cnt * a_bytes);
                             for (int j = 0; j < cnt; ++j) {
+                                if constexpr (CLUSTER) {
+                                    // MN-major panel `rank` of the k-block: this CTA's 32 output features
+                                    tma_load_2d(a_dst + j * a_bytes, p.maps + 2 * (l - 1) + 1, full_bar(s), 32 * rank, (kb0 + j) * kBlockK);
+                                } else {
 #pragma unroll
-                                for (int i = 0; i < 4; ++i)
-                                    tma_load_2d(a_dst + j * kABytes + i * kPanelBytes, p.maps + 2 * (l - 1) + 1, full_bar(s), 32 * i,
-                                                (kb0 + j) * kBlockK);
+                                    for (int i = 0; i < 4; ++i)
+                                        tma_load_2d(a_dst + j * kABytes + i * kPanelBytes, p.maps + 2 * (l - 1) + 1, full_bar(s), 32 * i,
+                                                    (kb0 + j) * kBlockK);
+                                }
                             }
                         }
                         __syncwarp();
@@ -156,9 +185,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         // MMAs of exactly the block its epilogue consumes, so accumulators never leave the warp's registers (lane r reads
         // feature row r through warp_acc_row16).  The activation tile of the next GEMM is written by all 8 warps and
         // published with one named barrier among them.
+        // CLUSTER: q is the warp's k-phase; every warp covers the CTA's 32 features and the (q == 0) warps run the
+        // epilogues on the reduced sums
         const int q = warp & 3;
         const int half = (warp - 1) >> 2;
-        const int m = q * 32 + lane;                         // feature handled by this thread in the epilogue
+        const int m = (CLUSTER ? 32 * rank : q * 32) + lane;   // feature handled by this thread in the epilogue
+        const bool epi = !CLUSTER || q == 0;                 // this warp runs the epilogues
         // column (= row of the micro-batch) range of this warp, in chunks of 16
         const int n_chunks = N / 16;
         const int c_lo = 16 * ((n_chunks * half) / 2), c_hi = 16 * ((n_chunks * (half + 1)) / 2);
@@ -166,29 +198,72 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         float acc[2][NTW][4];                                // this warp's block of the current layer's product
         int it = 0, gemm_i = 0;
         int wbuf = 0;                                        // activation buffer the NEXT epilogue writes
+        uint32_t recv_phase = 0u;                            // CLUSTER: parity of recv_bar(b) in bit b
+        // CLUSTER: the tile in abuf b is complete once the peers' panels landed (see exchange below)
+        auto wait_recv = [&](int b) {
+            mbar_wait(recv_bar(b), (recv_phase >> b) & 1u);
+            recv_phase ^= 1u << b;
+        };
+        // CLUSTER: acc of warp (0, half) += the partial sums of warps (1..3, half), in that order
+        auto reduce_kphases = [&]() {
+            constexpr int kFrag = 2 * NTW * 4;               // accumulator floats per lane
+            float* red = reinterpret_cast<float*>(smem_gen + scratch_off);   // [3 phases][2 halves][kFrag][32 lanes]
+            if (q != 0) {
+                float* dst = red + ((q - 1) * 2 + half) * kFrag * 32 + lane;
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+#pragma unroll
+                    for (int j = 0; j < NTW; ++j)
+                        if (j < nt)
+#pragma unroll
+                            for (int r = 0; r < 4; ++r) dst[((i * NTW + j) * 4 + r) * 32] = acc[i][j][r];
+            }
+            asm volatile("bar.sync 2, 256;" ::: "memory");
+            if (q == 0) {
+#pragma unroll
+                for (int ph = 0; ph < 3; ++ph) {
+                    const float* src = red + (ph * 2 + half) * kFrag * 32 + lane;
+#pragma unroll
+                    for (int i = 0; i < 2; ++i)
+#pragma unroll
+                        for (int j = 0; j < NTW; ++j)
+                            if (j < nt)
+#pragma unroll
+                                for (int r = 0; r < 4; ++r) acc[i][j][r] += src[((i * NTW + j) * 4 + r) * 32];
+                }
+            }
+        };
         // D[features, rows] of one layer: A = weights from the ring (K-major forward, MN-major backward), B = the
-        // activation tile (layer 1: X from the ring slots) -> acc
-        auto run_gemm = [&](int nkb, bool a_mn, bool b_from_stage, uint32_t bsrc) {
+        // activation tile (layer 1: X from the ring slots) -> acc.  skip: CLUSTER, no features here (see idle)
+        auto run_gemm = [&](int nkb, bool a_mn, bool b_from_stage, uint32_t bsrc, bool skip) {
             if (threadIdx.x == 32) DBG(1, 2 * gemm_i);
             warp_acc_zero(acc);
-            for (int kb0 = 0; kb0 < nkb; kb0 += p.kps, ++it) {
+            if constexpr (CLUSTER) {
+                if (!b_from_stage) wait_recv((int)((bsrc - abuf0) / abuf_bytes));
+            }
+            for (int kb0 = 0; kb0 < nkb && !skip; kb0 += p.kps, ++it) {
                 const int cnt = min(p.kps, nkb - kb0);
                 const int s = it % p.stages;
                 mbar_wait(full_bar(s), (it / p.stages) & 1);
                 const uint32_t a_src = smem_base + s * stage_bytes;
                 for (int j = 0; j < cnt; ++j) {
-                    const uint32_t a_j = a_src + j * kABytes;
+                    if constexpr (CLUSTER) {
+                        if (((kb0 + j) & 3) != q) continue;  // k-phase q of the GEMM
+                    }
+                    const uint32_t a_j = a_src + j * a_bytes;
                     const uint32_t b_j = b_from_stage ? a_src + stage_b_off + j * b_bytes : bsrc + (kb0 + j) * b_bytes;
+                    const uint32_t m_base = CLUSTER ? 0u : (uint32_t)q * 32u;
                     if (a_mn)
-                        warp_mma_kblock<NTW, true, false, SPLIT>(acc, a_j, (uint32_t)q * 32u, b_j, (uint32_t)c_lo, nt, lane);
+                        warp_mma_kblock<NTW, true, false, SPLIT>(acc, a_j, m_base, b_j, (uint32_t)c_lo, nt, lane);
                     else
-                        warp_mma_kblock<NTW, false, false, SPLIT>(acc, a_j, (uint32_t)q * 32u, b_j, (uint32_t)c_lo, nt, lane);
+                        warp_mma_kblock<NTW, false, false, SPLIT>(acc, a_j, m_base, b_j, (uint32_t)c_lo, nt, lane);
                 }
                 __syncwarp();
                 if (lane == 0) mbar_arrive(empty_bar(s));
             }
             if (threadIdx.x == 32) DBG(1, 2 * gemm_i + 1);
             ++gemm_i;
+            if constexpr (CLUSTER) reduce_kphases();
         };
         auto st_tile = [&](uint32_t dst, int n, int feat, float x) {   // operand tile for the next GEMM
             *reinterpret_cast<float*>(smem_gen + (dst - smem_base) + act_smem_off(n, feat, b_bytes)) = x;
@@ -203,6 +278,30 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         auto publish = [&]() {                               // smem tile complete -> every math warp may read it
             if (threadIdx.x == 32) DBG(2, gemm_i);
             asm volatile("bar.sync 2, 256;" ::: "memory");
+        };
+        // CLUSTER, instead of publish() for a tile another GEMM consumes: this CTA's panel of abuf b goes to the same
+        // offset in every peer, and recv_bar(b) is armed for the (C - 1) panels coming in (awaited by run_gemm).  Every
+        // CTA sends its panel, features or not, so that every CTA takes part in every exchange.  That is what makes the
+        // ping-pong reuse safe without a cluster barrier per tile: a peer writes the tile after next into my abuf b only
+        // after it received my panel of the next tile (abuf b^1), and I send that panel only after my GEMM finished
+        // reading abuf b, which it started after all of this tile's panels had landed here.  By the same chain my copies
+        // out of abuf b have completed (their peers waited for them) before my epilogue writes abuf b again, and every
+        // copy into this CTA has landed before it reaches the cluster barrier at the end of the kernel.
+        auto exchange = [&](int b) {
+            fence_proxy_async_smem();                        // my st.shared of the panel -> the bulk copy's reads
+            publish();
+            if (threadIdx.x == 32) {
+                const uint32_t bar = recv_bar(b);
+                const uint32_t src = abuf0 + (uint32_t)b * abuf_bytes + (uint32_t)rank * b_bytes;   // act_smem_off panel
+                mbar_arrive_expect_tx(bar, (uint32_t)(p.cluster - 1) * b_bytes);
+                for (int r = 0; r < p.cluster; ++r)
+                    if (r != rank) bulk_copy_s2cluster(mapa_shared(src, (uint32_t)r), src, b_bytes, mapa_shared(bar, (uint32_t)r));
+            }
+        };
+        // end of a tile the next GEMM reads
+        auto hand_over = [&](int b) {
+            if constexpr (CLUSTER) exchange(b);
+            else publish();
         };
         int buf = 0;                                         // activation buffer the NEXT gemm reads
         // ---------------- folded pipeline boundaries (see ChainParams): credit of the slots we will write, arrival of
@@ -241,7 +340,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 const int nkb_f = (ly.in + (int)kBlockK - 1) / (int)kBlockK;
                 // layer 1 reads X from its ring slots (TMA), or - folded pipeline input - from abuf 1 (staged above)
                 const bool x_glob = FOLD && (l == 1) && p.x_from_global;
-                run_gemm(nkb_f, false, l == 1 && !x_glob, abuf0 + (x_glob ? 1 : buf) * abuf_bytes);
+                run_gemm(nkb_f, false, l == 1 && !x_glob, abuf0 + (x_glob ? 1 : buf) * abuf_bytes, idle(ly.out));
                 if (l > 1) buf ^= 1;                         // layer l read buf, wrote buf^1
                 else buf = 0;                                // layer 1 writes abuf 0
                 if (p.sync_debug) asm volatile("bar.sync 2, 256;" ::: "memory");   // racecheck aid, see kernels.h
@@ -253,7 +352,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     const bool single = (c_hi - c_lo == 16);
                     float keep[16];
 #pragma unroll
-                    for (int ch = 0; ch < NTW / 2; ++ch) {
+                    for (int ch = 0; ch < NTW / 2 && epi; ++ch) {
                         const int c = c_lo + 16 * ch;
                         if (c >= c_hi) break;
                         float v[16];
@@ -272,8 +371,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                             }
                         }
                     }
-                    publish();
-                    if (single && m_ok) {
+                    if (l < L) hand_over(wbuf);
+                    else publish();
+                    if (epi && single && m_ok) {
 #pragma unroll
                         for (int j = 0; j < 16; ++j)
                             if (c_lo + j < p.mb_rows) {
@@ -289,9 +389,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     // Step 1: the class-lane warps (q == 0, both halves) transpose logits (+bias) into a [row][class]
                     // scratch in smem.  Step 2: each lane of warp (0, 0) owns ROWS, loops over the <= 32 classes in
                     // registers - no cross-lane reductions except one max and one sum for the whole micro-batch.
+                    // CLUSTER: the <= 32 classes are rank 0's features; the scratch is where the k-phase partials were
+                    // (all of them read before the barrier)
                     const int C = ly.out;
                     float* scratch = reinterpret_cast<float*>(smem_gen + scratch_off);   // [N][kScratchLd]
                     float loss = 0.f;
+                    if constexpr (CLUSTER) asm volatile("bar.sync 2, 256;" ::: "memory");
                     if (q == 0) {
 #pragma unroll
                         for (int ch = 0; ch < NTW / 2; ++ch) {
@@ -305,7 +408,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         }
                     }
                     asm volatile("bar.sync 2, 256;" ::: "memory");
-                    if (q == 0 && half == 0) {
+                    if (q == 0 && half == 0 && rank == 0) {
                         float gmax = -3.0e38f;
                         for (int n = lane; n < p.mb_rows; n += 32)
                             for (int k = 0; k < C; ++k) gmax = fmaxf(gmax, scratch[n * kScratchLd + k]);
@@ -376,10 +479,11 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                                 for (int k = C; k < 32; ++k) st_tile(dst, n, k, 0.f);
                         }
                         loss = warp_sum_f(loss);
-                        if (lane == 0 && p.loss != nullptr) p.loss[p.mu_base + blockIdx.x] = loss * p.inv_batch;
+                        if (lane == 0 && p.loss != nullptr) p.loss[p.mu_base + mb] = loss * p.inv_batch;
                     }
                     if (p.do_bwd) {
-                        publish();
+                        if (L >= bwd_lo) hand_over(wbuf);
+                        else publish();
                         wbuf ^= 1;
                     }
                     signal_ready(l);                          // dz[L] written by the class-lane warp; the others arrive empty
@@ -401,7 +505,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             const uint32_t dst = abuf0 + wbuf * abuf_bytes;
             float* __restrict__ g = p.dz[L] + (int64_t)row0 * p.act_ld[L];
             const float* __restrict__ y = p.act[L] + (int64_t)row0 * p.act_ld[L];
-            for (int n = c_lo; n < c_hi; ++n) {
+            for (int n = c_lo; n < c_hi && epi; ++n) {
                 float x = 0.f;
                 if (m_ok && n < p.mb_rows) {
                     asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(x) : "l"(g + (int64_t)n * p.act_ld[L] + m));   // may be peer-written
@@ -410,7 +514,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 }
                 st_tile(dst, n, m, x);
             }
-            publish();
+            if (L >= bwd_lo) hand_over(wbuf);
+            else publish();
             wbuf ^= 1;
         }
         if (p.do_bwd) {
@@ -424,13 +529,13 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 // the masks do not depend on the MMA: fetch them before it runs (N <= 32: all of them)
                 float mk0[16];
                 const bool pre = (c_hi - c_lo == 16);        // N <= 32: one chunk per warp, prefetch its masks
-                if (pre) {
+                if (pre && epi) {
 #pragma unroll
                     for (int j = 0; j < 16; ++j)
                         mk0[j] = (mask_on && m_ok && c_lo + j < p.mb_rows) ? yprev[(int64_t)(c_lo + j) * p.act_ld[l - 1] + m] : 1.f;
                 }
                 const int nkb = (ly.out + (int)kBlockK - 1) / (int)kBlockK;
-                run_gemm(nkb, true, false, abuf0 + buf * abuf_bytes);
+                run_gemm(nkb, true, false, abuf0 + buf * abuf_bytes, idle(ly.in));
                 buf ^= 1;
                 if (p.sync_debug) asm volatile("bar.sync 2, 256;" ::: "memory");   // racecheck aid, see kernels.h
                 const uint32_t dst = abuf0 + wbuf * abuf_bytes;
@@ -438,7 +543,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 const bool single = (c_hi - c_lo == 16);
                 float keep[16];
 #pragma unroll
-                for (int ch = 0; ch < NTW / 2; ++ch) {
+                for (int ch = 0; ch < NTW / 2 && epi; ++ch) {
                     const int c = c_lo + 16 * ch;
                     if (c >= c_hi) break;
                     float v[16];
@@ -464,10 +569,10 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     }
                 }
                 if (more) {
-                    publish();
+                    hand_over(wbuf);
                     wbuf ^= 1;
                 }
-                if (single && m_ok) {
+                if (epi && single && m_ok) {
 #pragma unroll
                     for (int j = 0; j < 16; ++j)
                         if (c_lo + j < p.mb_rows) {
@@ -487,6 +592,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             }
         }
     }
+    // no CTA leaves while a peer may still address its shared memory
+    if constexpr (CLUSTER) cluster_sync();
 }
 
 // =========================================================================== host side
@@ -517,6 +624,51 @@ bool chain_budget(int mb_rows, bool split, int* kps_out, int* stages_out, int* s
     return true;
 }
 
+// accumulator width (n8 tiles) of a math warp, the NTW instantiation chain_launch picks
+static int chain_ntw(int n_pad) {
+    const int cols = chain_warp_cols(n_pad);
+    return cols <= 16 ? 2 : cols <= 32 ? 4 : 8;
+}
+
+int chain_cluster_size(const ChainLayer* layers, int n_layers, bool do_fwd, bool do_loss, bool do_bwd, bool first_stage,
+                       bool gated, bool folded) {
+    // gated: the co-resident consumer's eligibility assumes the chain occupies one SM per micro-batch; folded: the
+    // flag / credit protocol of the pipeline boundaries runs per CTA
+    if (gated || folded || n_layers < 1) return 1;
+    int w = 0;
+    if (do_fwd)
+        for (int l = 0; l < n_layers; ++l) w = std::max(w, layers[l].out);
+    if (do_bwd) {
+        for (int l = first_stage ? 2 : 1; l <= n_layers; ++l) w = std::max(w, layers[l - 1].in);
+        if (!(do_fwd && do_loss)) w = std::max(w, layers[n_layers - 1].out);   // dZ_L staged from global memory
+    }
+    return std::min(4, std::max(1, (w + 31) / 32));
+}
+
+// Cluster form: the ring holds 32-row weight panels (plus the X tiles of layer 1), the k-phase partials of warps
+// (1..3, half) share the scratch with the loss head.
+bool chain_cluster_budget(int mb_rows, int cluster, bool split, int* kps_out, int* stages_out, int* smem_bytes_out) {
+    if (cluster <= 1) return chain_budget(mb_rows, split, kps_out, stages_out, smem_bytes_out);
+    if (cluster > 4 || mb_rows < 1 || mb_rows > 128) return false;
+    const int n_pad = (mb_rows + 15) / 16 * 16;
+    const int abuf_bytes = 4 * n_pad * 128;
+    const int partial_bytes = 3 * 2 * (2 * chain_ntw(n_pad) * 4) * 32 * 4;
+    const int scratch_bytes = std::max(partial_bytes, n_pad * kScratchLd * 4 + 256);
+    const int budget = 222 * 1024 - 2 * abuf_bytes - scratch_bytes;
+    int kps = 4, stage_bytes = 0, stages = 0;
+    for (; kps >= 1; kps >>= 1) {
+        stage_bytes = kps * ((int)kPanelBytes + n_pad * 128);
+        stages = budget / stage_bytes;
+        if (stages >= 2) break;
+    }
+    if (kps < 1 || stages < 2) return false;
+    if (stages > 8) stages = 8;
+    *kps_out = kps;
+    *stages_out = stages;
+    *smem_bytes_out = stages * stage_bytes + 2 * abuf_bytes + 1024 + 8 * (2 * stages + 2) + 128 + scratch_bytes;
+    return true;
+}
+
 static bool chain_smem_fits(int mb_rows, bool split) {
     int kps, stages, smem;
     return chain_budget(mb_rows, split, &kps, &stages, &smem);
@@ -541,10 +693,16 @@ const char* chain_plan(ChainPlan* plan, const ChainParams& params, const float* 
     const int L = p.n_layers;
     p.n_pad = (p.mb_rows + 15) / 16 * 16;
     p.split = split ? 1 : 0;                      // 3xTF32: the kernel derives the lo parts of its operands from the staged tiles
+    const bool fold = p.in_flag != nullptr || p.out_peer != nullptr || p.x_from_global != 0;
+    const int C = chain_cluster_size(p.layers, L, p.do_fwd != 0, p.do_loss != 0, p.do_bwd != 0, p.first_stage != 0,
+                                     p.ready != nullptr, fold);
+    if (C > 1 && (p.ready != nullptr || fold)) return "chain_plan: gated and folded launches run one CTA per micro-batch";
+    p.cluster = C;
     std::vector<CUtensorMap> host(2 * L + 1);
     for (int l = 0; l < L; ++l) {
         const ChainLayer& ly = p.layers[l];
-        if (const char* e = make_tmap_k(&host[2 * l], p.W + ly.w_off, ly.in, ly.out, ly.ldw, kBlockM)) return e;
+        // forward A operand: all 128 feature rows per k-block, or the 32 of one CTA of a cluster
+        if (const char* e = make_tmap_k(&host[2 * l], p.W + ly.w_off, ly.in, ly.out, ly.ldw, C > 1 ? 32 : (int)kBlockM)) return e;
         if (const char* e = make_tmap_mn(&host[2 * l + 1], p.W + ly.w_off, ly.in, ly.out, ly.ldw)) return e;
     }
     if (x != nullptr) {
@@ -559,11 +717,12 @@ const char* chain_plan(ChainPlan* plan, const ChainParams& params, const float* 
     plan->maps_dev = dev;
     p.maps = dev;
     int kps = 0, stages = 0, smem = 0;
-    if (!chain_budget(p.mb_rows, p.split != 0, &kps, &stages, &smem)) return "chain_plan: shared memory budget too small";
+    if (!chain_cluster_budget(p.mb_rows, C, p.split != 0, &kps, &stages, &smem)) return "chain_plan: shared memory budget too small";
     p.kps = kps;
     p.stages = stages;
     plan->smem_bytes = smem;
-    plan->grid = n_mubatches;
+    plan->grid = n_mubatches * C;
+    plan->cluster = C;
     return nullptr;
 }
 
@@ -576,10 +735,12 @@ template <int NTW>
 static cudaError_t chain_configure_ntw() {
     cudaError_t e;
     const int smem = 227 * 1024;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, true, NTW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    return cudaFuncSetAttribute(mlp_chain_kernel<true, true, NTW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, true, NTW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, true, NTW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    return cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
 }
 
 cudaError_t chain_configure() {
@@ -589,25 +750,47 @@ cudaError_t chain_configure() {
     return chain_configure_ntw<8>();
 }
 
+// grid = micro-batches x plan.cluster, cluster dims (plan.cluster, 1, 1)
+template <bool SPLIT, int NTW>
+static cudaError_t chain_launch_cluster(const ChainPlan& plan, cudaStream_t stream) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)plan.grid);
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = (size_t)plan.smem_bytes;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)plan.cluster;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, mlp_chain_kernel<SPLIT, false, NTW, true>, plan.p);
+}
+
 template <int NTW>
-static void chain_launch_ntw(const ChainPlan& plan, bool fold, cudaStream_t stream) {
+static cudaError_t chain_launch_ntw(const ChainPlan& plan, bool fold, cudaStream_t stream) {
     const ChainParams& p = plan.p;
-#define SSB_CHAIN_LAUNCH(S, F) mlp_chain_kernel<S, F, NTW><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(p)
+    if (plan.cluster > 1) return p.split ? chain_launch_cluster<true, NTW>(plan, stream) : chain_launch_cluster<false, NTW>(plan, stream);
+#define SSB_CHAIN_LAUNCH(S, F) mlp_chain_kernel<S, F, NTW, false><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(p)
     if (!p.split) {
         if (fold) SSB_CHAIN_LAUNCH(false, true); else SSB_CHAIN_LAUNCH(false, false);
     } else {
         if (fold) SSB_CHAIN_LAUNCH(true, true); else SSB_CHAIN_LAUNCH(true, false);
     }
 #undef SSB_CHAIN_LAUNCH
+    return cudaSuccess;
 }
 
 cudaError_t chain_launch(const ChainPlan& plan, cudaStream_t stream) {
     const ChainParams& p = plan.p;
     const bool fold = p.in_flag != nullptr || p.out_peer != nullptr || p.x_from_global != 0;
-    const int cols = chain_warp_cols(p.n_pad);
-    if (cols <= 16) chain_launch_ntw<2>(plan, fold, stream);
-    else if (cols <= 32) chain_launch_ntw<4>(plan, fold, stream);
-    else chain_launch_ntw<8>(plan, fold, stream);
+    const int ntw = chain_ntw(p.n_pad);
+    cudaError_t e;
+    if (ntw == 2) e = chain_launch_ntw<2>(plan, fold, stream);
+    else if (ntw == 4) e = chain_launch_ntw<4>(plan, fold, stream);
+    else e = chain_launch_ntw<8>(plan, fold, stream);
+    if (e != cudaSuccess) return e;
     return cudaGetLastError();
 }
 

@@ -94,6 +94,29 @@ __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.b
 // make generic-proxy smem writes visible to the async proxy (TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// ------------------------------------------------------------------ thread-block clusters (distributed shared memory)
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// the shared::cluster address of the same offset in CTA `rank` of this cluster
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t smem_addr, uint32_t rank) {
+    uint32_t d;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(d) : "r"(smem_addr), "r"(rank));
+    return d;
+}
+// every thread of every CTA of the cluster: release what it wrote before, acquire what the others wrote
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// contiguous bulk copy from this CTA's shared memory into a peer's (dst and bar: shared::cluster addresses from
+// mapa_shared); completion is counted as `bytes` of transaction on the peer's mbarrier
+__device__ __forceinline__ void bulk_copy_s2cluster(uint32_t dst, uint32_t src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(dst), "r"(src), "r"(bytes), "r"(bar) : "memory");
+}
+
 // ------------------------------------------------------------------ warp-level TF32 tensor-core tiles
 // Every operand tile in shared memory is made of 128-byte rows (32 fp32) in the TMA SWIZZLE_128B layout: the 16-byte
 // chunk index of an element is XOR-ed with (row & 7), rows 128 B apart, tile base 1024 B aligned.

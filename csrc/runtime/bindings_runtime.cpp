@@ -236,6 +236,7 @@ public:
     int64_t kernels_per_step() { return engine_->kernels_per_step(); }
     int64_t graph_nodes() { return engine_->graph_nodes(); }
     bool uses_chain() { return engine_->uses_chain(); }
+    int chain_cluster() { return engine_->chain_cluster(); }
     bool coalesced() { return engine_->coalesced(); }
     int64_t main_stream() { return reinterpret_cast<int64_t>(engine_->main_stream()); }
     std::string describe() { return engine_->describe(); }
@@ -316,6 +317,7 @@ void bind_runtime(py::module_& m) {
         .def("kernels_per_step", &PyEngine::kernels_per_step)
         .def("graph_nodes", &PyEngine::graph_nodes)
         .def("uses_chain", &PyEngine::uses_chain)
+        .def("chain_cluster", &PyEngine::chain_cluster)
         .def("coalesced", &PyEngine::coalesced)
         .def("main_stream", &PyEngine::main_stream)
         .def("describe", &PyEngine::describe)

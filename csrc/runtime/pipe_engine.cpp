@@ -846,6 +846,8 @@ void PipeEngine::build_coalesced() {
                 // the dgrad that reads W_l has produced dz[l-1] (layer 1 of the first stage has no dgrad)
                 ly.gate_flag = gate_ready_ + l;
                 ly.gate_w = l >= 2 ? gate_ready_ + (l - 1) : nullptr;
+                // 8 epilogue warps per micro-batch count up every counter: gated chain launches run one CTA per micro-batch
+                if (chain_cluster() != 1) throw std::runtime_error("PipeEngine: a gated chain launch must run one CTA per micro-batch");
                 ly.gate_mult = 8u * (uint32_t)M;
             }
             ll_layers.push_back(ly);

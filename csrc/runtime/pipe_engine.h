@@ -17,6 +17,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdint>
 #include <functional>
 #include <string>
@@ -134,6 +135,12 @@ public:
     int64_t graph_nodes() const { return graph_nodes_; }
     bool coalesced() const { return coalesced_; }
     bool uses_chain() const { return chain_ok_; }
+    // CTAs per micro-batch of the chain launches (the largest over the plan; 0 without chain launches)
+    int chain_cluster() const {
+        int c = 0;
+        for (const ChainPlan& cp : chain_plans_) c = std::max(c, cp.cluster);
+        return c;
+    }
     cudaStream_t main_stream() { return streams_[0]; }
     const EngineConfig& config() const { return cfg_; }
     // per layer: the DpProto under which its update runs (which replica owns which momentum entries)

@@ -112,8 +112,11 @@ static void linear_wgrad(const Tensor& dz, const Tensor& x, Tensor& G, bool accu
 }
 
 static void loss_head(const Tensor& logits, const c10::optional<Tensor>& target, const c10::optional<Tensor>& probs,
-                      const c10::optional<Tensor>& dlogits, const c10::optional<Tensor>& loss_out, double inv_batch) {
+                      const c10::optional<Tensor>& dlogits, const c10::optional<Tensor>& loss_out, double inv_batch,
+                      int loss) {
     check_mat(logits, "logits");
+    TORCH_CHECK(loss == ssb::LOSS_MSE || loss == ssb::LOSS_CROSS_ENTROPY, "loss_head: loss must be 0 (MSE) or 1 (cross-entropy)");
+    TORCH_CHECK(!target.has_value() || dlogits.has_value(), "loss_head: training (a target) needs dlogits");
     c10::cuda::CUDAGuard guard(logits.device());
     const int rows = logits.size(0), cols = logits.size(1);
     cuda_ok(ssb::launch_loss_head(logits.data_ptr<float>(), ld_of(logits),
@@ -121,7 +124,7 @@ static void loss_head(const Tensor& logits, const c10::optional<Tensor>& target,
                                   probs.has_value() ? probs->data_ptr<float>() : nullptr, probs.has_value() ? ld_of(*probs) : 0,
                                   dlogits.has_value() ? dlogits->data_ptr<float>() : nullptr, dlogits.has_value() ? ld_of(*dlogits) : 0,
                                   loss_out.has_value() ? loss_out->data_ptr<float>() : nullptr, rows, cols, (float)inv_batch,
-                                  cur_stream()), "loss_head");
+                                  cur_stream(), 0, loss), "loss_head");
 }
 
 static void softmax_grad(const Tensor& logits, const Tensor& upstream, Tensor& dlogits) {
@@ -185,7 +188,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("linear_wgrad", &linear_wgrad, py::arg("dz"), py::arg("x"), py::arg("G"), py::arg("accumulate"), py::arg("db"),
           py::arg("db_stride"), py::arg("W"), py::arg("lr"), py::arg("fuse_sgd"), py::arg("split") = false,
           py::arg("V") = py::none(), py::arg("momentum") = 0.0, py::arg("weight_decay") = 0.0, py::arg("nesterov") = false);
-    m.def("loss_head", &loss_head);
+    m.def("loss_head", &loss_head, py::arg("logits"), py::arg("target"), py::arg("probs"), py::arg("dlogits"),
+          py::arg("loss_out"), py::arg("inv_batch"), py::arg("loss") = (int)ssb::LOSS_MSE);
     m.def("softmax_grad", &softmax_grad);
     m.def("relu_mask_", &relu_mask_);
     m.def("relu_fwd", &relu_fwd);

@@ -38,6 +38,9 @@ __device__ float block_reduce(float v, float* scratch) {
 //   MODE 0: probs only (inference / functional.softmax)
 //   MODE 1: loss backward: dz = J_softmax^T * (-2 (t - p) * inv_batch), loss = sum (t-p)^2 * inv_batch
 //   MODE 2: generic softmax backward with a given upstream gradient
+// Softmax cross-entropy (per-row softmax, no global max, no +1e-7; the formulas are ptx.cuh's ce_*):
+//   MODE 3: loss backward: probs, dz = (p * sum(t) - t) * inv_batch, loss = sum t ((m - z) + log s) * inv_batch
+//   MODE 4: probs only (inference)
 template <int MODE>
 __global__ void __launch_bounds__(256) loss_head_kernel(const float* __restrict__ logits, int ldl,
                                                         const float* __restrict__ aux, int lda,   // target | upstream
@@ -55,6 +58,39 @@ __global__ void __launch_bounds__(256) loss_head_kernel(const float* __restrict_
     if (probs != nullptr) probs += (size_t)row0 * ldp;
     if (dlogits != nullptr) dlogits += (size_t)row0 * ldd;
     if (loss_out != nullptr) loss_out += blockIdx.x;
+
+    if constexpr (MODE >= 3) {
+        // one warp per row; every reduction is the warp's butterfly (fixed order), the loss then block_reduce's
+        float loss = 0.f;
+        for (int r = warp; r < rows; r += nw) {
+            const float* x = logits + (size_t)r * ldl;
+            const float* t = (MODE == 3) ? aux + (size_t)r * lda : nullptr;
+            float m = -FLT_MAX;
+            for (int c = lane; c < cols; c += 32) m = fmaxf(m, x[c]);
+            m = warp_max(m);
+            float s = 0.f, T = 0.f;
+            for (int c = lane; c < cols; c += 32) {
+                s += ce_exp(x[c], m);
+                if (MODE == 3) T += t[c];
+            }
+            s = warp_sum(s);
+            if (MODE == 3) T = warp_sum(T);
+            const float log_s = logf(s);
+            for (int c = lane; c < cols; c += 32) {
+                const float pc = ce_prob(ce_exp(x[c], m), s);
+                if (probs != nullptr) probs[(size_t)r * ldp + c] = pc;
+                if (MODE == 3) {
+                    loss += ce_loss_term(t[c], x[c], m, log_s);
+                    dlogits[(size_t)r * ldd + c] = ce_dlogit(pc, T, t[c], inv_batch);
+                }
+            }
+        }
+        if (MODE == 3 && loss_out != nullptr) {
+            const float total = block_reduce<false>(loss, scratch);
+            if (threadIdx.x == 0) loss_out[0] = total * inv_batch;
+        }
+        return;
+    }
 
     float mx = -FLT_MAX;
     for (int i = threadIdx.x; i < rows * cols; i += blockDim.x) mx = fmaxf(mx, logits[(size_t)(i / cols) * ldl + (i % cols)]);
@@ -97,13 +133,22 @@ __global__ void __launch_bounds__(256) loss_head_kernel(const float* __restrict_
 
 cudaError_t launch_loss_head(const float* logits, int ldl, const float* target, int ldt, float* probs, int ldp,
                              float* dlogits, int ldd, float* loss_out, int rows, int cols, float inv_batch,
-                             cudaStream_t stream, int rows_per_mubatch) {
+                             cudaStream_t stream, int rows_per_mubatch, int loss) {
+    if (loss != LOSS_MSE && loss != LOSS_CROSS_ENTROPY) return cudaErrorInvalidValue;
     const int rpb = rows_per_mubatch > 0 ? rows_per_mubatch : rows;
     const int blocks = (rows + rpb - 1) / rpb;
-    if (target != nullptr)
-        loss_head_kernel<1><<<blocks, 256, 0, stream>>>(logits, ldl, target, ldt, probs, ldp, dlogits, ldd, loss_out, rows, cols, inv_batch, rpb);
-    else
-        loss_head_kernel<0><<<blocks, 256, 0, stream>>>(logits, ldl, nullptr, 0, probs, ldp, nullptr, 0, nullptr, rows, cols, 0.f, rpb);
+    const bool ce = loss == LOSS_CROSS_ENTROPY;
+    if (target != nullptr) {
+        if (ce)
+            loss_head_kernel<3><<<blocks, 256, 0, stream>>>(logits, ldl, target, ldt, probs, ldp, dlogits, ldd, loss_out, rows, cols, inv_batch, rpb);
+        else
+            loss_head_kernel<1><<<blocks, 256, 0, stream>>>(logits, ldl, target, ldt, probs, ldp, dlogits, ldd, loss_out, rows, cols, inv_batch, rpb);
+    } else {
+        if (ce)
+            loss_head_kernel<4><<<blocks, 256, 0, stream>>>(logits, ldl, nullptr, 0, probs, ldp, nullptr, 0, nullptr, rows, cols, 0.f, rpb);
+        else
+            loss_head_kernel<0><<<blocks, 256, 0, stream>>>(logits, ldl, nullptr, 0, probs, ldp, nullptr, 0, nullptr, rows, cols, 0.f, rpb);
+    }
     return cudaGetLastError();
 }
 

@@ -10,6 +10,10 @@ namespace ssb {
 
 enum GemmMode : int { GEMM_FWD = 0, GEMM_DGRAD = 1, GEMM_WGRAD = 2 };
 
+// Loss of the last stage's head.  MSE: the reference's softmax (shift by the micro-batch's global max, +1e-7) followed by
+// the MSE loss.  CROSS_ENTROPY: softmax cross-entropy with probability targets, per-row softmax (ptx.cuh: ce_*).
+enum LossKind : int { LOSS_MSE = 0, LOSS_CROSS_ENTROPY = 1 };
+
 // Hyper-parameters of the SGD update beyond lr (torch.optim.SGD, dampening 0).  The default is plain SGD, w -= lr * g,
 // which runs the stateless kernels.  V: momentum buffer laid out like the weights it belongs to (nullptr when
 // momentum == 0: weight decay alone needs no state).
@@ -266,6 +270,9 @@ struct ChainParams {
     uint32_t* ready;                 // optional [n_layers + 1] device counters: every epilogue warp of every CTA adds 1 to
                                      // ready[l] once its part of dz[l] (and everything it wrote before) is globally visible
     unsigned long long* dbg;         // optional timeline buffer (3 roles x 256 globaltimer stamps), CTA 0 only
+    // LossKind of the loss head (selects the kernel instantiation; probs are the row softmax under CROSS_ENTROPY).  Last,
+    // so that the offsets of the other parameters are what they were before the field existed.
+    int loss_kind;
 };
 struct ChainPlan {
     ChainParams p;
@@ -291,9 +298,12 @@ cudaError_t chain_launch(const ChainPlan& plan, cudaStream_t stream);
 // ---- small fused kernels --------------------------------------------------------------
 // logits[rows, cols] (ld) -> probs (nullable) ; training: dlogits (softmax-Jacobian x MSE
 // grad, 1/batch_size inside) and loss_out[0] = sum((t-p)^2)/batch_size.
+// loss == LOSS_CROSS_ENTROPY: probs = row softmax; training: dlogits = (p * sum(t) - t)/batch_size and
+// loss_out[0] = sum(t * ((max - z) + log s))/batch_size (ptx.cuh: ce_*).  Other values: cudaErrorInvalidValue.
 cudaError_t launch_loss_head(const float* logits, int ldl, const float* target, int ldt, float* probs, int ldp,
                              float* dlogits, int ldd, float* loss_out, int rows, int cols, float inv_batch,
-                             cudaStream_t stream, int rows_per_mubatch = 0);   // >0: one CTA per micro-batch, loss_out[mu]
+                             cudaStream_t stream, int rows_per_mubatch = 0,    // >0: one CTA per micro-batch, loss_out[mu]
+                             int loss = LOSS_MSE);
 // generic softmax backward for the functional API: dz = p*up - p*sum(p*up)
 cudaError_t launch_softmax_grad(const float* logits, int ldl, const float* upstream, int ldu, float* dlogits, int ldd,
                                 int rows, int cols, cudaStream_t stream);

@@ -11,7 +11,7 @@
 //     flight while layer l is being computed;
 //   * accumulators live in the registers of the warp whose epilogue consumes them (mma.sync
 //     TF32, 3xTF32 for fp32-equivalent products); fused epilogues: bias + ReLU (forward),
-//     softmax + MSE gradient + softmax Jacobian (loss head), ReLU mask (backward).
+//     softmax + MSE gradient + softmax Jacobian, or softmax cross-entropy (loss head), ReLU mask (backward).
 //
 // This removes ~14 dependent kernel launches (and their prologues / cold starts) from the
 // critical path of the reference workload; the per-layer kernels in tc_gemm.cu remain the
@@ -70,7 +70,9 @@ __device__ __forceinline__ unsigned long long gtime() {
 // NTW: n8 tiles of a math warp's accumulator (chain_warp_cols / 8, rounded up to 2, 4 or 8) - sized at compile time
 // so that small micro-batches keep their accumulators in a few registers.
 // CLUSTER: the cluster form (see the top of the file); never combined with FOLD.
-template <bool SPLIT, bool FOLD, int NTW, bool CLUSTER>
+// CE: the loss head computes softmax cross-entropy (ChainParams::loss_kind); a compile-time switch, so the MSE
+// instantiations carry none of its code.
+template <bool SPLIT, bool FOLD, int NTW, bool CLUSTER, bool CE>
 __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParams p) {
     static_assert(!(FOLD && CLUSTER), "folded pipeline launches run one CTA per micro-batch");
     extern __shared__ uint8_t smem_raw[];
@@ -385,10 +387,11 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     if (l == 1) wbuf = 1;                    // layer 1 wrote abuf 0; layer 2 reads 0, writes 1
                 } else {
                     // ---------------- loss head on the logits tile (class = feature lane, row = column)
-                    // softmax contract of the reference: shift by the GLOBAL max of the micro-batch, +1e-7.
+                    // MSE: softmax contract of the reference: shift by the GLOBAL max of the micro-batch, +1e-7.
+                    // Cross-entropy: per-row softmax (ptx.cuh: ce_*), so no cross-lane max at all.
                     // Step 1: the class-lane warps (q == 0, both halves) transpose logits (+bias) into a [row][class]
                     // scratch in smem.  Step 2: each lane of warp (0, 0) owns ROWS, loops over the <= 32 classes in
-                    // registers - no cross-lane reductions except one max and one sum for the whole micro-batch.
+                    // registers - no cross-lane reductions except (MSE) one max and one sum for the whole micro-batch.
                     // CLUSTER: the <= 32 classes are rank 0's features; the scratch is where the k-phase partials were
                     // (all of them read before the barrier)
                     const int C = ly.out;
@@ -409,15 +412,70 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     }
                     asm volatile("bar.sync 2, 256;" ::: "memory");
                     if (q == 0 && half == 0 && rank == 0) {
+                        constexpr bool ce = CE;
                         float gmax = -3.0e38f;
-                        for (int n = lane; n < p.mb_rows; n += 32)
-                            for (int k = 0; k < C; ++k) gmax = fmaxf(gmax, scratch[n * kScratchLd + k]);
-                        gmax = warp_max_f(gmax);
+                        if (!ce) {
+                            for (int n = lane; n < p.mb_rows; n += 32)
+                                for (int k = 0; k < C; ++k) gmax = fmaxf(gmax, scratch[n * kScratchLd + k]);
+                            gmax = warp_max_f(gmax);
+                        }
                         for (int n = lane; n < N; n += 32) {
                             const bool row_ok = n < p.mb_rows;
                             const float* __restrict__ tg = p.target + (int64_t)(row0 + n) * p.ldt;
                             const float* __restrict__ zr = scratch + n * kScratchLd;
-                            if (C <= 16) {
+                            if (ce && C <= 16) {
+                                // cross-entropy fast path: the row max, sum(exp) and sum(t) in registers, constant bounds
+                                float tgv[16], ev[16];
+                                float mx = -3.0e38f;
+#pragma unroll
+                                for (int k = 0; k < 16; ++k) {
+                                    tgv[k] = (k < C && row_ok) ? __ldg(tg + k) : 0.f;
+                                    if (k < C) mx = fmaxf(mx, zr[k]);
+                                }
+                                float ssum = 0.f, tsum = 0.f;
+#pragma unroll
+                                for (int k = 0; k < 16; ++k) {
+                                    ev[k] = (k < C) ? ce_exp(zr[k], mx) : 0.f;
+                                    ssum += ev[k];
+                                    tsum += tgv[k];
+                                }
+                                const float log_s = logf(ssum);
+#pragma unroll
+                                for (int k = 0; k < 16; ++k) {
+                                    if (k < C) {
+                                        const float pr = ce_prob(ev[k], ssum);
+                                        const float dzv = row_ok ? ce_dlogit(pr, tsum, tgv[k], p.inv_batch) : 0.f;
+                                        if (row_ok) {
+                                            loss += ce_loss_term(tgv[k], zr[k], mx, log_s);
+                                            gout[(int64_t)n * p.act_ld[l] + k] = zr[k];
+                                            p.probs[(int64_t)(row0 + n) * p.ldp + k] = pr;
+                                            if (p.dz[l] != nullptr) p.dz[l][(int64_t)(row0 + n) * p.act_ld[l] + k] = dzv;
+                                        }
+                                        if (p.do_bwd) st_tile(dst, n, k, dzv);
+                                    }
+                                }
+                            } else if (ce) {
+                                float mx = -3.0e38f;
+                                for (int k = 0; k < C; ++k) mx = fmaxf(mx, zr[k]);
+                                float ssum = 0.f, tsum = 0.f;
+                                for (int k = 0; k < C; ++k) {
+                                    ssum += ce_exp(zr[k], mx);
+                                    tsum += row_ok ? __ldg(tg + k) : 0.f;
+                                }
+                                const float log_s = logf(ssum);
+                                for (int k = 0; k < C; ++k) {
+                                    const float pr = ce_prob(ce_exp(zr[k], mx), ssum);
+                                    const float t = row_ok ? __ldg(tg + k) : 0.f;
+                                    const float dzv = row_ok ? ce_dlogit(pr, tsum, t, p.inv_batch) : 0.f;
+                                    if (row_ok) {
+                                        loss += ce_loss_term(t, zr[k], mx, log_s);
+                                        gout[(int64_t)n * p.act_ld[l] + k] = zr[k];
+                                        p.probs[(int64_t)(row0 + n) * p.ldp + k] = pr;
+                                        if (p.dz[l] != nullptr) p.dz[l][(int64_t)(row0 + n) * p.act_ld[l] + k] = dzv;
+                                    }
+                                    if (p.do_bwd) st_tile(dst, n, k, dzv);
+                                }
+                            } else if (C <= 16) {
                                 // fast path (the usual 10-class head): everything in registers, loops fully
                                 // unrolled to a constant bound so the 16 target loads / exps are independent
                                 float tgv[16], ev[16];
@@ -731,27 +789,30 @@ void chain_plan_free(ChainPlan* plan) {
     plan->maps_dev = nullptr;
 }
 
-template <int NTW>
+template <int NTW, bool CE>
 static cudaError_t chain_configure_ntw() {
     cudaError_t e;
     const int smem = 227 * 1024;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, true, NTW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, true, NTW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    return cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, false, CE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, true, NTW, false, CE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, false, CE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, true, NTW, false, CE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, true, CE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    return cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, true, CE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
 }
 
 cudaError_t chain_configure() {
     cudaError_t e;
-    if ((e = chain_configure_ntw<2>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<4>()) != cudaSuccess) return e;
-    return chain_configure_ntw<8>();
+    if ((e = chain_configure_ntw<2, false>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<4, false>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<8, false>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<2, true>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<4, true>()) != cudaSuccess) return e;
+    return chain_configure_ntw<8, true>();
 }
 
 // grid = micro-batches x plan.cluster, cluster dims (plan.cluster, 1, 1)
-template <bool SPLIT, int NTW>
+template <bool SPLIT, int NTW, bool CE>
 static cudaError_t chain_launch_cluster(const ChainPlan& plan, cudaStream_t stream) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)plan.grid);
@@ -765,14 +826,15 @@ static cudaError_t chain_launch_cluster(const ChainPlan& plan, cudaStream_t stre
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, mlp_chain_kernel<SPLIT, false, NTW, true>, plan.p);
+    return cudaLaunchKernelEx(&cfg, mlp_chain_kernel<SPLIT, false, NTW, true, CE>, plan.p);
 }
 
-template <int NTW>
+template <int NTW, bool CE>
 static cudaError_t chain_launch_ntw(const ChainPlan& plan, bool fold, cudaStream_t stream) {
     const ChainParams& p = plan.p;
-    if (plan.cluster > 1) return p.split ? chain_launch_cluster<true, NTW>(plan, stream) : chain_launch_cluster<false, NTW>(plan, stream);
-#define SSB_CHAIN_LAUNCH(S, F) mlp_chain_kernel<S, F, NTW, false><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(p)
+    if (plan.cluster > 1)
+        return p.split ? chain_launch_cluster<true, NTW, CE>(plan, stream) : chain_launch_cluster<false, NTW, CE>(plan, stream);
+#define SSB_CHAIN_LAUNCH(S, F) mlp_chain_kernel<S, F, NTW, false, CE><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(p)
     if (!p.split) {
         if (fold) SSB_CHAIN_LAUNCH(false, true); else SSB_CHAIN_LAUNCH(false, false);
     } else {
@@ -786,10 +848,12 @@ cudaError_t chain_launch(const ChainPlan& plan, cudaStream_t stream) {
     const ChainParams& p = plan.p;
     const bool fold = p.in_flag != nullptr || p.out_peer != nullptr || p.x_from_global != 0;
     const int ntw = chain_ntw(p.n_pad);
+    if (p.loss_kind != LOSS_MSE && p.loss_kind != LOSS_CROSS_ENTROPY) return cudaErrorInvalidValue;
+    const bool ce = p.loss_kind == LOSS_CROSS_ENTROPY;
     cudaError_t e;
-    if (ntw == 2) e = chain_launch_ntw<2>(plan, fold, stream);
-    else if (ntw == 4) e = chain_launch_ntw<4>(plan, fold, stream);
-    else e = chain_launch_ntw<8>(plan, fold, stream);
+    if (ntw == 2) e = ce ? chain_launch_ntw<2, true>(plan, fold, stream) : chain_launch_ntw<2, false>(plan, fold, stream);
+    else if (ntw == 4) e = ce ? chain_launch_ntw<4, true>(plan, fold, stream) : chain_launch_ntw<4, false>(plan, fold, stream);
+    else e = ce ? chain_launch_ntw<8, true>(plan, fold, stream) : chain_launch_ntw<8, false>(plan, fold, stream);
     if (e != cudaSuccess) return e;
     return cudaGetLastError();
 }

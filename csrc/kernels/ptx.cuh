@@ -329,4 +329,24 @@ __device__ __forceinline__ float sgd_direction(float g, float w, float& v, float
     }
 }
 
+// ------------------------------------------------------------------ softmax cross-entropy, per element of one row
+// torch's F.cross_entropy(z, t, reduction="sum") / B with probability targets, for one row of logits z and target t:
+//     m = max_k z_k ;  s = sum_k exp(z_k - m) ;  p_k = exp(z_k - m) / s ;  T = sum_k t_k
+//     loss = sum_k t_k ((m - z_k) + log s) / B ;   dz_k = (p_k T - t_k) / B
+// The shift is the ROW's max, so s >= 1 and log s is exact to an ulp for every row, however far its logits lie below
+// the other rows' (the MSE head's reference contract shifts by the micro-batch's max and adds 1e-7).  The gradient is
+// the fused form: no division by p, which underflows for confidently wrong rows.  The chain kernel's loss head and
+// loss_head_kernel both call these, and the explicitly rounded operations keep the compiler from contracting them
+// differently in the two, so each element is formed alike from s, T and log s.  The sums themselves (s, T and the loss)
+// run in different orders: the chain head adds a row's classes in order in one lane, loss_head_kernel adds them per lane
+// and then across the warp.  The two paths' results can therefore differ in the last bits.
+__device__ __forceinline__ float ce_exp(float z, float m) { return expf(__fsub_rn(z, m)); }
+__device__ __forceinline__ float ce_prob(float e, float s) { return __fdiv_rn(e, s); }
+__device__ __forceinline__ float ce_loss_term(float t, float z, float m, float log_s) {
+    return __fmul_rn(t, __fadd_rn(__fsub_rn(m, z), log_s));
+}
+__device__ __forceinline__ float ce_dlogit(float p, float T, float t, float inv_batch) {
+    return __fmul_rn(__fmaf_rn(p, T, -t), inv_batch);
+}
+
 }  // namespace ssb

@@ -173,6 +173,9 @@ public:
         c.momentum = cfg.contains("momentum") ? cfg["momentum"].cast<float>() : 0.f;
         c.weight_decay = cfg.contains("weight_decay") ? cfg["weight_decay"].cast<float>() : 0.f;
         c.nesterov = geti("nesterov", 0);
+        c.loss = geti("loss", ssb::LOSS_MSE);
+        TORCH_CHECK(c.loss == ssb::LOSS_MSE || c.loss == ssb::LOSS_CROSS_ENTROPY,
+                    "PipeEngine: cfg['loss'] must be 0 (MSE) or 1 (cross-entropy), got ", c.loss);
         c10::cuda::CUDAGuard guard(weights.device());
         engine_ = std::make_unique<PipeEngine>(c, weights.data_ptr<float>(), grads.data_ptr<float>(), weights.numel(),
                                                momentum.has_value() ? momentum->data_ptr<float>() : nullptr);

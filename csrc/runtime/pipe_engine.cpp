@@ -220,6 +220,7 @@ int PipeEngine::add_chain(int stream, int mu_base, int n_mu, bool do_fwd, bool d
     cp.target = y_stage_; cp.ldt = y_ld_;
     cp.probs = probs_all_; cp.ldp = act_ld_[L_];
     cp.loss = loss_target();
+    cp.loss_kind = cfg_.loss;
     cp.mb_rows = cfg_.mb_rows; cp.mu_base = mu_base;
     cp.inv_batch = 1.0f / (float)cfg_.global_batch;
     cp.do_fwd = do_fwd; cp.do_loss = do_loss; cp.do_bwd = do_bwd; cp.first_stage = cfg_.is_first;
@@ -1010,11 +1011,11 @@ void PipeEngine::exec(const Op& op) {
         case OP_WGRAD_GROUP: CUDA_CHECK(gemm_group_launch(group_plans_[op.gemm], st)); break;
         case OP_LOSS_HEAD:
             CUDA_CHECK(launch_loss_head(op.a, op.lda, op.b, op.ldb, op.c, op.ldc, op.d, op.ldd, (op.f ? op.f : loss_dev_) + op.mu, op.rows,
-                                        op.cols, op.scalar, st, (int)op.n));
+                                        op.cols, op.scalar, st, (int)op.n, cfg_.loss));
             break;
         case OP_SOFTMAX:
             CUDA_CHECK(launch_loss_head(op.a, op.lda, nullptr, 0, op.b, op.ldb, nullptr, 0, nullptr, op.rows, op.cols, 0.f, st,
-                                        (int)op.n));
+                                        (int)op.n, cfg_.loss));
             break;
         case OP_ARGMAX:
             CUDA_CHECK(launch_argmax_correct(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, correct_dev_, st));
@@ -1297,6 +1298,7 @@ std::string PipeEngine::describe() const {
         if (cfg_.weight_decay != 0.f) os << ", weight_decay=" << cfg_.weight_decay;
         os << ")";
     }
+    if (cfg_.loss == LOSS_CROSS_ENTROPY) os << ", loss=cross_entropy";
     os << ")";
     return os.str();
 }

@@ -90,6 +90,7 @@ struct EngineConfig {
     // replica updates only the entries it owns (layer_protocols()).
     float momentum = 0.f, weight_decay = 0.f;
     int nesterov = 0;
+    int loss = LOSS_MSE;    // LossKind of the last stage's head (the chain kernel's and loss_head_kernel's)
 };
 
 class PipeEngine {

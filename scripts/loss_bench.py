@@ -1,0 +1,87 @@
+#!/usr/bin/env python
+"""Cost of the cross-entropy head: step time of an MSE Trainer vs a cross-entropy Trainer, alternated block by block in
+one process so that both see the same card, clocks and neighbours.
+
+    python scripts/loss_bench.py [--steps 200] [--repeats 7] [--warmup 50]
+
+Two workloads on one GPU: the reference model (784-128-127-126-125-124-123-10, global batch 128, 4 micro-batches), whose
+loss head is fused into the layer-chain kernel, and a 33-class model (784-128-127-126-125-124-123-33), which the chain
+refuses (more than 32 classes), so its head is the stand-alone loss_head_kernel after the layer-wise GEMMs.  Every block
+of ``--steps`` steps is timed with CUDA events on the engine's stream between two device synchronisations; each line
+reports the median block and the spread (min..max) over ``--repeats`` blocks.  The first line names the card and its
+power limit.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from scripts.optimizer_bench import card  # noqa: E402
+
+WORKLOADS = {"reference": [784, 128, 127, 126, 125, 124, 123, 10], "c33": [784, 128, 127, 126, 125, 124, 123, 33]}
+ARMS = ("mse", "cross_entropy")
+
+
+def main():
+    p = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    p.add_argument("--steps", type=int, default=200, help="steps per timed block")
+    p.add_argument("--repeats", type=int, default=7, help="timed blocks per arm (alternated)")
+    p.add_argument("--warmup", type=int, default=50, help="untimed steps per arm before the first block")
+    p.add_argument("--workloads", nargs="+", default=list(WORKLOADS), choices=list(WORKLOADS))
+    args = p.parse_args()
+
+    import torch
+
+    from shallowspeed_b200.parallel.engine import Trainer
+
+    if not torch.cuda.is_available():
+        raise SystemExit("loss_bench: no CUDA device")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    name, limits = card()
+    print(json.dumps({"card": name, "power_limit,max_sm_clock": limits}), flush=True)
+
+    for wl in args.workloads:
+        sizes = WORKLOADS[wl]
+        trainers = {arm: Trainer(sizes, global_batch_size=128, n_mubatches=4, lr=0.006, device=dev, loss=arm)
+                    for arm in ARMS}
+        pool = 16
+        gen = torch.Generator().manual_seed(0)
+        xs = torch.rand(pool, 128, sizes[0], generator=gen).to(dev)
+        ys = torch.nn.functional.one_hot(torch.randint(0, sizes[-1], (pool, 128), generator=gen), sizes[-1]).float().to(dev)
+
+        def block(tr, n):
+            torch.cuda.synchronize(dev)
+            st = torch.cuda.ExternalStream(tr.engine.main_stream(), device=dev)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(st)
+            for i in range(n):
+                tr.step_async(xs[i % pool], ys[i % pool])
+            e1.record(st)
+            torch.cuda.synchronize(dev)
+            return e0.elapsed_time(e1) / n
+
+        for tr in trainers.values():
+            block(tr, args.warmup)
+        times = {arm: [] for arm in trainers}
+        for _ in range(args.repeats):
+            for arm, tr in trainers.items():
+                times[arm].append(block(tr, args.steps))
+        for arm, ts in times.items():
+            s = sorted(ts)
+            eng = trainers[arm].engine
+            print(json.dumps({"workload": wl, "sizes": "-".join(map(str, sizes)), "loss": arm,
+                              "ms_per_step": round(s[len(s) // 2], 5), "min": round(s[0], 5), "max": round(s[-1], 5),
+                              "blocks": len(s), "steps": args.steps, "chain": bool(eng.uses_chain()),
+                              "kernels_per_step": int(eng.kernels_per_step()),
+                              "final_loss": round(float(trainers[arm].loss()), 6)}), flush=True)
+        del trainers
+        torch.cuda.empty_cache()
+
+
+if __name__ == "__main__":
+    main()

@@ -1,4 +1,4 @@
-"""Model layer: Parameter / Module / Linear / ReLU / Softmax / MSELoss / Sequential.
+"""Model layer: Parameter / Module / Linear / ReLU / Softmax / MSELoss / CrossEntropyLoss / Sequential.
 
 Capability parity with the reference's ``shallowspeed/layers.py:17-233``: explicit
 ``forward(inputs, mubatch_id)`` / ``backward(dout, mubatch_id)`` with a per-micro-batch
@@ -311,6 +311,32 @@ class MSELoss(Module):
 
     def __repr__(self):
         return "MSELoss()"
+
+
+class CrossEntropyLoss(Module):
+    """Softmax cross-entropy on logits: torch's ``F.cross_entropy(z, t, reduction="sum") / batch_size`` with
+    probability targets.  ``forward`` caches the logits and returns the per-row softmax, so the last stage's output is
+    still the class probabilities (argmax / accuracy are unchanged).  ``backward(target)`` records ``last_loss`` of the
+    micro-batch and returns dL/dz = (p * sum(t) - t) / batch_size, fused (ops.functional.loss_head_backward)."""
+
+    def __init__(self, batch_size: int):
+        super().__init__()
+        self.batch_size = batch_size
+        self.last_loss = None
+
+    def forward(self, input, mubatch_id=0):
+        if self._training:
+            self._cache[f"input_{mubatch_id}"] = input
+        return F.row_softmax(input)
+
+    def backward(self, target, mubatch_id=0):
+        assert self._training
+        z = self._cache.pop(f"input_{mubatch_id}")
+        dz, _, self.last_loss = F.loss_head_backward(z, target, self.batch_size, loss="cross_entropy")
+        return dz
+
+    def __repr__(self):
+        return "CrossEntropyLoss()"
 
 
 class Sequential(Module):

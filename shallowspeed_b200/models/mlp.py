@@ -3,16 +3,17 @@
 Parity with the reference's ``MLP(sizes, stage_idx, n_stages, batch_size)``
 (``shallowspeed/layers.py:236-270``): ``len(sizes) % n_stages == 0``; stage *s* owns
 ``sizes[s*k : s*k+k+1]`` (k = len(sizes)//n_stages), i.e. k Linears, the last stage
-k-1 Linears + Softmax + MSELoss; the final Linear carries no ReLU only when it sits on
+k-1 Linears + Softmax + MSELoss (or, with ``loss="cross_entropy"``, + CrossEntropyLoss); the final Linear carries no ReLU only when it sits on
 the last stage; ``in_dim`` / ``out_dim`` are exposed for buffer allocation.
 
 All Linears of a stage share one ``ParamArena`` (flat weights + flat grads).
 """
 from __future__ import annotations
 
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Union
 
-from .layers import Linear, MSELoss, ParamArena, Sequential, Softmax
+from ..ops.functional import check_loss
+from .layers import CrossEntropyLoss, Linear, MSELoss, ParamArena, Sequential, Softmax
 
 DEFAULT_LAYER_SIZES = [784, 128, 127, 126, 125, 124, 123, 10]  # reference train.py:98
 
@@ -47,15 +48,18 @@ def mlp_sizes(hidden: int, n_layers: int, in_dim: int = 784, out_dim: int = 10):
 
 class MLP(Sequential):
     def __init__(self, sizes: Sequence[int], stage_idx: int, n_stages: int, batch_size: int,
-                 device="cpu", seed_mode: str = "shape", verbose: bool = False):
+                 device="cpu", seed_mode: str = "shape", verbose: bool = False, loss: str = "mse"):
         """
         :param batch_size: the GLOBAL batch size - the loss gradient is scaled by
             1/batch_size so that summing over micro-batches and DP replicas reproduces
             sequential training (reference layers.py:237-241).
         :param seed_mode: "shape" = reference-identical shape-seeded init;
             "index" = additionally mixes the global layer index into the seed.
+        :param loss: "mse" = the reference's Softmax + MSELoss head; "cross_entropy" =
+            CrossEntropyLoss on the logits.  Every stage records it (the native engine reads it).
         """
         assert seed_mode in ("shape", "index")
+        self.loss = check_loss(loss)
         self.sizes = list(sizes)
         self.stage_idx, self.n_stages, self.batch_size = stage_idx, n_stages, batch_size
         specs = stage_layer_specs(sizes, stage_idx, n_stages)
@@ -68,7 +72,9 @@ class MLP(Sequential):
             for bi, (i, o, relu, gidx) in enumerate(specs)
         ]
         self.linears = list(layers)
-        if self.is_last_stage:
+        if self.is_last_stage and self.loss == "cross_entropy":
+            layers.append(CrossEntropyLoss(batch_size=batch_size))
+        elif self.is_last_stage:
             layers.append(Softmax())
             layers.append(MSELoss(batch_size=batch_size))
         super().__init__(layers)
@@ -82,5 +88,5 @@ class MLP(Sequential):
         return self
 
     @property
-    def loss_layer(self) -> Optional[MSELoss]:
+    def loss_layer(self) -> Optional[Union[MSELoss, CrossEntropyLoss]]:
         return self.layers[-1] if self.is_last_stage else None

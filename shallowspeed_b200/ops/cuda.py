@@ -116,10 +116,18 @@ def linear_bwd_accumulate(dout, x, w_block, g_block, in_dims):
 
 
 # ------------------------------------------------------------------ loss head / softmax
-def softmax(logits):
+def _loss_code(loss):
+    from .functional import LOSS_CODES, check_loss
+
+    return LOSS_CODES[check_loss(loss)]
+
+
+def softmax(logits, loss="mse"):
+    """The probabilities of a model with this loss: the reference's global-max softmax (``"mse"``) or the per-row
+    softmax (``"cross_entropy"``)."""
     logits = as_tma(logits)
     p = empty_padded(logits.size(0), logits.size(1), logits.device)
-    _C.loss_head(logits, None, p, None, None, 0.0)
+    _C.loss_head(logits, None, p, None, None, 0.0, _loss_code(loss))
     return p
 
 
@@ -130,13 +138,15 @@ def softmax_grad(grad_output, logits):
     return dz
 
 
-def loss_head_backward(logits, target, batch_size):
+def loss_head_backward(logits, target, batch_size, loss="mse"):
+    """(dlogits, probs, loss) of the whole ``logits`` as one micro-batch, for an MSE or a cross-entropy head."""
+    code = _loss_code(loss)
     logits, target = as_tma(logits), as_tma(target)
     r, c = logits.shape
     p, dz = empty_padded(r, c, logits.device), empty_padded(r, c, logits.device)
-    loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
-    _C.loss_head(logits, target, p, dz, loss, 1.0 / batch_size)
-    return dz, p, loss[0]
+    out = torch.zeros(1, dtype=torch.float32, device=logits.device)
+    _C.loss_head(logits, target, p, dz, out, 1.0 / batch_size, code)
+    return dz, p, out[0]
 
 
 def mse_loss_grad(input, target, batch_size):

@@ -16,12 +16,25 @@ Numerical contracts kept from the reference (SURVEY.md section 2.2(4)):
 softmax shifts by the *global* max of the whole micro-batch and adds 1e-7 to
 the denominator (functional.py:24-27); the 1/global_batch_size factor lives in
 the loss gradient so gradients are *summed* over micro-batches and replicas.
+
+Softmax cross-entropy (``loss="cross_entropy"``, beyond the reference) follows
+torch's ``F.cross_entropy(z, t, reduction="sum") / batch_size`` with probability
+targets instead: the softmax is per row (no global max, no +1e-7) and its gradient
+is the fused ``(p * sum(t) - t) / batch_size``.
 """
 from __future__ import annotations
 
 import torch
 
 SOFTMAX_EPS = 1e-7
+# the losses a model's head can compute, and their codes in the native runtime (csrc/kernels/kernels.h: LossKind)
+LOSS_CODES = {"mse": 0, "cross_entropy": 1}
+
+
+def check_loss(loss: str) -> str:
+    if loss not in LOSS_CODES:
+        raise ValueError(f"unknown loss {loss!r}: expected one of {sorted(LOSS_CODES)}")
+    return loss
 
 
 def _use_cuda(*tensors) -> bool:
@@ -68,6 +81,25 @@ def mse_loss_ref(input, target, batch_size: int):
 
 def mse_loss_grad_ref(input, target, batch_size: int):
     return -2 * (target - input) / batch_size
+
+
+def row_softmax_ref(input):
+    """softmax of every row on its own: torch.softmax(input, -1)."""
+    e = torch.exp(input - input.max(dim=1, keepdim=True).values)
+    return e / e.sum(dim=1, keepdim=True)
+
+
+def cross_entropy_ref(logits, target, batch_size: int):
+    """sum over rows and classes of t * (log-sum-exp(z) - z), divided by the global batch size."""
+    m = logits.max(dim=1, keepdim=True).values
+    log_s = torch.log(torch.exp(logits - m).sum(dim=1, keepdim=True))
+    return (target * ((m - logits) + log_s)).sum() / batch_size
+
+
+def cross_entropy_grad_ref(logits, target, batch_size: int):
+    """d cross_entropy / d logits = (softmax(z) * sum(t) - t) / batch_size, per row."""
+    p = row_softmax_ref(logits)
+    return (p * target.sum(dim=1, keepdim=True) - target) / batch_size
 
 
 # ----------------------------------------------------------------------------
@@ -136,15 +168,45 @@ def mse_loss_grad(input, target, batch_size: int):
     return mse_loss_grad_ref(input, target, batch_size)
 
 
-def loss_head_backward(logits, target, batch_size: int):
-    """Fused loss head: logits -> softmax -> MSE grad -> softmax Jacobian
-    product.  Returns (dlogits, probs, loss_sum).  Equivalent to the reference
-    chain MSELoss.backward -> Softmax.backward (layers.py:157-163, 89-93) in a
-    single pass (SURVEY.md K5)."""
+def row_softmax(input):
+    """Per-row softmax (the probabilities of a cross-entropy model)."""
+    if _use_cuda(input):
+        from . import cuda as K
+
+        return K.softmax(input, loss="cross_entropy")
+    return row_softmax_ref(input)
+
+
+def cross_entropy(logits, target, batch_size: int):
     if _use_cuda(logits, target):
         from . import cuda as K
 
-        return K.loss_head_backward(logits, target, batch_size)
+        return K.loss_head_backward(logits, target, batch_size, loss="cross_entropy")[2]
+    return cross_entropy_ref(logits, target, batch_size)
+
+
+def cross_entropy_grad(logits, target, batch_size: int):
+    if _use_cuda(logits, target):
+        from . import cuda as K
+
+        return K.loss_head_backward(logits, target, batch_size, loss="cross_entropy")[0]
+    return cross_entropy_grad_ref(logits, target, batch_size)
+
+
+def loss_head_backward(logits, target, batch_size: int, loss: str = "mse"):
+    """Fused loss head: logits -> softmax -> MSE grad -> softmax Jacobian
+    product.  Returns (dlogits, probs, loss_sum).  Equivalent to the reference
+    chain MSELoss.backward -> Softmax.backward (layers.py:157-163, 89-93) in a
+    single pass (SURVEY.md K5).  ``loss="cross_entropy"``: the row softmax and the
+    cross-entropy gradient (p * sum(t) - t) / batch_size instead."""
+    check_loss(loss)
+    if _use_cuda(logits, target):
+        from . import cuda as K
+
+        return K.loss_head_backward(logits, target, batch_size, loss=loss)
+    if loss == "cross_entropy":
+        return (cross_entropy_grad_ref(logits, target, batch_size), row_softmax_ref(logits),
+                cross_entropy_ref(logits, target, batch_size))
     p = softmax_ref(logits)
     dp = mse_loss_grad_ref(p, target, batch_size)
     g = p * dp

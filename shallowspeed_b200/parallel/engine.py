@@ -13,6 +13,7 @@ from typing import Optional
 
 import torch
 
+from ..ops.functional import LOSS_CODES
 from .comm import Comm, ProcessGrid, SelfComm, TorchComm
 from .instructions import encode, flatten
 from .schedules import Schedule
@@ -287,6 +288,8 @@ class NativeWorker:
         if training and (self.momentum != 0.0 or self.weight_decay != 0.0):
             cfg.update(momentum=self.momentum, weight_decay=self.weight_decay, nesterov=int(self.nesterov))
             momentum = m.arena.momentum if self.momentum > 0.0 else None
+        if m.loss != "mse":   # the head's loss kind (training and inference: the probabilities depend on it)
+            cfg.update(loss=LOSS_CODES[m.loss])
         eng = _C().PipeEngine(specs, cfg, m.arena.weights, m.arena.grads, momentum)
         if self._pp_nccl is not None:
             eng.set_pp_comm(self._pp_nccl)
@@ -454,7 +457,7 @@ class Trainer:
     def __init__(self, layer_sizes, global_batch_size=128, n_mubatches=4, lr=0.006, schedule="naive",
                  dp_comm=None, pp_comm=None, grid: Optional[ProcessGrid] = None, comm_mode="fused",
                  use_graph=True, device=None, seed_mode="shape", precision="fp32", watchdog_s=None, pp_transport=None,
-                 local_batch_size=None, momentum=0.0, weight_decay=0.0, nesterov=False):
+                 local_batch_size=None, momentum=0.0, weight_decay=0.0, nesterov=False, loss="mse"):
         from ..models.mlp import MLP
         from ..optimizer import SGD
         from .schedules import SCHEDULE_NAME_TO_CLS
@@ -468,7 +471,8 @@ class Trainer:
         # communication-free engine do one replica's share of a bigger job (bench.py's exposed-comm twin): the loss
         # scale stays 1 / global_batch_size.
         self.local_batch_size = int(local_batch_size) if local_batch_size else global_batch_size // dp
-        self.model = MLP(layer_sizes, self.pp_comm.Get_rank(), pp, global_batch_size, seed_mode=seed_mode).to(self.device)
+        self.model = MLP(layer_sizes, self.pp_comm.Get_rank(), pp, global_batch_size, seed_mode=seed_mode,
+                         loss=loss).to(self.device)
         self.optimizer = SGD(self.model.parameters(), lr, momentum=momentum, weight_decay=weight_decay, nesterov=nesterov,
                              arena=self.model.arena)
 

@@ -10,8 +10,8 @@ from pathlib import Path
 
 import torch
 
-# update-rule settings a checkpoint without them was written under (plain SGD)
-_HPARAM_DEFAULTS = {"momentum": 0.0, "weight_decay": 0.0, "nesterov": False}
+# settings a checkpoint without them was written under (plain SGD, the MSE loss)
+_HPARAM_DEFAULTS = {"momentum": 0.0, "weight_decay": 0.0, "nesterov": False, "loss": "mse"}
 
 
 def _path(directory, stage, n_stages):

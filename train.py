@@ -78,6 +78,8 @@ def build_parser():
     p.add_argument("--momentum", type=float, default=0.0, help="SGD momentum (torch.optim.SGD semantics, dampening 0)")
     p.add_argument("--weight-decay", type=float, default=0.0, help="L2 penalty added to the gradient (biases included)")
     p.add_argument("--nesterov", action="store_true", help="Nesterov momentum (needs --momentum > 0)")
+    p.add_argument("--loss", choices=["mse", "cross-entropy"], default="mse",
+                   help="mse: the reference's softmax + MSE; cross-entropy: softmax cross-entropy on the logits")
     p.add_argument("--layer-sizes", type=int, nargs="+", default=None, help="explicit layer widths (default: reference MLP)")
     p.add_argument("--hidden", type=int, default=None, help="with --n-layers: 784 -> hidden x (n-1) -> 10")
     p.add_argument("--n-layers", type=int, default=None)
@@ -160,14 +162,15 @@ def main(args):
     logger = StepLogger(args.log_json, rank=grid.rank)
     is_last = pp_comm.Get_rank() == args.pp - 1
 
+    loss = args.loss.replace("-", "_")
     model = MLP(layer_sizes, stage_idx=pp_comm.Get_rank(), n_stages=args.pp,
                 batch_size=args.global_batch_size, seed_mode=args.seed_mode,
-                verbose=(grid.rank == 0 or is_last))
+                verbose=(grid.rank == 0 or is_last), loss=loss)
     model.to(device)
     model.train()
     hparams = {"lr": float(args.lr), "global_batch_size": int(args.global_batch_size), "seed_mode": str(args.seed_mode),
                "n_mubatches": int(args.n_mubatches), "momentum": float(args.momentum),
-               "weight_decay": float(args.weight_decay), "nesterov": bool(args.nesterov)}
+               "weight_decay": float(args.weight_decay), "nesterov": bool(args.nesterov), "loss": loss}
     # before the resume: the momentum arena it restores is allocated here
     optimizer = SGD(model.parameters(), lr=args.lr, momentum=args.momentum, weight_decay=args.weight_decay,
                     nesterov=args.nesterov, arena=model.arena)

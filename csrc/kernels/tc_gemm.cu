@@ -493,6 +493,9 @@ const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const flo
     p.W = W; p.ldw = ldw; p.lr = lr; p.fuse_sgd = fuse_sgd;
     if (fuse_sgd && W == nullptr) return "fuse_sgd needs W";
     if (fuse_sgd && accumulate) return "fuse_sgd cannot be combined with accumulate (reduce into G, then run the SGD pass)";
+    // the fused update finds the bias at db's offset from G, taken in W (and V): only the arena layout's bias column
+    // (column `in` of G's block) names a slot of W
+    if (fuse_sgd && db != nullptr && db != G + in) return "fuse_sgd needs db to be G's bias column (G + in)";
     if (!opt.plain()) {
         if (!fuse_sgd) return "momentum / weight decay need fuse_sgd (the update rule runs in the epilogue)";
         if (const char* e = sgd_state_check(opt)) return e;

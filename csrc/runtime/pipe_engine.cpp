@@ -148,9 +148,11 @@ void PipeEngine::select_set(int set) {
     for (int mu = 0; mu < cfg_.n_mu; ++mu) act_[mu][0] = act_all_[0] + (size_t)mu * cfg_.mb_rows * act_ld_[0];
 }
 
-// Opt-in (SSB_SPLITK=1: automatic, SSB_SPLITK=k: force k where legal): give FWD / DGRAD GEMMs of wide layers
-// enough CTAs to saturate HBM (8192 outputs = only 64 tiles on 132 SMs).  Not yet the default: the kernel
-// variant still has to be validated on hardware.
+// SSB_SPLITK=1 (the default, tuning.json): automatic; SSB_SPLITK=k: force k where legal; SSB_SPLITK=0: off.  Gives
+// FWD / DGRAD GEMMs of wide layers enough CTAs to saturate HBM (8192 outputs = only 64 tiles on 132 SMs).  Each plan
+// owns its workspace and tile counters; the last CTA of a tile re-arms its counter, so every replay of the graph
+// reuses them.  tests/test_gpu_gemm.py checks the variant per element against an fp64 oracle, stand-alone and in the
+// engine over two steps.
 void PipeEngine::maybe_splitk(GemmPlan& g) {
     const char* env = getenv("SSB_SPLITK");
     if (!env || atoi(env) <= 0 || g.mode == GEMM_WGRAD) return;

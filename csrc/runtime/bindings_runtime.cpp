@@ -90,6 +90,48 @@ public:
         return torch::from_blob(ctx_->weights(), {ctx_->arena_numel()}, [](void*) {}, opts);
     }
     int64_t stage_bytes() { return ctx_->stage_bytes(); }
+    // test-facing: peers that live in this process (index = DP rank, own entry ignored; None allowed there)
+    void open_local_peers(const std::vector<std::shared_ptr<PyDpContext>>& ctxs) {
+        std::vector<const DpContext*> raw;
+        for (const auto& c : ctxs) raw.push_back(c ? c->ctx_.get() : nullptr);
+        ctx_->open_local_peers(raw);
+    }
+    // test-facing: {name: (device pointer, bytes)} of every buffer a peer reads or writes (llA / llC: (0, 0) without
+    // LL landing zones)
+    py::dict buffers() {
+        const DpContext& c = *ctx_;
+        py::dict d;
+        auto put = [&](const char* name, const void* p, int64_t bytes) {
+            d[name] = py::make_tuple((int64_t) reinterpret_cast<uintptr_t>(p), bytes);
+        };
+        put("W", c.weights(), c.arena_numel() * 4);
+        put("stage", c.stage(), c.stage_bytes());
+        put("arrive", c.arrive(), c.arrive_bytes());
+        put("done", c.done(), c.done_bytes());
+        put("epoch", c.epoch_ptr(), 64);
+        put("llA", c.ll_a(), c.ll_zone_bytes());
+        put("llC", c.ll_c(), c.ll_zone_bytes());
+        return d;
+    }
+    // test-facing: per layer, the geometry that addresses its staging slots and flags
+    py::list layer_geometry() {
+        const DpContext& c = *ctx_;
+        py::list out;
+        for (const DpLayerGeom& g : c.geometry()) {
+            py::dict d;
+            d["in"] = g.in; d["out"] = g.out; d["ld"] = g.ld; d["w_offset"] = g.w_offset;
+            d["block_n"] = g.block_n; d["n_tiles_m"] = g.n_tiles_m; d["n_tiles_n"] = g.n_tiles_n;
+            d["slots"] = g.slots; d["slot_floats"] = g.slot_floats; d["stage_offset"] = g.stage_offset;
+            d["tile_flag_base"] = g.tile_flag_base; d["slot_flag_base"] = g.slot_flag_base; d["one_shot"] = g.one_shot;
+            d["slots_per_src"] = c.slots_per_src(); d["stage_src_stride"] = c.stage_src_stride();
+            d["stage_parity_stride"] = c.stage_parity_stride();
+            out.append(d);
+        }
+        return out;
+    }
+    int dp() { return ctx_->dp(); }
+    int rank() { return ctx_->rank(); }
+    int ll_tiles() { return ctx_->ll_tiles(); }
     DpContext* get() { return ctx_.get(); }
 
 private:
@@ -273,7 +315,13 @@ void bind_runtime(py::module_& m) {
         .def("export_handles", &PyDpContext::export_handles)
         .def("open_peers", &PyDpContext::open_peers)
         .def("weights", &PyDpContext::weights)
-        .def("stage_bytes", &PyDpContext::stage_bytes);
+        .def("stage_bytes", &PyDpContext::stage_bytes)
+        .def("open_local_peers", &PyDpContext::open_local_peers)
+        .def("buffers", &PyDpContext::buffers)
+        .def("layer_geometry", &PyDpContext::layer_geometry)
+        .def("dp", &PyDpContext::dp)
+        .def("rank", &PyDpContext::rank)
+        .def("ll_tiles", &PyDpContext::ll_tiles);
     py::class_<PyNvlsContext, std::shared_ptr<PyNvlsContext>>(m, "NvlsContext")
         .def(py::init<int, int, int64_t, double>())
         .def_static("supported", &PyNvlsContext::supported)

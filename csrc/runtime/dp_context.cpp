@@ -110,6 +110,22 @@ void DpContext::open_peers(const std::vector<std::string>& handles) {
     }
 }
 
+void DpContext::open_local_peers(const std::vector<const DpContext*>& ctxs) {
+    if ((int)ctxs.size() != dp_) throw std::runtime_error("DpContext::open_local_peers: need one context per DP rank");
+    for (int r = 0; r < dp_; ++r) {
+        if (r == rank_) continue;
+        const DpContext* c = ctxs[r];
+        if (c == nullptr || c->dp_ != dp_ || c->rank_ != r || c->arena_numel_ != arena_numel_ ||
+            c->stage_src_stride_ != stage_src_stride_ || c->slots_per_src_ != slots_per_src_ ||
+            c->tiles_total_ != tiles_total_ || c->ll_tiles_ != ll_tiles_)
+            throw std::runtime_error("DpContext::open_local_peers: context " + std::to_string(r) +
+                                     " is not rank " + std::to_string(r) + " of the same group and geometry");
+        peers_.W[r] = c->W_; peers_.stage[r] = c->stage_;
+        peers_.arrive[r] = c->arrive_; peers_.done[r] = c->done_;
+        llA_peers_[r] = c->llA_; llC_peers_[r] = c->llC_;
+    }
+}
+
 DpLLParams DpContext::ll_params() const {
     DpLLParams p{};
     p.dp = dp_; p.rank = rank_; p.lr = lr_;

@@ -35,6 +35,10 @@ public:
 
     std::string export_handles() const;                       // 4 cudaIpcMemHandle_t, concatenated
     void open_peers(const std::vector<std::string>& handles); // index = DP rank (own entry ignored)
+    // Peers that are other contexts of this process (index = DP rank, own entry ignored): their buffers enter the
+    // pointer tables directly, without IPC.  Lets one GPU run one replica of a dp-way group against peers whose
+    // messages a test writes and reads.
+    void open_local_peers(const std::vector<const DpContext*>& ctxs);
 
     DpLayerParams layer_params(int layer_index) const;        // 0-based layer of the stage
     const DpPeers& peers() const { return peers_; }
@@ -44,6 +48,18 @@ public:
     int dp() const { return dp_; }
     int rank() const { return rank_; }
     int64_t stage_bytes() const { return (int64_t)dp_ * stage_src_stride_ * 4; }
+    // raw buffers and the strides that address them (tests)
+    float* stage() const { return stage_; }
+    uint32_t* arrive() const { return arrive_; }
+    uint32_t* done() const { return done_; }
+    uint4* ll_a() const { return llA_; }
+    uint4* ll_c() const { return llC_; }
+    int64_t arrive_bytes() const { return (int64_t)dp_ * slots_per_src_ * 4; }
+    int64_t done_bytes() const { return (int64_t)tiles_total_ * 4; }
+    int64_t ll_zone_bytes() const { return ll_tiles_ > 0 ? (int64_t)dp_ll_zone_lines(dp_, ll_tiles_) * (int64_t)sizeof(uint4) : 0; }
+    int slots_per_src() const { return slots_per_src_; }
+    int64_t stage_src_stride() const { return stage_src_stride_; }
+    int64_t stage_parity_stride() const { return stage_parity_stride_; }
     const std::vector<DpLayerGeom>& geometry() const { return geom_; }
     int total_ctas() const { return total_ctas_; }   // sum of tiles over layers: all co-resident if <= #SMs
     // LL two-shot path (dp_ll.cu): landing zones exist when every layer is narrow enough for all tiles to be co-resident

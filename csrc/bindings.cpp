@@ -28,6 +28,19 @@ static void cuda_ok(cudaError_t e, const char* what) {
 }
 static cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 
+// The update kernels read lr from device memory when they run.  `lr` is a Python number, written into a fresh device
+// scalar on the current stream, or a one-element fp32 tensor on `like`'s device that the caller may rewrite after the
+// launch has been enqueued.
+static Tensor lr_scalar(const py::handle& lr, const Tensor& like, const char* what) {
+    if (THPVariable_Check(lr.ptr())) {
+        Tensor t = py::cast<Tensor>(lr);
+        TORCH_CHECK(t.is_cuda() && t.device() == like.device() && t.scalar_type() == torch::kFloat32 && t.numel() == 1,
+                    what, ": a tensor lr must be one fp32 element on the kernel's device");
+        return t;
+    }
+    return torch::full({1}, py::cast<double>(lr), like.options().dtype(torch::kFloat32));
+}
+
 // k_splits: 0 / 1 = plain kernel, -1 = let the planner decide, k >= 2 = force k (must not leave a split empty).
 // The workspace and the tile counters are torch tensors owned by the caller's scope (stream-ordered reuse).
 static void enable_splitk(ssb::GemmPlan& plan, int64_t k_splits, const Tensor& like, Tensor& ws, Tensor& counters) {
@@ -87,7 +100,7 @@ static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<
 // With momentum / weight decay the fused update follows the stateful rule; V is the momentum buffer with W's layout
 // (same row pitch; its column `in` belongs to the bias).
 static void linear_wgrad(const Tensor& dz, const Tensor& x, Tensor& G, bool accumulate, const c10::optional<Tensor>& db,
-                         int64_t db_stride, const c10::optional<Tensor>& W, double lr, bool fuse_sgd,
+                         int64_t db_stride, const c10::optional<Tensor>& W, const py::object& lr, bool fuse_sgd,
                          bool split, const c10::optional<Tensor>& V, double momentum, double weight_decay, bool nesterov) {
     check_mat(dz, "dz"); check_mat(x, "x"); check_mat(G, "G");
     const int rows = dz.size(0), out = dz.size(1), in = x.size(1);
@@ -101,12 +114,14 @@ static void linear_wgrad(const Tensor& dz, const Tensor& x, Tensor& G, bool accu
         opt.V = V->data_ptr<float>();
     }
     c10::cuda::CUDAGuard guard(dz.device());
+    const Tensor lr_dev = fuse_sgd ? lr_scalar(lr, dz, "linear_wgrad") : Tensor();
     ssb::GemmPlan plan;
     const char* err = ssb::gemm_plan_wgrad(&plan, dz.data_ptr<float>(), ld_of(dz), x.data_ptr<float>(), ld_of(x),
                                            G.data_ptr<float>(), ld_of(G), rows, in, out, accumulate,
                                            db.has_value() ? db->data_ptr<float>() : nullptr, (int)db_stride,
                                            W.has_value() ? W->data_ptr<float>() : nullptr,
-                                           W.has_value() ? ld_of(*W) : 0, (float)lr, fuse_sgd, split, opt);
+                                           W.has_value() ? ld_of(*W) : 0, fuse_sgd ? lr_dev.data_ptr<float>() : nullptr,
+                                           fuse_sgd, split, opt);
     TORCH_CHECK(err == nullptr, "linear_wgrad: ", err ? err : "");
     cuda_ok(ssb::gemm_launch(plan, cur_stream()), "linear_wgrad launch");
 }
@@ -150,12 +165,13 @@ static void axpby(const Tensor& x, const Tensor& t, Tensor& y, double a, double 
     c10::cuda::CUDAGuard guard(x.device());
     cuda_ok(ssb::launch_axpby(x.data_ptr<float>(), t.data_ptr<float>(), y.data_ptr<float>(), (float)a, (float)b, x.numel(), cur_stream()), "axpby");
 }
-static void sgd_(Tensor& w, const Tensor& g, double lr) {
+static void sgd_(Tensor& w, const Tensor& g, const py::object& lr) {
     TORCH_CHECK(w.is_contiguous() && g.is_contiguous() && w.numel() == g.numel());
     c10::cuda::CUDAGuard guard(w.device());
-    cuda_ok(ssb::launch_sgd(w.data_ptr<float>(), g.data_ptr<float>(), (float)lr, w.numel(), cur_stream()), "sgd");
+    const Tensor lr_dev = lr_scalar(lr, w, "sgd_");
+    cuda_ok(ssb::launch_sgd(w.data_ptr<float>(), g.data_ptr<float>(), lr_dev.data_ptr<float>(), w.numel(), cur_stream()), "sgd");
 }
-static void sgd_momentum_(Tensor& w, const Tensor& g, const c10::optional<Tensor>& v, double lr, double momentum,
+static void sgd_momentum_(Tensor& w, const Tensor& g, const c10::optional<Tensor>& v, const py::object& lr, double momentum,
                           double weight_decay, bool nesterov) {
     TORCH_CHECK(w.is_contiguous() && g.is_contiguous() && w.numel() == g.numel());
     TORCH_CHECK(w.scalar_type() == torch::kFloat32 && g.scalar_type() == torch::kFloat32);
@@ -168,7 +184,8 @@ static void sgd_momentum_(Tensor& w, const Tensor& g, const c10::optional<Tensor
     const char* err = ssb::sgd_state_check(opt);
     TORCH_CHECK(err == nullptr, "sgd_momentum_: ", err ? err : "");
     c10::cuda::CUDAGuard guard(w.device());
-    cuda_ok(ssb::launch_sgd_momentum(w.data_ptr<float>(), g.data_ptr<float>(), (float)lr, opt, w.numel(), cur_stream()),
+    const Tensor lr_dev = lr_scalar(lr, w, "sgd_momentum_");
+    cuda_ok(ssb::launch_sgd_momentum(w.data_ptr<float>(), g.data_ptr<float>(), lr_dev.data_ptr<float>(), opt, w.numel(), cur_stream()),
             "sgd_momentum");
 }
 static void argmax_correct(const Tensor& pred, const Tensor& target, Tensor& correct) {

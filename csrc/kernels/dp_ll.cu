@@ -184,6 +184,7 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
             const int n_lines = my_rows * lpr;
             const float* mine0 = own + (p.rank * rpo) * kOwnLd;
             const uint4* zoneA = p.llA[p.rank] + (size_t)parity * DP * p.n_tiles * rpo * 17;
+            const float lr = *p.lr;                              // in flight with the first batch's loads
             for (int i0 = etid; i0 < n_lines; i0 += 128 * kLB) {
                 uint4 ln[kLB][DP];
                 float wv0[kLB], wv1[kLB];
@@ -247,10 +248,10 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
                     }
                     if (j < 16) {
                         const int n = e.n0 + 2 * j;
-                        if (n < e.n_total) { w0 = wv0[u] - p.lr * s0; wrow[n] = w0; }
-                        if (n + 1 < e.n_total) { w1 = wv1[u] - p.lr * s1; wrow[n + 1] = w1; }
+                        if (n < e.n_total) { w0 = wv0[u] - lr * s0; wrow[n] = w0; }
+                        if (n + 1 < e.n_total) { w1 = wv1[u] - lr * s1; wrow[n + 1] = w1; }
                     } else {
-                        w0 = wv0[u] - p.lr * s0;                 // bias lives in column `in` of the block
+                        w0 = wv0[u] - lr * s0;                 // bias lives in column `in` of the block
                         wrow[e.n_total] = w0;
                     }
 #pragma unroll
@@ -309,6 +310,7 @@ const char* dp_ll_plan(DpLLPlan* plan, const DpLLLayer* layers, int n_layers, in
     *plan = DpLLPlan{};
     plan->p = base;
     if (base.dp != 2 && base.dp != 4 && base.dp != 8) return "dp_ll_plan: dp must be 2, 4 or 8";
+    if (base.lr == nullptr) return "dp_ll_plan: lr (the device learning-rate slot) is not set";
     std::vector<DpLLEntry> host;
     int tile = 0;
     bool split = false;

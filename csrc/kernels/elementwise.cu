@@ -199,7 +199,9 @@ cudaError_t launch_axpby(const float* x, const float* t, float* y, float a, floa
 
 // flat-arena SGD: one launch for every parameter of the stage (n is a multiple of 4: the
 // arena is padded to 128 B); 2 x 16-byte loads in flight per thread per iteration.
-__global__ void __launch_bounds__(256) sgd_kernel(float4* __restrict__ w, const float4* __restrict__ g, float lr, long n4) {
+__global__ void __launch_bounds__(256) sgd_kernel(float4* __restrict__ w, const float4* __restrict__ g, const float* __restrict__ lr_ptr,
+                                                  long n4) {
+    const float lr = *lr_ptr;
     const long stride = (long)gridDim.x * blockDim.x;
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += stride) {
         float4 a = w[i];
@@ -208,11 +210,12 @@ __global__ void __launch_bounds__(256) sgd_kernel(float4* __restrict__ w, const 
         w[i] = a;
     }
 }
-__global__ void sgd_tail_kernel(float* w, const float* g, float lr, long start, long n) {
+__global__ void sgd_tail_kernel(float* w, const float* g, const float* lr, long start, long n) {
     const long i = start + blockIdx.x * (long)blockDim.x + threadIdx.x;
-    if (i < n) w[i] -= lr * g[i];
+    if (i < n) w[i] -= *lr * g[i];
 }
-cudaError_t launch_sgd(float* w, const float* g, float lr, long n, cudaStream_t stream) {
+cudaError_t launch_sgd(float* w, const float* g, const float* lr, long n, cudaStream_t stream) {
+    if (lr == nullptr) return cudaErrorInvalidValue;
     const bool aligned = ((reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(g)) & 15) == 0;
     const long n4 = aligned ? n / 4 : 0;
     if (n4 > 0) {
@@ -235,8 +238,9 @@ __device__ __forceinline__ float sgd_momentum_elem(float w, float g, float* v, l
     return w - lr * d;
 }
 __global__ void __launch_bounds__(256) sgd_momentum_kernel(float4* __restrict__ w, const float4* __restrict__ g,
-                                                           float4* __restrict__ v, float lr, float mu, float wd,
-                                                           int nesterov, long n4) {
+                                                           float4* __restrict__ v, const float* __restrict__ lr_ptr,
+                                                           float mu, float wd, int nesterov, long n4) {
+    const float lr = *lr_ptr;
     const long stride = (long)gridDim.x * blockDim.x;
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += stride) {
         float4 a = w[i];
@@ -251,13 +255,14 @@ __global__ void __launch_bounds__(256) sgd_momentum_kernel(float4* __restrict__ 
         w[i] = a;
     }
 }
-__global__ void sgd_momentum_tail_kernel(float* w, const float* g, float* v, float lr, float mu, float wd, int nesterov,
-                                         long start, long n) {
+__global__ void sgd_momentum_tail_kernel(float* w, const float* g, float* v, const float* lr, float mu, float wd,
+                                         int nesterov, long start, long n) {
     const long i = start + blockIdx.x * (long)blockDim.x + threadIdx.x;
-    if (i < n) w[i] = sgd_momentum_elem(w[i], g[i], v, i, lr, mu, wd, nesterov != 0);
+    if (i < n) w[i] = sgd_momentum_elem(w[i], g[i], v, i, *lr, mu, wd, nesterov != 0);
 }
-cudaError_t launch_sgd_momentum(float* w, const float* g, float lr, const SgdState& opt, long n, cudaStream_t stream) {
-    if (sgd_state_check(opt) != nullptr) return cudaErrorInvalidValue;
+cudaError_t launch_sgd_momentum(float* w, const float* g, const float* lr, const SgdState& opt, long n,
+                                cudaStream_t stream) {
+    if (lr == nullptr || sgd_state_check(opt) != nullptr) return cudaErrorInvalidValue;
     float* v = opt.V;
     const bool aligned = ((reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(v)) & 15) == 0;
     const long n4 = aligned ? n / 4 : 0;

@@ -81,6 +81,7 @@ template <bool STATEFUL>
 __device__ void dp_owner_reduce_tile(const DpPeers& peers, const DpLayerParams& p, const TileCoord& tc, uint32_t epoch,
                                      int tid, int nthreads, int bar_id, int part = 0, int nparts = 1, bool publish = true) {
     const int me = p.rank;
+    const float lr = *p.lr;                               // written before the launch: load it under the wait below
     // wait until every replica's partial of this tile has landed in my staging memory
     if (tid < p.dp) wait_flag_ge(peers.arrive[me] + (int64_t)tid * p.slots_per_src + p.slot_flag_base + tc.slot, epoch);
     asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(nthreads) : "memory");
@@ -145,7 +146,7 @@ __device__ void dp_owner_reduce_tile(const DpPeers& peers, const DpLayerParams& 
                     sum.w = sgd_direction<false>(sum.w, w.w, v.w, mu, wd, nv);
                     if (vp != nullptr) *vp = v;
                 }
-                w.x -= p.lr * sum.x; w.y -= p.lr * sum.y; w.z -= p.lr * sum.z; w.w -= p.lr * sum.w;
+                w.x -= lr * sum.x; w.y -= lr * sum.y; w.z -= lr * sum.z; w.w -= lr * sum.w;
                 if (n_pub == 1) *reinterpret_cast<float4*>(peers.W[me] + woff) = w;
                 else for (int r2 = 0; r2 < p.dp; ++r2) *reinterpret_cast<float4*>(peers.W[r2] + woff) = w;   // publish to all replicas
             } else {
@@ -153,7 +154,7 @@ __device__ void dp_owner_reduce_tile(const DpPeers& peers, const DpLayerParams& 
                 for (int e = 0; e < 4 && n + e < p.n_total; ++e) {
                     float d = sv[e];
                     if constexpr (STATEFUL) d = elem_direction(p, woff + e, d, peers.W[me][woff + e]);
-                    const float w = peers.W[me][woff + e] - p.lr * d;
+                    const float w = peers.W[me][woff + e] - lr * d;
                     if (n_pub == 1) peers.W[me][woff + e] = w;
                     else for (int r2 = 0; r2 < p.dp; ++r2) peers.W[r2][woff + e] = w;
                 }
@@ -169,7 +170,7 @@ __device__ void dp_owner_reduce_tile(const DpPeers& peers, const DpLayerParams& 
                 sum += ld_cg_f(st0 + (int64_t)s * p.stage_src_stride + (int64_t)kBlockM * p.block_n + r);
             const int64_t boff = p.w_offset + (int64_t)m * p.ldw + p.n_total;
             if constexpr (STATEFUL) sum = elem_direction(p, boff, sum, peers.W[me][boff]);
-            const float b = peers.W[me][boff] - p.lr * sum;
+            const float b = peers.W[me][boff] - lr * sum;
             if (n_pub == 1) peers.W[me][boff] = b;
             else for (int r2 = 0; r2 < p.dp; ++r2) peers.W[r2][boff] = b;
         }
@@ -447,6 +448,7 @@ void dp_layer_geometry(int in, int out, int dp, int* block_n, int* n_tiles_m, in
 const char* fused_dp_plan(FusedDpPlan* plan, const float* dZ, int lddz, const float* X, int ldx, int rows, const DpLayerParams& lp,
                           const DpPeers& peers, int max_ctas, bool split) {
     *plan = FusedDpPlan{};
+    if (lp.lr == nullptr) return "fused_dp_plan: lr (the device learning-rate slot) is not set";
     plan->p = lp;
     plan->peers = peers;
     DpLayerParams& p = plan->p;

@@ -55,10 +55,11 @@ struct GemmParams {
     float* db;          // nullable
     int db_stride;
     // WGRAD with the SGD update fused (single replica, not combinable with accumulate):
-    // the -lr-scaled tile is TMA-reduce-added into W; G is never touched
+    // the -lr-scaled tile is TMA-reduce-added into W; G is never touched.  lr: one device float, read once per thread
+    // at run time (a learning-rate schedule rewrites it between steps without re-planning)
     float* W;
     int ldw;
-    float lr;
+    const float* lr;
     int fuse_sgd;
     // stateful update rule of the fused SGD (see SgdState): V = momentum buffer with W's layout (pitch ldw, nullable
     // when momentum == 0), read and written per element; W is read as well when weight_decay != 0
@@ -95,7 +96,7 @@ const char* gemm_plan_dgrad(GemmPlan* plan, const float* W, int ldw, const float
                             int rows, int in, int out, const float* mask, int ldmask, bool split = false);
 const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const float* X, int ldx, float* G, int ldg,
                             int rows, int in, int out, int accumulate, float* db, int db_stride, float* W, int ldw,
-                            float lr, int fuse_sgd, bool split = false, const SgdState& opt = SgdState{});
+                            const float* lr, int fuse_sgd, bool split = false, const SgdState& opt = SgdState{});
 // Split-K for FWD / DGRAD plans whose output has fewer tiles than the chip has SMs (wide, weight-bound layers):
 // choice() returns the number of k-splits (1 = leave the plan alone); enable() rewires the plan (grid.z, ring
 // depth for two CTAs per SM).  workspace: gemm_splitk_workspace_floats() floats; counters: one zeroed uint per tile.
@@ -138,7 +139,7 @@ struct DpLayerParams {
     int64_t stage_offset;            // float offset of the layer's slots inside one src region
     int64_t stage_src_stride;        // floats per src region
     int tile_flag_base, slot_flag_base, slots_per_src;
-    float lr;
+    const float* lr;                 // device float: learning rate of the running step
     const uint32_t* epoch_ptr;       // device step counter (bumped once per step, same value on all ranks)
     const float* G;                  // dp_reduce_sgd: accumulated gradient block to reduce
     int ldg;
@@ -193,7 +194,7 @@ struct DpLLEntry {               // one CTA = one [128 x 32] tile of one layer's
 };
 struct DpLLParams {
     int dp, rank;
-    float lr;
+    const float* lr;             // device float: learning rate of the running step
     const uint32_t* epoch_ptr;   // DP step counter (same value on every replica)
     const uint32_t* gate_step;   // steps of the launching engine (gate target = gate_mult * *gate_step)
     int n_tiles, stages;
@@ -312,10 +313,10 @@ cudaError_t launch_relu_mask(float* g, int ldg, const float* y, int ldy, int row
 cudaError_t launch_relu_fwd(const float* x, float* y, long n, cudaStream_t stream);
 // y = a * x + b * t  (mse grad: a=2/B, b=-2/B)
 cudaError_t launch_axpby(const float* x, const float* t, float* y, float a, float b, long n, cudaStream_t stream);
-// w -= lr * g over a flat arena
-cudaError_t launch_sgd(float* w, const float* g, float lr, long n, cudaStream_t stream);
+// w -= *lr * g over a flat arena (lr: one device float, read when the kernel runs)
+cudaError_t launch_sgd(float* w, const float* g, const float* lr, long n, cudaStream_t stream);
 // the same pass with the stateful rule (momentum buffer opt.V over the same n elements, weight decay, Nesterov)
-cudaError_t launch_sgd_momentum(float* w, const float* g, float lr, const SgdState& opt, long n, cudaStream_t stream);
+cudaError_t launch_sgd_momentum(float* w, const float* g, const float* lr, const SgdState& opt, long n, cudaStream_t stream);
 // correct[0] += #rows with argmax(pred) == argmax(target)
 cudaError_t launch_argmax_correct(const float* pred, int ldp, const float* target, int ldt, int rows, int cols,
                                   int* correct, cudaStream_t stream);

@@ -41,6 +41,7 @@ template <bool SGD, bool STATEFUL = false>
 __global__ void __launch_bounds__(256) nvls_reduce_kernel(const NvlsParams p) {
     const uint32_t epoch = *p.epoch + 1u;                     // same value on every replica (one bump per launch)
     const uint32_t target = epoch * (uint32_t)p.dp;
+    const float lr = SGD ? *p.lr : 0.f;                      // learning rate of this step (device slot)
 
     // ---- my gradients are final (stream order: the wgrad kernels of this step precede this launch)
     if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -63,13 +64,13 @@ __global__ void __launch_bounds__(256) nvls_reduce_kernel(const NvlsParams p) {
                 float4 v = vp != nullptr ? *vp : make_float4(0.f, 0.f, 0.f, 0.f);
                 const float mu = p.opt.momentum, wd = p.opt.weight_decay;
                 const bool nv = p.opt.nesterov != 0;
-                w.x -= p.lr * sgd_direction<false>(g.x, w.x, v.x, mu, wd, nv);
-                w.y -= p.lr * sgd_direction<false>(g.y, w.y, v.y, mu, wd, nv);
-                w.z -= p.lr * sgd_direction<false>(g.z, w.z, v.z, mu, wd, nv);
-                w.w -= p.lr * sgd_direction<false>(g.w, w.w, v.w, mu, wd, nv);
+                w.x -= lr * sgd_direction<false>(g.x, w.x, v.x, mu, wd, nv);
+                w.y -= lr * sgd_direction<false>(g.y, w.y, v.y, mu, wd, nv);
+                w.z -= lr * sgd_direction<false>(g.z, w.z, v.z, mu, wd, nv);
+                w.w -= lr * sgd_direction<false>(g.w, w.w, v.w, mu, wd, nv);
                 if (vp != nullptr) *vp = v;
             } else {
-                w.x -= p.lr * g.x; w.y -= p.lr * g.y; w.z -= p.lr * g.z; w.w -= p.lr * g.w;
+                w.x -= lr * g.x; w.y -= lr * g.y; w.z -= lr * g.z; w.w -= lr * g.w;
             }
             multimem_st_f4(p.W_mc + 4 * c, w);
         } else {
@@ -103,6 +104,7 @@ static int nvls_grid(const NvlsParams& p, int max_ctas) {
 }
 
 cudaError_t launch_nvls_reduce_sgd(const NvlsParams& p, int max_ctas, cudaStream_t stream) {
+    if (p.lr == nullptr) return cudaErrorInvalidValue;
     if (p.opt.momentum != 0.f || p.opt.weight_decay != 0.f)
         nvls_reduce_kernel<true, true><<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
     else

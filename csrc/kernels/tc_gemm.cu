@@ -126,6 +126,10 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
         float acc[2][kMaxBlockN / 8][4];
         warp_acc_zero(acc);
         float dbsum = 0.f;
+        // the fused update's learning rate, loaded before the main loop so that its latency hides under the GEMM.  The
+        // STATEFUL epilogue loads it next to its momentum / weight loads instead: one more register live through the
+        // loop would take that instantiation past 200 registers (two CTAs per SM).
+        const float lr_pre = (MODE == GEMM_WGRAD && !STATEFUL && p.fuse_sgd) ? *p.lr : 0.f;
         for (int kb = 0; kb < num_kb; ++kb) {
             const int s = kb % p.stages;
             const uint32_t ph = (kb / p.stages) & 1;
@@ -250,7 +254,8 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             // 16 values into the step direction d (sgd_direction) - reading and writing its V entries, and reading W
             // only with weight decay - before the same -lr scaling and reduce-add.  Columns >= n_total get d = 0 and
             // are never stored: column n_total is the bias slot, which the bias path below updates.
-            const float scale = p.fuse_sgd ? -p.lr : 1.f;
+            const float lr = STATEFUL ? *p.lr : lr_pre;            // STATEFUL implies fuse_sgd
+            const float scale = p.fuse_sgd ? -lr : 1.f;
 #pragma unroll
             for (int ch = 0; ch < kChunks; ++ch) {
                 if (16 * ch >= p.block_n) break;
@@ -347,9 +352,9 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                         float vb = p.V != nullptr ? p.V[boff] : 0.f;
                         const float d = sgd_direction<false>(dbsum, *bp, vb, p.momentum, p.weight_decay, p.nesterov != 0);
                         if (p.V != nullptr) p.V[boff] = vb;
-                        *bp -= p.lr * d;
+                        *bp -= lr * d;
                     } else {
-                        *bp -= p.lr * dbsum;
+                        *bp -= lr * dbsum;
                     }
                 } else {
                     float* dbp = p.db + (size_t)m * p.db_stride;
@@ -483,7 +488,7 @@ const char* gemm_plan_dgrad(GemmPlan* plan, const float* W, int ldw, const float
 
 const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const float* X, int ldx, float* G, int ldg,
                             int rows, int in, int out, int accumulate, float* db, int db_stride, float* W, int ldw,
-                            float lr, int fuse_sgd, bool split, const SgdState& opt) {
+                            const float* lr, int fuse_sgd, bool split, const SgdState& opt) {
     *plan = GemmPlan{};
     plan->mode = GEMM_WGRAD;
     GemmParams& p = plan->p;
@@ -492,6 +497,7 @@ const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const flo
     p.G = G; p.ldg = ldg; p.accumulate = accumulate; p.db = db; p.db_stride = db_stride;
     p.W = W; p.ldw = ldw; p.lr = lr; p.fuse_sgd = fuse_sgd;
     if (fuse_sgd && W == nullptr) return "fuse_sgd needs W";
+    if (fuse_sgd && lr == nullptr) return "fuse_sgd needs lr (a device float)";
     if (fuse_sgd && accumulate) return "fuse_sgd cannot be combined with accumulate (reduce into G, then run the SGD pass)";
     // the fused update finds the bias at db's offset from G, taken in W (and V): only the arena layout's bias column
     // (column `in` of G's block) names a slot of W

@@ -155,8 +155,12 @@ public:
     void all_reduce_grads() {
         TORCH_CHECK(launch_nvls_allreduce(ctx_->params(), num_sms(), c10::cuda::getCurrentCUDAStream()) == cudaSuccess, "nvls allreduce launch");
     }
-    void reduce_sgd() {
-        TORCH_CHECK(launch_nvls_reduce_sgd(ctx_->params(), num_sms(), c10::cuda::getCurrentCUDAStream()) == cudaSuccess, "nvls reduce_sgd launch");
+    // lr: one-element fp32 tensor on this device, read by the kernel when it runs
+    void reduce_sgd(const torch::Tensor& lr) {
+        TORCH_CHECK(lr.is_cuda() && lr.scalar_type() == torch::kFloat32 && lr.numel() == 1, "reduce_sgd: lr must be a one-element fp32 CUDA tensor");
+        NvlsParams p = ctx_->params();
+        p.lr = lr.data_ptr<float>();
+        TORCH_CHECK(launch_nvls_reduce_sgd(p, num_sms(), c10::cuda::getCurrentCUDAStream()) == cudaSuccess, "nvls reduce_sgd launch");
     }
     NvlsContext* get() { return ctx_.get(); }
 
@@ -252,6 +256,11 @@ public:
     }
     int n_mubatches() { return engine_->config().n_mu; }
     void run() { engine_->run(); }
+    void set_lr(double lr) {
+        TORCH_CHECK(std::isfinite(lr) && lr >= 0.0, "PipeEngine.set_lr: the learning rate must be finite and >= 0, got ", lr);
+        engine_->set_lr((float)lr);
+    }
+    float lr() { return engine_->lr(); }
     void synchronize() { engine_->synchronize(); }
     bool wait(double timeout_s) {
         py::gil_scoped_release nogil;
@@ -333,7 +342,7 @@ void bind_runtime(py::module_& m) {
         .def("grads", &PyNvlsContext::grads)
         .def("bytes", &PyNvlsContext::bytes)
         .def("all_reduce_grads", &PyNvlsContext::all_reduce_grads)
-        .def("reduce_sgd", &PyNvlsContext::reduce_sgd);
+        .def("reduce_sgd", &PyNvlsContext::reduce_sgd, py::arg("lr"));
     py::class_<PyPpContext, std::shared_ptr<PyPpContext>>(m, "PpContext")
         .def(py::init<int, int, int, int, bool, bool>())
         .def("export_handles", &PyPpContext::export_handles)
@@ -353,6 +362,8 @@ void bind_runtime(py::module_& m) {
         .def("stage_inputs", &PyEngine::stage_inputs)
         .def("n_mubatches", &PyEngine::n_mubatches)
         .def("run", &PyEngine::run)
+        .def("set_lr", &PyEngine::set_lr, py::arg("lr"))
+        .def("lr", &PyEngine::lr)
         .def("synchronize", &PyEngine::synchronize)
         .def("wait", &PyEngine::wait)
         .def("comm_status", &PyEngine::comm_status)

@@ -17,8 +17,8 @@ namespace ssb {
 static int64_t round_up64(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
 
 DpContext::DpContext(int dp, int rank, int64_t arena_numel, const std::vector<std::tuple<int, int, int64_t, int>>& layers,
-                     float lr)
-    : dp_(dp), rank_(rank), arena_numel_(arena_numel), lr_(lr) {
+                     float /*lr: unused, see dp_context.h*/)
+    : dp_(dp), rank_(rank), arena_numel_(arena_numel) {
     if (dp < 1 || dp > kMaxDp) throw std::runtime_error("DpContext: dp must be in [1, 8]");
     int64_t stage_off = 0;
     int slot_base = 0, tile_base = 0;
@@ -128,7 +128,7 @@ void DpContext::open_local_peers(const std::vector<const DpContext*>& ctxs) {
 
 DpLLParams DpContext::ll_params() const {
     DpLLParams p{};
-    p.dp = dp_; p.rank = rank_; p.lr = lr_;
+    p.dp = dp_; p.rank = rank_; p.lr = nullptr;
     p.epoch_ptr = epoch_; p.gate_step = nullptr;
     p.n_tiles = ll_tiles_; p.stages = 2;
     p.W = W_;
@@ -146,7 +146,7 @@ DpLayerParams DpContext::layer_params(int i) const {
     p.w_offset = g.w_offset; p.ldw = g.ld;
     p.stage_offset = g.stage_offset; p.stage_src_stride = stage_src_stride_;
     p.tile_flag_base = g.tile_flag_base; p.slot_flag_base = g.slot_flag_base; p.slots_per_src = slots_per_src_;
-    p.lr = lr_;
+    p.lr = nullptr;
     p.epoch_ptr = epoch_;
     p.G = nullptr; p.ldg = g.ld;
     p.one_shot = g.one_shot;

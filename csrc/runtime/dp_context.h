@@ -29,7 +29,8 @@ struct DpLayerGeom {
 
 class DpContext {
 public:
-    // layers: (in, out, arena offset, ld)
+    // layers: (in, out, arena offset, ld).  lr is not used: the kernels read the learning rate from the device slot the
+    // engine sets in DpLayerParams::lr / DpLLParams::lr (nullptr in the params returned here).
     DpContext(int dp, int rank, int64_t arena_numel, const std::vector<std::tuple<int, int, int64_t, int>>& layers, float lr);
     ~DpContext();
 
@@ -70,7 +71,6 @@ public:
 private:
     int dp_, rank_;
     int64_t arena_numel_;
-    float lr_;
     std::vector<DpLayerGeom> geom_;
     int64_t stage_src_stride_ = 0, stage_parity_stride_ = 0;
     int total_ctas_ = 0;

@@ -68,8 +68,8 @@ bool NvlsContext::supported() {
     return flag != 0;
 }
 
-NvlsContext::NvlsContext(int dp, int rank, int64_t arena_numel, float lr)
-    : dp_(dp), rank_(rank), arena_numel_(arena_numel), lr_(lr) {
+NvlsContext::NvlsContext(int dp, int rank, int64_t arena_numel, float /*lr: unused, see nvls_context.h*/)
+    : dp_(dp), rank_(rank), arena_numel_(arena_numel) {
     if (dp < 2 || dp > 8) throw std::runtime_error("NvlsContext: dp must be in [2, 8]");
     CUDA_RT(cudaGetDevice(&dev_));
     CUDA_RT(cudaFree(nullptr));                                  // make sure the primary context exists
@@ -185,7 +185,7 @@ NvlsParams NvlsContext::params() const {
     p.cta_done = cta_done_;
     p.numel = numel_pad_;
     p.dp = dp_; p.rank = rank_;
-    p.lr = lr_;
+    p.lr = nullptr;
     return p;
 }
 

@@ -38,12 +38,14 @@ struct NvlsParams {
     unsigned int* cta_done; // local counter for the last-CTA election
     int64_t numel;          // floats to reduce / update (multiple of 4)
     int dp, rank;
-    float lr;
+    const float* lr;        // device float: learning rate of the running step (reduce_sgd only)
     SgdState opt;           // update rule; opt.V = LOCAL momentum arena (unicast), chunk c's entries live at rank c % dp
 };
 
 class NvlsContext {
 public:
+    // lr is not used: the kernel reads the learning rate from NvlsParams::lr, a device slot the caller sets (nullptr in
+    // params())
     NvlsContext(int dp, int rank, int64_t arena_numel, float lr);
     ~NvlsContext();
 
@@ -65,7 +67,6 @@ public:
 private:
     int dp_, rank_, dev_ = 0;
     int64_t arena_numel_, numel_pad_;
-    float lr_;
     size_t size_ = 0, gran_ = 0;
     CUmemGenericAllocationHandle mc_ = 0, mem_ = 0;
     bool have_mc_ = false, have_mem_ = false, bound_ = false;
@@ -75,7 +76,7 @@ private:
 };
 
 // kernels (csrc/kernels/nvls_dp.cu)
-//   reduce_sgd: W <- W - lr * sum_replicas(G), every replica ends with the same W (one kernel, whole arena)
+//   reduce_sgd: W <- W - *p.lr * sum_replicas(G), every replica ends with the same W (one kernel, whole arena)
 //   allreduce : G <- sum_replicas(G) in place (stand-alone collective, used by the NVLS bandwidth benchmark)
 cudaError_t launch_nvls_reduce_sgd(const NvlsParams& p, int max_ctas, cudaStream_t stream);
 cudaError_t launch_nvls_allreduce(const NvlsParams& p, int max_ctas, cudaStream_t stream);

@@ -7,6 +7,7 @@
 #include <chrono>
 #include <thread>
 #include <cstdlib>
+#include <cstring>
 #include <sstream>
 #include <stdexcept>
 
@@ -32,6 +33,24 @@ enum : int {
 };
 
 static int round_up(int x, int m) { return (x + m - 1) / m * m; }
+
+// cuMemsetD32Async, reached through the runtime so that the extension does not link libcuda (as in nvls_context.cpp):
+// writes the learning-rate slot by value.
+using MemsetD32AsyncFn = CUresult (*)(CUdeviceptr, unsigned int, size_t, CUstream);
+static MemsetD32AsyncFn memset_d32_async() {
+    static MemsetD32AsyncFn fn = [] {
+        void* ptr = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuMemsetD32Async", &ptr, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess || ptr == nullptr)
+            throw std::runtime_error("PipeEngine: driver entry point cuMemsetD32Async not available");
+        return reinterpret_cast<MemsetD32AsyncFn>(ptr);
+    }();
+    return fn;
+}
+static void cu_check(CUresult r, const char* what) {
+    if (r != CUDA_SUCCESS) throw std::runtime_error(std::string("PipeEngine: ") + what + " failed (" + std::to_string((int)r) + ")");
+}
 // leave some SMs to the concurrently running dgrad chain; also bounds co-residency needs
 static constexpr int kFusedDpMaxCtas = 120;
 
@@ -104,6 +123,10 @@ void PipeEngine::alloc_buffers() {
     }
     x_stage_ = x_stage_sets_[0];
     y_stage_ = y_stage_sets_[0];
+    lr_dev_ = dalloc(2);
+    lr_ = lr_written_[0] = lr_written_[1] = cfg_.lr;
+    const float lr_init[2] = {cfg_.lr, cfg_.lr};
+    CUDA_CHECK(cudaMemcpy(lr_dev_, lr_init, sizeof(lr_init), cudaMemcpyHostToDevice));
     loss_dev_ = dalloc(std::max(M, 16));
     CUDA_CHECK(cudaMallocHost(&loss_host_, 2 * sizeof(float) * std::max(M, 16)));   // one slot per staging set
     // opt-in (SSB_LOSS_ZEROCOPY=1, awaiting hardware validation): the loss head stores its per-micro-batch losses straight
@@ -555,7 +578,7 @@ void PipeEngine::plan_per_mubatch() {
                         emit_wait(w, ev_dz_all);
                         GemmPlan g;
                         check(gemm_plan_wgrad(&g, dz_[mu][l], act_ld_[l], act_[mu][l - 1], act_ld_[l - 1], Gl(l), ls.ld, mb,
-                                              ls.in, ls.out, first_write[l] ? 0 : 1, Gl(l) + ls.in, ls.ld, nullptr, 0, 0.f, 0,
+                                              ls.in, ls.out, first_write[l] ? 0 : 1, Gl(l) + ls.in, ls.ld, nullptr, 0, nullptr, 0,
                                               cfg_.split != 0));
                         add_gemm(g, w, l, mu);
                         first_write[l] = false;
@@ -595,7 +618,7 @@ void PipeEngine::plan_per_mubatch() {
                         emit_wait(w, ev_dz);
                         GemmPlan g;
                         check(gemm_plan_wgrad(&g, dz_[mu][l], act_ld_[l], act_[mu][l - 1], act_ld_[l - 1], Gl(l), ls.ld, mb,
-                                              ls.in, ls.out, first_write[l] ? 0 : 1, Gl(l) + ls.in, ls.ld, nullptr, 0, 0.f, 0,
+                                              ls.in, ls.out, first_write[l] ? 0 : 1, Gl(l) + ls.in, ls.ld, nullptr, 0, nullptr, 0,
                                               cfg_.split != 0));
                         add_gemm(g, w, l, mu);
                         first_write[l] = false;
@@ -630,6 +653,7 @@ void PipeEngine::plan_per_mubatch() {
                         emit_wait(s_dp_, pd.second);
                         DpLayerParams lp = dp_ctx_->layer_params(pd.first - 1);
                         lp.opt = opt_for(0);
+                        lp.lr = lr_slot();
                         layer_proto_[pd.first - 1] = lp.one_shot ? DP_PROTO_ALL : DP_PROTO_TWO_SHOT;
                         lp.G = Gl(pd.first);
                         FusedDpPlan fp;
@@ -656,7 +680,7 @@ void PipeEngine::plan_per_mubatch() {
                             const LayerSpec& ls = cfg_.layers[l - 1];
                             GemmPlan g;
                             check(gemm_plan_wgrad(&g, dz_all_[l], act_ld_[l], act_all_[l - 1], act_ld_[l - 1], Gl(l), ls.ld, rows_all, ls.in,
-                                                  ls.out, 0, Gl(l) + ls.in, ls.ld, Wl(l), ls.ld, cfg_.lr, 1, cfg_.split != 0,
+                                                  ls.out, 0, Gl(l) + ls.in, ls.ld, Wl(l), ls.ld, lr_slot(), 1, cfg_.split != 0,
                                                   opt_for(l)));
                             grouped.push_back(g);
                         }
@@ -678,6 +702,7 @@ void PipeEngine::plan_per_mubatch() {
                         DpLLPlan lp;
                         DpLLParams base = dp_ctx_->ll_params();
                         base.opt = opt_for(0);
+                        base.lr = lr_slot();
                         for (int l = 0; l < L_; ++l) layer_proto_[l] = DP_PROTO_LL;
                         check(dp_ll_plan(&lp, lls.data(), (int)lls.size(), rows_all, base));
                         ll_plans_.push_back(lp);
@@ -698,7 +723,7 @@ void PipeEngine::plan_per_mubatch() {
                     }
                     Op sg;
                     sg.kind = (cfg_.dp_mode == 3) ? OP_NVLS_SGD : OP_SGD;
-                    sg.stream = s_dp_; sg.a = W_; sg.b = G_; sg.scalar = cfg_.lr; sg.n = arena_numel_;
+                    sg.stream = s_dp_; sg.a = W_; sg.b = G_; sg.lr = lr_slot(); sg.n = arena_numel_;
                     ops_.push_back(sg);
                 }
                 break;
@@ -868,6 +893,7 @@ void PipeEngine::build_coalesced() {
             FusedDpPlan fp;
             DpLayerParams lp = dp_ctx_->layer_params(l - 1);
             lp.opt = opt_for(0);
+            lp.lr = lr_slot();
             layer_proto_[l - 1] = lp.one_shot ? DP_PROTO_ALL : DP_PROTO_TWO_SHOT;
             if (getenv("SSB_CHAIN_TIMELINE")) {
                 if (!chain_dbg_) {
@@ -893,7 +919,7 @@ void PipeEngine::build_coalesced() {
         }
         GemmPlan g;
         check(gemm_plan_wgrad(&g, dz_all_[l], act_ld_[l], act_all_[l - 1], act_ld_[l - 1], Gl(l), ls.ld, rows, ls.in, ls.out, 0,
-                              Gl(l) + ls.in, ls.ld, fuse ? Wl(l) : nullptr, ls.ld, cfg_.lr, fuse ? 1 : 0, cfg_.split != 0,
+                              Gl(l) + ls.in, ls.ld, fuse ? Wl(l) : nullptr, ls.ld, lr_slot(), fuse ? 1 : 0, cfg_.split != 0,
                               fuse ? opt_for(l) : SgdState{}));
         if (group_wgrad) {                                  // launched together after the loop
             grouped.push_back(g);
@@ -913,6 +939,7 @@ void PipeEngine::build_coalesced() {
         // deepest layer first: its tiles get the lowest block indices, i.e. they are resident first and their gate opens first
         DpLLParams base = dp_ctx_->ll_params();
         base.opt = opt_for(0);
+        base.lr = lr_slot();
         for (int l = 0; l < L_; ++l) layer_proto_[l] = DP_PROTO_LL;
         base.gate_step = gate_on_ ? gate_step_ : nullptr;
         if (getenv("SSB_CHAIN_TIMELINE")) {
@@ -955,7 +982,7 @@ void PipeEngine::build_coalesced() {
         }
         Op sg;
         sg.kind = (cfg_.dp_mode == 3) ? OP_NVLS_SGD : OP_SGD;
-        sg.stream = s_dp_; sg.a = W_; sg.b = G_; sg.scalar = cfg_.lr; sg.n = arena_numel_;
+        sg.stream = s_dp_; sg.a = W_; sg.b = G_; sg.lr = lr_slot(); sg.n = arena_numel_;
         ops_.push_back(sg);
     }
     for (size_t s = 1; s < streams_.size(); ++s)
@@ -1025,8 +1052,8 @@ void PipeEngine::exec(const Op& op) {
         case OP_RELU_MASK: CUDA_CHECK(launch_relu_mask(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, st)); break;
         case OP_SGD: {
             const SgdState opt = opt_for(0);
-            if (opt.plain()) CUDA_CHECK(launch_sgd(op.a, op.b, op.scalar, op.n, st));
-            else CUDA_CHECK(launch_sgd_momentum(op.a, op.b, op.scalar, opt, op.n, st));
+            if (opt.plain()) CUDA_CHECK(launch_sgd(op.a, op.b, op.lr, op.n, st));
+            else CUDA_CHECK(launch_sgd_momentum(op.a, op.b, op.lr, opt, op.n, st));
             break;
         }
         case OP_NVLS_SGD: {
@@ -1038,6 +1065,7 @@ void PipeEngine::exec(const Op& op) {
             CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
             NvlsParams np = nvls_ctx_->params();
             np.opt = opt_for(0);
+            np.lr = op.lr;
             CUDA_CHECK(launch_nvls_reduce_sgd(np, sms, st));
             break;
         }
@@ -1193,7 +1221,20 @@ void PipeEngine::stage_inputs(const float* x, const float* y) {
 void PipeEngine::run() {
     if (!built_) throw std::runtime_error("PipeEngine::run before build");
     const int set = fill_set_;
-    if (staged_) CUDA_CHECK(cudaStreamWaitEvent(streams_[0], ev_copy_[set], 0));
+    // The update ops of this set read lr_dev_[set].  A new value is written by value (captured now, not read from host
+    // memory later) on the copy stream, after the set's previous step - its last reader - and before ev_copy_[set],
+    // which the step waits for.  With or without staging, that previous step is ev_done_[set].
+    bool wait_copy = staged_;
+    if (cfg_.training && lr_written_[set] != lr_) {
+        uint32_t bits;
+        memcpy(&bits, &lr_, sizeof(bits));
+        CUDA_CHECK(cudaStreamWaitEvent(copy_stream_, ev_done_[set], 0));
+        cu_check(memset_d32_async()(reinterpret_cast<CUdeviceptr>(lr_dev_ + set), bits, 1, copy_stream_), "cuMemsetD32Async");
+        CUDA_CHECK(cudaEventRecord(ev_copy_[set], copy_stream_));
+        lr_written_[set] = lr_;
+        wait_copy = true;
+    }
+    if (wait_copy) CUDA_CHECK(cudaStreamWaitEvent(streams_[0], ev_copy_[set], 0));
     if (graph_exec_sets_[set]) CUDA_CHECK(cudaGraphLaunch(graph_exec_sets_[set], streams_[0]));
     else walk(set);
     CUDA_CHECK(cudaEventRecord(ev_done_[set], streams_[0]));
@@ -1295,7 +1336,7 @@ std::string PipeEngine::describe() const {
        << ", n_mu=" << cfg_.n_mu << ", ops=" << ops_sets_[0].size() << ", kernels/step=" << kernels_per_step_
        << ", graph_nodes=" << graph_nodes_ << ", splitk_gemms=" << splitk_gemms_ << ", streams=" << streams_.size() << ", events=" << events_.size();
     if (cfg_.training) {
-        os << ", update=sgd(lr=" << cfg_.lr;
+        os << ", update=sgd(lr=" << lr_;
         if (cfg_.momentum != 0.f) os << ", momentum=" << cfg_.momentum << (cfg_.nesterov ? ", nesterov" : "");
         if (cfg_.weight_decay != 0.f) os << ", weight_decay=" << cfg_.weight_decay;
         os << ")";

@@ -67,6 +67,7 @@ struct Op {
     float* f = nullptr;        // loss head: where the loss values go when not the default device scratch
     int lda = 0, ldb = 0, ldc = 0, ldd = 0, rows = 0, cols = 0;
     float scalar = 0.f;
+    const float* lr = nullptr; // OP_SGD / OP_NVLS_SGD: the learning-rate slot of the op's staging set
     int64_t n = 0;
 };
 
@@ -77,7 +78,7 @@ struct EngineConfig {
     int mb_rows = 32;       // rows per micro-batch
     int n_mu = 4;           // micro-batches per step (training) / per call (inference)
     int global_batch = 128; // for the 1/B loss scale
-    float lr = 0.006f;
+    float lr = 0.006f;      // initial learning rate (set_lr changes it between steps)
     int training = 1;
     int use_graph = 1;
     int dp_size = 1, dp_rank = 0;
@@ -113,6 +114,10 @@ public:
     // dense row-major host/device sources: x [n_mu*mb_rows, in_dim], y [n_mu*mb_rows, out_dim]
     void stage_inputs(const float* x, const float* y);
     void run();                       // one step (graph launch or eager plan walk) on the main stream
+    // learning rate of the steps run from now on.  Every update op reads it from the device slot of its staging set;
+    // run() rewrites that slot on the copy stream only when it holds a different value.
+    void set_lr(float lr) { lr_ = lr; }
+    float lr() const { return lr_; }
     void synchronize();
     bool wait(double timeout_s);      // watchdog: false if the step in flight did not finish in time
     std::string comm_status() const;  // NCCL async error state of the attached communicators
@@ -215,6 +220,12 @@ private:
     cudaGraph_t graph_sets_[2] = {nullptr, nullptr};
     cudaGraphExec_t graph_exec_sets_[2] = {nullptr, nullptr};
     float *x_stage_sets_[2] = {nullptr, nullptr}, *y_stage_sets_[2] = {nullptr, nullptr};
+    // learning rate: one device float per staging set (lr_dev_[set]), the value last written to each, and the value the
+    // next step runs with
+    float* lr_dev_ = nullptr;
+    float lr_written_[2] = {0.f, 0.f};
+    float lr_ = 0.f;
+    const float* lr_slot() const { return lr_dev_ + cur_set_; }
     cudaStream_t copy_stream_ = nullptr;
     cudaEvent_t ev_copy_[2], ev_done_[2];
     int fill_set_ = 0, run_set_ = 0, cur_set_ = 0;

@@ -89,10 +89,11 @@ def linear_wgrad(dz, x, grad_w, accumulate=False, grad_b=None, weight=None, lr=0
                  velocity=None, momentum=0.0, weight_decay=0.0, nesterov=False):
     """grad_w[out, in] (+)= dz^T @ x ; grad_b (+)= colsum(dz).  With ``fuse_sgd`` the update goes straight into
     ``weight`` (TMA reduce-add of -lr * dW).  ``momentum`` / ``weight_decay`` / ``nesterov`` select the stateful rule
-    in that epilogue; ``velocity`` is then the momentum buffer laid out like ``weight`` (same row pitch)."""
+    in that epilogue; ``velocity`` is then the momentum buffer laid out like ``weight`` (same row pitch).  ``lr`` is a
+    number or a one-element fp32 CUDA tensor (see ``_lr_arg``)."""
     dz, x = as_tma(dz), as_tma(x)
     b, bstride = _bias_arg(grad_b, dz.size(1))
-    _C.linear_wgrad(dz, x, grad_w, bool(accumulate), b, bstride, weight, float(lr), bool(fuse_sgd), _split(precision),
+    _C.linear_wgrad(dz, x, grad_w, bool(accumulate), b, bstride, weight, _lr_arg(lr), bool(fuse_sgd), _split(precision),
                     velocity, float(momentum), float(weight_decay), bool(nesterov))
     return grad_w
 
@@ -175,14 +176,21 @@ def relu_grad(grad_output, mask_or_output):
     return g
 
 
+def _lr_arg(lr):
+    """The update kernels read the learning rate from device memory when they run: a number is written into a device
+    scalar on the current stream; a one-element fp32 CUDA tensor is passed through, so its value may still change
+    (stream-ordered) after the call."""
+    return lr if isinstance(lr, torch.Tensor) else float(lr)
+
+
 def sgd_step_(weights_flat, grads_flat, lr):
-    _C.sgd_(weights_flat, grads_flat, float(lr))
+    _C.sgd_(weights_flat, grads_flat, _lr_arg(lr))
 
 
 def sgd_momentum_step_(weights_flat, grads_flat, momentum_flat, lr, momentum, weight_decay=0.0, nesterov=False):
     """torch.optim.SGD's rule (dampening 0) over flat buffers in one pass; ``momentum_flat`` (None when
     ``momentum == 0``) is updated in place."""
-    _C.sgd_momentum_(weights_flat, grads_flat, momentum_flat, float(lr), float(momentum), float(weight_decay),
+    _C.sgd_momentum_(weights_flat, grads_flat, momentum_flat, _lr_arg(lr), float(momentum), float(weight_decay),
                      bool(nesterov))
 
 

@@ -9,7 +9,8 @@ Beyond the reference, ``momentum``, ``weight_decay`` and ``nesterov`` follow ``t
     d  = g' + momentum * v if nesterov else v
     w -= lr * d
 
-The defaults are the reference's stateless rule, bit for bit.
+The defaults are the reference's stateless rule, bit for bit.  ``lr`` may change between steps (``SGD.lr`` is
+settable); the rule above uses the current value, so the momentum buffer evolves the same way at any ``lr``.
 
 GPU: when all parameters are views into one ``ParamArena`` the update is a single fused
 pass over the flat buffers (one multi-tensor kernel on CUDA, ``csrc/kernels/elementwise.cu``)
@@ -48,7 +49,14 @@ class SGD:
 
     @property
     def lr(self):
+        """Learning rate of the next ``step`` (and of the next native-engine step, which reads it per step).  Settable,
+        e.g. by a learning-rate schedule (``lr_schedule.LRSchedule``); validated like the constructor's."""
         return self._lr
+
+    @lr.setter
+    def lr(self, value):
+        check_hparams(float(value), self.momentum, self.weight_decay, self.nesterov)
+        self._lr = float(value)
 
     @property
     def plain(self):

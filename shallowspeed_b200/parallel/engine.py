@@ -233,7 +233,6 @@ class NativeWorker:
         else:
             self.dp_mode = comm_mode
         # native communicators are shared between the train and the validation worker
-        self.lr = optimizer.lr if optimizer is not None else 0.0
         # the update rule beyond lr (optimizer.SGD); the engine keeps the momentum in the model arena's buffer
         self.momentum = float(getattr(optimizer, "momentum", 0.0) or 0.0)
         self.weight_decay = float(getattr(optimizer, "weight_decay", 0.0) or 0.0)
@@ -263,6 +262,17 @@ class NativeWorker:
         self._engines = {}
         self._last_engine = None
         self._train_engine = None      # the training plan whose DP protocols decide who owns which momentum entries
+
+    @property
+    def lr(self):
+        """The optimizer's current learning rate: the rate the next training step runs with."""
+        return self.optimizer.lr if self.optimizer is not None else 0.0
+
+    def set_lr(self, eng, sched: Schedule):
+        """Hand the optimizer's current learning rate to ``eng`` before it runs a training step (the engine rewrites
+        its device slot only when the value changed)."""
+        if sched.training and self.optimizer is not None:
+            eng.set_lr(float(self.optimizer.lr))
 
     # ------------------------------------------------------------------ plan cache
     def _key(self, sched: Schedule):
@@ -332,6 +342,7 @@ class NativeWorker:
         eng = self.engine_for(sched)
         x, y = self.dataset.load_batch(batch_id)
         self._enter(eng)
+        self.set_lr(eng, sched)
         eng.stage_inputs(x if sched.is_first_stage else None, y if sched.is_last_stage else None)
         eng.run()
         self._last_engine = eng
@@ -340,6 +351,7 @@ class NativeWorker:
         """Run one step on explicit (pinned-host or device) batch tensors."""
         eng = self.engine_for(sched)
         self._enter(eng)
+        self.set_lr(eng, sched)
         eng.stage_inputs(x if sched.is_first_stage else None, y if sched.is_last_stage else None)
         eng.run()
         self._last_engine = eng
@@ -452,12 +464,16 @@ class Trainer:
         loss = trainer.step(x_host, y_host)        # pinned host tensors of the DP-local batch
 
     Every step copies its inputs host->device and reads its loss device->host.
+
+    ``lr`` is the base learning rate.  ``lr_schedule`` (an ``lr_schedule.LRSchedule`` or any callable ``step -> lr``)
+    sets ``optimizer.lr`` before every step from the number of steps run so far; ``Trainer.lr`` is the rate of the
+    next step.
     """
 
     def __init__(self, layer_sizes, global_batch_size=128, n_mubatches=4, lr=0.006, schedule="naive",
                  dp_comm=None, pp_comm=None, grid: Optional[ProcessGrid] = None, comm_mode="fused",
                  use_graph=True, device=None, seed_mode="shape", precision="fp32", watchdog_s=None, pp_transport=None,
-                 local_batch_size=None, momentum=0.0, weight_decay=0.0, nesterov=False, loss="mse"):
+                 local_batch_size=None, momentum=0.0, weight_decay=0.0, nesterov=False, loss="mse", lr_schedule=None):
         from ..models.mlp import MLP
         from ..optimizer import SGD
         from .schedules import SCHEDULE_NAME_TO_CLS
@@ -486,9 +502,18 @@ class Trainer:
         self.engine = self.worker.engine_for(self.schedule)
         self.is_first, self.is_last = self.schedule.is_first_stage, self.schedule.is_last_stage
         self._steps = 0
+        self.lr_schedule = lr_schedule
         self.watchdog_s = watchdog_seconds(watchdog_s)   # None = plain stream synchronisation (default)
 
+    @property
+    def lr(self):
+        """The learning rate of the next step."""
+        return self.lr_schedule(self._steps) if self.lr_schedule is not None else self.optimizer.lr
+
     def step_async(self, x_host, y_host):
+        if self.lr_schedule is not None:
+            self.optimizer.lr = self.lr_schedule(self._steps)
+        self.worker.set_lr(self.engine, self.schedule)
         self.engine.stage_inputs(x_host if self.is_first else None, y_host if self.is_last else None)
         self.engine.run()
         self._steps += 1

@@ -10,8 +10,9 @@ from pathlib import Path
 
 import torch
 
-# settings a checkpoint without them was written under (plain SGD, the MSE loss)
-_HPARAM_DEFAULTS = {"momentum": 0.0, "weight_decay": 0.0, "nesterov": False, "loss": "mse"}
+# settings a checkpoint without them was written under (plain SGD, the MSE loss, a constant learning rate)
+_HPARAM_DEFAULTS = {"momentum": 0.0, "weight_decay": 0.0, "nesterov": False, "loss": "mse",
+                    "lr_schedule": {"kind": "constant"}}
 
 
 def _path(directory, stage, n_stages):

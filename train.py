@@ -24,6 +24,7 @@ import torch
 
 from shallowspeed_b200.dataset import Dataset
 from shallowspeed_b200.layers import MLP, mlp_sizes
+from shallowspeed_b200.lr_schedule import DEFAULT_WARMUP_START_FACTOR, KINDS as LR_SCHEDULES, LRSchedule
 from shallowspeed_b200.models.mlp import DEFAULT_LAYER_SIZES
 from shallowspeed_b200.optimizer import SGD
 from shallowspeed_b200.parallel.comm import ProcessGrid, SelfComm, make_torch_comms
@@ -75,6 +76,18 @@ def build_parser():
     p.add_argument("--global-batch-size", type=int, default=GLOBAL_BATCH_SIZE)
     p.add_argument("--n-mubatches", type=int, default=N_MUBATCHES)
     p.add_argument("--lr", type=float, default=LEARNING_RATE)
+    p.add_argument("--lr-schedule", choices=LR_SCHEDULES, default="constant",
+                   help="learning rate after the warmup: constant, step (StepLR), cosine (CosineAnnealingLR to --lr-min) "
+                        "or linear (linear decay to --lr-min); --lr is the base rate")
+    p.add_argument("--warmup-steps", type=int, default=0, help="linear warmup over this many steps (LinearLR)")
+    p.add_argument("--warmup-start-factor", type=float, default=DEFAULT_WARMUP_START_FACTOR,
+                   help="the first warmup step runs at this fraction of --lr, in (0, 1]")
+    p.add_argument("--lr-min", type=float, default=0.0, help="cosine / linear: the rate the decay ends at")
+    p.add_argument("--lr-step-size", type=int, default=None, help="step: steps between two decays by --lr-gamma")
+    p.add_argument("--lr-gamma", type=float, default=0.1, help="step: decay factor")
+    p.add_argument("--lr-total-steps", type=int, default=None,
+                   help="cosine / linear: the schedule's horizon in steps (default: this run's total steps; set it when "
+                        "a run is split into several invocations with --save / --resume)")
     p.add_argument("--momentum", type=float, default=0.0, help="SGD momentum (torch.optim.SGD semantics, dampening 0)")
     p.add_argument("--weight-decay", type=float, default=0.0, help="L2 penalty added to the gradient (biases included)")
     p.add_argument("--nesterov", action="store_true", help="Nesterov momentum (needs --momentum > 0)")
@@ -168,17 +181,9 @@ def main(args):
                 verbose=(grid.rank == 0 or is_last), loss=loss)
     model.to(device)
     model.train()
-    hparams = {"lr": float(args.lr), "global_batch_size": int(args.global_batch_size), "seed_mode": str(args.seed_mode),
-               "n_mubatches": int(args.n_mubatches), "momentum": float(args.momentum),
-               "weight_decay": float(args.weight_decay), "nesterov": bool(args.nesterov), "loss": loss}
     # before the resume: the momentum arena it restores is allocated here
     optimizer = SGD(model.parameters(), lr=args.lr, momentum=args.momentum, weight_decay=args.weight_decay,
                     nesterov=args.nesterov, arena=model.arena)
-    resumed_step = 0
-    if args.resume:
-        from shallowspeed_b200.utils.checkpoint import load_stage
-
-        resumed_step = load_stage(model, args.resume, pp_comm.Get_rank(), args.pp, expect_hparams=hparams)
 
     dataset = Dataset(save_dir, global_batch_size=args.global_batch_size,
                       mubatch_size=local_batch_size // args.n_mubatches, validation=False,
@@ -188,6 +193,21 @@ def main(args):
                           mubatch_size=args.global_batch_size, validation=True,
                           synthetic=synthetic, device=device)
     val_dataset.load(DP_rank=0, DP_size=1)
+
+    n_batches = dataset.get_num_batches()
+    total_steps = args.steps if args.steps is not None else args.epochs * n_batches
+    lr_schedule = LRSchedule(args.lr, args.lr_schedule, total_steps=args.lr_total_steps or total_steps,
+                             warmup_steps=args.warmup_steps, warmup_start_factor=args.warmup_start_factor,
+                             min_lr=args.lr_min, step_size=args.lr_step_size, gamma=args.lr_gamma)
+    hparams = {"lr": float(args.lr), "global_batch_size": int(args.global_batch_size), "seed_mode": str(args.seed_mode),
+               "n_mubatches": int(args.n_mubatches), "momentum": float(args.momentum),
+               "weight_decay": float(args.weight_decay), "nesterov": bool(args.nesterov), "loss": loss,
+               "lr_schedule": lr_schedule.spec()}
+    resumed_step = 0
+    if args.resume:
+        from shallowspeed_b200.utils.checkpoint import load_stage
+
+        resumed_step = load_stage(model, args.resume, pp_comm.Get_rank(), args.pp, expect_hparams=hparams)
 
     if engine == "native":
         from shallowspeed_b200.parallel.engine import NativeWorker
@@ -201,8 +221,6 @@ def main(args):
         worker = Worker(dp_comm, pp_comm, model, dataset, optimizer, device=device)
         val_worker = Worker(None, pp_comm, model, val_dataset, None, device=device)
 
-    n_batches = dataset.get_num_batches()
-    total_steps = args.steps if args.steps is not None else args.epochs * n_batches
     start_time = time.time()
     # a resumed run continues where the checkpoint stopped: same global step, same position in the data
     step = min(resumed_step, total_steps)
@@ -223,6 +241,7 @@ def main(args):
         t_epoch = time.time()
         steps_this_epoch = min(n_batches - first_batch, total_steps - step)
         for batch_id in range(first_batch, first_batch + steps_this_epoch):
+            optimizer.lr = lr_schedule(step)        # both engines read the optimizer's rate when the step starts
             worker.execute(schedule, batch_id)
             step += 1
         first_batch = 0

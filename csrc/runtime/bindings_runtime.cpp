@@ -188,6 +188,30 @@ public:
     py::bytes export_handles() { return py::bytes(ctx_->export_handles()); }
     void open_prev(const std::string& h) { ctx_->open_prev(h); }
     void open_next(const std::string& h) { ctx_->open_next(h); }
+    // test-facing: neighbours that live in this process (None: no such neighbour)
+    void open_local(const std::shared_ptr<PyPpContext>& prev, const std::shared_ptr<PyPpContext>& next) {
+        ctx_->open_local(prev ? prev->ctx_.get() : nullptr, next ? next->ctx_.get() : nullptr);
+    }
+    // test-facing: {name: (device pointer, bytes)} of the receive slots, the epoch, the push completion counter, the whole
+    // flag array and its named word ranges
+    py::dict buffers() {
+        const PpContext& c = *ctx_;
+        py::dict d;
+        auto put = [&](const char* name, const void* p, int64_t bytes) {
+            d[name] = py::make_tuple((int64_t) reinterpret_cast<uintptr_t>(p), bytes);
+        };
+        const int64_t slots = (int64_t)c.n_mu() * c.mb_rows() * sizeof(float);
+        put("act_in", c.act_in(), slots * c.ld_in());
+        put("dz_in", c.dz_in(), slots * c.ld_out());
+        put("epoch", c.epoch_ptr(), 64);
+        put("push_done", c.push_done_ptr(), 64);
+        put("flags", c.flags(), PpContext::kFlagWords * 4);
+        put("act_arrived", c.act_arrived(0), PpContext::kMaxMu * 4);
+        put("dz_arrived", c.dz_arrived(0), PpContext::kMaxMu * 4);
+        put("act_credit", c.act_credit(), 4);
+        put("dz_credit", c.dz_credit(), 4);
+        return d;
+    }
     PpContext* get() { return ctx_.get(); }
 
 private:
@@ -275,13 +299,11 @@ public:
     void reset_correct() { engine_->reset_correct(); }
     torch::Tensor act(int mu, int l) {
         const auto& cfg = engine_->config();
-        const int cols = l == 0 ? cfg.layers[0].in : cfg.layers[l - 1].out;
-        return view_of(engine_->act_ptr(mu, l), cfg.mb_rows, cols, engine_->act_ld(l));
+        return view_of(engine_->act_ptr(mu, l), cfg.mb_rows, boundary_cols(l), engine_->act_ld(l));
     }
     torch::Tensor dz(int mu, int l) {
         const auto& cfg = engine_->config();
-        const int cols = l == 0 ? cfg.layers[0].in : cfg.layers[l - 1].out;
-        return view_of(engine_->dz_ptr(mu, l), cfg.mb_rows, cols, engine_->act_ld(l));
+        return view_of(engine_->dz_ptr(mu, l), cfg.mb_rows, boundary_cols(l), engine_->act_ld(l));
     }
     torch::Tensor probs(int mu) {
         const auto& cfg = engine_->config();
@@ -299,6 +321,13 @@ public:
     std::vector<unsigned long long> chain_timeline() { return engine_->chain_timeline(); }
 
 private:
+    // features at layer boundary l (l = 0: the stage's input; a stage without Linears has only that one, in_dim wide)
+    int boundary_cols(int l) const {
+        const auto& cfg = engine_->config();
+        TORCH_CHECK(l >= 0 && l <= (int)cfg.layers.size(), "PipeEngine: layer boundary ", l, " out of range");
+        if (l > 0) return cfg.layers[l - 1].out;
+        return cfg.layers.empty() ? cfg.in_dim : cfg.layers[0].in;
+    }
     torch::Tensor weights_, grads_;
     c10::optional<torch::Tensor> momentum_;   // kept alive: the plan holds raw pointers into it
     std::pair<c10::optional<torch::Tensor>, c10::optional<torch::Tensor>> held_[2];
@@ -347,7 +376,9 @@ void bind_runtime(py::module_& m) {
         .def(py::init<int, int, int, int, bool, bool>())
         .def("export_handles", &PyPpContext::export_handles)
         .def("open_prev", &PyPpContext::open_prev)
-        .def("open_next", &PyPpContext::open_next);
+        .def("open_next", &PyPpContext::open_next)
+        .def("open_local", &PyPpContext::open_local, py::arg("prev"), py::arg("next"))
+        .def("buffers", &PyPpContext::buffers);
     py::class_<PyEngine>(m, "PipeEngine")
         .def(py::init<const std::vector<std::tuple<int, int, int, int64_t, int>>&, py::dict, torch::Tensor, torch::Tensor,
                       c10::optional<torch::Tensor>>(),

@@ -69,4 +69,21 @@ void PpContext::open_next(const std::string& handles) {
     next_flags_ = (uint32_t*)p[2];
 }
 
+void PpContext::open_local(const PpContext* prev, const PpContext* next) {
+    if (prev != nullptr) {
+        if (first_) throw std::runtime_error("PpContext: the first stage has no predecessor");
+        if (prev->ld_out_ != ld_in_ || prev->n_mu_ != n_mu_ || prev->mb_ != mb_)
+            throw std::runtime_error("PpContext::open_local: the predecessor's geometry does not match this stage");
+        prev_dz_in_ = prev->dz_in_;
+        prev_flags_ = prev->flags_;
+    }
+    if (next != nullptr) {
+        if (last_) throw std::runtime_error("PpContext: the last stage has no successor");
+        if (next->ld_in_ != ld_out_ || next->n_mu_ != n_mu_ || next->mb_ != mb_)
+            throw std::runtime_error("PpContext::open_local: the successor's geometry does not match this stage");
+        next_act_in_ = next->act_in_;
+        next_flags_ = next->flags_;
+    }
+}
+
 }  // namespace ssb

@@ -28,6 +28,9 @@ public:
     std::string export_handles() const;                        // 3 cudaIpcMemHandle_t: act_in, dz_in, flags
     void open_prev(const std::string& handles);                // stage s-1's export
     void open_next(const std::string& handles);                // stage s+1's export
+    // test-facing: neighbours that are contexts of this process (CUDA IPC refuses the caller's own allocations); prev is
+    // null on the first stage, next on the last
+    void open_local(const PpContext* prev, const PpContext* next);
 
     // local views
     float* act_in() const { return act_in_; }
@@ -38,6 +41,7 @@ public:
     const uint32_t* dz_arrived(int mu) const { return flags_ + kMaxMu + mu; }
     const uint32_t* act_credit() const { return flags_ + 2 * kMaxMu; }          // written by next: my act pushes may reuse its slots
     const uint32_t* dz_credit() const { return flags_ + 2 * kMaxMu + 32; }      // written by prev
+    const uint32_t* flags() const { return flags_; }                            // all kFlagWords words
     // neighbour views (nullptr when there is no such neighbour)
     float* next_act_in(int mu) const { return next_act_in_ ? next_act_in_ + (size_t)mu * mb_ * ld_out_ : nullptr; }
     uint32_t* next_act_arrived(int mu) const { return next_flags_ ? next_flags_ + mu : nullptr; }

@@ -221,6 +221,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         const bool ok = ssb::chain_budget(mb_rows, split, &kps, &stages, &smem);
         return std::make_tuple(ok, kps, stages, smem);
     });
+    // tiles of one grouped weight gradient, no GPU needed: ([(m0, n0, rows, cols, owns_bias)], stages, smem bytes per CTA)
+    m.def("wgrad_group_tiles", [](int out, int in, int rows) {
+        std::vector<ssb::GemmGroupTile> tiles;
+        int stages = 0, smem = 0;
+        if (const char* e = ssb::gemm_group_tiles(out, in, rows, &tiles, &stages, &smem)) throw std::invalid_argument(e);
+        std::vector<std::tuple<int, int, int, int, bool>> list;
+        for (const auto& t : tiles) list.emplace_back(t.m0, t.n0, t.rows, t.cols, t.owns_bias);
+        return std::make_tuple(list, stages, smem);
+    });
     m.def("chain_cluster_budget", [](int mb_rows, int cluster, bool split) {
         int kps = 0, stages = 0, smem = 0;
         const bool ok = ssb::chain_cluster_budget(mb_rows, cluster, split, &kps, &stages, &smem);

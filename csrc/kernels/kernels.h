@@ -104,12 +104,21 @@ int gemm_splitk_choice(const GemmPlan& plan, int num_sms);
 size_t gemm_splitk_workspace_floats(const GemmPlan& plan, int k_splits);
 const char* gemm_plan_enable_splitk(GemmPlan* plan, int k_splits, float* workspace, unsigned int* counters);
 cudaError_t gemm_launch(const GemmPlan& plan, cudaStream_t stream);
-// Grouped launch of several WGRAD plans (different layers) as ONE grid: a device table holds one entry per CTA.
+// Grouped launch of several WGRAD plans (different layers) as ONE grid: a device table holds one entry per CTA.  Only
+// the GEMMs of chain-eligible stages are grouped (out <= 128, any in); they run on narrow tiles of 32 output features x
+// 32 input columns with the full K (rows) in one CTA, instead of the per-layer kernel's 128 x 64.
 struct alignas(128) GemmGroupEntry {
-    CUtensorMap tmA, tmB, tmC;
-    GemmParams p;
+    CUtensorMap tmA, tmB, tmC;     // tmC: the narrow tile's 32-row box over G (or W with the SGD update fused)
+    GemmParams p;                  // the layer's plan with the narrow tile's block_n and ring depth
     int bx, by;                    // tile coordinates of this CTA inside its GEMM
 };
+struct GemmGroupTile {
+    int m0, n0, rows, cols;        // output features m0 .. m0 + rows - 1, input columns n0 .. n0 + cols - 1 (clipped at out, in)
+    bool owns_bias;                // the last column tile of its feature tile: the only one that writes the bias column
+};
+// Tiles of one grouped [out, in] weight gradient over `rows` micro-batch rows (appended to *tiles), the ring depth and the
+// dynamic shared memory of one CTA.  Host arithmetic only; nullptr or an error (out > 128 is rejected).
+const char* gemm_group_tiles(int out, int in, int rows, std::vector<GemmGroupTile>* tiles, int* stages, int* smem_bytes);
 struct GemmGroupPlan {
     GemmGroupEntry* entries_dev;
     int n, smem_bytes, n_gemms;

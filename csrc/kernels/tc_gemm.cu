@@ -7,6 +7,7 @@
 //                               swizzled stages, then fused bias / ReLU / ReLU-mask / grad-accumulate / SGD and
 //                               coalesced global stores.  During the WGRAD main loop these warps also reduce
 //                               db = colsum(dZ) from the staged A tiles (exact fp32, no extra pass over dZ).
+//               The grouped weight-gradient kernel runs the same body on 32-row tiles, the warps splitting the columns.
 //
 // Operand staging (all tiles are 32 fp32 = 128 B wide, the SWIZZLE_128B span):
 //   K-major  tile: one TMA box [rows x 32 k]                       -> rows 128 B apart
@@ -30,6 +31,10 @@ static constexpr int kMaxBlockN = 64;                   // a math warp holds a 3
 static constexpr uint32_t kBlockK = 32;                 // fp32 elements = 128 B
 static constexpr uint32_t kABytes = kBlockM * 128;      // 16 KB per stage
 static constexpr uint32_t kPanelBytes = 32 * 128;       // MN-major panel: 32 k-rows x 128 B
+// grouped weight-gradient launch: [kGroupBM features x kGroupBlockN input columns] tiles, the full K in every CTA
+static constexpr int kGroupBM = 32;
+static constexpr int kGroupBlockN = 32;
+static constexpr int kGroupMinCtas = 3;                 // CTAs per SM the grouped kernel is compiled for
 
 // SPLITK (FWD / DGRAD only, wide layers with few output tiles): blockIdx.z owns a contiguous range of
 // k-blocks; every CTA writes its raw fp32 accumulator tile to a workspace and the LAST CTA to arrive at the
@@ -39,11 +44,20 @@ static constexpr uint32_t kPanelBytes = 32 * 128;       // MN-major panel: 32 k-
 // layers' tiles in ONE launch, tensor maps and parameters read from a device table).
 // STATEFUL (WGRAD with fuse_sgd only): the SGD update uses momentum / weight decay (GemmParams::V, ...); the false
 // instantiations are the plain w -= lr * dW code.
-template <int MODE, bool SPLITK, bool STATEFUL = false>
+// BM: output rows (features) of the tile.  128: the per-layer kernels, math warp q owns rows 32q .. 32q+31 and all block_n
+// columns.  kGroupBM = 32 (WGRAD only): the grouped launch, every math warp owns all 32 rows and a quarter of the columns,
+// so that the few k-blocks of a narrow stage spread over many small CTAs instead of a few long warps.  Each output element
+// goes through the same warp_mma_kblock arithmetic in both forms.
+template <int MODE, bool SPLITK, bool STATEFUL = false, int BM = (int)kBlockM>
 __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
                                              const GemmParams& p, const int bx, const int by, const int bz) {
     constexpr bool A_MN = (MODE != GEMM_FWD);
     constexpr bool B_MN = (MODE == GEMM_WGRAD);
+    static_assert(BM == (int)kBlockM || (BM == kGroupBM && MODE == GEMM_WGRAD && !SPLITK), "narrow tiles are WGRAD only");
+    constexpr int kWarpsM = BM / 32;                       // math warps along the tile's rows ...
+    constexpr int kWarpsN = 4 / kWarpsM;                   // ... and along its columns
+    constexpr int NT = kMaxBlockN / 8 / kWarpsN;           // n8 tiles a math warp holds at most
+    constexpr uint32_t kATile = (uint32_t)BM * 128u;       // A bytes per stage
 
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
@@ -51,7 +65,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
     uint8_t* smem_gen = smem_raw + (smem_base - raw);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m0 = bx * kBlockM;
+    const int m0 = bx * BM;
     const int n0 = by * p.block_n;
     int num_kb = (p.k_total + kBlockK - 1) / kBlockK;
     int kb0 = 0;                                           // first k-block of this CTA
@@ -60,10 +74,10 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
         kb0 = bz * per;
         num_kb = min(per, num_kb - kb0);
     }
-    const uint32_t stage_bytes = kABytes + p.block_n * 128u;    // [A][B]
-    // WGRAD stages its output tile (block_n/32 swizzled panels of [128 rows x 128 B]) behind the ring
+    const uint32_t stage_bytes = kATile + p.block_n * 128u;     // [A][B]
+    // WGRAD stages its output tile (block_n/32 swizzled panels of [BM rows x 128 B]) behind the ring
     const uint32_t epi_base = smem_base + p.stages * stage_bytes;
-    const uint32_t epi_bytes = (MODE == GEMM_WGRAD) ? (uint32_t)p.block_n * 512u : 0u;
+    const uint32_t epi_bytes = (MODE == GEMM_WGRAD) ? (uint32_t)p.block_n * (uint32_t)BM * 4u : 0u;
     const uint32_t bar_base = epi_base + epi_bytes;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
@@ -95,13 +109,13 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             if (elect_one()) {
                 mbar_arrive_expect_tx(full_bar(s), stage_bytes);
                 const uint32_t a_dst = smem_base + s * stage_bytes;
-                const uint32_t b_dst = a_dst + kABytes;
+                const uint32_t b_dst = a_dst + kATile;
                 const int k0 = (kb0 + kb) * kBlockK;
                 if (!A_MN) {
                     tma_load_2d(a_dst, &tmA, full_bar(s), k0, m0);
                 } else {
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) tma_load_2d(a_dst + i * kPanelBytes, &tmA, full_bar(s), m0 + 32 * i, k0);
+                    for (int i = 0; i < BM / 32; ++i) tma_load_2d(a_dst + i * kPanelBytes, &tmA, full_bar(s), m0 + 32 * i, k0);
                 }
                 if (!B_MN) {
                     tma_load_2d(b_dst, &tmB, full_bar(s), k0, n0);
@@ -114,16 +128,20 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
         }
     } else {
         // ------------------------------------------------------------ math + epilogue warps
-        // warp w owns the 32 output rows q*32 .. q*32+31 of the tile (all block_n columns): tensor-core MMAs from the
-        // staged tiles into registers, then one row per lane (warp_acc_row16) for the fused epilogue.
+        // warp w owns 32 output rows and nt n8 tiles of the tile (BM = 128: rows q*32 .. q*32+31, all block_n columns;
+        // BM = 32: all rows, columns nw0 .. nw0 + 8*nt - 1): tensor-core MMAs from the staged tiles into registers, then
+        // one row per lane (warp_acc_row16) for the fused epilogue.
         const int q = warp & 3;
-        const int m_local = q * 32 + lane;
+        const int m_local = (q % kWarpsM) * 32 + lane;
         const int m = m0 + m_local;
         const bool m_ok = m < p.m_total;
-        const int nt = p.block_n / 8;
-        constexpr int kChunks = kMaxBlockN / 16;
+        const int nt = p.block_n / 8 / kWarpsN;
+        const int nw0 = (q / kWarpsM) * 8 * nt;
+        constexpr int kChunks = NT / 2;
+        // the column sum db runs in one lane per row: in the warps of the first column quarter
+        const bool db_warp = db_active && q / kWarpsM == 0;
 
-        float acc[2][kMaxBlockN / 8][4];
+        float acc[2][NT][4];
         warp_acc_zero(acc);
         float dbsum = 0.f;
         // the fused update's learning rate, loaded before the main loop so that its latency hides under the GEMM.  The
@@ -135,11 +153,12 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             const uint32_t ph = (kb / p.stages) & 1;
             mbar_wait(full_bar(s), ph);
             const uint32_t a_src = smem_base + s * stage_bytes;
+            const uint32_t m_base = (uint32_t)(m_local - lane);
             if (p.split)
-                warp_mma_kblock<kMaxBlockN / 8, A_MN, B_MN, true>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, nt, lane);
+                warp_mma_kblock<NT, A_MN, B_MN, true>(acc, a_src, m_base, a_src + kATile, (uint32_t)nw0, nt, lane);
             else
-                warp_mma_kblock<kMaxBlockN / 8, A_MN, B_MN, false>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, nt, lane);
-            if (MODE == GEMM_WGRAD && db_active) {
+                warp_mma_kblock<NT, A_MN, B_MN, false>(acc, a_src, m_base, a_src + kATile, (uint32_t)nw0, nt, lane);
+            if (MODE == GEMM_WGRAD && db_warp) {
                 // db[m] = sum over micro-batch rows of dZ[row, m], read from the staged A panels (exact fp32)
 #pragma unroll 8
                 for (int r = 0; r < 32; ++r) dbsum += lds_f32(a_src + operand_off<true>((uint32_t)m_local, (uint32_t)r));
@@ -254,26 +273,30 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             // 16 values into the step direction d (sgd_direction) - reading and writing its V entries, and reading W
             // only with weight decay - before the same -lr scaling and reduce-add.  Columns >= n_total get d = 0 and
             // are never stored: column n_total is the bias slot, which the bias path below updates.
+            // Columns at or past n_lim are not this warp's (or not real): d = 0, no V / W access, and 8-column warps of the
+            // narrow tile stage only their own half of a 16-column chunk.
             const float lr = STATEFUL ? *p.lr : lr_pre;            // STATEFUL implies fuse_sgd
             const float scale = p.fuse_sgd ? -lr : 1.f;
+            const int wcols = 8 * nt;
+            const int n_lim = min(p.n_total, n0 + nw0 + wcols);
 #pragma unroll
             for (int ch = 0; ch < kChunks; ++ch) {
-                if (16 * ch >= p.block_n) break;
+                if (16 * ch >= wcols) break;
                 float v[16];
                 warp_acc_row16(acc, ch, v, lane);
                 if constexpr (STATEFUL) {
-                    const int nc = n0 + 16 * ch;
+                    const int nc = n0 + nw0 + 16 * ch;
                     const bool has_v = p.V != nullptr, has_wd = p.weight_decay != 0.f;
                     float vm[16], wv[16];
 #pragma unroll
                     for (int j = 0; j < 16; ++j) { vm[j] = 0.f; wv[j] = 0.f; }
                     // all loads in flight before any use; 16-byte accesses where all 4 columns are real (V and W rows
-                    // are 16-byte aligned: TMA-legal pitch, nc a multiple of 16)
+                    // are 16-byte aligned: TMA-legal pitch, nc a multiple of 8)
                     if (m_ok) {
                         const size_t row = (size_t)m * p.ldw + nc;
 #pragma unroll
                         for (int q4 = 0; q4 < 4; ++q4) {
-                            if (nc + 4 * q4 + 3 < p.n_total) {
+                            if (nc + 4 * q4 + 3 < n_lim) {
                                 if (has_v) {
                                     const float4 t = *reinterpret_cast<const float4*>(p.V + row + 4 * q4);
                                     vm[4 * q4] = t.x; vm[4 * q4 + 1] = t.y; vm[4 * q4 + 2] = t.z; vm[4 * q4 + 3] = t.w;
@@ -286,7 +309,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
 #pragma unroll
                                 for (int e = 0; e < 4; ++e) {
                                     const int j = 4 * q4 + e;
-                                    if (nc + j < p.n_total) {
+                                    if (nc + j < n_lim) {
                                         if (has_v) vm[j] = p.V[row + j];
                                         if (has_wd) wv[j] = p.W[row + j];
                                     }
@@ -296,7 +319,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                     }
 #pragma unroll
                     for (int j = 0; j < 16; ++j) {
-                        const bool ok = m_ok && nc + j < p.n_total;
+                        const bool ok = m_ok && nc + j < n_lim;
                         const float d = sgd_direction<false>(v[j], wv[j], vm[j], p.momentum, p.weight_decay, p.nesterov != 0);
                         v[j] = ok ? d : 0.f;
                     }
@@ -304,21 +327,23 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                         const size_t row = (size_t)m * p.ldw + nc;
 #pragma unroll
                         for (int q4 = 0; q4 < 4; ++q4) {
-                            if (nc + 4 * q4 + 3 < p.n_total) {
+                            if (nc + 4 * q4 + 3 < n_lim) {
                                 *reinterpret_cast<float4*>(p.V + row + 4 * q4) =
                                     make_float4(vm[4 * q4], vm[4 * q4 + 1], vm[4 * q4 + 2], vm[4 * q4 + 3]);
                             } else {
 #pragma unroll
                                 for (int e = 0; e < 4; ++e)
-                                    if (nc + 4 * q4 + e < p.n_total) p.V[row + 4 * q4 + e] = vm[4 * q4 + e];
+                                    if (nc + 4 * q4 + e < n_lim) p.V[row + 4 * q4 + e] = vm[4 * q4 + e];
                             }
                         }
                     }
                 }
-                const uint32_t prow = epi_base + (ch >> 1) * (kBlockM * 128u) + (uint32_t)m_local * 128u;
 #pragma unroll
                 for (int q4 = 0; q4 < 4; ++q4) {
-                    const uint32_t chunk = (uint32_t)((ch & 1) * 4 + q4) ^ ((uint32_t)m_local & 7u);
+                    if (16 * ch + 4 * q4 >= wcols) break;
+                    const uint32_t c = (uint32_t)(nw0 + 16 * ch + 4 * q4);       // tile column of v[4 * q4]
+                    const uint32_t chunk = ((c >> 2) & 7u) ^ ((uint32_t)m_local & 7u);
+                    const uint32_t prow = epi_base + (c >> 5) * ((uint32_t)BM * 128u) + (uint32_t)m_local * 128u;
                     asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(prow + (chunk << 4)),
                                  "f"(v[4 * q4] * scale), "f"(v[4 * q4 + 1] * scale), "f"(v[4 * q4 + 2] * scale),
                                  "f"(v[4 * q4 + 3] * scale)
@@ -331,7 +356,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                 const bool add = p.accumulate || p.fuse_sgd;
                 for (int pj = 0; pj < p.block_n / 32; ++pj) {
                     if (n0 + pj * 32 >= p.n_total) break;
-                    const uint32_t src = epi_base + pj * (kBlockM * 128u);
+                    const uint32_t src = epi_base + pj * ((uint32_t)BM * 128u);
                     if (add) tma_reduce_add_2d(&tmC, src, n0 + pj * 32, m0);
                     else tma_store_2d(&tmC, src, n0 + pj * 32, m0);
                 }
@@ -344,7 +369,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             // store retired, by this CTA only when it owns the last column tile: a CTA of another column tile could not
             // order its write against that store, and a plain (non-accumulating) store there would erase it.
             asm volatile("bar.sync 1, 128;" ::: "memory");
-            if (db_active && m_ok) {
+            if (db_warp && m_ok) {
                 if (p.fuse_sgd) {
                     const size_t boff = (size_t)m * p.ldw + (p.db - p.G);  // bias lives at the same offset in W (and V)
                     float* bp = p.W + boff;
@@ -374,12 +399,14 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
 // ---- grouped weight-gradient launch: the tiles of SEVERAL layers' WGRAD GEMMs in one grid (one table entry per CTA).
 // Removes the fork / join of one graph node per layer from the end of a step: with the zero-copy loss the fp32 training
-// step of a narrow stage is chain kernel -> grouped wgrad (+SGD) (or chain || LL kernel under DP).
+// step of a narrow stage is chain kernel -> grouped wgrad (+SGD) (or chain || LL kernel under DP).  The GEMMs of a narrow
+// stage have few k-blocks and at most 128 outputs, so the launch runs on narrow [32 x 32] tiles (gemm_group_tiles): several
+// small CTAs per SM, each warp with an eighth of the per-layer kernel's MMAs.
 template <bool STATEFUL = false>
-__global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const GemmGroupEntry* __restrict__ entries) {
+__global__ void __launch_bounds__(kThreads, kGroupMinCtas) tc_wgrad_group_kernel(const GemmGroupEntry* __restrict__ entries) {
     const GemmGroupEntry& e = entries[blockIdx.x];
     const GemmParams p = e.p;                      // private copy: the body reads these fields in every loop
-    tc_gemm_body<GEMM_WGRAD, false, STATEFUL>(e.tmA, e.tmB, e.tmC, p, e.bx, e.by, 0);
+    tc_gemm_body<GEMM_WGRAD, false, STATEFUL, kGroupBM>(e.tmA, e.tmB, e.tmC, p, e.bx, e.by, 0);
 }
 
 // =========================================================================== host side
@@ -556,6 +583,22 @@ const char* gemm_plan_enable_splitk(GemmPlan* plan, int k_splits, float* workspa
     return nullptr;
 }
 
+const char* gemm_group_tiles(int out, int in, int rows, std::vector<GemmGroupTile>* tiles, int* stages, int* smem_bytes) {
+    if (out < 1 || in < 1 || rows < 1) return "gemm_group_tiles: empty GEMM";
+    if (out > (int)kBlockM) return "gemm_group_tiles: grouped weight gradients need out <= 128 (chain-eligible stages)";
+    const int block_n = kGroupBlockN;
+    const int num_kb = (rows + (int)kBlockK - 1) / (int)kBlockK;
+    const int stage_bytes = kGroupBM * 128 + block_n * 128;
+    const int epi_bytes = kGroupBM * block_n * 4;
+    int s = num_kb < 6 ? num_kb : 6;
+    *stages = s;
+    *smem_bytes = s * stage_bytes + epi_bytes + 1024 /*align slack*/ + 8 * (2 * s) + 16;
+    const int tiles_n = (in + block_n - 1) / block_n;
+    for (int m0 = 0; m0 < out; m0 += kGroupBM)
+        for (int t = 0; t < tiles_n; ++t) tiles->push_back(GemmGroupTile{m0, t * block_n, kGroupBM, block_n, t == tiles_n - 1});
+    return nullptr;
+}
+
 const char* gemm_group_plan(GemmGroupPlan* out, const GemmPlan* plans, int n_plans) {
     *out = GemmGroupPlan{};
     if (n_plans < 1) return "gemm_group_plan: no plans";
@@ -567,15 +610,22 @@ const char* gemm_group_plan(GemmGroupPlan* out, const GemmPlan* plans, int n_pla
         if (g.mode != GEMM_WGRAD) return "gemm_group_plan: only weight-gradient GEMMs can be grouped";
         if (g.p.k_splits > 1) return "gemm_group_plan: split-K plans cannot be grouped";
         if (is_stateful(g.p) != stateful) return "gemm_group_plan: plans mix the plain and the stateful SGD rule";
-        if (g.smem_bytes > smem) smem = g.smem_bytes;
-        for (unsigned by = 0; by < g.grid.y; ++by)
-            for (unsigned bx = 0; bx < g.grid.x; ++bx) {
-                GemmGroupEntry e;
-                memset(&e, 0, sizeof(e));
-                e.tmA = g.tmA; e.tmB = g.tmB; e.tmC = g.tmC;
-                e.p = g.p; e.bx = (int)bx; e.by = (int)by;
-                host.push_back(e);
-            }
+        std::vector<GemmGroupTile> tiles;
+        int stages = 0, bytes = 0;
+        if (const char* e = gemm_group_tiles(g.p.m_total, g.p.n_total, g.p.k_total, &tiles, &stages, &bytes)) return e;
+        if (bytes > smem) smem = bytes;
+        // the output map of the narrow tile: a 32-row box over the same [out, in] block
+        CUtensorMap tmC;
+        const bool to_w = g.p.fuse_sgd != 0;
+        if (const char* e = make_tmap(&tmC, to_w ? g.p.W : g.p.G, g.p.n_total, g.p.m_total, to_w ? g.p.ldw : g.p.ldg, kGroupBM)) return e;
+        for (const GemmGroupTile& t : tiles) {
+            GemmGroupEntry e;
+            memset(&e, 0, sizeof(e));
+            e.tmA = g.tmA; e.tmB = g.tmB; e.tmC = tmC;
+            e.p = g.p; e.p.block_n = t.cols; e.p.stages = stages;
+            e.bx = t.m0 / t.rows; e.by = t.n0 / t.cols;       // the body derives the bias owner from by (last column tile)
+            host.push_back(e);
+        }
     }
     GemmGroupEntry* dev = nullptr;
     if (cudaMalloc(&dev, host.size() * sizeof(GemmGroupEntry)) != cudaSuccess) return "gemm_group_plan: cudaMalloc failed";
@@ -608,6 +658,9 @@ cudaError_t gemm_configure() {
     if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_WGRAD, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    // the narrow tiles are meant to share an SM: ask for the carveout that fits the most of them
+    if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_FWD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_DGRAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     g_configured = true;

@@ -18,11 +18,13 @@
 // general path (wide layers) and compute the weight gradients afterwards.
 //
 // Cluster form (CLUSTER, C = ChainParams::cluster CTAs per micro-batch): CTA rank c of the micro-batch's thread-block
-// cluster owns output features [32c, 32c + 32) of every GEMM and streams only that slice of each weight matrix.  Its
-// eight math warps split the k-blocks four ways (warp (q, half) takes the k-blocks kb with kb % 4 == q, for its half of
-// the rows) and add the four partial sums through shared memory in a fixed order.  The 32-feature output is exactly one
-// K-major panel of the next GEMM's B operand: it is written locally and copied into the same offset of every peer
-// (cp.async.bulk shared::cta -> shared::cluster, completion counted on the peer's per-buffer mbarrier).
+// cluster owns output features [32c, 32c + 32) of every GEMM and streams only that slice of each weight matrix.  In a
+// GEMM of at most 4 k-blocks (every GEMM but a first layer with more than 128 inputs) each of the eight math warps owns
+// m16n8 tiles of that output (chain_tile_lo), runs them over all k-blocks and runs their epilogue on its own fragments.
+// A longer GEMM splits its k-blocks four ways (warp (q, half) takes the k-blocks kb with kb % 4 == q, for its half of
+// the rows) and adds the four partial sums through shared memory in a fixed order.  The 32-feature output is exactly one
+// K-major panel of the next GEMM's B operand: it is written locally, and each warp stores its block of it into the same
+// offset of every peer (st.async, completion counted on the peer's per-buffer mbarrier; see exchange).
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -37,7 +39,55 @@ static constexpr uint32_t kABytes = kBlockM * 128;
 static constexpr uint32_t kPanelBytes = 32 * 128;
 static constexpr int kScratchLd = 33;                     // odd pitch: conflict-free row-per-lane access
 // columns (micro-batch rows) of one math warp: 16 * ceil(N / 32) <= 64
-static int chain_warp_cols(int n_pad) { return 16 * ((n_pad / 16 + 1) / 2); }
+static constexpr int chain_warp_cols(int n_pad) { return 16 * ((n_pad / 16 + 1) / 2); }
+
+// CLUSTER, full-K form: the CTA's 32 x N output is 2 x N/8 m16n8 tiles.  Math warp w (0..7) owns the m16 slab w & 1
+// (features 16 (w & 1) .. +15 of the CTA's 32) and the n8 tiles [chain_tile_lo(N/8, w >> 1), chain_tile_lo(N/8, (w >> 1) + 1))
+// of it: a quarter of the rows, contiguous, so that the tiles are one warp_mma_kblock block.
+__host__ __device__ constexpr int chain_tile_lo(int nj, int quarter) { return nj * quarter / 4; }
+// Every byte of a CTA's panel (N rows x 128 B) is in exactly one warp's tiles, so the bytes a peer receives from this
+// CTA's senders in one exchange are the N * 128 it armed its recv_bar with for this CTA; and no warp owns more n8
+// tiles than the NTW / 2 its accumulator holds.
+constexpr bool chain_tiles_cover_panel() {
+    for (int n_pad = 16; n_pad <= 128; n_pad += 16) {
+        const int cols = chain_warp_cols(n_pad), ntw = cols <= 16 ? 2 : cols <= 32 ? 4 : 8, nj = n_pad / 8;
+        int bytes = 0;
+        for (int w = 0; w < 8; ++w) {
+            const int tiles = chain_tile_lo(nj, (w >> 1) + 1) - chain_tile_lo(nj, w >> 1);
+            if (tiles > ntw / 2) return false;
+            bytes += tiles * 8 * 64;                      // 8 rows x 16 features x 4 B
+        }
+        if (bytes != n_pad * 128) return false;
+    }
+    return true;
+}
+static_assert(chain_tiles_cover_panel(), "the full-K tiles of the 8 math warps must cover the CTA's panel exactly once");
+
+// CLUSTER, full-K form: the cnt (= CNT when it is a template argument) k-blocks of one ring stage on this warp's tiles.
+// The k-block products are independent, so the unrolled CNT forms overlap them; the k-block sums are added into acc in
+// k-block order either way.  a: K-major / MN-major 32-feature weight panels, kPanelBytes apart; b: activation panels.
+template <int NT, bool A_MN, bool SPLIT, int CNT>
+__device__ __forceinline__ void tile_kblocks(float (&acc)[1][NT][4], int cnt, uint32_t a_src, uint32_t b_src, uint32_t b_step,
+                                             uint32_t m_base, uint32_t n_base, int nt, int lane) {
+#pragma unroll
+    for (int j = 0; j < (CNT > 0 ? CNT : 4); ++j)
+        if (CNT > 0 || j < cnt)
+            warp_mma_kblock<NT, A_MN, false, SPLIT, 1>(acc, a_src + j * kPanelBytes, m_base, b_src + j * b_step, n_base, nt, lane);
+}
+template <int NT, bool A_MN, bool SPLIT>
+__device__ __forceinline__ void tile_stage(float (&acc)[1][NT][4], int cnt, uint32_t a_src, uint32_t b_src, uint32_t b_step,
+                                           uint32_t m_base, uint32_t n_base, int nt, int lane) {
+    if (nt == NT) {                                       // every tile of the accumulator: constant bounds throughout
+        switch (cnt) {
+            case 4: tile_kblocks<NT, A_MN, SPLIT, 4>(acc, 4, a_src, b_src, b_step, m_base, n_base, NT, lane); break;
+            case 3: tile_kblocks<NT, A_MN, SPLIT, 3>(acc, 3, a_src, b_src, b_step, m_base, n_base, NT, lane); break;
+            case 2: tile_kblocks<NT, A_MN, SPLIT, 2>(acc, 2, a_src, b_src, b_step, m_base, n_base, NT, lane); break;
+            default: tile_kblocks<NT, A_MN, SPLIT, 1>(acc, 1, a_src, b_src, b_step, m_base, n_base, NT, lane); break;
+        }
+    } else if (nt > 0) {
+        tile_kblocks<NT, A_MN, SPLIT, 0>(acc, cnt, a_src, b_src, b_step, m_base, n_base, nt, lane);
+    }
+}
 
 __device__ __forceinline__ float warp_sum_f(float v) {
 #pragma unroll
@@ -187,8 +237,10 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         // MMAs of exactly the block its epilogue consumes, so accumulators never leave the warp's registers (lane r reads
         // feature row r through warp_acc_row16).  The activation tile of the next GEMM is written by all 8 warps and
         // published with one named barrier among them.
-        // CLUSTER: q is the warp's k-phase; every warp covers the CTA's 32 features and the (q == 0) warps run the
-        // epilogues on the reduced sums
+        // CLUSTER: a GEMM of more than 4 k-blocks (layer 1 with in > 128) runs in the k-phase form: q is the warp's
+        // k-phase, every warp covers the CTA's 32 features and the (q == 0) warps run the epilogues on the reduced sums.
+        // Every other GEMM runs in the full-K form: each warp owns its tiles (chain_tile_lo) over all k-blocks and runs
+        // their epilogue on its own fragments.
         const int q = warp & 3;
         const int half = (warp - 1) >> 2;
         const int m = (CLUSTER ? 32 * rank : q * 32) + lane;   // feature handled by this thread in the epilogue
@@ -198,6 +250,13 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         const int c_lo = 16 * ((n_chunks * half) / 2), c_hi = 16 * ((n_chunks * (half + 1)) / 2);
         const int nt = (c_hi - c_lo) / 8;
         float acc[2][NTW][4];                                // this warp's block of the current layer's product
+        // CLUSTER, full-K form: this warp's tiles (features t_f0 + g (+8) of fragment register r >> 1, rows
+        // t_n0 + 8 j + 2 (lane & 3) + (r & 1)) and their accumulators
+        const int t_m0 = 16 * ((warp - 1) & 1);              // first feature of the slab, of the CTA's 32
+        const int t_f0 = 32 * rank + t_m0 + (lane >> 2);     // feature of fragment registers 0, 1 (2, 3: +8)
+        const int t_j0 = chain_tile_lo(N / 8, (warp - 1) >> 1);
+        const int t_n0 = 8 * t_j0, tnt = chain_tile_lo(N / 8, ((warp - 1) >> 1) + 1) - t_j0;
+        float tacc[1][NTW / 2][4];
         int it = 0, gemm_i = 0;
         int wbuf = 0;                                        // activation buffer the NEXT epilogue writes
         uint32_t recv_phase = 0u;                            // CLUSTER: parity of recv_bar(b) in bit b
@@ -267,6 +326,32 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             ++gemm_i;
             if constexpr (CLUSTER) reduce_kphases();
         };
+        // CLUSTER, full-K form of run_gemm -> tacc: every k-block of this warp's tiles, summed in k-block order.  With
+        // at most 4 k-blocks that is the order reduce_kphases adds the k-phase partials in, so the two forms agree
+        // bit for bit.
+        auto run_gemm_tiles = [&](int nkb, bool a_mn, bool b_from_stage, uint32_t bsrc, bool skip) {
+            if (threadIdx.x == 32) DBG(1, 2 * gemm_i);
+            warp_acc_zero(tacc);
+            if (!b_from_stage) wait_recv((int)((bsrc - abuf0) / abuf_bytes));
+            for (int kb0 = 0; kb0 < nkb && !skip; kb0 += p.kps, ++it) {
+                const int cnt = min(p.kps, nkb - kb0);
+                const int s = it % p.stages;
+                mbar_wait(full_bar(s), (it / p.stages) & 1);
+                const uint32_t a_src = smem_base + s * stage_bytes;
+                const uint32_t b_src = b_from_stage ? a_src + stage_b_off : bsrc + kb0 * b_bytes;
+                if (a_mn)
+                    tile_stage<NTW / 2, true, SPLIT>(tacc, cnt, a_src, b_src, b_bytes, (uint32_t)t_m0, (uint32_t)t_n0, tnt, lane);
+                else
+                    tile_stage<NTW / 2, false, SPLIT>(tacc, cnt, a_src, b_src, b_bytes, (uint32_t)t_m0, (uint32_t)t_n0, tnt, lane);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty_bar(s));
+            }
+            if (threadIdx.x == 32) DBG(1, 2 * gemm_i + 1);
+            ++gemm_i;
+        };
+        // CLUSTER, full-K form: element r of this warp's tile j
+        auto t_row = [&](int j, int r) { return t_n0 + 8 * j + 2 * (lane & 3) + (r & 1); };
+        auto t_feat = [&](int r) { return t_f0 + 8 * (r >> 1); };
         auto st_tile = [&](uint32_t dst, int n, int feat, float x) {   // operand tile for the next GEMM
             *reinterpret_cast<float*>(smem_gen + (dst - smem_base) + act_smem_off(n, feat, b_bytes)) = x;
         };
@@ -282,27 +367,39 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             asm volatile("bar.sync 2, 256;" ::: "memory");
         };
         // CLUSTER, instead of publish() for a tile another GEMM consumes: this CTA's panel of abuf b goes to the same
-        // offset in every peer, and recv_bar(b) is armed for the (C - 1) panels coming in (awaited by run_gemm).  Every
-        // CTA sends its panel, features or not, so that every CTA takes part in every exchange.  That is what makes the
-        // ping-pong reuse safe without a cluster barrier per tile: a peer writes the tile after next into my abuf b only
-        // after it received my panel of the next tile (abuf b^1), and I send that panel only after my GEMM finished
-        // reading abuf b, which it started after all of this tile's panels had landed here.  By the same chain my copies
-        // out of abuf b have completed (their peers waited for them) before my epilogue writes abuf b again, and every
-        // copy into this CTA has landed before it reaches the cluster barrier at the end of the kernel.
-        auto exchange = [&](int b) {
-            fence_proxy_async_smem();                        // my st.shared of the panel -> the bulk copy's reads
-            publish();
-            if (threadIdx.x == 32) {
+        // offset in every peer, sent by the warps that wrote it.  A sending warp's block is rows [n0, n0 + rows) x the
+        // 16-byte chunks [ch0, ch0 + 2^lcpr) of each row; it reads the block back (each lane a chunk at a time) and
+        // stores it into every peer with st.async, each store counted as 16 bytes on the peer's recv_bar(b).  The
+        // blocks of one exchange cover the panel exactly once (chain_tiles_cover_panel), so every peer receives the
+        // (C - 1) * N * 128 bytes that one thread of it arms its recv_bar(b) with; run_gemm waits on that.
+        // Every CTA sends its whole panel, features or not, so that every CTA takes part in every exchange.  That is
+        // what makes the ping-pong reuse safe without a cluster barrier per tile.  A peer writes the tile after next
+        // into my abuf b in its epilogue after next, which follows its GEMM on the next tile (abuf b^1), which waited
+        // for all of my bytes of the next tile - those of every one of my warps.  Each of my warps sends its part of
+        // the next tile only after its own GEMM on this tile finished reading abuf b, so all of my warps are done
+        // with abuf b before any peer writes into it.  The same chain puts every byte of a tile on recv_bar(b) in the
+        // phase that is awaited for it, and every store into this CTA has landed before it reaches the cluster barrier
+        // at the end of the kernel.  The stores read registers, so my buffers carry no outgoing copy to wait for.
+        auto exchange = [&](int b, bool sender, int n0, int rows, int ch0, int lcpr) {
+            if (sender) {
+                __syncwarp();                                // the warp's st.shared of its block -> its lanes' reads
+                const uint32_t panel = abuf0 + (uint32_t)b * abuf_bytes + (uint32_t)rank * b_bytes;   // act_smem_off panel
                 const uint32_t bar = recv_bar(b);
-                const uint32_t src = abuf0 + (uint32_t)b * abuf_bytes + (uint32_t)rank * b_bytes;   // act_smem_off panel
-                mbar_arrive_expect_tx(bar, (uint32_t)(p.cluster - 1) * b_bytes);
-                for (int r = 0; r < p.cluster; ++r)
-                    if (r != rank) bulk_copy_s2cluster(mapa_shared(src, (uint32_t)r), src, b_bytes, mapa_shared(bar, (uint32_t)r));
+                for (int k = lane; k < (rows << lcpr); k += 32) {
+                    const int n = n0 + (k >> lcpr), c = ch0 + (k & ((1 << lcpr) - 1));
+                    const uint32_t src = panel + (uint32_t)n * 128u + ((uint32_t)(c ^ (n & 7)) << 4);
+                    const uint4 v = lds_v4(src);
+                    for (int r = 0; r < p.cluster; ++r)
+                        if (r != rank) st_async_v4(mapa_shared(src, (uint32_t)r), v, mapa_shared(bar, (uint32_t)r));
+                }
             }
+            publish();
+            if (threadIdx.x == 32) mbar_arrive_expect_tx(recv_bar(b), (uint32_t)(p.cluster - 1) * b_bytes);
         };
-        // end of a tile the next GEMM reads
-        auto hand_over = [&](int b) {
-            if constexpr (CLUSTER) exchange(b);
+        // end of a tile the next GEMM reads; CLUSTER: sender / n0 / rows / ch0 / lcpr describe this warp's block of it
+        // (see exchange)
+        auto hand_over = [&](int b, bool sender, int n0, int rows, int ch0, int lcpr) {
+            if constexpr (CLUSTER) exchange(b, sender, n0, rows, ch0, lcpr);
             else publish();
         };
         int buf = 0;                                         // activation buffer the NEXT gemm reads
@@ -340,15 +437,49 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 const float bias = m_ok ? __ldg(p.W + ly.w_off + (int64_t)m * ly.ldw + ly.in) : 0.f;
                 const bool is_logits = (l == L) && p.do_loss;
                 const int nkb_f = (ly.in + (int)kBlockK - 1) / (int)kBlockK;
+                const bool tile = CLUSTER && nkb_f <= 4;      // full-K form
+                float t_bias[2] = {0.f, 0.f};                // full-K form: the biases of features t_feat(0), t_feat(2)
+                if (tile) {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                        if (t_feat(2 * h) < ly.out) t_bias[h] = __ldg(p.W + ly.w_off + (int64_t)t_feat(2 * h) * ly.ldw + ly.in);
+                }
                 // layer 1 reads X from its ring slots (TMA), or - folded pipeline input - from abuf 1 (staged above)
                 const bool x_glob = FOLD && (l == 1) && p.x_from_global;
-                run_gemm(nkb_f, false, l == 1 && !x_glob, abuf0 + (x_glob ? 1 : buf) * abuf_bytes, idle(ly.out));
+                if (tile) run_gemm_tiles(nkb_f, false, l == 1, abuf0 + buf * abuf_bytes, idle(ly.out));
+                else run_gemm(nkb_f, false, l == 1 && !x_glob, abuf0 + (x_glob ? 1 : buf) * abuf_bytes, idle(ly.out));
                 if (l > 1) buf ^= 1;                         // layer l read buf, wrote buf^1
                 else buf = 0;                                // layer 1 writes abuf 0
                 if (p.sync_debug) asm volatile("bar.sync 2, 256;" ::: "memory");   // racecheck aid, see kernels.h
                 const uint32_t dst = abuf0 + wbuf * abuf_bytes;
                 float* __restrict__ gout = p.act[l] + (int64_t)row0 * p.act_ld[l];
-                if (!is_logits) {
+                if (!is_logits && tile) {
+                    // full-K form: bias, ReLU and the feature mask on this warp's fragments, 4 st.shared per tile into
+                    // the operand tile, this warp's block of it to the peers, then the global copy
+#pragma unroll
+                    for (int j = 0; j < NTW / 2; ++j) {
+                        if (j < tnt) {
+#pragma unroll
+                            for (int r = 0; r < 4; ++r) {
+                                float x = tacc[0][j][r] + t_bias[r >> 1];
+                                if (ly.relu) x = fmaxf(x, 0.f);
+                                x = t_feat(r) < ly.out ? x : 0.f;
+                                tacc[0][j][r] = x;
+                                st_tile(dst, t_row(j, r), t_feat(r), x);
+                            }
+                        }
+                    }
+                    if (l < L) hand_over(wbuf, true, t_n0, 8 * tnt, t_m0 / 4, 2);
+                    else publish();
+#pragma unroll
+                    for (int j = 0; j < NTW / 2; ++j)
+#pragma unroll
+                        for (int r = 0; r < 4; ++r)
+                            if (j < tnt && t_feat(r) < ly.out && t_row(j, r) < p.mb_rows)
+                                gout[(int64_t)t_row(j, r) * p.act_ld[l] + t_feat(r)] = tacc[0][j][r];
+                    wbuf ^= 1;
+                    if (l == 1) wbuf = 1;                    // layer 1 wrote abuf 0; layer 2 reads 0, writes 1
+                } else if (!is_logits) {
                     // one 16-row chunk per warp when N <= 32: write the operand tile for the next GEMM first,
                     // publish it, and only then drain the global copy (needed later by wgrad / the pipeline)
                     const bool single = (c_hi - c_lo == 16);
@@ -373,7 +504,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                             }
                         }
                     }
-                    if (l < L) hand_over(wbuf);
+                    if (l < L) hand_over(wbuf, epi, c_lo, c_hi - c_lo, 0, 3);
                     else publish();
                     if (epi && single && m_ok) {
 #pragma unroll
@@ -392,13 +523,20 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     // Step 1: the class-lane warps (q == 0, both halves) transpose logits (+bias) into a [row][class]
                     // scratch in smem.  Step 2: each lane of warp (0, 0) owns ROWS, loops over the <= 32 classes in
                     // registers - no cross-lane reductions except (MSE) one max and one sum for the whole micro-batch.
-                    // CLUSTER: the <= 32 classes are rank 0's features; the scratch is where the k-phase partials were
-                    // (all of them read before the barrier)
+                    // CLUSTER: the <= 32 classes are rank 0's features.  Full-K form: every warp transposes its own
+                    // tiles.  K-phase form: the scratch is where the k-phase partials were (all of them read before
+                    // the barrier)
                     const int C = ly.out;
                     float* scratch = reinterpret_cast<float*>(smem_gen + scratch_off);   // [N][kScratchLd]
                     float loss = 0.f;
-                    if constexpr (CLUSTER) asm volatile("bar.sync 2, 256;" ::: "memory");
-                    if (q == 0) {
+                    if constexpr (CLUSTER) { if (!tile) asm volatile("bar.sync 2, 256;" ::: "memory"); }
+                    if (tile) {
+#pragma unroll
+                        for (int j = 0; j < NTW / 2; ++j)
+#pragma unroll
+                            for (int r = 0; r < 4; ++r)
+                                if (j < tnt && t_feat(r) < C) scratch[t_row(j, r) * kScratchLd + t_feat(r)] = tacc[0][j][r] + t_bias[r >> 1];
+                    } else if (q == 0) {
 #pragma unroll
                         for (int ch = 0; ch < NTW / 2; ++ch) {
                             const int c = c_lo + 16 * ch;
@@ -540,7 +678,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         if (lane == 0 && p.loss != nullptr) p.loss[p.mu_base + mb] = loss * p.inv_batch;
                     }
                     if (p.do_bwd) {
-                        if (L >= bwd_lo) hand_over(wbuf);
+                        if (L >= bwd_lo) hand_over(wbuf, q == 0 && half == 0, 0, N, 0, 3);   // the head's warp: all N rows
                         else publish();
                         wbuf ^= 1;
                     }
@@ -572,7 +710,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 }
                 st_tile(dst, n, m, x);
             }
-            if (L >= bwd_lo) hand_over(wbuf);
+            if (L >= bwd_lo) hand_over(wbuf, epi, c_lo, c_hi - c_lo, 0, 3);
             else publish();
             wbuf ^= 1;
         }
@@ -584,6 +722,47 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 const bool mask_on = (l >= 2) && p.layers[l - 2].relu;
                 const float* __restrict__ yprev = p.act[l - 1] + (int64_t)row0 * p.act_ld[l - 1];
                 float* __restrict__ gprev = p.dz[l - 1] + (int64_t)row0 * p.act_ld[l - 1];
+                if constexpr (CLUSTER) {
+                    // full-K form (K = out <= 128: at most 4 k-blocks): the ReLU masks of this warp's fragments are
+                    // fetched before the MMAs, the epilogue runs on the fragments
+                    float t_mk[NTW / 2][4];
+#pragma unroll
+                    for (int j = 0; j < NTW / 2; ++j)
+#pragma unroll
+                        for (int r = 0; r < 4; ++r) {
+                            const int n = t_row(j, r), f = t_feat(r);
+                            t_mk[j][r] = (j < tnt && mask_on && f < ly.in && n < p.mb_rows) ? yprev[(int64_t)n * p.act_ld[l - 1] + f] : 1.f;
+                        }
+                    run_gemm_tiles((ly.out + (int)kBlockK - 1) / (int)kBlockK, true, false, abuf0 + buf * abuf_bytes, idle(ly.in));
+                    buf ^= 1;
+                    if (p.sync_debug) asm volatile("bar.sync 2, 256;" ::: "memory");   // racecheck aid, see kernels.h
+                    const uint32_t dst = abuf0 + wbuf * abuf_bytes;
+                    const bool more = (l > bwd_lo);          // another dgrad consumes this tile
+#pragma unroll
+                    for (int j = 0; j < NTW / 2; ++j) {
+                        if (j < tnt) {
+#pragma unroll
+                            for (int r = 0; r < 4; ++r) {
+                                float x = (t_mk[j][r] > 0.f) ? tacc[0][j][r] : 0.f;
+                                x = t_feat(r) < ly.in ? x : 0.f;
+                                tacc[0][j][r] = x;
+                                if (more) st_tile(dst, t_row(j, r), t_feat(r), x);
+                            }
+                        }
+                    }
+                    if (more) {
+                        hand_over(wbuf, true, t_n0, 8 * tnt, t_m0 / 4, 2);
+                        wbuf ^= 1;
+                    }
+#pragma unroll
+                    for (int j = 0; j < NTW / 2; ++j)
+#pragma unroll
+                        for (int r = 0; r < 4; ++r)
+                            if (j < tnt && t_feat(r) < ly.in && t_row(j, r) < p.mb_rows)
+                                gprev[(int64_t)t_row(j, r) * p.act_ld[l - 1] + t_feat(r)] = tacc[0][j][r];
+                    signal_ready(l - 1);
+                    continue;
+                }
                 // the masks do not depend on the MMA: fetch them before it runs (N <= 32: all of them)
                 float mk0[16];
                 const bool pre = (c_hi - c_lo == 16);        // N <= 32: one chunk per warp, prefetch its masks
@@ -627,7 +806,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     }
                 }
                 if (more) {
-                    hand_over(wbuf);
+                    hand_over(wbuf, epi, c_lo, c_hi - c_lo, 0, 3);
                     wbuf ^= 1;
                 }
                 if (epi && single && m_ok) {

@@ -110,11 +110,17 @@ __device__ __forceinline__ uint32_t mapa_shared(uint32_t smem_addr, uint32_t ran
 __device__ __forceinline__ void cluster_sync() {
     asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
 }
-// contiguous bulk copy from this CTA's shared memory into a peer's (dst and bar: shared::cluster addresses from
-// mapa_shared); completion is counted as `bytes` of transaction on the peer's mbarrier
-__device__ __forceinline__ void bulk_copy_s2cluster(uint32_t dst, uint32_t src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(dst), "r"(src), "r"(bytes), "r"(bar) : "memory");
+// 16 bytes from registers into a peer's shared memory (dst and bar: shared::cluster addresses from mapa_shared); the
+// store counts as 16 bytes of transaction on the peer's mbarrier, and a peer thread that observes that barrier's phase
+// complete also observes the data
+__device__ __forceinline__ void st_async_v4(uint32_t dst, uint4 v, uint32_t bar) {
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];"
+                 ::"r"(dst), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "r"(bar) : "memory");
+}
+__device__ __forceinline__ uint4 lds_v4(uint32_t addr) {
+    uint4 v;
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+    return v;
 }
 
 // ------------------------------------------------------------------ warp-level TF32 tensor-core tiles
@@ -153,22 +159,24 @@ __device__ __forceinline__ uint32_t tf32_hi_bits(float x) { return __float_as_ui
 // accumulator and then added to `acc` with an fp32 add, so the accumulated rounding error grows with the number of
 // 32-wide k-blocks, not with the number of MMA steps.  SPLIT: 3xTF32 products, the lo parts derived from the tile.
 // acc[i][j][r]: m16 tile i, n8 tile j, mma.sync C fragment register r (rows lane/4 (+8), columns 2*(lane%4) (+1)).
-template <int NT, bool A_MN, bool B_MN, bool SPLIT>
-__device__ __forceinline__ void warp_mma_kblock(float (&acc)[2][NT][4], uint32_t a_tile, uint32_t m_base, uint32_t b_tile,
+// MI: m16 tiles of the block (2: 32 rows of A, 1: the 16 rows m_base .. m_base+15).  Each (i, j) tile sees the same
+// instructions on the same operands whatever MI and NT are, so its sums do not depend on the block shape.
+template <int NT, bool A_MN, bool B_MN, bool SPLIT, int MI = 2>
+__device__ __forceinline__ void warp_mma_kblock(float (&acc)[MI][NT][4], uint32_t a_tile, uint32_t m_base, uint32_t b_tile,
                                                 uint32_t n_base, int nt, int lane) {
     const uint32_t g = (uint32_t)lane >> 2, t = (uint32_t)lane & 3u;
-    float part[2][NT][4];
+    float part[MI][NT][4];
 #pragma unroll
-    for (int i = 0; i < 2; ++i)
+    for (int i = 0; i < MI; ++i)
 #pragma unroll
         for (int j = 0; j < NT; ++j)
 #pragma unroll
             for (int r = 0; r < 4; ++r) part[i][j][r] = 0.f;
 #pragma unroll
     for (uint32_t k0 = 0; k0 < 32u; k0 += 8u) {
-        uint32_t ah[2][4], al[2][4];
+        uint32_t ah[MI][4], al[MI][4];
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
+        for (int i = 0; i < MI; ++i) {
             const uint32_t r0 = m_base + 16u * i + g;
             const float x[4] = {lds_f32(a_tile + operand_off<A_MN>(r0, k0 + t)), lds_f32(a_tile + operand_off<A_MN>(r0 + 8u, k0 + t)),
                                 lds_f32(a_tile + operand_off<A_MN>(r0, k0 + t + 4u)),
@@ -188,7 +196,7 @@ __device__ __forceinline__ void warp_mma_kblock(float (&acc)[2][NT][4], uint32_t
                 const uint32_t bh0 = tf32_hi_bits(y0), bh1 = tf32_hi_bits(y1);
                 const uint32_t bl0 = __float_as_uint(y0 - __uint_as_float(bh0)), bl1 = __float_as_uint(y1 - __uint_as_float(bh1));
 #pragma unroll
-                for (int i = 0; i < 2; ++i) {
+                for (int i = 0; i < MI; ++i) {
                     if (SPLIT) {
                         mma_tf32(part[i][j], al[i], bh0, bh1);
                         mma_tf32(part[i][j], ah[i], bl0, bl1);
@@ -199,17 +207,17 @@ __device__ __forceinline__ void warp_mma_kblock(float (&acc)[2][NT][4], uint32_t
         }
     }
 #pragma unroll
-    for (int i = 0; i < 2; ++i)
+    for (int i = 0; i < MI; ++i)
 #pragma unroll
         for (int j = 0; j < NT; ++j)
 #pragma unroll
             for (int r = 0; r < 4; ++r) acc[i][j][r] += part[i][j][r];
 }
 
-template <int NT>
-__device__ __forceinline__ void warp_acc_zero(float (&acc)[2][NT][4]) {
+template <int NT, int MI>
+__device__ __forceinline__ void warp_acc_zero(float (&acc)[MI][NT][4]) {
 #pragma unroll
-    for (int i = 0; i < 2; ++i)
+    for (int i = 0; i < MI; ++i)
 #pragma unroll
         for (int j = 0; j < NT; ++j)
 #pragma unroll

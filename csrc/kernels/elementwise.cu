@@ -174,6 +174,33 @@ cudaError_t launch_relu_mask(float* g, int ldg, const float* y, int ldy, int row
     relu_mask_kernel<<<blocks, 256, 0, stream>>>(g, ldg, y, ldy, rows, cols);
     return cudaGetLastError();
 }
+__global__ void relu_mask_scaled_kernel(float* __restrict__ g, int ldg, const float* __restrict__ y, int ldy, int rows,
+                                        int cols, float scale) {
+    const long total = (long)rows * cols;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int r = (int)(i / cols), c = (int)(i % cols);
+        float* gp = g + (size_t)r * ldg + c;
+        *gp = (y[(size_t)r * ldy + c] > 0.f) ? *gp * scale : 0.f;
+    }
+}
+cudaError_t launch_relu_mask_scaled(float* g, int ldg, const float* y, int ldy, int rows, int cols, float scale,
+                                    cudaStream_t stream) {
+    const long total = (long)rows * cols;
+    int blocks = (int)((total + 255) / 256);
+    if (blocks > 132 * 8) blocks = 132 * 8;
+    if (blocks < 1) blocks = 1;
+    relu_mask_scaled_kernel<<<blocks, 256, 0, stream>>>(g, ldg, y, ldy, rows, cols, scale);
+    return cudaGetLastError();
+}
+
+DropoutSpec dropout_spec(double p, uint64_t seed) {
+    DropoutSpec d{};
+    d.threshold = (uint32_t)(p * 4294967296.0);   // floor: p >= 0
+    d.scale = (float)(1.0 / (1.0 - p));
+    d.seed = seed;
+    d.dp = 1;
+    return d;
+}
 
 __global__ void relu_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, long n) {
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) y[i] = fmaxf(x[i], 0.f);

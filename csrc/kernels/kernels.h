@@ -6,6 +6,8 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 
+#include "dropout.h"
+
 namespace ssb {
 
 enum GemmMode : int { GEMM_FWD = 0, GEMM_DGRAD = 1, GEMM_WGRAD = 2 };
@@ -27,6 +29,9 @@ struct SgdState {
 // nullptr if the combination is valid: 0 <= momentum < 1, weight_decay >= 0, nesterov only with momentum, and a
 // buffer exactly when momentum > 0
 const char* sgd_state_check(const SgdState& s);
+
+// host: threshold and scale of drop probability p in [0, 1) (dropout.h)
+DropoutSpec dropout_spec(double p, uint64_t seed);
 
 // One description for the three Linear GEMMs.  Every GEMM is issued "swapped": the
 // FEATURE dimension sits on the M axis of the 128-row tile and the skinny dimension
@@ -73,6 +78,9 @@ struct GemmParams {
     int k_splits;                 // 0 / 1 = off
     float* partial;
     unsigned int* tile_counter;   // zero before the first launch; re-armed by the kernel
+    // FWD with relu: dropout after the ReLU; DGRAD with mask: the gradient is scaled by drop.scale where the mask passes
+    // (the masked layer's output was dropped).  Last, so that the offsets of the other fields are what they were.
+    DropoutSpec drop;
 };
 
 struct GemmPlan {          // a fully prepared launch (tensor maps are 128 B each)
@@ -104,6 +112,8 @@ int gemm_splitk_choice(const GemmPlan& plan, int num_sms);
 size_t gemm_splitk_workspace_floats(const GemmPlan& plan, int k_splits);
 const char* gemm_plan_enable_splitk(GemmPlan* plan, int k_splits, float* workspace, unsigned int* counters);
 cudaError_t gemm_launch(const GemmPlan& plan, cudaStream_t stream);
+// the plan runs the dropout variant: a FWD with relu or a DGRAD with mask, and plan.p.drop on
+bool gemm_drops(const GemmPlan& plan);
 // Grouped launch of several WGRAD plans (different layers) as ONE grid: a device table holds one entry per CTA.  Only
 // the GEMMs of chain-eligible stages are grouped (out <= 128, any in); they run on narrow tiles of 32 output features x
 // 32 input columns with the full K (rows) in one CTA, instead of the per-layer kernel's 128 x 64.
@@ -283,6 +293,9 @@ struct ChainParams {
     // LossKind of the loss head (selects the kernel instantiation; probs are the row softmax under CROSS_ENTROPY).  Last,
     // so that the offsets of the other parameters are what they were before the field existed.
     int loss_kind;
+    // dropout of every ReLU'd layer (drop.layer: global index of layer 1, drop.row_base 0: row0 is the DP-local row);
+    // drop.on() selects the kernel instantiation.  Last, for the same reason as loss_kind.
+    DropoutSpec drop;
 };
 struct ChainPlan {
     ChainParams p;
@@ -319,6 +332,9 @@ cudaError_t launch_softmax_grad(const float* logits, int ldl, const float* upstr
                                 int rows, int cols, cudaStream_t stream);
 // g[r, c] = y[r, c] > 0 ? g[r, c] : 0   (stage-boundary ReLU backward)
 cudaError_t launch_relu_mask(float* g, int ldg, const float* y, int ldy, int rows, int cols, cudaStream_t stream);
+// the same under dropout (y is the dropped output): g[r, c] = y[r, c] > 0 ? g[r, c] * scale : 0
+cudaError_t launch_relu_mask_scaled(float* g, int ldg, const float* y, int ldy, int rows, int cols, float scale,
+                                    cudaStream_t stream);
 cudaError_t launch_relu_fwd(const float* x, float* y, long n, cudaStream_t stream);
 // y = a * x + b * t  (mse grad: a=2/B, b=-2/B)
 cudaError_t launch_axpby(const float* x, const float* t, float* y, float a, float b, long n, cudaStream_t stream);

@@ -122,7 +122,10 @@ __device__ __forceinline__ unsigned long long gtime() {
 // CLUSTER: the cluster form (see the top of the file); never combined with FOLD.
 // CE: the loss head computes softmax cross-entropy (ChainParams::loss_kind); a compile-time switch, so the MSE
 // instantiations carry none of its code.
-template <bool SPLIT, bool FOLD, int NTW, bool CLUSTER, bool CE>
+// DROP: inverted dropout on every ReLU'd layer (ChainParams::drop); the same kind of switch.  The forward epilogues drop
+// and scale before any copy of the activation leaves the registers (operand tile, peer panels, act[l], the folded
+// out_peer slot); the dgrad epilogues scale where the mask of a dropped layer passes.
+template <bool SPLIT, bool FOLD, int NTW, bool CLUSTER, bool CE, bool DROP>
 __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParams p) {
     static_assert(!(FOLD && CLUSTER), "folded pipeline launches run one CTA per micro-batch");
     extern __shared__ uint8_t smem_raw[];
@@ -258,6 +261,13 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         const int t_n0 = 8 * t_j0, tnt = chain_tile_lo(N / 8, ((warp - 1) >> 1) + 1) - t_j0;
         float tacc[1][NTW / 2][4];
         int it = 0, gemm_i = 0;
+        // DROP: keep ? x * scale : 0 for feature f of row n of this micro-batch in local layer l (ptx.cuh: dropout_keep)
+        uint32_t drop_step = 0u;
+        if constexpr (DROP) drop_step = *p.drop.step;
+        auto drop_fwd = [&](float x, int l, int f, int n) {
+            const uint32_t sample = (uint32_t)((row0 + n) * p.drop.dp + p.drop.rank);
+            return dropout_keep(p.drop, (uint32_t)(p.drop.layer + l - 1), drop_step, (uint32_t)f, sample) ? x * p.drop.scale : 0.f;
+        };
         int wbuf = 0;                                        // activation buffer the NEXT epilogue writes
         uint32_t recv_phase = 0u;                            // CLUSTER: parity of recv_bar(b) in bit b
         // CLUSTER: the tile in abuf b is complete once the peers' panels landed (see exchange below)
@@ -463,6 +473,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                             for (int r = 0; r < 4; ++r) {
                                 float x = tacc[0][j][r] + t_bias[r >> 1];
                                 if (ly.relu) x = fmaxf(x, 0.f);
+                                if constexpr (DROP) { if (ly.relu) x = drop_fwd(x, l, t_feat(r), t_row(j, r)); }
                                 x = t_feat(r) < ly.out ? x : 0.f;
                                 tacc[0][j][r] = x;
                                 st_tile(dst, t_row(j, r), t_feat(r), x);
@@ -494,6 +505,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         for (int j = 0; j < 16; ++j) {
                             float x = v[j] + bias;
                             if (ly.relu) x = fmaxf(x, 0.f);
+                            if constexpr (DROP) { if (ly.relu) x = drop_fwd(x, l, m, c + j); }
                             x = m_ok ? x : 0.f;
                             const int n = c + j;
                             st_tile(dst, n, m, x);
@@ -706,6 +718,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 if (m_ok && n < p.mb_rows) {
                     asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(x) : "l"(g + (int64_t)n * p.act_ld[L] + m));   // may be peer-written
                     if (ly.relu && !(y[(int64_t)n * p.act_ld[L] + m] > 0.f)) x = 0.f;
+                    if constexpr (DROP) { if (ly.relu) x *= p.drop.scale; }   // act_L was dropped: dZ_L = g * s where it passes
                     g[(int64_t)n * p.act_ld[L] + m] = x;     // the wgrad GEMM reads the masked gradient
                 }
                 st_tile(dst, n, m, x);
@@ -744,6 +757,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
 #pragma unroll
                             for (int r = 0; r < 4; ++r) {
                                 float x = (t_mk[j][r] > 0.f) ? tacc[0][j][r] : 0.f;
+                                if constexpr (DROP) { if (mask_on) x *= p.drop.scale; }   // layer l - 1 was dropped
                                 x = t_feat(r) < ly.in ? x : 0.f;
                                 tacc[0][j][r] = x;
                                 if (more) st_tile(dst, t_row(j, r), t_feat(r), x);
@@ -796,6 +810,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     for (int j = 0; j < 16; ++j) {
                         const int n = c + j;
                         float x = (mk[j] > 0.f) ? v[j] : 0.f;
+                        if constexpr (DROP) { if (mask_on) x *= p.drop.scale; }   // layer l - 1 was dropped
                         x = m_ok ? x : 0.f;
                         if (more) st_tile(dst, n, m, x);
                         if (single) keep[j] = x;
@@ -968,30 +983,33 @@ void chain_plan_free(ChainPlan* plan) {
     plan->maps_dev = nullptr;
 }
 
-template <int NTW, bool CE>
+template <int NTW, bool CE, bool DROP>
 static cudaError_t chain_configure_ntw() {
     cudaError_t e;
     const int smem = 227 * 1024;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, false, CE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, true, NTW, false, CE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, false, CE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, true, NTW, false, CE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, true, CE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    return cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, true, CE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, false, CE, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, true, NTW, false, CE, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, false, CE, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, true, NTW, false, CE, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, true, CE, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    return cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, true, CE, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
 }
 
 cudaError_t chain_configure() {
     cudaError_t e;
-    if ((e = chain_configure_ntw<2, false>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<4, false>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<8, false>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<2, true>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<4, true>()) != cudaSuccess) return e;
-    return chain_configure_ntw<8, true>();
+    for (int drop = 0; drop < 2; ++drop) {
+        if ((e = drop ? chain_configure_ntw<2, false, true>() : chain_configure_ntw<2, false, false>()) != cudaSuccess) return e;
+        if ((e = drop ? chain_configure_ntw<4, false, true>() : chain_configure_ntw<4, false, false>()) != cudaSuccess) return e;
+        if ((e = drop ? chain_configure_ntw<8, false, true>() : chain_configure_ntw<8, false, false>()) != cudaSuccess) return e;
+        if ((e = drop ? chain_configure_ntw<2, true, true>() : chain_configure_ntw<2, true, false>()) != cudaSuccess) return e;
+        if ((e = drop ? chain_configure_ntw<4, true, true>() : chain_configure_ntw<4, true, false>()) != cudaSuccess) return e;
+        if ((e = drop ? chain_configure_ntw<8, true, true>() : chain_configure_ntw<8, true, false>()) != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 // grid = micro-batches x plan.cluster, cluster dims (plan.cluster, 1, 1)
-template <bool SPLIT, int NTW, bool CE>
+template <bool SPLIT, int NTW, bool CE, bool DROP>
 static cudaError_t chain_launch_cluster(const ChainPlan& plan, cudaStream_t stream) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)plan.grid);
@@ -1005,15 +1023,15 @@ static cudaError_t chain_launch_cluster(const ChainPlan& plan, cudaStream_t stre
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, mlp_chain_kernel<SPLIT, false, NTW, true, CE>, plan.p);
+    return cudaLaunchKernelEx(&cfg, mlp_chain_kernel<SPLIT, false, NTW, true, CE, DROP>, plan.p);
 }
 
-template <int NTW, bool CE>
+template <int NTW, bool CE, bool DROP>
 static cudaError_t chain_launch_ntw(const ChainPlan& plan, bool fold, cudaStream_t stream) {
     const ChainParams& p = plan.p;
     if (plan.cluster > 1)
-        return p.split ? chain_launch_cluster<true, NTW, CE>(plan, stream) : chain_launch_cluster<false, NTW, CE>(plan, stream);
-#define SSB_CHAIN_LAUNCH(S, F) mlp_chain_kernel<S, F, NTW, false, CE><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(p)
+        return p.split ? chain_launch_cluster<true, NTW, CE, DROP>(plan, stream) : chain_launch_cluster<false, NTW, CE, DROP>(plan, stream);
+#define SSB_CHAIN_LAUNCH(S, F) mlp_chain_kernel<S, F, NTW, false, CE, DROP><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(p)
     if (!p.split) {
         if (fold) SSB_CHAIN_LAUNCH(false, true); else SSB_CHAIN_LAUNCH(false, false);
     } else {
@@ -1030,9 +1048,15 @@ cudaError_t chain_launch(const ChainPlan& plan, cudaStream_t stream) {
     if (p.loss_kind != LOSS_MSE && p.loss_kind != LOSS_CROSS_ENTROPY) return cudaErrorInvalidValue;
     const bool ce = p.loss_kind == LOSS_CROSS_ENTROPY;
     cudaError_t e;
-    if (ntw == 2) e = ce ? chain_launch_ntw<2, true>(plan, fold, stream) : chain_launch_ntw<2, false>(plan, fold, stream);
-    else if (ntw == 4) e = ce ? chain_launch_ntw<4, true>(plan, fold, stream) : chain_launch_ntw<4, false>(plan, fold, stream);
-    else e = ce ? chain_launch_ntw<8, true>(plan, fold, stream) : chain_launch_ntw<8, false>(plan, fold, stream);
+    if (!p.drop.on()) {
+        if (ntw == 2) e = ce ? chain_launch_ntw<2, true, false>(plan, fold, stream) : chain_launch_ntw<2, false, false>(plan, fold, stream);
+        else if (ntw == 4) e = ce ? chain_launch_ntw<4, true, false>(plan, fold, stream) : chain_launch_ntw<4, false, false>(plan, fold, stream);
+        else e = ce ? chain_launch_ntw<8, true, false>(plan, fold, stream) : chain_launch_ntw<8, false, false>(plan, fold, stream);
+    } else {
+        if (ntw == 2) e = ce ? chain_launch_ntw<2, true, true>(plan, fold, stream) : chain_launch_ntw<2, false, true>(plan, fold, stream);
+        else if (ntw == 4) e = ce ? chain_launch_ntw<4, true, true>(plan, fold, stream) : chain_launch_ntw<4, false, true>(plan, fold, stream);
+        else e = ce ? chain_launch_ntw<8, true, true>(plan, fold, stream) : chain_launch_ntw<8, false, true>(plan, fold, stream);
+    }
     if (e != cudaSuccess) return e;
     return cudaGetLastError();
 }

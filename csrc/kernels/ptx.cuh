@@ -5,6 +5,8 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "dropout.h"
+
 namespace ssb {
 
 // ------------------------------------------------------------------ misc
@@ -355,6 +357,26 @@ __device__ __forceinline__ float ce_loss_term(float t, float z, float m, float l
 }
 __device__ __forceinline__ float ce_dlogit(float p, float T, float t, float inv_batch) {
     return __fmul_rn(__fmaf_rn(p, T, -t), inv_batch);
+}
+
+// ------------------------------------------------------------------ dropout masks
+// Philox4x32-10 (Salmon et al., SC'11; the Random123 constants): 10 rounds of two 32x32 -> 64-bit products, the key bumped
+// by the Weyl constants between rounds.  ops/functional.py: philox4x32_10 is the same generator on torch tensors.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        if (r) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+        const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+        const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+    }
+    return c;
+}
+// Inverted dropout (DropoutSpec): element (feature f, global sample s) of global Linear `layer`'s output in optimizer step
+// `step` is kept iff word 0 of Philox4x32-10 with counter (f, s, layer, step) and key (seed lo, seed hi) is >= threshold.
+// Every site that drops or scales calls this, so the kernels and the torch oracle draw the same bits.
+__device__ __forceinline__ bool dropout_keep(const DropoutSpec& d, uint32_t layer, uint32_t step, uint32_t f, uint32_t s) {
+    return philox4x32_10(make_uint4(f, s, layer, step), (uint32_t)d.seed, (uint32_t)(d.seed >> 32)).x >= d.threshold;
 }
 
 }  // namespace ssb

@@ -48,7 +48,9 @@ static constexpr int kGroupMinCtas = 3;                 // CTAs per SM the group
 // columns.  kGroupBM = 32 (WGRAD only): the grouped launch, every math warp owns all 32 rows and a quarter of the columns,
 // so that the few k-blocks of a narrow stage spread over many small CTAs instead of a few long warps.  Each output element
 // goes through the same warp_mma_kblock arithmetic in both forms.
-template <int MODE, bool SPLITK, bool STATEFUL = false, int BM = (int)kBlockM>
+// DROP (FWD with relu / DGRAD with mask, GemmParams::drop): dropout after the ReLU, or the gradient scaled where the mask
+// passes; a compile-time switch, so the dropout-free instantiations carry none of its code.
+template <int MODE, bool SPLITK, bool STATEFUL = false, int BM = (int)kBlockM, bool DROP = false>
 __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
                                              const GemmParams& p, const int bx, const int by, const int bz) {
     constexpr bool A_MN = (MODE != GEMM_FWD);
@@ -167,6 +169,12 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             if (lane == 0) mbar_arrive(empty_bar(s));
         }
 
+        // DROP, FWD: keep ? x * scale : 0 for output feature m of micro-batch row n (sample (row_base + n) * dp + rank)
+        const uint32_t drop_step = (DROP && MODE == GEMM_FWD) ? *p.drop.step : 0u;
+        auto drop_fwd = [&](float x, int n) {
+            const uint32_t sample = (uint32_t)((p.drop.row_base + n) * p.drop.dp + p.drop.rank);
+            return dropout_keep(p.drop, (uint32_t)p.drop.layer, drop_step, (uint32_t)m, sample) ? x * p.drop.scale : 0.f;
+        };
         if constexpr (SPLITK) {
             // ---- split-K: publish the raw partial, last arriver reduces (fixed split order) + epilogue
             const int tile = (int)(by * gridDim.x + bx);
@@ -218,12 +226,13 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
 #pragma unroll
                     for (int j = 0; j < 16; ++j) {
                         float x = v[j] + bias;
+                        const int n = n0 + c + j;
                         if (MODE == GEMM_FWD) {
                             if (p.relu) x = fmaxf(x, 0.f);
+                            if constexpr (DROP) x = drop_fwd(x, n);
                         } else if (mask != nullptr) {
-                            x = (mk[j] > 0.f) ? x : 0.f;
+                            x = (mk[j] > 0.f) ? (DROP ? x * p.drop.scale : x) : 0.f;
                         }
-                        const int n = n0 + c + j;
                         if (n < p.n_total) out[(size_t)n * p.ldo + m] = x;
                     }
                 }
@@ -253,8 +262,9 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                     float x = v[j] + bias;
                     if (MODE == GEMM_FWD) {
                         if (p.relu) x = fmaxf(x, 0.f);
+                        if constexpr (DROP) x = drop_fwd(x, n0 + c + j);
                     } else if (mask != nullptr) {
-                        x = (mk[j] > 0.f) ? x : 0.f;
+                        x = (mk[j] > 0.f) ? (DROP ? x * p.drop.scale : x) : 0.f;
                     }
                     v[j] = x;
                 }
@@ -395,6 +405,13 @@ __global__ void __launch_bounds__(kThreads, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
     tc_gemm_body<MODE, SPLITK, STATEFUL>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z);
+}
+// FWD / DGRAD under dropout (a kernel of its own, so that the names and code of the dropout-free ones stay as they are)
+template <int MODE, bool SPLITK>
+__global__ void __launch_bounds__(kThreads, 1)
+tc_gemm_drop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                    const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+    tc_gemm_body<MODE, SPLITK, false, (int)kBlockM, true>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z);
 }
 
 // ---- grouped weight-gradient launch: the tiles of SEVERAL layers' WGRAD GEMMs in one grid (one table entry per CTA).
@@ -663,6 +680,10 @@ cudaError_t gemm_configure() {
     if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_FWD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_DGRAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_drop_kernel<GEMM_FWD, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_drop_kernel<GEMM_FWD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_drop_kernel<GEMM_DGRAD, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_drop_kernel<GEMM_DGRAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     g_configured = true;
     return cudaSuccess;
 }
@@ -687,6 +708,14 @@ static cudaError_t launch_mode(const GemmPlan& plan, cudaStream_t stream) {
         if (e != cudaSuccess) return e;
     }
     if constexpr (MODE != GEMM_WGRAD) {
+        if (gemm_drops(plan)) {
+            if (plan.p.k_splits > 1)
+                tc_gemm_drop_kernel<MODE, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
+            else
+                tc_gemm_drop_kernel<MODE, false><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
+            g_launches.fetch_add(1, std::memory_order_relaxed);
+            return cudaGetLastError();
+        }
         if (plan.p.k_splits > 1) {
             tc_gemm_kernel<MODE, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
             g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -702,6 +731,11 @@ static cudaError_t launch_mode(const GemmPlan& plan, cudaStream_t stream) {
     tc_gemm_kernel<MODE><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return cudaGetLastError();
+}
+
+bool gemm_drops(const GemmPlan& plan) {
+    if (!plan.p.drop.on()) return false;
+    return plan.mode == GEMM_FWD ? plan.p.relu != 0 : (plan.mode == GEMM_DGRAD && plan.p.mask != nullptr);
 }
 
 cudaError_t gemm_launch(const GemmPlan& plan, cudaStream_t stream) {

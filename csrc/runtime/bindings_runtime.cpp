@@ -246,6 +246,10 @@ public:
         c.loss = geti("loss", ssb::LOSS_MSE);
         TORCH_CHECK(c.loss == ssb::LOSS_MSE || c.loss == ssb::LOSS_CROSS_ENTROPY,
                     "PipeEngine: cfg['loss'] must be 0 (MSE) or 1 (cross-entropy), got ", c.loss);
+        c.dropout = cfg.contains("dropout") ? cfg["dropout"].cast<double>() : 0.0;
+        TORCH_CHECK(c.dropout >= 0.0 && c.dropout < 1.0, "PipeEngine: cfg['dropout'] must be in [0, 1), got ", c.dropout);
+        c.dropout_seed = cfg.contains("dropout_seed") ? cfg["dropout_seed"].cast<uint64_t>() : 0;
+        c.layer_base = geti("layer_base", 0);
         c10::cuda::CUDAGuard guard(weights.device());
         engine_ = std::make_unique<PipeEngine>(c, weights.data_ptr<float>(), grads.data_ptr<float>(), weights.numel(),
                                                momentum.has_value() ? momentum->data_ptr<float>() : nullptr);
@@ -285,6 +289,10 @@ public:
         engine_->set_lr((float)lr);
     }
     float lr() { return engine_->lr(); }
+    void set_dropout_step(int64_t step) {
+        TORCH_CHECK(step >= 0, "PipeEngine.set_dropout_step: the step must be >= 0, got ", step);
+        engine_->set_dropout_step((uint32_t)(step & 0xffffffffLL));   // the masks' step counter is the step mod 2^32
+    }
     void synchronize() { engine_->synchronize(); }
     bool wait(double timeout_s) {
         py::gil_scoped_release nogil;
@@ -395,6 +403,7 @@ void bind_runtime(py::module_& m) {
         .def("run", &PyEngine::run)
         .def("set_lr", &PyEngine::set_lr, py::arg("lr"))
         .def("lr", &PyEngine::lr)
+        .def("set_dropout_step", &PyEngine::set_dropout_step, py::arg("step"))
         .def("synchronize", &PyEngine::synchronize)
         .def("wait", &PyEngine::wait)
         .def("comm_status", &PyEngine::comm_status)

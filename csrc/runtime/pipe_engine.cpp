@@ -127,6 +127,10 @@ void PipeEngine::alloc_buffers() {
     lr_ = lr_written_[0] = lr_written_[1] = cfg_.lr;
     const float lr_init[2] = {cfg_.lr, cfg_.lr};
     CUDA_CHECK(cudaMemcpy(lr_dev_, lr_init, sizeof(lr_init), cudaMemcpyHostToDevice));
+    if (dropout_on()) {
+        step_dev_ = reinterpret_cast<uint32_t*>(dalloc(2));   // zeroed: step 0
+        step_ = step_written_[0] = step_written_[1] = 0u;
+    }
     loss_dev_ = dalloc(std::max(M, 16));
     CUDA_CHECK(cudaMallocHost(&loss_host_, 2 * sizeof(float) * std::max(M, 16)));   // one slot per staging set
     // opt-in (SSB_LOSS_ZEROCOPY=1, awaiting hardware validation): the loss head stores its per-micro-batch losses straight
@@ -160,6 +164,17 @@ void PipeEngine::alloc_buffers() {
         }
         probs_[mu] = probs_all_ + (size_t)mu * mb * act_ld_[L_];
     }
+}
+
+DropoutSpec PipeEngine::drop_for(int layer, int row_base) const {
+    if (!dropout_on() || !cfg_.layers[layer - 1].relu) return DropoutSpec{};
+    DropoutSpec d = dropout_spec(cfg_.dropout, cfg_.dropout_seed);
+    d.step = step_dev_ + cur_set_;
+    d.layer = cfg_.layer_base + layer - 1;
+    d.row_base = row_base;
+    d.dp = cfg_.dp_size;
+    d.rank = cfg_.dp_rank;
+    return d;
 }
 
 // Point the planner at one of the two input-staging sets (stage input = act[.][0], targets).
@@ -246,6 +261,14 @@ int PipeEngine::add_chain(int stream, int mu_base, int n_mu, bool do_fwd, bool d
     cp.probs = probs_all_; cp.ldp = act_ld_[L_];
     cp.loss = loss_target();
     cp.loss_kind = cfg_.loss;
+    if (dropout_on()) {
+        // one spec for the launch: the kernel drops only the ReLU'd layers, layer l's counter is drop.layer + l - 1
+        cp.drop = dropout_spec(cfg_.dropout, cfg_.dropout_seed);
+        cp.drop.step = step_dev_ + cur_set_;
+        cp.drop.layer = cfg_.layer_base;
+        cp.drop.dp = cfg_.dp_size;
+        cp.drop.rank = cfg_.dp_rank;
+    }
     cp.mb_rows = cfg_.mb_rows; cp.mu_base = mu_base;
     cp.inv_batch = 1.0f / (float)cfg_.global_batch;
     cp.do_fwd = do_fwd; cp.do_loss = do_loss; cp.do_bwd = do_bwd; cp.first_stage = cfg_.is_first;
@@ -390,6 +413,9 @@ void PipeEngine::plan_per_mubatch() {
     auto add_gemm = [&](const GemmPlan& g, int stream, int layer, int mu) {
         gemms_.push_back(g);
         maybe_splitk(gemms_.back());
+        // FWD drops layer `layer`'s output, DGRAD scales by the mask of layer - 1 (the same p): the spec of the GEMM's
+        // rows, micro-batch mu of this stage
+        gemms_.back().p.drop = drop_for(g.mode == GEMM_DGRAD ? std::max(layer - 1, 1) : layer, mu * cfg_.mb_rows);
         Op op;
         op.kind = OP_GEMM; op.stream = stream; op.gemm = (int)gemms_.size() - 1; op.layer = layer; op.mu = mu;
         ops_.push_back(op);
@@ -608,6 +634,10 @@ void PipeEngine::plan_per_mubatch() {
                         rm.kind = OP_RELU_MASK; rm.stream = s;
                         rm.a = dz_[mu][L_]; rm.lda = act_ld_[L_]; rm.b = act_[mu][L_]; rm.ldb = act_ld_[L_];
                         rm.rows = mb; rm.cols = cfg_.layers[L_ - 1].out;
+                        if (dropout_on()) {                                     // act_L was dropped
+                            rm.dropout = true;
+                            rm.scalar = dropout_spec(cfg_.dropout, cfg_.dropout_seed).scale;
+                        }
                         ops_.push_back(rm);
                     }
                     for (int l = L_; l >= 1; --l) {
@@ -764,6 +794,7 @@ void PipeEngine::build_coalesced() {
     auto add_gemm = [&](const GemmPlan& g, int stream, int layer) {
         gemms_.push_back(g);
         maybe_splitk(gemms_.back());
+        gemms_.back().p.drop = drop_for(g.mode == GEMM_DGRAD ? std::max(layer - 1, 1) : layer, 0);   // all rows
         Op op;
         op.kind = OP_GEMM; op.stream = stream; op.gemm = (int)gemms_.size() - 1; op.layer = layer; op.mu = -1;
         ops_.push_back(op);
@@ -1049,7 +1080,10 @@ void PipeEngine::exec(const Op& op) {
         case OP_ARGMAX:
             CUDA_CHECK(launch_argmax_correct(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, correct_dev_, st));
             break;
-        case OP_RELU_MASK: CUDA_CHECK(launch_relu_mask(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, st)); break;
+        case OP_RELU_MASK:
+            if (op.dropout) CUDA_CHECK(launch_relu_mask_scaled(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, op.scalar, st));
+            else CUDA_CHECK(launch_relu_mask(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, st));
+            break;
         case OP_SGD: {
             const SgdState opt = opt_for(0);
             if (opt.plain()) CUDA_CHECK(launch_sgd(op.a, op.b, op.lr, op.n, st));
@@ -1234,6 +1268,13 @@ void PipeEngine::run() {
         lr_written_[set] = lr_;
         wait_copy = true;
     }
+    if (dropout_on() && step_written_[set] != step_) {   // the same protocol for the dropout step
+        CUDA_CHECK(cudaStreamWaitEvent(copy_stream_, ev_done_[set], 0));
+        cu_check(memset_d32_async()(reinterpret_cast<CUdeviceptr>(step_dev_ + set), step_, 1, copy_stream_), "cuMemsetD32Async");
+        CUDA_CHECK(cudaEventRecord(ev_copy_[set], copy_stream_));
+        step_written_[set] = step_;
+        wait_copy = true;
+    }
     if (wait_copy) CUDA_CHECK(cudaStreamWaitEvent(streams_[0], ev_copy_[set], 0));
     if (graph_exec_sets_[set]) CUDA_CHECK(cudaGraphLaunch(graph_exec_sets_[set], streams_[0]));
     else walk(set);
@@ -1320,6 +1361,12 @@ std::string PipeEngine::plan_text(int set) const {
         if (op.event >= 0) os << " event=" << op.event;
         if (op.layer >= 0) os << " layer=" << op.layer;
         if (op.mu >= 0) os << " mu=" << op.mu;
+        if (op.kind == OP_GEMM) {                      // the variant a GEMM launches beyond the plain one
+            const GemmPlan& g = gemms_[op.gemm];
+            if (g.p.k_splits > 1) os << " splits=" << g.p.k_splits;
+            if (gemm_drops(g)) os << " drop=" << (g.mode == GEMM_FWD ? "fwd" : "dgrad");
+        }
+        if (op.kind == OP_RELU_MASK && op.dropout) os << " drop=scaled";
         if (op.kind == OP_COMM_GROUP) {
             os << " [";
             for (const auto& it : op.comm) os << (it.is_send ? "send->" : "recv<-") << it.peer << ":" << it.count << " ";

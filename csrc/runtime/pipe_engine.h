@@ -67,6 +67,7 @@ struct Op {
     float* f = nullptr;        // loss head: where the loss values go when not the default device scratch
     int lda = 0, ldb = 0, ldc = 0, ldd = 0, rows = 0, cols = 0;
     float scalar = 0.f;
+    bool dropout = false;      // OP_RELU_MASK: the masked activation was dropped, the kept gradient is scaled by `scalar`
     const float* lr = nullptr; // OP_SGD / OP_NVLS_SGD: the learning-rate slot of the op's staging set
     int64_t n = 0;
 };
@@ -92,6 +93,11 @@ struct EngineConfig {
     float momentum = 0.f, weight_decay = 0.f;
     int nesterov = 0;
     int loss = LOSS_MSE;    // LossKind of the last stage's head (the chain kernel's and loss_head_kernel's)
+    // inverted dropout on every ReLU'd layer of a training plan (0 = off; inference plans ignore it).  layer_base: the
+    // global index of this stage's first Linear (the masks' layer counter); dp_size / dp_rank map rows to samples.
+    double dropout = 0.0;
+    uint64_t dropout_seed = 0;
+    int layer_base = 0;
 };
 
 class PipeEngine {
@@ -118,6 +124,11 @@ public:
     // run() rewrites that slot on the copy stream only when it holds a different value.
     void set_lr(float lr) { lr_ = lr; }
     float lr() const { return lr_; }
+    // optimizer step whose dropout masks the steps run from now on draw; kept like lr (a device slot per staging set,
+    // rewritten by run() only when it changed, and only by plans with dropout on)
+    void set_dropout_step(uint32_t step) { step_ = step; }
+    uint32_t dropout_step() const { return step_; }
+    bool dropout_on() const { return cfg_.training && cfg_.dropout > 0.0; }
     void synchronize();
     bool wait(double timeout_s);      // watchdog: false if the step in flight did not finish in time
     std::string comm_status() const;  // NCCL async error state of the attached communicators
@@ -226,6 +237,11 @@ private:
     float lr_written_[2] = {0.f, 0.f};
     float lr_ = 0.f;
     const float* lr_slot() const { return lr_dev_ + cur_set_; }
+    // dropout step: the same scheme as lr (allocated only when dropout_on())
+    uint32_t* step_dev_ = nullptr;
+    uint32_t step_written_[2] = {0u, 0u};
+    uint32_t step_ = 0u;
+    DropoutSpec drop_for(int layer, int row_base) const;   // layer l (1-based) of the plan being built; off when !dropout_on()
     cudaStream_t copy_stream_ = nullptr;
     cudaEvent_t ev_copy_[2], ev_done_[2];
     int fill_set_ = 0, run_set_ = 0, cur_set_ = 0;

@@ -176,7 +176,12 @@ class Module(ABC):
 class ReLU(Module):
     """Caches the sign mask per micro-batch.  On CUDA the fused Linear kernel hands us
     the *output* y = relu(z); ``y > 0`` is the same mask, so no extra tensor is
-    materialised (SURVEY.md K1)."""
+    materialised (SURVEY.md K1).
+
+    Under dropout the owning Linear stashes its dropped output a = relu(z) * keep * s instead, so ``a > 0`` is "active
+    and kept", and ``dropout_scale`` (s) multiplies the gradient where the mask passes it."""
+
+    dropout_scale = None
 
     def forward(self, inputs, mubatch_id=0):
         if self._training:
@@ -190,6 +195,8 @@ class ReLU(Module):
     def backward(self, dout, mubatch_id=0):
         assert self._training
         dout = F.relu_grad(dout, self._cache.pop(f"bitmask_{mubatch_id}"))
+        if self.dropout_scale is not None:
+            dout = dout * self.dropout_scale
         return dout
 
     def __repr__(self):
@@ -261,12 +268,30 @@ class Linear(Module):
 
             out = K.linear_fwd(inputs, W, b, relu=self.activation is not None)
             if self.activation is not None:
+                out = self._dropout(out)
                 self.activation.stash_output(out, mubatch_id)
             return out
         result = F.linear(inputs, W, b)
         if self.activation:
-            return self.activation(result, mubatch_id)
+            out = self.activation(result, mubatch_id)
+            if self._training and self.dropout is not None:
+                out = self._dropout(out)
+                self.activation.stash_output(out > 0, mubatch_id)
+            return out
         return result
+
+    # dropout of this Linear's ReLU output (set by models.mlp.MLP): None, or (p, seed, global layer index, scale); the
+    # samples and step of the next forward are in dropout_rows = (global sample index of every input row, step)
+    dropout = None
+    dropout_rows = None
+
+    def _dropout(self, out):
+        if not self._training or self.dropout is None:
+            return out
+        p, seed, layer, scale = self.dropout
+        samples, step = self.dropout_rows
+        keep = F.dropout_mask(p, seed, layer, step, samples.to(out.device), out.shape[1])
+        return F.dropout_ref(out, keep, scale)
 
     def backward(self, dout, mubatch_id=0):
         assert self._training

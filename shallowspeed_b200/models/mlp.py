@@ -12,7 +12,9 @@ from __future__ import annotations
 
 from typing import Optional, Sequence, Union
 
-from ..ops.functional import check_loss
+import torch
+
+from ..ops.functional import check_dropout, check_loss, dropout_scale
 from .layers import CrossEntropyLoss, Linear, MSELoss, ParamArena, Sequential, Softmax
 
 DEFAULT_LAYER_SIZES = [784, 128, 127, 126, 125, 124, 123, 10]  # reference train.py:98
@@ -48,7 +50,8 @@ def mlp_sizes(hidden: int, n_layers: int, in_dim: int = 784, out_dim: int = 10):
 
 class MLP(Sequential):
     def __init__(self, sizes: Sequence[int], stage_idx: int, n_stages: int, batch_size: int,
-                 device="cpu", seed_mode: str = "shape", verbose: bool = False, loss: str = "mse"):
+                 device="cpu", seed_mode: str = "shape", verbose: bool = False, loss: str = "mse",
+                 dropout: float = 0.0, dropout_seed: int = 0):
         """
         :param batch_size: the GLOBAL batch size - the loss gradient is scaled by
             1/batch_size so that summing over micro-batches and DP replicas reproduces
@@ -57,9 +60,17 @@ class MLP(Sequential):
             "index" = additionally mixes the global layer index into the seed.
         :param loss: "mse" = the reference's Softmax + MSELoss head; "cross_entropy" =
             CrossEntropyLoss on the logits.  Every stage records it (the native engine reads it).
+        :param dropout: inverted dropout with this drop probability on the output of every Linear that has a ReLU (every
+            hidden layer, never the logits), in training only.  The mask of an element is a pure function of
+            (dropout_seed, global layer index, feature, the sample's position in the global batch, dropout_step)
+            (ops.functional.dropout_mask), so every DP x PP layout draws the same masks.  Under pp=8 the default model's
+            stage 6 ends in a 123->10 Linear that carries a ReLU (the stage rule above); it is dropped like any other.
         """
         assert seed_mode in ("shape", "index")
         self.loss = check_loss(loss)
+        self.dropout, self.dropout_seed = check_dropout(dropout, dropout_seed)
+        self._dropout_step = 0
+        self.dropout_shard = (0, 1)   # (DP rank, DP size) of the rows this replica forwards (set by the pipeline VM)
         self.sizes = list(sizes)
         self.stage_idx, self.n_stages, self.batch_size = stage_idx, n_stages, batch_size
         specs = stage_layer_specs(sizes, stage_idx, n_stages)
@@ -72,6 +83,13 @@ class MLP(Sequential):
             for bi, (i, o, relu, gidx) in enumerate(specs)
         ]
         self.linears = list(layers)
+        self.layer_base = specs[0][3] if specs else 0   # global index of this stage's first Linear
+        if self.dropout > 0.0:
+            scale = dropout_scale(self.dropout)
+            for lin, (_, _, relu, gidx) in zip(layers, specs):
+                if relu:
+                    lin.dropout = (self.dropout, self.dropout_seed, gidx, scale)
+                    lin.activation.dropout_scale = scale
         if self.is_last_stage and self.loss == "cross_entropy":
             layers.append(CrossEntropyLoss(batch_size=batch_size))
         elif self.is_last_stage:
@@ -86,6 +104,27 @@ class MLP(Sequential):
     def to(self, device):
         self.arena.to(device)
         return self
+
+    @property
+    def dropout_step(self) -> int:
+        """The optimizer step (0-based, global) whose dropout masks the next training step draws."""
+        return self._dropout_step
+
+    @dropout_step.setter
+    def dropout_step(self, step):
+        if isinstance(step, bool) or not isinstance(step, int) or step < 0:
+            raise ValueError(f"dropout_step must be an integer >= 0, got {step!r}")
+        self._dropout_step = int(step)
+
+    def forward(self, inputs, mubatch_id=0):
+        if self._training and self.dropout > 0.0:
+            # row n of micro-batch mu of the DP-local batch on replica r of dp is sample (mu * rows + n) * dp + r
+            rank, dp = self.dropout_shard
+            n = inputs.shape[0]
+            samples = (mubatch_id * n + torch.arange(n, dtype=torch.int64)) * dp + rank
+            for lin in self.linears:
+                lin.dropout_rows = (samples, self._dropout_step)
+        return super().forward(inputs, mubatch_id)
 
     @property
     def loss_layer(self) -> Optional[Union[MSELoss, CrossEntropyLoss]]:

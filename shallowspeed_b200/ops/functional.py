@@ -103,6 +103,76 @@ def cross_entropy_grad_ref(logits, target, batch_size: int):
 
 
 # ----------------------------------------------------------------------------
+# dropout: masks drawn from a counter-based generator (Philox4x32-10), the same bits as csrc/kernels/ptx.cuh
+# ----------------------------------------------------------------------------
+PHILOX_M0, PHILOX_M1 = 0xD2511F53, 0xCD9E8D57
+PHILOX_W0, PHILOX_W1 = 0x9E3779B9, 0xBB67AE85
+_U32 = 0xFFFFFFFF
+
+
+def _mulhilo32(a: torch.Tensor, m: int):
+    """(hi, lo) 32-bit words of a * m for int64 tensors a in [0, 2^32): the 64-bit product is formed from 16-bit halves of
+    m so that no intermediate leaves int64."""
+    p_lo = a * (m & 0xFFFF)                       # < 2^48
+    p_hi = a * (m >> 16)                          # < 2^48, weighs 2^16
+    low = p_lo + ((p_hi & 0xFFFF) << 16)          # < 2^49
+    return (p_hi >> 16) + (low >> 32), low & _U32
+
+
+def philox4x32_10(counter, key):
+    """Philox4x32-10 (Random123) over broadcastable int64 tensors or ints holding 32-bit words.  ``counter`` is a 4-tuple,
+    ``key`` a 2-tuple; returns the 4 output words as int64 tensors."""
+    like = next((t for t in (*counter, *key) if isinstance(t, torch.Tensor)), None)
+    dev = like.device if like is not None else None
+    c0, c1, c2, c3 = (torch.as_tensor(c, dtype=torch.int64, device=dev) & _U32 for c in counter)
+    k0, k1 = (torch.as_tensor(k, dtype=torch.int64, device=dev) & _U32 for k in key)
+    for r in range(10):
+        if r:
+            k0, k1 = (k0 + PHILOX_W0) & _U32, (k1 + PHILOX_W1) & _U32
+        hi0, lo0 = _mulhilo32(c0, PHILOX_M0)
+        hi1, lo1 = _mulhilo32(c2, PHILOX_M1)
+        c0, c1, c2, c3 = hi1 ^ c1 ^ k0, lo1, hi0 ^ c3 ^ k1, lo0
+    return c0, c1, c2, c3
+
+
+def check_dropout(p, seed):
+    """Validated (p, seed): 0 <= p < 1 and 0 <= seed < 2**64, else ValueError."""
+    if isinstance(p, bool) or not isinstance(p, (int, float)) or not (0.0 <= float(p) < 1.0):
+        raise ValueError(f"dropout must be a number in [0, 1), got {p!r}")
+    if isinstance(seed, bool) or not isinstance(seed, int) or not (0 <= seed < 2 ** 64):
+        raise ValueError(f"dropout_seed must be an integer in [0, 2**64), got {seed!r}")
+    return float(p), int(seed)
+
+
+def dropout_threshold(p: float) -> int:
+    """floor(p * 2^32) in fp64: a unit is dropped iff Philox word 0 < threshold."""
+    return int(float(p) * 4294967296.0)
+
+
+def dropout_scale(p: float) -> float:
+    """float32(1 / (1 - p)): 1 / (1 - p) in fp64, rounded to fp32 once."""
+    import numpy as np
+
+    return float(np.float32(1.0 / (1.0 - float(p))))
+
+
+def dropout_mask(p: float, seed: int, layer: int, step: int, samples, n_features: int, device=None) -> torch.Tensor:
+    """Keep mask [len(samples), n_features] (bool) of the output of global Linear ``layer`` in optimizer step ``step``.
+    ``samples``: the rows' positions in the global batch (row n of DP rank r of dp is n * dp + r).  Element (s, f) is
+    kept iff word 0 of Philox4x32-10 with counter (f, s, layer, step mod 2^32) and key (seed lo, seed hi) is at least
+    ``dropout_threshold(p)``: a pure function of the sample, the layer, the feature and the step."""
+    samples = torch.as_tensor(samples, dtype=torch.int64, device=device)
+    f = torch.arange(n_features, dtype=torch.int64, device=samples.device).view(1, -1)
+    u, _, _, _ = philox4x32_10((f, samples.view(-1, 1), int(layer), int(step) & _U32), (seed & _U32, seed >> 32))
+    return u >= dropout_threshold(p)
+
+
+def dropout_ref(a: torch.Tensor, keep: torch.Tensor, scale: float) -> torch.Tensor:
+    """Inverted dropout of ReLU outputs: keep ? a * scale : 0 (one multiply in a's dtype)."""
+    return torch.where(keep, a * scale, torch.zeros_like(a))
+
+
+# ----------------------------------------------------------------------------
 # public API (dispatching)
 # ----------------------------------------------------------------------------
 def relu(input):

@@ -273,6 +273,8 @@ class NativeWorker:
         its device slot only when the value changed)."""
         if sched.training and self.optimizer is not None:
             eng.set_lr(float(self.optimizer.lr))
+        if sched.training and getattr(self.model, "dropout", 0.0) > 0.0:   # the step whose dropout masks this step draws
+            eng.set_dropout_step(int(self.model.dropout_step))
 
     # ------------------------------------------------------------------ plan cache
     def _key(self, sched: Schedule):
@@ -300,6 +302,8 @@ class NativeWorker:
             momentum = m.arena.momentum if self.momentum > 0.0 else None
         if m.loss != "mse":   # the head's loss kind (training and inference: the probabilities depend on it)
             cfg.update(loss=LOSS_CODES[m.loss])
+        if training and getattr(m, "dropout", 0.0) > 0.0:   # inference plans run without dropout
+            cfg.update(dropout=m.dropout, dropout_seed=m.dropout_seed, layer_base=m.layer_base)
         eng = _C().PipeEngine(specs, cfg, m.arena.weights, m.arena.grads, momentum)
         if self._pp_nccl is not None:
             eng.set_pp_comm(self._pp_nccl)
@@ -468,12 +472,16 @@ class Trainer:
     ``lr`` is the base learning rate.  ``lr_schedule`` (an ``lr_schedule.LRSchedule`` or any callable ``step -> lr``)
     sets ``optimizer.lr`` before every step from the number of steps run so far; ``Trainer.lr`` is the rate of the
     next step.
+
+    ``dropout`` / ``dropout_seed``: inverted dropout on every hidden layer (``models.mlp.MLP``); step i draws the masks
+    of ``dropout_step`` i, the number of steps run so far.
     """
 
     def __init__(self, layer_sizes, global_batch_size=128, n_mubatches=4, lr=0.006, schedule="naive",
                  dp_comm=None, pp_comm=None, grid: Optional[ProcessGrid] = None, comm_mode="fused",
                  use_graph=True, device=None, seed_mode="shape", precision="fp32", watchdog_s=None, pp_transport=None,
-                 local_batch_size=None, momentum=0.0, weight_decay=0.0, nesterov=False, loss="mse", lr_schedule=None):
+                 local_batch_size=None, momentum=0.0, weight_decay=0.0, nesterov=False, loss="mse", lr_schedule=None,
+                 dropout=0.0, dropout_seed=0):
         from ..models.mlp import MLP
         from ..optimizer import SGD
         from .schedules import SCHEDULE_NAME_TO_CLS
@@ -488,7 +496,7 @@ class Trainer:
         # scale stays 1 / global_batch_size.
         self.local_batch_size = int(local_batch_size) if local_batch_size else global_batch_size // dp
         self.model = MLP(layer_sizes, self.pp_comm.Get_rank(), pp, global_batch_size, seed_mode=seed_mode,
-                         loss=loss).to(self.device)
+                         loss=loss, dropout=dropout, dropout_seed=dropout_seed).to(self.device)
         self.optimizer = SGD(self.model.parameters(), lr, momentum=momentum, weight_decay=weight_decay, nesterov=nesterov,
                              arena=self.model.arena)
 
@@ -513,6 +521,7 @@ class Trainer:
     def step_async(self, x_host, y_host):
         if self.lr_schedule is not None:
             self.optimizer.lr = self.lr_schedule(self._steps)
+        self.model.dropout_step = self._steps
         self.worker.set_lr(self.engine, self.schedule)
         self.engine.stage_inputs(x_host if self.is_first else None, y_host if self.is_last else None)
         self.engine.run()

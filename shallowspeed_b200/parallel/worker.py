@@ -146,6 +146,8 @@ class Worker:
         self.pp_comm.batch([self._comm_op(RecvOutputGrad(buffer_id))])
 
     def forward(self, buffer_id, mubatch_id):
+        if hasattr(self.model, "dropout_shard"):   # dropout masks are drawn per global sample: rank-strided shards
+            self.model.dropout_shard = (self.dp_comm.Get_rank(), self.dp_comm.Get_size())
         out = self.model.forward(self.input_buffers[buffer_id], mubatch_id=mubatch_id)
         self.output_buffers[buffer_id] = out if out.is_contiguous() else out.contiguous()
 

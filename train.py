@@ -93,6 +93,9 @@ def build_parser():
     p.add_argument("--nesterov", action="store_true", help="Nesterov momentum (needs --momentum > 0)")
     p.add_argument("--loss", choices=["mse", "cross-entropy"], default="mse",
                    help="mse: the reference's softmax + MSE; cross-entropy: softmax cross-entropy on the logits")
+    p.add_argument("--dropout", type=float, default=0.0,
+                   help="inverted dropout with this drop probability on every hidden layer's output, in [0, 1)")
+    p.add_argument("--dropout-seed", type=int, default=0, help="seed of the dropout masks, in [0, 2**64)")
     p.add_argument("--layer-sizes", type=int, nargs="+", default=None, help="explicit layer widths (default: reference MLP)")
     p.add_argument("--hidden", type=int, default=None, help="with --n-layers: 784 -> hidden x (n-1) -> 10")
     p.add_argument("--n-layers", type=int, default=None)
@@ -178,7 +181,8 @@ def main(args):
     loss = args.loss.replace("-", "_")
     model = MLP(layer_sizes, stage_idx=pp_comm.Get_rank(), n_stages=args.pp,
                 batch_size=args.global_batch_size, seed_mode=args.seed_mode,
-                verbose=(grid.rank == 0 or is_last), loss=loss)
+                verbose=(grid.rank == 0 or is_last), loss=loss, dropout=args.dropout,
+                dropout_seed=args.dropout_seed)
     model.to(device)
     model.train()
     # before the resume: the momentum arena it restores is allocated here
@@ -202,7 +206,8 @@ def main(args):
     hparams = {"lr": float(args.lr), "global_batch_size": int(args.global_batch_size), "seed_mode": str(args.seed_mode),
                "n_mubatches": int(args.n_mubatches), "momentum": float(args.momentum),
                "weight_decay": float(args.weight_decay), "nesterov": bool(args.nesterov), "loss": loss,
-               "lr_schedule": lr_schedule.spec()}
+               "lr_schedule": lr_schedule.spec(), "dropout": float(args.dropout),
+               "dropout_seed": int(args.dropout_seed)}
     resumed_step = 0
     if args.resume:
         from shallowspeed_b200.utils.checkpoint import load_stage
@@ -242,6 +247,7 @@ def main(args):
         steps_this_epoch = min(n_batches - first_batch, total_steps - step)
         for batch_id in range(first_batch, first_batch + steps_this_epoch):
             optimizer.lr = lr_schedule(step)        # both engines read the optimizer's rate when the step starts
+            model.dropout_step = step               # ... and the model's dropout step
             worker.execute(schedule, batch_id)
             step += 1
         first_batch = 0

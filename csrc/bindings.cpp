@@ -235,6 +235,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         const bool ok = ssb::chain_cluster_budget(mb_rows, cluster, split, &kps, &stages, &smem);
         return std::make_tuple(ok, kps, stages, smem);
     });
+    // k-split layer 1, no GPU needed: the k-blocks of a GEMM of nkb k-blocks that part 0 (owner) / 1 (helper) multiplies
+    m.def("chain_ksplit_kblocks", [](int nkb, int part) {
+        std::vector<int> kb((size_t)std::max(nkb, 0));
+        kb.resize((size_t)ssb::chain_ksplit_kblocks(nkb, part, kb.data()));
+        return kb;
+    });
     m.def("chain_cluster_size", [](const std::vector<std::pair<int, int>>& in_out, bool do_fwd, bool do_loss, bool do_bwd,
                                    bool first_stage, bool gated, bool folded) {
         std::vector<ssb::ChainLayer> ls(in_out.size());

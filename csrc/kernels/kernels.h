@@ -296,12 +296,16 @@ struct ChainParams {
     // dropout of every ReLU'd layer (drop.layer: global index of layer 1, drop.row_base 0: row0 is the DP-local row);
     // drop.on() selects the kernel instantiation.  Last, for the same reason as loss_kind.
     DropoutSpec drop;
+    // CTAs per feature slice in layer 1 (set by chain_plan): 2 when a cluster launch's layer 1 has more than 4 k-blocks
+    // (cluster ranks >= cluster are the helpers that multiply half of them), else 1.  Last, for the same reason.
+    int ksplit;
 };
 struct ChainPlan {
     ChainParams p;
     CUtensorMap* maps_dev;
     int grid, smem_bytes;
-    int cluster;                     // CTAs per micro-batch (grid = micro-batches x cluster)
+    int cluster;                     // CTAs per feature slice (grid = micro-batches x cluster x ksplit)
+    int ksplit;                      // CTAs per feature slice in layer 1 (ChainParams::ksplit)
 };
 bool chain_eligible(const ChainLayer* layers, int n_layers, int mb_rows, int out_dim, bool has_loss, bool split = false);
 const char* chain_plan(ChainPlan* plan, const ChainParams& params, const float* x, int ldx, int total_rows, int n_mubatches,
@@ -314,6 +318,9 @@ bool chain_budget(int mb_rows, bool split, int* kps, int* stages, int* smem_byte
 int chain_cluster_size(const ChainLayer* layers, int n_layers, bool do_fwd, bool do_loss, bool do_bwd, bool first_stage,
                        bool gated, bool folded);
 bool chain_cluster_budget(int mb_rows, int cluster, bool split, int* kps, int* stages, int* smem_bytes);
+// k-split layer 1 (host arithmetic only): the k-blocks of a GEMM of nkb k-blocks that part 0 (the owner) or 1 (the
+// helper) of a feature slice multiplies, in the order it streams them, into kblocks; returns their number
+int chain_ksplit_kblocks(int nkb, int part, int* kblocks);
 void chain_plan_free(ChainPlan* plan);
 cudaError_t chain_configure();
 cudaError_t chain_launch(const ChainPlan& plan, cudaStream_t stream);

@@ -17,14 +17,17 @@
 // critical path of the reference workload; the per-layer kernels in tc_gemm.cu remain the
 // general path (wide layers) and compute the weight gradients afterwards.
 //
-// Cluster form (CLUSTER, C = ChainParams::cluster CTAs per micro-batch): CTA rank c of the micro-batch's thread-block
-// cluster owns output features [32c, 32c + 32) of every GEMM and streams only that slice of each weight matrix.  In a
-// GEMM of at most 4 k-blocks (every GEMM but a first layer with more than 128 inputs) each of the eight math warps owns
-// m16n8 tiles of that output (chain_tile_lo), runs them over all k-blocks and runs their epilogue on its own fragments.
-// A longer GEMM splits its k-blocks four ways (warp (q, half) takes the k-blocks kb with kb % 4 == q, for its half of
-// the rows) and adds the four partial sums through shared memory in a fixed order.  The 32-feature output is exactly one
-// K-major panel of the next GEMM's B operand: it is written locally, and each warp stores its block of it into the same
-// offset of every peer (st.async, completion counted on the peer's per-buffer mbarrier; see exchange).
+// Cluster form (CLUSTER, C = ChainParams::cluster CTAs per feature slice): CTA rank c < C of the micro-batch's
+// thread-block cluster owns output features [32c, 32c + 32) of every GEMM and streams only that slice of each weight
+// matrix.  Each of its eight math warps owns m16n8 tiles of that output (chain_tile_lo), runs them over all k-blocks and
+// runs their epilogue on its own fragments.  A first layer of more than 4 k-blocks (more than 128 inputs) is spread over
+// P = ChainParams::ksplit = 2 CTAs per slice: rank C + c, the helper of slice c, streams the k-blocks kb with kb % 4 in
+// {2, 3} of W_1's 32 rows and of X (chain_ksplit_kblock), the owner those with kb % 4 in {0, 1}.  Every warp sums its
+// tiles per k-phase kb % 4; the helper's warps store their two phase sums into the owner (st.async), which adds the four
+// in phase order, runs the epilogue and goes on alone - the helper is done after layer 1.  The 32-feature output is
+// exactly one K-major panel of the next GEMM's B operand: it is written locally, and each warp stores its block of it
+// into the same offset of every other owner (st.async, completion counted on the peer's per-buffer mbarrier; see
+// exchange).
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -63,9 +66,23 @@ constexpr bool chain_tiles_cover_panel() {
 }
 static_assert(chain_tiles_cover_panel(), "the full-K tiles of the 8 math warps must cover the CTA's panel exactly once");
 
-// CLUSTER, full-K form: the cnt (= CNT when it is a template argument) k-blocks of one ring stage on this warp's tiles.
-// The k-block products are independent, so the unrolled CNT forms overlap them; the k-block sums are added into acc in
-// k-block order either way.  a: K-major / MN-major 32-feature weight panels, kPanelBytes apart; b: activation panels.
+// CLUSTER, k-split first layer: the i-th k-block that part h (0: the owner, 1: the helper) of a feature slice streams and
+// multiplies, and how many of a GEMM's nkb k-blocks that part has.  Part h takes the k-phases kb % 4 in {2h, 2h + 1}, in
+// increasing kb, so its i-th k-block is in phase 2h + (i & 1) and each phase's k-blocks come in k-block order.
+__host__ __device__ constexpr int chain_ksplit_kblock(int i, int part) { return 4 * (i >> 1) + 2 * part + (i & 1); }
+__host__ __device__ constexpr int chain_ksplit_count(int nkb, int part) {
+    const int tail = nkb % 4 - 2 * part;                  // k-blocks of the last, partial group of 4 in this part's phases
+    return 2 * (nkb / 4) + (tail < 0 ? 0 : tail > 2 ? 2 : tail);
+}
+int chain_ksplit_kblocks(int nkb, int part, int* kblocks) {
+    const int n = chain_ksplit_count(nkb, part);
+    for (int i = 0; i < n; ++i) kblocks[i] = chain_ksplit_kblock(i, part);
+    return n;
+}
+
+// CLUSTER: the cnt (= CNT when it is a template argument) k-blocks of one ring stage on this warp's tiles.  The k-block
+// products are independent, so the unrolled CNT forms overlap them; the k-block sums are added into acc in k-block order
+// either way.  a: K-major / MN-major 32-feature weight panels, kPanelBytes apart; b: activation panels.
 template <int NT, bool A_MN, bool SPLIT, int CNT>
 __device__ __forceinline__ void tile_kblocks(float (&acc)[1][NT][4], int cnt, uint32_t a_src, uint32_t b_src, uint32_t b_step,
                                              uint32_t m_base, uint32_t n_base, int nt, int lane) {
@@ -86,6 +103,32 @@ __device__ __forceinline__ void tile_stage(float (&acc)[1][NT][4], int cnt, uint
         }
     } else if (nt > 0) {
         tile_kblocks<NT, A_MN, SPLIT, 0>(acc, cnt, a_src, b_src, b_step, m_base, n_base, nt, lane);
+    }
+}
+// CLUSTER, k-split layer 1: the cnt (= CNT when it is a template argument) k-blocks of one ring stage, slot j into acc0
+// for even j and into acc1 for odd j, so that the products of both k-phases overlap; each accumulator still receives
+// its k-blocks in k-block order.  a: K-major 32-feature weight panels; b: the X panels of the stage.
+template <int NT, bool SPLIT, int CNT>
+__device__ __forceinline__ void ksplit_kblocks(float (&acc0)[1][NT][4], float (&acc1)[1][NT][4], int cnt, uint32_t a_src,
+                                               uint32_t b_src, uint32_t b_step, uint32_t m_base, uint32_t n_base, int nt, int lane) {
+#pragma unroll
+    for (int j = 0; j < (CNT > 0 ? CNT : 4); ++j)
+        if (CNT > 0 || j < cnt)
+            warp_mma_kblock<NT, false, false, SPLIT, 1>((j & 1) ? acc1 : acc0, a_src + j * kPanelBytes, m_base, b_src + j * b_step,
+                                                        n_base, nt, lane);
+}
+template <int NT, bool SPLIT>
+__device__ __forceinline__ void ksplit_stage(float (&acc0)[1][NT][4], float (&acc1)[1][NT][4], int cnt, uint32_t a_src,
+                                             uint32_t b_src, uint32_t b_step, uint32_t m_base, uint32_t n_base, int nt, int lane) {
+    if (nt == NT) {                                       // every tile of the accumulators: constant bounds throughout
+        switch (cnt) {
+            case 4: ksplit_kblocks<NT, SPLIT, 4>(acc0, acc1, 4, a_src, b_src, b_step, m_base, n_base, NT, lane); break;
+            case 3: ksplit_kblocks<NT, SPLIT, 3>(acc0, acc1, 3, a_src, b_src, b_step, m_base, n_base, NT, lane); break;
+            case 2: ksplit_kblocks<NT, SPLIT, 2>(acc0, acc1, 2, a_src, b_src, b_step, m_base, n_base, NT, lane); break;
+            default: ksplit_kblocks<NT, SPLIT, 1>(acc0, acc1, 1, a_src, b_src, b_step, m_base, n_base, NT, lane); break;
+        }
+    } else if (nt > 0) {
+        ksplit_kblocks<NT, SPLIT, 0>(acc0, acc1, cnt, a_src, b_src, b_step, m_base, n_base, nt, lane);
     }
 }
 
@@ -136,8 +179,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int L = p.n_layers;
     const int N = p.n_pad;                                   // tile N (rows of this micro-batch, padded to 16)
-    const int rank = CLUSTER ? (int)cluster_ctarank() : 0;  // feature slice [32 rank, 32 rank + 32) of every GEMM
-    const int mb = CLUSTER ? (int)blockIdx.x / p.cluster : (int)blockIdx.x;   // micro-batch of this CTA (in the launch)
+    const int crank = CLUSTER ? (int)cluster_ctarank() : 0;
+    // CLUSTER: ranks >= C are the helpers of a k-split layer 1 (p.ksplit == 2); rank: the feature slice
+    // [32 rank, 32 rank + 32) of every GEMM, which the helper shares with its owner, rank crank - C
+    const bool helper = CLUSTER && crank >= p.cluster;
+    const int rank = helper ? crank - p.cluster : crank;
+    const int mb = CLUSTER ? (int)blockIdx.x / (p.cluster * p.ksplit) : (int)blockIdx.x;   // micro-batch of this CTA (in the launch)
     const int row0 = (p.mu_base + mb) * p.mb_rows;           // first global row of this micro-batch
     const uint32_t a_bytes = CLUSTER ? kPanelBytes : kABytes;   // one k-block of the weight operand: 32 or 128 features
     const uint32_t b_bytes = (uint32_t)N * 128u;             // one 32-feature panel of an activation tile
@@ -149,8 +196,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
     auto recv_bar = [&](int b) { return bar_base + 8u * (2 * p.stages + b); };   // CLUSTER: peer panels of abuf b landed
-    // loss-head transpose scratch [N][kScratchLd] floats behind the barriers (CLUSTER: shared with the k-phase partials)
-    const uint32_t scratch_off = p.stages * stage_bytes + 2u * abuf_bytes + 8u * (2 * p.stages + (CLUSTER ? 2 : 0)) + 128u;
+    const uint32_t land_bar = bar_base + 8u * (2 * p.stages + 2);   // CLUSTER, k-split: the helper's phase sums landed
+    const uint32_t bars_end = p.stages * stage_bytes + 2u * abuf_bytes + 8u * (2 * p.stages + (CLUSTER ? 3 : 0));
+    // CLUSTER, k-split: the helper's phase sums, [2 phases][2 slabs][N / 8 n8 tiles][32 lanes][4] floats = 256 N bytes
+    const uint32_t land_off = (bars_end + 15u) & ~15u;
+    // loss-head transpose scratch [N][kScratchLd] floats behind the barriers (and the landing area)
+    const uint32_t scratch_off = (CLUSTER ? land_off + 256u * (uint32_t)N : bars_end) + 128u;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < p.stages; ++s) {
@@ -160,6 +211,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         if constexpr (CLUSTER) {
             mbar_init(recv_bar(0), 1);                       // the local arm; the peers' bytes are transaction counts
             mbar_init(recv_bar(1), 1);
+            mbar_init(land_bar, 1);
         }
         fence_barrier_init();
     }
@@ -185,28 +237,33 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             };
             if (p.do_fwd) {
                 for (int l = 1; l <= L; ++l) {
+                    if (helper && l > 1) break;              // the helper streams layer 1 only
                     if (idle(p.layers[l - 1].out)) continue;
                     const int nkb = (p.layers[l - 1].in + (int)kBlockK - 1) / (int)kBlockK;
                     const bool with_x = (l == 1) && !(FOLD && p.x_from_global);   // folded pipeline input: staged by the epilogue warps
-                    for (int kb0 = 0; kb0 < nkb; kb0 += p.kps, ++it) {
-                        const int cnt = min(p.kps, nkb - kb0);
+                    // CLUSTER, k-split layer 1: this part's k-blocks (chain_ksplit_kblock), i-th in ring slot i % kps
+                    const bool ks = CLUSTER && l == 1 && p.ksplit > 1;
+                    const int n_kb = ks ? chain_ksplit_count(nkb, helper ? 1 : 0) : nkb;
+                    for (int kb0 = 0; kb0 < n_kb; kb0 += p.kps, ++it) {
+                        const int cnt = min(p.kps, n_kb - kb0);
                         const int s = acquire();
                         const uint32_t a_dst = smem_base + s * stage_bytes;
                         if (elect_one()) {
                             DBG(0, it);
                             mbar_arrive_expect_tx(full_bar(s), (uint32_t)cnt * (a_bytes + (with_x ? b_bytes : 0u)));
                             for (int j = 0; j < cnt; ++j) {
+                                const int kb = ks ? chain_ksplit_kblock(kb0 + j, helper ? 1 : 0) : kb0 + j;
                                 // CLUSTER: the 32 rows of W_l this CTA's features need (32-row box)
-                                tma_load_2d(a_dst + j * a_bytes, p.maps + 2 * (l - 1), full_bar(s), (kb0 + j) * kBlockK, 32 * rank);
+                                tma_load_2d(a_dst + j * a_bytes, p.maps + 2 * (l - 1), full_bar(s), kb * kBlockK, 32 * rank);
                                 if (with_x)
-                                    tma_load_2d(a_dst + stage_b_off + j * b_bytes, p.maps + 2 * L, full_bar(s), (kb0 + j) * kBlockK, row0);
+                                    tma_load_2d(a_dst + stage_b_off + j * b_bytes, p.maps + 2 * L, full_bar(s), kb * kBlockK, row0);
                             }
                         }
                         __syncwarp();
                     }
                 }
             }
-            if (p.do_bwd) {
+            if (p.do_bwd && !helper) {
                 for (int l = L; l >= bwd_lo; --l) {
                     if (idle(p.layers[l - 1].in)) continue;
                     const int nkb = (p.layers[l - 1].out + (int)kBlockK - 1) / (int)kBlockK;
@@ -240,26 +297,25 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         // MMAs of exactly the block its epilogue consumes, so accumulators never leave the warp's registers (lane r reads
         // feature row r through warp_acc_row16).  The activation tile of the next GEMM is written by all 8 warps and
         // published with one named barrier among them.
-        // CLUSTER: a GEMM of more than 4 k-blocks (layer 1 with in > 128) runs in the k-phase form: q is the warp's
-        // k-phase, every warp covers the CTA's 32 features and the (q == 0) warps run the epilogues on the reduced sums.
-        // Every other GEMM runs in the full-K form: each warp owns its tiles (chain_tile_lo) over all k-blocks and runs
-        // their epilogue on its own fragments.
+        // CLUSTER: every GEMM runs in the full-K form: each warp owns its tiles (chain_tile_lo) over all k-blocks and
+        // runs their epilogue on its own fragments (a k-split layer 1: over the k-blocks of the owner and the helper).
+        // The (q == 0) warps stage a dZ_L read from global memory, feature lane by feature lane.
         const int q = warp & 3;
         const int half = (warp - 1) >> 2;
         const int m = (CLUSTER ? 32 * rank : q * 32) + lane;   // feature handled by this thread in the epilogue
-        const bool epi = !CLUSTER || q == 0;                 // this warp runs the epilogues
+        const bool epi = !CLUSTER || q == 0;                 // this warp runs the row-wise epilogues
         // column (= row of the micro-batch) range of this warp, in chunks of 16
         const int n_chunks = N / 16;
         const int c_lo = 16 * ((n_chunks * half) / 2), c_hi = 16 * ((n_chunks * (half + 1)) / 2);
         const int nt = (c_hi - c_lo) / 8;
         float acc[2][NTW][4];                                // this warp's block of the current layer's product
         // CLUSTER, full-K form: this warp's tiles (features t_f0 + g (+8) of fragment register r >> 1, rows
-        // t_n0 + 8 j + 2 (lane & 3) + (r & 1)) and their accumulators
+        // t_n0 + 8 j + 2 (lane & 3) + (r & 1)) and their accumulators (tacc2: the second k-phase of a k-split layer 1)
         const int t_m0 = 16 * ((warp - 1) & 1);              // first feature of the slab, of the CTA's 32
         const int t_f0 = 32 * rank + t_m0 + (lane >> 2);     // feature of fragment registers 0, 1 (2, 3: +8)
         const int t_j0 = chain_tile_lo(N / 8, (warp - 1) >> 1);
         const int t_n0 = 8 * t_j0, tnt = chain_tile_lo(N / 8, ((warp - 1) >> 1) + 1) - t_j0;
-        float tacc[1][NTW / 2][4];
+        float tacc[1][NTW / 2][4], tacc2[1][NTW / 2][4];
         int it = 0, gemm_i = 0;
         // DROP: keep ? x * scale : 0 for feature f of row n of this micro-batch in local layer l (ptx.cuh: dropout_keep)
         uint32_t drop_step = 0u;
@@ -275,55 +331,20 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             mbar_wait(recv_bar(b), (recv_phase >> b) & 1u);
             recv_phase ^= 1u << b;
         };
-        // CLUSTER: acc of warp (0, half) += the partial sums of warps (1..3, half), in that order
-        auto reduce_kphases = [&]() {
-            constexpr int kFrag = 2 * NTW * 4;               // accumulator floats per lane
-            float* red = reinterpret_cast<float*>(smem_gen + scratch_off);   // [3 phases][2 halves][kFrag][32 lanes]
-            if (q != 0) {
-                float* dst = red + ((q - 1) * 2 + half) * kFrag * 32 + lane;
-#pragma unroll
-                for (int i = 0; i < 2; ++i)
-#pragma unroll
-                    for (int j = 0; j < NTW; ++j)
-                        if (j < nt)
-#pragma unroll
-                            for (int r = 0; r < 4; ++r) dst[((i * NTW + j) * 4 + r) * 32] = acc[i][j][r];
-            }
-            asm volatile("bar.sync 2, 256;" ::: "memory");
-            if (q == 0) {
-#pragma unroll
-                for (int ph = 0; ph < 3; ++ph) {
-                    const float* src = red + (ph * 2 + half) * kFrag * 32 + lane;
-#pragma unroll
-                    for (int i = 0; i < 2; ++i)
-#pragma unroll
-                        for (int j = 0; j < NTW; ++j)
-                            if (j < nt)
-#pragma unroll
-                                for (int r = 0; r < 4; ++r) acc[i][j][r] += src[((i * NTW + j) * 4 + r) * 32];
-                }
-            }
-        };
         // D[features, rows] of one layer: A = weights from the ring (K-major forward, MN-major backward), B = the
-        // activation tile (layer 1: X from the ring slots) -> acc.  skip: CLUSTER, no features here (see idle)
+        // activation tile (layer 1: X from the ring slots) -> acc.  One CTA per micro-batch only.
         auto run_gemm = [&](int nkb, bool a_mn, bool b_from_stage, uint32_t bsrc, bool skip) {
             if (threadIdx.x == 32) DBG(1, 2 * gemm_i);
             warp_acc_zero(acc);
-            if constexpr (CLUSTER) {
-                if (!b_from_stage) wait_recv((int)((bsrc - abuf0) / abuf_bytes));
-            }
             for (int kb0 = 0; kb0 < nkb && !skip; kb0 += p.kps, ++it) {
                 const int cnt = min(p.kps, nkb - kb0);
                 const int s = it % p.stages;
                 mbar_wait(full_bar(s), (it / p.stages) & 1);
                 const uint32_t a_src = smem_base + s * stage_bytes;
                 for (int j = 0; j < cnt; ++j) {
-                    if constexpr (CLUSTER) {
-                        if (((kb0 + j) & 3) != q) continue;  // k-phase q of the GEMM
-                    }
                     const uint32_t a_j = a_src + j * a_bytes;
                     const uint32_t b_j = b_from_stage ? a_src + stage_b_off + j * b_bytes : bsrc + (kb0 + j) * b_bytes;
-                    const uint32_t m_base = CLUSTER ? 0u : (uint32_t)q * 32u;
+                    const uint32_t m_base = (uint32_t)q * 32u;
                     if (a_mn)
                         warp_mma_kblock<NTW, true, false, SPLIT>(acc, a_j, m_base, b_j, (uint32_t)c_lo, nt, lane);
                     else
@@ -334,11 +355,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             }
             if (threadIdx.x == 32) DBG(1, 2 * gemm_i + 1);
             ++gemm_i;
-            if constexpr (CLUSTER) reduce_kphases();
         };
-        // CLUSTER, full-K form of run_gemm -> tacc: every k-block of this warp's tiles, summed in k-block order.  With
-        // at most 4 k-blocks that is the order reduce_kphases adds the k-phase partials in, so the two forms agree
-        // bit for bit.
+        // CLUSTER, full-K form of run_gemm -> tacc: every k-block of this warp's tiles, summed in k-block order.
         auto run_gemm_tiles = [&](int nkb, bool a_mn, bool b_from_stage, uint32_t bsrc, bool skip) {
             if (threadIdx.x == 32) DBG(1, 2 * gemm_i);
             warp_acc_zero(tacc);
@@ -358,6 +376,65 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             }
             if (threadIdx.x == 32) DBG(1, 2 * gemm_i + 1);
             ++gemm_i;
+        };
+        // CLUSTER, k-split layer 1 (p.ksplit == 2) -> tacc of the owner: the CTA's k-blocks of this warp's tiles
+        // (chain_ksplit_kblock: ring slot j of a stage holds the CTA's k-block kb0 + j, in k-phase 2 part + ((kb0 + j) & 1)),
+        // the CTA's first k-phase summed into tacc and its second into tacc2, each in k-block order.  The helper's warp
+        // stores its two phase sums into the owner's landing area (st.async, counted on the owner's land_bar); the
+        // owner's warp adds them as ((phase 0 + phase 1) + phase 2) + phase 3.  That is the order in which the four
+        // k-phase partial sums were added when four warps of one CTA split the k-blocks, so the results are unchanged.
+        // Every warp stores and adds, with or without tiles or features (see idle), so the owner's land_bar always
+        // receives the 256 N bytes it is armed with.
+        auto run_gemm_ksplit = [&](int nkb, bool skip) {
+            if (threadIdx.x == 32) DBG(1, 2 * gemm_i);
+            warp_acc_zero(tacc);
+            warp_acc_zero(tacc2);
+            const int n_kb = chain_ksplit_count(nkb, helper ? 1 : 0);
+            for (int kb0 = 0; kb0 < n_kb && !skip; kb0 += p.kps, ++it) {
+                const int cnt = min(p.kps, n_kb - kb0);
+                const int s = it % p.stages;
+                mbar_wait(full_bar(s), (it / p.stages) & 1);
+                const uint32_t a_src = smem_base + s * stage_bytes, b_src = a_src + stage_b_off;
+                // kb0 is a multiple of kps, so an odd kb0 means one slot per stage (kps == 1), of the second k-phase
+                if ((kb0 & 1) == 0)
+                    ksplit_stage<NTW / 2, SPLIT>(tacc, tacc2, cnt, a_src, b_src, b_bytes, (uint32_t)t_m0, (uint32_t)t_n0, tnt, lane);
+                else
+                    ksplit_stage<NTW / 2, SPLIT>(tacc2, tacc, 1, a_src, b_src, b_bytes, (uint32_t)t_m0, (uint32_t)t_n0, tnt, lane);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty_bar(s));
+            }
+            if (threadIdx.x == 32) DBG(1, 2 * gemm_i + 1);
+            ++gemm_i;
+            // this lane's 16 bytes of tile j, phase 2 + h: land + h * 128 N + j * 512 (tiles numbered slab-major)
+            const uint32_t land = smem_base + land_off + (uint32_t)(((((warp - 1) & 1) * (N / 8) + t_j0) * 512) + 16 * lane);
+            const uint32_t phase_bytes = 128u * (uint32_t)N;
+            if (helper) {
+#pragma unroll
+                for (int j = 0; j < NTW / 2; ++j) {
+                    if (j < tnt) {
+                        const uint32_t bar = mapa_shared(land_bar, (uint32_t)rank);
+                        const uint4 v2 = make_uint4(__float_as_uint(tacc[0][j][0]), __float_as_uint(tacc[0][j][1]),
+                                                    __float_as_uint(tacc[0][j][2]), __float_as_uint(tacc[0][j][3]));
+                        const uint4 v3 = make_uint4(__float_as_uint(tacc2[0][j][0]), __float_as_uint(tacc2[0][j][1]),
+                                                    __float_as_uint(tacc2[0][j][2]), __float_as_uint(tacc2[0][j][3]));
+                        st_async_v4(mapa_shared(land + j * 512u, (uint32_t)rank), v2, bar);
+                        st_async_v4(mapa_shared(land + phase_bytes + j * 512u, (uint32_t)rank), v3, bar);
+                    }
+                }
+                return;
+            }
+            if (threadIdx.x == 32) mbar_arrive_expect_tx(land_bar, 2u * phase_bytes);
+            mbar_wait(land_bar, 0);
+#pragma unroll
+            for (int j = 0; j < NTW / 2; ++j) {
+                if (j < tnt) {
+                    const uint4 v2 = lds_v4(land + j * 512u), v3 = lds_v4(land + phase_bytes + j * 512u);
+                    const float h2[4] = {__uint_as_float(v2.x), __uint_as_float(v2.y), __uint_as_float(v2.z), __uint_as_float(v2.w)};
+                    const float h3[4] = {__uint_as_float(v3.x), __uint_as_float(v3.y), __uint_as_float(v3.z), __uint_as_float(v3.w)};
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) tacc[0][j][r] = ((tacc[0][j][r] + tacc2[0][j][r]) + h2[r]) + h3[r];
+                }
+            }
         };
         // CLUSTER, full-K form: element r of this warp's tile j
         auto t_row = [&](int j, int r) { return t_n0 + 8 * j + 2 * (lane & 3) + (r & 1); };
@@ -447,17 +524,19 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 const float bias = m_ok ? __ldg(p.W + ly.w_off + (int64_t)m * ly.ldw + ly.in) : 0.f;
                 const bool is_logits = (l == L) && p.do_loss;
                 const int nkb_f = (ly.in + (int)kBlockK - 1) / (int)kBlockK;
-                const bool tile = CLUSTER && nkb_f <= 4;      // full-K form
+                const bool tile = CLUSTER;                   // full-K form
                 float t_bias[2] = {0.f, 0.f};                // full-K form: the biases of features t_feat(0), t_feat(2)
-                if (tile) {
+                if (tile && !helper) {
 #pragma unroll
                     for (int h = 0; h < 2; ++h)
                         if (t_feat(2 * h) < ly.out) t_bias[h] = __ldg(p.W + ly.w_off + (int64_t)t_feat(2 * h) * ly.ldw + ly.in);
                 }
                 // layer 1 reads X from its ring slots (TMA), or - folded pipeline input - from abuf 1 (staged above)
                 const bool x_glob = FOLD && (l == 1) && p.x_from_global;
-                if (tile) run_gemm_tiles(nkb_f, false, l == 1, abuf0 + buf * abuf_bytes, idle(ly.out));
+                if (tile && l == 1 && p.ksplit > 1) run_gemm_ksplit(nkb_f, idle(ly.out));
+                else if (tile) run_gemm_tiles(nkb_f, false, l == 1, abuf0 + buf * abuf_bytes, idle(ly.out));
                 else run_gemm(nkb_f, false, l == 1 && !x_glob, abuf0 + (x_glob ? 1 : buf) * abuf_bytes, idle(ly.out));
+                if (helper) break;                           // its phase sums are in the owner: the helper is done
                 if (l > 1) buf ^= 1;                         // layer l read buf, wrote buf^1
                 else buf = 0;                                // layer 1 writes abuf 0
                 if (p.sync_debug) asm volatile("bar.sync 2, 256;" ::: "memory");   // racecheck aid, see kernels.h
@@ -535,13 +614,10 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     // Step 1: the class-lane warps (q == 0, both halves) transpose logits (+bias) into a [row][class]
                     // scratch in smem.  Step 2: each lane of warp (0, 0) owns ROWS, loops over the <= 32 classes in
                     // registers - no cross-lane reductions except (MSE) one max and one sum for the whole micro-batch.
-                    // CLUSTER: the <= 32 classes are rank 0's features.  Full-K form: every warp transposes its own
-                    // tiles.  K-phase form: the scratch is where the k-phase partials were (all of them read before
-                    // the barrier)
+                    // CLUSTER: the <= 32 classes are rank 0's features, and every warp transposes its own tiles.
                     const int C = ly.out;
                     float* scratch = reinterpret_cast<float*>(smem_gen + scratch_off);   // [N][kScratchLd]
                     float loss = 0.f;
-                    if constexpr (CLUSTER) { if (!tile) asm volatile("bar.sync 2, 256;" ::: "memory"); }
                     if (tile) {
 #pragma unroll
                         for (int j = 0; j < NTW / 2; ++j)
@@ -706,7 +782,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 st_relaxed_sys(p.out_flag, pp_epoch);
             }
         }
-        if (p.do_bwd && !(p.do_fwd && p.do_loss)) {
+        if (p.do_bwd && !(p.do_fwd && p.do_loss) && !helper) {
             // backward-only launch (pipeline stage): stage dZ_L = gout (.) relu'(act_L) into smem
             const ChainLayer& ly = p.layers[L - 1];
             const bool m_ok = m < ly.out;
@@ -727,7 +803,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             else publish();
             wbuf ^= 1;
         }
-        if (p.do_bwd) {
+        if (p.do_bwd && !helper) {
             // the loss head / boundary loader wrote dZ_L into the buffer after the last forward output
             for (int l = L; l >= bwd_lo; --l) {
                 const ChainLayer& ly = p.layers[l - 1];
@@ -897,15 +973,14 @@ int chain_cluster_size(const ChainLayer* layers, int n_layers, bool do_fwd, bool
     return std::min(4, std::max(1, (w + 31) / 32));
 }
 
-// Cluster form: the ring holds 32-row weight panels (plus the X tiles of layer 1), the k-phase partials of warps
-// (1..3, half) share the scratch with the loss head.
+// Cluster form: the ring holds 32-row weight panels (plus the X tiles of layer 1); behind the three cluster-form
+// barriers, the landing area of a k-split layer 1's helper (256 N bytes, 16-byte aligned) and the loss head's scratch.
 bool chain_cluster_budget(int mb_rows, int cluster, bool split, int* kps_out, int* stages_out, int* smem_bytes_out) {
     if (cluster <= 1) return chain_budget(mb_rows, split, kps_out, stages_out, smem_bytes_out);
     if (cluster > 4 || mb_rows < 1 || mb_rows > 128) return false;
     const int n_pad = (mb_rows + 15) / 16 * 16;
     const int abuf_bytes = 4 * n_pad * 128;
-    const int partial_bytes = 3 * 2 * (2 * chain_ntw(n_pad) * 4) * 32 * 4;
-    const int scratch_bytes = std::max(partial_bytes, n_pad * kScratchLd * 4 + 256);
+    const int scratch_bytes = 16 + 256 * n_pad + n_pad * kScratchLd * 4 + 256;
     const int budget = 222 * 1024 - 2 * abuf_bytes - scratch_bytes;
     int kps = 4, stage_bytes = 0, stages = 0;
     for (; kps >= 1; kps >>= 1) {
@@ -917,7 +992,7 @@ bool chain_cluster_budget(int mb_rows, int cluster, bool split, int* kps_out, in
     if (stages > 8) stages = 8;
     *kps_out = kps;
     *stages_out = stages;
-    *smem_bytes_out = stages * stage_bytes + 2 * abuf_bytes + 1024 + 8 * (2 * stages + 2) + 128 + scratch_bytes;
+    *smem_bytes_out = stages * stage_bytes + 2 * abuf_bytes + 1024 + 8 * (2 * stages + 3) + 128 + scratch_bytes;
     return true;
 }
 
@@ -950,6 +1025,9 @@ const char* chain_plan(ChainPlan* plan, const ChainParams& params, const float* 
                                      p.ready != nullptr, fold);
     if (C > 1 && (p.ready != nullptr || fold)) return "chain_plan: gated and folded launches run one CTA per micro-batch";
     p.cluster = C;
+    // a cluster launch whose layer 1 has more than 4 k-blocks runs it on P = 2 CTAs per feature slice (k-split)
+    const int P = C > 1 && p.do_fwd && (p.layers[0].in + (int)kBlockK - 1) / (int)kBlockK > 4 ? 2 : 1;
+    p.ksplit = P;
     std::vector<CUtensorMap> host(2 * L + 1);
     for (int l = 0; l < L; ++l) {
         const ChainLayer& ly = p.layers[l];
@@ -973,8 +1051,9 @@ const char* chain_plan(ChainPlan* plan, const ChainParams& params, const float* 
     p.kps = kps;
     p.stages = stages;
     plan->smem_bytes = smem;
-    plan->grid = n_mubatches * C;
+    plan->grid = n_mubatches * C * P;
     plan->cluster = C;
+    plan->ksplit = P;
     return nullptr;
 }
 
@@ -1008,7 +1087,7 @@ cudaError_t chain_configure() {
     return cudaSuccess;
 }
 
-// grid = micro-batches x plan.cluster, cluster dims (plan.cluster, 1, 1)
+// grid = micro-batches x plan.cluster x plan.ksplit, cluster dims (plan.cluster x plan.ksplit, 1, 1)
 template <bool SPLIT, int NTW, bool CE, bool DROP>
 static cudaError_t chain_launch_cluster(const ChainPlan& plan, cudaStream_t stream) {
     cudaLaunchConfig_t cfg = {};
@@ -1018,7 +1097,7 @@ static cudaError_t chain_launch_cluster(const ChainPlan& plan, cudaStream_t stre
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)plan.cluster;
+    attr[0].val.clusterDim.x = (unsigned)(plan.cluster * plan.ksplit);
     attr[0].val.clusterDim.y = 1;
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;

@@ -321,6 +321,7 @@ public:
     int64_t graph_nodes() { return engine_->graph_nodes(); }
     bool uses_chain() { return engine_->uses_chain(); }
     int chain_cluster() { return engine_->chain_cluster(); }
+    int chain_ksplit() { return engine_->chain_ksplit(); }
     bool coalesced() { return engine_->coalesced(); }
     int64_t main_stream() { return reinterpret_cast<int64_t>(engine_->main_stream()); }
     std::string describe() { return engine_->describe(); }
@@ -420,6 +421,7 @@ void bind_runtime(py::module_& m) {
         .def("graph_nodes", &PyEngine::graph_nodes)
         .def("uses_chain", &PyEngine::uses_chain)
         .def("chain_cluster", &PyEngine::chain_cluster)
+        .def("chain_ksplit", &PyEngine::chain_ksplit)
         .def("coalesced", &PyEngine::coalesced)
         .def("main_stream", &PyEngine::main_stream)
         .def("describe", &PyEngine::describe)

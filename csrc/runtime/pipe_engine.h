@@ -158,6 +158,12 @@ public:
         for (const ChainPlan& cp : chain_plans_) c = std::max(c, cp.cluster);
         return c;
     }
+    // CTAs per feature slice in layer 1 of the chain launches (the largest over the plan; 0 without chain launches)
+    int chain_ksplit() const {
+        int k = 0;
+        for (const ChainPlan& cp : chain_plans_) k = std::max(k, cp.ksplit);
+        return k;
+    }
     cudaStream_t main_stream() { return streams_[0]; }
     const EngineConfig& config() const { return cfg_; }
     // per layer: the DpProto under which its update runs (which replica owns which momentum entries)

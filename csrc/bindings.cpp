@@ -196,6 +196,58 @@ static void argmax_correct(const Tensor& pred, const Tensor& target, Tensor& cor
                                        pred.size(0), pred.size(1), correct.data_ptr<int>(), cur_stream()), "argmax_correct");
 }
 
+// the device permutation of the training set (ptx.cuh: shuffle_index) at int64 positions in [0, n)
+static Tensor shuffle_index(int64_t n, uint64_t seed, int64_t epoch, const Tensor& positions) {
+    TORCH_CHECK(n >= 1 && n < (int64_t(1) << 32), "shuffle_index: n must lie in [1, 2**32)");
+    TORCH_CHECK(positions.is_cuda() && positions.scalar_type() == torch::kInt64, "shuffle_index: positions must be int64 CUDA");
+    TORCH_CHECK(epoch >= 0, "shuffle_index: the epoch must be >= 0");
+    const Tensor q = positions.contiguous();
+    if (q.numel() > 0)
+        TORCH_CHECK(q.min().item<int64_t>() >= 0 && q.max().item<int64_t>() < n, "shuffle_index: positions must lie in [0, n)");
+    c10::cuda::CUDAGuard guard(q.device());
+    Tensor out = torch::empty_like(q);
+    cuda_ok(ssb::launch_shuffle_index((uint32_t)n, seed, (uint32_t)(epoch & 0xffffffffLL), q.data_ptr<int64_t>(),
+                                      out.data_ptr<int64_t>(), (long)q.numel(), cur_stream()), "shuffle_index");
+    return out;
+}
+// the staging gather on its own (launch_gather_rows): rows of global batch `batch` of this rank into x_dst / y_dst, whose
+// row pitch is their stride(0); x_src / y_src are the whole dense dataset
+static void gather_rows(const c10::optional<Tensor>& x_src, const c10::optional<Tensor>& y_src, uint64_t seed, int64_t epoch,
+                        int64_t gbs, int64_t dp, int64_t rank, int64_t batch, const c10::optional<Tensor>& x_dst,
+                        const c10::optional<Tensor>& y_dst) {
+    TORCH_CHECK(x_src.has_value() == x_dst.has_value() && y_src.has_value() == y_dst.has_value(),
+                "gather_rows: every source needs a destination and the reverse");
+    TORCH_CHECK(x_src.has_value() || y_src.has_value(), "gather_rows: nothing to gather");
+    const Tensor& any_src = x_src.has_value() ? *x_src : *y_src;
+    const Tensor& any_dst = x_dst.has_value() ? *x_dst : *y_dst;
+    for (const auto* s : {&x_src, &y_src}) {
+        if (!s->has_value()) continue;
+        const Tensor& t = **s;
+        TORCH_CHECK(t.is_cuda() && t.scalar_type() == torch::kFloat32 && t.dim() == 2 && t.is_contiguous(),
+                    "gather_rows: sources must be dense 2-D fp32 CUDA tensors");
+        TORCH_CHECK(t.size(0) == any_src.size(0) && t.device() == any_src.device(), "gather_rows: sources disagree");
+    }
+    for (const auto* d : {&x_dst, &y_dst}) {
+        if (!d->has_value()) continue;
+        check_mat(**d, "gather_rows destination");
+        TORCH_CHECK((*d)->size(0) == any_dst.size(0) && (*d)->device() == any_src.device(), "gather_rows: destinations disagree");
+    }
+    if (x_src.has_value()) TORCH_CHECK(x_dst->size(1) == x_src->size(1), "gather_rows: x widths differ");
+    if (y_src.has_value()) TORCH_CHECK(y_dst->size(1) == y_src->size(1), "gather_rows: y widths differ");
+    TORCH_CHECK(any_src.size(0) < (int64_t(1) << 32) && epoch >= 0 && gbs < (1 << 30) && dp < (1 << 30) && batch < (1 << 30),
+                "gather_rows: argument out of range");
+    const ssb::ShuffleSpec spec{(uint32_t)any_src.size(0), seed, (uint32_t)(epoch & 0xffffffffLL), (int)gbs, (int)dp, (int)rank};
+    const int rows = (int)any_dst.size(0);
+    const char* err = ssb::shuffle_spec_check(spec, (int)batch, rows);
+    TORCH_CHECK(err == nullptr, "gather_rows: ", err ? err : "");
+    c10::cuda::CUDAGuard guard(any_src.device());
+    cuda_ok(ssb::launch_gather_rows(x_src ? x_src->data_ptr<float>() : nullptr, y_src ? y_src->data_ptr<float>() : nullptr,
+                                    spec, (int)batch, x_dst ? x_dst->data_ptr<float>() : nullptr, x_dst ? ld_of(*x_dst) : 0,
+                                    y_dst ? y_dst->data_ptr<float>() : nullptr, y_dst ? ld_of(*y_dst) : 0, rows,
+                                    x_src ? (int)x_src->size(1) : 0, y_src ? (int)y_src->size(1) : 0, cur_stream()),
+            "gather_rows");
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.doc() = "shallowspeed_b200 native module: sm_90a kernels + C++ pipeline runtime";
     m.def("linear_fwd", &linear_fwd, py::arg("x"), py::arg("W"), py::arg("bias"), py::arg("bias_stride"), py::arg("relu"),
@@ -215,6 +267,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("sgd_momentum_", &sgd_momentum_, py::arg("w"), py::arg("g"), py::arg("v"), py::arg("lr"), py::arg("momentum"),
           py::arg("weight_decay"), py::arg("nesterov"));
     m.def("argmax_correct", &argmax_correct);
+    m.def("shuffle_index", &shuffle_index, py::arg("n"), py::arg("seed"), py::arg("epoch"), py::arg("positions"));
+    m.def("gather_rows", &gather_rows, py::arg("x_src"), py::arg("y_src"), py::arg("seed"), py::arg("epoch"), py::arg("gbs"),
+          py::arg("dp"), py::arg("rank"), py::arg("batch"), py::arg("x_dst"), py::arg("y_dst"));
     m.def("gemm_kernel_count", &ssb::gemm_kernel_count);
     m.def("chain_budget", [](int mb_rows, bool split) {
         int kps = 0, stages = 0, smem = 0;

@@ -335,4 +335,73 @@ cudaError_t launch_argmax_correct(const float* pred, int ldp, const float* targe
     return cudaGetLastError();
 }
 
+// ---------------------------------------------------------------- shuffled input staging
+// one warp per destination row: lane 0 walks the permutation, the warp copies the sample's x and y rows
+__global__ void __launch_bounds__(256) gather_rows_kernel(const float* __restrict__ x_src, const float* __restrict__ y_src,
+                                                          ShuffleSpec spec, int batch, float* __restrict__ x_dst, int ldx,
+                                                          float* __restrict__ y_dst, int ldy, int rows, int in_dim,
+                                                          int out_dim, int vec) {
+    const int lane = threadIdx.x & 31;
+    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= rows) return;
+    uint32_t s = 0;
+    if (lane == 0) {
+        const int64_t q = (int64_t)batch * spec.gbs + (int64_t)row * spec.dp + spec.rank;
+        s = shuffle_index(spec.n, spec.seed, spec.epoch, (uint32_t)q);
+    }
+    s = __shfl_sync(0xffffffffu, s, 0);
+    if (x_src != nullptr) {
+        const float* src = x_src + (size_t)s * in_dim;
+        float* dst = x_dst + (size_t)row * ldx;
+        if (vec) {
+            const float4* s4 = reinterpret_cast<const float4*>(src);
+            float4* d4 = reinterpret_cast<float4*>(dst);
+#pragma unroll 4
+            for (int c = lane; c < (in_dim >> 2); c += 32) d4[c] = __ldg(s4 + c);
+        } else {
+            for (int c = lane; c < in_dim; c += 32) dst[c] = __ldg(src + c);
+        }
+    }
+    if (y_src != nullptr) {
+        const float* src = y_src + (size_t)s * out_dim;
+        float* dst = y_dst + (size_t)row * ldy;
+        for (int c = lane; c < out_dim; c += 32) dst[c] = __ldg(src + c);
+    }
+}
+const char* shuffle_spec_check(const ShuffleSpec& spec, int batch, int rows) {
+    if (spec.n == 0u) return "the dataset is empty";
+    if (spec.dp < 1 || spec.rank < 0 || spec.rank >= spec.dp) return "the DP rank must lie in [0, dp)";
+    if (spec.gbs < 1 || rows < 0 || (int64_t)rows * spec.dp > spec.gbs) return "the rows of a rank exceed its share of the global batch";
+    if (batch < 0 || (int64_t)(batch + 1) * spec.gbs > (int64_t)spec.n) return "the batch lies past the last full global batch";
+    return nullptr;
+}
+
+cudaError_t launch_gather_rows(const float* x_src, const float* y_src, const ShuffleSpec& spec, int batch, float* x_dst,
+                               int ldx, float* y_dst, int ldy, int rows, int in_dim, int out_dim, cudaStream_t stream) {
+    if (shuffle_spec_check(spec, batch, rows) != nullptr) return cudaErrorInvalidValue;
+    if ((x_src != nullptr && (x_dst == nullptr || ldx < in_dim)) || (y_src != nullptr && (y_dst == nullptr || ldy < out_dim)))
+        return cudaErrorInvalidValue;
+    if (rows == 0 || (x_src == nullptr && y_src == nullptr)) return cudaSuccess;
+    const int vec = x_src != nullptr && in_dim % 4 == 0 && ldx % 4 == 0 &&
+                    ((reinterpret_cast<uintptr_t>(x_src) | reinterpret_cast<uintptr_t>(x_dst)) & 15) == 0;
+    gather_rows_kernel<<<(rows + 7) / 8, 256, 0, stream>>>(x_src, y_src, spec, batch, x_dst, ldx, y_dst, ldy, rows, in_dim,
+                                                          out_dim, vec);
+    return cudaGetLastError();
+}
+
+__global__ void shuffle_index_kernel(uint32_t n, uint64_t seed, uint32_t epoch, const int64_t* __restrict__ q,
+                                     int64_t* __restrict__ out, long count) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < count; i += (long)gridDim.x * blockDim.x)
+        out[i] = (int64_t)shuffle_index(n, seed, epoch, (uint32_t)q[i]);
+}
+cudaError_t launch_shuffle_index(uint32_t n, uint64_t seed, uint32_t epoch, const int64_t* q, int64_t* out, long count,
+                                 cudaStream_t stream) {
+    if (n == 0u) return cudaErrorInvalidValue;
+    if (count <= 0) return cudaSuccess;
+    long blocks = (count + 255) / 256;
+    if (blocks > 132 * 8) blocks = 132 * 8;
+    shuffle_index_kernel<<<(int)blocks, 256, 0, stream>>>(n, seed, epoch, q, out, count);
+    return cudaGetLastError();
+}
+
 }  // namespace ssb

@@ -7,6 +7,7 @@
 #include <cuda_runtime.h>
 
 #include "dropout.h"
+#include "shuffle.h"
 
 namespace ssb {
 
@@ -352,5 +353,17 @@ cudaError_t launch_sgd_momentum(float* w, const float* g, const float* lr, const
 // correct[0] += #rows with argmax(pred) == argmax(target)
 cudaError_t launch_argmax_correct(const float* pred, int ldp, const float* target, int ldt, int rows, int cols,
                                   int* correct, cudaStream_t stream);
+// Shuffled input staging (shuffle.h): destination row j of global batch `batch` receives dataset row
+// shuffle_index(spec.n, spec.seed, spec.epoch, batch * spec.gbs + j * spec.dp + spec.rank).  x_src [spec.n, in_dim] and
+// y_src [spec.n, out_dim] are dense; columns [0, in_dim) of x_dst (pitch ldx) and [0, out_dim) of y_dst (pitch ldy) are
+// written, the pitch padding is not.  Either source may be nullptr (its destination is then untouched).  One warp per row;
+// x rows move as float4 when in_dim % 4 == 0, ldx % 4 == 0 and both x pointers are 16-byte aligned.
+// shuffle_spec_check: nullptr if `rows` rows of global batch `batch` are in range under spec, else the reason (host only).
+const char* shuffle_spec_check(const ShuffleSpec& spec, int batch, int rows);
+cudaError_t launch_gather_rows(const float* x_src, const float* y_src, const ShuffleSpec& spec, int batch, float* x_dst,
+                               int ldx, float* y_dst, int ldy, int rows, int in_dim, int out_dim, cudaStream_t stream);
+// out[i] = shuffle_index(n, seed, epoch, q[i]) for count positions q[i] < n (test surface of the device helper)
+cudaError_t launch_shuffle_index(uint32_t n, uint64_t seed, uint32_t epoch, const int64_t* q, int64_t* out, long count,
+                                 cudaStream_t stream);
 
 }  // namespace ssb

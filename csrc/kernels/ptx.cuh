@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include "dropout.h"
+#include "shuffle.h"
 
 namespace ssb {
 
@@ -377,6 +378,33 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1
 // Every site that drops or scales calls this, so the kernels and the torch oracle draw the same bits.
 __device__ __forceinline__ bool dropout_keep(const DropoutSpec& d, uint32_t layer, uint32_t step, uint32_t f, uint32_t s) {
     return philox4x32_10(make_uint4(f, s, layer, step), (uint32_t)d.seed, (uint32_t)(d.seed >> 32)).x >= d.threshold;
+}
+
+// ------------------------------------------------------------------ training-set shuffling
+// Dataset row held by position q < n in epoch `epoch` (ShuffleSpec): a 6-round balanced Feistel network on w bits (w the
+// smallest even integer >= 2 with 2^w >= n, halves of h = w / 2 bits), whose round function is word 0 of Philox4x32-10
+// with counter (R, round, epoch, "SHUF") and key (seed lo, seed hi), masked to h bits.  Cycle walking (apply the network
+// again while the value is >= n) turns the permutation of [0, 2^w) into one of [0, n); 2^w <= 4n bounds the expected
+// number of passes by 4.  ops/functional.py: shuffle_index is the same map on torch tensors.
+__device__ __forceinline__ uint32_t shuffle_index(uint32_t n, uint64_t seed, uint32_t epoch, uint32_t q) {
+    int w = 2;
+    while ((1ull << w) < (uint64_t)n) w += 2;
+    const int h = w >> 1;
+    const uint32_t mask = (1u << h) - 1u;
+    const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
+    uint32_t x = q;
+    do {
+        uint32_t L = x >> h, R = x & mask;
+#pragma unroll 1
+        for (uint32_t i = 0; i < 6; ++i) {
+            const uint32_t f = philox4x32_10(make_uint4(R, i, epoch, 0x53485546u), k0, k1).x & mask;
+            const uint32_t t = L ^ f;
+            L = R;
+            R = t;
+        }
+        x = (L << h) | R;
+    } while (x >= n);
+    return x;
 }
 
 }  // namespace ssb

@@ -282,6 +282,46 @@ public:
         held_[hold_i_ & 1] = {x, y};
         ++hold_i_;
     }
+    // shuffled staging (PipeEngine::stage_gather): x_all [n, in_dim] / y_all [n, out_dim], the whole dataset on this
+    // engine's device (each is ignored by a stage that does not take it); rows of global batch `batch` of DP rank `rank`
+    // under the epoch's permutation
+    void stage_gather(const c10::optional<torch::Tensor>& x_all, const c10::optional<torch::Tensor>& y_all, uint64_t seed,
+                      int64_t epoch, int64_t gbs, int64_t dp, int64_t rank, int64_t batch) {
+        const auto& cfg = engine_->config();
+        const int64_t rows = (int64_t)cfg.n_mu * cfg.mb_rows;
+        int64_t n = -1;
+        const float *xp = nullptr, *yp = nullptr;
+        auto check = [&](const torch::Tensor& t, int64_t cols, const char* name) {
+            TORCH_CHECK(t.is_cuda() && t.device() == weights_.device(), "stage_gather: ", name, " must live on the engine's device");
+            TORCH_CHECK(t.scalar_type() == torch::kFloat32 && t.is_contiguous() && t.dim() == 2 && t.size(1) == cols,
+                        "stage_gather: ", name, " must be a dense fp32 [n, ", cols, "] tensor");
+            TORCH_CHECK(n < 0 || t.size(0) == n, "stage_gather: x and y hold different numbers of rows");
+            n = t.size(0);
+        };
+        // like stage_inputs, a stage ignores the source it does not take (x unless first, y unless last)
+        if (x_all.has_value() && cfg.is_first) { check(*x_all, cfg.in_dim, "x"); xp = x_all->data_ptr<float>(); }
+        if (y_all.has_value() && cfg.is_last) { check(*y_all, cfg.out_dim, "y"); yp = y_all->data_ptr<float>(); }
+        TORCH_CHECK(n < (int64_t(1) << 32) && epoch >= 0 && gbs < (1 << 30) && dp < (1 << 30) && batch < (1 << 30),
+                    "stage_gather: argument out of range");
+        const ShuffleSpec spec{(uint32_t)std::max<int64_t>(n, 0), seed, (uint32_t)(epoch & 0xffffffffLL), (int)gbs, (int)dp,
+                               (int)rank};
+        if (n >= 0) {   // a stage without inputs gathers nothing (it only keeps the staging-set protocol)
+            const char* err = shuffle_spec_check(spec, (int)batch, (int)rows);
+            TORCH_CHECK(err == nullptr, "stage_gather: ", err ? err : "");
+        }
+        engine_->stage_gather(xp, yp, spec, (int)batch);
+        held_[hold_i_ & 1] = {x_all, y_all};   // the gather is asynchronous, like the copies of stage_inputs
+        ++hold_i_;
+    }
+    // test-facing: the two staging buffers of set `set`, over their whole row pitch (x [rows, act ld 0], y [rows, y ld])
+    std::pair<torch::Tensor, torch::Tensor> staging(int set) {
+        const auto& cfg = engine_->config();
+        TORCH_CHECK(set == 0 || set == 1, "PipeEngine.staging: set must be 0 or 1");
+        const int64_t rows = (int64_t)cfg.n_mu * cfg.mb_rows;
+        return {view_of(engine_->x_staging_set(set), rows, engine_->act_ld(0), engine_->act_ld(0)),
+                view_of(engine_->y_staging_set(set), rows, engine_->y_ld(), engine_->y_ld())};
+    }
+    int fill_set() { return engine_->fill_set(); }
     int n_mubatches() { return engine_->config().n_mu; }
     void run() { engine_->run(); }
     void set_lr(double lr) {
@@ -400,6 +440,10 @@ void bind_runtime(py::module_& m) {
         .def("boundary_lds", &PyEngine::boundary_lds)
         .def("build", &PyEngine::build)
         .def("stage_inputs", &PyEngine::stage_inputs)
+        .def("stage_gather", &PyEngine::stage_gather, py::arg("x_all"), py::arg("y_all"), py::arg("seed"), py::arg("epoch"),
+             py::arg("gbs"), py::arg("dp"), py::arg("rank"), py::arg("batch"))
+        .def("staging", &PyEngine::staging, py::arg("set"))
+        .def("fill_set", &PyEngine::fill_set)
         .def("n_mubatches", &PyEngine::n_mubatches)
         .def("run", &PyEngine::run)
         .def("set_lr", &PyEngine::set_lr, py::arg("lr"))

@@ -1252,6 +1252,22 @@ void PipeEngine::stage_inputs(const float* x, const float* y) {
     staged_ = true;
 }
 
+// The shuffled counterpart of stage_inputs, with the same staging-set protocol: one gather launch on the copy stream picks
+// global batch `batch`'s rows of this rank out of the device-resident dataset (x_all / y_all: [spec.n, in_dim / out_dim],
+// nullptr where this stage takes no such input).  The spec travels by value, so the captured step graphs do not change.
+void PipeEngine::stage_gather(const float* x_all, const float* y_all, const ShuffleSpec& spec, int batch) {
+    const int set = fill_set_;
+    const int rows = cfg_.n_mu * cfg_.mb_rows;
+    const float* x = cfg_.is_first ? x_all : nullptr;
+    const float* y = cfg_.is_last ? y_all : nullptr;
+    CUDA_CHECK(cudaStreamWaitEvent(copy_stream_, ev_done_[set], 0));
+    if (x != nullptr || y != nullptr)   // a middle stage launches nothing
+        CUDA_CHECK(launch_gather_rows(x, y, spec, batch, x_stage_sets_[set], act_ld_[0], y_stage_sets_[set], y_ld_, rows,
+                                      cfg_.in_dim, cfg_.out_dim, copy_stream_));
+    CUDA_CHECK(cudaEventRecord(ev_copy_[set], copy_stream_));
+    staged_ = true;
+}
+
 void PipeEngine::run() {
     if (!built_) throw std::runtime_error("PipeEngine::run before build");
     const int set = fill_set_;

@@ -119,7 +119,10 @@ public:
     // input staging ------------------------------------------------------------------
     // dense row-major host/device sources: x [n_mu*mb_rows, in_dim], y [n_mu*mb_rows, out_dim]
     void stage_inputs(const float* x, const float* y);
-    void run();                       // one step (graph launch or eager plan walk) on the main stream
+    // the same staging from a device-resident dataset, rows picked by the epoch's permutation (shuffle.h): x_all
+    // [spec.n, in_dim], y_all [spec.n, out_dim], either nullable; one gather launch on the copy stream
+    void stage_gather(const float* x_all, const float* y_all, const ShuffleSpec& spec, int batch);
+    void run();                      // one step (graph launch or eager plan walk) on the main stream
     // learning rate of the steps run from now on.  Every update op reads it from the device slot of its staging set;
     // run() rewrites that slot on the copy stream only when it holds a different value.
     void set_lr(float lr) { lr_ = lr; }
@@ -147,6 +150,9 @@ public:
     float* probs_ptr(int mu) { return probs_[mu]; }
     float* x_staging() { return x_stage_; }
     float* y_staging() { return y_stage_; }
+    float* x_staging_set(int set) { return x_stage_sets_[set & 1]; }
+    float* y_staging_set(int set) { return y_stage_sets_[set & 1]; }
+    int fill_set() const { return fill_set_; }        // the staging set the next stage_inputs / stage_gather fills
     int y_ld() const { return y_ld_; }
     int64_t kernels_per_step() const { return kernels_per_step_; }
     int64_t graph_nodes() const { return graph_nodes_; }

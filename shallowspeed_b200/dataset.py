@@ -16,6 +16,13 @@ per step) or resident in HBM (``device=...``; 59 500 x 784 fp32 = 187 MB, nothin
 80 GB); ``write_reference_files`` stores any dataset in the reference's on-disk format
 (x_{split}.parquet + y_{split}.npy) so the unmodified reference can train on identical
 data.
+
+Shuffling (``shuffle_seed=...``, training data only): every rank keeps the whole file, and
+global position q of epoch e (``set_epoch``) holds row ``shuffle_index(N, seed, e, q)`` of
+it (``ops.functional``: a keyed Feistel permutation of [0, N)).  Local row n of DP rank r
+in global batch b stays position ``b * GBS + n * dp + r``; an epoch has ``N // GBS``
+batches, and the ``N mod GBS`` positions past the last one are dropped (different samples
+every epoch).  ``shuffle_seed=None`` is the unshuffled layout above.
 """
 from __future__ import annotations
 
@@ -24,6 +31,8 @@ from typing import Optional
 
 import numpy as np
 import torch
+
+from .ops import functional as F
 
 N_TRAIN, N_VAL, N_FEATURES, N_CLASSES = 59500, 10500, 784, 10  # reference download_dataset.py:16-18
 
@@ -64,7 +73,14 @@ def write_reference_files(save_dir, overwrite: bool = False, **kw):
 class Dataset:
     def __init__(self, save_dir, global_batch_size, mubatch_size, validation=False,
                  synthetic: Optional[bool] = None, device=None, pin_memory: bool = False,
-                 n_samples: Optional[int] = None, n_features: int = N_FEATURES, n_classes: int = N_CLASSES):
+                 n_samples: Optional[int] = None, n_features: int = N_FEATURES, n_classes: int = N_CLASSES,
+                 shuffle_seed: Optional[int] = None):
+        self.shuffle_seed = F.check_shuffle_seed(shuffle_seed)
+        if validation and self.shuffle_seed is not None:
+            raise ValueError("a validation dataset is never shuffled (shuffle_seed must be None)")
+        self.epoch = 0
+        self.dp_rank, self.dp_size = 0, 1
+        self._ids = None          # (epoch, batch_id, file rows of the local batch on the data's device)
         if save_dir is not None:
             save_dir = Path(save_dir)
         if synthetic is None:
@@ -99,13 +115,21 @@ class Dataset:
         assert self.global_batch_size % DP_size == 0
         assert (self.global_batch_size // DP_size) % self.mubatch_size == 0, "μBatchsize must divide batchsize!"
         self.local_batch_size = self.global_batch_size // DP_size
+        self.dp_rank, self.dp_size = int(DP_rank), int(DP_size)
         x, y = self._read_all()
         assert len(x) == len(y)
+        if self.shuffle:   # every rank keeps the whole file: the permutation picks any row for any rank
+            return self.from_arrays(x, y, DP_rank=DP_rank, DP_size=DP_size)
         full = len(x) - (len(x) % self.global_batch_size)
         return self.from_arrays(x[DP_rank:full:DP_size], y[DP_rank:full:DP_size])
 
-    def from_arrays(self, x, y):
-        """Install an already sharded (x, y) pair (numpy or torch)."""
+    def from_arrays(self, x, y, DP_rank=None, DP_size=None):
+        """Install an already sharded (x, y) pair (numpy or torch).  A shuffled dataset installs the whole file instead,
+        and ``DP_rank`` / ``DP_size`` name the rank whose rows it serves (default: the ones recorded before)."""
+        if DP_size is not None:
+            assert 0 <= DP_rank < DP_size and self.global_batch_size % DP_size == 0
+            self.dp_rank, self.dp_size = int(DP_rank), int(DP_size)
+            self.local_batch_size = self.global_batch_size // DP_size
         if self.local_batch_size is None:
             self.local_batch_size = self.global_batch_size
         xt = torch.as_tensor(np.ascontiguousarray(x) if isinstance(x, np.ndarray) else x, dtype=torch.float32).contiguous()
@@ -115,9 +139,42 @@ class Dataset:
         elif self.pin_memory and torch.cuda.is_available():
             xt, yt = xt.pin_memory(), yt.pin_memory()
         self.input_X, self.target_y = xt, yt
+        self._ids = None
+        if self.shuffle:
+            assert self.local_batch_size % self.mubatch_size == 0
+            assert len(xt) == len(yt) and self.global_batch_size <= len(xt) < 2 ** 32, "need 1 <= N // GBS and N < 2**32"
+            return self
         assert len(self.input_X) % self.mubatch_size == 0
         assert len(self.input_X) % self.local_batch_size == 0
         return self
+
+    # -- shuffling ----------------------------------------------------------
+    @property
+    def shuffle(self) -> bool:
+        return self.shuffle_seed is not None
+
+    def set_epoch(self, epoch: int):
+        """The epoch whose permutation the batches follow from now on (used mod 2**32), like
+        ``DistributedSampler.set_epoch``.  No effect on an unshuffled dataset."""
+        if isinstance(epoch, bool) or not isinstance(epoch, int) or epoch < 0:
+            raise ValueError(f"epoch must be an integer >= 0, got {epoch!r}")
+        self.epoch = int(epoch)
+
+    def sample_ids(self, batch_id, mubatch_id=None) -> torch.Tensor:
+        """Rows of the file (int64, on the data's device) that this rank's local batch ``batch_id`` holds - or its micro-batch
+        ``mubatch_id``: local row n is global position q = batch_id * GBS + n * dp + rank, the file row
+        ``shuffle_index(N, seed, epoch, q)`` when shuffled and q itself otherwise."""
+        assert 0 <= batch_id < self.get_num_batches()
+        key = (self.epoch, batch_id)
+        if self._ids is None or self._ids[0] != key:
+            q = batch_id * self.global_batch_size + torch.arange(self.local_batch_size) * self.dp_size + self.dp_rank
+            ids = F.shuffle_index(len(self.input_X), self.shuffle_seed, self.epoch, q) if self.shuffle else q
+            self._ids = (key, ids.to(self.input_X.device))
+        ids = self._ids[1]
+        if mubatch_id is None:
+            return ids
+        assert 0 <= mubatch_id < self.get_num_mubatches()
+        return ids[mubatch_id * self.mubatch_size:(mubatch_id + 1) * self.mubatch_size]
 
     # -- access -------------------------------------------------------------
     def __len__(self):
@@ -132,20 +189,30 @@ class Dataset:
         return start, end
 
     def load_micro_batch_input(self, batch_id, mubatch_id):
+        if self.shuffle:
+            return self.input_X.index_select(0, self.sample_ids(batch_id, mubatch_id))
         s, e = self._range(batch_id, mubatch_id)
         return self.input_X[s:e]
 
     def load_micro_batch_target(self, batch_id, mubatch_id):
+        if self.shuffle:
+            return self.target_y.index_select(0, self.sample_ids(batch_id, mubatch_id))
         s, e = self._range(batch_id, mubatch_id)
         return self.target_y[s:e]
 
     def load_batch(self, batch_id):
         """The whole DP-local batch (all micro-batches) - what the native engine stages
-        with one copy per step."""
+        with one copy per step (a shuffled dataset: gathered rows, which the native engine
+        gathers itself on the device instead)."""
+        if self.shuffle:
+            ids = self.sample_ids(batch_id)
+            return self.input_X.index_select(0, ids), self.target_y.index_select(0, ids)
         s = batch_id * self.local_batch_size
         return self.input_X[s : s + self.local_batch_size], self.target_y[s : s + self.local_batch_size]
 
     def get_num_batches(self):
+        if self.shuffle:
+            return len(self) // self.global_batch_size
         return len(self) // self.local_batch_size
 
     def get_num_mubatches(self):

@@ -173,6 +173,59 @@ def dropout_ref(a: torch.Tensor, keep: torch.Tensor, scale: float) -> torch.Tens
 
 
 # ----------------------------------------------------------------------------
+# training-set shuffling: a keyed permutation of the dataset rows per epoch, the same map as csrc/kernels/ptx.cuh
+# ----------------------------------------------------------------------------
+SHUFFLE_WORD = 0x53485546   # "SHUF": the fourth counter word, which keeps these draws apart from dropout's
+SHUFFLE_ROUNDS = 6
+
+
+def check_shuffle_seed(seed):
+    """Validated shuffle seed: None (no shuffling) or an integer in [0, 2**64), else ValueError."""
+    if seed is None:
+        return None
+    if isinstance(seed, bool) or not isinstance(seed, int) or not (0 <= seed < 2 ** 64):
+        raise ValueError(f"shuffle_seed must be None or an integer in [0, 2**64), got {seed!r}")
+    return int(seed)
+
+
+def shuffle_width(n: int) -> int:
+    """w: the smallest even integer >= 2 with 2^w >= n (the Feistel network permutes w-bit values)."""
+    w = 2
+    while (1 << w) < n:
+        w += 2
+    return w
+
+
+def shuffle_index(n: int, seed: int, epoch: int, positions) -> torch.Tensor:
+    """Dataset row held by each global position q in [0, n) in epoch ``epoch`` (used mod 2^32): a 6-round balanced
+    Feistel network on w = shuffle_width(n) bits, halves of h = w / 2 bits, round i mapping (L, R) to
+    (R, L ^ (philox4x32_10((R, i, epoch, SHUFFLE_WORD), (seed lo, seed hi)).x & (2^h - 1))), applied once and then again
+    while the value is >= n (cycle walking).  A bijection on [0, n); int64 tensor of positions' shape."""
+    if not (1 <= int(n) < 2 ** 32):
+        raise ValueError(f"the dataset must hold between 1 and 2**32 - 1 rows, got {n}")
+    q = torch.as_tensor(positions, dtype=torch.int64)
+    if q.numel() and (int(q.min()) < 0 or int(q.max()) >= n):
+        raise ValueError(f"positions must lie in [0, {n})")
+    h = shuffle_width(int(n)) // 2
+    mask = (1 << h) - 1
+    key, e = (seed & _U32, seed >> 32), int(epoch) & _U32
+
+    def network(x):
+        L, R = x >> h, x & mask
+        for i in range(SHUFFLE_ROUNDS):
+            f = philox4x32_10((R, i, e, SHUFFLE_WORD), key)[0] & mask
+            L, R = R, L ^ f
+        return (L << h) | R
+
+    x = network(q.clone())
+    walk = x >= n
+    while bool(walk.any()):   # masked cycle walk: only the values still outside [0, n) take another pass
+        x[walk] = network(x[walk])
+        walk = x >= n
+    return x
+
+
+# ----------------------------------------------------------------------------
 # public API (dispatching)
 # ----------------------------------------------------------------------------
 def relu(input):

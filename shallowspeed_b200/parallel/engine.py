@@ -344,7 +344,21 @@ class NativeWorker:
 
     def execute(self, sched: Schedule, batch_id: int):
         eng = self.engine_for(sched)
-        x, y = self.dataset.load_batch(batch_id)
+        ds = self.dataset
+        if getattr(ds, "shuffle", False):
+            # the whole file stays on the device; the engine gathers this rank's rows of the epoch's permutation itself
+            if ds.input_X.device != self.device:
+                raise ValueError(f"a shuffled dataset must live on the engine's device {self.device}, "
+                                 f"not {ds.input_X.device} (Dataset(..., device=...))")
+            assert 0 <= batch_id < ds.get_num_batches()
+            self._enter(eng)
+            self.set_lr(eng, sched)
+            eng.stage_gather(ds.input_X if sched.is_first_stage else None, ds.target_y if sched.is_last_stage else None,
+                             ds.shuffle_seed, ds.epoch, ds.global_batch_size, ds.dp_size, ds.dp_rank, batch_id)
+            eng.run()
+            self._last_engine = eng
+            return
+        x, y = ds.load_batch(batch_id)
         self._enter(eng)
         self.set_lr(eng, sched)
         eng.stage_inputs(x if sched.is_first_stage else None, y if sched.is_last_stage else None)

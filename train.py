@@ -26,6 +26,7 @@ from shallowspeed_b200.dataset import Dataset
 from shallowspeed_b200.layers import MLP, mlp_sizes
 from shallowspeed_b200.lr_schedule import DEFAULT_WARMUP_START_FACTOR, KINDS as LR_SCHEDULES, LRSchedule
 from shallowspeed_b200.models.mlp import DEFAULT_LAYER_SIZES
+from shallowspeed_b200.ops.functional import check_shuffle_seed
 from shallowspeed_b200.optimizer import SGD
 from shallowspeed_b200.parallel.comm import ProcessGrid, SelfComm, make_torch_comms
 from shallowspeed_b200.pipe import (GPipeSchedule, InferenceSchedule, NaiveParallelSchedule,
@@ -96,6 +97,10 @@ def build_parser():
     p.add_argument("--dropout", type=float, default=0.0,
                    help="inverted dropout with this drop probability on every hidden layer's output, in [0, 1)")
     p.add_argument("--dropout-seed", type=int, default=0, help="seed of the dropout masks, in [0, 2**64)")
+    p.add_argument("--shuffle", action="store_true",
+                   help="visit the training set in a fresh order every epoch (a keyed permutation of the epoch, the same "
+                        "for every DP x PP layout; the native engine gathers the rows on the GPU)")
+    p.add_argument("--shuffle-seed", type=int, default=0, help="seed of the per-epoch permutation, in [0, 2**64)")
     p.add_argument("--layer-sizes", type=int, nargs="+", default=None, help="explicit layer widths (default: reference MLP)")
     p.add_argument("--hidden", type=int, default=None, help="with --n-layers: 784 -> hidden x (n-1) -> 10")
     p.add_argument("--n-layers", type=int, default=None)
@@ -189,9 +194,10 @@ def main(args):
     optimizer = SGD(model.parameters(), lr=args.lr, momentum=args.momentum, weight_decay=args.weight_decay,
                     nesterov=args.nesterov, arena=model.arena)
 
+    shuffle_seed = check_shuffle_seed(args.shuffle_seed)
     dataset = Dataset(save_dir, global_batch_size=args.global_batch_size,
                       mubatch_size=local_batch_size // args.n_mubatches, validation=False,
-                      synthetic=synthetic, device=device)
+                      synthetic=synthetic, device=device, shuffle_seed=shuffle_seed if args.shuffle else None)
     dataset.load(dp_comm.Get_rank(), dp_comm.Get_size())
     val_dataset = Dataset(save_dir, global_batch_size=args.global_batch_size,
                           mubatch_size=args.global_batch_size, validation=True,
@@ -207,7 +213,7 @@ def main(args):
                "n_mubatches": int(args.n_mubatches), "momentum": float(args.momentum),
                "weight_decay": float(args.weight_decay), "nesterov": bool(args.nesterov), "loss": loss,
                "lr_schedule": lr_schedule.spec(), "dropout": float(args.dropout),
-               "dropout_seed": int(args.dropout_seed)}
+               "dropout_seed": int(args.dropout_seed), "shuffle": bool(args.shuffle), "shuffle_seed": shuffle_seed}
     resumed_step = 0
     if args.resume:
         from shallowspeed_b200.utils.checkpoint import load_stage
@@ -244,6 +250,7 @@ def main(args):
                     logger.log(event="eval", epoch=epoch, step=step, accuracy=accuracy,
                                time_s=time.time() - start_time)
         t_epoch = time.time()
+        dataset.set_epoch(epoch)                    # the epoch's permutation (a resume re-derives it from the step)
         steps_this_epoch = min(n_batches - first_batch, total_steps - step)
         for batch_id in range(first_batch, first_batch + steps_this_epoch):
             optimizer.lr = lr_schedule(step)        # both engines read the optimizer's rate when the step starts

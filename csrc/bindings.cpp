@@ -160,6 +160,24 @@ static void relu_fwd(const Tensor& x, Tensor& y) {
     c10::cuda::CUDAGuard guard(x.device());
     cuda_ok(ssb::launch_relu_fwd(x.data_ptr<float>(), y.data_ptr<float>(), x.numel(), cur_stream()), "relu_fwd");
 }
+// smooth activation (ptx.cuh: act_fwd) of a dense tensor: y = f(z), gamma = f'(z)
+static void act_fwd(int64_t kind, const Tensor& z, Tensor& y, Tensor& gamma) {
+    TORCH_CHECK(ssb::act_smooth((int)kind), "act_fwd: kind must be GELU (1), SiLU (2) or tanh (3), got ", kind);
+    for (const Tensor* t : std::initializer_list<const Tensor*>{&z, &y, &gamma})
+        TORCH_CHECK(t->is_cuda() && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->numel() == z.numel(),
+                    "act_fwd: z, y and gamma must be dense fp32 CUDA tensors of one size");
+    c10::cuda::CUDAGuard guard(z.device());
+    cuda_ok(ssb::launch_act_fwd((int)kind, z.data_ptr<float>(), y.data_ptr<float>(), gamma.data_ptr<float>(), z.numel(),
+                                cur_stream()), "act_fwd");
+}
+// g *= gamma (the backward of a smooth activation)
+static void gate_mul_(Tensor& g, const Tensor& gamma) {
+    check_mat(g, "g"); check_mat(gamma, "gamma");
+    TORCH_CHECK(g.size(0) == gamma.size(0) && g.size(1) == gamma.size(1), "gate_mul_: g and gamma differ in shape");
+    c10::cuda::CUDAGuard guard(g.device());
+    cuda_ok(ssb::launch_gate_mul(g.data_ptr<float>(), ld_of(g), gamma.data_ptr<float>(), ld_of(gamma), g.size(0), g.size(1),
+                                 cur_stream()), "gate_mul");
+}
 static void axpby(const Tensor& x, const Tensor& t, Tensor& y, double a, double b) {
     TORCH_CHECK(x.is_contiguous() && t.is_contiguous() && y.is_contiguous() && x.numel() == y.numel() && t.numel() == y.numel());
     c10::cuda::CUDAGuard guard(x.device());
@@ -262,6 +280,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("softmax_grad", &softmax_grad);
     m.def("relu_mask_", &relu_mask_);
     m.def("relu_fwd", &relu_fwd);
+    m.def("act_fwd", &act_fwd, py::arg("kind"), py::arg("z"), py::arg("y"), py::arg("gamma"));
+    m.def("gate_mul_", &gate_mul_, py::arg("g"), py::arg("gamma"));
     m.def("axpby", &axpby);
     m.def("sgd_", &sgd_);
     m.def("sgd_momentum_", &sgd_momentum_, py::arg("w"), py::arg("g"), py::arg("v"), py::arg("lr"), py::arg("momentum"),

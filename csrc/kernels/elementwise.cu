@@ -213,6 +213,42 @@ cudaError_t launch_relu_fwd(const float* x, float* y, long n, cudaStream_t strea
     return cudaGetLastError();
 }
 
+// stage-boundary backward of a smooth activation: the gate replaces the ReLU mask (and its dropout scale)
+__global__ void gate_mul_kernel(float* __restrict__ g, int ldg, const float* __restrict__ gamma, int ldgam, int rows,
+                                int cols) {
+    const long total = (long)rows * cols;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int r = (int)(i / cols), c = (int)(i % cols);
+        g[(size_t)r * ldg + c] *= gamma[(size_t)r * ldgam + c];
+    }
+}
+cudaError_t launch_gate_mul(float* g, int ldg, const float* gamma, int ldgam, int rows, int cols, cudaStream_t stream) {
+    const long total = (long)rows * cols;
+    int blocks = (int)((total + 255) / 256);
+    if (blocks > 132 * 8) blocks = 132 * 8;
+    if (blocks < 1) blocks = 1;
+    gate_mul_kernel<<<blocks, 256, 0, stream>>>(g, ldg, gamma, ldgam, rows, cols);
+    return cudaGetLastError();
+}
+
+__global__ void act_fwd_kernel(int kind, const float* __restrict__ z, float* __restrict__ y, float* __restrict__ gamma,
+                               long n) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+        float a, g;
+        act_fwd(kind, z[i], a, g);
+        y[i] = a;
+        gamma[i] = g;
+    }
+}
+cudaError_t launch_act_fwd(int kind, const float* z, float* y, float* gamma, long n, cudaStream_t stream) {
+    if (!act_smooth(kind)) return cudaErrorInvalidValue;
+    int blocks = (int)((n + 255) / 256);
+    if (blocks > 132 * 8) blocks = 132 * 8;
+    if (blocks < 1) blocks = 1;
+    act_fwd_kernel<<<blocks, 256, 0, stream>>>(kind, z, y, gamma, n);
+    return cudaGetLastError();
+}
+
 __global__ void axpby_kernel(const float* __restrict__ x, const float* __restrict__ t, float* __restrict__ y, float a, float b, long n) {
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) y[i] = a * x[i] + b * t[i];
 }

@@ -6,6 +6,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 
+#include "activation.h"
 #include "dropout.h"
 #include "shuffle.h"
 
@@ -82,6 +83,11 @@ struct GemmParams {
     // FWD with relu: dropout after the ReLU; DGRAD with mask: the gradient is scaled by drop.scale where the mask passes
     // (the masked layer's output was dropped).  Last, so that the offsets of the other fields are what they were.
     DropoutSpec drop;
+    // ActKind of the layer (activation.h).  A smooth kind runs the gated variant: FWD with relu applies f instead of the
+    // ReLU and stores the gate gamma = f'(z) (* keep * s under dropout) to gate[n * ldo + m] (nullable: inference);
+    // DGRAD with mask reads the mask as the previous layer's gate and multiplies by it.  Last, like drop.
+    int act_kind;
+    float* gate;
 };
 
 struct GemmPlan {          // a fully prepared launch (tensor maps are 128 B each)
@@ -115,6 +121,8 @@ const char* gemm_plan_enable_splitk(GemmPlan* plan, int k_splits, float* workspa
 cudaError_t gemm_launch(const GemmPlan& plan, cudaStream_t stream);
 // the plan runs the dropout variant: a FWD with relu or a DGRAD with mask, and plan.p.drop on
 bool gemm_drops(const GemmPlan& plan);
+// the plan runs the gated variant: a FWD with relu or a DGRAD with mask, and a smooth plan.p.act_kind
+bool gemm_gated(const GemmPlan& plan);
 // Grouped launch of several WGRAD plans (different layers) as ONE grid: a device table holds one entry per CTA.  Only
 // the GEMMs of chain-eligible stages are grouped (out <= 128, any in); they run on narrow tiles of 32 output features x
 // 32 input columns with the full K (rows) in one CTA, instead of the per-layer kernel's 128 x 64.
@@ -300,6 +308,11 @@ struct ChainParams {
     // CTAs per feature slice in layer 1 (set by chain_plan): 2 when a cluster launch's layer 1 has more than 4 k-blocks
     // (cluster ranks >= cluster are the helpers that multiply half of them), else 1.  Last, for the same reason.
     int ksplit;
+    // ActKind of every layer with relu set (activation.h); a smooth kind selects the GATE instantiation.  gate[l]: the
+    // gate gamma of layer l's output ([all rows, act_ld[l]], like act[l]); nullptr in inference plans, which store
+    // none.  Last, for the same reason as loss_kind.
+    int act_kind;
+    float* gate[kChainMaxLayers + 1];
 };
 struct ChainPlan {
     ChainParams p;
@@ -344,6 +357,10 @@ cudaError_t launch_relu_mask(float* g, int ldg, const float* y, int ldy, int row
 cudaError_t launch_relu_mask_scaled(float* g, int ldg, const float* y, int ldy, int rows, int cols, float scale,
                                     cudaStream_t stream);
 cudaError_t launch_relu_fwd(const float* x, float* y, long n, cudaStream_t stream);
+// stage-boundary backward of a smooth activation: g[r, c] *= gamma[r, c] (gamma already holds keep * s under dropout)
+cudaError_t launch_gate_mul(float* g, int ldg, const float* gamma, int ldgam, int rows, int cols, cudaStream_t stream);
+// stand-alone smooth activation over n dense elements (ptx.cuh: act_fwd): y = f(z), gamma = f'(z)
+cudaError_t launch_act_fwd(int kind, const float* z, float* y, float* gamma, long n, cudaStream_t stream);
 // y = a * x + b * t  (mse grad: a=2/B, b=-2/B)
 cudaError_t launch_axpby(const float* x, const float* t, float* y, float a, float b, long n, cudaStream_t stream);
 // w -= *lr * g over a flat arena (lr: one device float, read when the kernel runs)

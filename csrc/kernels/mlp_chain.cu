@@ -168,7 +168,11 @@ __device__ __forceinline__ unsigned long long gtime() {
 // DROP: inverted dropout on every ReLU'd layer (ChainParams::drop); the same kind of switch.  The forward epilogues drop
 // and scale before any copy of the activation leaves the registers (operand tile, peer panels, act[l], the folded
 // out_peer slot); the dgrad epilogues scale where the mask of a dropped layer passes.
-template <bool SPLIT, bool FOLD, int NTW, bool CLUSTER, bool CE, bool DROP>
+// GATE: a smooth activation (ChainParams::act_kind) on every layer with relu set; the same kind of switch.  The forward
+// epilogues apply f (ptx.cuh: act_fwd) instead of the ReLU and store the gate f'(z) (* keep * s under DROP) to
+// gate[l] next to the global copy of act[l] (not in inference plans: gate[l] == nullptr); the dZ_L staging and the dgrad
+// epilogues multiply by the gate where they test the stored activation, which leaves nothing for DROP to scale there.
+template <bool SPLIT, bool FOLD, int NTW, bool CLUSTER, bool CE, bool DROP, bool GATE>
 __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParams p) {
     static_assert(!(FOLD && CLUSTER), "folded pipeline launches run one CTA per micro-batch");
     extern __shared__ uint8_t smem_raw[];
@@ -323,6 +327,18 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         auto drop_fwd = [&](float x, int l, int f, int n) {
             const uint32_t sample = (uint32_t)((row0 + n) * p.drop.dp + p.drop.rank);
             return dropout_keep(p.drop, (uint32_t)(p.drop.layer + l - 1), drop_step, (uint32_t)f, sample) ? x * p.drop.scale : 0.f;
+        };
+        // GATE: a = f(z) and its gate g for feature f of row n in local layer l, both dropped like drop_fwd under DROP
+        auto gate_fwd = [&](float z, int l, int f, int n, float& g) {
+            float a;
+            act_fwd(p.act_kind, z, a, g);
+            if constexpr (DROP) {
+                const uint32_t sample = (uint32_t)((row0 + n) * p.drop.dp + p.drop.rank);
+                const bool keep = dropout_keep(p.drop, (uint32_t)(p.drop.layer + l - 1), drop_step, (uint32_t)f, sample);
+                a = keep ? a * p.drop.scale : 0.f;
+                g = keep ? g * p.drop.scale : 0.f;
+            }
+            return a;
         };
         int wbuf = 0;                                        // activation buffer the NEXT epilogue writes
         uint32_t recv_phase = 0u;                            // CLUSTER: parity of recv_bar(b) in bit b
@@ -542,17 +558,25 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 if (p.sync_debug) asm volatile("bar.sync 2, 256;" ::: "memory");   // racecheck aid, see kernels.h
                 const uint32_t dst = abuf0 + wbuf * abuf_bytes;
                 float* __restrict__ gout = p.act[l] + (int64_t)row0 * p.act_ld[l];
+                float* __restrict__ ggout = nullptr;         // GATE: where this layer's gates go (none: inference)
+                if constexpr (GATE) { if (ly.relu && p.gate[l] != nullptr) ggout = p.gate[l] + (int64_t)row0 * p.act_ld[l]; }
                 if (!is_logits && tile) {
                     // full-K form: bias, ReLU and the feature mask on this warp's fragments, 4 st.shared per tile into
                     // the operand tile, this warp's block of it to the peers, then the global copy
+                    float tgam[NTW / 2][4];                  // GATE: the gates of this warp's fragments
 #pragma unroll
                     for (int j = 0; j < NTW / 2; ++j) {
                         if (j < tnt) {
 #pragma unroll
                             for (int r = 0; r < 4; ++r) {
                                 float x = tacc[0][j][r] + t_bias[r >> 1];
-                                if (ly.relu) x = fmaxf(x, 0.f);
-                                if constexpr (DROP) { if (ly.relu) x = drop_fwd(x, l, t_feat(r), t_row(j, r)); }
+                                if constexpr (GATE) {
+                                    tgam[j][r] = 0.f;
+                                    if (ly.relu) x = gate_fwd(x, l, t_feat(r), t_row(j, r), tgam[j][r]);
+                                } else {
+                                    if (ly.relu) x = fmaxf(x, 0.f);
+                                    if constexpr (DROP) { if (ly.relu) x = drop_fwd(x, l, t_feat(r), t_row(j, r)); }
+                                }
                                 x = t_feat(r) < ly.out ? x : 0.f;
                                 tacc[0][j][r] = x;
                                 st_tile(dst, t_row(j, r), t_feat(r), x);
@@ -567,13 +591,23 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         for (int r = 0; r < 4; ++r)
                             if (j < tnt && t_feat(r) < ly.out && t_row(j, r) < p.mb_rows)
                                 gout[(int64_t)t_row(j, r) * p.act_ld[l] + t_feat(r)] = tacc[0][j][r];
+                    if constexpr (GATE) {
+                        if (ggout != nullptr) {
+#pragma unroll
+                            for (int j = 0; j < NTW / 2; ++j)
+#pragma unroll
+                                for (int r = 0; r < 4; ++r)
+                                    if (j < tnt && t_feat(r) < ly.out && t_row(j, r) < p.mb_rows)
+                                        ggout[(int64_t)t_row(j, r) * p.act_ld[l] + t_feat(r)] = tgam[j][r];
+                        }
+                    }
                     wbuf ^= 1;
                     if (l == 1) wbuf = 1;                    // layer 1 wrote abuf 0; layer 2 reads 0, writes 1
                 } else if (!is_logits) {
                     // one 16-row chunk per warp when N <= 32: write the operand tile for the next GEMM first,
                     // publish it, and only then drain the global copy (needed later by wgrad / the pipeline)
                     const bool single = (c_hi - c_lo == 16);
-                    float keep[16];
+                    float keep[16], gkeep[16];               // gkeep: GATE, the gates of `keep`
 #pragma unroll
                     for (int ch = 0; ch < NTW / 2 && epi; ++ch) {
                         const int c = c_lo + 16 * ch;
@@ -583,14 +617,22 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
 #pragma unroll
                         for (int j = 0; j < 16; ++j) {
                             float x = v[j] + bias;
-                            if (ly.relu) x = fmaxf(x, 0.f);
-                            if constexpr (DROP) { if (ly.relu) x = drop_fwd(x, l, m, c + j); }
+                            float gm = 0.f;
+                            if constexpr (GATE) {
+                                if (ly.relu) x = gate_fwd(x, l, m, c + j, gm);
+                            } else {
+                                if (ly.relu) x = fmaxf(x, 0.f);
+                                if constexpr (DROP) { if (ly.relu) x = drop_fwd(x, l, m, c + j); }
+                            }
                             x = m_ok ? x : 0.f;
                             const int n = c + j;
                             st_tile(dst, n, m, x);
-                            if (single) keep[j] = x;
-                            else if (m_ok && n < p.mb_rows) {
+                            if (single) {
+                                keep[j] = x;
+                                if constexpr (GATE) gkeep[j] = gm;
+                            } else if (m_ok && n < p.mb_rows) {
                                 gout[(int64_t)n * p.act_ld[l] + m] = x;
+                                if constexpr (GATE) { if (ggout != nullptr) ggout[(int64_t)n * p.act_ld[l] + m] = gm; }
                                 if constexpr (FOLD) { if (l == L && p.out_peer != nullptr) p.out_peer[(int64_t)n * p.act_ld[l] + m] = x; }
                             }
                         }
@@ -602,6 +644,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         for (int j = 0; j < 16; ++j)
                             if (c_lo + j < p.mb_rows) {
                                 gout[(int64_t)(c_lo + j) * p.act_ld[l] + m] = keep[j];
+                                if constexpr (GATE) { if (ggout != nullptr) ggout[(int64_t)(c_lo + j) * p.act_ld[l] + m] = gkeep[j]; }
                                 if constexpr (FOLD) { if (l == L && p.out_peer != nullptr) p.out_peer[(int64_t)(c_lo + j) * p.act_ld[l] + m] = keep[j]; }
                             }
                     }
@@ -783,18 +826,22 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             }
         }
         if (p.do_bwd && !(p.do_fwd && p.do_loss) && !helper) {
-            // backward-only launch (pipeline stage): stage dZ_L = gout (.) relu'(act_L) into smem
+            // backward-only launch (pipeline stage): stage dZ_L = gout (.) relu'(act_L) into smem (GATE: gout (.) gate_L)
             const ChainLayer& ly = p.layers[L - 1];
             const bool m_ok = m < ly.out;
             const uint32_t dst = abuf0 + wbuf * abuf_bytes;
             float* __restrict__ g = p.dz[L] + (int64_t)row0 * p.act_ld[L];
-            const float* __restrict__ y = p.act[L] + (int64_t)row0 * p.act_ld[L];
+            const float* __restrict__ y = (GATE ? p.gate[L] : p.act[L]) + (int64_t)row0 * p.act_ld[L];
             for (int n = c_lo; n < c_hi && epi; ++n) {
                 float x = 0.f;
                 if (m_ok && n < p.mb_rows) {
                     asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(x) : "l"(g + (int64_t)n * p.act_ld[L] + m));   // may be peer-written
-                    if (ly.relu && !(y[(int64_t)n * p.act_ld[L] + m] > 0.f)) x = 0.f;
-                    if constexpr (DROP) { if (ly.relu) x *= p.drop.scale; }   // act_L was dropped: dZ_L = g * s where it passes
+                    if constexpr (GATE) {
+                        if (ly.relu) x *= y[(int64_t)n * p.act_ld[L] + m];   // the gate holds keep * s already
+                    } else {
+                        if (ly.relu && !(y[(int64_t)n * p.act_ld[L] + m] > 0.f)) x = 0.f;
+                        if constexpr (DROP) { if (ly.relu) x *= p.drop.scale; }   // act_L was dropped: dZ_L = g * s where it passes
+                    }
                     g[(int64_t)n * p.act_ld[L] + m] = x;     // the wgrad GEMM reads the masked gradient
                 }
                 st_tile(dst, n, m, x);
@@ -809,7 +856,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 const ChainLayer& ly = p.layers[l - 1];
                 const bool m_ok = m < ly.in;                 // output feature of dgrad = input feature of layer l
                 const bool mask_on = (l >= 2) && p.layers[l - 2].relu;
-                const float* __restrict__ yprev = p.act[l - 1] + (int64_t)row0 * p.act_ld[l - 1];
+                // the mask of layer l - 1: its stored output (ReLU), or its gate (GATE: multiplied in, 1 where no mask)
+                const float* __restrict__ yprev = (GATE ? p.gate[l - 1] : p.act[l - 1]) + (int64_t)row0 * p.act_ld[l - 1];
                 float* __restrict__ gprev = p.dz[l - 1] + (int64_t)row0 * p.act_ld[l - 1];
                 if constexpr (CLUSTER) {
                     // full-K form (K = out <= 128: at most 4 k-blocks): the ReLU masks of this warp's fragments are
@@ -832,8 +880,13 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         if (j < tnt) {
 #pragma unroll
                             for (int r = 0; r < 4; ++r) {
-                                float x = (t_mk[j][r] > 0.f) ? tacc[0][j][r] : 0.f;
-                                if constexpr (DROP) { if (mask_on) x *= p.drop.scale; }   // layer l - 1 was dropped
+                                float x;
+                                if constexpr (GATE) {
+                                    x = tacc[0][j][r] * t_mk[j][r];
+                                } else {
+                                    x = (t_mk[j][r] > 0.f) ? tacc[0][j][r] : 0.f;
+                                    if constexpr (DROP) { if (mask_on) x *= p.drop.scale; }   // layer l - 1 was dropped
+                                }
                                 x = t_feat(r) < ly.in ? x : 0.f;
                                 tacc[0][j][r] = x;
                                 if (more) st_tile(dst, t_row(j, r), t_feat(r), x);
@@ -885,8 +938,13 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
 #pragma unroll
                     for (int j = 0; j < 16; ++j) {
                         const int n = c + j;
-                        float x = (mk[j] > 0.f) ? v[j] : 0.f;
-                        if constexpr (DROP) { if (mask_on) x *= p.drop.scale; }   // layer l - 1 was dropped
+                        float x;
+                        if constexpr (GATE) {
+                            x = v[j] * mk[j];
+                        } else {
+                            x = (mk[j] > 0.f) ? v[j] : 0.f;
+                            if constexpr (DROP) { if (mask_on) x *= p.drop.scale; }   // layer l - 1 was dropped
+                        }
                         x = m_ok ? x : 0.f;
                         if (more) st_tile(dst, n, m, x);
                         if (single) keep[j] = x;
@@ -1062,33 +1120,39 @@ void chain_plan_free(ChainPlan* plan) {
     plan->maps_dev = nullptr;
 }
 
-template <int NTW, bool CE, bool DROP>
+template <int NTW, bool CE, bool DROP, bool GATE>
 static cudaError_t chain_configure_ntw() {
     cudaError_t e;
     const int smem = 227 * 1024;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, false, CE, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, true, NTW, false, CE, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, false, CE, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, true, NTW, false, CE, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, true, CE, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    return cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, true, CE, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, false, CE, DROP, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, true, NTW, false, CE, DROP, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, false, CE, DROP, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<true, true, NTW, false, CE, DROP, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<false, false, NTW, true, CE, DROP, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    return cudaFuncSetAttribute(mlp_chain_kernel<true, false, NTW, true, CE, DROP, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+}
+
+template <bool DROP, bool GATE>
+static cudaError_t chain_configure_kind() {
+    cudaError_t e;
+    if ((e = chain_configure_ntw<2, false, DROP, GATE>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<4, false, DROP, GATE>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<8, false, DROP, GATE>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<2, true, DROP, GATE>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<4, true, DROP, GATE>()) != cudaSuccess) return e;
+    return chain_configure_ntw<8, true, DROP, GATE>();
 }
 
 cudaError_t chain_configure() {
     cudaError_t e;
-    for (int drop = 0; drop < 2; ++drop) {
-        if ((e = drop ? chain_configure_ntw<2, false, true>() : chain_configure_ntw<2, false, false>()) != cudaSuccess) return e;
-        if ((e = drop ? chain_configure_ntw<4, false, true>() : chain_configure_ntw<4, false, false>()) != cudaSuccess) return e;
-        if ((e = drop ? chain_configure_ntw<8, false, true>() : chain_configure_ntw<8, false, false>()) != cudaSuccess) return e;
-        if ((e = drop ? chain_configure_ntw<2, true, true>() : chain_configure_ntw<2, true, false>()) != cudaSuccess) return e;
-        if ((e = drop ? chain_configure_ntw<4, true, true>() : chain_configure_ntw<4, true, false>()) != cudaSuccess) return e;
-        if ((e = drop ? chain_configure_ntw<8, true, true>() : chain_configure_ntw<8, true, false>()) != cudaSuccess) return e;
-    }
-    return cudaSuccess;
+    if ((e = chain_configure_kind<false, false>()) != cudaSuccess) return e;
+    if ((e = chain_configure_kind<true, false>()) != cudaSuccess) return e;
+    if ((e = chain_configure_kind<false, true>()) != cudaSuccess) return e;
+    return chain_configure_kind<true, true>();
 }
 
 // grid = micro-batches x plan.cluster x plan.ksplit, cluster dims (plan.cluster x plan.ksplit, 1, 1)
-template <bool SPLIT, int NTW, bool CE, bool DROP>
+template <bool SPLIT, int NTW, bool CE, bool DROP, bool GATE>
 static cudaError_t chain_launch_cluster(const ChainPlan& plan, cudaStream_t stream) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)plan.grid);
@@ -1102,15 +1166,16 @@ static cudaError_t chain_launch_cluster(const ChainPlan& plan, cudaStream_t stre
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, mlp_chain_kernel<SPLIT, false, NTW, true, CE, DROP>, plan.p);
+    return cudaLaunchKernelEx(&cfg, mlp_chain_kernel<SPLIT, false, NTW, true, CE, DROP, GATE>, plan.p);
 }
 
-template <int NTW, bool CE, bool DROP>
+template <int NTW, bool CE, bool DROP, bool GATE>
 static cudaError_t chain_launch_ntw(const ChainPlan& plan, bool fold, cudaStream_t stream) {
     const ChainParams& p = plan.p;
     if (plan.cluster > 1)
-        return p.split ? chain_launch_cluster<true, NTW, CE, DROP>(plan, stream) : chain_launch_cluster<false, NTW, CE, DROP>(plan, stream);
-#define SSB_CHAIN_LAUNCH(S, F) mlp_chain_kernel<S, F, NTW, false, CE, DROP><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(p)
+        return p.split ? chain_launch_cluster<true, NTW, CE, DROP, GATE>(plan, stream)
+                       : chain_launch_cluster<false, NTW, CE, DROP, GATE>(plan, stream);
+#define SSB_CHAIN_LAUNCH(S, F) mlp_chain_kernel<S, F, NTW, false, CE, DROP, GATE><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(p)
     if (!p.split) {
         if (fold) SSB_CHAIN_LAUNCH(false, true); else SSB_CHAIN_LAUNCH(false, false);
     } else {
@@ -1120,22 +1185,25 @@ static cudaError_t chain_launch_ntw(const ChainPlan& plan, bool fold, cudaStream
     return cudaSuccess;
 }
 
+template <bool DROP, bool GATE>
+static cudaError_t chain_launch_kind(const ChainPlan& plan, int ntw, bool ce, bool fold, cudaStream_t stream) {
+    if (ntw == 2) return ce ? chain_launch_ntw<2, true, DROP, GATE>(plan, fold, stream) : chain_launch_ntw<2, false, DROP, GATE>(plan, fold, stream);
+    if (ntw == 4) return ce ? chain_launch_ntw<4, true, DROP, GATE>(plan, fold, stream) : chain_launch_ntw<4, false, DROP, GATE>(plan, fold, stream);
+    return ce ? chain_launch_ntw<8, true, DROP, GATE>(plan, fold, stream) : chain_launch_ntw<8, false, DROP, GATE>(plan, fold, stream);
+}
+
 cudaError_t chain_launch(const ChainPlan& plan, cudaStream_t stream) {
     const ChainParams& p = plan.p;
     const bool fold = p.in_flag != nullptr || p.out_peer != nullptr || p.x_from_global != 0;
     const int ntw = chain_ntw(p.n_pad);
     if (p.loss_kind != LOSS_MSE && p.loss_kind != LOSS_CROSS_ENTROPY) return cudaErrorInvalidValue;
-    const bool ce = p.loss_kind == LOSS_CROSS_ENTROPY;
+    if (!act_valid(p.act_kind)) return cudaErrorInvalidValue;
+    const bool ce = p.loss_kind == LOSS_CROSS_ENTROPY, drop = p.drop.on();
     cudaError_t e;
-    if (!p.drop.on()) {
-        if (ntw == 2) e = ce ? chain_launch_ntw<2, true, false>(plan, fold, stream) : chain_launch_ntw<2, false, false>(plan, fold, stream);
-        else if (ntw == 4) e = ce ? chain_launch_ntw<4, true, false>(plan, fold, stream) : chain_launch_ntw<4, false, false>(plan, fold, stream);
-        else e = ce ? chain_launch_ntw<8, true, false>(plan, fold, stream) : chain_launch_ntw<8, false, false>(plan, fold, stream);
-    } else {
-        if (ntw == 2) e = ce ? chain_launch_ntw<2, true, true>(plan, fold, stream) : chain_launch_ntw<2, false, true>(plan, fold, stream);
-        else if (ntw == 4) e = ce ? chain_launch_ntw<4, true, true>(plan, fold, stream) : chain_launch_ntw<4, false, true>(plan, fold, stream);
-        else e = ce ? chain_launch_ntw<8, true, true>(plan, fold, stream) : chain_launch_ntw<8, false, true>(plan, fold, stream);
-    }
+    if (!act_smooth(p.act_kind))
+        e = drop ? chain_launch_kind<true, false>(plan, ntw, ce, fold, stream) : chain_launch_kind<false, false>(plan, ntw, ce, fold, stream);
+    else
+        e = drop ? chain_launch_kind<true, true>(plan, ntw, ce, fold, stream) : chain_launch_kind<false, true>(plan, ntw, ce, fold, stream);
     if (e != cudaSuccess) return e;
     return cudaGetLastError();
 }

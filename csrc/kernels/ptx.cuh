@@ -5,6 +5,7 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "activation.h"
 #include "dropout.h"
 #include "shuffle.h"
 
@@ -378,6 +379,26 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1
 // Every site that drops or scales calls this, so the kernels and the torch oracle draw the same bits.
 __device__ __forceinline__ bool dropout_keep(const DropoutSpec& d, uint32_t layer, uint32_t step, uint32_t f, uint32_t s) {
     return philox4x32_10(make_uint4(f, s, layer, step), (uint32_t)d.seed, (uint32_t)(d.seed >> 32)).x >= d.threshold;
+}
+
+// ------------------------------------------------------------------ smooth hidden activations (activation.h)
+// a = f(z) and the gate g = f'(z) of one pre-activation, for kind GELU (erf form), SiLU or tanh; every kernel that applies
+// a smooth activation calls this, and ops/functional.py: activation_ref is the same math in torch.  Precise erff /
+// expf / tanhf (no fast-math).  Dropout multiplies both by keep * s afterwards, so the backward is g * dout alone.
+__device__ __forceinline__ void act_fwd(int kind, float z, float& a, float& g) {
+    if (kind == ACT_GELU) {
+        const float c = 0.5f * (1.f + erff(z * 0.70710678118654752f));       // Phi(z)
+        a = z * c;
+        g = c + z * (expf(-0.5f * z * z) * 0.39894228040143268f);          // Phi(z) + z phi(z)
+    } else if (kind == ACT_SILU) {
+        const float s = 1.f / (1.f + expf(-z));                            // sigma(z); 0 once expf overflows
+        a = z * s;
+        g = s * (1.f + z * (1.f - s));
+    } else {
+        const float t = tanhf(z);
+        a = t;
+        g = 1.f - t * t;
+    }
 }
 
 // ------------------------------------------------------------------ training-set shuffling

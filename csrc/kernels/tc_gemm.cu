@@ -50,7 +50,10 @@ static constexpr int kGroupMinCtas = 3;                 // CTAs per SM the group
 // goes through the same warp_mma_kblock arithmetic in both forms.
 // DROP (FWD with relu / DGRAD with mask, GemmParams::drop): dropout after the ReLU, or the gradient scaled where the mask
 // passes; a compile-time switch, so the dropout-free instantiations carry none of its code.
-template <int MODE, bool SPLITK, bool STATEFUL = false, int BM = (int)kBlockM, bool DROP = false>
+// GATE (FWD with relu / DGRAD with mask, a smooth GemmParams::act_kind): the FWD applies f (ptx.cuh: act_fwd) instead of the
+// ReLU and stores the gate f'(z) (* keep * s under DROP) to GemmParams::gate; the DGRAD multiplies by the mask, which
+// is the previous layer's gate (its dropout scale is inside).  The same kind of switch.
+template <int MODE, bool SPLITK, bool STATEFUL = false, int BM = (int)kBlockM, bool DROP = false, bool GATE = false>
 __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
                                              const GemmParams& p, const int bx, const int by, const int bz) {
     constexpr bool A_MN = (MODE != GEMM_FWD);
@@ -175,6 +178,18 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             const uint32_t sample = (uint32_t)((p.drop.row_base + n) * p.drop.dp + p.drop.rank);
             return dropout_keep(p.drop, (uint32_t)p.drop.layer, drop_step, (uint32_t)m, sample) ? x * p.drop.scale : 0.f;
         };
+        // GATE, FWD: a = f(z) and the gate of output feature m of row n (dropped like drop_fwd under DROP)
+        auto gate_fwd = [&](float z, int n, float& g) {
+            float a;
+            act_fwd(p.act_kind, z, a, g);
+            if constexpr (DROP) {
+                const uint32_t sample = (uint32_t)((p.drop.row_base + n) * p.drop.dp + p.drop.rank);
+                const bool keep = dropout_keep(p.drop, (uint32_t)p.drop.layer, drop_step, (uint32_t)m, sample);
+                a = keep ? a * p.drop.scale : 0.f;
+                g = keep ? g * p.drop.scale : 0.f;
+            }
+            return a;
+        };
         if constexpr (SPLITK) {
             // ---- split-K: publish the raw partial, last arriver reduces (fixed split order) + epilogue
             const int tile = (int)(by * gridDim.x + bx);
@@ -227,7 +242,17 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                     for (int j = 0; j < 16; ++j) {
                         float x = v[j] + bias;
                         const int n = n0 + c + j;
-                        if (MODE == GEMM_FWD) {
+                        if constexpr (GATE) {
+                            if (MODE == GEMM_FWD) {
+                                if (p.relu) {
+                                    float g;
+                                    x = gate_fwd(x, n, g);
+                                    if (n < p.n_total && p.gate != nullptr) p.gate[(size_t)n * p.ldo + m] = g;
+                                }
+                            } else if (mask != nullptr) {
+                                x *= mk[j];
+                            }
+                        } else if (MODE == GEMM_FWD) {
                             if (p.relu) x = fmaxf(x, 0.f);
                             if constexpr (DROP) x = drop_fwd(x, n);
                         } else if (mask != nullptr) {
@@ -257,10 +282,17 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                 float v[16];
                 warp_acc_row16(acc, ch, v, lane);
                 if (!m_ok) continue;
+                float gv[16];                            // GATE, FWD: the gates of the 16 outputs
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
                     float x = v[j] + bias;
-                    if (MODE == GEMM_FWD) {
+                    if constexpr (GATE) {
+                        if (MODE == GEMM_FWD) {
+                            if (p.relu) x = gate_fwd(x, n0 + c + j, gv[j]);
+                        } else if (mask != nullptr) {
+                            x *= mk[j];
+                        }
+                    } else if (MODE == GEMM_FWD) {
                         if (p.relu) x = fmaxf(x, 0.f);
                         if constexpr (DROP) x = drop_fwd(x, n0 + c + j);
                     } else if (mask != nullptr) {
@@ -272,6 +304,15 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                 for (int j = 0; j < 16; ++j) {
                     const int n = n0 + c + j;
                     if (n < p.n_total) out[(size_t)n * p.ldo + m] = v[j];     // lanes -> consecutive m: coalesced
+                }
+                if constexpr (GATE && MODE == GEMM_FWD) {
+                    if (p.relu && p.gate != nullptr) {
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) {
+                            const int n = n0 + c + j;
+                            if (n < p.n_total) p.gate[(size_t)n * p.ldo + m] = gv[j];
+                        }
+                    }
                 }
             }
         } else {
@@ -412,6 +453,14 @@ __global__ void __launch_bounds__(kThreads, 1)
 tc_gemm_drop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
     tc_gemm_body<MODE, SPLITK, false, (int)kBlockM, true>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z);
+}
+// FWD / DGRAD of a smooth activation, with or without dropout in the FWD (a kernel of its own, like tc_gemm_drop_kernel)
+template <int MODE, bool SPLITK, bool DROP>
+__global__ void __launch_bounds__(kThreads, 1)
+tc_gemm_gate_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                    const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+    tc_gemm_body<MODE, SPLITK, false, (int)kBlockM, DROP, true>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y,
+                                                                (int)blockIdx.z);
 }
 
 // ---- grouped weight-gradient launch: the tiles of SEVERAL layers' WGRAD GEMMs in one grid (one table entry per CTA).
@@ -684,6 +733,12 @@ cudaError_t gemm_configure() {
     if ((e = cudaFuncSetAttribute(tc_gemm_drop_kernel<GEMM_FWD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_drop_kernel<GEMM_DGRAD, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_drop_kernel<GEMM_DGRAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_FWD, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_FWD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_FWD, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_FWD, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_DGRAD, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_DGRAD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     g_configured = true;
     return cudaSuccess;
 }
@@ -708,6 +763,17 @@ static cudaError_t launch_mode(const GemmPlan& plan, cudaStream_t stream) {
         if (e != cudaSuccess) return e;
     }
     if constexpr (MODE != GEMM_WGRAD) {
+        if (gemm_gated(plan)) {
+            // the DGRAD's gate already holds the dropout scale: only the FWD has a dropout form
+            const bool drop = MODE == GEMM_FWD && plan.p.drop.on();
+            const bool sk = plan.p.k_splits > 1;
+#define SSB_GATE_LAUNCH(S, D) tc_gemm_gate_kernel<MODE, S, D><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p)
+            if (sk) { if (drop) SSB_GATE_LAUNCH(true, MODE == GEMM_FWD); else SSB_GATE_LAUNCH(true, false); }
+            else { if (drop) SSB_GATE_LAUNCH(false, MODE == GEMM_FWD); else SSB_GATE_LAUNCH(false, false); }
+#undef SSB_GATE_LAUNCH
+            g_launches.fetch_add(1, std::memory_order_relaxed);
+            return cudaGetLastError();
+        }
         if (gemm_drops(plan)) {
             if (plan.p.k_splits > 1)
                 tc_gemm_drop_kernel<MODE, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
@@ -731,6 +797,11 @@ static cudaError_t launch_mode(const GemmPlan& plan, cudaStream_t stream) {
     tc_gemm_kernel<MODE><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return cudaGetLastError();
+}
+
+bool gemm_gated(const GemmPlan& plan) {
+    if (!act_smooth(plan.p.act_kind)) return false;
+    return plan.mode == GEMM_FWD ? plan.p.relu != 0 : (plan.mode == GEMM_DGRAD && plan.p.mask != nullptr);
 }
 
 bool gemm_drops(const GemmPlan& plan) {

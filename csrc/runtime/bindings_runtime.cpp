@@ -250,6 +250,9 @@ public:
         TORCH_CHECK(c.dropout >= 0.0 && c.dropout < 1.0, "PipeEngine: cfg['dropout'] must be in [0, 1), got ", c.dropout);
         c.dropout_seed = cfg.contains("dropout_seed") ? cfg["dropout_seed"].cast<uint64_t>() : 0;
         c.layer_base = geti("layer_base", 0);
+        c.activation = geti("activation", ssb::ACT_RELU);
+        TORCH_CHECK(ssb::act_valid(c.activation), "PipeEngine: cfg['activation'] must be 0 (relu), 1 (gelu), 2 (silu) or 3 (tanh), got ",
+                    c.activation);
         c10::cuda::CUDAGuard guard(weights.device());
         engine_ = std::make_unique<PipeEngine>(c, weights.data_ptr<float>(), grads.data_ptr<float>(), weights.numel(),
                                                momentum.has_value() ? momentum->data_ptr<float>() : nullptr);
@@ -352,6 +355,13 @@ public:
     torch::Tensor dz(int mu, int l) {
         const auto& cfg = engine_->config();
         return view_of(engine_->dz_ptr(mu, l), cfg.mb_rows, boundary_cols(l), engine_->act_ld(l));
+    }
+    // the gates f'(z) * keep * s of layer l's output (a gated training plan's activated layers only)
+    torch::Tensor gate(int mu, int l) {
+        const auto& cfg = engine_->config();
+        float* g = engine_->gate_ptr(mu, l);
+        TORCH_CHECK(g != nullptr, "PipeEngine.gate: layer ", l, " has no gate buffer (ReLU, inference, or no activation)");
+        return view_of(g, cfg.mb_rows, boundary_cols(l), engine_->act_ld(l));
     }
     torch::Tensor probs(int mu) {
         const auto& cfg = engine_->config();
@@ -460,6 +470,7 @@ void bind_runtime(py::module_& m) {
         .def("reset_correct", &PyEngine::reset_correct)
         .def("act", &PyEngine::act)
         .def("dz", &PyEngine::dz)
+        .def("gate", &PyEngine::gate)
         .def("probs", &PyEngine::probs)
         .def("kernels_per_step", &PyEngine::kernels_per_step)
         .def("graph_nodes", &PyEngine::graph_nodes)

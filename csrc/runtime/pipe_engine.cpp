@@ -154,6 +154,15 @@ void PipeEngine::alloc_buffers() {
     if (cfg_.training)
         for (int l = 0; l <= L_; ++l) dz_all_[l] = dalloc((size_t)M * mb * act_ld_[l]);
     probs_all_ = dalloc((size_t)M * mb * act_ld_[L_]);
+    if (gated()) {
+        gamma_all_.assign(L_ + 1, nullptr);
+        for (int l = 1; l <= L_; ++l)
+            if (cfg_.layers[l - 1].relu) gamma_all_[l] = dalloc((size_t)M * mb * act_ld_[l]);
+        gamma_.assign(M, std::vector<float*>(L_ + 1, nullptr));
+        for (int mu = 0; mu < M; ++mu)
+            for (int l = 1; l <= L_; ++l)
+                if (gamma_all_[l]) gamma_[mu][l] = gamma_all_[l] + (size_t)mu * mb * act_ld_[l];
+    }
     act_.assign(M, std::vector<float*>(L_ + 1, nullptr));
     dz_.assign(M, std::vector<float*>(L_ + 1, nullptr));
     probs_.assign(M, nullptr);
@@ -175,6 +184,24 @@ DropoutSpec PipeEngine::drop_for(int layer, int row_base) const {
     d.dp = cfg_.dp_size;
     d.rank = cfg_.dp_rank;
     return d;
+}
+
+float* PipeEngine::gamma_of(const float* act) const {
+    const size_t rows = (size_t)cfg_.n_mu * cfg_.mb_rows;
+    for (int l = 1; l <= L_; ++l)
+        if (gamma_all_[l] != nullptr && act >= act_all_[l] && act < act_all_[l] + rows * act_ld_[l])
+            return gamma_all_[l] + (act - act_all_[l]);
+    throw std::runtime_error("PipeEngine: no gate buffer behind an activated layer's output");
+}
+
+// A smooth activation runs the gated GEMM variants: a FWD with relu applies f (and, training, stores its gates next to
+// its output), a DGRAD with mask multiplies by the previous layer's gates instead of testing its output.
+void PipeEngine::gate_gemm(GemmPlan& g) const {
+    if (!act_smooth(cfg_.activation)) return;
+    g.p.act_kind = cfg_.activation;
+    if (!gated()) return;                                         // inference: f, no gates
+    if (g.mode == GEMM_FWD && g.p.relu) g.p.gate = gamma_of(g.p.out);
+    else if (g.mode == GEMM_DGRAD && g.p.mask != nullptr) g.p.mask = gamma_of(g.p.mask);
 }
 
 // Point the planner at one of the two input-staging sets (stage input = act[.][0], targets).
@@ -261,6 +288,9 @@ int PipeEngine::add_chain(int stream, int mu_base, int n_mu, bool do_fwd, bool d
     cp.probs = probs_all_; cp.ldp = act_ld_[L_];
     cp.loss = loss_target();
     cp.loss_kind = cfg_.loss;
+    cp.act_kind = cfg_.activation;
+    if (gated())
+        for (int l = 0; l <= L_; ++l) cp.gate[l] = gamma_all_[l];
     if (dropout_on()) {
         // one spec for the launch: the kernel drops only the ReLU'd layers, layer l's counter is drop.layer + l - 1
         cp.drop = dropout_spec(cfg_.dropout, cfg_.dropout_seed);
@@ -416,6 +446,7 @@ void PipeEngine::plan_per_mubatch() {
         // FWD drops layer `layer`'s output, DGRAD scales by the mask of layer - 1 (the same p): the spec of the GEMM's
         // rows, micro-batch mu of this stage
         gemms_.back().p.drop = drop_for(g.mode == GEMM_DGRAD ? std::max(layer - 1, 1) : layer, mu * cfg_.mb_rows);
+        gate_gemm(gemms_.back());
         Op op;
         op.kind = OP_GEMM; op.stream = stream; op.gemm = (int)gemms_.size() - 1; op.layer = layer; op.mu = mu;
         ops_.push_back(op);
@@ -638,6 +669,7 @@ void PipeEngine::plan_per_mubatch() {
                             rm.dropout = true;
                             rm.scalar = dropout_spec(cfg_.dropout, cfg_.dropout_seed).scale;
                         }
+                        if (gated()) { rm.gated = true; rm.b = gamma_[mu][L_]; }   // the gate (with the scale) replaces both
                         ops_.push_back(rm);
                     }
                     for (int l = L_; l >= 1; --l) {
@@ -795,6 +827,7 @@ void PipeEngine::build_coalesced() {
         gemms_.push_back(g);
         maybe_splitk(gemms_.back());
         gemms_.back().p.drop = drop_for(g.mode == GEMM_DGRAD ? std::max(layer - 1, 1) : layer, 0);   // all rows
+        gate_gemm(gemms_.back());
         Op op;
         op.kind = OP_GEMM; op.stream = stream; op.gemm = (int)gemms_.size() - 1; op.layer = layer; op.mu = -1;
         ops_.push_back(op);
@@ -1081,7 +1114,8 @@ void PipeEngine::exec(const Op& op) {
             CUDA_CHECK(launch_argmax_correct(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, correct_dev_, st));
             break;
         case OP_RELU_MASK:
-            if (op.dropout) CUDA_CHECK(launch_relu_mask_scaled(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, op.scalar, st));
+            if (op.gated) CUDA_CHECK(launch_gate_mul(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, st));
+            else if (op.dropout) CUDA_CHECK(launch_relu_mask_scaled(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, op.scalar, st));
             else CUDA_CHECK(launch_relu_mask(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, st));
             break;
         case OP_SGD: {
@@ -1381,8 +1415,11 @@ std::string PipeEngine::plan_text(int set) const {
             const GemmPlan& g = gemms_[op.gemm];
             if (g.p.k_splits > 1) os << " splits=" << g.p.k_splits;
             if (gemm_drops(g)) os << " drop=" << (g.mode == GEMM_FWD ? "fwd" : "dgrad");
+            if (gemm_gated(g)) os << " act=" << act_name(g.p.act_kind);
         }
         if (op.kind == OP_RELU_MASK && op.dropout) os << " drop=scaled";
+        if (op.kind == OP_RELU_MASK && op.gated) os << " act=" << act_name(cfg_.activation);
+        if (op.kind == OP_CHAIN && act_smooth(cfg_.activation)) os << " act=" << act_name(cfg_.activation);
         if (op.kind == OP_COMM_GROUP) {
             os << " [";
             for (const auto& it : op.comm) os << (it.is_send ? "send->" : "recv<-") << it.peer << ":" << it.count << " ";

@@ -68,6 +68,7 @@ struct Op {
     int lda = 0, ldb = 0, ldc = 0, ldd = 0, rows = 0, cols = 0;
     float scalar = 0.f;
     bool dropout = false;      // OP_RELU_MASK: the masked activation was dropped, the kept gradient is scaled by `scalar`
+    bool gated = false;        // OP_RELU_MASK of a smooth activation: b is the layer's gate, multiplied in (scale included)
     const float* lr = nullptr; // OP_SGD / OP_NVLS_SGD: the learning-rate slot of the op's staging set
     int64_t n = 0;
 };
@@ -98,6 +99,9 @@ struct EngineConfig {
     double dropout = 0.0;
     uint64_t dropout_seed = 0;
     int layer_base = 0;
+    // ActKind (activation.h) of every layer with relu set.  A smooth kind makes training plans keep one gate buffer
+    // gamma = f'(z) * keep * s per activated layer and micro-batch, laid out like act (gate_ptr).
+    int activation = ACT_RELU;
 };
 
 class PipeEngine {
@@ -132,6 +136,8 @@ public:
     void set_dropout_step(uint32_t step) { step_ = step; }
     uint32_t dropout_step() const { return step_; }
     bool dropout_on() const { return cfg_.training && cfg_.dropout > 0.0; }
+    // a training plan of a smooth activation: the forward stores gates, the backward multiplies by them
+    bool gated() const { return cfg_.training && act_smooth(cfg_.activation); }
     void synchronize();
     bool wait(double timeout_s);      // watchdog: false if the step in flight did not finish in time
     std::string comm_status() const;  // NCCL async error state of the attached communicators
@@ -147,6 +153,7 @@ public:
     float* act_ptr(int mu, int l) { return act_[mu][l]; }
     int act_ld(int l) const { return act_ld_[l]; }
     float* dz_ptr(int mu, int l) { return dz_[mu][l]; }
+    float* gate_ptr(int mu, int l) { return gamma_.empty() ? nullptr : gamma_[mu][l]; }   // nullptr unless gated()
     float* probs_ptr(int mu) { return probs_[mu]; }
     float* x_staging() { return x_stage_; }
     float* y_staging() { return y_stage_; }
@@ -203,6 +210,11 @@ private:
     std::vector<std::vector<float*>> act_, dz_;  // [mu][l]
     std::vector<float*> probs_;
     std::vector<float*> act_all_, dz_all_;       // [l] contiguous over micro-batches
+    // gated(): the gates of act, [mu][l] / [l] like act_ / act_all_ (layers without relu and l = 0: nullptr); empty otherwise
+    std::vector<std::vector<float*>> gamma_;
+    std::vector<float*> gamma_all_;
+    float* gamma_of(const float* act) const;     // the gate element of an element of act_all_[l], l >= 1
+    void gate_gemm(GemmPlan& g) const;           // the activation of a FWD / DGRAD plan being built (gemm_gated)
     bool gate_on_ = false;           // grouped wgrad forked next to the chain kernel, gated by device counters
     uint32_t* gate_ready_ = nullptr; // [L + 1] per-layer counters written by the chain kernel
     uint32_t* gate_step_ = nullptr;  // steps of THIS engine (bumped in front of the gated kernel)

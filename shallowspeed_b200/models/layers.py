@@ -1,4 +1,4 @@
-"""Model layer: Parameter / Module / Linear / ReLU / Softmax / MSELoss / CrossEntropyLoss / Sequential.
+"""Model layer: Parameter / Module / Linear / ReLU / GELU / SiLU / Tanh / Softmax / MSELoss / CrossEntropyLoss / Sequential.
 
 Capability parity with the reference's ``shallowspeed/layers.py:17-233``: explicit
 ``forward(inputs, mubatch_id)`` / ``backward(dout, mubatch_id)`` with a per-micro-batch
@@ -203,6 +203,49 @@ class ReLU(Module):
         return "ReLU()"
 
 
+class _Gated(Module):
+    """A smooth activation f: ``forward`` returns f(z) and caches the gate gamma = f'(z) per micro-batch; ``backward``
+    is dout * gamma.  Under dropout the owning Linear stashes gamma * keep * s instead (``stash_gate``), so the
+    backward needs no mask of its own (ops.functional.activation_ref is the math)."""
+
+    kind = None
+
+    def forward(self, inputs, mubatch_id=0):
+        a, gamma = F.activation(self.kind, inputs)
+        self.stash_gate(gamma, mubatch_id)
+        return a
+
+    def stash_gate(self, gamma, mubatch_id=0):
+        if self._training:
+            self._cache[f"gate_{mubatch_id}"] = gamma
+
+    def backward(self, dout, mubatch_id=0):
+        assert self._training
+        return F.gate_grad(dout, self._cache.pop(f"gate_{mubatch_id}"))
+
+    def __repr__(self):
+        return f"{type(self).__name__}()"
+
+
+class GELU(_Gated):
+    """0.5 z (1 + erf(z / sqrt(2))): torch's ``nn.GELU()`` (the erf form)."""
+
+    kind = "gelu"
+
+
+class SiLU(_Gated):
+    """z sigmoid(z): torch's ``nn.SiLU()``."""
+
+    kind = "silu"
+
+
+class Tanh(_Gated):
+    kind = "tanh"
+
+
+ACTIVATIONS = {"relu": ReLU, "gelu": GELU, "silu": SiLU, "tanh": Tanh}
+
+
 class Softmax(Module):
     def forward(self, inputs, mubatch_id=0):
         if self._training:
@@ -228,14 +271,16 @@ def _init_seed(in_dims: int, out_dims: int, layer_index: Optional[int]):
 
 
 class Linear(Module):
-    """y = relu?(x @ W^T + b) with hand-written backward (reference: layers.py:99-142)."""
+    """y = f?(x @ W^T + b) with hand-written backward (reference: layers.py:99-142); f is ReLU, GELU, SiLU or tanh
+    (``activation``: "relu", "gelu", "silu", "tanh" or None)."""
 
     def __init__(self, in_dims, out_dims, activation="relu", arena: Optional[ParamArena] = None,
                  block_index: int = 0, layer_index: Optional[int] = None, device="cpu"):
         super().__init__()
-        assert activation is None or activation == "relu"
+        if activation is not None:
+            F.check_activation(activation)
         self.in_dims, self.out_dims = in_dims, out_dims
-        self.activation = ReLU() if activation == "relu" else None
+        self.activation = ACTIVATIONS[activation]() if activation is not None else None
         if arena is None:
             arena = ParamArena([(out_dims, in_dims)], device=device)
             block_index = 0
@@ -263,6 +308,13 @@ class Linear(Module):
         if self._training:
             self._cache[f"input_{mubatch_id}"] = inputs
         W, b = self._params["W"].data, self._params["b"].data
+        if isinstance(self.activation, _Gated):
+            # z, then (f(z), f'(z)) in one pass; dropout drops both, so the stashed gate is the whole backward
+            a, gamma = F.activation(self.activation.kind, F.linear(inputs, W, b))
+            if self._training and self.dropout is not None:
+                a, gamma = self._dropout(a), self._dropout(gamma)
+            self.activation.stash_gate(gamma, mubatch_id)
+            return a
         if inputs.is_cuda:
             from ..ops import cuda as K
 

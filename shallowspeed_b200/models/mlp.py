@@ -14,7 +14,7 @@ from typing import Optional, Sequence, Union
 
 import torch
 
-from ..ops.functional import check_dropout, check_loss, dropout_scale
+from ..ops.functional import check_activation, check_dropout, check_loss, dropout_scale
 from .layers import CrossEntropyLoss, Linear, MSELoss, ParamArena, Sequential, Softmax
 
 DEFAULT_LAYER_SIZES = [784, 128, 127, 126, 125, 124, 123, 10]  # reference train.py:98
@@ -51,7 +51,7 @@ def mlp_sizes(hidden: int, n_layers: int, in_dim: int = 784, out_dim: int = 10):
 class MLP(Sequential):
     def __init__(self, sizes: Sequence[int], stage_idx: int, n_stages: int, batch_size: int,
                  device="cpu", seed_mode: str = "shape", verbose: bool = False, loss: str = "mse",
-                 dropout: float = 0.0, dropout_seed: int = 0):
+                 dropout: float = 0.0, dropout_seed: int = 0, activation: str = "relu"):
         """
         :param batch_size: the GLOBAL batch size - the loss gradient is scaled by
             1/batch_size so that summing over micro-batches and DP replicas reproduces
@@ -65,9 +65,12 @@ class MLP(Sequential):
             (dropout_seed, global layer index, feature, the sample's position in the global batch, dropout_step)
             (ops.functional.dropout_mask), so every DP x PP layout draws the same masks.  Under pp=8 the default model's
             stage 6 ends in a 123->10 Linear that carries a ReLU (the stage rule above); it is dropped like any other.
+        :param activation: the activation of every Linear that has one (every hidden layer, never the logits): "relu"
+            (the reference's), "gelu" (erf form), "silu" or "tanh".  The pp=8 stage-6 Linear above carries it as well.
         """
         assert seed_mode in ("shape", "index")
         self.loss = check_loss(loss)
+        self.activation = check_activation(activation)
         self.dropout, self.dropout_seed = check_dropout(dropout, dropout_seed)
         self._dropout_step = 0
         self.dropout_shard = (0, 1)   # (DP rank, DP size) of the rows this replica forwards (set by the pipeline VM)
@@ -78,7 +81,7 @@ class MLP(Sequential):
         self.is_last_stage = stage_idx == n_stages - 1
         self.arena = ParamArena([(o, i) for i, o, _, _ in specs], device=device)
         layers = [
-            Linear(i, o, activation="relu" if relu else None, arena=self.arena, block_index=bi,
+            Linear(i, o, activation=self.activation if relu else None, arena=self.arena, block_index=bi,
                    layer_index=gidx if seed_mode == "index" else None)
             for bi, (i, o, relu, gidx) in enumerate(specs)
         ]

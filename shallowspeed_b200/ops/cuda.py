@@ -176,6 +176,25 @@ def relu_grad(grad_output, mask_or_output):
     return g
 
 
+def act_fwd(kind, z):
+    """(f(z), f'(z)) of a smooth activation ("gelu", "silu" or "tanh") in one pass of the stand-alone kernel."""
+    from .functional import ACTIVATION_CODES, check_activation
+
+    code = ACTIVATION_CODES[check_activation(kind)]
+    zc = z.contiguous()
+    a, g = torch.empty_like(zc), torch.empty_like(zc)
+    _C.act_fwd(code, zc, a, g)
+    return a, g
+
+
+def gate_grad(grad_output, gamma):
+    """grad_output * gamma (the backward of a smooth activation)."""
+    g = empty_padded(grad_output.size(0), grad_output.size(1), grad_output.device)
+    g.copy_(grad_output)
+    _C.gate_mul_(g, as_tma(gamma))
+    return g
+
+
 def _lr_arg(lr):
     """The update kernels read the learning rate from device memory when they run: a number is written into a device
     scalar on the current stream; a one-element fp32 CUDA tensor is passed through, so its value may still change

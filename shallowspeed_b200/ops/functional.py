@@ -173,6 +173,54 @@ def dropout_ref(a: torch.Tensor, keep: torch.Tensor, scale: float) -> torch.Tens
 
 
 # ----------------------------------------------------------------------------
+# hidden-layer activations: f and the gate f' in one pass, the same math as csrc/kernels/ptx.cuh: act_fwd
+# ----------------------------------------------------------------------------
+# the activations of the hidden Linears and their codes in the native runtime (csrc/kernels/activation.h: ActKind)
+ACTIVATION_CODES = {"relu": 0, "gelu": 1, "silu": 2, "tanh": 3}
+
+
+def check_activation(activation) -> str:
+    """The activation name, or ValueError for anything else than relu, gelu, silu or tanh."""
+    if not isinstance(activation, str) or activation not in ACTIVATION_CODES:
+        raise ValueError(f"unknown activation {activation!r}: expected one of {sorted(ACTIVATION_CODES)}")
+    return activation
+
+
+def activation_ref(kind: str, z: torch.Tensor):
+    """(a, gamma) = (f(z), f'(z)) in z's dtype.  gelu: the erf form, torch's ``F.gelu(approximate="none")``; silu:
+    ``F.silu``; tanh: ``torch.tanh``; relu: clamp and the 0 / 1 step (its derivative at 0 taken as 0)."""
+    check_activation(kind)
+    if kind == "gelu":
+        c = 0.5 * (1.0 + torch.erf(z * 0.7071067811865476))
+        return z * c, c + z * (torch.exp(-0.5 * z * z) * 0.3989422804014327)
+    if kind == "silu":
+        s = torch.sigmoid(z)
+        return z * s, s * (1.0 + z * (1.0 - s))
+    if kind == "tanh":
+        t = torch.tanh(z)
+        return t, 1.0 - t * t
+    return z.clamp_min(0.0), (z > 0).to(z.dtype)
+
+
+def activation(kind: str, z: torch.Tensor):
+    """(f(z), f'(z)) of a smooth activation: the stand-alone kernel on CUDA, activation_ref elsewhere."""
+    if _use_cuda(z) and kind != "relu":
+        from . import cuda as K
+
+        return K.act_fwd(kind, z)
+    return activation_ref(kind, z)
+
+
+def gate_grad(grad_output, gamma):
+    """The backward of a smooth activation: grad_output * gamma (gamma already holds dropout's keep * s)."""
+    if _use_cuda(grad_output):
+        from . import cuda as K
+
+        return K.gate_grad(grad_output, gamma)
+    return grad_output * gamma
+
+
+# ----------------------------------------------------------------------------
 # training-set shuffling: a keyed permutation of the dataset rows per epoch, the same map as csrc/kernels/ptx.cuh
 # ----------------------------------------------------------------------------
 SHUFFLE_WORD = 0x53485546   # "SHUF": the fourth counter word, which keeps these draws apart from dropout's

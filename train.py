@@ -26,7 +26,7 @@ from shallowspeed_b200.dataset import Dataset
 from shallowspeed_b200.layers import MLP, mlp_sizes
 from shallowspeed_b200.lr_schedule import DEFAULT_WARMUP_START_FACTOR, KINDS as LR_SCHEDULES, LRSchedule
 from shallowspeed_b200.models.mlp import DEFAULT_LAYER_SIZES
-from shallowspeed_b200.ops.functional import check_shuffle_seed
+from shallowspeed_b200.ops.functional import ACTIVATION_CODES, check_activation, check_shuffle_seed
 from shallowspeed_b200.optimizer import SGD
 from shallowspeed_b200.parallel.comm import ProcessGrid, SelfComm, make_torch_comms
 from shallowspeed_b200.pipe import (GPipeSchedule, InferenceSchedule, NaiveParallelSchedule,
@@ -94,6 +94,8 @@ def build_parser():
     p.add_argument("--nesterov", action="store_true", help="Nesterov momentum (needs --momentum > 0)")
     p.add_argument("--loss", choices=["mse", "cross-entropy"], default="mse",
                    help="mse: the reference's softmax + MSE; cross-entropy: softmax cross-entropy on the logits")
+    p.add_argument("--activation", default="relu", metavar="{" + ",".join(ACTIVATION_CODES) + "}",
+                   help="activation of every hidden layer: relu, gelu (erf form), silu or tanh")
     p.add_argument("--dropout", type=float, default=0.0,
                    help="inverted dropout with this drop probability on every hidden layer's output, in [0, 1)")
     p.add_argument("--dropout-seed", type=int, default=0, help="seed of the dropout masks, in [0, 2**64)")
@@ -184,10 +186,11 @@ def main(args):
     is_last = pp_comm.Get_rank() == args.pp - 1
 
     loss = args.loss.replace("-", "_")
+    activation = check_activation(args.activation)
     model = MLP(layer_sizes, stage_idx=pp_comm.Get_rank(), n_stages=args.pp,
                 batch_size=args.global_batch_size, seed_mode=args.seed_mode,
                 verbose=(grid.rank == 0 or is_last), loss=loss, dropout=args.dropout,
-                dropout_seed=args.dropout_seed)
+                dropout_seed=args.dropout_seed, activation=activation)
     model.to(device)
     model.train()
     # before the resume: the momentum arena it restores is allocated here
@@ -213,7 +216,8 @@ def main(args):
                "n_mubatches": int(args.n_mubatches), "momentum": float(args.momentum),
                "weight_decay": float(args.weight_decay), "nesterov": bool(args.nesterov), "loss": loss,
                "lr_schedule": lr_schedule.spec(), "dropout": float(args.dropout),
-               "dropout_seed": int(args.dropout_seed), "shuffle": bool(args.shuffle), "shuffle_seed": shuffle_seed}
+               "dropout_seed": int(args.dropout_seed), "shuffle": bool(args.shuffle), "shuffle_seed": shuffle_seed,
+               "activation": activation}
     resumed_step = 0
     if args.resume:
         from shallowspeed_b200.utils.checkpoint import load_stage

@@ -60,30 +60,71 @@ static void enable_splitk(ssb::GemmPlan& plan, int64_t k_splits, const Tensor& l
     TORCH_CHECK(err == nullptr, "split-K: ", err ? err : "");
 }
 
-// y[rows, out] = relu?(x @ W^T + b); split: 3xTF32 (fp32-equivalent) products
+// The dropout of a stand-alone GEMM: None, or (p, seed, layer, step, row_base, dp, rank) as DropoutSpec describes them.
+// `step` goes into a fresh device scalar on the current stream, which `step_dev` keeps alive until the launch is enqueued.
+static ssb::DropoutSpec drop_arg(const py::object& drop, const Tensor& like, Tensor& step_dev, const char* what) {
+    if (drop.is_none()) return ssb::DropoutSpec{};
+    const auto d = py::cast<std::tuple<double, uint64_t, int64_t, int64_t, int64_t, int64_t, int64_t>>(drop);
+    const double p = std::get<0>(d);
+    const int64_t layer = std::get<2>(d), step = std::get<3>(d), row_base = std::get<4>(d), dp = std::get<5>(d),
+                  rank = std::get<6>(d);
+    TORCH_CHECK(p > 0.0 && p < 1.0, what, ": dropout p must lie in (0, 1)");
+    TORCH_CHECK(layer >= 0 && layer < (1 << 30) && step >= 0 && step < (int64_t(1) << 32) && row_base >= 0 &&
+                    row_base < (1 << 30) && dp >= 1 && dp < (1 << 30) && rank >= 0 && rank < dp,
+                what, ": dropout argument out of range");
+    ssb::DropoutSpec spec = ssb::dropout_spec(p, std::get<1>(d));
+    step_dev = torch::full({1}, (int32_t)(uint32_t)step, like.options().dtype(torch::kInt32));
+    spec.step = reinterpret_cast<const uint32_t*>(step_dev.data_ptr<int32_t>());
+    spec.layer = (int)layer; spec.row_base = (int)row_base; spec.dp = (int)dp; spec.rank = (int)rank;
+    return spec;
+}
+
+// y[rows, out] = act?(x @ W^T + b); split: 3xTF32 (fp32-equivalent) products.  relu selects the layer's activation
+// act_kind (activation.h: ReLU by default); a smooth kind can store its gate f'(z) (* keep * s under dropout) to `gate`,
+// which the kernel addresses with y's row pitch.  drop: see drop_arg, applied after the activation.
 static void linear_fwd(const Tensor& x, const Tensor& W, const c10::optional<Tensor>& bias, int64_t bias_stride,
-                       bool relu, Tensor& y, bool split, int64_t k_splits) {
+                       bool relu, Tensor& y, bool split, int64_t k_splits, int64_t act_kind,
+                       const c10::optional<Tensor>& gate, const py::object& drop) {
     check_mat(x, "x"); check_mat(W, "W"); check_mat(y, "y");
     const int rows = x.size(0), in = x.size(1), out = W.size(0);
     TORCH_CHECK(W.size(1) == in && y.size(0) == rows && y.size(1) == out, "linear_fwd: shape mismatch");
+    TORCH_CHECK(ssb::act_valid((int)act_kind), "linear_fwd: act_kind must be 0 (ReLU), 1 (GELU), 2 (SiLU) or 3 (tanh)");
+    TORCH_CHECK(relu || (act_kind == ssb::ACT_RELU && !gate.has_value() && drop.is_none()),
+                "linear_fwd: an activation kind, a gate or dropout needs relu (an activated layer)");
+    if (gate.has_value()) {
+        check_mat(*gate, "gate");
+        TORCH_CHECK(ssb::act_smooth((int)act_kind), "linear_fwd: only a smooth activation stores a gate");
+        TORCH_CHECK(gate->size(0) == rows && gate->size(1) == out && gate->device() == y.device(), "linear_fwd: gate shape");
+        TORCH_CHECK(ld_of(*gate) == ld_of(y), "linear_fwd: the gate must have y's row pitch (the kernel writes it with y's)");
+    }
     c10::cuda::CUDAGuard guard(x.device());
     ssb::GemmPlan plan;
     const char* err = ssb::gemm_plan_fwd(&plan, W.data_ptr<float>(), ld_of(W), x.data_ptr<float>(), ld_of(x),
                                          y.data_ptr<float>(), ld_of(y), rows, in, out,
                                          bias.has_value() ? bias->data_ptr<float>() : nullptr, (int)bias_stride, relu, split);
     TORCH_CHECK(err == nullptr, "linear_fwd: ", err ? err : "");
+    Tensor step_dev;
+    plan.p.act_kind = (int)act_kind;
+    plan.p.gate = gate.has_value() ? gate->data_ptr<float>() : nullptr;
+    plan.p.drop = drop_arg(drop, x, step_dev, "linear_fwd");
     Tensor ws, counters;
     enable_splitk(plan, k_splits, x, ws, counters);
     cuda_ok(ssb::gemm_launch(plan, cur_stream()), "linear_fwd launch");
 }
 
-// dx[rows, in] = (dz @ W) * (mask > 0)
+// dx[rows, in] = (dz @ W) * (mask > 0), or * s where the mask passes under dropout (only its p is read), or * mask for a
+// smooth act_kind (the mask is then the previous layer's gate, which holds the dropout scale itself)
 static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<Tensor>& mask, Tensor& dx,
-                         bool split, int64_t k_splits) {
+                         bool split, int64_t k_splits, int64_t act_kind, const py::object& drop) {
     check_mat(dz, "dz"); check_mat(W, "W"); check_mat(dx, "dx");
     const int rows = dz.size(0), out = dz.size(1), in = W.size(1);
     TORCH_CHECK(W.size(0) == out && dx.size(0) == rows && dx.size(1) == in, "linear_dgrad: shape mismatch");
     if (mask.has_value()) { check_mat(*mask, "mask"); TORCH_CHECK(mask->size(0) == rows && mask->size(1) == in, "mask shape"); }
+    TORCH_CHECK(ssb::act_valid((int)act_kind), "linear_dgrad: act_kind must be 0 (ReLU), 1 (GELU), 2 (SiLU) or 3 (tanh)");
+    TORCH_CHECK(mask.has_value() || (act_kind == ssb::ACT_RELU && drop.is_none()),
+                "linear_dgrad: an activation kind or dropout needs a mask");
+    TORCH_CHECK(drop.is_none() || !ssb::act_smooth((int)act_kind),
+                "linear_dgrad: a gate holds its dropout scale already; pass no dropout with a smooth act_kind");
     c10::cuda::CUDAGuard guard(dz.device());
     ssb::GemmPlan plan;
     const char* err = ssb::gemm_plan_dgrad(&plan, W.data_ptr<float>(), ld_of(W), dz.data_ptr<float>(), ld_of(dz),
@@ -91,6 +132,9 @@ static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<
                                            mask.has_value() ? mask->data_ptr<float>() : nullptr,
                                            mask.has_value() ? ld_of(*mask) : 0, split);
     TORCH_CHECK(err == nullptr, "linear_dgrad: ", err ? err : "");
+    Tensor step_dev;
+    plan.p.act_kind = (int)act_kind;
+    plan.p.drop = drop_arg(drop, dz, step_dev, "linear_dgrad");
     Tensor ws, counters;
     enable_splitk(plan, k_splits, dz, ws, counters);
     cuda_ok(ssb::gemm_launch(plan, cur_stream()), "linear_dgrad launch");
@@ -269,9 +313,11 @@ static void gather_rows(const c10::optional<Tensor>& x_src, const c10::optional<
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.doc() = "shallowspeed_b200 native module: sm_90a kernels + C++ pipeline runtime";
     m.def("linear_fwd", &linear_fwd, py::arg("x"), py::arg("W"), py::arg("bias"), py::arg("bias_stride"), py::arg("relu"),
-          py::arg("y"), py::arg("split") = false, py::arg("k_splits") = 0);
+          py::arg("y"), py::arg("split") = false, py::arg("k_splits") = 0, py::arg("act_kind") = (int)ssb::ACT_RELU,
+          py::arg("gate") = py::none(), py::arg("drop") = py::none());
     m.def("linear_dgrad", &linear_dgrad, py::arg("dz"), py::arg("W"), py::arg("mask"), py::arg("dx"),
-          py::arg("split") = false, py::arg("k_splits") = 0);
+          py::arg("split") = false, py::arg("k_splits") = 0, py::arg("act_kind") = (int)ssb::ACT_RELU,
+          py::arg("drop") = py::none());
     m.def("linear_wgrad", &linear_wgrad, py::arg("dz"), py::arg("x"), py::arg("G"), py::arg("accumulate"), py::arg("db"),
           py::arg("db_stride"), py::arg("W"), py::arg("lr"), py::arg("fuse_sgd"), py::arg("split") = false,
           py::arg("V") = py::none(), py::arg("momentum") = 0.0, py::arg("weight_decay") = 0.0, py::arg("nesterov") = false);

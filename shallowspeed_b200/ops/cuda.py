@@ -67,21 +67,42 @@ def _split(precision):
     return (precision or PRECISION) in ("fp32", "fp32x3", "3xtf32")
 
 
-def linear_fwd(x, weight, bias=None, relu=False, out=None, precision=None, k_splits=0):
-    """k_splits: 0 = plain kernel, -1 = planner decides, k >= 2 = force k k-splits (experimental wide-layer variant)."""
+def _act_code(activation):
+    from .functional import ACTIVATION_CODES, check_activation
+
+    return ACTIVATION_CODES[check_activation(activation)]
+
+
+def _drop_arg(dropout):
+    """None, or the dropout of the launch as (p, seed, layer, step, row_base, dp, rank): row n of the launch draws the mask
+    of sample (row_base + n) * dp + rank (``functional.dropout_mask``)."""
+    if dropout is None:
+        return None
+    p, seed, layer, step, row_base, dp, rank = dropout
+    return float(p), int(seed), int(layer), int(step), int(row_base), int(dp), int(rank)
+
+
+def linear_fwd(x, weight, bias=None, relu=False, out=None, precision=None, k_splits=0, activation="relu", gate=None,
+               dropout=None):
+    """k_splits: 0 = plain kernel, -1 = planner decides, k >= 2 = force k k-splits (experimental wide-layer variant).
+    With ``relu`` the layer is activated by ``activation``; a smooth one stores f'(z) into ``gate`` (a view with ``out``'s
+    row pitch) when one is given.  ``dropout`` (see ``_drop_arg``) drops the activated output and its gate."""
     x, weight = as_tma(x), as_tma(weight)
     rows, out_dims = x.size(0), weight.size(0)
     y = out if out is not None else empty_padded(rows, out_dims, x.device)
     b, bstride = _bias_arg(bias, out_dims)
-    _C.linear_fwd(x, weight, b, bstride, bool(relu), y, _split(precision), int(k_splits))
+    _C.linear_fwd(x, weight, b, bstride, bool(relu), y, _split(precision), int(k_splits), _act_code(activation), gate,
+                  _drop_arg(dropout))
     return y
 
 
-def linear_dgrad(dz, weight, mask=None, out=None, precision=None, k_splits=0):
+def linear_dgrad(dz, weight, mask=None, out=None, precision=None, k_splits=0, activation="relu", dropout=None):
+    """dX = dz @ W, masked where ``mask <= 0`` (ReLU; times the dropout scale where it passes when ``dropout`` is given), or
+    times ``mask`` for a smooth ``activation``, whose mask is the previous layer's gate."""
     dz, weight = as_tma(dz), as_tma(weight)
     dx = out if out is not None else empty_padded(dz.size(0), weight.size(1), dz.device)
     m = None if mask is None else as_tma(mask)
-    _C.linear_dgrad(dz, weight, m, dx, _split(precision), int(k_splits))
+    _C.linear_dgrad(dz, weight, m, dx, _split(precision), int(k_splits), _act_code(activation), _drop_arg(dropout))
     return dx
 
 

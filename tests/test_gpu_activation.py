@@ -1,12 +1,15 @@
 """GELU, SiLU and tanh hidden layers on one GPU, against fp64 (ops.functional.activation_ref, dropout_mask):
 
-* per layer and micro-batch, from the engine's own buffers after one Trainer step: act[l] matches f(z) * keep * s, the
-  gate gate[l] matches f'(z) * keep * s, every dgrad matches (dz[l] @ W) * gamma, and the update matches act and dz.  The
+* per layer, micro-batch and element, from the engine's own buffers after one Trainer step (test_gpu_chain:
+  check_layers): act[l] matches f(z) * keep * s, the gate gate[l] matches f'(z) * keep * s, every dgrad matches
+  (dz[l] @ W) * gamma, and the update matches act and dz.  The
   cluster chain (k-split layer 1), the one-CTA chain, per-micro-batch launches, the layer-wise GEMMs, split-K on wide
   layers; fp32 and tf32, MSE and cross-entropy, with and without dropout;
 * a pipeline stage with its neighbours replayed from memory: folded and unfolded boundaries and the layer-wise plan,
   the last forward layer's gate applied to the received gradient;
 * several engine steps against the Python VM on the CPU;
+* the stand-alone act_fwd kernel across the fp32 range within the device formulas' rounding bound, gate_mul_ on
+  pitched buffers bitwise;
 * inference plans apply f and keep no gates; gated plans launch as many kernels and graph nodes as ReLU's and differ
   from its plan text only by their act= tags; activation="relu" is the default model bit for bit.
 """
@@ -15,13 +18,14 @@ import re
 import pytest
 import torch
 
+from test_gpu_chain import check_layers, worst_table  # noqa: F401  (the table of worst err / bound)
+
 pytestmark = pytest.mark.gpu
 
 SIZES = [784, 128, 127, 126, 125, 124, 123, 10]
 KINDS = ["gelu", "silu", "tanh"]
 P, SEED = 0.3, 0xDEAD_BEEF_1234_5678
-ACT_TOL = {"fp32": 1e-5, "tf32": 5e-3}     # relative Frobenius error of one layer against fp64, from its own inputs
-UPD_TOL = 2e-2
+UPD_TOL = 2e-2                              # whole trajectories against the Python VM
 
 
 def _frob(a, b):
@@ -34,51 +38,6 @@ def _batch(rows, in_dim, classes, seed=0):
     y = torch.zeros(rows, classes)
     y[torch.arange(rows), torch.randint(0, classes, (rows,), generator=g)] = 1.0
     return x.pin_memory(), y.pin_memory()
-
-
-def check_layers(eng, model, W0, x, n_mu, mb, precision, lr, samples_of, p, step=0, check_update=True):
-    """Every layer of the step that just ran, per micro-batch, from the engine's own buffers against fp64."""
-    from shallowspeed_b200.ops import functional as F
-
-    kind = model.activation
-    L, tol = len(model.linears), ACT_TOL[precision]
-    upd = [torch.zeros(lin.out_dims, lin.in_dims + 1, dtype=torch.float64) for lin in model.linears]
-    for mu in range(n_mu):
-        samples = samples_of(mu)
-        acts = [x[mu * mb:(mu + 1) * mb].double()] + [eng.act(mu, l).double().cpu() for l in range(1, L + 1)]
-        dzs = [eng.dz(mu, l).double().cpu() for l in range(L + 1)]
-        gammas = [None] * (L + 1)
-        for l, lin in enumerate(model.linears, start=1):
-            blk = W0[model.arena.offsets[lin.block_index]:][: lin.out_dims * model.arena.lds[lin.block_index]]
-            blk = blk.view(lin.out_dims, -1).double().cpu()
-            W, b = blk[:, : lin.in_dims], blk[:, lin.in_dims]
-            z = acts[l - 1] @ W.T + b
-            if lin.activation is not None:
-                a, g = F.activation_ref(kind, z)
-                if p > 0:
-                    keep = F.dropout_mask(p, SEED, lin.dropout[2], step, samples, lin.out_dims)
-                    s = F.dropout_scale(p)
-                    a, g = a * keep * s, g * keep * s
-                    assert torch.all(acts[l][~keep] == 0) and int((~keep).sum()) > 0, (mu, l)
-                got_g = eng.gate(mu, l).double().cpu()
-                assert _frob(acts[l], a) < tol, (mu, l, _frob(acts[l], a))
-                assert _frob(got_g, g) < tol, (mu, l, _frob(got_g, g))
-                gammas[l] = g
-            if l >= 2:
-                want = dzs[l] @ W
-                if gammas[l - 1] is not None:
-                    want = want * gammas[l - 1]
-                assert _frob(dzs[l - 1], want) < tol, (mu, l, _frob(dzs[l - 1], want))
-            upd[l - 1][:, : lin.in_dims] += dzs[l].T @ acts[l - 1]
-            upd[l - 1][:, lin.in_dims] += dzs[l].sum(0)
-    if not check_update:
-        return
-    W1 = model.arena.weights.detach().double().cpu()
-    for lin, u in zip(model.linears, upd):
-        o, ld = lin.out_dims, model.arena.lds[lin.block_index]
-        off = model.arena.offsets[lin.block_index]
-        d = (W1[off:off + o * ld] - W0[off:off + o * ld].double().cpu()).view(o, ld)[:, : lin.in_dims + 1]
-        assert _frob(d, -lr * u) < UPD_TOL, lin
 
 
 NO_COALESCE = {"SSB_NO_COALESCE": "1"}
@@ -131,7 +90,7 @@ def test_every_layer_matches_fp64(case, kind, p, monkeypatch):
     tr.step(x, y)
     tr.synchronize()
     mb = gbs // n_mu
-    check_layers(eng, model, W0, x, n_mu, mb, precision, lr, lambda mu: mu * mb + torch.arange(mb), p)
+    check_layers(eng, model, W0, x, n_mu, mb, precision, lr, lambda mu: mu * mb + torch.arange(mb))
 
 
 # ---------------------------------------------------------------- pipeline stages, neighbours replayed from memory
@@ -211,7 +170,7 @@ def test_pipeline_stage_applies_its_gates_at_the_boundary(case, kind, monkeypatc
     check_tiles(nb["prev"].dz_in.cpu(), dz_0, 127, "dz pushed to stage 0")
     # the received gradient times this stage's last gate (which holds keep * s): one fp32 multiply
     assert torch.equal(dz_L[..., :125], dz_in.view(n_mu, mb, 125) * gate_L[..., :125])
-    check_layers(eng, model, W0, x, n_mu, mb, "fp32", lr, lambda mu: mu * mb + torch.arange(mb), P, step=3,
+    check_layers(eng, model, W0, x, n_mu, mb, "fp32", lr, lambda mu: mu * mb + torch.arange(mb), step=3,
                  check_update=False)
     assert not torch.equal(W0, model.arena.weights.detach())
 
@@ -320,17 +279,60 @@ def test_explicit_relu_is_the_default_bit_for_bit():
     assert not torch.equal(a.model.arena.weights, other.model.arena.weights)
 
 
+def _sweep():
+    """fp32 inputs of the stand-alone act_fwd check: every 2^10-th bit pattern with |z| in [2^-20, 2^8], +-0, subnormals,
+    +-FLT_MAX, and 64 consecutive patterns on either side of SiLU's expf overflow (88.72), of GELU's z * z overflow
+    (sqrt(FLT_MAX) = 1.84e19) and of tanh's saturation (9), all with both signs."""
+    f32 = lambda v: torch.tensor([v], dtype=torch.float32).view(torch.int32).item()
+    pats = [torch.arange(f32(2.0**-20), f32(2.0**8) + 1, 1024, dtype=torch.int64)]
+    pats.append(torch.tensor([0, 1, 2, 3, 0x3FFFFF, 0x7FFFFF, 0x800000, f32(3.4028234663852886e38)], dtype=torch.int64))
+    for edge in (88.72283935546875, 1.8446742974197924e19, 9.0):
+        pats.append(f32(edge) + torch.arange(-64, 65, dtype=torch.int64))
+    bits = torch.cat(pats).to(torch.int32)
+    z = bits.view(torch.float32)
+    return torch.cat([z, -z])
+
+
+ACT_WORST = {}
+
+
 @pytest.mark.parametrize("kind", KINDS)
 def test_module_path_kernels_match_the_oracle(kind):
-    """The stand-alone activation and gate-multiply kernels (the Module API on CUDA) against fp64."""
-    from shallowspeed_b200.ops import cuda as K
-    from shallowspeed_b200.ops import functional as F
+    """The stand-alone activation kernel (ptx.cuh: act_fwd) per element against fp64 across the fp32 range, within the
+    device formulas' rounding bound (test_gpu_chain: act_rounding_bound); every finite input gives finite outputs."""
+    from test_gpu_chain import ATOL, act_ref, act_rounding_bound
 
-    z = torch.cat([torch.linspace(-30, 30, 4001), torch.tensor([-1e30, -120.0, 120.0, 1e30])])
+    from shallowspeed_b200.ops import cuda as K
+
+    z = _sweep()
     a, g = K.act_fwd(kind, z.cuda())
-    ra, rg = F.activation_ref(kind, z.double())
-    assert torch.allclose(a.double().cpu(), ra, rtol=2e-6, atol=1e-6)
-    assert torch.allclose(g.double().cpu(), rg, rtol=2e-6, atol=1e-6)
-    dout = torch.randn(64, 45, generator=torch.Generator().manual_seed(1)).cuda()
-    gam = torch.rand(64, 45, generator=torch.Generator().manual_seed(2)).cuda()
-    assert torch.equal(K.gate_grad(dout, gam), dout * gam)
+    a, g = a.cpu(), g.cpu()
+    assert bool(torch.isfinite(a).all()) and bool(torch.isfinite(g).all()), kind
+    f, f1, _ = act_ref(kind, z)
+    Ba, Bg = act_rounding_bound(kind, z, 0.0)
+    ra = ((a.double() - f).abs() / (Ba + ATOL))
+    rg = ((g.double() - f1).abs() / (Bg + ATOL))
+    worst = {"a": (float(ra.max()), float(z[ra.argmax()])), "g": (float(rg.max()), float(z[rg.argmax()]))}
+    print(f"\n[act_fwd] {kind}: {z.numel()} inputs, worst err/bound a {worst['a'][0]:.3g} at z={worst['a'][1]:.6g}, "
+          f"g {worst['g'][0]:.3g} at z={worst['g'][1]:.6g}")
+    assert worst["a"][0] <= 1.0 and worst["g"][0] <= 1.0, worst
+
+
+def test_gate_mul_on_pitched_buffers():
+    """g *= gamma bitwise in fp32 on buffers of different row pitches, NaN in both paddings, which keep their bits."""
+    from shallowspeed_b200 import _C
+
+    gen = torch.Generator().manual_seed(4)
+    rows, cols = 37, 45
+    gbuf = torch.full((rows, 48), float("nan"))
+    gbuf[:, :cols] = torch.randn(rows, cols, generator=gen)
+    hbuf = torch.full((rows, 56), float("nan"))
+    hbuf[:, :cols] = torch.randn(rows, cols, generator=gen)
+    want = gbuf[:, :cols] * hbuf[:, :cols]
+    gd, hd = gbuf.cuda(), hbuf.cuda()
+    _C.gate_mul_(gd[:, :cols], hd[:, :cols])
+    torch.cuda.synchronize()
+    got = gd.cpu()
+    bits = lambda t: t.contiguous().view(torch.int32)
+    assert torch.equal(bits(got[:, :cols]), bits(want))
+    assert torch.equal(bits(got[:, cols:]), bits(gbuf[:, cols:])) and torch.equal(bits(hd.cpu()), bits(hbuf))

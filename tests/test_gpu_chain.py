@@ -114,19 +114,234 @@ def tf32_trunc(x):
     return (x.float().contiguous().view(torch.int32) & -8192).view(torch.float32)
 
 
+# ================================================================================================== activated layers
+# The forward epilogue of an activated layer computes z in fp32 (the GEMM), then a = f(z) and the gate g = f'(z) with the
+# device formulas of ptx.cuh: act_fwd, then, under dropout, keep ? (a * s, g * s) : (0, 0).  Against the fp64 reference
+# f(z_ref) * s, with z_ref and e_z = rtol * mag + ATOL from fwd_oracle, the error of a kept element is at most
+#   (a) s * e_z * sup |f'| over [z_ref - e_z, z_ref + e_z]   (z carried through f; sup |f'| <= |f'(z_ref)| + e_z * M2)
+#   (b) s * B(z): the rounding of the device formula itself, for any fp32 z in that interval
+#   (c) U * s * |f|: the one rounding of "* s"
+# and the same for g with f' and f'' in place of f and f'.  M1, M2, M3 = sup |f'|, |f''|, |f'''| over the reals.
+#
+# (b), by operation, with U = 2^-24: a product or a sum adds U of its result, a correctly rounded division the same,
+# and erff, expf and tanhf add 2 ulp <= 4U of theirs (the CUDA Math API's maximum ulp errors; no fast-math).  An input
+# error carries through the operation's derivative.  First order in U (the dropped U^2 terms are below 1e-6 of these):
+#   GELU  c = 0.5 (1 + erff(z * fl(1/sqrt2))): 2U of the product, carried through erf' (at most (2/sqrt(pi)) u e^-u^2
+#         * 2U < U), 4U of erff, U * 2c of the sum:        |dc| <= 2.5U + U c (absolute: the 1 + erf cancellation)
+#         a = z c:                                          |da| <= U |z| (2.5 + 2c)
+#         g = c + z (expf(-0.5 z z) * fl(1/sqrt(2 pi))): U z^2 / 2 of the exponent carried through exp, 4U of expf, U
+#         of the constant, 3U of the products, U of the sum: |dg| <= U (2.5 + c + |g| + |z| phi(z) (7 + z^2 / 2))
+#   SiLU  s = 1 / (1 + expf(-z)): 4U of expf, U of the sum, U of the division: |ds| <= 6U s, and, since 1 is a
+#         rounding candidate of both the sum and the quotient, |ds| <= (2 + 4U)(1 - s) as well (s rounds to 1 once
+#         e^-z < U: the error is then e^-z, not 6U); q = 1 - s: |dq| <= |ds| + U q
+#         a = z s:                                          |da| <= |z| |ds| + U |a|
+#         g = s (1 + z q): r = z q, |dr| <= |z| |dq| + U |z| q ; w = 1 + r, |dw| <= |dr| + U |w|
+#                                                           |dg| <= |w| |ds| + s |dw| + U |g|
+#   tanh  t = tanhf(z), |dt| <= 4U |t| ;  a = t:             |da| <= 4U |t|
+#         g = 1 - t t:                                      |dg| <= 9U t^2 + U |g| (1 - t^2 cancels: absolute)
+# Each magnitude is taken at its supremum over [z_ref - e_z, z_ref + e_z] (|z| + e_z, sigma and Phi at the upper end,
+# |f| + e_z M1, ...).  ATOL (1e-30) covers what the first-order terms do not: expf overflowing to inf below z = -88.72
+# (SiLU's s = 0 where sigma(z) < 3e-39) and subnormal intermediates, all below 1e-36 in absolute terms.
+# These terms are absolute errors of order |z| * 2^-24 where f or f' is small against |z| (GELU below z = -5, tanh' above
+# |z| = 8): the tests accept that tail cancellation; act_fwd does not change.
+ACT_LIP = {"gelu": (1.13, 0.80, 0.78), "silu": (1.10, 0.50, 0.31), "tanh": (1.0, 0.77, 2.0)}   # M1, M2, M3, rounded up
+U = 2.0**-24
+_SQRT2 = math.sqrt(2.0)
+
+
+def act_ref(kind, z):
+    """(f, f', f'') of a smooth activation in fp64 (GELU through erfc, so that its left tail keeps its digits)."""
+    z = z.double()
+    if kind == "gelu":
+        Phi = 0.5 * torch.special.erfc(-z / _SQRT2)
+        phi = torch.exp(-0.5 * z * z) / math.sqrt(2.0 * math.pi)
+        return z * Phi, Phi + z * phi, phi * (2.0 - z * z)
+    if kind == "silu":
+        s, q = torch.sigmoid(z), torch.sigmoid(-z)
+        return z * s, s * (1.0 + z * q), s * q * (2.0 - z * torch.tanh(0.5 * z))
+    t, sech2 = torch.tanh(z), 1.0 / torch.cosh(z) ** 2
+    return t, sech2, -2.0 * t * sech2
+
+
+def act_rounding_bound(kind, z, e):
+    """Bound (b) on |f_dev(y) - f(y)| and |f'_dev(y) - f'(y)| for every fp32 y within ``e`` of ``z`` (see above)."""
+    z, e = z.double(), torch.as_tensor(e, dtype=torch.float64)
+    M1, M2, _ = ACT_LIP[kind]
+    f, f1, _ = act_ref(kind, z)
+    lo, hi = z - e, z + e
+    Z = z.abs() + e
+    A, G = f.abs() + e * M1, f1.abs() + e * M2
+    if kind == "gelu":
+        C = 0.5 * torch.special.erfc(-hi / _SQRT2)
+        zmin = (z.abs() - e).clamp_min(0.0)
+        tail = torch.exp(-0.5 * zmin * zmin) / math.sqrt(2.0 * math.pi) * Z * (7.0 + 0.5 * Z * Z)
+        return U * Z * (2.5 + 2.0 * C), U * (2.5 + C + G + tail)
+    if kind == "silu":
+        S, Q = torch.sigmoid(hi), torch.sigmoid(-lo)
+        ds = torch.minimum(6.0 * U * S, (2.0 + 4.0 * U) * Q)
+        dq = ds + U * Q
+        Wm = 1.0 + Z * Q
+        dw = Z * dq + U * Z * Q + U * Wm
+        return Z * ds + U * A, Wm * ds + S * dw + U * G
+    T = torch.maximum(torch.tanh(lo).abs(), torch.tanh(hi).abs())
+    return 4.0 * U * T, 9.0 * U * T * T + U * G
+
+
+def act_fwd_oracle(kind, a_prev, W, b, keep, s, rtol):
+    """An activated layer from the kernel's own input: ((act, bound), (gate, bound) or None, z_ref) in fp64.  ``keep``:
+    the dropout mask (None: no dropout), ``s``: the fp32 scale the kernel multiplies by.  Dropped elements have the
+    reference 0 and the bound ATOL; the caller checks them bitwise."""
+    z, e = fwd_oracle(a_prev, W, b, False, rtol)
+    keep_f = torch.ones_like(z) if keep is None else keep.to(z.device).double()
+    if kind == "relu":
+        a = z.clamp_min(0.0)
+        return (a * s * keep_f, (s * e + U * s * a) * keep_f + ATOL), None, z
+    M1, M2, M3 = ACT_LIP[kind]
+    f, f1, f2 = act_ref(kind, z)
+    Ba, Bg = act_rounding_bound(kind, z, e)
+    ba = s * (e * (f1.abs() + e * M2) + Ba) + U * s * (f.abs() + e * M1)
+    bg = s * (e * (f2.abs() + e * M3) + Bg) + U * s * (f1.abs() + e * M2)
+    return (f * s * keep_f, ba * keep_f + ATOL), (f1 * s * keep_f, bg * keep_f + ATOL), z
+
+
+def act_dgrad_oracle(dz, W, kind, act_prev, gate_prev, s, rtol):
+    """dgrad through an activated layer, from the kernel's own stored mask: (dz @ W) * gate_prev for a smooth kind,
+    (dz @ W) * (act_prev > 0) * s for ReLU (s = 1 without dropout), and its bound.  One more rounding, of the multiply."""
+    dz, W = dz.double(), W.double()
+    m = gate_prev.double() if kind != "relu" else (act_prev > 0).double() * s
+    ref = (dz @ W) * m
+    return ref, rtol * (dz.abs() @ W.abs()) * m.abs() + U * ref.abs() + ATOL
+
+
+def rows_update_oracle(dz, a_prev, W0, lr, rtol):
+    """update_oracle plus the bias column's fp32 sum over the rows in order (one rounding per row, as test_gpu_gemm's
+    grad_oracle): the engines sum up to 1024 rows, past RTOL's margin for it in fp32."""
+    d, bound = update_oracle(dz, a_prev, W0, lr, rtol)
+    bound[:, -1] += dz.shape[0] * U * lr * dz.double().abs().sum(0)
+    return d, bound
+
+
+WORST = {}                    # (kernel, activation, dropout, precision) -> (worst err / bound, its check and case)
+
+
+def note_worst(key, res, what):
+    for k, v in res.items():
+        if v > WORST.get(key, (-1.0, ""))[0]:
+            WORST[key] = (v, f"{k} at {what}")
+
+
+@pytest.fixture(scope="module", autouse=True)
+def worst_table():
+    yield
+    print()
+    for (kernel, kind, drop, precision), (v, what) in sorted(WORST.items()):
+        print(f"[worst] {kernel:>10} {kind:>4} {'drop' if drop else 'nodrop':>6} {precision}: {v:.3g} ({what})")
+
+
+def check_layers(eng, model, W0, x, n_mu, mb, precision, lr, samples_of, step=0, check_update=True):
+    """Every layer of the step that just ran, per micro-batch and per element, from the engine's own buffers against
+    fp64: act (and the gate) of every activated layer through act_fwd_oracle, with the masks of
+    ``ops.functional.dropout_mask`` and dropped elements exactly 0; every dgrad through act_dgrad_oracle from the stored
+    act / gate; the update through rows_update_oracle.  ``samples_of(mu)``: the global sample index of every row of
+    micro-batch mu; ``x``: the stage input of the step; ``W0``: the flat weight arena before the step.  Returns
+    {check: max err / bound}."""
+    from shallowspeed_b200.ops import functional as F
+
+    kind, p, rtol = model.activation, model.dropout, RTOL[precision]
+    s = F.dropout_scale(p) if p > 0 else 1.0
+    L = len(model.linears)
+    res, n_dropped, tails = {}, 0, [0, 0]
+    upd_dz = [[] for _ in range(L)]
+    upd_a = [[] for _ in range(L)]
+    blocks = []
+    for lin in model.linears:
+        blk = W0[model.arena.offsets[lin.block_index]:][: lin.out_dims * model.arena.lds[lin.block_index]]
+        blocks.append(blk.view(lin.out_dims, -1)[:, : lin.in_dims + 1].double().cpu())
+
+    def put(k, v):
+        res[k] = max(res.get(k, 0.0), v)
+
+    for mu in range(n_mu):
+        samples = samples_of(mu)
+        # act[0] of the engine is the staging set of the NEXT step; the step's input is x itself
+        acts = [x[mu * mb:(mu + 1) * mb].double()] + [eng.act(mu, l).double().cpu() for l in range(1, L + 1)]
+        raw = [None] + [eng.act(mu, l).cpu() for l in range(1, L + 1)]
+        dzs = [eng.dz(mu, l).double().cpu() for l in range(L + 1)]
+        gates = [None] * (L + 1)
+        for l, lin in enumerate(model.linears, start=1):
+            W, b = blocks[l - 1][:, :-1], blocks[l - 1][:, -1]
+            if lin.activation is not None:
+                keep = F.dropout_mask(p, model.dropout_seed, lin.dropout[2], step, samples, lin.out_dims) if p > 0 else None
+                (ra, ba), gam, z = act_fwd_oracle(kind, acts[l - 1], W, b, keep, s, rtol)
+                put(f"act{l}", excess(acts[l], ra, ba))
+                tails[0] += int((z.abs() > 4).sum())
+                tails[1] += int((z.abs() > 9).sum())
+                if kind != "relu":
+                    gates[l] = eng.gate(mu, l).cpu()
+                    put(f"gate{l}", excess(gates[l], *gam))
+                if keep is not None:
+                    assert int((~keep).sum()) > 0, (mu, l)
+                    n_dropped += int((~keep & ((z > 0) if kind == "relu" else (z != 0))).sum())
+                    dropped = [raw[l][~keep]] + ([gates[l][~keep]] if gates[l] is not None else [])
+                    for t in dropped:
+                        assert bool((t.view(torch.int32) == 0).all()), f"mu {mu} layer {l}: a dropped element is not +0"
+            else:
+                ref, bound = fwd_oracle(acts[l - 1], W, b, False, rtol)
+                put(f"fwd{l}", excess(acts[l], ref, bound))
+            if l >= 2:
+                prev = model.linears[l - 2]
+                if prev.activation is None:
+                    ref, bound = dgrad_oracle(dzs[l], W, torch.ones_like(acts[l - 1]), rtol)
+                else:
+                    ref, bound = act_dgrad_oracle(dzs[l], W, kind, acts[l - 1], gates[l - 1], s, rtol)
+                    if kind == "relu":
+                        assert bool((dzs[l - 1][acts[l - 1] == 0] == 0).all()), (mu, l)
+                put(f"dgrad{l}", excess(dzs[l - 1], ref, bound))
+            upd_dz[l - 1].append(dzs[l])
+            upd_a[l - 1].append(acts[l - 1])
+    if p > 0:
+        assert n_dropped > 0                     # the masks removed live units: the checks above are not vacuous
+    if check_update:
+        W1 = model.arena.weights.detach().double().cpu()
+        for l, lin in enumerate(model.linears, start=1):
+            o, ld = lin.out_dims, model.arena.lds[lin.block_index]
+            off = model.arena.offsets[lin.block_index]
+            d = (W1[off:off + o * ld] - W0[off:off + o * ld].double().cpu()).view(o, ld)[:, : lin.in_dims + 1]
+            ref, bound = rows_update_oracle(torch.cat(upd_dz[l - 1]), torch.cat(upd_a[l - 1]), blocks[l - 1], lr, rtol)
+            put(f"upd{l}", excess(d, ref, bound))
+    kernel = "chain" if eng.uses_chain() else "layer-wise"
+    note_worst((kernel, kind, p > 0, precision), res, f"L={L} n_mu={n_mu} mb={mb} step={step}")
+    worst = max(res, key=res.get)
+    print(f"\n[layers] {kernel} {kind} p={p} {precision} n_mu={n_mu} mb={mb}: max err/bound {res[worst]:.3g} ({worst}); "
+          f"|z|>4: {tails[0]}, |z|>9: {tails[1]}; " + " ".join(f"{k}={v:.2g}" for k, v in res.items()))
+    bad = {k: v for k, v in res.items() if not v <= 1.0}
+    assert not bad, bad
+    return res
+
+
 # ================================================================================================== GPU side
-def _init_weights(sizes, x, n_mu, gen):
+FAR_BIASES = (12.0, -12.0, 6.0, -6.0)    # features 0..3 of every hidden layer: the tails of f and f' (|z| > 9 and > 4)
+
+
+def _init_weights(sizes, x, n_mu, gen, activation="relu", far=False):
     """He-scaled weights and non-zero biases (a zero bias would hide a kernel that drops it), with the last layer scaled
-    so that the logits of the widest micro-batch span LOGIT_SPREAD."""
+    so that the logits of the widest micro-batch span LOGIT_SPREAD through the hidden activation ``activation``.
+    ``far``: the first features of every hidden layer get FAR_BIASES."""
+    from shallowspeed_b200.ops import functional as F
+
     Ws, bs = [], []
     for i, o in zip(sizes[:-1], sizes[1:]):
         Ws.append(torch.randn(o, i, generator=gen, dtype=torch.float64) * math.sqrt(2.0 / i))
         bs.append(torch.randn(o, generator=gen, dtype=torch.float64) * 0.1)
+    if far:
+        for b in bs[:-1]:
+            n = min(len(FAR_BIASES), b.numel())
+            b[:n] = torch.tensor(FAR_BIASES[:n], dtype=torch.float64)
     a = x.double()
     for l, (W, b) in enumerate(zip(Ws, bs)):
         a = a @ W.T + b
         if l < len(Ws) - 1:
-            a = a.clamp_min(0.0)
+            a = F.activation_ref(activation, a)[0]
     spread = max(float(z.max() - z.min()) for z in a.chunk(n_mu))
     s = LOGIT_SPREAD / spread
     Ws[-1], bs[-1] = Ws[-1] * s, bs[-1] * s
@@ -146,11 +361,13 @@ def _pitched(view, rows):
     return torch.as_tensor(_Buf(), device=view.device)
 
 
-def _poison(eng, model, sizes, rows, training):
-    """NaN into every padding column the kernels must not read: act / dz of l >= 1 in [cols, ld) and the weight arena
-    in [in + 1, ld)."""
+def _poison(eng, model, sizes, rows, training, gated=False):
+    """NaN into every padding column the kernels must not read: act / dz of l >= 1 in [cols, ld), the gate of every
+    activated layer in [cols, ld) when ``gated``, and the weight arena in [in + 1, ld)."""
     for l in range(1, len(sizes)):
         bufs = [eng.act(0, l)] + ([eng.dz(0, l)] if training else [])
+        if gated and l < len(sizes) - 1:
+            bufs.append(eng.gate(0, l))
         for v in bufs:
             _pitched(v, rows)[:, sizes[l]:] = float("nan")
     for i, (o, k) in enumerate(model.arena.blocks):
@@ -161,20 +378,31 @@ def _gather(fn, n_mu):
     return torch.cat([fn(mu).double().cpu() for mu in range(n_mu)])
 
 
-def _run(sizes, mb_rows, n_mu, precision, expect_chain, inference=False, env=(), monkeypatch=None):
-    """One step at the given shape; returns {check: max err / bound} after asserting the path and non-vacuity."""
+KINDS = ["relu", "gelu", "silu", "tanh"]
+DROP_P, DROP_SEED = 0.3, 0xC0FF_EE00_1234_5678
+
+
+def _run(sizes, mb_rows, n_mu, precision, expect_chain, inference=False, env=(), monkeypatch=None, activation="relu",
+         dropout=0.0, loss="mse"):
+    """One step at the given shape; returns {check: max err / bound} after asserting the path and non-vacuity.  With a
+    smooth ``activation`` or ``dropout`` > 0, every hidden layer has features with far biases, the gate padding is
+    poisoned, and the layers are checked per element by ``check_layers``."""
     from shallowspeed_b200.parallel.engine import Trainer
     from shallowspeed_b200.pipe import InferenceSchedule
 
     for k in env:
         monkeypatch.setenv(k, "1")
+    plain = activation == "relu" and dropout == 0.0
+    gated = activation != "relu" and not inference
+    loss_kind = loss
     L, C, rows = len(sizes) - 1, sizes[-1], mb_rows * n_mu
     gen = torch.Generator().manual_seed(hash((tuple(sizes), mb_rows, n_mu)) & 0xFFFFFFFF)
     x = torch.randn(rows, sizes[0], generator=gen)
     t = torch.nn.functional.one_hot(torch.randint(0, C, (rows,), generator=gen), C).float()
-    Ws, bs = _init_weights(sizes, x, n_mu, gen)
+    Ws, bs = _init_weights(sizes, x, n_mu, gen, activation, far=not plain)
 
-    tr = Trainer(sizes, global_batch_size=rows, n_mubatches=n_mu, lr=LR, precision=precision)
+    tr = Trainer(sizes, global_batch_size=rows, n_mubatches=n_mu, lr=LR, precision=precision, loss=loss_kind,
+                 activation=activation, dropout=dropout, dropout_seed=DROP_SEED)
     model = tr.model
     for i, (W, b) in enumerate(zip(Ws, bs)):
         model.arena.weight_view(i).copy_(W)
@@ -187,8 +415,9 @@ def _run(sizes, mb_rows, n_mu, precision, expect_chain, inference=False, env=(),
     assert eng.uses_chain() == expect_chain
     if "SSB_NO_COALESCE" in env:
         assert not eng.coalesced()
-    _poison(eng, model, sizes, rows, not inference)
+    _poison(eng, model, sizes, rows, not inference, gated)
     W0 = [model.arena.block(i)[:, : k + 1].double().cpu() for i, (_, k) in enumerate(model.arena.blocks)]
+    W0_flat = model.arena.weights.detach().clone()
     xh, th = x.pin_memory(), t.pin_memory()
     if inference:
         tr.worker.step_from(sched, xh, th)
@@ -206,12 +435,31 @@ def _run(sizes, mb_rows, n_mu, precision, expect_chain, inference=False, env=(),
     for l in range(1, L):
         frac = float((act[l] > 0).double().mean())
         assert 0.05 <= frac <= 0.95, f"layer {l}: {frac:.3f} of the activations are positive"
-    # forward, every layer from the kernel's own input (act[L] holds the logits: no ReLU)
-    for l in range(1, L + 1):
-        W, b = W0[l - 1][:, :-1], W0[l - 1][:, -1]
-        ref, bound = fwd_oracle(act[l - 1], W, b, l < L, rtol)
-        res[f"fwd{l}"] = excess(act[l], ref, bound)
-    # loss head, per micro-batch (the softmax shift is the micro-batch's global max)
+    if not plain:
+        # the tails of f and f' are reached inside the kernel: every activated layer has |z| > 4 and |z| > 9
+        for l in range(1, L):
+            z = act[l - 1] @ W0[l - 1][:, :-1].T + W0[l - 1][:, -1]
+            assert bool((z.abs() > 4).any()) and bool((z.abs() > 9).any()), f"layer {l}: no pre-activation in the tails"
+    if plain:
+        # forward, every layer from the kernel's own input (act[L] holds the logits: no ReLU)
+        for l in range(1, L + 1):
+            W, b = W0[l - 1][:, :-1], W0[l - 1][:, -1]
+            ref, bound = fwd_oracle(act[l - 1], W, b, l < L, rtol)
+            res[f"fwd{l}"] = excess(act[l], ref, bound)
+    elif inference:
+        # inference applies f and neither drops nor stores gates
+        for l in range(1, L + 1):
+            W, b = W0[l - 1][:, :-1], W0[l - 1][:, -1]
+            if l < L:
+                (ref, bound), _, _ = act_fwd_oracle(activation, act[l - 1], W, b, None, 1.0, rtol)
+            else:
+                ref, bound = fwd_oracle(act[l - 1], W, b, False, rtol)
+            res[f"fwd{l}"] = excess(act[l], ref, bound)
+    # loss head, per micro-batch (MSE: the softmax shift is the micro-batch's global max)
+    if loss_kind == "mse":
+        head = head_oracle
+    else:
+        from test_gpu_cross_entropy import ce_head_oracle as head
     dz = None
     if not inference:
         dz = [None] + [_gather(lambda mu, l=l: eng.dz(mu, l), n_mu) for l in range(1, L + 1)]
@@ -220,13 +468,14 @@ def _run(sizes, mb_rows, n_mu, precision, expect_chain, inference=False, env=(),
     loss_ref = loss_bound = 0.0
     for mu in range(n_mu):
         r = slice(mu * mb_rows, (mu + 1) * mb_rows)
-        (p, bp), (g, bg), (lv, bl) = head_oracle(act[L][r], t[r], rows, HEAD_RTOL)
+        (p, bp), (g, bg), (lv, bl) = head(act[L][r], t[r], rows, HEAD_RTOL)
         res["probs"] = max(res.get("probs", 0.0), excess(probs[r], p, bp))
         if not inference:
             res["dzL"] = max(res.get("dzL", 0.0), excess(dz[L][r], g, bg))
         loss_ref, loss_bound = loss_ref + lv, loss_bound + bl
     if not inference:
         res["loss"] = abs(loss - loss_ref) / loss_bound if math.isfinite(loss) else math.inf
+    if not inference and plain:
         # dgrad chain (layer 1's dgrad is skipped on the first stage)
         for l in range(L, 1, -1):
             ref, bound = dgrad_oracle(dz[l], W0[l - 1][:, :-1], act[l - 1], rtol)
@@ -236,9 +485,19 @@ def _run(sizes, mb_rows, n_mu, precision, expect_chain, inference=False, env=(),
             W1 = model.arena.block(i)[:, : k + 1].double().cpu()
             ref, bound = update_oracle(dz[i + 1], act[i], W0[i], LR, rtol)
             res[f"upd{i + 1}"] = excess(W1 - W0[i], ref, bound)
+    elif not inference:
+        res.update(check_layers(eng, model, W0_flat, x, n_mu, mb_rows, precision, LR,
+                                lambda mu: mu * mb_rows + torch.arange(mb_rows)))
+    if gated:
+        for l in range(1, L):
+            pad = _pitched(eng.gate(0, l), rows)[:, sizes[l]:]
+            assert bool(pad.isnan().all()), f"layer {l}: a kernel wrote into the gate's padding"
     worst = max(res, key=res.get)
+    if not plain:
+        note_worst(("chain" if expect_chain else "layer-wise", activation, dropout > 0, precision), res,
+                   f"sizes={sizes} mb_rows={mb_rows} env={list(env)} inference={inference}")
     print(f"\n[chain] sizes={sizes} mb_rows={mb_rows} n_mu={n_mu} {precision} chain={expect_chain} env={list(env)} "
-          f"inference={inference}: max err/bound {res[worst]:.3g} ({worst}); "
+          f"inference={inference} {activation} p={dropout} {loss_kind}: max err/bound {res[worst]:.3g} ({worst}); "
           + " ".join(f"{k}={v:.2g}" for k, v in res.items()))
     bad = {k: v for k, v in res.items() if not v <= 1.0}
     assert not bad, bad
@@ -286,6 +545,41 @@ def test_launch_forms(sizes, mb_rows, form, monkeypatch):
 @pytest.mark.parametrize("sizes,mb_rows", [(BASE, 40), (SHAPES["straddle-c17"], 100)])
 def test_chain_inference(sizes, mb_rows):
     _run(sizes, mb_rows, 2, "fp32", expect_chain=True, inference=True)
+
+
+# ---------------------------------------------------------------- the same grid with every activation and dropout
+ACT_VARIANTS = [("relu", DROP_P)] + [(k, p) for k in KINDS[1:] for p in (0.0, DROP_P)]
+
+
+def _act_grid():
+    """(sizes, mb_rows, n_mu, precision, launch form, inference, loss) of every case run for each ACT_VARIANTS pair: the
+    micro-batch sizes in both precisions, the shapes with a hidden layer (cross-entropy in tf32), the launch forms and
+    inference."""
+    cases = [(BASE, mb, _n_mu(mb), pr, "coalesced", False, "mse") for mb in MB_GRID for pr in ("fp32", "tf32")]
+    cases += [(SHAPES[s], mb, _n_mu(mb), pr, "coalesced", False, "cross_entropy" if pr == "tf32" else "mse")
+              for s in SHAPES if len(SHAPES[s]) > 2 for mb in (24, 128) for pr in ("fp32", "tf32")]
+    cases += [(BASE, mb, 2, "fp32", form, False, "mse") for form in LAUNCH_FORMS for mb in (24, 40, 100)]
+    cases += [(BASE, 40, 2, "fp32", "coalesced", True, "mse"), (SHAPES["straddle-c17"], 100, 2, "fp32", "coalesced", True, "mse")]
+    return cases
+
+
+ACT_GRID = _act_grid()
+
+
+def _act_case_id(c):
+    sizes, mb, _, pr, form, inference, loss = c
+    name = next((k for k, v in SHAPES.items() if v == sizes), "base")
+    return f"{name}-mb{mb}-{pr}-{form}{'-inference' if inference else ''}{'-ce' if loss != 'mse' else ''}"
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", ACT_GRID, ids=[_act_case_id(c) for c in ACT_GRID])
+@pytest.mark.parametrize("activation,dropout", ACT_VARIANTS, ids=[f"{k}-{'drop' if p else 'nodrop'}" for k, p in ACT_VARIANTS])
+def test_activation_dropout_grid(activation, dropout, case, monkeypatch):
+    sizes, mb_rows, n_mu, precision, form, inference, loss = case
+    env = LAUNCH_FORMS[form]
+    _run(sizes, mb_rows, n_mu, precision, expect_chain="SSB_NO_CHAIN" not in env, inference=inference, env=env,
+         monkeypatch=monkeypatch, activation=activation, dropout=dropout, loss=loss)
 
 
 # ================================================================================================== CPU side
@@ -409,3 +703,121 @@ def test_checker_rejects_injected_faults():
     assert excess(d, d, bd) <= 1.0
     d_half, _ = update_oracle(dzu[:32], a_prev[:32], W0, LR, rtol)
     assert excess(d_half, d, bd) > 1.0
+
+
+def test_activation_grid_reaches_every_form_for_every_variant():
+    """Every (activation, dropout) pair of the grid reaches NTW 2 / 4 / 8, ragged micro-batches, the k-split cluster and
+    the one-CTA chain, per-micro-batch launches, the layer-wise fallback, inference and both losses."""
+    from shallowspeed_b200 import _C
+
+    assert {k for k, _ in ACT_VARIANTS} == set(KINDS)
+    assert {(k, p > 0) for k, p in ACT_VARIANTS} == {(k, d) for k in KINDS for d in (False, True)} - {("relu", False)}
+    seen = {"ntw": set(), "ragged": False, "ksplit": False, "one-cta": False, "forms": set(), "losses": set(),
+            "inference": False, "precisions": set()}
+    for sizes, mb, _n, pr, form, inference, loss in ACT_GRID:
+        layers = list(zip(sizes[:-1], sizes[1:]))
+        seen["forms"].add(form)
+        seen["losses"].add(loss)
+        seen["inference"] |= inference
+        seen["precisions"].add(pr)
+        if "SSB_NO_CHAIN" in LAUNCH_FORMS[form]:
+            continue
+        assert _C.chain_eligible(layers, mb, sizes[-1], True, pr == "fp32"), (sizes, mb)
+        seen["ntw"].add(_chain_geometry(mb)[1])
+        seen["ragged"] |= mb % 16 != 0
+        c = _C.chain_cluster_size(layers, True, True, True, True, False, False)
+        assert _C.chain_cluster_budget(mb, c, pr == "fp32")[0] if c > 1 else True
+        seen["one-cta"] |= c == 1
+        seen["ksplit"] |= c > 1 and -(-sizes[0] // 32) > 4              # test_gpu_chain_ksplit: > 4 k-blocks
+    assert seen["ntw"] == {2, 4, 8} and seen["ragged"] and seen["ksplit"] and seen["one-cta"]
+    assert seen["forms"] == set(LAUNCH_FORMS) and seen["losses"] == {"mse", "cross_entropy"} and seen["inference"]
+    assert seen["precisions"] == {"fp32", "tf32"}
+
+
+def _device_formulas_fp32(kind, z):
+    """ptx.cuh: act_fwd evaluated op by op in fp32 on the CPU (torch's erf / exp / tanh instead of the CUDA Math API)."""
+    z = z.float()
+    if kind == "gelu":
+        c = 0.5 * (1.0 + torch.erf(z * 0.70710678118654752))
+        return z * c, c + z * (torch.exp(-0.5 * z * z) * 0.39894228040143268)
+    if kind == "silu":
+        s = 1.0 / (1.0 + torch.exp(-z))
+        return z * s, s * (1.0 + z * (1.0 - s))
+    t = torch.tanh(z)
+    return t, 1.0 - t * t
+
+
+def test_activation_oracles_reject_injected_faults():
+    """The activated-layer oracles accept the exact result and an fp32 evaluation of the device formulas, and reject:
+    the tanh-approximate GELU, a GELU gate without its z phi(z) term, a gate without keep * s, a dgrad element without
+    the dropout scale, one mask element drawn for the wrong sample or step, a gate shifted by one row, an update without
+    its bias column.  All against the fp32 bounds; the tf32 bounds reject the same faults except where noted."""
+    from shallowspeed_b200.ops import functional as F
+
+    g = torch.Generator().manual_seed(11)
+    rows, k, n = 32, 64, 48
+    x = torch.randn(rows, k, generator=g)
+    W = torch.randn(n, k, generator=g) * math.sqrt(2.0 / k)
+    b = torch.randn(n, generator=g) * 0.1
+    b[:4] = torch.tensor(FAR_BIASES)
+    s = F.dropout_scale(DROP_P)
+    samples = 3 + torch.arange(rows) * 2 + 1                      # row_base 3, dp 2, rank 1
+    keep = F.dropout_mask(DROP_P, DROP_SEED, 5, 7, samples, n)
+    kf = keep.double()
+    for precision in ("fp32", "tf32"):
+        rtol = RTOL[precision]
+        strict = precision == "fp32"
+        for kind in KINDS[1:]:
+            (ra, ba), (rg, bg), z = act_fwd_oracle(kind, x, W, b, keep, s, rtol)
+            assert excess(ra, ra, ba) <= 1.0 and excess(rg, rg, bg) <= 1.0
+            # the device formulas in fp32 from an fp32 z: accepted
+            a32, g32 = _device_formulas_fp32(kind, (x @ W.T + b))
+            keep32 = keep.float()
+            assert excess(a32 * s * keep32, ra, ba) <= 1.0 and excess(g32 * s * keep32, rg, bg) <= 1.0
+            # gate without keep * s: rejected in both precisions
+            assert excess(g32.double(), rg, bg) > 1.0
+            # one mask element from the wrong sample (row_base off by one) or the wrong step
+            for wrong in (F.dropout_mask(DROP_P, DROP_SEED, 5, 7, samples + 2, n),
+                          F.dropout_mask(DROP_P, DROP_SEED, 5, 8, samples, n)):
+                i, j = ((wrong != keep) & (a32.abs() > 0.1)).nonzero()[0].tolist()
+                bad = a32 * s * keep32
+                bad[i, j] = (a32[i, j] * s) if wrong[i, j] else 0.0
+                assert excess(bad, ra, ba) > 1.0, (kind, precision)
+            # a gate shifted by one row
+            assert excess(torch.roll(g32 * s * keep32, 1, dims=0), rg, bg) > 1.0
+        # GELU: the tanh approximation, and the gate without z phi(z)
+        (ra, ba), (rg, bg), z = act_fwd_oracle("gelu", x, W, b, None, 1.0, rtol)
+        z32 = (x @ W.T + b)
+        approx = torch.nn.functional.gelu(z32.double(), approximate="tanh")
+        if strict:                                                     # tf32's bound is wider than its 5e-4 difference
+            assert excess(approx, ra, ba) > 1.0
+        Phi = 0.5 * torch.special.erfc(-z / _SQRT2)
+        assert excess(Phi, rg, bg) > 1.0
+
+    rtol = RTOL["fp32"]
+    # dgrad through ReLU + dropout: the scale missing on one kept element
+    dz = torch.randn(rows, n, generator=g) * 1e-2
+    W2 = torch.randn(n, k, generator=g) / math.sqrt(n)
+    act_prev = torch.where(torch.rand(rows, k, generator=g) < 0.7, torch.rand(rows, k, generator=g), torch.zeros(()))
+    ref, bound = act_dgrad_oracle(dz, W2, "relu", act_prev, None, s, rtol)
+    got = ((dz @ W2) * (act_prev > 0) * s).double()
+    assert excess(got, ref, bound) <= 1.0
+    i, j = (act_prev > 0).nonzero()[0].tolist()
+    got[i, j] /= s
+    assert excess(got, ref, bound) > 1.0
+    # dgrad through a gate: the gate shifted by one row
+    gam = torch.rand(rows, k, generator=g) * s * (act_prev > 0)
+    ref, bound = act_dgrad_oracle(dz, W2, "gelu", None, gam, s, rtol)
+    assert excess((dz @ W2) * gam, ref, bound) <= 1.0
+    assert excess((dz.double() @ W2.double()) * torch.roll(gam, 1, dims=0).double(), ref, bound) > 1.0
+
+    # the update without its bias column (1024 rows: the bias bound carries its per-row roundings)
+    dzu = torch.randn(1024, n, generator=g) * 1e-3
+    au = torch.randn(1024, k, generator=g).clamp_min(0.0)
+    W0 = torch.cat([W, b[:, None]], 1)
+    for precision in ("fp32", "tf32"):
+        d, bd = rows_update_oracle(dzu, au, W0, LR, RTOL[precision])
+        assert excess(d, d, bd) <= 1.0
+        nob = d.clone()
+        nob[:, -1] = 0.0
+        assert excess(nob, d, bd) > 1.0

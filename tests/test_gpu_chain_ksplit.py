@@ -129,7 +129,8 @@ def test_ksplit_cross_entropy_matches_the_fp64_oracle(k, mb_rows, precision):
 @pytest.mark.parametrize("k,gbs,n_mu", [(160, 128, 4), (200, 80, 2)])
 def test_ksplit_dropout_matches_fp64(k, gbs, n_mu, precision, loss):
     from shallowspeed_b200.parallel.engine import Trainer
-    from test_gpu_dropout import P, SEED, _batch, check_layers
+    from test_gpu_chain import check_layers
+    from test_gpu_dropout import P, SEED, _batch
 
     sizes = _sizes(k)
     lr = 0.05

@@ -1,7 +1,8 @@
 """Dropout on one GPU.  The masks come from ops.functional.dropout_mask (the torch Philox), the numbers from fp64:
 
-* per layer, from the kernels' own buffers after one Trainer step: where the mask drops, act[l] is exactly 0; where it
-  keeps, act[l] matches relu(z) * s; every dgrad matches (dz @ W) * (a > 0) * s; the update matches act and dz.  The
+* per layer and per element, from the kernels' own buffers after one Trainer step (test_gpu_chain: check_layers): where
+  the mask drops, act[l] is +0 bitwise; where it keeps, act[l] matches relu(z) * s; every dgrad matches
+  (dz @ W) * (a > 0) * s; the update matches act and dz.  The
   chain kernel (cluster and one-CTA launches, MSE and cross-entropy, fp32 and tf32), the layer-wise GEMMs (a 129-wide
   layer, 33 classes, 256-row micro-batches) and a wide model whose forward runs split-K;
 * several engine steps against the Python VM on the CPU;
@@ -11,12 +12,13 @@
 import pytest
 import torch
 
+from test_gpu_chain import check_layers, worst_table  # noqa: F401  (the table of worst err / bound)
+
 pytestmark = pytest.mark.gpu
 
 SIZES = [784, 128, 127, 126, 125, 124, 123, 10]
 P, SEED = 0.3, 0xDEAD_BEEF_1234_5678
-ACT_TOL = {"fp32": 1e-5, "tf32": 5e-3}     # relative Frobenius error of one layer against fp64, from its own inputs
-UPD_TOL = 2e-2                              # as tests/test_gpu_lr_schedule.py
+UPD_TOL = 2e-2                              # whole trajectories against the Python VM (as tests/test_gpu_lr_schedule.py)
 
 
 def _frob(a, b):
@@ -29,50 +31,6 @@ def _batch(rows, in_dim, classes, seed=0):
     y = torch.zeros(rows, classes)
     y[torch.arange(rows), torch.randint(0, classes, (rows,), generator=g)] = 1.0
     return x.pin_memory(), y.pin_memory()
-
-
-def check_layers(eng, model, W0, x, n_mu, mb, precision, lr, samples_of, step=0, check_update=True):
-    """Every layer of the step that just ran, per micro-batch, from the engine's own buffers against fp64.
-    ``samples_of(mu)``: the global sample index of every row of micro-batch mu; ``x``: the stage input of the step."""
-    from shallowspeed_b200.ops import functional as F
-
-    s = F.dropout_scale(P)
-    L, tol = len(model.linears), ACT_TOL[precision]
-    upd = [torch.zeros(lin.out_dims, lin.in_dims + 1, dtype=torch.float64) for lin in model.linears]
-    n_dropped = 0
-    for mu in range(n_mu):
-        samples = samples_of(mu)
-        # act[0] of the engine is the staging set of the NEXT step; the step's input is x itself
-        acts = [x[mu * mb:(mu + 1) * mb].double()] + [eng.act(mu, l).double().cpu() for l in range(1, L + 1)]
-        dzs = [eng.dz(mu, l).double().cpu() for l in range(L + 1)]
-        for l, lin in enumerate(model.linears, start=1):
-            blk = W0[model.arena.offsets[lin.block_index]:][: lin.out_dims * model.arena.lds[lin.block_index]]
-            blk = blk.view(lin.out_dims, -1).double().cpu()
-            W, b = blk[:, : lin.in_dims], blk[:, lin.in_dims]
-            z = acts[l - 1] @ W.T + b
-            if lin.activation is not None:
-                keep = F.dropout_mask(P, SEED, lin.dropout[2], step, samples, lin.out_dims)
-                assert torch.all(acts[l][~keep] == 0), (mu, l)
-                n_dropped += int((~keep & (z > 0)).sum())
-                want = torch.where(keep, z.clamp_min(0) * s, torch.zeros_like(z))
-                assert _frob(acts[l], want) < tol, (mu, l, _frob(acts[l], want))
-            if l >= 2:
-                g = dzs[l] @ W
-                if model.linears[l - 2].activation is not None:
-                    g = g * (acts[l - 1] > 0) * s
-                    assert torch.all(dzs[l - 1][acts[l - 1] == 0] == 0), (mu, l)
-                assert _frob(dzs[l - 1], g) < tol, (mu, l, _frob(dzs[l - 1], g))
-            upd[l - 1][:, : lin.in_dims] += dzs[l].T @ acts[l - 1]
-            upd[l - 1][:, lin.in_dims] += dzs[l].sum(0)
-    assert n_dropped > 0                       # the masks removed active units: the check above is not vacuous
-    if not check_update:
-        return
-    W1 = model.arena.weights.detach().double().cpu()
-    for lin, u in zip(model.linears, upd):
-        o, ld = lin.out_dims, model.arena.lds[lin.block_index]
-        off = model.arena.offsets[lin.block_index]
-        d = (W1[off:off + o * ld] - W0[off:off + o * ld].double().cpu()).view(o, ld)[:, : lin.in_dims + 1]
-        assert _frob(d, -lr * u) < UPD_TOL, lin
 
 
 NO_COALESCE = {"SSB_NO_COALESCE": "1"}

@@ -25,8 +25,9 @@ import zlib
 import pytest
 import torch
 
-from test_gpu_chain import (ATOL, FP32_ULP, HEAD_RTOL, LR, RTOL, _gather, _init_weights, _n_mu, _poison,
-                            _selftest_data, dgrad_oracle, excess, fwd_oracle, head_oracle, update_oracle)
+from test_gpu_chain import (ATOL, FAR_BIASES, FP32_ULP, HEAD_RTOL, LR, RTOL, _gather, _init_weights, _n_mu, _poison,
+                            _selftest_data, act_dgrad_oracle, act_fwd_oracle, dgrad_oracle, excess, fwd_oracle,
+                            head_oracle, update_oracle)
 
 U = 2.0**-24                  # unit roundoff of fp32
 SENTINEL = -1234.5            # output padding: finite and non-zero, so x + (-0.0) keeps its bits
@@ -205,6 +206,141 @@ def test_dgrad_per_element(rows, m, k, precision):
     _note(("dgrad", precision), res, f"rows={rows} m={m} k={k}")
 
 
+# ---------------------------------------------------------------- the activated and dropout variants
+# every forward variant gemm_configure registers: ReLU + dropout (tc_gemm_drop_kernel) and each smooth kind with and
+# without dropout (tc_gemm_gate_kernel); the launch's rows are samples (row_base + n) * dp + rank of the masks
+FWD_VARIANTS = [("relu", True)] + [(k, d) for k in ("gelu", "silu", "tanh") for d in (False, True)]
+DROP = (0.3, 0x1234_5678_9ABC_DEF0, 6, 9, 5, 3, 2)            # p, seed, layer, step, row_base, dp, rank
+
+
+def _variant(kind, drop):
+    return f"{kind}{'+drop' if drop else ''}"
+
+
+def _keep(rows, m):
+    from shallowspeed_b200.ops import functional as F
+
+    p, seed, layer, step, row_base, dp, rank = DROP
+    return F.dropout_mask(p, seed, layer, step, (row_base + torch.arange(rows)) * dp + rank, m), F.dropout_scale(p)
+
+
+def _fwd_inputs(tag, rows, m, k):
+    """x, the arena block's W and bias (features 0..3 with FAR_BIASES: the tails of f and f')."""
+    gen = _gen(tag, rows, m, k)
+    _, x = _pitched(rows, k, gen)
+    wbuf, _ = _pitched(m, k + 1, gen, scale=1.0 / math.sqrt(k))
+    bias = torch.randn(m, generator=gen) * 0.5
+    bias[: min(4, m)] = torch.tensor(FAR_BIASES[: min(4, m)])
+    wbuf[:, k] = bias.cuda()
+    return x, wbuf[:, :k], wbuf[:, k]
+
+
+def _check_fwd_variant(kind, drop, y, ybuf, gbuf, x, W, b, rtol, res, tag):
+    """act and gate of one activated forward launch against act_fwd_oracle; dropped elements +0 bitwise; the padding of
+    y and of the gate buffer keeps its sentinel."""
+    rows, m = y.shape
+    keep, s = _keep(rows, m) if drop else (None, 1.0)
+    (ra, ba), gam, _ = act_fwd_oracle(kind, x.cpu(), W.cpu(), b.cpu(), keep, s, rtol)
+    res[tag + "-act"] = excess(y, ra, ba)
+    got = [y.cpu()]
+    if gam is not None:
+        res[tag + "-gate"] = excess(gbuf[:, :m], *gam)
+        got.append(gbuf[:, :m].cpu())
+    if keep is not None:
+        for t in got:
+            assert bool((t[~keep].view(torch.int32) == 0).all()), f"{tag}: a dropped element is not +0"
+    assert bool((ybuf[:, m:] == SENTINEL).all()), f"{tag}: FWD wrote into the output's padding"
+    assert bool((gbuf[:, m:] == SENTINEL).all()), f"{tag}: FWD wrote into the gate's padding"
+    if gam is None:
+        assert bool((gbuf == SENTINEL).all()), f"{tag}: a ReLU launch wrote a gate"
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("precision", ["fp32", "tf32"])
+@pytest.mark.parametrize("rows,m,k", GRID)
+def test_fwd_activation_and_dropout_per_element(rows, m, k, precision):
+    K = _K()
+    x, W, b = _fwd_inputs("fwd-act", rows, m, k)
+    rtol = rtol_for(precision, k)
+    for kind, drop in FWD_VARIANTS:
+        res = {}
+        ybuf, y = _out(rows, m)
+        gbuf, gate = _out(rows, m)
+        K.linear_fwd(x, W, b, relu=True, out=y, precision=precision, activation=kind,
+                     gate=gate if kind != "relu" else None, dropout=DROP if drop else None)
+        torch.cuda.synchronize()
+        _check_fwd_variant(kind, drop, y, ybuf, gbuf, x, W, b, rtol, res, _variant(kind, drop))
+        _note((f"fwd-{_variant(kind, drop)}", precision), res, f"rows={rows} m={m} k={k}")
+
+
+def _gate_values(rows, cols, gen):
+    """A gate: any sign (GELU and SiLU have negative derivatives), exact zeros where dropout dropped."""
+    g = torch.randn(rows, cols, generator=gen) * 0.7
+    g.view(-1)[0::7] = 0.0
+    return g
+
+
+def _dgrad_inputs(tag, rows, m, k):
+    gen = _gen(tag, rows, m, k)
+    _, dz = _pitched(rows, k, gen)
+    _, W = _pitched(k, m, gen, scale=1.0 / math.sqrt(k))
+    masks = []
+    for fill in (_mask_values, _gate_values):
+        mbuf = torch.full((rows, _ld(m, 8)), NAN)                  # a pitch unlike dX's
+        mbuf[:, :m] = fill(rows, m, gen)
+        masks.append(mbuf.cuda()[:, :m])
+    return dz, W, masks
+
+
+def _dgrad_variant(K, dz, W, mask, gate, variant, y, precision, k_splits=0):
+    if variant == "relu+drop":
+        K.linear_dgrad(dz, W, mask=mask, out=y, precision=precision, k_splits=k_splits, dropout=DROP)
+    else:
+        K.linear_dgrad(dz, W, mask=gate, out=y, precision=precision, k_splits=k_splits, activation="gelu")
+
+
+def _dgrad_variant_oracle(variant, dz, W, mask, gate, rtol):
+    if variant == "relu+drop":
+        return act_dgrad_oracle(dz.cpu(), W.cpu(), "relu", mask.cpu(), None, _keep(1, 1)[1], rtol)
+    return act_dgrad_oracle(dz.cpu(), W.cpu(), "gelu", None, gate.cpu(), 1.0, rtol)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("precision", ["fp32", "tf32"])
+@pytest.mark.parametrize("rows,m,k", GRID)
+def test_dgrad_gate_and_dropout_per_element(rows, m, k, precision):
+    """DGRAD through ReLU + dropout (the stored output as the mask, times s where it passes, exactly 0 elsewhere) and
+    through a gate (times the gate), each mask with a pitch of its own and NaN in its padding."""
+    K = _K()
+    dz, W, (mask, gate) = _dgrad_inputs("dgrad-act", rows, m, k)
+    rtol = rtol_for(precision, k)
+    for variant in ("relu+drop", "gate"):
+        dxbuf, dx = _out(rows, m)
+        _dgrad_variant(K, dz, W, mask, gate, variant, dx, precision)
+        torch.cuda.synchronize()
+        ref, bound = _dgrad_variant_oracle(variant, dz, W, mask, gate, rtol)
+        if variant == "relu+drop":
+            assert bool((dx.cpu()[mask.cpu() <= 0] == 0).all()), "a masked element is not 0"
+        assert bool((dxbuf[:, m:] == SENTINEL).all()), "DGRAD wrote into the output's padding"
+        _note((f"dgrad-{variant}", precision), {variant: excess(dx, ref, bound)}, f"rows={rows} m={m} k={k}")
+
+
+@pytest.mark.gpu
+def test_linear_fwd_refuses_a_gate_with_another_pitch():
+    """The gated epilogue writes the gate with y's row pitch: a gate of another pitch is refused before any launch."""
+    K = _K()
+    x, W, b = _fwd_inputs("refuse-gate", 16, 40, 33)
+    ybuf, y = _out(16, 40)
+    gbuf, gate = _out(16, 40, extra=8)
+    assert gate.stride(0) != y.stride(0)
+    with pytest.raises(RuntimeError, match="row pitch"):
+        K.linear_fwd(x, W, b, relu=True, out=y, activation="gelu", gate=gate)
+    with pytest.raises(RuntimeError, match="relu"):
+        K.linear_fwd(x, W, b, relu=False, out=y, dropout=DROP)
+    torch.cuda.synchronize()
+    assert bool((ybuf == SENTINEL).all()) and bool((gbuf == SENTINEL).all())
+
+
 # ================================================================================================== split-K
 # (rows, M, K, forced split counts that leave no split empty).  Every shape has >= 2 M tiles and >= 2 N tiles.
 SPLITK_CASES = [
@@ -257,6 +393,46 @@ def test_splitk_per_element_and_deterministic(rows, m, k, forced, mode, precisio
         res[f"ks{ks if ks >= 0 else 'auto'}"] = excess(outs[0].view(torch.float32), ref, bound)
         assert torch.equal(outs[0], outs[1]) and torch.equal(outs[0], outs[2]), f"k_splits={ks} is not deterministic"
     _note((f"splitk-{mode}", precision), res, f"rows={rows} m={m} k={k} planner={planner}")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("precision", ["fp32", "tf32"])
+@pytest.mark.parametrize("mode", ["fwd", "dgrad"])
+@pytest.mark.parametrize("rows,m,k,forced", SPLITK_CASES, ids=[f"rows{c[0]}-m{c[1]}-k{c[2]}" for c in SPLITK_CASES])
+def test_splitk_activation_and_dropout_per_element(rows, m, k, forced, mode, precision):
+    """The split-K instantiations of the activated and dropout variants (FWD: every FWD_VARIANTS entry; DGRAD: ReLU +
+    dropout and the gate) at the first forced split count and the planner's, per element, and two launches bit-identical."""
+    K = _K()
+    res = {}
+    for ks in (forced[0], -1):
+        if mode == "fwd":
+            x, W, b = _fwd_inputs("splitk-act", rows, m, k)
+            for kind, drop in FWD_VARIANTS:
+                outs = []
+                for _ in range(2):
+                    ybuf, y = _out(rows, m)
+                    gbuf, gate = _out(rows, m)
+                    K.linear_fwd(x, W, b, relu=True, out=y, precision=precision, k_splits=ks, activation=kind,
+                                 gate=gate if kind != "relu" else None, dropout=DROP if drop else None)
+                    torch.cuda.synchronize()
+                    outs.append((_bits(ybuf), _bits(gbuf)))
+                tag = f"ks{ks if ks >= 0 else 'auto'}-{_variant(kind, drop)}"
+                _check_fwd_variant(kind, drop, y, ybuf, gbuf, x, W, b, rtol_for(precision, k, 8), res, tag)
+                assert all(torch.equal(u, v) for u, v in zip(*outs)), f"{tag} is not deterministic"
+        else:
+            dz, W, (mask, gate) = _dgrad_inputs("splitk-act", rows, m, k)
+            for variant in ("relu+drop", "gate"):
+                outs = []
+                for _ in range(2):
+                    dxbuf, dx = _out(rows, m)
+                    _dgrad_variant(K, dz, W, mask, gate, variant, dx, precision, k_splits=ks)
+                    torch.cuda.synchronize()
+                    outs.append(_bits(dxbuf))
+                tag = f"ks{ks if ks >= 0 else 'auto'}-{variant}"
+                res[tag] = excess(dx, *_dgrad_variant_oracle(variant, dz, W, mask, gate, rtol_for(precision, k, 8)))
+                assert torch.equal(outs[0], outs[1]), f"{tag} is not deterministic"
+                assert bool((dxbuf[:, m:] == SENTINEL).all()), f"{tag} wrote into the output's padding"
+    _note((f"splitk-{mode}-act", precision), res, f"rows={rows} m={m} k={k}")
 
 
 # ================================================================================================== WGRAD

@@ -62,8 +62,6 @@ PipeEngine::PipeEngine(const EngineConfig& cfg, float* weights, float* grads, in
     layer_proto_.assign(L_, (cfg_.training && cfg_.dp_mode == 3 && cfg_.dp_size > 1) ? DP_PROTO_NVLS : DP_PROTO_ALL);
     n_mu_streams_ = std::max(1, std::min(cfg_.n_mu, 8));   // one stream per micro-batch in flight (GPipe with 8 micro-batches: all 8)
     n_w_streams_ = std::max(1, std::min(L_, 8));        // one stream per layer's wgrad when possible
-    if (const char* e = getenv("SSB_MU_STREAMS")) n_mu_streams_ = std::max(1, std::min(atoi(e), std::max(1, cfg_.n_mu)));
-    if (const char* e = getenv("SSB_W_STREAMS")) n_w_streams_ = std::max(1, atoi(e));
     const int n_streams = 1 + n_mu_streams_ + n_w_streams_ + 2;
     s_comm_ = 1 + n_mu_streams_ + n_w_streams_;
     s_dp_ = s_comm_ + 1;
@@ -131,12 +129,10 @@ void PipeEngine::alloc_buffers() {
         step_dev_ = reinterpret_cast<uint32_t*>(dalloc(2));   // zeroed: step 0
         step_ = step_written_[0] = step_written_[1] = 0u;
     }
-    loss_dev_ = dalloc(std::max(M, 16));
-    CUDA_CHECK(cudaMallocHost(&loss_host_, 2 * sizeof(float) * std::max(M, 16)));   // one slot per staging set
-    // opt-in (SSB_LOSS_ZEROCOPY=1, awaiting hardware validation): the loss head stores its per-micro-batch losses straight
-    // into this pinned, device-mapped host buffer (16 bytes over PCIe), which drops the D2H copy node from the step
-    loss_zero_copy_ = getenv("SSB_LOSS_ZEROCOPY") != nullptr && atoi(getenv("SSB_LOSS_ZEROCOPY")) > 0;
-    for (int i = 0; i < 2 * std::max(M, 16); ++i) loss_host_[i] = 0.f;
+    // the loss head stores its per-micro-batch losses straight into this pinned, device-mapped host buffer (16 bytes over
+    // PCIe): no D2H copy node in the step
+    CUDA_CHECK(cudaMallocHost(&loss_host_, 2 * sizeof(float) * loss_stride()));   // one slot per staging set
+    for (int i = 0; i < 2 * loss_stride(); ++i) loss_host_[i] = 0.f;
     {
         int* p = nullptr;
         CUDA_CHECK(cudaMalloc(&p, 64));
@@ -213,20 +209,21 @@ void PipeEngine::select_set(int set) {
     for (int mu = 0; mu < cfg_.n_mu; ++mu) act_[mu][0] = act_all_[0] + (size_t)mu * cfg_.mb_rows * act_ld_[0];
 }
 
-// SSB_SPLITK=1 (the default, tuning.json): automatic; SSB_SPLITK=k: force k where legal; SSB_SPLITK=0: off.  Gives
+// Automatic by default (gemm_splitk_choice); SSB_SPLITK=k forces k splits where legal, SSB_SPLITK=0 turns it off.  Gives
 // FWD / DGRAD GEMMs of wide layers enough CTAs to saturate HBM (8192 outputs = only 64 tiles on 132 SMs).  Each plan
 // owns its workspace and tile counters; the last CTA of a tile re-arms its counter, so every replay of the graph
 // reuses them.  tests/test_gpu_gemm.py checks the variant per element against an fp64 oracle, stand-alone and in the
 // engine over two steps.
 void PipeEngine::maybe_splitk(GemmPlan& g) {
     const char* env = getenv("SSB_SPLITK");
-    if (!env || atoi(env) <= 0 || g.mode == GEMM_WGRAD) return;
+    const int want = env ? atoi(env) : 1;
+    if (want <= 0 || g.mode == GEMM_WGRAD) return;
     int dev = 0, sms = 132;
     CUDA_CHECK(cudaGetDevice(&dev));
     CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     int splits = gemm_splitk_choice(g, sms);
-    if (atoi(env) > 1) {
-        const int num_kb = (g.p.k_total + 31) / 32, want = atoi(env);
+    if (want > 1) {
+        const int num_kb = (g.p.k_total + 31) / 32;
         const int per = (num_kb + want - 1) / want;
         if (per >= 1 && (num_kb + per - 1) / per == want) splits = want;
     }
@@ -243,11 +240,6 @@ void PipeEngine::maybe_splitk(GemmPlan& g) {
     if (const char* err = gemm_plan_enable_splitk(&g, splits, ws, counters))
         throw std::runtime_error(std::string("PipeEngine split-K: ") + err);
     ++splitk_gemms_;
-}
-
-// where the loss values of the plan being built go: device scratch (then a D2H copy), or directly the host slot
-float* PipeEngine::loss_target() const {
-    return loss_zero_copy_ ? loss_host_ + cur_set_ * std::max(cfg_.n_mu, 16) : loss_dev_;
 }
 
 int PipeEngine::new_event() {
@@ -286,7 +278,7 @@ int PipeEngine::add_chain(int stream, int mu_base, int n_mu, bool do_fwd, bool d
     }
     cp.target = y_stage_; cp.ldt = y_ld_;
     cp.probs = probs_all_; cp.ldp = act_ld_[L_];
-    cp.loss = loss_target();
+    cp.loss = loss_slot(cur_set_);
     cp.loss_kind = cfg_.loss;
     cp.act_kind = cfg_.activation;
     if (gated())
@@ -658,7 +650,6 @@ void PipeEngine::plan_per_mubatch() {
                         lh.c = probs_[mu]; lh.ldc = act_ld_[L_];
                         lh.d = dz_[mu][L_]; lh.ldd = act_ld_[L_];
                         lh.rows = mb; lh.cols = cfg_.out_dim; lh.scalar = 1.0f / (float)cfg_.global_batch; lh.mu = mu;
-                        lh.f = loss_zero_copy_ ? loss_target() : nullptr;
                         ops_.push_back(lh);
                     } else if (L_ > 0 && cfg_.layers[L_ - 1].relu) {
                         Op rm;
@@ -805,11 +796,6 @@ void PipeEngine::plan_per_mubatch() {
         cr.b = cfg_.training ? reinterpret_cast<float*>(pp_ctx_->next_dz_credit()) : nullptr;
         ops_.push_back(cr);
     }
-    if (cfg_.training && last && !loss_zero_copy_) {
-        Op cp;
-        cp.kind = OP_MEMCPY_LOSS; cp.stream = 0; cp.a = loss_host_ + cur_set_ * std::max(cfg_.n_mu, 16);
-        ops_.push_back(cp);
-    }
 }
 
 // Stage without pipeline communication (pp == 1): micro-batches are independent until the
@@ -847,7 +833,6 @@ void PipeEngine::build_coalesced() {
     // globally visible; the tiles of layer l wait for ready[l] before their first TMA load and for ready[l-1] (the dgrad
     // that reads W_l retired) before they update W_l in place.  Only layer 1's tiles remain behind the chain kernel.
     // (The same gate in front of the single-GPU grouped wgrad launch was measured neutral - 79.7 vs 78.7 us - and removed.)
-    const bool group_env = getenv("SSB_WGRAD_GROUP") != nullptr && atoi(getenv("SSB_WGRAD_GROUP")) > 0;
     auto env_on = [](const char* name, bool dflt) { const char* v = getenv(name); return v ? atoi(v) > 0 : dflt; };
     // fused DP over narrow layers: the LL two-shot kernel (dp_ll.cu), all layers in one launch, gated the same way
     const bool ll_on = chain && cfg_.training && cfg_.dp_mode == 2 && dp_ctx_ != nullptr && dp_ctx_->ll_enabled();
@@ -895,15 +880,14 @@ void PipeEngine::build_coalesced() {
         lh.a = act_all_[L_]; lh.lda = act_ld_[L_]; lh.b = y_stage_; lh.ldb = y_ld_; lh.c = probs_all_; lh.ldc = act_ld_[L_];
         lh.d = dz_all_[L_]; lh.ldd = act_ld_[L_]; lh.rows = rows; lh.cols = cfg_.out_dim;
         lh.scalar = 1.0f / (float)cfg_.global_batch; lh.mu = 0; lh.n = mb;
-        lh.f = loss_zero_copy_ ? loss_target() : nullptr;
         ops_.push_back(lh);
     }
     const bool fuse = (cfg_.dp_mode == 0);
     const bool fused_dp = (cfg_.dp_mode == 2);
-    // opt-in (SSB_WGRAD_GROUP=1): all layers' weight-gradient tiles in ONE launch on the main stream right behind the
-    // chain kernel (which has produced every dZ and is the last reader of every W) - no fork / join per layer
-    // (also with the NVLS path, whose single reduce+SGD kernel follows the whole wgrad wave anyway)
-    const bool group_wgrad = (fuse || cfg_.dp_mode == 3) && chain && group_env;
+    // chain stages: all layers' weight-gradient tiles in ONE launch on the main stream right behind the chain kernel
+    // (which has produced every dZ and is the last reader of every W) - no fork / join per layer (also with the NVLS
+    // path, whose single reduce+SGD kernel follows the whole wgrad wave anyway)
+    const bool group_wgrad = chain && (fuse || cfg_.dp_mode == 3);
     std::vector<GemmPlan> grouped;
     std::vector<DpLLLayer> ll_layers;
     int ev_bump = -1;
@@ -1051,11 +1035,6 @@ void PipeEngine::build_coalesced() {
     }
     for (size_t s = 1; s < streams_.size(); ++s)
         if (started[s]) { const int e = emit_record((int)s); emit_wait(0, e); }
-    if (!loss_zero_copy_) {
-        Op cp;
-        cp.kind = OP_MEMCPY_LOSS; cp.stream = 0; cp.a = loss_host_ + cur_set_ * std::max(cfg_.n_mu, 16);
-        ops_.push_back(cp);
-    }
 }
 
 void PipeEngine::finish_build() {
@@ -1095,7 +1074,7 @@ cudaStream_t PipeEngine::stream_of(const Op& op) const {
     return streams_[serialize ? 0 : op.stream];
 }
 
-void PipeEngine::exec(const Op& op) {
+void PipeEngine::exec(const Op& op, int set) {
     cudaStream_t st = stream_of(op);
     switch (op.kind) {
         case OP_WAIT: CUDA_CHECK(cudaStreamWaitEvent(st, events_[op.event], 0)); break;
@@ -1103,7 +1082,7 @@ void PipeEngine::exec(const Op& op) {
         case OP_GEMM: CUDA_CHECK(gemm_launch(gemms_[op.gemm], st)); break;
         case OP_WGRAD_GROUP: CUDA_CHECK(gemm_group_launch(group_plans_[op.gemm], st)); break;
         case OP_LOSS_HEAD:
-            CUDA_CHECK(launch_loss_head(op.a, op.lda, op.b, op.ldb, op.c, op.ldc, op.d, op.ldd, (op.f ? op.f : loss_dev_) + op.mu, op.rows,
+            CUDA_CHECK(launch_loss_head(op.a, op.lda, op.b, op.ldb, op.c, op.ldc, op.d, op.ldd, loss_slot(set) + op.mu, op.rows,
                                         op.cols, op.scalar, st, (int)op.n, cfg_.loss));
             break;
         case OP_SOFTMAX:
@@ -1166,9 +1145,6 @@ void PipeEngine::exec(const Op& op) {
         case OP_PP_CREDIT:
             CUDA_CHECK(launch_pp_credit(reinterpret_cast<uint32_t*>(op.a), reinterpret_cast<uint32_t*>(op.b), pp_ctx_->epoch_ptr(), st));
             break;
-        case OP_MEMCPY_LOSS:
-            CUDA_CHECK(cudaMemcpyAsync(op.a, loss_dev_, sizeof(float) * cfg_.n_mu, cudaMemcpyDeviceToHost, st));
-            break;
         default: throw std::runtime_error("PipeEngine: bad op");
     }
 }
@@ -1194,7 +1170,6 @@ static const char* op_name(int kind) {
         case OP_PP_WAIT: return "pp_wait";
         case OP_PP_CREDIT: return "pp_credit";
         case OP_CHAIN: return "mlp_chain";
-        case OP_MEMCPY_LOSS: return "loss_d2h";
         case OP_ARGMAX: return "argmax_correct";
         case OP_WAIT: return "wait_event";
         case OP_RECORD: return "record_event";
@@ -1245,7 +1220,7 @@ void PipeEngine::walk(int set) {
             a = tev();
             CUDA_CHECK(cudaEventRecord(a, stream_of(op)));
         }
-        exec(op);
+        exec(op, set);
         if (bracket) {
             b = tev();
             CUDA_CHECK(cudaEventRecord(b, stream_of(op)));
@@ -1366,7 +1341,7 @@ std::string PipeEngine::comm_status() const {
 
 float PipeEngine::last_loss() {
     synchronize();
-    const float* h = loss_host_ + run_set_ * std::max(cfg_.n_mu, 16);
+    const float* h = loss_slot(run_set_);
     float s = 0.f;
     for (int i = 0; i < cfg_.n_mu; ++i) s += h[i];
     return s;
@@ -1377,7 +1352,7 @@ float PipeEngine::last_loss() {
 float PipeEngine::prev_loss() {
     const int set = run_set_ ^ 1;
     CUDA_CHECK(cudaEventSynchronize(ev_done_[set]));
-    const float* h = loss_host_ + set * std::max(cfg_.n_mu, 16);
+    const float* h = loss_slot(set);
     float s = 0.f;
     for (int i = 0; i < cfg_.n_mu; ++i) s += h[i];
     return s;

@@ -11,9 +11,14 @@
 //     stream; wgrad GEMMs run on side streams in a fixed accumulation order (bitwise
 //     deterministic); the graph exposes all of that parallelism to the hardware;
 //   * ZeroGrad is free (first wgrad of a layer overwrites), OptimizerStep is fused into the
-//     last wgrad of each layer (single replica) or into the in-kernel DP reduction;
-//   * pipeline p2p uses NCCL send/recv on a dedicated stream, grouped exactly like the
-//     schedule validator's rendezvous model.
+//     weight-gradient epilogue (single replica: one grouped launch of every layer's tiles
+//     behind the chain kernel, else the last wgrad of each layer) or into the in-kernel DP
+//     reduction;
+//   * the loss head stores the per-micro-batch losses straight into pinned, device-mapped
+//     host memory: no read-back copy;
+//   * pipeline boundaries are one-sided pushes into the neighbour's memory with epoch flags
+//     (PpContext); NCCL send/recv on a dedicated stream, grouped exactly like the schedule
+//     validator's rendezvous model, is the alternative transport.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -44,7 +49,7 @@ struct LayerSpec {
 
 enum OpKind : int {
     OP_GEMM = 0, OP_LOSS_HEAD, OP_SOFTMAX, OP_RELU_MASK, OP_SGD, OP_COMM_GROUP, OP_ALLREDUCE, OP_FUSED_DP,
-    OP_WAIT, OP_RECORD, OP_MEMCPY_LOSS, OP_ARGMAX, OP_DP_REDUCE, OP_BUMP_EPOCH, OP_CHAIN, OP_NVLS_SGD,
+    OP_WAIT, OP_RECORD, OP_ARGMAX, OP_DP_REDUCE, OP_BUMP_EPOCH, OP_CHAIN, OP_NVLS_SGD,
     OP_PP_PUSH, OP_PP_WAIT, OP_PP_CREDIT, OP_PP_BUMP, OP_WGRAD_GROUP, OP_BUMP_STEP, OP_DP_LL
 };
 
@@ -64,7 +69,6 @@ struct Op {
     std::vector<CommItem> comm;
     // generic pointers for the small kernels
     float *a = nullptr, *b = nullptr, *c = nullptr, *d = nullptr;
-    float* f = nullptr;        // loss head: where the loss values go when not the default device scratch
     int lda = 0, ldb = 0, ldc = 0, ldd = 0, rows = 0, cols = 0;
     float scalar = 0.f;
     bool dropout = false;      // OP_RELU_MASK: the masked activation was dropped, the kept gradient is scaled by `scalar`
@@ -192,12 +196,11 @@ private:
     void select_set(int set);
     void finish_build();
     int new_event();
-    float* loss_target() const;
     void maybe_splitk(GemmPlan& g);
     void emit_wait(int stream, int ev);
     int emit_record(int stream);
     void walk(int set);
-    void exec(const Op& op);
+    void exec(const Op& op, int set);   // set: the staging set whose plan the op belongs to
     cudaStream_t stream_of(const Op& op) const;
 
     SgdState opt_for(int layer) const;   // the update rule for layer l's block (l = 0: the whole arena)
@@ -220,7 +223,9 @@ private:
     uint32_t* gate_step_ = nullptr;  // steps of THIS engine (bumped in front of the gated kernel)
     float* probs_all_ = nullptr;
     bool coalesced_ = false;
-    float *x_stage_ = nullptr, *y_stage_ = nullptr, *loss_dev_ = nullptr, *loss_host_ = nullptr;
+    float *x_stage_ = nullptr, *y_stage_ = nullptr;
+    // per-micro-batch losses, one slot per staging set, pinned and mapped: the loss head stores them here directly
+    float* loss_host_ = nullptr;
     int* correct_dev_ = nullptr;
     int y_ld_ = 0;
     std::vector<void*> owned_;
@@ -230,7 +235,6 @@ private:
     std::vector<cudaEvent_t> timing_events_;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> exposed_pairs_, busy_pairs_;
     bool comm_timing_ = false;
-    bool loss_zero_copy_ = false;
     std::vector<GemmPlan> gemms_;
     std::vector<FusedDpPlan> dp_plans_;
     std::vector<ChainPlan> chain_plans_;
@@ -261,6 +265,8 @@ private:
     float lr_written_[2] = {0.f, 0.f};
     float lr_ = 0.f;
     const float* lr_slot() const { return lr_dev_ + cur_set_; }
+    int loss_stride() const { return std::max(cfg_.n_mu, 16); }   // floats per staging set in loss_host_
+    float* loss_slot(int set) const { return loss_host_ + set * loss_stride(); }
     // dropout step: the same scheme as lr (allocated only when dropout_on())
     uint32_t* step_dev_ = nullptr;
     uint32_t step_written_[2] = {0u, 0u};

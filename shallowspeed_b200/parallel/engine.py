@@ -221,10 +221,8 @@ class NativeWorker:
         self.model, self.dataset, self.optimizer = model, dataset, optimizer
         self.use_graph, self.precision = use_graph, precision
         self.validate_schedules = validate_schedules
-        import os as _os
-
-        # pipeline boundaries: NCCL send/recv (default) or one-sided pushes into the neighbour's memory (opt-in)
-        self.pp_transport = pp_transport or ("peer" if _os.environ.get("SSB_PP_PEER", "0") not in ("", "0") else "nccl")
+        # pipeline boundaries: one-sided pushes into the neighbour's memory (None = "peer") or NCCL send/recv ("nccl")
+        self.pp_transport = pp_transport or "peer"
         assert self.pp_transport in ("nccl", "peer")
         self.device = model.arena.weights.device
         assert self.device.type == "cuda", "NativeWorker needs the model on a CUDA device (model.to('cuda'))"

@@ -108,35 +108,16 @@ def test_parsers_know_the_runtime_knobs():
     assert b.precision == "fp32" and b.comm == "fused" and b.pp_transport is None and not b.no_alt
 
 
-def test_tuning_file_ships_with_every_variant_off_and_env_wins(tmp_path, monkeypatch):
-    import json
-
-    import shallowspeed_b200 as pkg
-
-    cfg = json.load(open(os.path.join(ROOT, "shallowspeed_b200", "tuning.json")))
-    # a switch is flipped only together with its documentation: every enabled one is named in DESIGN.md
-    notes = open(os.path.join(ROOT, "DESIGN.md")).read()
-    assert all(k in notes for k, v in cfg.items() if k.startswith("SSB_") and v), "flip a switch only together with its documentation"
-    assert pkg.TUNING == {} or all(k in os.environ for k in pkg.TUNING)
-    # semantics of the loader, on a scratch copy
-    import importlib.util
-
-    src = open(os.path.join(ROOT, "shallowspeed_b200", "__init__.py")).read().split("TUNING = _apply_tuning()")[0]
-    scratch = tmp_path / "pkgcopy"
-    scratch.mkdir()
-    (scratch / "__init__.py").write_text(src.replace("from . import", "# from . import"))
-    (scratch / "tuning.json").write_text(json.dumps({"SSB_DEMO_ON": True, "SSB_SPLITK": 4, "SSB_DEMO_OFF": False, "other": 1}))
-    monkeypatch.delenv("SSB_DEMO_ON", raising=False)
-    monkeypatch.setenv("SSB_SPLITK", "2")
-    monkeypatch.delenv("SSB_DEMO_OFF", raising=False)
-    spec = importlib.util.spec_from_file_location("pkgcopy", scratch / "__init__.py")
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    applied = mod._apply_tuning()
-    try:
-        assert applied == {"SSB_DEMO_ON": "1", "SSB_SPLITK": "2"} and "SSB_DEMO_OFF" not in os.environ
-    finally:
-        os.environ.pop("SSB_DEMO_ON", None)        # set by the loader itself, not by monkeypatch
+def test_importing_the_package_leaves_the_environment_alone():
+    """Every default lives in the code that reads it: importing the package (and the native engine's front end) sets
+    no environment variable, so a process and the workers it spawns build the same plans whatever imported what."""
+    code = ("import json, os, sys; sys.path.insert(0, sys.argv[1]); import torch; before = dict(os.environ); "
+            "import shallowspeed_b200, shallowspeed_b200.parallel.engine; print(json.dumps([before, dict(os.environ)]))")
+    env = {k: v for k, v in os.environ.items() if not k.startswith("SSB_")}
+    r = subprocess.run([sys.executable, "-c", code, ROOT], cwd=ROOT, env=env, capture_output=True, text=True, timeout=300)
+    assert r.returncode == 0, r.stderr[-2000:]
+    before, after = json.loads(r.stdout.strip().splitlines()[-1])
+    assert after == before, sorted(set(after.items()) ^ set(before.items()))
 
 
 def test_bench_dump_outputs_stays_within_its_budget(tmp_path):

@@ -130,8 +130,7 @@ def _setup(schedule_cls, steps=1, opt_kw=None, seed_v=True, n_mu=4, lr=0.05, pre
     return out, v0
 
 
-ENV_CASES = [{}, {"SSB_NO_CHAIN": "1"}, {"SSB_NO_COALESCE": "1"}, {"SSB_NO_COALESCE": "1", "SSB_NO_CHAIN": "1"},
-             {"SSB_WGRAD_GROUP": "0"}]
+ENV_CASES = [{}, {"SSB_NO_CHAIN": "1"}, {"SSB_NO_COALESCE": "1"}, {"SSB_NO_COALESCE": "1", "SSB_NO_CHAIN": "1"}]
 
 
 @pytest.mark.parametrize("env", ENV_CASES, ids=lambda e: "+".join(sorted(e)) or "default")

@@ -23,7 +23,8 @@ WIDE = [784, 1024, 1000, 1024, 520, 1024, 130, 10]     # > 128 wide: per-layer G
 GBS, N_MU, LR, STEPS = 128, 4, 0.05, 4
 
 
-def _worker(rank, world, dp, pp, sched_name, comm_mode, port, out_dir, coalesce, two_shot=False, sizes=None, extra_env=None, steps=STEPS):
+def _worker(rank, world, dp, pp, sched_name, comm_mode, port, out_dir, coalesce, two_shot=False, sizes=None, extra_env=None, steps=STEPS,
+            pp_transport=None):
     sizes = sizes or SIZES
     os.environ.update(extra_env or {})
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
@@ -52,7 +53,7 @@ def _worker(rank, world, dp, pp, sched_name, comm_mode, port, out_dir, coalesce,
     ds = Dataset(None, GBS, GBS // dp // N_MU, device=f"cuda:{rank}")
     ds.local_batch_size = GBS // dp
     ds.from_arrays(x[grid.replica::dp], y[grid.replica::dp])
-    w = NativeWorker(dp_comm, pp_comm, model, ds, opt, grid=grid, comm_mode=comm_mode)
+    w = NativeWorker(dp_comm, pp_comm, model, ds, opt, grid=grid, comm_mode=comm_mode, pp_transport=pp_transport)
     sched = SCHEDULE_NAME_TO_CLS[sched_name](N_MU, pp, grid.stage)
     losses = []
     for b in range(steps):
@@ -85,14 +86,16 @@ def _cpu_oracle(sizes=None, steps=STEPS):
     return [p.data.clone() for p in model.parameters()], MLP(sizes, 0, 1, GBS)
 
 
-def _run(dp, pp, sched, comm_mode, tmp_path, coalesce=True, two_shot=False, sizes=None, extra_env=None, steps=STEPS, tight=False):
+def _run(dp, pp, sched, comm_mode, tmp_path, coalesce=True, two_shot=False, sizes=None, extra_env=None, steps=STEPS, tight=False,
+         pp_transport=None):
     import torch.multiprocessing as mp
 
     world = dp * pp
     if torch.cuda.device_count() < world:
         pytest.skip(f"needs {world} GPUs")
     port = 29800 + (os.getpid() + dp * 7 + pp * 13 + len(sched)) % 150
-    mp.spawn(_worker, args=(world, dp, pp, sched, comm_mode, port, str(tmp_path), coalesce, two_shot, sizes, extra_env, steps), nprocs=world,
+    mp.spawn(_worker, args=(world, dp, pp, sched, comm_mode, port, str(tmp_path), coalesce, two_shot, sizes, extra_env, steps,
+                            pp_transport), nprocs=world,
              join=True)
     got = [p for s in range(pp) for p in torch.load(tmp_path / f"stage{s}.pt")["params"]]
     ref, init = _cpu_oracle(sizes, steps)
@@ -177,14 +180,14 @@ def test_nvls_reduce_sgd_matches_oracle(dp, pp, sched, coalesce, tmp_path):
 
 
 # ---------------------------------------------------------------------------------------------------------
-# Peer-memory pipeline transport (--pp-transport peer / SSB_PP_PEER=1): one-sided pushes + epoch flags instead of
+# Peer-memory pipeline transport (--pp-transport peer, the default): one-sided pushes + epoch flags instead of
 # NCCL send/recv.
 # ---------------------------------------------------------------------------------------------------------
 
 
 @pytest.mark.parametrize("dp,pp,sched", [(1, 2, "naive"), (1, 2, "gpipe"), (1, 2, "pipedream"), (1, 4, "gpipe"), (2, 2, "pipedream")])
 def test_pp_peer_transport_matches_oracle(dp, pp, sched, tmp_path):
-    _run(dp, pp, sched, "fused", tmp_path, extra_env={"SSB_PP_PEER": "1"})
+    _run(dp, pp, sched, "fused", tmp_path, pp_transport="peer")
 
 
 # ---------------------------------------------------------------------------------------------------------

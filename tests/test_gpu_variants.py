@@ -1,7 +1,7 @@
-"""Kernel variants:
-split-K FWD / DGRAD GEMMs, zero-copy loss read-back and the grouped weight-gradient launch.  Every variant is compared against the path it replaces: bit for bit where the MMAs and
-their order are unchanged, against an fp64 oracle otherwise.  Switches live in ``shallowspeed_b200/tuning.json``; an
-explicit environment variable always wins, which is how these tests pin each side of a comparison."""
+"""Kernel variants the engine runs by default:
+split-K FWD / DGRAD GEMMs (against an fp64 oracle and the plain kernels, which ``SSB_SPLITK=0`` selects), the zero-copy
+loss read-back and the two-node training step of the chain kernel and the grouped weight-gradient launch
+(tests/test_gpu_wgrad_group_tiles.py checks that launch bit for bit against the per-layer kernel)."""
 import pytest
 import torch
 
@@ -78,10 +78,10 @@ def test_engine_splitk_trains_like_the_plain_kernels(monkeypatch):
 
 
 # ---------------------------------------------------------------------------------------------------------
-# Loss values stored straight into pinned host memory (SSB_LOSS_ZEROCOPY=1), no D2H copy node.
+# Loss values stored straight into pinned host memory by the loss head: no D2H copy node.
 # ---------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("env", [{}, {"SSB_NO_CHAIN": "1"}, {"SSB_NO_COALESCE": "1"}])
-def test_loss_zero_copy_readback_matches(monkeypatch, env):
+def test_loss_zero_copy_readback_has_no_copy_node(monkeypatch, env):
     from shallowspeed_b200.dataset import synthetic_mnist
     from shallowspeed_b200.parallel.engine import Trainer
 
@@ -89,15 +89,9 @@ def test_loss_zero_copy_readback_matches(monkeypatch, env):
         monkeypatch.setenv(k, v)
     x, y = synthetic_mnist(n=128 * 4)
     xh, yh = torch.from_numpy(x).pin_memory(), torch.from_numpy(y).pin_memory()
-    monkeypatch.setenv("SSB_LOSS_ZEROCOPY", "0")
-    base = Trainer(SIZES, lr=0.1)
-    assert "loss_d2h" in base.engine.plan_text(0)
-    ref = [base.step(xh[i * 128:(i + 1) * 128], yh[i * 128:(i + 1) * 128]) for i in range(4)]
-    monkeypatch.setenv("SSB_LOSS_ZEROCOPY", "1")
     tr = Trainer(SIZES, lr=0.1)
-    assert "loss_d2h" not in tr.engine.plan_text(0)
-    got = [tr.step(xh[i * 128:(i + 1) * 128], yh[i * 128:(i + 1) * 128]) for i in range(4)]
-    assert got == ref
+    assert "loss_d2h" not in tr.engine.plan_text(0) + tr.engine.plan_text(1)
+    ref = [tr.step(xh[i * 128:(i + 1) * 128], yh[i * 128:(i + 1) * 128]) for i in range(4)]
     # pipelined read-back: loss of step i is returned by call i + 1
     tr2 = Trainer(SIZES, lr=0.1)
     lag = [tr2.step_pipelined(xh[i * 128:(i + 1) * 128], yh[i * 128:(i + 1) * 128]) for i in range(4)] + [tr2.flush()]
@@ -105,31 +99,11 @@ def test_loss_zero_copy_readback_matches(monkeypatch, env):
 
 
 # ---------------------------------------------------------------------------------------------------------
-# All layers' weight-gradient tiles in ONE launch (SSB_WGRAD_GROUP=1); with the zero-copy loss the whole step is two
+# All layers' weight-gradient tiles in ONE launch behind the chain kernel; with the zero-copy loss the whole step is two
 # graph nodes.
 # ---------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("precision", ["tf32", "fp32"])
-def test_wgrad_group_launch_is_bitwise_identical(monkeypatch, precision):
-    from shallowspeed_b200.dataset import synthetic_mnist
-    from shallowspeed_b200.parallel.engine import Trainer
-
-    x, y = synthetic_mnist(n=128 * 4)
-    xh, yh = torch.from_numpy(x).pin_memory(), torch.from_numpy(y).pin_memory()
-    monkeypatch.setenv("SSB_WGRAD_GROUP", "0")
-    base = Trainer(SIZES, lr=0.1, precision=precision)
-    assert "wgrad_group" not in base.engine.plan_text(0)
-    ref = [base.step(xh[i * 128:(i + 1) * 128], yh[i * 128:(i + 1) * 128]) for i in range(4)]
-    monkeypatch.setenv("SSB_WGRAD_GROUP", "1")
-    tr = Trainer(SIZES, lr=0.1, precision=precision)
-    plan = tr.engine.plan_text(0)
-    assert "wgrad_group" in plan and " gemm " not in plan
-    got = [tr.step(xh[i * 128:(i + 1) * 128], yh[i * 128:(i + 1) * 128]) for i in range(4)]
-    assert got == ref
-    assert torch.equal(tr.model.arena.weights, base.model.arena.weights)
-
-
-@pytest.mark.parametrize("precision", ["tf32", "fp32"])
-def test_default_training_step_is_a_two_or_three_node_line(monkeypatch, precision):
+def test_default_training_step_is_a_two_or_three_node_line(precision):
     """chain kernel -> grouped wgrad + SGD in both precisions (3xTF32 derives its lo parts in the kernels): no loss copy
     node, no per-layer fork / join."""
     from shallowspeed_b200.dataset import synthetic_mnist
@@ -138,16 +112,10 @@ def test_default_training_step_is_a_two_or_three_node_line(monkeypatch, precisio
 
     x, y = synthetic_mnist(n=128 * 4)
     xh, yh = torch.from_numpy(x).pin_memory(), torch.from_numpy(y).pin_memory()
-    for k in ("SSB_WGRAD_GROUP", "SSB_LOSS_ZEROCOPY"):
-        monkeypatch.setenv(k, "0")
-    base = Trainer(SIZES, lr=0.1, precision=precision)
-    ref = [base.step(xh[i * 128:(i + 1) * 128], yh[i * 128:(i + 1) * 128]) for i in range(4)]
-    for k in ("SSB_WGRAD_GROUP", "SSB_LOSS_ZEROCOPY"):
-        monkeypatch.setenv(k, "1")
     tr = Trainer(SIZES, lr=0.1, precision=precision)
     stats = check_plan(tr.engine.plan_text(0))
     want = 2
     assert stats["kernels_and_copies"] == want, tr.engine.plan_text(0)
     assert int(tr.engine.graph_nodes()) == want
-    got = [tr.step(xh[i * 128:(i + 1) * 128], yh[i * 128:(i + 1) * 128]) for i in range(4)]
-    assert got == ref and torch.equal(tr.model.arena.weights, base.model.arena.weights)
+    losses = [tr.step(xh[i * 128:(i + 1) * 128], yh[i * 128:(i + 1) * 128]) for i in range(4)]
+    assert all(0.0 < v < 10.0 for v in losses), losses

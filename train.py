@@ -118,7 +118,7 @@ def build_parser():
                    help="native engine DP path: in-kernel reduction over peer memory, or plain NCCL all-reduce (A/B baseline)")
     p.add_argument("--pp-transport", choices=["nccl", "peer"], default=None,
                    help="native engine, stage boundaries: one-sided pushes into the neighbour's memory over NVLink with "
-                        "epoch flags (peer; the default through SSB_PP_PEER in tuning.json) or NCCL send/recv")
+                        "epoch flags (peer, the default) or NCCL send/recv")
     p.add_argument("--no-graph", action="store_true", help="native engine: do not capture the step in a CUDA graph")
     p.add_argument("--precision", choices=["tf32", "fp32"], default="fp32",
                    help="tensor-core math: fp32 = 3xTF32 split (fp32-equivalent, the reference's contract); tf32 = single pass")

@@ -79,11 +79,11 @@ static ssb::DropoutSpec drop_arg(const py::object& drop, const Tensor& like, Ten
     return spec;
 }
 
-// y[rows, out] = act?(x @ W^T + b); split: 3xTF32 (fp32-equivalent) products.  relu selects the layer's activation
+// y[rows, out] = act?(x @ W^T + b); prec: the products' Precision (precision.h; a bool: false TF32, true 3xTF32).  relu selects the layer's activation
 // act_kind (activation.h: ReLU by default); a smooth kind can store its gate f'(z) (* keep * s under dropout) to `gate`,
 // which the kernel addresses with y's row pitch.  drop: see drop_arg, applied after the activation.
 static void linear_fwd(const Tensor& x, const Tensor& W, const c10::optional<Tensor>& bias, int64_t bias_stride,
-                       bool relu, Tensor& y, bool split, int64_t k_splits, int64_t act_kind,
+                       bool relu, Tensor& y, int64_t prec, int64_t k_splits, int64_t act_kind,
                        const c10::optional<Tensor>& gate, const py::object& drop) {
     check_mat(x, "x"); check_mat(W, "W"); check_mat(y, "y");
     const int rows = x.size(0), in = x.size(1), out = W.size(0);
@@ -101,7 +101,7 @@ static void linear_fwd(const Tensor& x, const Tensor& W, const c10::optional<Ten
     ssb::GemmPlan plan;
     const char* err = ssb::gemm_plan_fwd(&plan, W.data_ptr<float>(), ld_of(W), x.data_ptr<float>(), ld_of(x),
                                          y.data_ptr<float>(), ld_of(y), rows, in, out,
-                                         bias.has_value() ? bias->data_ptr<float>() : nullptr, (int)bias_stride, relu, split);
+                                         bias.has_value() ? bias->data_ptr<float>() : nullptr, (int)bias_stride, relu, (int)prec);
     TORCH_CHECK(err == nullptr, "linear_fwd: ", err ? err : "");
     Tensor step_dev;
     plan.p.act_kind = (int)act_kind;
@@ -115,7 +115,7 @@ static void linear_fwd(const Tensor& x, const Tensor& W, const c10::optional<Ten
 // dx[rows, in] = (dz @ W) * (mask > 0), or * s where the mask passes under dropout (only its p is read), or * mask for a
 // smooth act_kind (the mask is then the previous layer's gate, which holds the dropout scale itself)
 static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<Tensor>& mask, Tensor& dx,
-                         bool split, int64_t k_splits, int64_t act_kind, const py::object& drop) {
+                         int64_t prec, int64_t k_splits, int64_t act_kind, const py::object& drop) {
     check_mat(dz, "dz"); check_mat(W, "W"); check_mat(dx, "dx");
     const int rows = dz.size(0), out = dz.size(1), in = W.size(1);
     TORCH_CHECK(W.size(0) == out && dx.size(0) == rows && dx.size(1) == in, "linear_dgrad: shape mismatch");
@@ -130,7 +130,7 @@ static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<
     const char* err = ssb::gemm_plan_dgrad(&plan, W.data_ptr<float>(), ld_of(W), dz.data_ptr<float>(), ld_of(dz),
                                            dx.data_ptr<float>(), ld_of(dx), rows, in, out,
                                            mask.has_value() ? mask->data_ptr<float>() : nullptr,
-                                           mask.has_value() ? ld_of(*mask) : 0, split);
+                                           mask.has_value() ? ld_of(*mask) : 0, (int)prec);
     TORCH_CHECK(err == nullptr, "linear_dgrad: ", err ? err : "");
     Tensor step_dev;
     plan.p.act_kind = (int)act_kind;
@@ -145,7 +145,7 @@ static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<
 // (same row pitch; its column `in` belongs to the bias).
 static void linear_wgrad(const Tensor& dz, const Tensor& x, Tensor& G, bool accumulate, const c10::optional<Tensor>& db,
                          int64_t db_stride, const c10::optional<Tensor>& W, const py::object& lr, bool fuse_sgd,
-                         bool split, const c10::optional<Tensor>& V, double momentum, double weight_decay, bool nesterov) {
+                         int64_t prec, const c10::optional<Tensor>& V, double momentum, double weight_decay, bool nesterov) {
     check_mat(dz, "dz"); check_mat(x, "x"); check_mat(G, "G");
     const int rows = dz.size(0), out = dz.size(1), in = x.size(1);
     TORCH_CHECK(x.size(0) == rows && G.size(0) == out && G.size(1) == in, "linear_wgrad: shape mismatch");
@@ -165,7 +165,7 @@ static void linear_wgrad(const Tensor& dz, const Tensor& x, Tensor& G, bool accu
                                            db.has_value() ? db->data_ptr<float>() : nullptr, (int)db_stride,
                                            W.has_value() ? W->data_ptr<float>() : nullptr,
                                            W.has_value() ? ld_of(*W) : 0, fuse_sgd ? lr_dev.data_ptr<float>() : nullptr,
-                                           fuse_sgd, split, opt);
+                                           fuse_sgd, (int)prec, opt);
     TORCH_CHECK(err == nullptr, "linear_wgrad: ", err ? err : "");
     cuda_ok(ssb::gemm_launch(plan, cur_stream()), "linear_wgrad launch");
 }
@@ -313,13 +313,13 @@ static void gather_rows(const c10::optional<Tensor>& x_src, const c10::optional<
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.doc() = "shallowspeed_b200 native module: sm_90a kernels + C++ pipeline runtime";
     m.def("linear_fwd", &linear_fwd, py::arg("x"), py::arg("W"), py::arg("bias"), py::arg("bias_stride"), py::arg("relu"),
-          py::arg("y"), py::arg("split") = false, py::arg("k_splits") = 0, py::arg("act_kind") = (int)ssb::ACT_RELU,
+          py::arg("y"), py::arg("prec") = (int)ssb::PREC_TF32, py::arg("k_splits") = 0, py::arg("act_kind") = (int)ssb::ACT_RELU,
           py::arg("gate") = py::none(), py::arg("drop") = py::none());
     m.def("linear_dgrad", &linear_dgrad, py::arg("dz"), py::arg("W"), py::arg("mask"), py::arg("dx"),
-          py::arg("split") = false, py::arg("k_splits") = 0, py::arg("act_kind") = (int)ssb::ACT_RELU,
+          py::arg("prec") = (int)ssb::PREC_TF32, py::arg("k_splits") = 0, py::arg("act_kind") = (int)ssb::ACT_RELU,
           py::arg("drop") = py::none());
     m.def("linear_wgrad", &linear_wgrad, py::arg("dz"), py::arg("x"), py::arg("G"), py::arg("accumulate"), py::arg("db"),
-          py::arg("db_stride"), py::arg("W"), py::arg("lr"), py::arg("fuse_sgd"), py::arg("split") = false,
+          py::arg("db_stride"), py::arg("W"), py::arg("lr"), py::arg("fuse_sgd"), py::arg("prec") = (int)ssb::PREC_TF32,
           py::arg("V") = py::none(), py::arg("momentum") = 0.0, py::arg("weight_decay") = 0.0, py::arg("nesterov") = false);
     m.def("loss_head", &loss_head, py::arg("logits"), py::arg("target"), py::arg("probs"), py::arg("dlogits"),
           py::arg("loss_out"), py::arg("inv_batch"), py::arg("loss") = (int)ssb::LOSS_MSE);
@@ -337,9 +337,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("gather_rows", &gather_rows, py::arg("x_src"), py::arg("y_src"), py::arg("seed"), py::arg("epoch"), py::arg("gbs"),
           py::arg("dp"), py::arg("rank"), py::arg("batch"), py::arg("x_dst"), py::arg("y_dst"));
     m.def("gemm_kernel_count", &ssb::gemm_kernel_count);
-    m.def("chain_budget", [](int mb_rows, bool split) {
+    m.def("chain_budget", [](int mb_rows, int prec) {
         int kps = 0, stages = 0, smem = 0;
-        const bool ok = ssb::chain_budget(mb_rows, split, &kps, &stages, &smem);
+        const bool ok = ssb::chain_budget(mb_rows, prec, &kps, &stages, &smem);
         return std::make_tuple(ok, kps, stages, smem);
     });
     // tiles of one grouped weight gradient, no GPU needed: ([(m0, n0, rows, cols, owns_bias)], stages, smem bytes per CTA)
@@ -351,9 +351,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         for (const auto& t : tiles) list.emplace_back(t.m0, t.n0, t.rows, t.cols, t.owns_bias);
         return std::make_tuple(list, stages, smem);
     });
-    m.def("chain_cluster_budget", [](int mb_rows, int cluster, bool split) {
+    m.def("chain_cluster_budget", [](int mb_rows, int cluster, int prec) {
         int kps = 0, stages = 0, smem = 0;
-        const bool ok = ssb::chain_cluster_budget(mb_rows, cluster, split, &kps, &stages, &smem);
+        const bool ok = ssb::chain_cluster_budget(mb_rows, cluster, prec, &kps, &stages, &smem);
         return std::make_tuple(ok, kps, stages, smem);
     });
     // k-split layer 1, no GPU needed: the k-blocks of a GEMM of nkb k-blocks that part 0 (owner) / 1 (helper) multiplies
@@ -368,10 +368,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         for (size_t i = 0; i < in_out.size(); ++i) { ls[i] = ssb::ChainLayer{}; ls[i].in = in_out[i].first; ls[i].out = in_out[i].second; }
         return ssb::chain_cluster_size(ls.data(), (int)ls.size(), do_fwd, do_loss, do_bwd, first_stage, gated, folded);
     });
-    m.def("chain_eligible", [](const std::vector<std::pair<int, int>>& in_out, int mb_rows, int out_dim, bool has_loss, bool split) {
+    m.def("chain_eligible", [](const std::vector<std::pair<int, int>>& in_out, int mb_rows, int out_dim, bool has_loss, int prec) {
         std::vector<ssb::ChainLayer> ls(in_out.size());
         for (size_t i = 0; i < in_out.size(); ++i) { ls[i] = ssb::ChainLayer{}; ls[i].in = in_out[i].first; ls[i].out = in_out[i].second; }
-        return ssb::chain_eligible(ls.data(), (int)ls.size(), mb_rows, out_dim, has_loss, split);
+        return ssb::chain_eligible(ls.data(), (int)ls.size(), mb_rows, out_dim, has_loss, prec);
     });
     m.def("dp_layer_geometry", [](int in, int out, int dp, bool one_shot) {
         int block_n = 0, tm = 0, tn = 0;

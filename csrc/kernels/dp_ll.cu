@@ -139,8 +139,9 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
             const int s = kb % p.stages;
             mbar_wait(full_bar(s), (kb / p.stages) & 1);
             const uint32_t a_src = smem_base + s * stage_bytes;
-            if (e.split) warp_mma_kblock<4, true, true, true>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, 4, lane);
-            else warp_mma_kblock<4, true, true, false>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, 4, lane);
+            if (e.prec == PREC_3XTF32) warp_mma_kblock<4, true, true, PREC_3XTF32>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, 4, lane);
+            else if (e.prec == PREC_BF16) warp_mma_kblock<4, true, true, PREC_BF16>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, 4, lane);
+            else warp_mma_kblock<4, true, true, PREC_TF32>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, 4, lane);
             if (e.has_bias) {
 #pragma unroll 8
                 for (int r = 0; r < 32; ++r) dbsum += lds_f32(a_src + operand_off<true>((uint32_t)m_local, (uint32_t)r));
@@ -313,14 +314,12 @@ const char* dp_ll_plan(DpLLPlan* plan, const DpLLLayer* layers, int n_layers, in
     if (base.lr == nullptr) return "dp_ll_plan: lr (the device learning-rate slot) is not set";
     std::vector<DpLLEntry> host;
     int tile = 0;
-    bool split = false;
     for (int l = 0; l < n_layers; ++l) {
         const DpLLLayer& ly = layers[l];
         CUtensorMap tmA, tmB;
         if (const char* err = make_tmap_mn(&tmA, ly.dZ, ly.out, rows, ly.lddz)) return err;
         if (const char* err = make_tmap_mn(&tmB, ly.X, ly.in, rows, ly.ldx)) return err;
-        const bool sp = ly.split != 0;                              // 3xTF32: the kernel derives the lo parts from the tiles
-        split = split || sp;
+        if (!prec_valid(ly.prec)) return "dp_ll_plan: unknown precision";
         const int tm = (ly.out + (int)kBlockM - 1) / (int)kBlockM, tn = (ly.in + 31) / 32;
         for (int mt = 0; mt < tm; ++mt)
             for (int nt = 0; nt < tn; ++nt) {
@@ -329,7 +328,7 @@ const char* dp_ll_plan(DpLLPlan* plan, const DpLLLayer* layers, int n_layers, in
                 e.tmA = tmA; e.tmB = tmB;
                 e.m0 = mt * (int)kBlockM; e.n0 = nt * 32;
                 e.m_total = ly.out; e.n_total = ly.in; e.k_total = rows;
-                e.split = sp ? 1 : 0;
+                e.prec = ly.prec;                                    // 3xTF32: the kernel derives the lo parts from the tiles
                 e.has_bias = nt == 0 ? 1 : 0;
                 e.tile = tile++;
                 e.w_offset = ly.w_offset; e.ldw = ly.ldw;

@@ -271,8 +271,12 @@ fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 const uint32_t ph = (it / p.stages) & 1;
                 mbar_wait(full_bar(s), ph);
                 const uint32_t a_src = smem_base + s * stage_bytes;
-                if (p.split) warp_mma_kblock<kMaxBlockN / 8, true, true, true>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, nt, lane);
-                else warp_mma_kblock<kMaxBlockN / 8, true, true, false>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, nt, lane);
+                if (p.prec == PREC_3XTF32)
+                    warp_mma_kblock<kMaxBlockN / 8, true, true, PREC_3XTF32>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, nt, lane);
+                else if (p.prec == PREC_BF16)
+                    warp_mma_kblock<kMaxBlockN / 8, true, true, PREC_BF16>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, nt, lane);
+                else
+                    warp_mma_kblock<kMaxBlockN / 8, true, true, PREC_TF32>(acc, a_src, (uint32_t)q * 32u, a_src + kABytes, 0u, nt, lane);
                 if (tc.nt == 0) {
 #pragma unroll 8
                     for (int r = 0; r < 32; ++r) dbsum += lds_f32(a_src + operand_off<true>((uint32_t)m_local, (uint32_t)r));
@@ -446,8 +450,9 @@ void dp_layer_geometry(int in, int out, int dp, int* block_n, int* n_tiles_m, in
 }
 
 const char* fused_dp_plan(FusedDpPlan* plan, const float* dZ, int lddz, const float* X, int ldx, int rows, const DpLayerParams& lp,
-                          const DpPeers& peers, int max_ctas, bool split) {
+                          const DpPeers& peers, int max_ctas, int prec) {
     *plan = FusedDpPlan{};
+    if (!prec_valid(prec)) return "fused_dp_plan: unknown precision";
     if (lp.lr == nullptr) return "fused_dp_plan: lr (the device learning-rate slot) is not set";
     plan->p = lp;
     plan->peers = peers;
@@ -456,7 +461,7 @@ const char* fused_dp_plan(FusedDpPlan* plan, const float* dZ, int lddz, const fl
     if (dZ != nullptr) {
         if (const char* e = make_tmap_mn(&plan->tmA, dZ, p.m_total, rows, lddz)) return e;
         if (const char* e = make_tmap_mn(&plan->tmB, X, p.n_total, rows, ldx)) return e;
-        p.split = split ? 1 : 0;                  // 3xTF32: the kernel derives the lo parts from the tiles
+        p.prec = prec;                            // 3xTF32: the kernel derives the lo parts from the tiles
     }
     const int num_kb = (rows + (int)kBlockK - 1) / (int)kBlockK;
     const int stage_bytes = (int)kABytes + p.block_n * 128;

@@ -8,6 +8,7 @@
 
 #include "activation.h"
 #include "dropout.h"
+#include "precision.h"
 #include "shuffle.h"
 
 namespace ssb {
@@ -73,8 +74,8 @@ struct GemmParams {
     float* V;
     float momentum, weight_decay;
     int nesterov;
-    // fp32-equivalent mode (3xTF32 products, the operands' lo parts x - trunc_tf32(x) derived in the kernel)
-    int split;
+    // Precision of the products (precision.h); PREC_3XTF32 derives the operands' lo parts x - trunc_tf32(x) in the kernel
+    int prec;
     // split-K (FWD / DGRAD, see gemm_plan_enable_splitk): blockIdx.z owns a k-range, partial tiles go through
     // `partial` [tile][split][block_n][128], the last arriver at tile_counter[tile] reduces + runs the epilogue
     int k_splits;                 // 0 / 1 = off
@@ -103,15 +104,15 @@ struct GemmPlan {          // a fully prepared launch (tensor maps are 128 B eac
 //   FWD:   W[out, in] (ldw), X[rows, in] (ldx)            -> Y[rows, out] (ldy)
 //   DGRAD: W[out, in] (ldw), dZ[rows, out] (lddz)         -> dX[rows, in] (lddx)
 //   WGRAD: dZ[rows, out] (lddz), X[rows, in] (ldx)        -> G[out, in] (ldg)
-// split: false = plain TF32 products; true = 3xTF32 (fp32-equivalent; the kernels derive the operands' lo parts
-// x - trunc_tf32(x) from the staged tiles)
+// prec: the products' Precision (precision.h): PREC_TF32 (0, false), PREC_3XTF32 (1, true; fp32-equivalent, the kernels
+// derive the operands' lo parts x - trunc_tf32(x) from the staged tiles) or PREC_BF16 (operands rounded in registers)
 const char* gemm_plan_fwd(GemmPlan* plan, const float* W, int ldw, const float* X, int ldx, float* Y, int ldy,
-                          int rows, int in, int out, const float* bias, int bias_stride, int relu, bool split = false);
+                          int rows, int in, int out, const float* bias, int bias_stride, int relu, int prec = PREC_TF32);
 const char* gemm_plan_dgrad(GemmPlan* plan, const float* W, int ldw, const float* dZ, int lddz, float* dX, int lddx,
-                            int rows, int in, int out, const float* mask, int ldmask, bool split = false);
+                            int rows, int in, int out, const float* mask, int ldmask, int prec = PREC_TF32);
 const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const float* X, int ldx, float* G, int ldg,
                             int rows, int in, int out, int accumulate, float* db, int db_stride, float* W, int ldw,
-                            const float* lr, int fuse_sgd, bool split = false, const SgdState& opt = SgdState{});
+                            const float* lr, int fuse_sgd, int prec = PREC_TF32, const SgdState& opt = SgdState{});
 // Split-K for FWD / DGRAD plans whose output has fewer tiles than the chip has SMs (wide, weight-bound layers):
 // choice() returns the number of k-splits (1 = leave the plan alone); enable() rewires the plan (grid.z, ring
 // depth for two CTAs per SM).  workspace: gemm_splitk_workspace_floats() floats; counters: one zeroed uint per tile.
@@ -176,7 +177,7 @@ struct DpLayerParams {
     // one NVLink hop instead of two).  Staging is double-buffered by epoch parity (stage_parity_stride).
     int one_shot;
     int64_t stage_parity_stride;
-    int split;                       // 3xTF32 products (lo parts derived from the staged dZ / X tiles)
+    int prec;                        // Precision of the products (3xTF32: lo parts derived from the staged dZ / X tiles)
     int helpers;                     // CTAs per tile: CTA 0 computes + pushes, all of them share the reduce rows
     int bulk_push;                   // 1: push tiles with cp.async.bulk (TMA engine), 0: coalesced st.global
     unsigned long long* dbg;         // optional: 8 globaltimer stamps of CTA 0 (phase timeline)
@@ -201,7 +202,7 @@ void dp_layer_geometry(int in, int out, int dp, int* block_n, int* n_tiles_m, in
                        int64_t* slot_floats, int one_shot);
 // dZ == nullptr: plan for dp_reduce_sgd (no GEMM)
 const char* fused_dp_plan(FusedDpPlan* plan, const float* dZ, int lddz, const float* X, int ldx, int rows,
-                          const DpLayerParams& lp, const DpPeers& peers, int max_ctas, bool split = false);
+                          const DpLayerParams& lp, const DpPeers& peers, int max_ctas, int prec = PREC_TF32);
 cudaError_t fused_dp_configure();
 cudaError_t launch_fused_wgrad_dp(const FusedDpPlan& plan, cudaStream_t stream);
 cudaError_t launch_dp_reduce_sgd(const FusedDpPlan& plan, cudaStream_t stream);
@@ -212,7 +213,7 @@ struct DpLLEntry {               // one CTA = one [128 x 32] tile of one layer's
     CUtensorMap tmA, tmB;        // dZ (MN-major A), X (MN-major B)
     int m0, n0;                  // tile origin in (out, in)
     int m_total, n_total, k_total;
-    int split, has_bias;
+    int prec, has_bias;
     int tile;                    // index in the landing zones
     int64_t w_offset;            // float offset of the layer's [out, ld] block in the arena
     int ldw;
@@ -234,7 +235,7 @@ struct DpLLParams {
 };
 struct DpLLLayer {
     const float *dZ, *X;
-    int split;                   // 3xTF32 products
+    int prec;                    // Precision of the products
     int lddz, ldx, in, out, ldw;
     int64_t w_offset;
     const uint32_t* gate_flag;
@@ -263,7 +264,7 @@ struct ChainParams {
     int n_layers;
     ChainLayer layers[kChainMaxLayers];
     const CUtensorMap* maps;         // device array: [2l] W_l K-major (fwd), [2l+1] W_l MN-major (dgrad), [2L] X
-    int split;                       // 3xTF32 (fp32-equivalent) products
+    int prec;                        // Precision of the products
     const float* W;                  // weight arena (bias reads)
     float* act[kChainMaxLayers + 1]; // act[0] = stage input, act[l] = output of layer l  ([all rows, ld])
     float* dz[kChainMaxLayers + 1];  // dz[l] = gradient w.r.t. the pre-activation of layer l (dz[0]: stage input grad)
@@ -321,17 +322,17 @@ struct ChainPlan {
     int cluster;                     // CTAs per feature slice (grid = micro-batches x cluster x ksplit)
     int ksplit;                      // CTAs per feature slice in layer 1 (ChainParams::ksplit)
 };
-bool chain_eligible(const ChainLayer* layers, int n_layers, int mb_rows, int out_dim, bool has_loss, bool split = false);
+bool chain_eligible(const ChainLayer* layers, int n_layers, int mb_rows, int out_dim, bool has_loss, int prec = PREC_TF32);
 const char* chain_plan(ChainPlan* plan, const ChainParams& params, const float* x, int ldx, int total_rows, int n_mubatches,
-                       bool split = false);
-bool chain_budget(int mb_rows, bool split, int* kps, int* stages, int* smem_bytes);   // host arithmetic only
+                       int prec = PREC_TF32);
+bool chain_budget(int mb_rows, int prec, int* kps, int* stages, int* smem_bytes);   // host arithmetic only
 // Cluster plan of one chain launch (host arithmetic only).  chain_cluster_size: CTAs per micro-batch, ceil(w / 32) for the
 // widest tile w the launch writes into shared memory (every forward output, every dgrad output, and dZ_L when a
 // backward-only launch stages it), and 1 for launches gated for a co-resident consumer or with folded pipeline
 // boundaries.  chain_cluster_budget: the shared-memory plan at that size (chain_budget's when cluster == 1).
 int chain_cluster_size(const ChainLayer* layers, int n_layers, bool do_fwd, bool do_loss, bool do_bwd, bool first_stage,
                        bool gated, bool folded);
-bool chain_cluster_budget(int mb_rows, int cluster, bool split, int* kps, int* stages, int* smem_bytes);
+bool chain_cluster_budget(int mb_rows, int cluster, int prec, int* kps, int* stages, int* smem_bytes);
 // k-split layer 1 (host arithmetic only): the k-blocks of a GEMM of nkb k-blocks that part 0 (the owner) or 1 (the
 // helper) of a feature slice multiplies, in the order it streams them, into kblocks; returns their number
 int chain_ksplit_kblocks(int nkb, int part, int* kblocks);

@@ -7,6 +7,7 @@
 
 #include "activation.h"
 #include "dropout.h"
+#include "precision.h"
 #include "shuffle.h"
 
 namespace ssb {
@@ -153,19 +154,36 @@ __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], 
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
+// bf16 products: the m16n8k16 BF16 MMA, fp32 accumulate.  Operands are packed two per register, the lower k in the
+// lower half.
+__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+                 "{%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// (bf16(lo), bf16(hi)) rounded to nearest even; cvt's first source operand goes to the upper half
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+    uint32_t r;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+    return r;
+}
+
 // 3xTF32: x = hi + lo with hi = trunc_tf32(x) (the top 19 bits) and lo = x - hi exact in fp32, so
 // a*b ~= lo_a*hi_b + hi_a*lo_b + hi_a*hi_b  (error ~2^-20 relative).  The hi operand is truncated explicitly, so the
 // split does not depend on how the tensor core treats the low 13 mantissa bits of its inputs.
 __device__ __forceinline__ uint32_t tf32_hi_bits(float x) { return __float_as_uint(x) & 0xFFFFE000u; }
 
+// Tensor-core precision of a product (kernels.h: PREC_TF32 / PREC_3XTF32 / PREC_BF16).
 // One warp: D[32 x 8*nt] += A[m_base .. m_base+31, one 32-wide k-block] * B[n_base .. n_base+8*nt-1, same k-block]^T,
 // both operands read from swizzled tiles (operand_off).  The k-block's products are summed into a fresh tensor-core
 // accumulator and then added to `acc` with an fp32 add, so the accumulated rounding error grows with the number of
-// 32-wide k-blocks, not with the number of MMA steps.  SPLIT: 3xTF32 products, the lo parts derived from the tile.
+// 32-wide k-blocks, not with the number of MMA steps.  PREC_3XTF32: 3xTF32 products, the lo parts derived from the tile.
+// PREC_BF16: two m16n8k16 BF16 MMAs per k-block, operands rounded to bf16 in registers (see below).
 // acc[i][j][r]: m16 tile i, n8 tile j, mma.sync C fragment register r (rows lane/4 (+8), columns 2*(lane%4) (+1)).
 // MI: m16 tiles of the block (2: 32 rows of A, 1: the 16 rows m_base .. m_base+15).  Each (i, j) tile sees the same
 // instructions on the same operands whatever MI and NT are, so its sums do not depend on the block shape.
-template <int NT, bool A_MN, bool B_MN, bool SPLIT, int MI = 2>
+template <int NT, bool A_MN, bool B_MN, int PREC, int MI = 2>
 __device__ __forceinline__ void warp_mma_kblock(float (&acc)[MI][NT][4], uint32_t a_tile, uint32_t m_base, uint32_t b_tile,
                                                 uint32_t n_base, int nt, int lane) {
     const uint32_t g = (uint32_t)lane >> 2, t = (uint32_t)lane & 3u;
@@ -176,36 +194,70 @@ __device__ __forceinline__ void warp_mma_kblock(float (&acc)[MI][NT][4], uint32_
         for (int j = 0; j < NT; ++j)
 #pragma unroll
             for (int r = 0; r < 4; ++r) part[i][j][r] = 0.f;
+    if constexpr (PREC == PREC_BF16) {
+        // The loads are the TF32 fragments' at k0 and k0 + 8.  Thread (g, t) holds logical k {2t, 2t+1, 2t+8, 2t+9} of
+        // the k16 fragment; they are fed physical k {k0+t, k0+t+4, k0+8+t, k0+12+t}, the same map for A and B, which
+        // covers k0 .. k0+15 once over t = 0..3.  A sum over k does not depend on how its terms are numbered, so the
+        // shared-memory layout is the TF32 one.
 #pragma unroll
-    for (uint32_t k0 = 0; k0 < 32u; k0 += 8u) {
-        uint32_t ah[MI][4], al[MI][4];
+        for (uint32_t k0 = 0; k0 < 32u; k0 += 16u) {
+            uint32_t a[MI][4];
 #pragma unroll
-        for (int i = 0; i < MI; ++i) {
-            const uint32_t r0 = m_base + 16u * i + g;
-            const float x[4] = {lds_f32(a_tile + operand_off<A_MN>(r0, k0 + t)), lds_f32(a_tile + operand_off<A_MN>(r0 + 8u, k0 + t)),
-                                lds_f32(a_tile + operand_off<A_MN>(r0, k0 + t + 4u)),
-                                lds_f32(a_tile + operand_off<A_MN>(r0 + 8u, k0 + t + 4u))};
+            for (int i = 0; i < MI; ++i) {
+                const uint32_t r0 = m_base + 16u * i + g;
+                a[i][0] = pack_bf16x2(lds_f32(a_tile + operand_off<A_MN>(r0, k0 + t)), lds_f32(a_tile + operand_off<A_MN>(r0, k0 + t + 4u)));
+                a[i][1] = pack_bf16x2(lds_f32(a_tile + operand_off<A_MN>(r0 + 8u, k0 + t)),
+                                      lds_f32(a_tile + operand_off<A_MN>(r0 + 8u, k0 + t + 4u)));
+                a[i][2] = pack_bf16x2(lds_f32(a_tile + operand_off<A_MN>(r0, k0 + t + 8u)),
+                                      lds_f32(a_tile + operand_off<A_MN>(r0, k0 + t + 12u)));
+                a[i][3] = pack_bf16x2(lds_f32(a_tile + operand_off<A_MN>(r0 + 8u, k0 + t + 8u)),
+                                      lds_f32(a_tile + operand_off<A_MN>(r0 + 8u, k0 + t + 12u)));
+            }
 #pragma unroll
-            for (int r = 0; r < 4; ++r) {
-                ah[i][r] = tf32_hi_bits(x[r]);
-                al[i][r] = __float_as_uint(x[r] - __uint_as_float(ah[i][r]));
+            for (int j = 0; j < NT; ++j) {
+                if (j < nt) {
+                    const uint32_t n = n_base + 8u * j + g;
+                    const uint32_t b0 = pack_bf16x2(lds_f32(b_tile + operand_off<B_MN>(n, k0 + t)),
+                                                    lds_f32(b_tile + operand_off<B_MN>(n, k0 + t + 4u)));
+                    const uint32_t b1 = pack_bf16x2(lds_f32(b_tile + operand_off<B_MN>(n, k0 + t + 8u)),
+                                                    lds_f32(b_tile + operand_off<B_MN>(n, k0 + t + 12u)));
+#pragma unroll
+                    for (int i = 0; i < MI; ++i) mma_bf16(part[i][j], a[i], b0, b1);
+                }
             }
         }
+    } else {
 #pragma unroll
-        for (int j = 0; j < NT; ++j) {
-            if (j < nt) {
-                const uint32_t n = n_base + 8u * j + g;
-                const float y0 = lds_f32(b_tile + operand_off<B_MN>(n, k0 + t));
-                const float y1 = lds_f32(b_tile + operand_off<B_MN>(n, k0 + t + 4u));
-                const uint32_t bh0 = tf32_hi_bits(y0), bh1 = tf32_hi_bits(y1);
-                const uint32_t bl0 = __float_as_uint(y0 - __uint_as_float(bh0)), bl1 = __float_as_uint(y1 - __uint_as_float(bh1));
+        for (uint32_t k0 = 0; k0 < 32u; k0 += 8u) {
+            uint32_t ah[MI][4], al[MI][4];
 #pragma unroll
-                for (int i = 0; i < MI; ++i) {
-                    if (SPLIT) {
-                        mma_tf32(part[i][j], al[i], bh0, bh1);
-                        mma_tf32(part[i][j], ah[i], bl0, bl1);
+            for (int i = 0; i < MI; ++i) {
+                const uint32_t r0 = m_base + 16u * i + g;
+                const float x[4] = {lds_f32(a_tile + operand_off<A_MN>(r0, k0 + t)), lds_f32(a_tile + operand_off<A_MN>(r0 + 8u, k0 + t)),
+                                    lds_f32(a_tile + operand_off<A_MN>(r0, k0 + t + 4u)),
+                                    lds_f32(a_tile + operand_off<A_MN>(r0 + 8u, k0 + t + 4u))};
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+                    ah[i][r] = tf32_hi_bits(x[r]);
+                    al[i][r] = __float_as_uint(x[r] - __uint_as_float(ah[i][r]));
+                }
+            }
+#pragma unroll
+            for (int j = 0; j < NT; ++j) {
+                if (j < nt) {
+                    const uint32_t n = n_base + 8u * j + g;
+                    const float y0 = lds_f32(b_tile + operand_off<B_MN>(n, k0 + t));
+                    const float y1 = lds_f32(b_tile + operand_off<B_MN>(n, k0 + t + 4u));
+                    const uint32_t bh0 = tf32_hi_bits(y0), bh1 = tf32_hi_bits(y1);
+                    const uint32_t bl0 = __float_as_uint(y0 - __uint_as_float(bh0)), bl1 = __float_as_uint(y1 - __uint_as_float(bh1));
+#pragma unroll
+                    for (int i = 0; i < MI; ++i) {
+                        if (PREC == PREC_3XTF32) {
+                            mma_tf32(part[i][j], al[i], bh0, bh1);
+                            mma_tf32(part[i][j], ah[i], bl0, bl1);
+                        }
+                        mma_tf32(part[i][j], ah[i], bh0, bh1);
                     }
-                    mma_tf32(part[i][j], ah[i], bh0, bh1);
                 }
             }
         }

@@ -3,7 +3,8 @@
 // One warp-specialised kernel, three instantiations (see GemmMode in kernels.h):
 //   warp 0    : TMA producer  - cp.async.bulk.tensor tiles (SWIZZLE_128B) into a ring of smem stages
 //   warps 1-4 : math + epilogue - each warp owns 32 rows of the 128-row tile: mma.sync TF32 (fp32 data, fp32
-//                               accumulate in registers, 3xTF32 for fp32-equivalent products) straight from the
+//                               accumulate in registers, 3xTF32 for fp32-equivalent products, or BF16 products of
+//                               operands rounded in registers; GemmParams::prec) straight from the
 //                               swizzled stages, then fused bias / ReLU / ReLU-mask / grad-accumulate / SGD and
 //                               coalesced global stores.  During the WGRAD main loop these warps also reduce
 //                               db = colsum(dZ) from the staged A tiles (exact fp32, no extra pass over dZ).
@@ -159,10 +160,12 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             mbar_wait(full_bar(s), ph);
             const uint32_t a_src = smem_base + s * stage_bytes;
             const uint32_t m_base = (uint32_t)(m_local - lane);
-            if (p.split)
-                warp_mma_kblock<NT, A_MN, B_MN, true>(acc, a_src, m_base, a_src + kATile, (uint32_t)nw0, nt, lane);
+            if (p.prec == PREC_3XTF32)
+                warp_mma_kblock<NT, A_MN, B_MN, PREC_3XTF32>(acc, a_src, m_base, a_src + kATile, (uint32_t)nw0, nt, lane);
+            else if (p.prec == PREC_BF16)
+                warp_mma_kblock<NT, A_MN, B_MN, PREC_BF16>(acc, a_src, m_base, a_src + kATile, (uint32_t)nw0, nt, lane);
             else
-                warp_mma_kblock<NT, A_MN, B_MN, false>(acc, a_src, m_base, a_src + kATile, (uint32_t)nw0, nt, lane);
+                warp_mma_kblock<NT, A_MN, B_MN, PREC_TF32>(acc, a_src, m_base, a_src + kATile, (uint32_t)nw0, nt, lane);
             if (MODE == GEMM_WGRAD && db_warp) {
                 // db[m] = sum over micro-batch rows of dZ[row, m], read from the staged A panels (exact fp32)
 #pragma unroll 8
@@ -548,8 +551,9 @@ static void finish_plan(GemmPlan* plan) {
 }
 
 const char* gemm_plan_fwd(GemmPlan* plan, const float* W, int ldw, const float* X, int ldx, float* Y, int ldy, int rows,
-                          int in, int out, const float* bias, int bias_stride, int relu, bool split) {
+                          int in, int out, const float* bias, int bias_stride, int relu, int prec) {
     *plan = GemmPlan{};
+    if (!prec_valid(prec)) return "unknown precision";
     plan->mode = GEMM_FWD;
     GemmParams& p = plan->p;
     p.m_total = out; p.n_total = rows; p.k_total = in;
@@ -558,14 +562,15 @@ const char* gemm_plan_fwd(GemmPlan* plan, const float* W, int ldw, const float* 
     if (const char* e = make_tmap(&plan->tmA, W, in, out, ldw, kBlockM)) return e;
     if (const char* e = make_tmap(&plan->tmB, X, in, rows, ldx, p.block_n)) return e;
     plan->tmC = plan->tmA;
-    p.split = split ? 1 : 0;
+    p.prec = prec;
     finish_plan(plan);
     return nullptr;
 }
 
 const char* gemm_plan_dgrad(GemmPlan* plan, const float* W, int ldw, const float* dZ, int lddz, float* dX, int lddx,
-                            int rows, int in, int out, const float* mask, int ldmask, bool split) {
+                            int rows, int in, int out, const float* mask, int ldmask, int prec) {
     *plan = GemmPlan{};
+    if (!prec_valid(prec)) return "unknown precision";
     plan->mode = GEMM_DGRAD;
     GemmParams& p = plan->p;
     p.m_total = in; p.n_total = rows; p.k_total = out;
@@ -574,15 +579,16 @@ const char* gemm_plan_dgrad(GemmPlan* plan, const float* W, int ldw, const float
     if (const char* e = make_tmap(&plan->tmA, W, in, out, ldw, 32)) return e;          // MN-major panels [32 k x 32 m]
     if (const char* e = make_tmap(&plan->tmB, dZ, out, rows, lddz, p.block_n)) return e;
     plan->tmC = plan->tmA;
-    p.split = split ? 1 : 0;
+    p.prec = prec;
     finish_plan(plan);
     return nullptr;
 }
 
 const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const float* X, int ldx, float* G, int ldg,
                             int rows, int in, int out, int accumulate, float* db, int db_stride, float* W, int ldw,
-                            const float* lr, int fuse_sgd, bool split, const SgdState& opt) {
+                            const float* lr, int fuse_sgd, int prec, const SgdState& opt) {
     *plan = GemmPlan{};
+    if (!prec_valid(prec)) return "unknown precision";
     plan->mode = GEMM_WGRAD;
     GemmParams& p = plan->p;
     p.m_total = out; p.n_total = in; p.k_total = rows;
@@ -604,7 +610,7 @@ const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const flo
     if (const char* e = make_tmap(&plan->tmC, fuse_sgd ? W : G, in, out, fuse_sgd ? ldw : ldg, kBlockM)) return e;
     if (const char* e = make_tmap(&plan->tmA, dZ, out, rows, lddz, 32)) return e;
     if (const char* e = make_tmap(&plan->tmB, X, in, rows, ldx, 32)) return e;
-    p.split = split ? 1 : 0;
+    p.prec = prec;
     finish_plan(plan);
     return nullptr;
 }

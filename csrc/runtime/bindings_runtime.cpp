@@ -239,7 +239,8 @@ public:
         c.training = geti("training", 1); c.use_graph = geti("use_graph", 1);
         c.dp_size = geti("dp_size", 1); c.dp_rank = geti("dp_rank", 0); c.dp_mode = geti("dp_mode", 0);
         c.in_dim = geti("in_dim", 784); c.out_dim = geti("out_dim", 10);
-        c.split = geti("split", 0);
+        c.prec = geti("prec", ssb::PREC_TF32);
+        TORCH_CHECK(ssb::prec_valid(c.prec), "PipeEngine: cfg['prec'] must be 0 (tf32), 1 (3xtf32) or 2 (bf16), got ", c.prec);
         c.momentum = cfg.contains("momentum") ? cfg["momentum"].cast<float>() : 0.f;
         c.weight_decay = cfg.contains("weight_decay") ? cfg["weight_decay"].cast<float>() : 0.f;
         c.nesterov = geti("nesterov", 0);

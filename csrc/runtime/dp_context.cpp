@@ -152,7 +152,7 @@ DpLayerParams DpContext::layer_params(int i) const {
     p.one_shot = g.one_shot;
     p.dbg = nullptr;
     p.helpers = 1;
-    p.split = 0;
+    p.prec = PREC_TF32;
     p.bulk_push = getenv("SSB_DP_BULK") ? atoi(getenv("SSB_DP_BULK")) : 1;   // TMA bulk copies to peer memory (verified on NVLink)
     p.stage_parity_stride = stage_parity_stride_;
     return p;

@@ -311,7 +311,7 @@ int PipeEngine::add_chain(int stream, int mu_base, int n_mu, bool do_fwd, bool d
         cp.dbg = chain_dbg_;
     }
     ChainPlan plan;
-    const char* err = chain_plan(&plan, cp, act_all_[0], act_ld_[0], cfg_.n_mu * cfg_.mb_rows, n_mu, cfg_.split != 0);
+    const char* err = chain_plan(&plan, cp, act_all_[0], act_ld_[0], cfg_.n_mu * cfg_.mb_rows, n_mu, cfg_.prec);
     if (err) throw std::runtime_error(std::string("PipeEngine chain plan: ") + err);
     chain_plans_.push_back(plan);
     Op op;
@@ -359,7 +359,7 @@ void PipeEngine::build(const std::vector<std::tuple<int, int, int>>& instrs) {
         const int nl = std::min(L_, (int)kChainMaxLayers);
         for (int l = 0; l < nl; ++l) { cl[l].in = cfg_.layers[l].in; cl[l].out = cfg_.layers[l].out; }
         chain_ok_ = L_ >= 1 && L_ <= kChainMaxLayers && !getenv("SSB_NO_CHAIN") &&
-                    chain_eligible(cl, L_, cfg_.mb_rows, cfg_.out_dim, cfg_.is_last != 0, cfg_.split != 0);
+                    chain_eligible(cl, L_, cfg_.mb_rows, cfg_.out_dim, cfg_.is_last != 0, cfg_.prec);
     }
     if (pp_ctx_) {
         // peer-memory transport: the neighbours write straight into my receive slots, which therefore live in the
@@ -582,7 +582,7 @@ void PipeEngine::plan_per_mubatch() {
                         const LayerSpec& ls = cfg_.layers[l - 1];
                         GemmPlan g;
                         check(gemm_plan_fwd(&g, Wl(l), ls.ld, act_[mu][l - 1], act_ld_[l - 1], act_[mu][l], act_ld_[l], mb,
-                                            ls.in, ls.out, Wl(l) + ls.in, ls.ld, ls.relu, cfg_.split != 0));
+                                            ls.in, ls.out, Wl(l) + ls.in, ls.ld, ls.relu, cfg_.prec));
                         add_gemm(g, s, l, mu);
                     }
                     if (!cfg_.training && last) {
@@ -628,7 +628,7 @@ void PipeEngine::plan_per_mubatch() {
                         GemmPlan g;
                         check(gemm_plan_wgrad(&g, dz_[mu][l], act_ld_[l], act_[mu][l - 1], act_ld_[l - 1], Gl(l), ls.ld, mb,
                                               ls.in, ls.out, first_write[l] ? 0 : 1, Gl(l) + ls.in, ls.ld, nullptr, 0, nullptr, 0,
-                                              cfg_.split != 0));
+                                              cfg_.prec));
                         add_gemm(g, w, l, mu);
                         first_write[l] = false;
                         if (final_bwd && cfg_.dp_mode == 1 && cfg_.dp_size > 1) {
@@ -672,7 +672,7 @@ void PipeEngine::plan_per_mubatch() {
                         GemmPlan g;
                         check(gemm_plan_wgrad(&g, dz_[mu][l], act_ld_[l], act_[mu][l - 1], act_ld_[l - 1], Gl(l), ls.ld, mb,
                                               ls.in, ls.out, first_write[l] ? 0 : 1, Gl(l) + ls.in, ls.ld, nullptr, 0, nullptr, 0,
-                                              cfg_.split != 0));
+                                              cfg_.prec));
                         add_gemm(g, w, l, mu);
                         first_write[l] = false;
                         if (final_bwd && cfg_.dp_mode == 1 && cfg_.dp_size > 1) {
@@ -688,7 +688,7 @@ void PipeEngine::plan_per_mubatch() {
                             const float* mask = (l >= 2 && cfg_.layers[l - 2].relu) ? act_[mu][l - 1] : nullptr;
                             GemmPlan g2;
                             check(gemm_plan_dgrad(&g2, Wl(l), ls.ld, dz_[mu][l], act_ld_[l], dz_[mu][l - 1], act_ld_[l - 1], mb, ls.in,
-                                                  ls.out, mask, act_ld_[l - 1], cfg_.split != 0));
+                                                  ls.out, mask, act_ld_[l - 1], cfg_.prec));
                             add_gemm(g2, s, l, mu);
                         }
                     }
@@ -733,7 +733,7 @@ void PipeEngine::plan_per_mubatch() {
                             const LayerSpec& ls = cfg_.layers[l - 1];
                             GemmPlan g;
                             check(gemm_plan_wgrad(&g, dz_all_[l], act_ld_[l], act_all_[l - 1], act_ld_[l - 1], Gl(l), ls.ld, rows_all, ls.in,
-                                                  ls.out, 0, Gl(l) + ls.in, ls.ld, Wl(l), ls.ld, lr_slot(), 1, cfg_.split != 0,
+                                                  ls.out, 0, Gl(l) + ls.in, ls.ld, Wl(l), ls.ld, lr_slot(), 1, cfg_.prec,
                                                   opt_for(l)));
                             grouped.push_back(g);
                         }
@@ -748,7 +748,7 @@ void PipeEngine::plan_per_mubatch() {
                         for (int l = L_; l >= 1; --l) {
                             const LayerSpec& ls = cfg_.layers[l - 1];
                             DpLLLayer ly{};
-                            ly.dZ = dz_all_[l]; ly.X = act_all_[l - 1]; ly.split = cfg_.split;
+                            ly.dZ = dz_all_[l]; ly.X = act_all_[l - 1]; ly.prec = cfg_.prec;
                             ly.lddz = act_ld_[l]; ly.ldx = act_ld_[l - 1]; ly.in = ls.in; ly.out = ls.out; ly.ldw = ls.ld; ly.w_offset = ls.offset;
                             lls.push_back(ly);
                         }
@@ -860,7 +860,7 @@ void PipeEngine::build_coalesced() {
             const LayerSpec& ls = cfg_.layers[l - 1];
             GemmPlan g;
             check(gemm_plan_fwd(&g, Wl(l), ls.ld, act_all_[l - 1], act_ld_[l - 1], act_all_[l], act_ld_[l], rows, ls.in, ls.out,
-                                Wl(l) + ls.in, ls.ld, ls.relu, cfg_.split != 0));
+                                Wl(l) + ls.in, ls.ld, ls.relu, cfg_.prec));
             add_gemm(g, 0, l);
         }
         if (!cfg_.training) {
@@ -908,14 +908,14 @@ void PipeEngine::build_coalesced() {
             const float* mask = cfg_.layers[l - 2].relu ? act_all_[l - 1] : nullptr;
             GemmPlan g;
             check(gemm_plan_dgrad(&g, Wl(l), ls.ld, dz_all_[l], act_ld_[l], dz_all_[l - 1], act_ld_[l - 1], rows, ls.in, ls.out,
-                                  mask, act_ld_[l - 1], cfg_.split != 0));
+                                  mask, act_ld_[l - 1], cfg_.prec));
             add_gemm(g, 0, l);
             ev_dg = emit_record(0);
         }
         if (fused_dp && ll_on) {
             DpLLLayer ly{};
             ly.dZ = dz_all_[l]; ly.X = act_all_[l - 1];
-            ly.split = cfg_.split;
+            ly.prec = cfg_.prec;
             ly.lddz = act_ld_[l]; ly.ldx = act_ld_[l - 1]; ly.in = ls.in; ly.out = ls.out; ly.ldw = ls.ld; ly.w_offset = ls.offset;
             if (gate_on_) {
                 // GEMM + reduce-scatter hop start when dz[l] is final; the in-place update of W_l additionally waits until
@@ -952,7 +952,7 @@ void PipeEngine::build_coalesced() {
                 lp.dbg = chain_dbg_ + 3 * 256 + 8 * l;
             }
             check(fused_dp_plan(&fp, dz_all_[l], act_ld_[l], act_all_[l - 1], act_ld_[l - 1], rows, lp, dp_ctx_->peers(), kFusedDpMaxCtas,
-                                cfg_.split != 0));
+                                cfg_.prec));
             dp_plans_.push_back(fp);
             Op fo;
             fo.kind = OP_FUSED_DP; fo.stream = sdp; fo.gemm = (int)dp_plans_.size() - 1; fo.layer = l;
@@ -967,7 +967,7 @@ void PipeEngine::build_coalesced() {
         }
         GemmPlan g;
         check(gemm_plan_wgrad(&g, dz_all_[l], act_ld_[l], act_all_[l - 1], act_ld_[l - 1], Gl(l), ls.ld, rows, ls.in, ls.out, 0,
-                              Gl(l) + ls.in, ls.ld, fuse ? Wl(l) : nullptr, ls.ld, lr_slot(), fuse ? 1 : 0, cfg_.split != 0,
+                              Gl(l) + ls.in, ls.ld, fuse ? Wl(l) : nullptr, ls.ld, lr_slot(), fuse ? 1 : 0, cfg_.prec,
                               fuse ? opt_for(l) : SgdState{}));
         if (group_wgrad) {                                  // launched together after the loop
             grouped.push_back(g);

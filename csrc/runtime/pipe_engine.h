@@ -91,7 +91,7 @@ struct EngineConfig {
     int dp_mode = 0;        // 0 = none/fused-sgd (dp=1), 1 = NCCL all-reduce + SGD, 2 = fused in-kernel reduction,
                             // 3 = NVLS: one kernel reduces the gradient arena in the switch, applies SGD, multicasts W
     int in_dim = 784, out_dim = 10;
-    int split = 0;          // 1 = fp32-equivalent tensor-core products (3xTF32), 0 = single-pass TF32
+    int prec = 0;           // Precision of the tensor-core products (precision.h): 0 TF32, 1 3xTF32, 2 BF16
     // SGD beyond lr (torch.optim.SGD, dampening 0).  All zero = plain SGD and the stateless kernels.  Momentum needs
     // the engine's momentum arena (same layout as the weights); under the in-kernel DP reductions (dp_mode 2, 3) each
     // replica updates only the entries it owns (layer_protocols()).

@@ -59,12 +59,16 @@ def _bias_arg(bias, out_dims):
 # ------------------------------------------------------------------ GEMMs
 # precision: "tf32" = one TF32 tensor-core pass (operands truncated to 10 mantissa bits);
 #            "fp32" = 3xTF32: lo parts (x - trunc(x)) of both operands, derived in the kernel, three MMAs per k-slice,
-#            error ~2^-20.
+#            error ~2^-20;
+#            "bf16" = operands rounded to bf16 (nearest even) in registers, one BF16 MMA per 16 k, fp32 accumulation.
+# Other names raise ValueError (functional.precision_code).
 PRECISION = "fp32"
 
 
-def _split(precision):
-    return (precision or PRECISION) in ("fp32", "fp32x3", "3xtf32")
+def _prec(precision):
+    from .functional import precision_code
+
+    return precision_code(precision or PRECISION)
 
 
 def _act_code(activation):
@@ -91,7 +95,7 @@ def linear_fwd(x, weight, bias=None, relu=False, out=None, precision=None, k_spl
     rows, out_dims = x.size(0), weight.size(0)
     y = out if out is not None else empty_padded(rows, out_dims, x.device)
     b, bstride = _bias_arg(bias, out_dims)
-    _C.linear_fwd(x, weight, b, bstride, bool(relu), y, _split(precision), int(k_splits), _act_code(activation), gate,
+    _C.linear_fwd(x, weight, b, bstride, bool(relu), y, _prec(precision), int(k_splits), _act_code(activation), gate,
                   _drop_arg(dropout))
     return y
 
@@ -102,7 +106,7 @@ def linear_dgrad(dz, weight, mask=None, out=None, precision=None, k_splits=0, ac
     dz, weight = as_tma(dz), as_tma(weight)
     dx = out if out is not None else empty_padded(dz.size(0), weight.size(1), dz.device)
     m = None if mask is None else as_tma(mask)
-    _C.linear_dgrad(dz, weight, m, dx, _split(precision), int(k_splits), _act_code(activation), _drop_arg(dropout))
+    _C.linear_dgrad(dz, weight, m, dx, _prec(precision), int(k_splits), _act_code(activation), _drop_arg(dropout))
     return dx
 
 
@@ -114,7 +118,7 @@ def linear_wgrad(dz, x, grad_w, accumulate=False, grad_b=None, weight=None, lr=0
     number or a one-element fp32 CUDA tensor (see ``_lr_arg``)."""
     dz, x = as_tma(dz), as_tma(x)
     b, bstride = _bias_arg(grad_b, dz.size(1))
-    _C.linear_wgrad(dz, x, grad_w, bool(accumulate), b, bstride, weight, _lr_arg(lr), bool(fuse_sgd), _split(precision),
+    _C.linear_wgrad(dz, x, grad_w, bool(accumulate), b, bstride, weight, _lr_arg(lr), bool(fuse_sgd), _prec(precision),
                     velocity, float(momentum), float(weight_decay), bool(nesterov))
     return grad_w
 

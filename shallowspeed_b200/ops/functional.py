@@ -173,6 +173,21 @@ def dropout_ref(a: torch.Tensor, keep: torch.Tensor, scale: float) -> torch.Tens
 
 
 # ----------------------------------------------------------------------------
+# tensor-core precision of the native GEMMs: the names a user passes and their codes in the native runtime
+# (csrc/kernels/precision.h: Precision).  fp32 (the default) = 3xTF32, fp32-equivalent products; tf32 = one TF32 pass;
+# bf16 = operands rounded to bf16 (nearest even) in registers, fp32 accumulation.  Storage is fp32 in every mode.
+# ----------------------------------------------------------------------------
+PRECISION_CODES = {"fp32": 1, "fp32x3": 1, "3xtf32": 1, "tf32": 0, "bf16": 2}
+
+
+def precision_code(precision) -> int:
+    """The native code of a precision name, or ValueError for a name that is not in ``PRECISION_CODES``."""
+    if not isinstance(precision, str) or precision not in PRECISION_CODES:
+        raise ValueError(f"unknown precision {precision!r}: expected one of {sorted(PRECISION_CODES)}")
+    return PRECISION_CODES[precision]
+
+
+# ----------------------------------------------------------------------------
 # hidden-layer activations: f and the gate f' in one pass, the same math as csrc/kernels/ptx.cuh: act_fwd
 # ----------------------------------------------------------------------------
 # the activations of the hidden Linears and their codes in the native runtime (csrc/kernels/activation.h: ActKind)

@@ -13,7 +13,7 @@ from typing import Optional
 
 import torch
 
-from ..ops.functional import ACTIVATION_CODES, LOSS_CODES
+from ..ops.functional import ACTIVATION_CODES, LOSS_CODES, precision_code
 from .comm import Comm, ProcessGrid, SelfComm, TorchComm
 from .instructions import encode, flatten
 from .schedules import Schedule
@@ -220,6 +220,7 @@ class NativeWorker:
         self.pipeline_depth = self.pp_comm.Get_size()
         self.model, self.dataset, self.optimizer = model, dataset, optimizer
         self.use_graph, self.precision = use_graph, precision
+        precision_code(precision)   # ValueError now for a name the engine does not know
         self.validate_schedules = validate_schedules
         # pipeline boundaries: one-sided pushes into the neighbour's memory (None = "peer") or NCCL send/recv ("nccl")
         self.pp_transport = pp_transport or "peer"
@@ -293,7 +294,7 @@ class NativeWorker:
                    global_batch=m.batch_size, lr=float(self.lr), training=int(training), use_graph=int(self.use_graph),
                    dp_size=self.dp_comm.Get_size(), dp_rank=self.dp_comm.Get_rank(),
                    dp_mode=DP_MODE[self.dp_mode] if training else 0, in_dim=m.in_dim, out_dim=m.out_dim,
-                   split=1 if self.precision in ("fp32", "fp32x3", "3xtf32") else 0)
+                   prec=precision_code(self.precision))
         momentum = None
         if training and (self.momentum != 0.0 or self.weight_decay != 0.0):
             cfg.update(momentum=self.momentum, weight_decay=self.weight_decay, nesterov=int(self.nesterov))

@@ -120,8 +120,9 @@ def build_parser():
                    help="native engine, stage boundaries: one-sided pushes into the neighbour's memory over NVLink with "
                         "epoch flags (peer, the default) or NCCL send/recv")
     p.add_argument("--no-graph", action="store_true", help="native engine: do not capture the step in a CUDA graph")
-    p.add_argument("--precision", choices=["tf32", "fp32"], default="fp32",
-                   help="tensor-core math: fp32 = 3xTF32 split (fp32-equivalent, the reference's contract); tf32 = single pass")
+    p.add_argument("--precision", choices=["tf32", "fp32", "bf16"], default="fp32",
+                   help="tensor-core math: fp32 = 3xTF32 split (fp32-equivalent, the reference's contract); tf32 = single pass; "
+                        "bf16 = BF16 products of operands rounded in registers, fp32 accumulation (storage stays fp32)")
     p.add_argument("--watchdog-s", type=float, default=None,
                    help="native engine: abort (and tear the NCCL communicators down) if an epoch's work is still in "
                         "flight after this many seconds; default: SSB_WATCHDOG_S or disabled")

@@ -231,6 +231,24 @@ cudaError_t launch_gate_mul(float* g, int ldg, const float* gamma, int ldgam, in
     return cudaGetLastError();
 }
 
+__global__ void gate_mul_to_kernel(float* __restrict__ out, int ldo, const float* __restrict__ g, int ldg,
+                                   const float* __restrict__ gamma, int ldgam, int rows, int cols) {
+    const long total = (long)rows * cols;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int r = (int)(i / cols), c = (int)(i % cols);
+        out[(size_t)r * ldo + c] = g[(size_t)r * ldg + c] * gamma[(size_t)r * ldgam + c];
+    }
+}
+cudaError_t launch_gate_mul_to(float* out, int ldo, const float* g, int ldg, const float* gamma, int ldgam, int rows, int cols,
+                               cudaStream_t stream) {
+    const long total = (long)rows * cols;
+    int blocks = (int)((total + 255) / 256);
+    if (blocks > 132 * 8) blocks = 132 * 8;
+    if (blocks < 1) blocks = 1;
+    gate_mul_to_kernel<<<blocks, 256, 0, stream>>>(out, ldo, g, ldg, gamma, ldgam, rows, cols);
+    return cudaGetLastError();
+}
+
 __global__ void act_fwd_kernel(int kind, const float* __restrict__ z, float* __restrict__ y, float* __restrict__ gamma,
                                long n) {
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {

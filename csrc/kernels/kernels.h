@@ -89,6 +89,17 @@ struct GemmParams {
     // DGRAD with mask reads the mask as the previous layer's gate and multiplies by it.  Last, like drop.
     int act_kind;
     float* gate;
+    // Residual form (tc_gemm_res_kernel), set by a plan with identity skips.  res: the FWD with relu / DGRAD with mask runs
+    // gated for every act_kind, ReLU included (its gate is 1[z > 0] * keep * s), and the skip fields apply (both nullable):
+    //   FWD:   out = skip[n * ldskip + m] + f(z)          (skip: the layer's input X)
+    //   DGRAD: x = W^T dZ + skip[n * ldskip + m]          (skip: the gradient of the layer's output)
+    //          gpre[n * ldgpre + m] = x, then out = x * mask   (gpre: the previous layer is residual and needs x as ITS skip)
+    // Last, like drop and act_kind.
+    int res;
+    const float* skip;
+    int ldskip;
+    float* gpre;
+    int ldgpre;
 };
 
 struct GemmPlan {          // a fully prepared launch (tensor maps are 128 B each)
@@ -122,8 +133,12 @@ const char* gemm_plan_enable_splitk(GemmPlan* plan, int k_splits, float* workspa
 cudaError_t gemm_launch(const GemmPlan& plan, cudaStream_t stream);
 // the plan runs the dropout variant: a FWD with relu or a DGRAD with mask, and plan.p.drop on
 bool gemm_drops(const GemmPlan& plan);
-// the plan runs the gated variant: a FWD with relu or a DGRAD with mask, and a smooth plan.p.act_kind
+// the plan runs the gated variant: a FWD with relu or a DGRAD with mask, and a smooth plan.p.act_kind (or the residual form)
 bool gemm_gated(const GemmPlan& plan);
+// the plan runs the residual form (GemmParams::res): tc_gemm_res_kernel
+bool gemm_residual(const GemmPlan& plan);
+// the plan adds an identity skip (GemmParams::skip) or stores the pre-gate gradient (GemmParams::gpre)
+bool gemm_skips(const GemmPlan& plan);
 // Grouped launch of several WGRAD plans (different layers) as ONE grid: a device table holds one entry per CTA.  Only
 // the GEMMs of chain-eligible stages are grouped (out <= 128, any in); they run on narrow tiles of 32 output features x
 // 32 input columns with the full K (rows) in one CTA, instead of the per-layer kernel's 128 x 64.
@@ -314,6 +329,14 @@ struct ChainParams {
     // none.  Last, for the same reason as loss_kind.
     int act_kind;
     float* gate[kChainMaxLayers + 1];
+    // Residual model (selects the RES instantiation, always with GATE: every activated layer is gated, ReLU included).
+    // res_mask bit l - 1: layer l is residual, a = x + f(z) (in == out); its dgrad adds g_l = dL/da_l before the gate of
+    // layer l - 1.  gout: the received gradient g_L of a residual last layer (backward-only launch of a non-last stage),
+    // which the staging gates into dz[L] and the dgrad of layer L adds as its skip gradient; nullptr otherwise.  Last,
+    // for the same reason as loss_kind.
+    int res;
+    uint32_t res_mask;
+    const float* gout;
 };
 struct ChainPlan {
     ChainParams p;
@@ -360,6 +383,9 @@ cudaError_t launch_relu_mask_scaled(float* g, int ldg, const float* y, int ldy, 
 cudaError_t launch_relu_fwd(const float* x, float* y, long n, cudaStream_t stream);
 // stage-boundary backward of a smooth activation: g[r, c] *= gamma[r, c] (gamma already holds keep * s under dropout)
 cudaError_t launch_gate_mul(float* g, int ldg, const float* gamma, int ldgam, int rows, int cols, cudaStream_t stream);
+// out = g * gamma out of place (a residual last layer keeps the received gradient g as the skip gradient of its dgrad)
+cudaError_t launch_gate_mul_to(float* out, int ldo, const float* g, int ldg, const float* gamma, int ldgam, int rows, int cols,
+                               cudaStream_t stream);
 // stand-alone smooth activation over n dense elements (ptx.cuh: act_fwd): y = f(z), gamma = f'(z)
 cudaError_t launch_act_fwd(int kind, const float* z, float* y, float* gamma, long n, cudaStream_t stream);
 // y = a * x + b * t  (mse grad: a=2/B, b=-2/B)

@@ -115,6 +115,8 @@ const char* chain_plan(ChainPlan* plan, const ChainParams& params, const float* 
     // a cluster launch whose layer 1 has more than 4 k-blocks runs it on P = 2 CTAs per feature slice (k-split)
     const int P = C > 1 && p.do_fwd && (p.layers[0].in + (int)kBlockK - 1) / (int)kBlockK > 4 ? 2 : 1;
     p.ksplit = P;
+    // a k-split layer 1 has more than 128 inputs and at most 128 outputs: never residual, and the split has no skip form
+    if (P > 1 && (p.res_mask & 1u)) return "chain_plan: a k-split layer 1 cannot be residual";
     std::vector<CUtensorMap> host(2 * L + 1);
     for (int l = 0; l < L; ++l) {
         const ChainLayer& ly = p.layers[l];

@@ -169,9 +169,19 @@ __device__ __forceinline__ unsigned long long gtime() {
 // epilogues apply f (ptx.cuh: act_fwd) instead of the ReLU and store the gate f'(z) (* keep * s under DROP) to
 // gate[l] next to the global copy of act[l] (not in inference plans: gate[l] == nullptr); the dZ_L staging and the dgrad
 // epilogues multiply by the gate where they test the stored activation, which leaves nothing for DROP to scale there.
-template <int PREC, bool FOLD, int NTW, bool CLUSTER, bool CE, bool DROP, bool GATE>
+// RES: a residual model (ChainParams::res), only together with GATE: every activated layer is gated, ReLU included
+// (ptx.cuh: act_fwd_any), and the layers in res_mask carry an identity skip.  Because such a layer has in == out, the
+// math warp that owns a fragment (feature, row) of its output owns the same fragment of its input tile and of the
+// gradients on either side of it, in both forms (chain_tile_lo; warp (q, half)):
+//   * forward: a = x + f(z), x read back from the resident input tile (abuf) in shared memory - the stage's first layer
+//     reads it from act[0] (the staged or received input) instead, since its input tile may be in ring slots already
+//     reused.  See exchange for why the input tile is still intact when the epilogue reads it;
+//   * dgrad of layer l: W_l^T dz_l + g_l before the gate of layer l - 1, where g_l (the pre-gate sum of the dgrad of layer
+//     l + 1) stayed in the registers of the warp that produced it; a backward-only launch reads g_L from gout.
+template <int PREC, bool FOLD, int NTW, bool CLUSTER, bool CE, bool DROP, bool GATE, bool RES>
 __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParams p) {
     static_assert(!(FOLD && CLUSTER), "folded pipeline launches run one CTA per micro-batch");
+    static_assert(!RES || GATE, "residual models run gated");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t smem_base = (raw + 1023u) & ~1023u;
@@ -328,7 +338,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         // GATE: a = f(z) and its gate g for feature f of row n in local layer l, both dropped like drop_fwd under DROP
         auto gate_fwd = [&](float z, int l, int f, int n, float& g) {
             float a;
-            act_fwd(p.act_kind, z, a, g);
+            if constexpr (RES) act_fwd_any(p.act_kind, z, a, g);
+            else act_fwd(p.act_kind, z, a, g);
             if constexpr (DROP) {
                 const uint32_t sample = (uint32_t)((row0 + n) * p.drop.dp + p.drop.rank);
                 const bool keep = dropout_keep(p.drop, (uint32_t)(p.drop.layer + l - 1), drop_step, (uint32_t)f, sample);
@@ -336,6 +347,25 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 g = keep ? g * p.drop.scale : 0.f;
             }
             return a;
+        };
+        // RES: layer l carries a skip; the skip input x of element (row n, feature f) of layer l, read from the input tile
+        // `src` (l >= 2) or from act[0] (l == 1, rows of this micro-batch only); the received g_L of element (n, f)
+        auto is_res = [&](int l) { return RES && l >= 1 && l <= L && ((p.res_mask >> (l - 1)) & 1u) != 0u; };
+        auto skip_in = [&](int l, uint32_t src, int n, int f) {
+            float x = 0.f;
+            if (l == 1) {
+                if (n < p.mb_rows)
+                    asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(x) : "l"(p.act[0] + (int64_t)(row0 + n) * p.act_ld[0] + f));
+            } else {
+                x = *reinterpret_cast<const float*>(smem_gen + (src - smem_base) + act_smem_off(n, f, b_bytes));
+            }
+            return x;
+        };
+        auto g_recv = [&](int n, int f) {
+            float x = 0.f;
+            if (n < p.mb_rows)
+                asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(x) : "l"(p.gout + (int64_t)(row0 + n) * p.act_ld[L] + f));
+            return x;
         };
         int wbuf = 0;                                        // activation buffer the NEXT epilogue writes
         uint32_t recv_phase = 0u;                            // CLUSTER: parity of recv_bar(b) in bit b
@@ -480,6 +510,11 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
         // with abuf b before any peer writes into it.  The same chain puts every byte of a tile on recv_bar(b) in the
         // phase that is awaited for it, and every store into this CTA has landed before it reaches the cluster barrier
         // at the end of the kernel.  The stores read registers, so my buffers carry no outgoing copy to wait for.
+        // RES: the forward epilogue of a residual layer reads its skip input from the tile it consumed (abuf b ^ 1 when
+        // it writes abuf b).  Nothing overwrites that tile before every warp of every CTA has read it: my warps write it
+        // again only in the epilogue after next, behind the publish of this tile, which each of them reaches after its
+        // reads; a peer writes it only after its next GEMM, which waits for all my bytes of this tile, and each of my
+        // warps sends its part only after its own reads.
         auto exchange = [&](int b, bool sender, int n0, int rows, int ch0, int lcpr) {
             if (sender) {
                 __syncwarp();                                // the warp's st.shared of its block -> its lanes' reads
@@ -554,6 +589,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                 else buf = 0;                                // layer 1 writes abuf 0
                 if (p.sync_debug) asm volatile("bar.sync 2, 256;" ::: "memory");   // racecheck aid, see kernels.h
                 const uint32_t dst = abuf0 + wbuf * abuf_bytes;
+                const uint32_t src = abuf0 + (wbuf ^ 1) * abuf_bytes;   // RES, l >= 2: the tile this layer consumed
+                const bool res_l = is_res(l);
                 float* __restrict__ gout = p.act[l] + (int64_t)row0 * p.act_ld[l];
                 float* __restrict__ ggout = nullptr;         // GATE: where this layer's gates go (none: inference)
                 if constexpr (GATE) { if (ly.relu && p.gate[l] != nullptr) ggout = p.gate[l] + (int64_t)row0 * p.act_ld[l]; }
@@ -574,6 +611,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                                     if (ly.relu) x = fmaxf(x, 0.f);
                                     if constexpr (DROP) { if (ly.relu) x = drop_fwd(x, l, t_feat(r), t_row(j, r)); }
                                 }
+                                if constexpr (RES) { if (res_l && t_feat(r) < ly.out) x += skip_in(l, src, t_row(j, r), t_feat(r)); }
                                 x = t_feat(r) < ly.out ? x : 0.f;
                                 tacc[0][j][r] = x;
                                 st_tile(dst, t_row(j, r), t_feat(r), x);
@@ -621,6 +659,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                                 if (ly.relu) x = fmaxf(x, 0.f);
                                 if constexpr (DROP) { if (ly.relu) x = drop_fwd(x, l, m, c + j); }
                             }
+                            if constexpr (RES) { if (res_l && m_ok) x += skip_in(l, src, c + j, m); }
                             x = m_ok ? x : 0.f;
                             const int n = c + j;
                             st_tile(dst, n, m, x);
@@ -829,10 +868,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             const uint32_t dst = abuf0 + wbuf * abuf_bytes;
             float* __restrict__ g = p.dz[L] + (int64_t)row0 * p.act_ld[L];
             const float* __restrict__ y = (GATE ? p.gate[L] : p.act[L]) + (int64_t)row0 * p.act_ld[L];
+            // RES, residual layer L: the received gradient is in gout (kept: the dgrad of layer L adds it), dz[L] is its own
+            const float* __restrict__ gin = (RES && p.gout != nullptr) ? p.gout + (int64_t)row0 * p.act_ld[L] : g;
             for (int n = c_lo; n < c_hi && epi; ++n) {
                 float x = 0.f;
                 if (m_ok && n < p.mb_rows) {
-                    asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(x) : "l"(g + (int64_t)n * p.act_ld[L] + m));   // may be peer-written
+                    asm volatile("ld.global.cg.f32 %0, [%1];" : "=f"(x) : "l"(gin + (int64_t)n * p.act_ld[L] + m));   // may be peer-written
                     if constexpr (GATE) {
                         if (ly.relu) x *= y[(int64_t)n * p.act_ld[L] + m];   // the gate holds keep * s already
                     } else {
@@ -848,11 +889,25 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
             wbuf ^= 1;
         }
         if (p.do_bwd && !helper) {
+            // RES: g_l of this warp's fragments, the pre-gate output of the previous dgrad (cluster: t_g; one CTA: r_g per
+            // 16-row chunk), carried into the dgrad of layer l when layer l is residual
+            float t_g[NTW / 2][4], r_g[NTW / 2][16];
+            if constexpr (RES) {
+#pragma unroll
+                for (int j = 0; j < NTW / 2; ++j) {
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) t_g[j][r] = 0.f;
+#pragma unroll
+                    for (int r = 0; r < 16; ++r) r_g[j][r] = 0.f;
+                }
+            }
             // the loss head / boundary loader wrote dZ_L into the buffer after the last forward output
             for (int l = L; l >= bwd_lo; --l) {
                 const ChainLayer& ly = p.layers[l - 1];
                 const bool m_ok = m < ly.in;                 // output feature of dgrad = input feature of layer l
                 const bool mask_on = (l >= 2) && p.layers[l - 2].relu;
+                const bool res_l = is_res(l), res_prev = is_res(l - 1);   // RES: add g_l / keep g_{l-1}
+                const bool g_from_gout = RES && res_l && l == L && p.gout != nullptr;   // g_L: the received gradient
                 // the mask of layer l - 1: its stored output (ReLU), or its gate (GATE: multiplied in, 1 where no mask)
                 const float* __restrict__ yprev = (GATE ? p.gate[l - 1] : p.act[l - 1]) + (int64_t)row0 * p.act_ld[l - 1];
                 float* __restrict__ gprev = p.dz[l - 1] + (int64_t)row0 * p.act_ld[l - 1];
@@ -866,6 +921,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         for (int r = 0; r < 4; ++r) {
                             const int n = t_row(j, r), f = t_feat(r);
                             t_mk[j][r] = (j < tnt && mask_on && f < ly.in && n < p.mb_rows) ? yprev[(int64_t)n * p.act_ld[l - 1] + f] : 1.f;
+                            if constexpr (RES) { if (g_from_gout) t_g[j][r] = (j < tnt && f < ly.in) ? g_recv(n, f) : 0.f; }
                         }
                     run_gemm_tiles((ly.out + (int)kBlockK - 1) / (int)kBlockK, true, false, abuf0 + buf * abuf_bytes, idle(ly.in));
                     buf ^= 1;
@@ -878,7 +934,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
 #pragma unroll
                             for (int r = 0; r < 4; ++r) {
                                 float x;
-                                if constexpr (GATE) {
+                                if constexpr (RES) {
+                                    float pre = tacc[0][j][r];
+                                    if (res_l) pre += t_g[j][r];
+                                    if (res_prev) t_g[j][r] = pre;
+                                    x = pre * t_mk[j][r];
+                                } else if constexpr (GATE) {
                                     x = tacc[0][j][r] * t_mk[j][r];
                                 } else {
                                     x = (t_mk[j][r] > 0.f) ? tacc[0][j][r] : 0.f;
@@ -936,7 +997,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                     for (int j = 0; j < 16; ++j) {
                         const int n = c + j;
                         float x;
-                        if constexpr (GATE) {
+                        if constexpr (RES) {
+                            float pre = v[j];
+                            if (res_l) pre += g_from_gout ? (m_ok ? g_recv(n, m) : 0.f) : r_g[ch][j];
+                            if (res_prev) r_g[ch][j] = pre;
+                            x = pre * mk[j];
+                        } else if constexpr (GATE) {
                             x = v[j] * mk[j];
                         } else {
                             x = (mk[j] > 0.f) ? v[j] : 0.f;
@@ -982,25 +1048,30 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
 
 // =========================================================================== host side: the launches of one precision
 // Every translation unit that includes this file instantiates the kernel for the precisions it dispatches:
-// mlp_chain.cu PREC_TF32 and PREC_3XTF32, mlp_chain_bf16.cu PREC_BF16, so that neither grows the longest compile.
-template <int PREC, int NTW, bool CE, bool DROP, bool GATE>
+// mlp_chain.cu PREC_TF32 and PREC_3XTF32, mlp_chain_bf16.cu PREC_BF16, mlp_chain_res.cu the RES forms of all three, so
+// that none grows the longest compile.
+
+// mlp_chain_res.cu: configuration and launch of the RES instantiations of one precision
+cudaError_t chain_configure_res(int prec);
+cudaError_t chain_launch_res(const ChainPlan& plan, int ntw, bool fold, cudaStream_t stream);
+template <int PREC, int NTW, bool CE, bool DROP, bool GATE, bool RES = false>
 static cudaError_t chain_configure_ntw() {
     cudaError_t e;
     const int smem = 227 * 1024;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<PREC, false, NTW, false, CE, DROP, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<PREC, true, NTW, false, CE, DROP, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    return cudaFuncSetAttribute(mlp_chain_kernel<PREC, false, NTW, true, CE, DROP, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<PREC, false, NTW, false, CE, DROP, GATE, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<PREC, true, NTW, false, CE, DROP, GATE, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
+    return cudaFuncSetAttribute(mlp_chain_kernel<PREC, false, NTW, true, CE, DROP, GATE, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
 }
 
-template <int PREC, bool DROP, bool GATE>
+template <int PREC, bool DROP, bool GATE, bool RES = false>
 static cudaError_t chain_configure_kind() {
     cudaError_t e;
-    if ((e = chain_configure_ntw<PREC, 2, false, DROP, GATE>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<PREC, 4, false, DROP, GATE>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<PREC, 8, false, DROP, GATE>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<PREC, 2, true, DROP, GATE>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<PREC, 4, true, DROP, GATE>()) != cudaSuccess) return e;
-    return chain_configure_ntw<PREC, 8, true, DROP, GATE>();
+    if ((e = chain_configure_ntw<PREC, 2, false, DROP, GATE, RES>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<PREC, 4, false, DROP, GATE, RES>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<PREC, 8, false, DROP, GATE, RES>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<PREC, 2, true, DROP, GATE, RES>()) != cudaSuccess) return e;
+    if ((e = chain_configure_ntw<PREC, 4, true, DROP, GATE, RES>()) != cudaSuccess) return e;
+    return chain_configure_ntw<PREC, 8, true, DROP, GATE, RES>();
 }
 
 template <int PREC>
@@ -1009,11 +1080,12 @@ static cudaError_t chain_configure_prec() {
     if ((e = chain_configure_kind<PREC, false, false>()) != cudaSuccess) return e;
     if ((e = chain_configure_kind<PREC, true, false>()) != cudaSuccess) return e;
     if ((e = chain_configure_kind<PREC, false, true>()) != cudaSuccess) return e;
-    return chain_configure_kind<PREC, true, true>();
+    if ((e = chain_configure_kind<PREC, true, true>()) != cudaSuccess) return e;
+    return chain_configure_res(PREC);
 }
 
 // grid = micro-batches x plan.cluster x plan.ksplit, cluster dims (plan.cluster x plan.ksplit, 1, 1)
-template <int PREC, int NTW, bool CE, bool DROP, bool GATE>
+template <int PREC, int NTW, bool CE, bool DROP, bool GATE, bool RES>
 static cudaError_t chain_launch_cluster(const ChainPlan& plan, cudaStream_t stream) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)plan.grid);
@@ -1027,24 +1099,24 @@ static cudaError_t chain_launch_cluster(const ChainPlan& plan, cudaStream_t stre
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, mlp_chain_kernel<PREC, false, NTW, true, CE, DROP, GATE>, plan.p);
+    return cudaLaunchKernelEx(&cfg, mlp_chain_kernel<PREC, false, NTW, true, CE, DROP, GATE, RES>, plan.p);
 }
 
-template <int PREC, int NTW, bool CE, bool DROP, bool GATE>
+template <int PREC, int NTW, bool CE, bool DROP, bool GATE, bool RES>
 static cudaError_t chain_launch_ntw(const ChainPlan& plan, bool fold, cudaStream_t stream) {
-    if (plan.cluster > 1) return chain_launch_cluster<PREC, NTW, CE, DROP, GATE>(plan, stream);
+    if (plan.cluster > 1) return chain_launch_cluster<PREC, NTW, CE, DROP, GATE, RES>(plan, stream);
     if (fold)
-        mlp_chain_kernel<PREC, true, NTW, false, CE, DROP, GATE><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.p);
+        mlp_chain_kernel<PREC, true, NTW, false, CE, DROP, GATE, RES><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.p);
     else
-        mlp_chain_kernel<PREC, false, NTW, false, CE, DROP, GATE><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.p);
+        mlp_chain_kernel<PREC, false, NTW, false, CE, DROP, GATE, RES><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.p);
     return cudaSuccess;
 }
 
-template <int PREC, bool DROP, bool GATE>
+template <int PREC, bool DROP, bool GATE, bool RES = false>
 static cudaError_t chain_launch_kind(const ChainPlan& plan, int ntw, bool ce, bool fold, cudaStream_t stream) {
-    if (ntw == 2) return ce ? chain_launch_ntw<PREC, 2, true, DROP, GATE>(plan, fold, stream) : chain_launch_ntw<PREC, 2, false, DROP, GATE>(plan, fold, stream);
-    if (ntw == 4) return ce ? chain_launch_ntw<PREC, 4, true, DROP, GATE>(plan, fold, stream) : chain_launch_ntw<PREC, 4, false, DROP, GATE>(plan, fold, stream);
-    return ce ? chain_launch_ntw<PREC, 8, true, DROP, GATE>(plan, fold, stream) : chain_launch_ntw<PREC, 8, false, DROP, GATE>(plan, fold, stream);
+    if (ntw == 2) return ce ? chain_launch_ntw<PREC, 2, true, DROP, GATE, RES>(plan, fold, stream) : chain_launch_ntw<PREC, 2, false, DROP, GATE, RES>(plan, fold, stream);
+    if (ntw == 4) return ce ? chain_launch_ntw<PREC, 4, true, DROP, GATE, RES>(plan, fold, stream) : chain_launch_ntw<PREC, 4, false, DROP, GATE, RES>(plan, fold, stream);
+    return ce ? chain_launch_ntw<PREC, 8, true, DROP, GATE, RES>(plan, fold, stream) : chain_launch_ntw<PREC, 8, false, DROP, GATE, RES>(plan, fold, stream);
 }
 
 // the launch of a validated plan (chain_launch checks the loss and activation kinds); ntw: chain_ntw(p.n_pad)
@@ -1052,6 +1124,7 @@ template <int PREC>
 static cudaError_t chain_launch_prec(const ChainPlan& plan, int ntw, bool fold, cudaStream_t stream) {
     const ChainParams& p = plan.p;
     const bool ce = p.loss_kind == LOSS_CROSS_ENTROPY, drop = p.drop.on();
+    if (p.res) return chain_launch_res(plan, ntw, fold, stream);   // a residual model: gated for every activation kind
     if (!act_smooth(p.act_kind))
         return drop ? chain_launch_kind<PREC, true, false>(plan, ntw, ce, fold, stream) : chain_launch_kind<PREC, false, false>(plan, ntw, ce, fold, stream);
     return drop ? chain_launch_kind<PREC, true, true>(plan, ntw, ce, fold, stream) : chain_launch_kind<PREC, false, true>(plan, ntw, ce, fold, stream);

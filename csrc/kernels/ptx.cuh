@@ -452,6 +452,17 @@ __device__ __forceinline__ void act_fwd(int kind, float z, float& a, float& g) {
         g = 1.f - t * t;
     }
 }
+// act_fwd for every ActKind, ReLU included: a = max(z, 0) and g = 1[z > 0].  The residual kernels store the gate of a
+// ReLU layer too (its output x + relu(z) is no longer its own mask); the smooth-only act_fwd stays as the gated kernels
+// compile it.
+__device__ __forceinline__ void act_fwd_any(int kind, float z, float& a, float& g) {
+    if (kind == ACT_RELU) {
+        a = fmaxf(z, 0.f);
+        g = z > 0.f ? 1.f : 0.f;
+    } else {
+        act_fwd(kind, z, a, g);
+    }
+}
 
 // ------------------------------------------------------------------ training-set shuffling
 // Dataset row held by position q < n in epoch `epoch` (ShuffleSpec): a 6-round balanced Feistel network on w bits (w the

@@ -54,7 +54,11 @@ static constexpr int kGroupMinCtas = 3;                 // CTAs per SM the group
 // GATE (FWD with relu / DGRAD with mask, a smooth GemmParams::act_kind): the FWD applies f (ptx.cuh: act_fwd) instead of the
 // ReLU and stores the gate f'(z) (* keep * s under DROP) to GemmParams::gate; the DGRAD multiplies by the mask, which
 // is the previous layer's gate (its dropout scale is inside).  The same kind of switch.
-template <int MODE, bool SPLITK, bool STATEFUL = false, int BM = (int)kBlockM, bool DROP = false, bool GATE = false>
+// RES (with GATE; FWD / DGRAD, GemmParams::res): the residual form.  act_fwd_any applies ReLU as a gated kind too; the FWD
+// adds the skip input after the activation, the DGRAD adds the skip gradient before the mask and stores that pre-mask sum
+// to gpre.  The same kind of switch: the other instantiations compile as they did without it.
+template <int MODE, bool SPLITK, bool STATEFUL = false, int BM = (int)kBlockM, bool DROP = false, bool GATE = false,
+          bool RES = false>
 __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
                                              const GemmParams& p, const int bx, const int by, const int bz) {
     constexpr bool A_MN = (MODE != GEMM_FWD);
@@ -184,7 +188,8 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
         // GATE, FWD: a = f(z) and the gate of output feature m of row n (dropped like drop_fwd under DROP)
         auto gate_fwd = [&](float z, int n, float& g) {
             float a;
-            act_fwd(p.act_kind, z, a, g);
+            if constexpr (RES) act_fwd_any(p.act_kind, z, a, g);
+            else act_fwd(p.act_kind, z, a, g);
             if constexpr (DROP) {
                 const uint32_t sample = (uint32_t)((p.drop.row_base + n) * p.drop.dp + p.drop.rank);
                 const bool keep = dropout_keep(p.drop, (uint32_t)p.drop.layer, drop_step, (uint32_t)m, sample);
@@ -232,6 +237,14 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                             mk[j] = (n < p.n_total) ? __ldg(mask + (size_t)n * p.ldmask + m) : 0.f;
                         }
                     }
+                    float sk[16];                            // RES: the skip input (FWD) or skip gradient (DGRAD)
+                    if constexpr (RES) {
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) {
+                            const int n = n0 + c + j;
+                            sk[j] = (p.skip != nullptr && m_ok && n < p.n_total) ? __ldcg(p.skip + (size_t)n * p.ldskip + m) : 0.f;
+                        }
+                    }
                     float v[16];
 #pragma unroll
                     for (int j = 0; j < 16; ++j) v[j] = 0.f;
@@ -245,7 +258,20 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                     for (int j = 0; j < 16; ++j) {
                         float x = v[j] + bias;
                         const int n = n0 + c + j;
-                        if constexpr (GATE) {
+                        if constexpr (RES) {
+                            if (MODE == GEMM_FWD) {
+                                if (p.relu) {
+                                    float g;
+                                    x = gate_fwd(x, n, g);
+                                    if (n < p.n_total && p.gate != nullptr) p.gate[(size_t)n * p.ldo + m] = g;
+                                }
+                                x += sk[j];
+                            } else {
+                                x += sk[j];
+                                if (n < p.n_total && p.gpre != nullptr) p.gpre[(size_t)n * p.ldgpre + m] = x;
+                                if (mask != nullptr) x *= mk[j];
+                            }
+                        } else if constexpr (GATE) {
                             if (MODE == GEMM_FWD) {
                                 if (p.relu) {
                                     float g;
@@ -282,6 +308,14 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                         mk[j] = (n < p.n_total) ? __ldg(mask + (size_t)n * p.ldmask + m) : 0.f;
                     }
                 }
+                float sk[16];                            // RES: the skip input (FWD) or skip gradient (DGRAD)
+                if constexpr (RES) {
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const int n = n0 + c + j;
+                        sk[j] = (p.skip != nullptr && m_ok && n < p.n_total) ? __ldcg(p.skip + (size_t)n * p.ldskip + m) : 0.f;
+                    }
+                }
                 float v[16];
                 warp_acc_row16(acc, ch, v, lane);
                 if (!m_ok) continue;
@@ -289,7 +323,16 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
                     float x = v[j] + bias;
-                    if constexpr (GATE) {
+                    if constexpr (RES) {
+                        if (MODE == GEMM_FWD) {
+                            if (p.relu) x = gate_fwd(x, n0 + c + j, gv[j]);
+                            x += sk[j];
+                        } else {
+                            x += sk[j];
+                            if (n0 + c + j < p.n_total && p.gpre != nullptr) p.gpre[(size_t)(n0 + c + j) * p.ldgpre + m] = x;
+                            if (mask != nullptr) x *= mk[j];
+                        }
+                    } else if constexpr (GATE) {
                         if (MODE == GEMM_FWD) {
                             if (p.relu) x = gate_fwd(x, n0 + c + j, gv[j]);
                         } else if (mask != nullptr) {
@@ -464,6 +507,16 @@ tc_gemm_gate_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                     const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
     tc_gemm_body<MODE, SPLITK, false, (int)kBlockM, DROP, true>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y,
                                                                 (int)blockIdx.z);
+}
+
+// FWD / DGRAD of a residual plan (GemmParams::res), with or without dropout in the FWD (a kernel of its own, like
+// tc_gemm_gate_kernel)
+template <int MODE, bool SPLITK, bool DROP>
+__global__ void __launch_bounds__(kThreads, 1)
+tc_gemm_res_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+    tc_gemm_body<MODE, SPLITK, false, (int)kBlockM, DROP, true, true>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y,
+                                                                      (int)blockIdx.z);
 }
 
 // ---- grouped weight-gradient launch: the tiles of SEVERAL layers' WGRAD GEMMs in one grid (one table entry per CTA).
@@ -745,6 +798,12 @@ cudaError_t gemm_configure() {
     if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_FWD, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_DGRAD, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_DGRAD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_res_kernel<GEMM_FWD, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_res_kernel<GEMM_FWD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_res_kernel<GEMM_FWD, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_res_kernel<GEMM_FWD, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_res_kernel<GEMM_DGRAD, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_res_kernel<GEMM_DGRAD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     g_configured = true;
     return cudaSuccess;
 }
@@ -769,6 +828,16 @@ static cudaError_t launch_mode(const GemmPlan& plan, cudaStream_t stream) {
         if (e != cudaSuccess) return e;
     }
     if constexpr (MODE != GEMM_WGRAD) {
+        if (gemm_residual(plan)) {
+            const bool drop = MODE == GEMM_FWD && plan.p.drop.on() && plan.p.relu;
+            const bool sk = plan.p.k_splits > 1;
+#define SSB_RES_LAUNCH(S, D) tc_gemm_res_kernel<MODE, S, D><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p)
+            if (sk) { if (drop) SSB_RES_LAUNCH(true, MODE == GEMM_FWD); else SSB_RES_LAUNCH(true, false); }
+            else { if (drop) SSB_RES_LAUNCH(false, MODE == GEMM_FWD); else SSB_RES_LAUNCH(false, false); }
+#undef SSB_RES_LAUNCH
+            g_launches.fetch_add(1, std::memory_order_relaxed);
+            return cudaGetLastError();
+        }
         if (gemm_gated(plan)) {
             // the DGRAD's gate already holds the dropout scale: only the FWD has a dropout form
             const bool drop = MODE == GEMM_FWD && plan.p.drop.on();
@@ -805,8 +874,12 @@ static cudaError_t launch_mode(const GemmPlan& plan, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
+bool gemm_residual(const GemmPlan& plan) { return plan.mode != GEMM_WGRAD && plan.p.res != 0; }
+
+bool gemm_skips(const GemmPlan& plan) { return gemm_residual(plan) && (plan.p.skip != nullptr || plan.p.gpre != nullptr); }
+
 bool gemm_gated(const GemmPlan& plan) {
-    if (!act_smooth(plan.p.act_kind)) return false;
+    if (!act_smooth(plan.p.act_kind) && !gemm_residual(plan)) return false;
     return plan.mode == GEMM_FWD ? plan.p.relu != 0 : (plan.mode == GEMM_DGRAD && plan.p.mask != nullptr);
 }
 

@@ -254,6 +254,17 @@ public:
         c.activation = geti("activation", ssb::ACT_RELU);
         TORCH_CHECK(ssb::act_valid(c.activation), "PipeEngine: cfg['activation'] must be 0 (relu), 1 (gelu), 2 (silu) or 3 (tanh), got ",
                     c.activation);
+        if (cfg.contains("residual")) {   // one 0 / 1 per layer: an identity skip around it
+            const auto res = cfg["residual"].cast<std::vector<int>>();
+            TORCH_CHECK(res.size() == c.layers.size(), "PipeEngine: cfg['residual'] needs one entry per layer");
+            for (size_t l = 0; l < res.size(); ++l) {
+                const ssb::LayerSpec& ls = c.layers[l];
+                TORCH_CHECK(!res[l] || (ls.relu && ls.in == ls.out),
+                            "PipeEngine: a residual layer needs an activation and as many outputs as inputs (layer ", l + 1, ")");
+                c.layers[l].res = res[l] ? 1 : 0;
+                c.residual |= c.layers[l].res;
+            }
+        }
         c10::cuda::CUDAGuard guard(weights.device());
         engine_ = std::make_unique<PipeEngine>(c, weights.data_ptr<float>(), grads.data_ptr<float>(), weights.numel(),
                                                momentum.has_value() ? momentum->data_ptr<float>() : nullptr);
@@ -364,6 +375,13 @@ public:
         TORCH_CHECK(g != nullptr, "PipeEngine.gate: layer ", l, " has no gate buffer (ReLU, inference, or no activation)");
         return view_of(g, cfg.mb_rows, boundary_cols(l), engine_->act_ld(l));
     }
+    // the skip gradient dL/da of residual layer l's output (a residual training plan only)
+    torch::Tensor g(int mu, int l) {
+        const auto& cfg = engine_->config();
+        float* p = engine_->g_ptr(mu, l);
+        TORCH_CHECK(p != nullptr, "PipeEngine.g: layer ", l, " has no skip-gradient buffer (not residual, or inference)");
+        return view_of(p, cfg.mb_rows, boundary_cols(l), engine_->act_ld(l));
+    }
     torch::Tensor probs(int mu) {
         const auto& cfg = engine_->config();
         return view_of(engine_->probs_ptr(mu), cfg.mb_rows, cfg.out_dim, engine_->act_ld((int)cfg.layers.size()));
@@ -472,6 +490,7 @@ void bind_runtime(py::module_& m) {
         .def("act", &PyEngine::act)
         .def("dz", &PyEngine::dz)
         .def("gate", &PyEngine::gate)
+        .def("g", &PyEngine::g)
         .def("probs", &PyEngine::probs)
         .def("kernels_per_step", &PyEngine::kernels_per_step)
         .def("graph_nodes", &PyEngine::graph_nodes)

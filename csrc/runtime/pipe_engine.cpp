@@ -159,6 +159,15 @@ void PipeEngine::alloc_buffers() {
             for (int l = 1; l <= L_; ++l)
                 if (gamma_all_[l]) gamma_[mu][l] = gamma_all_[l] + (size_t)mu * mb * act_ld_[l];
     }
+    if (cfg_.training && cfg_.residual) {
+        gres_all_.assign(L_ + 1, nullptr);
+        for (int l = 1; l <= L_; ++l)
+            if (res_layer(l)) gres_all_[l] = dalloc((size_t)M * mb * act_ld_[l]);
+        gres_.assign(M, std::vector<float*>(L_ + 1, nullptr));
+        for (int mu = 0; mu < M; ++mu)
+            for (int l = 1; l <= L_; ++l)
+                if (gres_all_[l]) gres_[mu][l] = gres_all_[l] + (size_t)mu * mb * act_ld_[l];
+    }
     act_.assign(M, std::vector<float*>(L_ + 1, nullptr));
     dz_.assign(M, std::vector<float*>(L_ + 1, nullptr));
     probs_.assign(M, nullptr);
@@ -193,11 +202,32 @@ float* PipeEngine::gamma_of(const float* act) const {
 // A smooth activation runs the gated GEMM variants: a FWD with relu applies f (and, training, stores its gates next to
 // its output), a DGRAD with mask multiplies by the previous layer's gates instead of testing its output.
 void PipeEngine::gate_gemm(GemmPlan& g) const {
-    if (!act_smooth(cfg_.activation)) return;
+    if (!act_smooth(cfg_.activation) && !cfg_.residual) return;   // a residual model gates ReLU too
     g.p.act_kind = cfg_.activation;
     if (!gated()) return;                                         // inference: f, no gates
     if (g.mode == GEMM_FWD && g.p.relu) g.p.gate = gamma_of(g.p.out);
     else if (g.mode == GEMM_DGRAD && g.p.mask != nullptr) g.p.mask = gamma_of(g.p.mask);
+}
+
+// A residual plan's FWD / DGRAD of layer l (mu: its micro-batch, -1 for all rows) runs the residual GEMM form where it adds a
+// skip, stores a skip gradient, or applies a ReLU gate (gated(): every activated layer of a residual training plan).
+//   FWD of a residual layer:  + act[l - 1] (for l = 1 the staged stage input or the received tile)
+//   DGRAD of layer l:         + g[l] when layer l is residual; stores g[l - 1] (before the gate) when layer l - 1 is
+//                             residual
+void PipeEngine::skip_gemm(GemmPlan& g, int l, int mu) const {
+    if (!cfg_.residual) return;
+    auto act = [&](int k) { return mu >= 0 ? act_[mu][k] : act_all_[k]; };
+    auto gres = [&](int k) { return mu >= 0 ? gres_[mu][k] : gres_all_[k]; };
+    if (g.mode == GEMM_FWD) {
+        if (res_layer(l)) { g.p.skip = act(l - 1); g.p.ldskip = act_ld_[l - 1]; }
+        g.p.res = (g.p.skip != nullptr || (gated() && g.p.relu)) ? 1 : 0;
+    } else if (g.mode == GEMM_DGRAD) {
+        if (res_layer(l)) { g.p.skip = gres(l); g.p.ldskip = act_ld_[l]; }
+        if (res_layer(l - 1)) { g.p.gpre = gres(l - 1); g.p.ldgpre = act_ld_[l - 1]; }
+        g.p.res = (g.p.skip != nullptr || g.p.gpre != nullptr || g.p.mask != nullptr) ? 1 : 0;
+        if ((res_layer(l) && g.p.skip == nullptr) || (res_layer(l - 1) && g.p.gpre == nullptr))
+            throw std::runtime_error("PipeEngine: no skip-gradient buffer behind a residual layer");
+    }
 }
 
 // Point the planner at one of the two input-staging sets (stage input = act[.][0], targets).
@@ -283,6 +313,13 @@ int PipeEngine::add_chain(int stream, int mu_base, int n_mu, bool do_fwd, bool d
     cp.act_kind = cfg_.activation;
     if (gated())
         for (int l = 0; l <= L_; ++l) cp.gate[l] = gamma_all_[l];
+    if (cfg_.residual) {                                  // training and inference: the RES form adds the skips
+        cp.res = 1;
+        for (int l = 1; l <= L_; ++l)
+            if (res_layer(l)) cp.res_mask |= 1u << (l - 1);
+        // a residual last layer of a non-last stage: the received gradient stays in g[L], the staging gates it into dz[L]
+        if (cfg_.training && do_bwd && !(do_fwd && do_loss) && res_layer(L_)) cp.gout = gres_all_[L_];
+    }
     if (dropout_on()) {
         // one spec for the launch: the kernel drops only the ReLU'd layers, layer l's counter is drop.layer + l - 1
         cp.drop = dropout_spec(cfg_.dropout, cfg_.dropout_seed);
@@ -361,13 +398,26 @@ void PipeEngine::build(const std::vector<std::tuple<int, int, int>>& instrs) {
         chain_ok_ = L_ >= 1 && L_ <= kChainMaxLayers && !getenv("SSB_NO_CHAIN") &&
                     chain_eligible(cl, L_, cfg_.mb_rows, cfg_.out_dim, cfg_.is_last != 0, cfg_.prec);
     }
+    if (chain_ok_ && !gres_all_.empty()) {
+        // the chain kernel carries the skip gradients in registers: only a residual last layer of a non-last stage keeps
+        // one, the gradient it receives
+        for (int l = 1; l <= L_; ++l) {
+            if (l == L_ && !cfg_.is_last) continue;
+            gres_all_[l] = nullptr;
+            for (int mu = 0; mu < M; ++mu) gres_[mu][l] = nullptr;
+        }
+    }
     if (pp_ctx_) {
         // peer-memory transport: the neighbours write straight into my receive slots, which therefore live in the
         // IPC-shared PpContext (one set of slots; reuse across steps is protected by the credit flags)
         if (pp_ctx_->n_mu() != M || pp_ctx_->mb_rows() != cfg_.mb_rows || pp_ctx_->ld_in() != act_ld_[0] || pp_ctx_->ld_out() != act_ld_[L_])
             throw std::runtime_error("PipeEngine: PpContext geometry does not match this stage");
         if (!cfg_.is_first) x_stage_sets_[0] = x_stage_sets_[1] = pp_ctx_->act_in();
-        if (!cfg_.is_last && cfg_.training) {
+        if (!cfg_.is_last && cfg_.training && res_layer(L_)) {
+            // a residual last layer keeps the received gradient as its skip gradient g[L]; dz[L] = g[L] * gamma_L is its own
+            gres_all_[L_] = pp_ctx_->dz_in();
+            for (int mu = 0; mu < M; ++mu) gres_[mu][L_] = gres_all_[L_] + (size_t)mu * cfg_.mb_rows * act_ld_[L_];
+        } else if (!cfg_.is_last && cfg_.training) {
             dz_all_[L_] = pp_ctx_->dz_in();
             for (int mu = 0; mu < M; ++mu) dz_[mu][L_] = dz_all_[L_] + (size_t)mu * cfg_.mb_rows * act_ld_[L_];
         }
@@ -439,6 +489,7 @@ void PipeEngine::plan_per_mubatch() {
         // rows, micro-batch mu of this stage
         gemms_.back().p.drop = drop_for(g.mode == GEMM_DGRAD ? std::max(layer - 1, 1) : layer, mu * cfg_.mb_rows);
         gate_gemm(gemms_.back());
+        skip_gemm(gemms_.back(), layer, mu);
         Op op;
         op.kind = OP_GEMM; op.stream = stream; op.gemm = (int)gemms_.size() - 1; op.layer = layer; op.mu = mu;
         ops_.push_back(op);
@@ -530,8 +581,8 @@ void PipeEngine::plan_per_mubatch() {
                 } else if (o == I_SEND_GRAD) {
                     it = {1, cfg_.stage - 1, dz_[mu][0], (size_t)mb * act_ld_[0]};
                     if (ev_bwd[mu] >= 0) emit_wait(s_comm_, ev_bwd[mu]);
-                } else {
-                    it = {0, cfg_.stage + 1, dz_[mu][L_], (size_t)mb * act_ld_[L_]};
+                } else {   // a residual last layer receives its skip gradient g[L] (gated into dz[L] below)
+                    it = {0, cfg_.stage + 1, res_layer(L_) && cfg_.training ? gres_[mu][L_] : dz_[mu][L_], (size_t)mb * act_ld_[L_]};
                     recvs.push_back({mu, 0});
                 }
                 grp.comm.push_back(it);
@@ -661,6 +712,7 @@ void PipeEngine::plan_per_mubatch() {
                             rm.scalar = dropout_spec(cfg_.dropout, cfg_.dropout_seed).scale;
                         }
                         if (gated()) { rm.gated = true; rm.b = gamma_[mu][L_]; }   // the gate (with the scale) replaces both
+                        if (res_layer(L_)) { rm.c = gres_[mu][L_]; rm.ldc = act_ld_[L_]; }   // out of place: g[L] stays
                         ops_.push_back(rm);
                     }
                     for (int l = L_; l >= 1; --l) {
@@ -814,6 +866,7 @@ void PipeEngine::build_coalesced() {
         maybe_splitk(gemms_.back());
         gemms_.back().p.drop = drop_for(g.mode == GEMM_DGRAD ? std::max(layer - 1, 1) : layer, 0);   // all rows
         gate_gemm(gemms_.back());
+        skip_gemm(gemms_.back(), layer, -1);
         Op op;
         op.kind = OP_GEMM; op.stream = stream; op.gemm = (int)gemms_.size() - 1; op.layer = layer; op.mu = -1;
         ops_.push_back(op);
@@ -1093,7 +1146,8 @@ void PipeEngine::exec(const Op& op, int set) {
             CUDA_CHECK(launch_argmax_correct(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, correct_dev_, st));
             break;
         case OP_RELU_MASK:
-            if (op.gated) CUDA_CHECK(launch_gate_mul(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, st));
+            if (op.gated && op.c != nullptr) CUDA_CHECK(launch_gate_mul_to(op.a, op.lda, op.c, op.ldc, op.b, op.ldb, op.rows, op.cols, st));
+            else if (op.gated) CUDA_CHECK(launch_gate_mul(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, st));
             else if (op.dropout) CUDA_CHECK(launch_relu_mask_scaled(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, op.scalar, st));
             else CUDA_CHECK(launch_relu_mask(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, st));
             break;
@@ -1391,10 +1445,13 @@ std::string PipeEngine::plan_text(int set) const {
             if (g.p.k_splits > 1) os << " splits=" << g.p.k_splits;
             if (gemm_drops(g)) os << " drop=" << (g.mode == GEMM_FWD ? "fwd" : "dgrad");
             if (gemm_gated(g)) os << " act=" << act_name(g.p.act_kind);
+            if (gemm_skips(g)) os << " res=1";
         }
         if (op.kind == OP_RELU_MASK && op.dropout) os << " drop=scaled";
         if (op.kind == OP_RELU_MASK && op.gated) os << " act=" << act_name(cfg_.activation);
+        if (op.kind == OP_RELU_MASK && op.c != nullptr) os << " res=1";
         if (op.kind == OP_CHAIN && act_smooth(cfg_.activation)) os << " act=" << act_name(cfg_.activation);
+        if (op.kind == OP_CHAIN && cfg_.residual) os << " res=1";
         if (op.kind == OP_COMM_GROUP) {
             os << " [";
             for (const auto& it : op.comm) os << (it.is_send ? "send->" : "recv<-") << it.peer << ":" << it.count << " ";

@@ -45,6 +45,7 @@ struct LayerSpec {
     int relu;
     int64_t offset;   // float offset of the [out, ld] block inside the W / G arenas
     int ld;           // row pitch of the block (floats); bias lives in column `in`
+    int res = 0;      // identity skip around the layer: a = x + f(z) (relu set, in == out)
 };
 
 enum OpKind : int {
@@ -106,6 +107,11 @@ struct EngineConfig {
     // ActKind (activation.h) of every layer with relu set.  A smooth kind makes training plans keep one gate buffer
     // gamma = f'(z) * keep * s per activated layer and micro-batch, laid out like act (gate_ptr).
     int activation = ACT_RELU;
+    // some layer has res set.  Training plans are then gated for every activation kind, ReLU included (a residual
+    // layer's output is not its own mask), and keep one skip-gradient buffer g[l] = dL/da_l per residual layer and
+    // micro-batch, laid out like act (g_ptr); chain plans keep only the one a residual last layer receives (the chain
+    // kernel carries the others in registers).
+    int residual = 0;
 };
 
 class PipeEngine {
@@ -141,7 +147,8 @@ public:
     uint32_t dropout_step() const { return step_; }
     bool dropout_on() const { return cfg_.training && cfg_.dropout > 0.0; }
     // a training plan of a smooth activation: the forward stores gates, the backward multiplies by them
-    bool gated() const { return cfg_.training && act_smooth(cfg_.activation); }
+    // (or of a residual model, any activation)
+    bool gated() const { return cfg_.training && (act_smooth(cfg_.activation) || cfg_.residual); }
     void synchronize();
     bool wait(double timeout_s);      // watchdog: false if the step in flight did not finish in time
     std::string comm_status() const;  // NCCL async error state of the attached communicators
@@ -158,6 +165,7 @@ public:
     int act_ld(int l) const { return act_ld_[l]; }
     float* dz_ptr(int mu, int l) { return dz_[mu][l]; }
     float* gate_ptr(int mu, int l) { return gamma_.empty() ? nullptr : gamma_[mu][l]; }   // nullptr unless gated()
+    float* g_ptr(int mu, int l) { return gres_.empty() ? nullptr : gres_[mu][l]; }   // nullptr unless layer l is residual (training)
     float* probs_ptr(int mu) { return probs_[mu]; }
     float* x_staging() { return x_stage_; }
     float* y_staging() { return y_stage_; }
@@ -216,6 +224,13 @@ private:
     // gated(): the gates of act, [mu][l] / [l] like act_ / act_all_ (layers without relu and l = 0: nullptr); empty otherwise
     std::vector<std::vector<float*>> gamma_;
     std::vector<float*> gamma_all_;
+    // residual training plans: g[l] = dL/da_l of every residual layer l, [mu][l] / [l] like act_ / act_all_ (nullptr
+    // elsewhere; empty without residual layers).  The dgrad of layer l + 1 stores it before the gate of layer l, the dgrad of
+    // layer l adds it as its skip gradient; for a residual last layer of a non-last stage it is the received gradient.
+    std::vector<std::vector<float*>> gres_;
+    std::vector<float*> gres_all_;
+    void skip_gemm(GemmPlan& g, int layer, int mu) const;   // the skip fields of a FWD / DGRAD plan of layer l being built
+    bool res_layer(int l) const { return l >= 1 && l <= L_ && cfg_.layers[l - 1].res != 0; }
     float* gamma_of(const float* act) const;     // the gate element of an element of act_all_[l], l >= 1
     void gate_gemm(GemmPlan& g) const;           // the activation of a FWD / DGRAD plan being built (gemm_gated)
     bool gate_on_ = false;           // grouped wgrad forked next to the chain kernel, gated by device counters

@@ -182,6 +182,7 @@ class ReLU(Module):
     and kept", and ``dropout_scale`` (s) multiplies the gradient where the mask passes it."""
 
     dropout_scale = None
+    kind = "relu"
 
     def forward(self, inputs, mubatch_id=0):
         if self._training:
@@ -272,13 +273,23 @@ def _init_seed(in_dims: int, out_dims: int, layer_index: Optional[int]):
 
 class Linear(Module):
     """y = f?(x @ W^T + b) with hand-written backward (reference: layers.py:99-142); f is ReLU, GELU, SiLU or tanh
-    (``activation``: "relu", "gelu", "silu", "tanh" or None)."""
+    (``activation``: "relu", "gelu", "silu", "tanh" or None).
+
+    ``residual=True`` adds an identity skip around the layer: a = x + drop(f(x W^T + b)).  It needs an activation and
+    ``in_dims == out_dims``.  The branch always goes through the gated route (F.activation, ReLU included), since the
+    output x + relu(z) is no longer its own mask; the backward is linear_grad(g * gamma) + g."""
 
     def __init__(self, in_dims, out_dims, activation="relu", arena: Optional[ParamArena] = None,
-                 block_index: int = 0, layer_index: Optional[int] = None, device="cpu"):
+                 block_index: int = 0, layer_index: Optional[int] = None, device="cpu", residual: bool = False):
         super().__init__()
         if activation is not None:
             F.check_activation(activation)
+        if not isinstance(residual, bool):
+            raise ValueError(f"residual must be a bool, got {residual!r}")
+        if residual and (activation is None or in_dims != out_dims):
+            raise ValueError(f"a residual Linear needs an activation and in_dims == out_dims, got {in_dims}->{out_dims}, "
+                             f"activation {activation!r}")
+        self.residual = residual
         self.in_dims, self.out_dims = in_dims, out_dims
         self.activation = ACTIVATIONS[activation]() if activation is not None else None
         if arena is None:
@@ -308,6 +319,14 @@ class Linear(Module):
         if self._training:
             self._cache[f"input_{mubatch_id}"] = inputs
         W, b = self._params["W"].data, self._params["b"].data
+        if self.residual:
+            # x + drop(f(z)); the gate (with dropout's keep * s) is the whole backward of the branch
+            a, gamma = F.activation(self.activation.kind, F.linear(inputs, W, b))
+            if self._training and self.dropout is not None:
+                a, gamma = self._dropout(a), self._dropout(gamma)
+            if self._training:
+                self._cache[f"gate_{mubatch_id}"] = gamma
+            return inputs + a
         if isinstance(self.activation, _Gated):
             # z, then (f(z), f'(z)) in one pass; dropout drops both, so the stashed gate is the whole backward
             a, gamma = F.activation(self.activation.kind, F.linear(inputs, W, b))
@@ -347,22 +366,27 @@ class Linear(Module):
 
     def backward(self, dout, mubatch_id=0):
         assert self._training
-        if self.activation:
+        skip = None
+        if self.residual:
+            skip = dout                                     # the skip's gradient passes through unchanged
+            dout = F.gate_grad(dout, self._cache.pop(f"gate_{mubatch_id}"))
+        elif self.activation:
             dout = self.activation.backward(dout, mubatch_id)
         x = self._cache.pop(f"input_{mubatch_id}")
         if dout.is_cuda:
             from ..ops import cuda as K
 
             # dW / db accumulate in place inside the wgrad kernel's epilogue
-            return K.linear_bwd_accumulate(dout, x, self.arena.block(self.block_index),
-                                           self.arena.block(self.block_index, True), self.in_dims)
+            dx = K.linear_bwd_accumulate(dout, x, self.arena.block(self.block_index),
+                                         self.arena.block(self.block_index, True), self.in_dims)
+            return dx if skip is None else dx + skip
         dx, dW, db = F.linear_grad(dout, x, self._params["W"].data)
         self._params["W"].grad += dW
         self._params["b"].grad += db.reshape(1, -1)
-        return dx
+        return dx if skip is None else dx + skip
 
     def __repr__(self):
-        return f"Linear({self.in_dims}->{self.out_dims}, act: {self.activation})"
+        return f"Linear({self.in_dims}->{self.out_dims}, act: {self.activation}{', residual' if self.residual else ''})"
 
 
 class MSELoss(Module):

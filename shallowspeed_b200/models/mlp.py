@@ -42,6 +42,12 @@ def stage_layer_specs(sizes: Sequence[int], stage_idx: int, n_stages: int):
     return specs
 
 
+def residual_layers(sizes: Sequence[int], n_stages: int = 1):
+    """Global indices of the Linears a residual model wraps in a skip: those with an activation (stage_layer_specs) and
+    equal widths.  The same set for every stage of a layout."""
+    return [g for s in range(n_stages) for i, o, relu, g in stage_layer_specs(sizes, s, n_stages) if relu and i == o]
+
+
 def mlp_sizes(hidden: int, n_layers: int, in_dim: int = 784, out_dim: int = 10):
     """``n_layers`` Linears: in_dim -> hidden x (n_layers-1) -> out_dim."""
     assert n_layers >= 1
@@ -51,7 +57,7 @@ def mlp_sizes(hidden: int, n_layers: int, in_dim: int = 784, out_dim: int = 10):
 class MLP(Sequential):
     def __init__(self, sizes: Sequence[int], stage_idx: int, n_stages: int, batch_size: int,
                  device="cpu", seed_mode: str = "shape", verbose: bool = False, loss: str = "mse",
-                 dropout: float = 0.0, dropout_seed: int = 0, activation: str = "relu"):
+                 dropout: float = 0.0, dropout_seed: int = 0, activation: str = "relu", residual: bool = False):
         """
         :param batch_size: the GLOBAL batch size - the loss gradient is scaled by
             1/batch_size so that summing over micro-batches and DP replicas reproduces
@@ -67,7 +73,17 @@ class MLP(Sequential):
             stage 6 ends in a 123->10 Linear that carries a ReLU (the stage rule above); it is dropped like any other.
         :param activation: the activation of every Linear that has one (every hidden layer, never the logits): "relu"
             (the reference's), "gelu" (erf form), "silu" or "tanh".  The pp=8 stage-6 Linear above carries it as well.
+        :param residual: an identity skip around every Linear that has an activation and as many outputs as inputs,
+            a = x + drop(f(x W^T + b)) (models.layers.Linear).  ValueError when no Linear of the whole model (all stages
+            of the layout) qualifies, e.g. the reference's 784-128-127-...-10.
         """
+        if not isinstance(residual, bool):
+            raise ValueError(f"residual must be a bool, got {residual!r}")
+        res_layers = set(residual_layers(sizes, n_stages)) if residual else set()
+        if residual and not res_layers:
+            raise ValueError(f"residual=True, but no Linear of the model {list(sizes)} has an activation and equal input and "
+                             "output widths")
+        self.residual = residual
         assert seed_mode in ("shape", "index")
         self.loss = check_loss(loss)
         self.activation = check_activation(activation)
@@ -82,7 +98,7 @@ class MLP(Sequential):
         self.arena = ParamArena([(o, i) for i, o, _, _ in specs], device=device)
         layers = [
             Linear(i, o, activation=self.activation if relu else None, arena=self.arena, block_index=bi,
-                   layer_index=gidx if seed_mode == "index" else None)
+                   layer_index=gidx if seed_mode == "index" else None, residual=gidx in res_layers)
             for bi, (i, o, relu, gidx) in enumerate(specs)
         ]
         self.linears = list(layers)

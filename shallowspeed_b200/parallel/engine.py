@@ -303,6 +303,8 @@ class NativeWorker:
             cfg.update(loss=LOSS_CODES[m.loss])
         if getattr(m, "activation", "relu") != "relu":   # training and inference: f applies in both
             cfg.update(activation=ACTIVATION_CODES[m.activation])
+        if getattr(m, "residual", False):   # training and inference: the skips apply in both
+            cfg.update(residual=[int(lin.residual) for lin in m.linears])
         if training and getattr(m, "dropout", 0.0) > 0.0:   # inference plans run without dropout
             cfg.update(dropout=m.dropout, dropout_seed=m.dropout_seed, layer_base=m.layer_base)
         eng = _C().PipeEngine(specs, cfg, m.arena.weights, m.arena.grads, momentum)
@@ -492,13 +494,15 @@ class Trainer:
     of ``dropout_step`` i, the number of steps run so far.
 
     ``activation``: the hidden layers' activation, "relu" (default), "gelu", "silu" or "tanh" (``models.mlp.MLP``).
+
+    ``residual``: an identity skip around every hidden layer whose width does not change (``models.mlp.MLP``).
     """
 
     def __init__(self, layer_sizes, global_batch_size=128, n_mubatches=4, lr=0.006, schedule="naive",
                  dp_comm=None, pp_comm=None, grid: Optional[ProcessGrid] = None, comm_mode="fused",
                  use_graph=True, device=None, seed_mode="shape", precision="fp32", watchdog_s=None, pp_transport=None,
                  local_batch_size=None, momentum=0.0, weight_decay=0.0, nesterov=False, loss="mse", lr_schedule=None,
-                 dropout=0.0, dropout_seed=0, activation="relu"):
+                 dropout=0.0, dropout_seed=0, activation="relu", residual=False):
         from ..models.mlp import MLP
         from ..optimizer import SGD
         from .schedules import SCHEDULE_NAME_TO_CLS
@@ -513,7 +517,8 @@ class Trainer:
         # scale stays 1 / global_batch_size.
         self.local_batch_size = int(local_batch_size) if local_batch_size else global_batch_size // dp
         self.model = MLP(layer_sizes, self.pp_comm.Get_rank(), pp, global_batch_size, seed_mode=seed_mode,
-                         loss=loss, dropout=dropout, dropout_seed=dropout_seed, activation=activation).to(self.device)
+                         loss=loss, dropout=dropout, dropout_seed=dropout_seed, activation=activation,
+                         residual=residual).to(self.device)
         self.optimizer = SGD(self.model.parameters(), lr, momentum=momentum, weight_decay=weight_decay, nesterov=nesterov,
                              arena=self.model.arena)
 

@@ -11,10 +11,11 @@ from pathlib import Path
 import torch
 
 # settings a checkpoint without them was written under (plain SGD, the MSE loss, a constant learning rate, no dropout,
-# no shuffling, ReLU)
+# no shuffling, ReLU, no skips)
 _HPARAM_DEFAULTS = {"momentum": 0.0, "weight_decay": 0.0, "nesterov": False, "loss": "mse",
                     "lr_schedule": {"kind": "constant"}, "dropout": 0.0, "dropout_seed": 0,
-                    "shuffle": False, "shuffle_seed": 0, "activation": "relu"}
+                    "shuffle": False, "shuffle_seed": 0, "activation": "relu",
+                    "residual": False}
 
 
 def _path(directory, stage, n_stages):

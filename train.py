@@ -96,6 +96,8 @@ def build_parser():
                    help="mse: the reference's softmax + MSE; cross-entropy: softmax cross-entropy on the logits")
     p.add_argument("--activation", default="relu", metavar="{" + ",".join(ACTIVATION_CODES) + "}",
                    help="activation of every hidden layer: relu, gelu (erf form), silu or tanh")
+    p.add_argument("--residual", action="store_true",
+                   help="identity skip around every hidden layer whose width does not change: a = x + f(x W^T + b)")
     p.add_argument("--dropout", type=float, default=0.0,
                    help="inverted dropout with this drop probability on every hidden layer's output, in [0, 1)")
     p.add_argument("--dropout-seed", type=int, default=0, help="seed of the dropout masks, in [0, 2**64)")
@@ -191,7 +193,7 @@ def main(args):
     model = MLP(layer_sizes, stage_idx=pp_comm.Get_rank(), n_stages=args.pp,
                 batch_size=args.global_batch_size, seed_mode=args.seed_mode,
                 verbose=(grid.rank == 0 or is_last), loss=loss, dropout=args.dropout,
-                dropout_seed=args.dropout_seed, activation=activation)
+                dropout_seed=args.dropout_seed, activation=activation, residual=bool(args.residual))
     model.to(device)
     model.train()
     # before the resume: the momentum arena it restores is allocated here
@@ -218,7 +220,7 @@ def main(args):
                "weight_decay": float(args.weight_decay), "nesterov": bool(args.nesterov), "loss": loss,
                "lr_schedule": lr_schedule.spec(), "dropout": float(args.dropout),
                "dropout_seed": int(args.dropout_seed), "shuffle": bool(args.shuffle), "shuffle_seed": shuffle_seed,
-               "activation": activation}
+               "activation": activation, "residual": bool(args.residual)}
     resumed_step = 0
     if args.resume:
         from shallowspeed_b200.utils.checkpoint import load_stage

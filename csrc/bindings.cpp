@@ -145,7 +145,8 @@ static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<
 // (same row pitch; its column `in` belongs to the bias).
 static void linear_wgrad(const Tensor& dz, const Tensor& x, Tensor& G, bool accumulate, const c10::optional<Tensor>& db,
                          int64_t db_stride, const c10::optional<Tensor>& W, const py::object& lr, bool fuse_sgd,
-                         int64_t prec, const c10::optional<Tensor>& V, double momentum, double weight_decay, bool nesterov) {
+                         int64_t prec, const c10::optional<Tensor>& V, double momentum, double weight_decay, bool nesterov,
+                         const c10::optional<Tensor>& E, const py::object& ema_alpha) {
     check_mat(dz, "dz"); check_mat(x, "x"); check_mat(G, "G");
     const int rows = dz.size(0), out = dz.size(1), in = x.size(1);
     TORCH_CHECK(x.size(0) == rows && G.size(0) == out && G.size(1) == in, "linear_wgrad: shape mismatch");
@@ -156,6 +157,16 @@ static void linear_wgrad(const Tensor& dz, const Tensor& x, Tensor& G, bool accu
         TORCH_CHECK(W.has_value() && V->size(0) == out && V->size(1) == in && ld_of(*V) == ld_of(*W),
                     "linear_wgrad: V must have W's shape and row pitch");
         opt.V = V->data_ptr<float>();
+    }
+    TORCH_CHECK(E.has_value() == !ema_alpha.is_none(), "linear_wgrad: ema and ema_alpha go together");
+    Tensor alpha_dev;
+    if (E.has_value()) {
+        check_mat(*E, "ema");
+        TORCH_CHECK(W.has_value() && E->size(0) == out && E->size(1) == in && ld_of(*E) == ld_of(*W),
+                    "linear_wgrad: ema must have W's shape and row pitch");
+        alpha_dev = lr_scalar(ema_alpha, dz, "linear_wgrad (ema_alpha)");
+        opt.E = E->data_ptr<float>();
+        opt.ema_alpha = alpha_dev.data_ptr<float>();
     }
     c10::cuda::CUDAGuard guard(dz.device());
     const Tensor lr_dev = fuse_sgd ? lr_scalar(lr, dz, "linear_wgrad") : Tensor();
@@ -234,7 +245,7 @@ static void sgd_(Tensor& w, const Tensor& g, const py::object& lr) {
     cuda_ok(ssb::launch_sgd(w.data_ptr<float>(), g.data_ptr<float>(), lr_dev.data_ptr<float>(), w.numel(), cur_stream()), "sgd");
 }
 static void sgd_momentum_(Tensor& w, const Tensor& g, const c10::optional<Tensor>& v, const py::object& lr, double momentum,
-                          double weight_decay, bool nesterov) {
+                          double weight_decay, bool nesterov, const c10::optional<Tensor>& e, const py::object& ema_alpha) {
     TORCH_CHECK(w.is_contiguous() && g.is_contiguous() && w.numel() == g.numel());
     TORCH_CHECK(w.scalar_type() == torch::kFloat32 && g.scalar_type() == torch::kFloat32);
     ssb::SgdState opt;
@@ -242,6 +253,14 @@ static void sgd_momentum_(Tensor& w, const Tensor& g, const c10::optional<Tensor
     if (v.has_value()) {
         TORCH_CHECK(v->is_contiguous() && v->numel() == w.numel() && v->scalar_type() == torch::kFloat32 && v->is_cuda());
         opt.V = v->data_ptr<float>();
+    }
+    TORCH_CHECK(e.has_value() == !ema_alpha.is_none(), "sgd_momentum_: ema and ema_alpha go together");
+    Tensor alpha_dev;
+    if (e.has_value()) {
+        TORCH_CHECK(e->is_contiguous() && e->numel() == w.numel() && e->scalar_type() == torch::kFloat32 && e->is_cuda());
+        alpha_dev = lr_scalar(ema_alpha, w, "sgd_momentum_ (ema_alpha)");
+        opt.E = e->data_ptr<float>();
+        opt.ema_alpha = alpha_dev.data_ptr<float>();
     }
     const char* err = ssb::sgd_state_check(opt);
     TORCH_CHECK(err == nullptr, "sgd_momentum_: ", err ? err : "");
@@ -320,7 +339,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("drop") = py::none());
     m.def("linear_wgrad", &linear_wgrad, py::arg("dz"), py::arg("x"), py::arg("G"), py::arg("accumulate"), py::arg("db"),
           py::arg("db_stride"), py::arg("W"), py::arg("lr"), py::arg("fuse_sgd"), py::arg("prec") = (int)ssb::PREC_TF32,
-          py::arg("V") = py::none(), py::arg("momentum") = 0.0, py::arg("weight_decay") = 0.0, py::arg("nesterov") = false);
+          py::arg("V") = py::none(), py::arg("momentum") = 0.0, py::arg("weight_decay") = 0.0, py::arg("nesterov") = false,
+          py::arg("ema") = py::none(), py::arg("ema_alpha") = py::none());
     m.def("loss_head", &loss_head, py::arg("logits"), py::arg("target"), py::arg("probs"), py::arg("dlogits"),
           py::arg("loss_out"), py::arg("inv_batch"), py::arg("loss") = (int)ssb::LOSS_MSE);
     m.def("softmax_grad", &softmax_grad);
@@ -331,7 +351,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("axpby", &axpby);
     m.def("sgd_", &sgd_);
     m.def("sgd_momentum_", &sgd_momentum_, py::arg("w"), py::arg("g"), py::arg("v"), py::arg("lr"), py::arg("momentum"),
-          py::arg("weight_decay"), py::arg("nesterov"));
+          py::arg("weight_decay"), py::arg("nesterov"), py::arg("ema") = py::none(), py::arg("ema_alpha") = py::none());
     m.def("argmax_correct", &argmax_correct);
     m.def("shuffle_index", &shuffle_index, py::arg("n"), py::arg("seed"), py::arg("epoch"), py::arg("positions"));
     m.def("gather_rows", &gather_rows, py::arg("x_src"), py::arg("y_src"), py::arg("seed"), py::arg("epoch"), py::arg("gbs"),

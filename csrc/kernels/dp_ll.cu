@@ -69,7 +69,9 @@ __device__ __forceinline__ unsigned long long gtime_ll() {
 
 // STATEFUL: momentum / weight decay in phase B through sgd_direction; the owner of a row keeps its momentum in its LOCAL
 // arena (p.opt.V, loaded with the weights before the first wait) and never sends it.
-template <int DP, bool STATEFUL = false>
+// EMA (with STATEFUL): the owner of a row also moves its LOCAL EMA entries (p.opt.E) towards the new weights it forms;
+// with a plain rule the step direction stays the reduced gradient.
+template <int DP, bool STATEFUL = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntry* __restrict__ entries, const DpLLParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
@@ -186,6 +188,8 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
             const float* mine0 = own + (p.rank * rpo) * kOwnLd;
             const uint4* zoneA = p.llA[p.rank] + (size_t)parity * DP * p.n_tiles * rpo * 17;
             const float lr = *p.lr;                              // in flight with the first batch's loads
+            const float alpha = EMA ? *p.opt.ema_alpha : 0.f;
+            const bool rule = !EMA || p.opt.has_rule();
             for (int i0 = etid; i0 < n_lines; i0 += 128 * kLB) {
                 uint4 ln[kLB][DP];
                 float wv0[kLB], wv1[kLB];
@@ -234,8 +238,10 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
                     if constexpr (STATEFUL) {                    // s0 / s1 become the step directions
                         const float mu = p.opt.momentum, wd = p.opt.weight_decay;
                         const bool nv = p.opt.nesterov != 0;
-                        s0 = sgd_direction<false>(s0, wv0[u], vv0[u], mu, wd, nv);
-                        s1 = sgd_direction<false>(s1, wv1[u], vv1[u], mu, wd, nv);
+                        if (rule) {
+                            s0 = sgd_direction<false>(s0, wv0[u], vv0[u], mu, wd, nv);
+                            s1 = sgd_direction<false>(s1, wv1[u], vv1[u], mu, wd, nv);
+                        }
                         if (p.opt.V != nullptr) {
                             float* vrow = p.opt.V + (wrow - p.W);
                             if (j < 16) {
@@ -251,9 +257,18 @@ __global__ void __launch_bounds__(kThreads, 1) dp_ll_wgrad_kernel(const DpLLEntr
                         const int n = e.n0 + 2 * j;
                         if (n < e.n_total) { w0 = wv0[u] - lr * s0; wrow[n] = w0; }
                         if (n + 1 < e.n_total) { w1 = wv1[u] - lr * s1; wrow[n + 1] = w1; }
+                        if constexpr (EMA) {
+                            float* erow = p.opt.E + (wrow - p.W);
+                            if (n < e.n_total) erow[n] = ema_lerp(erow[n], w0, alpha);
+                            if (n + 1 < e.n_total) erow[n + 1] = ema_lerp(erow[n + 1], w1, alpha);
+                        }
                     } else {
                         w0 = wv0[u] - lr * s0;                 // bias lives in column `in` of the block
                         wrow[e.n_total] = w0;
+                        if constexpr (EMA) {
+                            float* erow = p.opt.E + (wrow - p.W);
+                            erow[e.n_total] = ema_lerp(erow[e.n_total], w0, alpha);
+                        }
                     }
 #pragma unroll
                     for (int d = 0; d < DP; ++d)
@@ -367,22 +382,28 @@ cudaError_t dp_ll_configure() {
     if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
     if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
     if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
-    return cudaFuncSetAttribute(dp_ll_wgrad_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
+    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<2, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
+    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<4, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
+    return cudaFuncSetAttribute(dp_ll_wgrad_kernel<8, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
 }
 
 cudaError_t launch_dp_ll(const DpLLPlan& plan, cudaStream_t stream) {
-    const bool stateful = plan.p.opt.momentum != 0.f || plan.p.opt.weight_decay != 0.f;
+    const bool stateful = plan.p.opt.has_rule(), ema = plan.p.opt.E != nullptr;
     switch (plan.p.dp) {
         case 2:
-            if (stateful) dp_ll_wgrad_kernel<2, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
+            if (ema) dp_ll_wgrad_kernel<2, true, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
+            else if (stateful) dp_ll_wgrad_kernel<2, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
             else dp_ll_wgrad_kernel<2><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
             break;
         case 4:
-            if (stateful) dp_ll_wgrad_kernel<4, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
+            if (ema) dp_ll_wgrad_kernel<4, true, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
+            else if (stateful) dp_ll_wgrad_kernel<4, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
             else dp_ll_wgrad_kernel<4><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
             break;
         case 8:
-            if (stateful) dp_ll_wgrad_kernel<8, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
+            if (ema) dp_ll_wgrad_kernel<8, true, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
+            else if (stateful) dp_ll_wgrad_kernel<8, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
             else dp_ll_wgrad_kernel<8><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
             break;
         default: return cudaErrorInvalidValue;

@@ -311,53 +311,89 @@ cudaError_t launch_sgd(float* w, const float* g, const float* lr, long n, cudaSt
 
 // flat-arena SGD with the stateful rule (sgd_direction): same float4 body and scalar tail as sgd_kernel, plus the
 // momentum buffer v (nullptr when momentum == 0: weight decay alone keeps no state).
+// EMA: the EMA buffer e moves towards each new weight (ema_lerp, alpha read from the device); without a rule (plain SGD
+// with an EMA) the weight update is sgd_kernel's own expression, so the weights do not depend on the EMA.
+template <bool EMA>
 __device__ __forceinline__ float sgd_momentum_elem(float w, float g, float* v, long i, float lr, float mu, float wd,
-                                                   bool nesterov) {
+                                                   bool nesterov, bool rule) {
+    if (EMA && !rule) return w - lr * g;
     float vi = v != nullptr ? v[i] : 0.f;
     const float d = sgd_direction<false>(g, w, vi, mu, wd, nesterov);
     if (v != nullptr) v[i] = vi;
     return w - lr * d;
 }
+template <bool EMA = false>
 __global__ void __launch_bounds__(256) sgd_momentum_kernel(float4* __restrict__ w, const float4* __restrict__ g,
                                                            float4* __restrict__ v, const float* __restrict__ lr_ptr,
-                                                           float mu, float wd, int nesterov, long n4) {
+                                                           float mu, float wd, int nesterov, long n4,
+                                                           float4* __restrict__ e, const float* __restrict__ alpha_ptr) {
     const float lr = *lr_ptr;
+    const float alpha = EMA ? *alpha_ptr : 0.f;
+    const bool rule = !EMA || mu != 0.f || wd != 0.f;
     const long stride = (long)gridDim.x * blockDim.x;
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += stride) {
         float4 a = w[i];
         const float4 b = g[i];
-        float4 m = v != nullptr ? v[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-        const bool nv = nesterov != 0;
-        a.x -= lr * sgd_direction<false>(b.x, a.x, m.x, mu, wd, nv);
-        a.y -= lr * sgd_direction<false>(b.y, a.y, m.y, mu, wd, nv);
-        a.z -= lr * sgd_direction<false>(b.z, a.z, m.z, mu, wd, nv);
-        a.w -= lr * sgd_direction<false>(b.w, a.w, m.w, mu, wd, nv);
-        if (v != nullptr) v[i] = m;
+        if (rule) {
+            float4 m = v != nullptr ? v[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+            const bool nv = nesterov != 0;
+            a.x -= lr * sgd_direction<false>(b.x, a.x, m.x, mu, wd, nv);
+            a.y -= lr * sgd_direction<false>(b.y, a.y, m.y, mu, wd, nv);
+            a.z -= lr * sgd_direction<false>(b.z, a.z, m.z, mu, wd, nv);
+            a.w -= lr * sgd_direction<false>(b.w, a.w, m.w, mu, wd, nv);
+            if (v != nullptr) v[i] = m;
+        } else {
+            a.x -= lr * b.x; a.y -= lr * b.y; a.z -= lr * b.z; a.w -= lr * b.w;
+        }
         w[i] = a;
+        if constexpr (EMA) {
+            float4 t = e[i];
+            t.x = ema_lerp(t.x, a.x, alpha); t.y = ema_lerp(t.y, a.y, alpha);
+            t.z = ema_lerp(t.z, a.z, alpha); t.w = ema_lerp(t.w, a.w, alpha);
+            e[i] = t;
+        }
     }
 }
+template <bool EMA = false>
 __global__ void sgd_momentum_tail_kernel(float* w, const float* g, float* v, const float* lr, float mu, float wd,
-                                         int nesterov, long start, long n) {
+                                         int nesterov, long start, long n, float* e, const float* alpha) {
     const long i = start + blockIdx.x * (long)blockDim.x + threadIdx.x;
-    if (i < n) w[i] = sgd_momentum_elem(w[i], g[i], v, i, *lr, mu, wd, nesterov != 0);
+    if (i < n) {
+        const float nw = sgd_momentum_elem<EMA>(w[i], g[i], v, i, *lr, mu, wd, nesterov != 0, mu != 0.f || wd != 0.f);
+        w[i] = nw;
+        if constexpr (EMA) e[i] = ema_lerp(e[i], nw, *alpha);
+    }
 }
 cudaError_t launch_sgd_momentum(float* w, const float* g, const float* lr, const SgdState& opt, long n,
                                 cudaStream_t stream) {
     if (lr == nullptr || sgd_state_check(opt) != nullptr) return cudaErrorInvalidValue;
     float* v = opt.V;
-    const bool aligned = ((reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(v)) & 15) == 0;
+    float* e = opt.E;
+    const bool aligned = ((reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(v) |
+                           reinterpret_cast<uintptr_t>(e)) & 15) == 0;
     const long n4 = aligned ? n / 4 : 0;
     if (n4 > 0) {
         long blocks = (n4 + 255) / 256;
         if (blocks > 132 * 8) blocks = 132 * 8;
-        sgd_momentum_kernel<<<(int)blocks, 256, 0, stream>>>(reinterpret_cast<float4*>(w), reinterpret_cast<const float4*>(g),
-                                                             reinterpret_cast<float4*>(v), lr, opt.momentum, opt.weight_decay,
-                                                             opt.nesterov, n4);
+        if (e != nullptr)
+            sgd_momentum_kernel<true><<<(int)blocks, 256, 0, stream>>>(
+                reinterpret_cast<float4*>(w), reinterpret_cast<const float4*>(g), reinterpret_cast<float4*>(v), lr, opt.momentum,
+                opt.weight_decay, opt.nesterov, n4, reinterpret_cast<float4*>(e), opt.ema_alpha);
+        else
+            sgd_momentum_kernel<<<(int)blocks, 256, 0, stream>>>(
+                reinterpret_cast<float4*>(w), reinterpret_cast<const float4*>(g), reinterpret_cast<float4*>(v), lr, opt.momentum,
+                opt.weight_decay, opt.nesterov, n4, nullptr, nullptr);
     }
     const long done = n4 * 4;
-    if (done < n)
-        sgd_momentum_tail_kernel<<<(int)((n - done + 255) / 256), 256, 0, stream>>>(w, g, v, lr, opt.momentum, opt.weight_decay,
-                                                                                  opt.nesterov, done, n);
+    if (done < n) {
+        const int blocks = (int)((n - done + 255) / 256);
+        if (e != nullptr)
+            sgd_momentum_tail_kernel<true><<<blocks, 256, 0, stream>>>(w, g, v, lr, opt.momentum, opt.weight_decay, opt.nesterov,
+                                                                     done, n, e, opt.ema_alpha);
+        else
+            sgd_momentum_tail_kernel<<<blocks, 256, 0, stream>>>(w, g, v, lr, opt.momentum, opt.weight_decay, opt.nesterov, done,
+                                                                 n, nullptr, nullptr);
+    }
     return cudaGetLastError();
 }
 

@@ -77,11 +77,15 @@ __device__ __forceinline__ float elem_direction(const DpLayerParams& p, int64_t 
 // Executed by `nthreads` threads (tid in [0, nthreads)), all of which must call it.
 // STATEFUL: momentum / weight decay through sgd_direction; the momentum of the tile lives in the reducing replica's
 // LOCAL arena p.opt.V (the owner's, or every replica's own with one_shot) and is never published.
-template <bool STATEFUL>
+// EMA (with STATEFUL): the reducing replica also moves its LOCAL EMA entries (p.opt.E) towards the new weights it forms;
+// with a plain rule the step direction stays the reduced gradient.
+template <bool STATEFUL, bool EMA = false>
 __device__ void dp_owner_reduce_tile(const DpPeers& peers, const DpLayerParams& p, const TileCoord& tc, uint32_t epoch,
                                      int tid, int nthreads, int bar_id, int part = 0, int nparts = 1, bool publish = true) {
     const int me = p.rank;
     const float lr = *p.lr;                               // written before the launch: load it under the wait below
+    const float alpha = EMA ? *p.opt.ema_alpha : 0.f;
+    const bool rule = !EMA || p.opt.has_rule();
     // wait until every replica's partial of this tile has landed in my staging memory
     if (tid < p.dp) wait_flag_ge(peers.arrive[me] + (int64_t)tid * p.slots_per_src + p.slot_flag_base + tc.slot, epoch);
     asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(nthreads) : "memory");
@@ -140,21 +144,31 @@ __device__ void dp_owner_reduce_tile(const DpPeers& peers, const DpLayerParams& 
                     float4 v = vp != nullptr ? *vp : make_float4(0.f, 0.f, 0.f, 0.f);
                     const float mu = p.opt.momentum, wd = p.opt.weight_decay;
                     const bool nv = p.opt.nesterov != 0;
-                    sum.x = sgd_direction<false>(sum.x, w.x, v.x, mu, wd, nv);
-                    sum.y = sgd_direction<false>(sum.y, w.y, v.y, mu, wd, nv);
-                    sum.z = sgd_direction<false>(sum.z, w.z, v.z, mu, wd, nv);
-                    sum.w = sgd_direction<false>(sum.w, w.w, v.w, mu, wd, nv);
+                    if (rule) {
+                        sum.x = sgd_direction<false>(sum.x, w.x, v.x, mu, wd, nv);
+                        sum.y = sgd_direction<false>(sum.y, w.y, v.y, mu, wd, nv);
+                        sum.z = sgd_direction<false>(sum.z, w.z, v.z, mu, wd, nv);
+                        sum.w = sgd_direction<false>(sum.w, w.w, v.w, mu, wd, nv);
+                    }
                     if (vp != nullptr) *vp = v;
                 }
                 w.x -= lr * sum.x; w.y -= lr * sum.y; w.z -= lr * sum.z; w.w -= lr * sum.w;
+                if constexpr (EMA) {
+                    float4* ep = reinterpret_cast<float4*>(p.opt.E + woff);
+                    float4 t = *ep;
+                    t.x = ema_lerp(t.x, w.x, alpha); t.y = ema_lerp(t.y, w.y, alpha);
+                    t.z = ema_lerp(t.z, w.z, alpha); t.w = ema_lerp(t.w, w.w, alpha);
+                    *ep = t;
+                }
                 if (n_pub == 1) *reinterpret_cast<float4*>(peers.W[me] + woff) = w;
                 else for (int r2 = 0; r2 < p.dp; ++r2) *reinterpret_cast<float4*>(peers.W[r2] + woff) = w;   // publish to all replicas
             } else {
                 const float sv[4] = {sum.x, sum.y, sum.z, sum.w};
                 for (int e = 0; e < 4 && n + e < p.n_total; ++e) {
                     float d = sv[e];
-                    if constexpr (STATEFUL) d = elem_direction(p, woff + e, d, peers.W[me][woff + e]);
+                    if constexpr (STATEFUL) { if (rule) d = elem_direction(p, woff + e, d, peers.W[me][woff + e]); }
                     const float w = peers.W[me][woff + e] - lr * d;
+                    if constexpr (EMA) p.opt.E[woff + e] = ema_lerp(p.opt.E[woff + e], w, alpha);
                     if (n_pub == 1) peers.W[me][woff + e] = w;
                     else for (int r2 = 0; r2 < p.dp; ++r2) peers.W[r2][woff + e] = w;
                 }
@@ -169,8 +183,9 @@ __device__ void dp_owner_reduce_tile(const DpPeers& peers, const DpLayerParams& 
             for (int s = 0; s < p.dp; ++s)
                 sum += ld_cg_f(st0 + (int64_t)s * p.stage_src_stride + (int64_t)kBlockM * p.block_n + r);
             const int64_t boff = p.w_offset + (int64_t)m * p.ldw + p.n_total;
-            if constexpr (STATEFUL) sum = elem_direction(p, boff, sum, peers.W[me][boff]);
+            if constexpr (STATEFUL) { if (rule) sum = elem_direction(p, boff, sum, peers.W[me][boff]); }
             const float b = peers.W[me][boff] - lr * sum;
+            if constexpr (EMA) p.opt.E[boff] = ema_lerp(p.opt.E[boff], b, alpha);
             if (n_pub == 1) peers.W[me][boff] = b;
             else for (int r2 = 0; r2 < p.dp; ++r2) peers.W[r2][boff] = b;
         }
@@ -190,7 +205,7 @@ __device__ __forceinline__ void dp_wait_tile_done(const DpPeers& peers, const Dp
 // =============================================================================================
 // Kernel 1: WGRAD GEMM fused with the DP reduction + SGD + weight broadcast (persistent tiles)
 // =============================================================================================
-template <bool STATEFUL = false>
+template <bool STATEFUL = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads, 1)
 fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       const DpLayerParams p, const DpPeers peers) {
@@ -206,7 +221,7 @@ fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         // helper CTA (one-shot layers, one tile per CTA group): no GEMM - just its share of the reduce
         const uint32_t epoch_h = *reinterpret_cast<const volatile uint32_t*>(p.epoch_ptr);
         const TileCoord tc = tile_coord(p, blockIdx.x / p.helpers);
-        dp_owner_reduce_tile<STATEFUL>(peers, p, tc, epoch_h, threadIdx.x, kThreads, 1, blockIdx.x % p.helpers, p.helpers);
+        dp_owner_reduce_tile<STATEFUL, EMA>(peers, p, tc, epoch_h, threadIdx.x, kThreads, 1, blockIdx.x % p.helpers, p.helpers);
         return;
     }
     const int cta = p.helpers > 1 ? blockIdx.x / p.helpers : blockIdx.x;      // tile-group index
@@ -350,7 +365,7 @@ fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         for (int t = cta; t < num_tiles; t += n_cta) {
             const TileCoord tc = tile_coord(p, t);
             if (p.one_shot || tc.owner == p.rank)
-                dp_owner_reduce_tile<STATEFUL>(peers, p, tc, epoch, etid, 128, 1, 0, p.helpers > 1 ? p.helpers : 1, /*publish=*/!batch_flags);
+                dp_owner_reduce_tile<STATEFUL, EMA>(peers, p, tc, epoch, etid, 128, 1, 0, p.helpers > 1 ? p.helpers : 1, /*publish=*/!batch_flags);
         }
         if (batch_flags && !p.one_shot) {
             // all owned tiles of this CTA are reduced and their new weights stored into every replica: one fence, all flags
@@ -378,7 +393,7 @@ fused_wgrad_dp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 // =============================================================================================
 // Kernel 2: the same protocol on an already accumulated gradient block G (no GEMM)
 // =============================================================================================
-template <bool STATEFUL = false>
+template <bool STATEFUL = false, bool EMA = false>
 __global__ void __launch_bounds__(128, 1) dp_reduce_sgd_kernel(const DpLayerParams p, const DpPeers peers) {
     const uint32_t epoch = *reinterpret_cast<const volatile uint32_t*>(p.epoch_ptr);
     const int num_tiles = p.n_tiles_m * p.n_tiles_n;
@@ -422,7 +437,7 @@ __global__ void __launch_bounds__(128, 1) dp_reduce_sgd_kernel(const DpLayerPara
     }
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         const TileCoord tc = tile_coord(p, t);
-        if (p.one_shot || tc.owner == p.rank) dp_owner_reduce_tile<STATEFUL>(peers, p, tc, epoch, tid, 128, 1);
+        if (p.one_shot || tc.owner == p.rank) dp_owner_reduce_tile<STATEFUL, EMA>(peers, p, tc, epoch, tid, 128, 1);
     }
     if (tid == 0 && !p.one_shot) {
         for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
@@ -482,7 +497,7 @@ const char* fused_dp_plan(FusedDpPlan* plan, const float* dZ, int lddz, const fl
     return nullptr;
 }
 
-static bool stateful(const DpLayerParams& p) { return p.opt.momentum != 0.f || p.opt.weight_decay != 0.f; }
+static bool stateful(const DpLayerParams& p) { return p.opt.has_rule(); }
 
 int dp_element_owner(int proto, int in, int out, int ld, int64_t offset, int dp, int m, int n) {
     if (dp <= 1) return -1;
@@ -503,7 +518,9 @@ int dp_element_owner(int proto, int in, int out, int ld, int64_t offset, int dp,
 cudaError_t fused_dp_configure() {
     cudaError_t e = cudaFuncSetAttribute(fused_wgrad_dp_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
     if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(fused_wgrad_dp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+    e = cudaFuncSetAttribute(fused_wgrad_dp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(fused_wgrad_dp_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
 }
 cudaError_t launch_fused_wgrad_dp(const FusedDpPlan& plan, cudaStream_t stream) {
     static bool configured = false;
@@ -512,14 +529,17 @@ cudaError_t launch_fused_wgrad_dp(const FusedDpPlan& plan, cudaStream_t stream) 
         if (e != cudaSuccess) return e;
         configured = true;
     }
-    if (stateful(plan.p))
+    if (plan.p.opt.E != nullptr)
+        fused_wgrad_dp_kernel<true, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.p, plan.peers);
+    else if (stateful(plan.p))
         fused_wgrad_dp_kernel<true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.p, plan.peers);
     else
         fused_wgrad_dp_kernel<false><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.p, plan.peers);
     return cudaGetLastError();
 }
 cudaError_t launch_dp_reduce_sgd(const FusedDpPlan& plan, cudaStream_t stream) {
-    if (stateful(plan.p)) dp_reduce_sgd_kernel<true><<<plan.grid, 128, 0, stream>>>(plan.p, plan.peers);
+    if (plan.p.opt.E != nullptr) dp_reduce_sgd_kernel<true, true><<<plan.grid, 128, 0, stream>>>(plan.p, plan.peers);
+    else if (stateful(plan.p)) dp_reduce_sgd_kernel<true><<<plan.grid, 128, 0, stream>>>(plan.p, plan.peers);
     else dp_reduce_sgd_kernel<false><<<plan.grid, 128, 0, stream>>>(plan.p, plan.peers);
     return cudaGetLastError();
 }

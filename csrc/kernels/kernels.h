@@ -22,15 +22,21 @@ enum LossKind : int { LOSS_MSE = 0, LOSS_CROSS_ENTROPY = 1 };
 // Hyper-parameters of the SGD update beyond lr (torch.optim.SGD, dampening 0).  The default is plain SGD, w -= lr * g,
 // which runs the stateless kernels.  V: momentum buffer laid out like the weights it belongs to (nullptr when
 // momentum == 0: weight decay alone needs no state).
+// E: exponential moving average of the weights, laid out like them (nullptr: no EMA).  The lane that forms an element's
+// new weight w' also updates e = ema_lerp(e, w', *ema_alpha) (ptx.cuh); ema_alpha is one device float.  The EMA only
+// observes the update: w' is formed exactly as without it.
 struct SgdState {
     float* V = nullptr;
     float momentum = 0.f;
     float weight_decay = 0.f;
     int nesterov = 0;
-    bool plain() const { return momentum == 0.f && weight_decay == 0.f; }
+    float* E = nullptr;
+    const float* ema_alpha = nullptr;
+    bool plain() const { return momentum == 0.f && weight_decay == 0.f && E == nullptr; }
+    __host__ __device__ bool has_rule() const { return momentum != 0.f || weight_decay != 0.f; }   // the update direction is not the gradient
 };
-// nullptr if the combination is valid: 0 <= momentum < 1, weight_decay >= 0, nesterov only with momentum, and a
-// buffer exactly when momentum > 0
+// nullptr if the combination is valid: 0 <= momentum < 1, weight_decay >= 0, nesterov only with momentum, a buffer
+// exactly when momentum > 0, and E with ema_alpha or neither
 const char* sgd_state_check(const SgdState& s);
 
 // host: threshold and scale of drop probability p in [0, 1) (dropout.h)
@@ -100,6 +106,10 @@ struct GemmParams {
     int ldskip;
     float* gpre;
     int ldgpre;
+    // WGRAD with fuse_sgd: the EMA of the weights (SgdState::E, pitch ldw) and its device alpha.  E set runs the STATEFUL
+    // epilogue with EMA (tc_gemm_ema_kernel), whatever the rule.  Last, like drop.
+    float* E;
+    const float* ema_alpha;
 };
 
 struct GemmPlan {          // a fully prepared launch (tensor maps are 128 B each)
@@ -158,6 +168,7 @@ struct GemmGroupPlan {
     GemmGroupEntry* entries_dev;
     int n, smem_bytes, n_gemms;
     int stateful;                  // the plans use the stateful SGD rule (all of them or none)
+    int ema;                       // the plans update an EMA of the weights (all of them or none; implies stateful)
 };
 const char* gemm_group_plan(GemmGroupPlan* out, const GemmPlan* plans, int n_plans);
 cudaError_t gemm_group_launch(const GemmGroupPlan& plan, cudaStream_t stream);

@@ -37,11 +37,15 @@ __device__ __forceinline__ void multimem_red_release_add(uint32_t* mc_addr, uint
 
 // STATEFUL (SGD only): momentum / weight decay through sgd_direction; the owner of chunk c reads and writes its unicast
 // momentum V[c] (never multicast: no other replica touches chunk c's state).
-template <bool SGD, bool STATEFUL = false>
+// EMA (with STATEFUL): the owner of chunk c also moves its unicast EMA chunk (p.opt.E) towards the new weights; with a
+// plain rule the update is the stateless one.
+template <bool SGD, bool STATEFUL = false, bool EMA = false>
 __global__ void __launch_bounds__(256) nvls_reduce_kernel(const NvlsParams p) {
     const uint32_t epoch = *p.epoch + 1u;                     // same value on every replica (one bump per launch)
     const uint32_t target = epoch * (uint32_t)p.dp;
     const float lr = SGD ? *p.lr : 0.f;                      // learning rate of this step (device slot)
+    const float alpha = EMA ? *p.opt.ema_alpha : 0.f;
+    const bool rule = !EMA || p.opt.has_rule();
 
     // ---- my gradients are final (stream order: the wgrad kernels of this step precede this launch)
     if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -60,17 +64,28 @@ __global__ void __launch_bounds__(256) nvls_reduce_kernel(const NvlsParams p) {
         if (SGD) {
             float4 w = *reinterpret_cast<const float4*>(p.W_uc + 4 * c);
             if constexpr (STATEFUL) {
-                float4* vp = p.opt.V != nullptr ? reinterpret_cast<float4*>(p.opt.V + 4 * c) : nullptr;
-                float4 v = vp != nullptr ? *vp : make_float4(0.f, 0.f, 0.f, 0.f);
-                const float mu = p.opt.momentum, wd = p.opt.weight_decay;
-                const bool nv = p.opt.nesterov != 0;
-                w.x -= lr * sgd_direction<false>(g.x, w.x, v.x, mu, wd, nv);
-                w.y -= lr * sgd_direction<false>(g.y, w.y, v.y, mu, wd, nv);
-                w.z -= lr * sgd_direction<false>(g.z, w.z, v.z, mu, wd, nv);
-                w.w -= lr * sgd_direction<false>(g.w, w.w, v.w, mu, wd, nv);
-                if (vp != nullptr) *vp = v;
+                if (rule) {
+                    float4* vp = p.opt.V != nullptr ? reinterpret_cast<float4*>(p.opt.V + 4 * c) : nullptr;
+                    float4 v = vp != nullptr ? *vp : make_float4(0.f, 0.f, 0.f, 0.f);
+                    const float mu = p.opt.momentum, wd = p.opt.weight_decay;
+                    const bool nv = p.opt.nesterov != 0;
+                    w.x -= lr * sgd_direction<false>(g.x, w.x, v.x, mu, wd, nv);
+                    w.y -= lr * sgd_direction<false>(g.y, w.y, v.y, mu, wd, nv);
+                    w.z -= lr * sgd_direction<false>(g.z, w.z, v.z, mu, wd, nv);
+                    w.w -= lr * sgd_direction<false>(g.w, w.w, v.w, mu, wd, nv);
+                    if (vp != nullptr) *vp = v;
+                } else {
+                    w.x -= lr * g.x; w.y -= lr * g.y; w.z -= lr * g.z; w.w -= lr * g.w;
+                }
             } else {
                 w.x -= lr * g.x; w.y -= lr * g.y; w.z -= lr * g.z; w.w -= lr * g.w;
+            }
+            if constexpr (EMA) {
+                float4* ep = reinterpret_cast<float4*>(p.opt.E + 4 * c);
+                float4 t = *ep;
+                t.x = ema_lerp(t.x, w.x, alpha); t.y = ema_lerp(t.y, w.y, alpha);
+                t.z = ema_lerp(t.z, w.z, alpha); t.w = ema_lerp(t.w, w.w, alpha);
+                *ep = t;
             }
             multimem_st_f4(p.W_mc + 4 * c, w);
         } else {
@@ -105,7 +120,9 @@ static int nvls_grid(const NvlsParams& p, int max_ctas) {
 
 cudaError_t launch_nvls_reduce_sgd(const NvlsParams& p, int max_ctas, cudaStream_t stream) {
     if (p.lr == nullptr) return cudaErrorInvalidValue;
-    if (p.opt.momentum != 0.f || p.opt.weight_decay != 0.f)
+    if (p.opt.E != nullptr)
+        nvls_reduce_kernel<true, true, true><<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
+    else if (p.opt.has_rule())
         nvls_reduce_kernel<true, true><<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
     else
         nvls_reduce_kernel<true><<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);

@@ -393,6 +393,15 @@ __device__ __forceinline__ float sgd_direction(float g, float w, float& v, float
     }
 }
 
+// Exponential moving average of one weight: e moves towards the new weight w by alpha, with torch.lerp's formula
+//     alpha < 0.5 :  e + alpha * (w - e)          else :  w - (w - e) * (1 - alpha)
+// so alpha = 1 gives e = w exactly.  Every update site calls this, and the explicitly rounded operations keep the
+// compiler from contracting differently at different sites (ops.functional.ema_lerp_ref is the same formula in torch).
+__device__ __forceinline__ float ema_lerp(float e, float w, float alpha) {
+    const float diff = __fsub_rn(w, e);
+    return alpha < 0.5f ? __fadd_rn(e, __fmul_rn(alpha, diff)) : __fsub_rn(w, __fmul_rn(diff, __fsub_rn(1.f, alpha)));
+}
+
 // ------------------------------------------------------------------ softmax cross-entropy, per element of one row
 // torch's F.cross_entropy(z, t, reduction="sum") / B with probability targets, for one row of logits z and target t:
 //     m = max_k z_k ;  s = sum_k exp(z_k - m) ;  p_k = exp(z_k - m) / s ;  T = sum_k t_k

@@ -57,13 +57,17 @@ static constexpr int kGroupMinCtas = 3;                 // CTAs per SM the group
 // RES (with GATE; FWD / DGRAD, GemmParams::res): the residual form.  act_fwd_any applies ReLU as a gated kind too; the FWD
 // adds the skip input after the activation, the DGRAD adds the skip gradient before the mask and stores that pre-mask sum
 // to gpre.  The same kind of switch: the other instantiations compile as they did without it.
+// EMA (WGRAD with STATEFUL only, GemmParams::E): each lane also forms its elements' new weights w' = W + (-lr * d) with the
+// rounding of the TMA reduce-add that writes them, and moves its EMA entries towards them (ema_lerp).  With a plain rule
+// d is the gradient itself, as in the stateless code.  The same kind of switch.
 template <int MODE, bool SPLITK, bool STATEFUL = false, int BM = (int)kBlockM, bool DROP = false, bool GATE = false,
-          bool RES = false>
+          bool RES = false, bool EMA = false>
 __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
                                              const GemmParams& p, const int bx, const int by, const int bz) {
     constexpr bool A_MN = (MODE != GEMM_FWD);
     constexpr bool B_MN = (MODE == GEMM_WGRAD);
     static_assert(BM == (int)kBlockM || (BM == kGroupBM && MODE == GEMM_WGRAD && !SPLITK), "narrow tiles are WGRAD only");
+    static_assert(!EMA || (MODE == GEMM_WGRAD && STATEFUL), "the EMA rides on the STATEFUL update epilogue");
     constexpr int kWarpsM = BM / 32;                       // math warps along the tile's rows ...
     constexpr int kWarpsN = 4 / kWarpsM;                   // ... and along its columns
     constexpr int NT = kMaxBlockN / 8 / kWarpsN;           // n8 tiles a math warp holds at most
@@ -374,6 +378,9 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
             // narrow tile stage only their own half of a 16-column chunk.
             const float lr = STATEFUL ? *p.lr : lr_pre;            // STATEFUL implies fuse_sgd
             const float scale = p.fuse_sgd ? -lr : 1.f;
+            const float alpha = EMA ? *p.ema_alpha : 0.f;
+            // EMA with a plain rule: d is the gradient, exactly as in the stateless epilogue
+            const bool rule = !EMA || p.momentum != 0.f || p.weight_decay != 0.f;
             const int wcols = 8 * nt;
             const int n_lim = min(p.n_total, n0 + nw0 + wcols);
 #pragma unroll
@@ -383,7 +390,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                 warp_acc_row16(acc, ch, v, lane);
                 if constexpr (STATEFUL) {
                     const int nc = n0 + nw0 + 16 * ch;
-                    const bool has_v = p.V != nullptr, has_wd = p.weight_decay != 0.f;
+                    const bool has_v = p.V != nullptr, read_w = EMA || p.weight_decay != 0.f;   // weight decay and the EMA read W
                     float vm[16], wv[16];
 #pragma unroll
                     for (int j = 0; j < 16; ++j) { vm[j] = 0.f; wv[j] = 0.f; }
@@ -398,7 +405,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                                     const float4 t = *reinterpret_cast<const float4*>(p.V + row + 4 * q4);
                                     vm[4 * q4] = t.x; vm[4 * q4 + 1] = t.y; vm[4 * q4 + 2] = t.z; vm[4 * q4 + 3] = t.w;
                                 }
-                                if (has_wd) {
+                                if (read_w) {
                                     const float4 t = *reinterpret_cast<const float4*>(p.W + row + 4 * q4);
                                     wv[4 * q4] = t.x; wv[4 * q4 + 1] = t.y; wv[4 * q4 + 2] = t.z; wv[4 * q4 + 3] = t.w;
                                 }
@@ -408,7 +415,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                                     const int j = 4 * q4 + e;
                                     if (nc + j < n_lim) {
                                         if (has_v) vm[j] = p.V[row + j];
-                                        if (has_wd) wv[j] = p.W[row + j];
+                                        if (read_w) wv[j] = p.W[row + j];
                                     }
                                 }
                             }
@@ -417,8 +424,31 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
 #pragma unroll
                     for (int j = 0; j < 16; ++j) {
                         const bool ok = m_ok && nc + j < n_lim;
-                        const float d = sgd_direction<false>(v[j], wv[j], vm[j], p.momentum, p.weight_decay, p.nesterov != 0);
+                        const float d = rule ? sgd_direction<false>(v[j], wv[j], vm[j], p.momentum, p.weight_decay, p.nesterov != 0)
+                                             : v[j];
                         v[j] = ok ? d : 0.f;
+                    }
+                    if constexpr (EMA) {
+                        // w' = W + (-lr * d): the product the tile stores, then the fp32 add of the TMA reduce-add
+                        if (m_ok) {
+                            float* erow = p.E + (size_t)m * p.ldw + nc;
+#pragma unroll
+                            for (int q4 = 0; q4 < 4; ++q4) {
+                                float nw[4];
+#pragma unroll
+                                for (int e = 0; e < 4; ++e) nw[e] = __fadd_rn(wv[4 * q4 + e], __fmul_rn(v[4 * q4 + e], scale));
+                                if (nc + 4 * q4 + 3 < n_lim) {
+                                    float4 t = *reinterpret_cast<const float4*>(erow + 4 * q4);
+                                    t.x = ema_lerp(t.x, nw[0], alpha); t.y = ema_lerp(t.y, nw[1], alpha);
+                                    t.z = ema_lerp(t.z, nw[2], alpha); t.w = ema_lerp(t.w, nw[3], alpha);
+                                    *reinterpret_cast<float4*>(erow + 4 * q4) = t;
+                                } else {
+#pragma unroll
+                                    for (int e = 0; e < 4; ++e)
+                                        if (nc + 4 * q4 + e < n_lim) erow[4 * q4 + e] = ema_lerp(erow[4 * q4 + e], nw[e], alpha);
+                                }
+                            }
+                        }
                     }
                     if (m_ok && has_v) {
                         const size_t row = (size_t)m * p.ldw + nc;
@@ -470,7 +500,15 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                 if (p.fuse_sgd) {
                     const size_t boff = (size_t)m * p.ldw + (p.db - p.G);  // bias lives at the same offset in W (and V)
                     float* bp = p.W + boff;
-                    if constexpr (STATEFUL) {
+                    if constexpr (EMA) {
+                        float vb = p.V != nullptr ? p.V[boff] : 0.f;
+                        const float d = rule ? sgd_direction<false>(dbsum, *bp, vb, p.momentum, p.weight_decay, p.nesterov != 0)
+                                             : dbsum;
+                        if (p.V != nullptr) p.V[boff] = vb;
+                        const float nb = *bp - lr * d;              // formed once: the stored bias is what the EMA sees
+                        *bp = nb;
+                        p.E[boff] = ema_lerp(p.E[boff], nb, alpha);
+                    } else if constexpr (STATEFUL) {
                         float vb = p.V != nullptr ? p.V[boff] : 0.f;
                         const float d = sgd_direction<false>(dbsum, *bp, vb, p.momentum, p.weight_decay, p.nesterov != 0);
                         if (p.V != nullptr) p.V[boff] = vb;
@@ -531,6 +569,20 @@ __global__ void __launch_bounds__(kThreads, kGroupMinCtas) tc_wgrad_group_kernel
     tc_gemm_body<GEMM_WGRAD, false, STATEFUL, kGroupBM>(e.tmA, e.tmB, e.tmC, p, e.bx, e.by, 0);
 }
 
+// The fused update with an EMA of the weights (GemmParams::E): the per-layer and the grouped launch, kernels of their own
+// like tc_gemm_drop_kernel
+__global__ void __launch_bounds__(kThreads, 1)
+tc_gemm_ema_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+    tc_gemm_body<GEMM_WGRAD, false, true, (int)kBlockM, false, false, false, true>(tmA, tmB, tmC, p, (int)blockIdx.x,
+                                                                                  (int)blockIdx.y, 0);
+}
+__global__ void __launch_bounds__(kThreads, kGroupMinCtas) tc_wgrad_group_ema_kernel(const GemmGroupEntry* __restrict__ entries) {
+    const GemmGroupEntry& e = entries[blockIdx.x];
+    const GemmParams p = e.p;
+    tc_gemm_body<GEMM_WGRAD, false, true, kGroupBM, false, false, false, true>(e.tmA, e.tmB, e.tmC, p, e.bx, e.by, 0);
+}
+
 // =========================================================================== host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -579,13 +631,15 @@ const char* make_tmap_k(CUtensorMap* map, const float* base, int inner, int oute
 
 static int round_up_i(int x, int m) { return (x + m - 1) / m * m; }
 
-static bool is_stateful(const GemmParams& p) { return p.fuse_sgd && (p.momentum != 0.f || p.weight_decay != 0.f); }
+static bool is_stateful(const GemmParams& p) { return p.fuse_sgd && (p.momentum != 0.f || p.weight_decay != 0.f || p.E != nullptr); }
+static bool has_ema(const GemmParams& p) { return p.fuse_sgd && p.E != nullptr; }
 
 const char* sgd_state_check(const SgdState& s) {
     if (!(s.momentum >= 0.f && s.momentum < 1.f)) return "momentum must be in [0, 1)";
     if (!(s.weight_decay >= 0.f)) return "weight_decay must be >= 0";
     if (s.nesterov && s.momentum == 0.f) return "nesterov needs momentum > 0";
     if ((s.momentum > 0.f) != (s.V != nullptr)) return "a momentum buffer is needed exactly when momentum > 0";
+    if ((s.E != nullptr) != (s.ema_alpha != nullptr)) return "an EMA buffer needs its alpha (a device float), and only it";
     return nullptr;
 }
 
@@ -655,9 +709,10 @@ const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const flo
     // (column `in` of G's block) names a slot of W
     if (fuse_sgd && db != nullptr && db != G + in) return "fuse_sgd needs db to be G's bias column (G + in)";
     if (!opt.plain()) {
-        if (!fuse_sgd) return "momentum / weight decay need fuse_sgd (the update rule runs in the epilogue)";
+        if (!fuse_sgd) return "momentum / weight decay / an EMA need fuse_sgd (the update rule runs in the epilogue)";
         if (const char* e = sgd_state_check(opt)) return e;
         p.V = opt.V; p.momentum = opt.momentum; p.weight_decay = opt.weight_decay; p.nesterov = opt.nesterov;
+        p.E = opt.E; p.ema_alpha = opt.ema_alpha;
     }
     // output tile map: [out, in] with the block's row pitch; fused SGD targets W itself
     if (const char* e = make_tmap(&plan->tmC, fuse_sgd ? W : G, in, out, fuse_sgd ? ldw : ldg, kBlockM)) return e;
@@ -729,12 +784,13 @@ const char* gemm_group_plan(GemmGroupPlan* out, const GemmPlan* plans, int n_pla
     if (n_plans < 1) return "gemm_group_plan: no plans";
     std::vector<GemmGroupEntry> host;
     int smem = 0;
-    const bool stateful = is_stateful(plans[0].p);
+    const bool stateful = is_stateful(plans[0].p), ema = has_ema(plans[0].p);
     for (int i = 0; i < n_plans; ++i) {
         const GemmPlan& g = plans[i];
         if (g.mode != GEMM_WGRAD) return "gemm_group_plan: only weight-gradient GEMMs can be grouped";
         if (g.p.k_splits > 1) return "gemm_group_plan: split-K plans cannot be grouped";
         if (is_stateful(g.p) != stateful) return "gemm_group_plan: plans mix the plain and the stateful SGD rule";
+        if (has_ema(g.p) != ema) return "gemm_group_plan: plans mix updates with and without an EMA";
         std::vector<GemmGroupTile> tiles;
         int stages = 0, bytes = 0;
         if (const char* e = gemm_group_tiles(g.p.m_total, g.p.n_total, g.p.k_total, &tiles, &stages, &bytes)) return e;
@@ -760,6 +816,7 @@ const char* gemm_group_plan(GemmGroupPlan* out, const GemmPlan* plans, int n_pla
     }
     out->entries_dev = dev; out->n = (int)host.size(); out->smem_bytes = smem; out->n_gemms = n_plans;
     out->stateful = stateful ? 1 : 0;
+    out->ema = ema ? 1 : 0;
     return nullptr;
 }
 
@@ -786,6 +843,9 @@ cudaError_t gemm_configure() {
     // the narrow tiles are meant to share an SM: ask for the carveout that fits the most of them
     if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_gemm_ema_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_wgrad_group_ema_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(tc_wgrad_group_ema_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_FWD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_DGRAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(tc_gemm_drop_kernel<GEMM_FWD, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
@@ -813,7 +873,9 @@ cudaError_t gemm_group_launch(const GemmGroupPlan& plan, cudaStream_t stream) {
         cudaError_t e = gemm_configure();
         if (e != cudaSuccess) return e;
     }
-    if (plan.stateful)
+    if (plan.ema)
+        tc_wgrad_group_ema_kernel<<<plan.n, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev);
+    else if (plan.stateful)
         tc_wgrad_group_kernel<true><<<plan.n, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev);
     else
         tc_wgrad_group_kernel<false><<<plan.n, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev);
@@ -863,6 +925,11 @@ static cudaError_t launch_mode(const GemmPlan& plan, cudaStream_t stream) {
             return cudaGetLastError();
         }
     } else {
+        if (has_ema(plan.p)) {
+            tc_gemm_ema_kernel<<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
+            g_launches.fetch_add(1, std::memory_order_relaxed);
+            return cudaGetLastError();
+        }
         if (is_stateful(plan.p)) {
             tc_gemm_kernel<MODE, false, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
             g_launches.fetch_add(1, std::memory_order_relaxed);

@@ -221,14 +221,18 @@ private:
 class PyEngine {
 public:
     PyEngine(const std::vector<std::tuple<int, int, int, int64_t, int>>& layers, py::dict cfg, torch::Tensor weights,
-             torch::Tensor grads, c10::optional<torch::Tensor> momentum)
-        : weights_(weights), grads_(grads), momentum_(momentum) {
+             torch::Tensor grads, c10::optional<torch::Tensor> momentum, c10::optional<torch::Tensor> ema)
+        : weights_(weights), grads_(grads), momentum_(momentum), ema_(ema) {
         TORCH_CHECK(weights.is_cuda() && grads.is_cuda() && weights.is_contiguous() && grads.is_contiguous());
         TORCH_CHECK(weights.scalar_type() == torch::kFloat32 && grads.scalar_type() == torch::kFloat32);
         if (momentum.has_value())
             TORCH_CHECK(momentum->is_cuda() && momentum->is_contiguous() && momentum->scalar_type() == torch::kFloat32 &&
                             momentum->numel() >= weights.numel() && momentum->device() == weights.device(),
                         "PipeEngine: the momentum arena must be a contiguous fp32 CUDA buffer covering the weight arena");
+        if (ema.has_value())
+            TORCH_CHECK(ema->is_cuda() && ema->is_contiguous() && ema->scalar_type() == torch::kFloat32 &&
+                            ema->numel() >= weights.numel() && ema->device() == weights.device(),
+                        "PipeEngine: the EMA arena must be a contiguous fp32 CUDA buffer covering the weight arena");
         EngineConfig c;
         for (auto& t : layers) c.layers.push_back({std::get<0>(t), std::get<1>(t), std::get<2>(t), std::get<3>(t), std::get<4>(t)});
         auto geti = [&](const char* k, int dflt) { return cfg.contains(k) ? cfg[k].cast<int>() : dflt; };
@@ -244,6 +248,10 @@ public:
         c.momentum = cfg.contains("momentum") ? cfg["momentum"].cast<float>() : 0.f;
         c.weight_decay = cfg.contains("weight_decay") ? cfg["weight_decay"].cast<float>() : 0.f;
         c.nesterov = geti("nesterov", 0);
+        c.ema_decay = cfg.contains("ema_decay") ? cfg["ema_decay"].cast<float>() : 0.f;
+        TORCH_CHECK(c.ema_decay == 0.f || (c.ema_decay > 0.f && c.ema_decay < 1.f),
+                    "PipeEngine: cfg['ema_decay'] must be in (0, 1), got ", c.ema_decay);
+        TORCH_CHECK((c.ema_decay > 0.f) == ema.has_value(), "PipeEngine: an EMA arena is needed exactly when cfg['ema_decay'] is set");
         c.loss = geti("loss", ssb::LOSS_MSE);
         TORCH_CHECK(c.loss == ssb::LOSS_MSE || c.loss == ssb::LOSS_CROSS_ENTROPY,
                     "PipeEngine: cfg['loss'] must be 0 (MSE) or 1 (cross-entropy), got ", c.loss);
@@ -267,7 +275,8 @@ public:
         }
         c10::cuda::CUDAGuard guard(weights.device());
         engine_ = std::make_unique<PipeEngine>(c, weights.data_ptr<float>(), grads.data_ptr<float>(), weights.numel(),
-                                               momentum.has_value() ? momentum->data_ptr<float>() : nullptr);
+                                               momentum.has_value() ? momentum->data_ptr<float>() : nullptr,
+                                               ema.has_value() ? ema->data_ptr<float>() : nullptr);
     }
     void set_pp_comm(std::shared_ptr<NcclComm> c) { pp_ = c; engine_->set_pp_comm(c->get()); }
     void set_dp_comm(std::shared_ptr<NcclComm> c) { dp_ = c; engine_->set_dp_comm(c->get()); }
@@ -344,6 +353,10 @@ public:
         engine_->set_lr((float)lr);
     }
     float lr() { return engine_->lr(); }
+    void set_ema_alpha(double alpha) {
+        TORCH_CHECK(alpha > 0.0 && alpha <= 1.0, "PipeEngine.set_ema_alpha: alpha must be in (0, 1], got ", alpha);
+        engine_->set_ema_alpha((float)alpha);
+    }
     void set_dropout_step(int64_t step) {
         TORCH_CHECK(step >= 0, "PipeEngine.set_dropout_step: the step must be >= 0, got ", step);
         engine_->set_dropout_step((uint32_t)(step & 0xffffffffLL));   // the masks' step counter is the step mod 2^32
@@ -408,6 +421,7 @@ private:
     }
     torch::Tensor weights_, grads_;
     c10::optional<torch::Tensor> momentum_;   // kept alive: the plan holds raw pointers into it
+    c10::optional<torch::Tensor> ema_;        // the same
     std::pair<c10::optional<torch::Tensor>, c10::optional<torch::Tensor>> held_[2];
     unsigned hold_i_ = 0;
     std::shared_ptr<NcclComm> pp_, dp_;
@@ -459,8 +473,9 @@ void bind_runtime(py::module_& m) {
         .def("buffers", &PyPpContext::buffers);
     py::class_<PyEngine>(m, "PipeEngine")
         .def(py::init<const std::vector<std::tuple<int, int, int, int64_t, int>>&, py::dict, torch::Tensor, torch::Tensor,
-                      c10::optional<torch::Tensor>>(),
-             py::arg("layers"), py::arg("cfg"), py::arg("weights"), py::arg("grads"), py::arg("momentum") = py::none())
+                      c10::optional<torch::Tensor>, c10::optional<torch::Tensor>>(),
+             py::arg("layers"), py::arg("cfg"), py::arg("weights"), py::arg("grads"), py::arg("momentum") = py::none(),
+             py::arg("ema") = py::none())
         .def("set_pp_comm", &PyEngine::set_pp_comm)
         .def("set_dp_comm", &PyEngine::set_dp_comm)
         .def("set_dp_context", &PyEngine::set_dp_context)
@@ -478,6 +493,7 @@ void bind_runtime(py::module_& m) {
         .def("set_lr", &PyEngine::set_lr, py::arg("lr"))
         .def("lr", &PyEngine::lr)
         .def("set_dropout_step", &PyEngine::set_dropout_step, py::arg("step"))
+        .def("set_ema_alpha", &PyEngine::set_ema_alpha, py::arg("alpha"))
         .def("synchronize", &PyEngine::synchronize)
         .def("wait", &PyEngine::wait)
         .def("comm_status", &PyEngine::comm_status)

@@ -54,9 +54,12 @@ static void cu_check(CUresult r, const char* what) {
 // leave some SMs to the concurrently running dgrad chain; also bounds co-residency needs
 static constexpr int kFusedDpMaxCtas = 120;
 
-PipeEngine::PipeEngine(const EngineConfig& cfg, float* weights, float* grads, int64_t arena_numel, float* momentum)
-    : cfg_(cfg), W_(weights), G_(grads), V_(momentum), arena_numel_(arena_numel), L_((int)cfg.layers.size()) {
-    const SgdState opt = opt_for(0);
+PipeEngine::PipeEngine(const EngineConfig& cfg, float* weights, float* grads, int64_t arena_numel, float* momentum, float* ema)
+    : cfg_(cfg), W_(weights), G_(grads), V_(momentum), E_(ema), arena_numel_(arena_numel), L_((int)cfg.layers.size()) {
+    if ((cfg_.ema_decay > 0.f) != (E_ != nullptr)) throw std::runtime_error("PipeEngine: an EMA arena is needed exactly when ema_decay > 0");
+    if (!(cfg_.ema_decay >= 0.f && cfg_.ema_decay < 1.f)) throw std::runtime_error("PipeEngine: ema_decay must be 0 (no EMA) or in (0, 1)");
+    SgdState opt = opt_for(0);
+    opt.E = nullptr;                                      // the rule alone: the EMA alpha slot does not exist yet
     if (const char* e = sgd_state_check(opt)) throw std::runtime_error(std::string("PipeEngine: ") + e);
     // who owns which momentum entries: every replica unless a layer's update runs in an owner-based DP reduction
     layer_proto_.assign(L_, (cfg_.training && cfg_.dp_mode == 3 && cfg_.dp_size > 1) ? DP_PROTO_NVLS : DP_PROTO_ALL);
@@ -75,10 +78,14 @@ PipeEngine::PipeEngine(const EngineConfig& cfg, float* weights, float* grads, in
     alloc_buffers();
 }
 
-SgdState PipeEngine::opt_for(int layer) const {
+SgdState PipeEngine::opt_for(int layer, int set) const {
     SgdState s;
     s.momentum = cfg_.momentum; s.weight_decay = cfg_.weight_decay; s.nesterov = cfg_.nesterov;
     if (V_ != nullptr) s.V = V_ + (layer >= 1 ? cfg_.layers[layer - 1].offset : 0);
+    if (ema_on()) {
+        s.E = E_ + (layer >= 1 ? cfg_.layers[layer - 1].offset : 0);
+        s.ema_alpha = alpha_dev_ + (set >= 0 ? set : cur_set_);
+    }
     return s;
 }
 
@@ -125,6 +132,11 @@ void PipeEngine::alloc_buffers() {
     lr_ = lr_written_[0] = lr_written_[1] = cfg_.lr;
     const float lr_init[2] = {cfg_.lr, cfg_.lr};
     CUDA_CHECK(cudaMemcpy(lr_dev_, lr_init, sizeof(lr_init), cudaMemcpyHostToDevice));
+    if (ema_on()) {
+        alpha_dev_ = dalloc(2);
+        const float alpha_init[2] = {alpha_, alpha_};
+        CUDA_CHECK(cudaMemcpy(alpha_dev_, alpha_init, sizeof(alpha_init), cudaMemcpyHostToDevice));
+    }
     if (dropout_on()) {
         step_dev_ = reinterpret_cast<uint32_t*>(dalloc(2));   // zeroed: step 0
         step_ = step_written_[0] = step_written_[1] = 0u;
@@ -1152,7 +1164,7 @@ void PipeEngine::exec(const Op& op, int set) {
             else CUDA_CHECK(launch_relu_mask(op.a, op.lda, op.b, op.ldb, op.rows, op.cols, st));
             break;
         case OP_SGD: {
-            const SgdState opt = opt_for(0);
+            const SgdState opt = opt_for(0, set);
             if (opt.plain()) CUDA_CHECK(launch_sgd(op.a, op.b, op.lr, op.n, st));
             else CUDA_CHECK(launch_sgd_momentum(op.a, op.b, op.lr, opt, op.n, st));
             break;
@@ -1165,7 +1177,7 @@ void PipeEngine::exec(const Op& op, int set) {
             CUDA_CHECK(cudaGetDevice(&dev));
             CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
             NvlsParams np = nvls_ctx_->params();
-            np.opt = opt_for(0);
+            np.opt = opt_for(0, set);
             np.lr = op.lr;
             CUDA_CHECK(launch_nvls_reduce_sgd(np, sms, st));
             break;
@@ -1354,6 +1366,15 @@ void PipeEngine::run() {
         step_written_[set] = step_;
         wait_copy = true;
     }
+    if (ema_on() && alpha_written_[set] != alpha_) {   // the same protocol for the EMA alpha
+        uint32_t bits;
+        memcpy(&bits, &alpha_, sizeof(bits));
+        CUDA_CHECK(cudaStreamWaitEvent(copy_stream_, ev_done_[set], 0));
+        cu_check(memset_d32_async()(reinterpret_cast<CUdeviceptr>(alpha_dev_ + set), bits, 1, copy_stream_), "cuMemsetD32Async");
+        CUDA_CHECK(cudaEventRecord(ev_copy_[set], copy_stream_));
+        alpha_written_[set] = alpha_;
+        wait_copy = true;
+    }
     if (wait_copy) CUDA_CHECK(cudaStreamWaitEvent(streams_[0], ev_copy_[set], 0));
     if (graph_exec_sets_[set]) CUDA_CHECK(cudaGraphLaunch(graph_exec_sets_[set], streams_[0]));
     else walk(set);
@@ -1471,6 +1492,7 @@ std::string PipeEngine::describe() const {
         os << ", update=sgd(lr=" << lr_;
         if (cfg_.momentum != 0.f) os << ", momentum=" << cfg_.momentum << (cfg_.nesterov ? ", nesterov" : "");
         if (cfg_.weight_decay != 0.f) os << ", weight_decay=" << cfg_.weight_decay;
+        if (ema_on()) os << ", ema=" << cfg_.ema_decay;
         os << ")";
     }
     if (cfg_.loss == LOSS_CROSS_ENTROPY) os << ", loss=cross_entropy";

@@ -98,6 +98,10 @@ struct EngineConfig {
     // replica updates only the entries it owns (layer_protocols()).
     float momentum = 0.f, weight_decay = 0.f;
     int nesterov = 0;
+    // EMA of the weights (0 = none): the engine's EMA arena (the weights' layout) moves towards every new weight by the
+    // alpha of set_ema_alpha, in the lane that forms it; under the in-kernel DP reductions only the owner's entries.
+    // The decay itself is only named by describe(): the alpha sequence is the caller's.
+    float ema_decay = 0.f;
     int loss = LOSS_MSE;    // LossKind of the last stage's head (the chain kernel's and loss_head_kernel's)
     // inverted dropout on every ReLU'd layer of a training plan (0 = off; inference plans ignore it).  layer_base: the
     // global index of this stage's first Linear (the masks' layer counter); dp_size / dp_rank map rows to samples.
@@ -117,7 +121,9 @@ struct EngineConfig {
 class PipeEngine {
 public:
     // momentum: flat momentum arena (arena_numel floats, the weights' offsets), nullptr unless cfg.momentum > 0
-    explicit PipeEngine(const EngineConfig& cfg, float* weights, float* grads, int64_t arena_numel, float* momentum = nullptr);
+    // ema: flat EMA arena (the same layout), nullptr unless cfg.ema_decay > 0
+    explicit PipeEngine(const EngineConfig& cfg, float* weights, float* grads, int64_t arena_numel, float* momentum = nullptr,
+                        float* ema = nullptr);
     ~PipeEngine();
 
     // communicators (optional): created by the caller from ncclUniqueIds exchanged over torch.distributed
@@ -145,6 +151,11 @@ public:
     // rewritten by run() only when it changed, and only by plans with dropout on)
     void set_dropout_step(uint32_t step) { step_ = step; }
     uint32_t dropout_step() const { return step_; }
+    // alpha of the EMA updates of the steps run from now on; kept like lr (a device slot per staging set, rewritten by
+    // run() only when it changed, and only by training plans with an EMA)
+    void set_ema_alpha(float alpha) { alpha_ = alpha; }
+    float ema_alpha() const { return alpha_; }
+    bool ema_on() const { return cfg_.training && E_ != nullptr; }
     bool dropout_on() const { return cfg_.training && cfg_.dropout > 0.0; }
     // a training plan of a smooth activation: the forward stores gates, the backward multiplies by them
     // (or of a residual model, any activation)
@@ -211,9 +222,11 @@ private:
     void exec(const Op& op, int set);   // set: the staging set whose plan the op belongs to
     cudaStream_t stream_of(const Op& op) const;
 
-    SgdState opt_for(int layer) const;   // the update rule for layer l's block (l = 0: the whole arena)
+    // the update rule for layer l's block (l = 0: the whole arena), with the EMA alpha slot of staging set `set` (< 0: the
+    // set being planned)
+    SgdState opt_for(int layer, int set = -1) const;
     EngineConfig cfg_;
-    float *W_, *G_, *V_;
+    float *W_, *G_, *V_, *E_;
     std::vector<int> layer_proto_;
     int64_t arena_numel_;
     int L_;
@@ -286,6 +299,10 @@ private:
     uint32_t* step_dev_ = nullptr;
     uint32_t step_written_[2] = {0u, 0u};
     uint32_t step_ = 0u;
+    // EMA alpha: the same scheme as lr (allocated only when ema_on())
+    float* alpha_dev_ = nullptr;
+    float alpha_written_[2] = {1.f, 1.f};
+    float alpha_ = 1.f;
     DropoutSpec drop_for(int layer, int row_base) const;   // layer l (1-based) of the plan being built; off when !dropout_on()
     cudaStream_t copy_stream_ = nullptr;
     cudaEvent_t ev_copy_[2], ev_done_[2];

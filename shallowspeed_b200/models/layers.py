@@ -70,6 +70,9 @@ class ParamArena:
         # plain SGD costs no memory.  Ordinary device memory even when the weights live in memory shared with peers:
         # only this replica ever reads or writes it.
         self.momentum: Optional[torch.Tensor] = None
+        # exponential moving average of the weights, the same layout; allocated by ``enable_ema`` only, and ordinary
+        # device memory for the same reason as ``momentum``
+        self.ema: Optional[torch.Tensor] = None
         self._listeners: list[Callable[[], None]] = []
 
     # -- views ---------------------------------------------------------------
@@ -99,6 +102,20 @@ class ParamArena:
             self.momentum = torch.zeros(self.numel, dtype=torch.float32, device=self.weights.device)
         return self.momentum
 
+    def ema_block(self, i: int) -> torch.Tensor:
+        """The ``[out, ld]`` block *i* of the EMA buffer (bias in column ``in``)."""
+        o, _ = self.blocks[i]
+        return self.ema[self.offsets[i] : self.offsets[i] + o * self.lds[i]].view(o, self.lds[i])
+
+    def enable_ema(self):
+        """Allocate the EMA buffer on the weights' device as a copy of the current weights (padding stays zero); a
+        no-op when it exists."""
+        if self.ema is None:
+            self.ema = torch.zeros(self.numel, dtype=torch.float32, device=self.weights.device)
+            for i, (_, k) in enumerate(self.blocks):
+                self.ema_block(i)[:, : k + 1].copy_(self.block(i)[:, : k + 1])
+        return self.ema
+
     def on_rebind(self, fn: Callable[[], None]):
         self._listeners.append(fn)
 
@@ -113,6 +130,8 @@ class ParamArena:
         self.weights, self.grads = weights, grads
         if self.momentum is not None and self.momentum.device != weights.device:
             self.momentum = self.momentum.to(weights.device)
+        if self.ema is not None and self.ema.device != weights.device:
+            self.ema = self.ema.to(weights.device)
         for fn in self._listeners:
             fn()
 

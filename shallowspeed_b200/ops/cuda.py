@@ -111,15 +111,18 @@ def linear_dgrad(dz, weight, mask=None, out=None, precision=None, k_splits=0, ac
 
 
 def linear_wgrad(dz, x, grad_w, accumulate=False, grad_b=None, weight=None, lr=0.0, fuse_sgd=False, precision=None,
-                 velocity=None, momentum=0.0, weight_decay=0.0, nesterov=False):
+                 velocity=None, momentum=0.0, weight_decay=0.0, nesterov=False, ema=None, ema_alpha=None):
     """grad_w[out, in] (+)= dz^T @ x ; grad_b (+)= colsum(dz).  With ``fuse_sgd`` the update goes straight into
     ``weight`` (TMA reduce-add of -lr * dW).  ``momentum`` / ``weight_decay`` / ``nesterov`` select the stateful rule
     in that epilogue; ``velocity`` is then the momentum buffer laid out like ``weight`` (same row pitch).  ``lr`` is a
-    number or a one-element fp32 CUDA tensor (see ``_lr_arg``)."""
+    number or a one-element fp32 CUDA tensor (see ``_lr_arg``).  ``ema`` (laid out like ``weight``, bias in column
+    ``in`` with ``grad_b``) moves towards the new weights by ``ema_alpha`` (a number or a device scalar, like ``lr``):
+    ``ops.functional.ema_lerp_ref``."""
     dz, x = as_tma(dz), as_tma(x)
     b, bstride = _bias_arg(grad_b, dz.size(1))
     _C.linear_wgrad(dz, x, grad_w, bool(accumulate), b, bstride, weight, _lr_arg(lr), bool(fuse_sgd), _prec(precision),
-                    velocity, float(momentum), float(weight_decay), bool(nesterov))
+                    velocity, float(momentum), float(weight_decay), bool(nesterov), ema,
+                    None if ema_alpha is None else _lr_arg(ema_alpha))
     return grad_w
 
 
@@ -231,11 +234,13 @@ def sgd_step_(weights_flat, grads_flat, lr):
     _C.sgd_(weights_flat, grads_flat, _lr_arg(lr))
 
 
-def sgd_momentum_step_(weights_flat, grads_flat, momentum_flat, lr, momentum, weight_decay=0.0, nesterov=False):
+def sgd_momentum_step_(weights_flat, grads_flat, momentum_flat, lr, momentum, weight_decay=0.0, nesterov=False, ema=None,
+                       ema_alpha=None):
     """torch.optim.SGD's rule (dampening 0) over flat buffers in one pass; ``momentum_flat`` (None when
-    ``momentum == 0``) is updated in place."""
+    ``momentum == 0``) is updated in place.  ``ema`` (flat, like the weights) moves towards the new weights by
+    ``ema_alpha`` (``ops.functional.ema_lerp_ref``); with a plain rule the weights round as in ``sgd_step_``."""
     _C.sgd_momentum_(weights_flat, grads_flat, momentum_flat, _lr_arg(lr), float(momentum), float(weight_decay),
-                     bool(nesterov))
+                     bool(nesterov), ema, None if ema_alpha is None else _lr_arg(ema_alpha))
 
 
 def count_correct(pred, target):

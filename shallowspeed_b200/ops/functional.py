@@ -173,6 +173,37 @@ def dropout_ref(a: torch.Tensor, keep: torch.Tensor, scale: float) -> torch.Tens
 
 
 # ----------------------------------------------------------------------------
+# exponential moving average of the weights (torch.optim.swa_utils.get_ema_multi_avg_fn), the same math as
+# csrc/kernels/ptx.cuh: ema_lerp
+# ----------------------------------------------------------------------------
+def check_ema_decay(decay):
+    """``decay`` itself, or ValueError unless it is None or a float with 0 < decay < 1."""
+    if decay is None:
+        return None
+    if isinstance(decay, bool) or not isinstance(decay, (int, float)) or not 0.0 < float(decay) < 1.0:
+        raise ValueError(f"ema_decay must be None or a float in (0, 1), got {decay!r}")
+    return float(decay)
+
+
+def ema_alpha(decay: float, n: int) -> float:
+    """Weight of the new weights in EMA update ``n`` (0-based): 1 for the first update (the EMA becomes the weights),
+    else 1 - decay, computed in fp64 and rounded to fp32 once."""
+    if n == 0:
+        return 1.0
+    return float(torch.tensor(1.0 - float(decay), dtype=torch.float64).to(torch.float32))
+
+
+def ema_lerp_ref(e: torch.Tensor, w: torch.Tensor, alpha: float) -> torch.Tensor:
+    """torch.lerp(e, w, alpha)'s formula in fp32, one tensor op per rounding, so nothing can be contracted:
+    ``e + alpha * (w - e)`` for alpha < 0.5, else ``w - (w - e) * (1 - alpha)``.  The native kernels match it bit for bit."""
+    a = torch.tensor(alpha, dtype=torch.float32, device=e.device)
+    diff = w - e
+    if alpha < 0.5:
+        return e + a * diff
+    return w - diff * (torch.ones((), dtype=torch.float32, device=e.device) - a)
+
+
+# ----------------------------------------------------------------------------
 # tensor-core precision of the native GEMMs: the names a user passes and their codes in the native runtime
 # (csrc/kernels/precision.h: Precision).  fp32 (the default) = 3xTF32, fp32-equivalent products; tf32 = one TF32 pass;
 # bf16 = operands rounded to bf16 (nearest even) in registers, fp32 accumulation.  Storage is fp32 in every mode.

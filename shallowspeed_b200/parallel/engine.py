@@ -239,6 +239,10 @@ class NativeWorker:
         if self.momentum > 0.0 and getattr(optimizer, "arena", None) is not model.arena:
             raise ValueError("NativeWorker: SGD with momentum must be built with arena=model.arena (the engine keeps the "
                              "momentum in the arena's buffer)")
+        self.ema_decay = getattr(optimizer, "ema_decay", None)
+        if self.ema_decay is not None and getattr(optimizer, "arena", None) is not model.arena:
+            raise ValueError("NativeWorker: SGD with an EMA must be built with arena=model.arena (the engine keeps the "
+                             "EMA in the arena's buffer)")
         self._dp_ctx = None
         self._nvls_ctx = None
         # Engines that share a communicator (train + validation worker on one pipeline group) run on their own
@@ -269,9 +273,13 @@ class NativeWorker:
 
     def set_lr(self, eng, sched: Schedule):
         """Hand the optimizer's current learning rate to ``eng`` before it runs a training step (the engine rewrites
-        its device slot only when the value changed)."""
+        its device slot only when the value changed).  Every call precedes exactly one run of ``eng``, so a training
+        call also hands over the alpha of that step's EMA update and counts the update."""
         if sched.training and self.optimizer is not None:
             eng.set_lr(float(self.optimizer.lr))
+            if self.ema_decay is not None:
+                eng.set_ema_alpha(float(self.optimizer.ema_alpha))
+                self.optimizer.ema_updates += 1
         if sched.training and getattr(self.model, "dropout", 0.0) > 0.0:   # the step whose dropout masks this step draws
             eng.set_dropout_step(int(self.model.dropout_step))
 
@@ -299,6 +307,10 @@ class NativeWorker:
         if training and (self.momentum != 0.0 or self.weight_decay != 0.0):
             cfg.update(momentum=self.momentum, weight_decay=self.weight_decay, nesterov=int(self.nesterov))
             momentum = m.arena.momentum if self.momentum > 0.0 else None
+        ema = None
+        if training and self.ema_decay is not None:
+            cfg.update(ema_decay=self.ema_decay)
+            ema = m.arena.ema
         if m.loss != "mse":   # the head's loss kind (training and inference: the probabilities depend on it)
             cfg.update(loss=LOSS_CODES[m.loss])
         if getattr(m, "activation", "relu") != "relu":   # training and inference: f applies in both
@@ -307,7 +319,7 @@ class NativeWorker:
             cfg.update(residual=[int(lin.residual) for lin in m.linears])
         if training and getattr(m, "dropout", 0.0) > 0.0:   # inference plans run without dropout
             cfg.update(dropout=m.dropout, dropout_seed=m.dropout_seed, layer_base=m.layer_base)
-        eng = _C().PipeEngine(specs, cfg, m.arena.weights, m.arena.grads, momentum)
+        eng = _C().PipeEngine(specs, cfg, m.arena.weights, m.arena.grads, momentum, ema)
         if self._pp_nccl is not None:
             eng.set_pp_comm(self._pp_nccl)
         if self._dp_nccl is not None and training:
@@ -425,8 +437,21 @@ class NativeWorker:
         """Collective over the DP group: the canonical full momentum arena of this stage (CPU, None without momentum),
         each entry taken from the replica that owns it, so the result does not depend on the DP transport.  Entries
         every replica owns come from DP rank 0; the rest of the arena (padding) is zero everywhere."""
-        buf = self.model.arena.momentum
-        if self.momentum == 0.0 or buf is None:
+        if self.momentum == 0.0:
+            return None
+        return self._owned_state(self.model.arena.momentum)
+
+    def ema_state(self):
+        """Collective over the DP group: the stage's full EMA arena (CPU, None without an EMA), assembled from the
+        owners exactly like ``optimizer_state``."""
+        if self.ema_decay is None:
+            return None
+        return self._owned_state(self.model.arena.ema)
+
+    def _owned_state(self, buf):
+        """The full arena of a per-element optimizer buffer whose entries live with their owners (see
+        ``optimizer_state``)."""
+        if buf is None:
             return None
         self.sync_to_model()
         n = self.model.arena.numel
@@ -445,11 +470,17 @@ class NativeWorker:
     def load_optimizer_state(self, full):
         """Restore a buffer returned by ``optimizer_state`` into this replica (every replica loads the full buffer; the
         entries it does not own are never read)."""
+        self._load_owned_state(full, self.model.arena.momentum, "momentum")
+
+    def load_ema_state(self, full):
+        """Restore a buffer returned by ``ema_state`` into this replica, like ``load_optimizer_state``."""
+        self._load_owned_state(full, self.model.arena.ema, "EMA")
+
+    def _load_owned_state(self, full, buf, what):
         if full is None:
             return
-        buf = self.model.arena.momentum
         if buf is None or full.numel() != self.model.arena.numel:
-            raise ValueError("optimizer state does not match this model's momentum arena")
+            raise ValueError(f"optimizer state does not match this model's {what} arena")
         self.sync_to_model()
         buf[: full.numel()].copy_(full.to(buf.device))
         torch.cuda.synchronize(self.device)
@@ -496,13 +527,16 @@ class Trainer:
     ``activation``: the hidden layers' activation, "relu" (default), "gelu", "silu" or "tanh" (``models.mlp.MLP``).
 
     ``residual``: an identity skip around every hidden layer whose width does not change (``models.mlp.MLP``).
+
+    ``ema_decay``: keep an exponential moving average of the weights (``optimizer.SGD``), updated inside the update
+    kernels; ``ema_state()`` returns it.
     """
 
     def __init__(self, layer_sizes, global_batch_size=128, n_mubatches=4, lr=0.006, schedule="naive",
                  dp_comm=None, pp_comm=None, grid: Optional[ProcessGrid] = None, comm_mode="fused",
                  use_graph=True, device=None, seed_mode="shape", precision="fp32", watchdog_s=None, pp_transport=None,
                  local_batch_size=None, momentum=0.0, weight_decay=0.0, nesterov=False, loss="mse", lr_schedule=None,
-                 dropout=0.0, dropout_seed=0, activation="relu", residual=False):
+                 dropout=0.0, dropout_seed=0, activation="relu", residual=False, ema_decay=None):
         from ..models.mlp import MLP
         from ..optimizer import SGD
         from .schedules import SCHEDULE_NAME_TO_CLS
@@ -520,7 +554,7 @@ class Trainer:
                          loss=loss, dropout=dropout, dropout_seed=dropout_seed, activation=activation,
                          residual=residual).to(self.device)
         self.optimizer = SGD(self.model.parameters(), lr, momentum=momentum, weight_decay=weight_decay, nesterov=nesterov,
-                             arena=self.model.arena)
+                             arena=self.model.arena, ema_decay=ema_decay)
 
         class _Shape:  # the worker only needs the micro-batch size from the dataset
             mubatch_size = self.local_batch_size // n_mubatches
@@ -571,6 +605,10 @@ class Trainer:
 
     def loss(self):
         return self.engine.last_loss() if self.is_last else None
+
+    def ema_state(self):
+        """Collective over the DP group: this stage's full EMA arena (CPU), or None without an EMA."""
+        return self.worker.ema_state()
 
     def synchronize(self):
         if self.watchdog_s is not None:

@@ -92,6 +92,9 @@ def build_parser():
     p.add_argument("--momentum", type=float, default=0.0, help="SGD momentum (torch.optim.SGD semantics, dampening 0)")
     p.add_argument("--weight-decay", type=float, default=0.0, help="L2 penalty added to the gradient (biases included)")
     p.add_argument("--nesterov", action="store_true", help="Nesterov momentum (needs --momentum > 0)")
+    p.add_argument("--ema-decay", type=float, default=None,
+                   help="keep an exponential moving average of the weights with this decay, in (0, 1), and report its "
+                        "accuracy next to the trained weights' at every evaluation")
     p.add_argument("--loss", choices=["mse", "cross-entropy"], default="mse",
                    help="mse: the reference's softmax + MSE; cross-entropy: softmax cross-entropy on the logits")
     p.add_argument("--activation", default="relu", metavar="{" + ",".join(ACTIVATION_CODES) + "}",
@@ -198,7 +201,14 @@ def main(args):
     model.train()
     # before the resume: the momentum arena it restores is allocated here
     optimizer = SGD(model.parameters(), lr=args.lr, momentum=args.momentum, weight_decay=args.weight_decay,
-                    nesterov=args.nesterov, arena=model.arena)
+                    nesterov=args.nesterov, arena=model.arena, ema_decay=args.ema_decay)
+    # the EMA is evaluated as a model of its own: the same stage, its arena loaded with the EMA before every evaluation
+    ema_model = None
+    if args.ema_decay is not None:
+        ema_model = MLP(layer_sizes, stage_idx=pp_comm.Get_rank(), n_stages=args.pp, batch_size=args.global_batch_size,
+                        seed_mode=args.seed_mode, verbose=False, loss=loss, activation=activation,
+                        residual=bool(args.residual))
+        ema_model.to(device)
 
     shuffle_seed = check_shuffle_seed(args.shuffle_seed)
     dataset = Dataset(save_dir, global_batch_size=args.global_batch_size,
@@ -220,12 +230,14 @@ def main(args):
                "weight_decay": float(args.weight_decay), "nesterov": bool(args.nesterov), "loss": loss,
                "lr_schedule": lr_schedule.spec(), "dropout": float(args.dropout),
                "dropout_seed": int(args.dropout_seed), "shuffle": bool(args.shuffle), "shuffle_seed": shuffle_seed,
-               "activation": activation, "residual": bool(args.residual)}
+               "activation": activation, "residual": bool(args.residual), "ema_decay": args.ema_decay}
     resumed_step = 0
     if args.resume:
         from shallowspeed_b200.utils.checkpoint import load_stage
 
         resumed_step = load_stage(model, args.resume, pp_comm.Get_rank(), args.pp, expect_hparams=hparams)
+        if args.ema_decay is not None:
+            optimizer.ema_updates = resumed_step          # one EMA update per step of the run so far
 
     if engine == "native":
         from shallowspeed_b200.parallel.engine import NativeWorker
@@ -235,9 +247,24 @@ def main(args):
         val_worker = NativeWorker(None, pp_comm, model, val_dataset, None, grid=grid, comm_mode="nccl",
                                   use_graph=not args.no_graph, precision=args.precision, share=worker,
                                   pp_transport=args.pp_transport)
+        ema_worker = None if ema_model is None else NativeWorker(
+            None, pp_comm, ema_model, val_dataset, None, grid=grid, comm_mode="nccl", use_graph=not args.no_graph,
+            precision=args.precision, share=worker, pp_transport=args.pp_transport)
     else:
         worker = Worker(dp_comm, pp_comm, model, dataset, optimizer, device=device)
         val_worker = Worker(None, pp_comm, model, val_dataset, None, device=device)
+        ema_worker = None if ema_model is None else Worker(None, pp_comm, ema_model, val_dataset, None, device=device)
+
+    def evaluate():
+        """Accuracy of the trained weights and of their EMA (None without one) on the last stage, None elsewhere."""
+        accuracy = compute_accuracy(model, val_worker, val_dataset)
+        if ema_model is None:
+            return accuracy, None
+        # collective over the DP group (native engine): every replica takes part, each owner contributes its entries
+        ema = worker.ema_state() if engine == "native" else model.arena.ema
+        n = ema_model.arena.numel
+        ema_model.arena.weights[:n].copy_(ema[:n].to(ema_model.arena.weights.device))
+        return accuracy, compute_accuracy(ema_model, ema_worker, val_dataset)
 
     start_time = time.time()
     # a resumed run continues where the checkpoint stopped: same global step, same position in the data
@@ -249,13 +276,16 @@ def main(args):
     schedule = sched_cls(num_micro_batches=args.n_mubatches, num_stages=args.pp, stage_id=pp_comm.Get_rank())
     while step < total_steps:
         if not args.no_eval:
-            accuracy = compute_accuracy(model, val_worker, val_dataset)
+            accuracy, ema_accuracy = evaluate()
             if accuracy is not None:
                 print(f"Epoch: {epoch}, Time Spent: {time.time() - start_time:.2f}s, Accuracy: {accuracy * 100:.2f}%",
                       flush=True)
+                if ema_accuracy is not None:
+                    print(f"EMA accuracy: {ema_accuracy * 100:.2f}%", flush=True)
                 if dp_comm.Get_rank() == 0:
+                    extra = {} if ema_accuracy is None else {"ema_accuracy": ema_accuracy}
                     logger.log(event="eval", epoch=epoch, step=step, accuracy=accuracy,
-                               time_s=time.time() - start_time)
+                               time_s=time.time() - start_time, **extra)
         t_epoch = time.time()
         dataset.set_epoch(epoch)                    # the epoch's permutation (a resume re-derives it from the step)
         steps_this_epoch = min(n_batches - first_batch, total_steps - step)
@@ -278,10 +308,12 @@ def main(args):
         epoch += 1
 
     if not args.no_eval:
-        accuracy = compute_accuracy(model, val_worker, val_dataset)
+        accuracy, ema_accuracy = evaluate()
         if accuracy is not None:
             print(f"Epoch: {epoch}, Time Spent: {time.time() - start_time:.2f}s, Accuracy: {accuracy * 100:.2f}%",
                   flush=True)
+            if ema_accuracy is not None:
+                print(f"EMA accuracy: {ema_accuracy * 100:.2f}%", flush=True)
 
     if hasattr(worker, "sync_to_model"):
         worker.sync_to_model()
@@ -291,11 +323,13 @@ def main(args):
         from shallowspeed_b200.utils.checkpoint import save_stage
 
         if engine == "native":
-            momentum = worker.optimizer_state()
+            momentum, ema = worker.optimizer_state(), worker.ema_state()
         else:
             momentum = model.arena.momentum if optimizer.momentum > 0.0 else None
+            ema = model.arena.ema
         if dp_comm.Get_rank() == 0:
-            save_stage(model, args.save, pp_comm.Get_rank(), args.pp, step=step, hparams=hparams, momentum=momentum)
+            save_stage(model, args.save, pp_comm.Get_rank(), args.pp, step=step, hparams=hparams, momentum=momentum,
+                       ema=ema)
     logger.close()
     if args.dp * args.pp > 1:
         import torch.distributed as dist

@@ -4,7 +4,8 @@ test_gpu_pp_replay (a pipeline stage, its neighbours' boundary tiles and flags r
 The replays run unchanged; for the duration of a case their GEMM oracles are swapped for the bf16 ones of test_gpu_bf16:
 every product from the operands rounded to bf16, within RTOL_BF16 = 2^-16 of sum |a'||b'| (plus test_gpu_gemm's K > 4096
 term), the bias gradient the fp32 column sum of the unrounded dZ.  So every owned update, every copied or untouched peer
-element and every outbound tile or line is checked per element against the bf16 oracle."""
+element and every outbound tile or line is checked per element against the bf16 oracle, in the dp x pp stages as well
+(an LL and a flag-protocol stage, whose DP checks run on the partials of the swapped oracle)."""
 import pytest
 import torch
 
@@ -35,9 +36,10 @@ def _grad_oracle(dz, x, rtol):
     return g, bound
 
 
-def _bf16_oracles(monkeypatch, module):
-    monkeypatch.setattr(module, "grad_oracle", _grad_oracle)
-    monkeypatch.setattr(module, "rtol_for", _rtol_for)
+def _bf16_oracles(monkeypatch, *modules):
+    for module in modules:
+        monkeypatch.setattr(module, "grad_oracle", _grad_oracle)
+        monkeypatch.setattr(module, "rtol_for", _rtol_for)
 
 
 @pytest.mark.parametrize("dp,rank,gate", [(2, 1, "1"), (4, 2, "0"), (8, 7, "1")])
@@ -69,12 +71,16 @@ PP_CASES = {
     "ref-pp2-s0-unfolded": PP._case(PP.REF, 2, 0, "1f1b", env=PP.UNFOLD, push="small", precision="bf16"),
     "ref-pp4-s2-unfolded-mb128": PP._case(PP.REF, 4, 2, "gpipe", mb=128, n_mu=2, env=PP.UNFOLD, push="multi",
                                           precision="bf16"),
+    # dp x pp: the LL wave over act_in, and the flag protocol behind per-micro-batch weight gradients
+    "ref-pp2-s1-dp2-r0-1f1b": PP._case(PP.REF, 2, 1, "1f1b", dp=2, rank=0, precision="bf16"),
+    "ref-pp4-s1-dp4-r2-flags-two-shot-stateful": PP._case(PP.REF, 4, 1, "gpipe", env={"SSB_DP_LL": "0", "SSB_DP_TWO_SHOT": "1"},
+                                                          stateful=True, dp=4, rank=2, precision="bf16"),
 }
 
 
 @pytest.mark.parametrize("name", list(PP_CASES))
 def test_pp_stage_replay(name, monkeypatch):
-    _bf16_oracles(monkeypatch, PP)
+    _bf16_oracles(monkeypatch, PP, DP)        # DP: the partials dp_check compares the outbound messages with
     # the stage's forward and dgrad products from the rounded operands; the replay looks its rtol up by precision
     monkeypatch.setattr(PP, "RTOL", {"bf16": RTOL_BF16})
     monkeypatch.setattr(PP, "fwd_oracle", lambda x, W, b, relu, rtol: fwd_oracle(bf(x), bf(W), b, relu, rtol))

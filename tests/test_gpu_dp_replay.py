@@ -29,6 +29,9 @@ Elements owned by a peer: under LL, bit-equal to the injected phase-C line (the 
 protocol, untouched by r; under one-shot, updated by r like its own.  The momentum must change exactly on the elements
 ``_C.dp_owner_map`` assigns to r (the map ``NativeWorker.optimizer_state`` assembles checkpoints with) and nowhere else.
 
+The DP half of the replay is ``dp_setup`` / ``dp_prefill`` / ``dp_check``; ``test_gpu_pp_replay.py`` calls the same
+functions to run a pipeline stage as one replica of a dp x pp layout, where the kernels read the stage's receive slots.
+
 Not covered here, and left to ``test_gpu_multi.py``: concurrent peers, the single-copy atomicity of LL lines over
 NVLink, and bit-identity across real replicas.
 """
@@ -373,25 +376,12 @@ def _build_replica(sizes, dp, rank, mb_rows, n_mu, precision, stateful, monkeypa
     from shallowspeed_b200.optimizer import SGD
     from shallowspeed_b200.parallel import engine as E
 
-    C = _C()
     rows = mb_rows * n_mu
     model = MLP(sizes, 0, 1, rows * dp).to("cuda")
     rule = dict(momentum=MU, weight_decay=WD, nesterov=True) if stateful else {}
     opt = SGD(model.parameters(), LR, arena=model.arena, **rule)
     ctxs = []
-
-    def make_dp_context(comm, model, lr):
-        # make_dp_context with peers that are contexts of this process instead of CUDA IPC mappings
-        arena = model.arena
-        layers = [(lin.in_dims, lin.out_dims, int(arena.offsets[lin.block_index]), int(arena.lds[lin.block_index]))
-                  for lin in model.linears]
-        ctxs[:] = [C.DpContext(comm.size, p, int(arena.weights.numel()), layers, float(lr)) for p in range(comm.size)]
-        ctx = ctxs[comm.rank]
-        ctx.open_local_peers(ctxs)
-        arena.rebind(ctx.weights(), arena.grads, copy=True)
-        torch.cuda.synchronize()
-        return ctx
-
+    make_dp_context = local_dp_context(ctxs)
     monkeypatch.setattr(E, "make_dp_context", make_dp_context)
 
     class _Shape:
@@ -405,6 +395,208 @@ def _build_replica(sizes, dp, rank, mb_rows, n_mu, precision, stateful, monkeypa
         w.dp_mode = "fused"
         w._dp_ctx = make_dp_context(comm, model, w.lr)
     return w, model, ctxs
+
+
+def local_dp_context(ctxs):
+    """A ``make_dp_context`` whose peers are DpContexts of this process (``open_local_peers``) instead of CUDA IPC
+    mappings; every context of the group lands in ``ctxs``, rank order."""
+    def make_dp_context(comm, model, lr):
+        arena = model.arena
+        layers = [(lin.in_dims, lin.out_dims, int(arena.offsets[lin.block_index]), int(arena.lds[lin.block_index]))
+                  for lin in model.linears]
+        ctxs[:] = [_C().DpContext(comm.size, p, int(arena.weights.numel()), layers, float(lr)) for p in range(comm.size)]
+        ctx = ctxs[comm.rank]
+        ctx.open_local_peers(ctxs)
+        arena.rebind(ctx.weights(), arena.grads, copy=True)
+        torch.cuda.synchronize()
+        return ctx
+
+    return make_dp_context
+
+
+def dp_setup(ctxs, rank, protocol, sizes, env, arena, protos):
+    """What ``dp_prefill`` / ``dp_check`` need about replica ``rank`` of the group ``ctxs``: device views of every
+    context's buffers, the LL tiles (``protocol`` "ll") or the flag geometry of the layers ``sizes``, and per layer the
+    owner map of the protocol it ran (``protos``) and the elements ``rank`` owns."""
+    C = _C()
+    dp = len(ctxs)
+    d = dict(dp=dp, rank=rank, ll=protocol == "ll", bufs=[_Buffers(c) for c in ctxs], protos=protos)
+    d["me"] = d["bufs"][rank]
+    if d["ll"]:
+        d["tiles"] = ll_tiles(sizes)
+    else:
+        d["geom"] = flag_geometry(sizes, dp, two_shot="SSB_DP_TWO_SHOT" in env, one_shot="SSB_DP_ONE_SHOT" in env,
+                                  wide_tiles="SSB_DP_WIDE_TILES" in env)
+    d["owners"] = [C.dp_owner_map(int(protos[i]), k, o, int(arena.lds[i]), int(arena.offsets[i]), dp).long()
+                   for i, (o, k) in enumerate(arena.blocks)]
+    d["owned"] = [(ow == rank) | (ow < 0) for ow in d["owners"]]
+    return d
+
+
+def dp_peer_data(d, gen, blocks, scale, W0, lr):
+    """What the peers contribute to one step: their partials ``P`` ([out, in + 1] per layer, of the magnitude
+    ``scale``) and, under LL, the new weights ``Wc`` they send for their rows (phase C), an update's distance from the
+    current ones."""
+    P = {p: [(torch.randn(o, k + 1, generator=gen, dtype=torch.float64) * sc).float() for (o, k), sc in zip(blocks, scale)]
+         for p in range(d["dp"]) if p != d["rank"]}
+    Wc = {p: [(W0[i] - lr * torch.randn(o, k + 1, generator=gen, dtype=torch.float64) * scale[i]).float()
+              for i, (o, k) in enumerate(blocks)] for p in P} if d["ll"] else {}
+    return P, Wc
+
+
+def dp_prefill(d, P, Wc, epoch):
+    """Before a step of DP epoch ``epoch``: the peers' messages into my buffers (LL lines in llA / llC, or partial tiles
+    in the staging buffer and arrive / done flags), decoys everywhere else, my outbound targets in the peers cleared."""
+    dp, rank, me, bufs, parity = d["dp"], d["rank"], d["me"], d["bufs"], epoch & 1
+    if d["ll"]:
+        tiles = d["tiles"]
+        lines = me.llA.shape[0]
+        pre = ll_prefill_lines(tiles, dp, rank, parity)
+        zones = {}
+        for z, vals in (("A", P), ("C", Wc)):
+            zone = decoy_zone(lines, epoch)
+            for p, f in pre[z]:
+                write_lines(zone, f, vals[p], epoch)
+            zones[z] = zone
+        polls = ll_polls(tiles, dp, rank, parity)
+        for z in ("A", "C"):
+            sent = torch.cat([f["idx"] for _, f in pre[z]]).sort().values
+            assert torch.equal(sent, polls[z].sort().values), f"{z}: the prefill misses a polled line"
+            assert bool((zones[z][polls[z], 1] == epoch).all() and (zones[z][polls[z], 3] == epoch).all())
+        me.llA.copy_(zones["A"].cuda())
+        me.llC.copy_(zones["C"].cuda())
+        for p in P:
+            bufs[p].llA.zero_()
+            bufs[p].llC.zero_()
+    else:
+        geom = d["geom"]
+        arrive_pre, done_pre, msgs = flag_prefill(geom, dp, rank, parity)
+        polled_arrive, polled_done = flag_polls(geom, dp, rank)
+        sps = geom[0]["slots_per_src"] if geom else 1      # a stage without layers keeps one arrive flag per source
+        own_src = set(range(rank * sps, (rank + 1) * sps))
+        assert arrive_pre == polled_arrive - own_src and done_pre == polled_done
+        stage = torch.full_like(me.stage, NAN, device="cpu")
+        for p, m in msgs:
+            g = geom[m["layer"]]
+            tile, bias = _slot(P[p][m["layer"]], g, m["mt"], m["nt"])
+            stage[m["base"]: m["base"] + 128 * g["block_n"]] = tile.reshape(-1)
+            stage[m["base"] + 128 * g["block_n"]: m["base"] + g["slot_floats"]] = bias
+        arrive = torch.full(me.arrive.shape, epoch, dtype=torch.int32)
+        arrive[_idx(own_src)] = 0
+        done = torch.full(me.done.shape, epoch, dtype=torch.int32)
+        done[_idx(flag_done_writes(geom, dp, rank))] = 0
+        assert bool((arrive[_idx(arrive_pre)] == epoch).all()) and bool((done[_idx(done_pre)] == epoch).all())
+        me.stage.copy_(stage.cuda())
+        me.arrive.copy_(arrive.cuda())
+        me.done.copy_(done.cuda())
+        for p in P:
+            bufs[p].stage.fill_(NAN)
+            bufs[p].arrive.zero_()
+            bufs[p].done.zero_()
+    for p in P:
+        bufs[p].W.fill_(NAN)
+
+
+def check_owned_update(W1, own, own_b, peers, W0, V0, V1, lr, stateful, owned, res, key):
+    """The owned elements of one layer's [out, in + 1] block after the step against ``reduced_oracle`` +
+    ``sgd_oracle``: the weights' err / bound into ``res[key % "upd"]``, the momentum's (``stateful``) into
+    ``res[key % "mom"]``."""
+    tot, tb = reduced_oracle(own, own_b, peers)
+    v0 = V0 if stateful else torch.zeros_like(W0)
+    Wr, bW, Vr, bV = sgd_oracle(tot, tb, W0, v0, lr, MU if stateful else 0.0, WD if stateful else 0.0, stateful)
+    res[key % "upd"] = excess(W1[owned], Wr[owned], bW[owned])
+    if stateful:
+        res[key % "mom"] = excess(V1[owned], Vr[owned], bV[owned])
+
+
+def dp_check(d, res, step, arena, own, own_b, P, Wc, W0, V0, lr, stateful, epoch):
+    """After a step of DP epoch ``epoch``, from my own partials ``own`` / ``own_b`` (the oracle of the engine's own act /
+    dz): every owned update and momentum entry, every copied or untouched peer element, every outbound LL line or
+    staging tile and arrive / done flag, the weights published to the peers, and the momentum ownership."""
+    C = _C()
+    dp, rank, bufs, protos, parity = d["dp"], d["rank"], d["bufs"], d["protos"], epoch & 1
+    owners, owned = d["owners"], d["owned"]
+    s = f"s{step + 1}."
+    assert int(d["me"].epoch[0].item()) == epoch, "the DP epoch did not advance by one"
+    # ---- 1. owned elements (and 2. for one-shot): per element against fp64
+    W1 = [arena.block(i)[:, : k + 1].cpu() for i, (_, k) in enumerate(arena.blocks)]
+    for i, (o, k) in enumerate(arena.blocks):
+        pad = arena.block(i)[:, k + 1:]
+        assert bool(torch.isnan(pad).all()), f"step {step + 1}: the padding of layer {i + 1}'s weights changed"
+        V1 = arena.momentum_block(i)[:, : k + 1].cpu() if stateful else None
+        check_owned_update(W1[i], own[i], own_b[i], [P[p][i] for p in P], W0[i], V0[i] if stateful else None, V1, lr,
+                           stateful, owned[i], res, s + "%s" + str(i + 1))
+        if stateful:
+            check_momentum_ownership(V0[i].float(), V1, owned[i], f"step {step + 1} layer {i + 1}")
+        # ---- 2. elements owned by peers
+        for p in P:
+            pm = owners[i] == p
+            if d["ll"]:
+                assert torch.equal(W1[i][pm].view(torch.int32), Wc[p][i][pm].view(torch.int32)), \
+                    f"step {step + 1} layer {i + 1}: rows of rank {p} differ from its phase-C lines"
+            else:
+                assert torch.equal(W1[i][pm].view(torch.int32), W0[i][pm].float().view(torch.int32)), \
+                    f"step {step + 1} layer {i + 1}: replica {rank} wrote a tile rank {p} owns"
+
+    # ---- 3. outbound messages, read from the peers' buffers
+    if d["ll"]:
+        mine = ll_messages(d["tiles"], dp, rank, parity)
+        for p in P:
+            zA, zC = bufs[p].llA.cpu(), bufs[p].llC.cpu()
+            res[s + "lineA"] = max(res.get(s + "lineA", 0.0),
+                                   check_lines(zA, mine[("A", p)], own, own_b, epoch, f"phase A to {p}"))
+            check_lines(zC, mine[("C", p)], W1, None, epoch, f"phase C to {p}")
+            check_only(zA, mine[("A", p)], epoch, f"llA of {p}")
+            check_only(zC, mine[("C", p)], epoch, f"llC of {p}")
+        for p in P:
+            assert bool(torch.isnan(bufs[p].W).all()), f"the LL kernel wrote into the weights of {p}"
+        return
+    geom = d["geom"]
+    sent = [m for m in flag_messages(geom, dp, rank, parity)]
+    pub = flag_done_writes(geom, dp, rank)
+    for p in range(dp):
+        stage_p, arrive_p, done_p = bufs[p].stage.cpu(), bufs[p].arrive.cpu(), bufs[p].done.cpu()
+        to_p = [m for m in sent if m["dst"] == p]
+        want = torch.zeros_like(arrive_p, dtype=torch.bool)
+        want[_idx(m["arrive"] for m in to_p)] = True
+        got = arrive_p == epoch
+        if p == rank:
+            assert bool(got[want].all()), "an own-source arrive flag was not set"
+            assert bool((done_p[_idx(pub)] == epoch).all()), "a done flag of an owned tile was not set"
+            continue
+        assert torch.equal(got, want) and bool((arrive_p[~want] == 0).all()), f"arrive flags of {p}"
+        dwant = torch.zeros_like(done_p, dtype=torch.bool)
+        dwant[_idx(pub)] = True
+        assert torch.equal(done_p == epoch, dwant) and bool((done_p[~dwant] == 0).all()), f"done flags of {p}"
+        written = torch.zeros_like(stage_p, dtype=torch.bool)
+        for m in to_p:
+            g = geom[m["layer"]]
+            bn = g["block_n"]
+            tile = stage_p[m["base"]: m["base"] + 128 * bn].view(128, bn)
+            bias = stage_p[m["base"] + 128 * bn: m["base"] + g["slot_floats"]]
+            rt, rb = _slot(own[m["layer"]], g, m["mt"], m["nt"], torch.float64)
+            bt, bb = _slot(own_b[m["layer"]], g, m["mt"], m["nt"], torch.float64)
+            v = ~torch.isnan(rt)
+            res[s + "push"] = max(res.get(s + "push", 0.0), excess(tile[v], rt[v], bt[v]))
+            written[m["base"]: m["base"] + 128 * bn] = True
+            if m["nt"] == 0:
+                v = ~torch.isnan(rb)
+                res[s + "push"] = max(res[s + "push"], excess(bias[v], rb[v], bb[v]))
+                written[m["base"] + 128 * bn: m["base"] + g["slot_floats"]] = True
+        assert bool(torch.isfinite(stage_p[written]).all()), f"a pushed slot of {p} holds a non-finite value"
+        assert bool(torch.isnan(stage_p[~written]).all()), f"the staging buffer of {p} was written outside the slots"
+        # published weights: the two-shot tiles I own, bit for bit; nothing else
+        Wp = bufs[p].W.cpu()
+        touched = torch.zeros_like(Wp, dtype=torch.bool)
+        for i, (o, k) in enumerate(arena.blocks):
+            off, ld = int(arena.offsets[i]), int(arena.lds[i])
+            blk, tb = Wp[off: off + o * ld].view(o, ld), touched[off: off + o * ld].view(o, ld)
+            if protos[i] == C.DP_PROTO_TWO_SHOT:
+                pm = owners[i] == rank
+                tb[:, : k + 1] = pm
+                assert torch.equal(blk[:, : k + 1][pm].view(torch.int32), W1[i][pm].view(torch.int32)), \
+                    f"layer {i + 1}: the weights published to {p} differ from mine"
+        assert bool(torch.isnan(Wp[~touched]).all()), f"weights of {p} written outside my published tiles"
 
 
 def _run(case, sizes, dp, rank, protocol, env=None, mb_rows=32, n_mu=2, precision="fp32", stateful=False,
@@ -437,22 +629,19 @@ def _run(case, sizes, dp, rank, protocol, env=None, mb_rows=32, n_mu=2, precisio
     # ---- the path this case is meant to exercise
     plan, protos = eng.plan_text(0), list(eng.layer_protocols())
     assert (f"momentum={MU:g}" in eng.describe()) == stateful, eng.describe()
-    bufs = [_Buffers(c) for c in ctxs]
-    me = bufs[rank]
     coalesced = "SSB_NO_COALESCE" not in env
     assert eng.coalesced() == coalesced
+    d = dp_setup(ctxs, rank, protocol, sizes, env, arena, protos)
     if protocol == "ll":
-        assert ctxs[rank].ll_tiles() == len(ll_tiles(sizes)) and eng.uses_chain()
+        assert ctxs[rank].ll_tiles() == len(d["tiles"]) and eng.uses_chain()
         assert "dp_ll" in plan and "fused_wgrad_dp" not in plan and "dp_reduce_sgd" not in plan, plan
         assert ("bump_step" in plan) == (env.get("SSB_DP_GATE", "1") != "0"), plan
         assert protos == [C.DP_PROTO_LL] * L
-        tiles = ll_tiles(sizes)
     else:
         assert ctxs[rank].ll_tiles() == 0 and "dp_ll" not in plan, plan
         kernel = "fused_wgrad_dp" if coalesced else "dp_reduce_sgd"
         assert plan.count(f" {kernel} ") == L and ("fused_wgrad_dp" in plan) == coalesced, plan
-        geom = flag_geometry(sizes, dp, two_shot="SSB_DP_TWO_SHOT" in env, one_shot="SSB_DP_ONE_SHOT" in env,
-                             wide_tiles="SSB_DP_WIDE_TILES" in env)
+        geom = d["geom"]
         got = ctxs[rank].layer_geometry()
         for g, h in zip(geom, got):
             assert all(g[key] == h[key] for key in g), (g, h)
@@ -464,77 +653,20 @@ def _run(case, sizes, dp, rank, protocol, env=None, mb_rows=32, n_mu=2, precisio
             assert max(g["n_tiles_m"] * g["n_tiles_n"] for g in geom) > MAX_CTAS
     _poison(eng, model, sizes, rows, True)
 
-    owners = []
-    for i, lin in enumerate(model.linears):
-        o, k = arena.blocks[i]
-        owners.append(C.dp_owner_map(int(protos[i]), k, o, int(arena.lds[i]), int(arena.offsets[i]), dp).long())
-    owned = [(ow == rank) | (ow < 0) for ow in owners]
     res = {}
     for step in range(steps):
-        s = f"s{step + 1}."
-        epoch = int(me.epoch[0].item()) + 1
-        parity = epoch & 1
+        epoch = int(d["me"].epoch[0].item()) + 1
         W0 = [arena.block(i)[:, : k + 1].double().cpu() for i, (_, k) in enumerate(arena.blocks)]
         V0 = [arena.momentum_block(i)[:, : k + 1].double().cpu() for i, (_, k) in enumerate(arena.blocks)] if stateful else None
         scale = _grad_scale(sizes, W0, xs[step], ts[step], n_mu, model.batch_size)
-        P = {p: [(torch.randn(o, k + 1, generator=gen, dtype=torch.float64) * sc).float()
-                 for (o, k), sc in zip(arena.blocks, scale)] for p in range(dp) if p != rank}
-        # LL: the new weights a peer sends for its rows (phase C), an update's distance from the current ones
-        Wc = {p: [(W0[i] - LR * torch.randn(o, k + 1, generator=gen, dtype=torch.float64) * scale[i]).float()
-                  for i, (o, k) in enumerate(arena.blocks)] for p in P} if protocol == "ll" else {}
+        P, Wc = dp_peer_data(d, gen, arena.blocks, scale, W0, LR)
         torch.cuda.synchronize()
-
-        # ---- prefill: the peers' messages into my buffers, decoys everywhere else; my outbound targets cleared
-        if protocol == "ll":
-            lines = me.llA.shape[0]
-            pre = ll_prefill_lines(tiles, dp, rank, parity)
-            zones = {}
-            for z, vals in (("A", P), ("C", Wc)):
-                zone = decoy_zone(lines, epoch)
-                for p, f in pre[z]:
-                    write_lines(zone, f, vals[p], epoch)
-                zones[z] = zone
-            polls = ll_polls(tiles, dp, rank, parity)
-            for z in ("A", "C"):
-                sent = torch.cat([f["idx"] for _, f in pre[z]]).sort().values
-                assert torch.equal(sent, polls[z].sort().values), f"{z}: the prefill misses a polled line"
-                assert bool((zones[z][polls[z], 1] == epoch).all() and (zones[z][polls[z], 3] == epoch).all())
-            me.llA.copy_(zones["A"].cuda())
-            me.llC.copy_(zones["C"].cuda())
-            for p in P:
-                bufs[p].llA.zero_()
-                bufs[p].llC.zero_()
-        else:
-            arrive_pre, done_pre, msgs = flag_prefill(geom, dp, rank, parity)
-            polled_arrive, polled_done = flag_polls(geom, dp, rank)
-            own_src = set(range(rank * geom[0]["slots_per_src"], (rank + 1) * geom[0]["slots_per_src"]))
-            assert arrive_pre == polled_arrive - own_src and done_pre == polled_done
-            stage = torch.full_like(me.stage, NAN, device="cpu")
-            for p, m in msgs:
-                g = geom[m["layer"]]
-                tile, bias = _slot(P[p][m["layer"]], g, m["mt"], m["nt"])
-                stage[m["base"]: m["base"] + 128 * g["block_n"]] = tile.reshape(-1)
-                stage[m["base"] + 128 * g["block_n"]: m["base"] + g["slot_floats"]] = bias
-            arrive = torch.full(me.arrive.shape, epoch, dtype=torch.int32)
-            arrive[_idx(own_src)] = 0
-            done = torch.full(me.done.shape, epoch, dtype=torch.int32)
-            done[_idx(flag_done_writes(geom, dp, rank))] = 0
-            assert bool((arrive[_idx(arrive_pre)] == epoch).all()) and bool((done[_idx(done_pre)] == epoch).all())
-            me.stage.copy_(stage.cuda())
-            me.arrive.copy_(arrive.cuda())
-            me.done.copy_(done.cuda())
-            for p in P:
-                bufs[p].stage.fill_(NAN)
-                bufs[p].arrive.zero_()
-                bufs[p].done.zero_()
-        for p in P:
-            bufs[p].W.fill_(NAN)
+        dp_prefill(d, P, Wc, epoch)
         torch.cuda.synchronize()
 
         w.step_from(sched, xs[step].pin_memory(), ts[step].pin_memory())
         eng.synchronize()
         torch.cuda.synchronize()
-        assert int(me.epoch[0].item()) == epoch
 
         act = [xs[step].double()] + [_gather(lambda mu, l=l: eng.act(mu, l), n_mu) for l in range(1, L)]
         dz = [None] + [_gather(lambda mu, l=l: eng.dz(mu, l), n_mu) for l in range(1, L + 1)]
@@ -550,90 +682,7 @@ def _run(case, sizes, dp, rank, protocol, env=None, mb_rows=32, n_mu=2, precisio
                 gb = gb + (n_mu - 1) * FP32_ULP * mag
             own.append(g)
             own_b.append(gb)
-
-        # ---- 1. owned elements (and 2. for one-shot): per element against fp64
-        W1 = [arena.block(i)[:, : k + 1].cpu() for i, (_, k) in enumerate(arena.blocks)]
-        for i, (o, k) in enumerate(arena.blocks):
-            pad = arena.block(i)[:, k + 1:]
-            assert bool(torch.isnan(pad).all()), f"step {step + 1}: the padding of layer {i + 1}'s weights changed"
-            tot, tb = reduced_oracle(own[i], own_b[i], [P[p][i] for p in P])
-            v0 = V0[i] if stateful else torch.zeros_like(W0[i])
-            Wr, bW, Vr, bV = sgd_oracle(tot, tb, W0[i], v0, LR, MU if stateful else 0.0, WD if stateful else 0.0, stateful)
-            mask = owned[i]
-            res[s + f"upd{i + 1}"] = excess(W1[i][mask], Wr[mask], bW[mask])
-            if stateful:
-                V1 = arena.momentum_block(i)[:, : k + 1].cpu()
-                res[s + f"mom{i + 1}"] = excess(V1[mask], Vr[mask], bV[mask])
-                check_momentum_ownership(V0[i].float(), V1, mask, f"step {step + 1} layer {i + 1}")
-            # ---- 2. elements owned by peers
-            for p in P:
-                pm = owners[i] == p
-                if protocol == "ll":
-                    assert torch.equal(W1[i][pm].view(torch.int32), Wc[p][i][pm].view(torch.int32)), \
-                        f"step {step + 1} layer {i + 1}: rows of rank {p} differ from its phase-C lines"
-                else:
-                    assert torch.equal(W1[i][pm].view(torch.int32), W0[i][pm].float().view(torch.int32)), \
-                        f"step {step + 1} layer {i + 1}: replica {rank} wrote a tile rank {p} owns"
-
-        # ---- 3. outbound messages, read from the peers' buffers
-        if protocol == "ll":
-            mine = ll_messages(tiles, dp, rank, parity)
-            for p in P:
-                zA, zC = bufs[p].llA.cpu(), bufs[p].llC.cpu()
-                res[s + "lineA"] = max(res.get(s + "lineA", 0.0),
-                                       check_lines(zA, mine[("A", p)], own, own_b, epoch, f"phase A to {p}"))
-                check_lines(zC, mine[("C", p)], W1, None, epoch, f"phase C to {p}")
-                check_only(zA, mine[("A", p)], epoch, f"llA of {p}")
-                check_only(zC, mine[("C", p)], epoch, f"llC of {p}")
-        else:
-            sent = [m for m in flag_messages(geom, dp, rank, parity)]
-            pub = flag_done_writes(geom, dp, rank)
-            for p in range(dp):
-                stage_p, arrive_p, done_p = bufs[p].stage.cpu(), bufs[p].arrive.cpu(), bufs[p].done.cpu()
-                to_p = [m for m in sent if m["dst"] == p]
-                want = torch.zeros_like(arrive_p, dtype=torch.bool)
-                want[_idx(m["arrive"] for m in to_p)] = True
-                got = arrive_p == epoch
-                if p == rank:
-                    assert bool(got[want].all()), "an own-source arrive flag was not set"
-                    assert bool((done_p[_idx(pub)] == epoch).all()), "a done flag of an owned tile was not set"
-                    continue
-                assert torch.equal(got, want) and bool((arrive_p[~want] == 0).all()), f"arrive flags of {p}"
-                dwant = torch.zeros_like(done_p, dtype=torch.bool)
-                dwant[_idx(pub)] = True
-                assert torch.equal(done_p == epoch, dwant) and bool((done_p[~dwant] == 0).all()), f"done flags of {p}"
-                written = torch.zeros_like(stage_p, dtype=torch.bool)
-                for m in to_p:
-                    g = geom[m["layer"]]
-                    bn = g["block_n"]
-                    tile = stage_p[m["base"]: m["base"] + 128 * bn].view(128, bn)
-                    bias = stage_p[m["base"] + 128 * bn: m["base"] + g["slot_floats"]]
-                    rt, rb = _slot(own[m["layer"]], g, m["mt"], m["nt"], torch.float64)
-                    bt, bb = _slot(own_b[m["layer"]], g, m["mt"], m["nt"], torch.float64)
-                    v = ~torch.isnan(rt)
-                    res[s + "push"] = max(res.get(s + "push", 0.0), excess(tile[v], rt[v], bt[v]))
-                    written[m["base"]: m["base"] + 128 * bn] = True
-                    if m["nt"] == 0:
-                        v = ~torch.isnan(rb)
-                        res[s + "push"] = max(res[s + "push"], excess(bias[v], rb[v], bb[v]))
-                        written[m["base"] + 128 * bn: m["base"] + g["slot_floats"]] = True
-                assert bool(torch.isfinite(stage_p[written]).all()), f"a pushed slot of {p} holds a non-finite value"
-                assert bool(torch.isnan(stage_p[~written]).all()), f"the staging buffer of {p} was written outside the slots"
-                # published weights: the two-shot tiles I own, bit for bit; nothing else
-                Wp = bufs[p].W.cpu()
-                touched = torch.zeros_like(Wp, dtype=torch.bool)
-                for i, (o, k) in enumerate(arena.blocks):
-                    off, ld = int(arena.offsets[i]), int(arena.lds[i])
-                    blk, tb = Wp[off: off + o * ld].view(o, ld), touched[off: off + o * ld].view(o, ld)
-                    if protos[i] == C.DP_PROTO_TWO_SHOT:
-                        pm = owners[i] == rank
-                        tb[:, : k + 1] = pm
-                        assert torch.equal(blk[:, : k + 1][pm].view(torch.int32), W1[i][pm].view(torch.int32)), \
-                            f"layer {i + 1}: the weights published to {p} differ from mine"
-                assert bool(torch.isnan(Wp[~touched]).all()), f"weights of {p} written outside my published tiles"
-        if protocol == "ll":
-            for p in P:
-                assert bool(torch.isnan(bufs[p].W).all()), f"the LL kernel wrote into the weights of {p}"
+        dp_check(d, res, step, arena, own, own_b, P, Wc, W0, V0, LR, stateful, epoch)
     _note(case, res)
     eng.synchronize()
     del eng, w
@@ -713,9 +762,13 @@ def _grid_flags():
 
 @pytest.mark.parametrize("dp,rank", _grid_ll())
 def test_ll_prefill_covers_exactly_the_polled_lines(dp, rank):
+    check_ll_prefill(REF, dp, rank)
+
+
+def check_ll_prefill(sizes, dp, rank):
     """For both parities: the lines the peers send to ``rank`` are exactly the ones it polls, each once; none of them
     is a line it writes itself, and they stay inside the landing zone DpContext allocates."""
-    tiles = ll_tiles(REF)
+    tiles = ll_tiles(sizes)
     zone = _C().dp_ll_zone_lines(dp, len(tiles))
     for parity in (0, 1):
         pre = ll_prefill_lines(tiles, dp, rank, parity)
@@ -726,7 +779,8 @@ def test_ll_prefill_covers_exactly_the_polled_lines(dp, rank):
             sent = torch.cat([f["idx"] for _, f in pre[z]])
             assert sent.unique().numel() == sent.numel(), "two peers write one line"
             assert torch.equal(sent.sort().values, polls[z].sort().values)
-            assert int(sent.min()) >= parity * zone // 2 and int(sent.max()) < (parity + 1) * zone // 2
+            # (a replica whose rows lie past every layer's end, rank 1 of dp 2 on 48-wide layers, polls no phase-A line)
+            assert sent.numel() == 0 or (int(sent.min()) >= parity * zone // 2 and int(sent.max()) < (parity + 1) * zone // 2)
         # every valid row of every tile is either mine (phase B) or arrives in phase C, exactly once
         rows = sum(min(128, o - 128 * mt) * (17 if nt == 0 else 16) for _l, _i, o, mt, nt in tiles)
         n_mine = sum(f["idx"].numel() for key, f in mine.items() if key[0] == "C") // (dp - 1)
@@ -735,14 +789,18 @@ def test_ll_prefill_covers_exactly_the_polled_lines(dp, rank):
 
 @pytest.mark.parametrize("case", range(len(_grid_flags())))
 def test_flag_prefill_covers_exactly_the_polled_flags(case):
+    sizes, dp, rank, switches = _grid_flags()[case]
+    check_flag_prefill(sizes, dp, rank, switches)
+
+
+def check_flag_prefill(sizes, dp, rank, switches):
     """The arrive / done flags the peers set for ``rank`` are exactly the ones it polls but does not set itself, the
     slots they guard do not overlap, and they stay inside the buffers DpContext allocates."""
-    sizes, dp, rank, switches = _grid_flags()[case]
     geom = flag_geometry(sizes, dp, **switches)
     for parity in (0, 1):
         arrive, done, msgs = flag_prefill(geom, dp, rank, parity)
         polled_arrive, polled_done = flag_polls(geom, dp, rank)
-        sps = geom[0]["slots_per_src"]
+        sps = geom[0]["slots_per_src"] if geom else 1
         own_src = set(range(rank * sps, (rank + 1) * sps))
         mine = flag_messages(geom, dp, rank, parity)
         assert {m["arrive"] for m in mine if m["dst"] == rank} == polled_arrive & own_src

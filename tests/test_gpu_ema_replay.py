@@ -154,9 +154,11 @@ def test_dp1_flag_protocol_ema(name, monkeypatch):
 
 
 # pipeline stages: the deferred grouped wave (default), the per-micro-batch accumulation + flat-arena update
-# (SSB_PP_DEFER_WGRAD=0) and the layer-wise path
+# (SSB_PP_DEFER_WGRAD=0) and the layer-wise path; dp x pp stages under the LL wave and under dp_reduce_sgd, where the
+# owned entries are owned_elements of the stage's own layers
 PP_NAMES = ["ref-pp2-s0-naive", "ref-pp2-s1-1f1b-mb24-tf32", "ref-pp4-s2-gpipe-stateful", "ref-pp4-s3-1f1b",
-            "ref-pp4-s2-no-defer", "ref-pp4-s0-no-chain", "wide-pp2-s1-gpipe"]
+            "ref-pp4-s2-no-defer", "ref-pp4-s0-no-chain", "wide-pp2-s1-gpipe", "ref-pp4-s1-dp4-r3-1f1b",
+            "ref-pp4-s1-dp2-r1-no-defer"]
 
 
 @pytest.mark.parametrize("name", PP_NAMES)

@@ -25,9 +25,27 @@ Checked per element and per micro-batch, from the engine's own buffers (the orac
 * outbound flags: exactly the neighbours' arrival flags of the n_mu micro-batches and the one credit per neighbour hold e,
   every other neighbour word still the sentinel, my own flags untouched.
 
-Not covered here, and left to ``test_gpu_multi.py``: concurrent neighbours, real waiting on credits and flags (every
-wait is satisfied before the launch), NVLink visibility ordering, the NCCL transport, and dp x pp stages, where the LL
-kernel reads a receive slot.  This replay is not composed with the data-parallel one (``test_gpu_dp_replay.py``).
+dp x pp (``dp`` / ``rank`` of a case): the stage is also replica ``rank`` of a dp-way group (a stand-in DP communicator,
+``comm_mode="fused"``, peer DpContexts of this process), and the DP half of ``test_gpu_dp_replay.py`` runs next to the
+pipeline half: ``dp_prefill`` writes the DP peers' LL lines or partial tiles and flags before every step, ``dp_check``
+replaces the local update check (5.) with the owned updates against the reduced fp64 oracle, the copied or untouched
+peer elements, every outbound LL line or staging tile and flag, and the momentum ownership, all from the stage's own act
+(act[0] IS the injected receive slot) and dz (dz[L] IS the masked receive slot, or, for a residual last layer, the
+engine's own gated copy).  The plan must run the deferred LL wave (``dp_ll``, every layer ``DP_PROTO_LL``) or one
+``dp_reduce_sgd`` per layer behind per-micro-batch weight gradients, one DP epoch bump and one pipeline epoch bump; both
+epochs advance by one per step.  The stage's MLP and the loss-head oracle scale by the global batch mb * n_mu * dp; the
+injected peer partials take the scale of the stage's own (from its input and received gradient).  The Linear-less last
+stage of pp = 8 runs its head with a DpContext without layers: no DP kernel, nothing sent to the peers, both epochs
+advance.  The residual GELU stage with dropout is checked per element by ``test_gpu_residual.check_residual_layers``
+with the masks of samples (mu * mb + n) * dp + rank at the stage's layer_base.
+
+Measured on an H100 80GB HBM3 (700 W): the worst err / bound of the 16 dp x pp cases is 0.499 (the update of
+wide-pp2-s1-dp4-r3-gpipe), of all cases 0.887 (the tf32 update of ref-pp2-s1-1f1b-mb24-tf32); the whole file, CPU
+tests included, runs in 39 s.
+
+Not covered here, and left to ``test_gpu_multi.py``: concurrent neighbours and peers, real waiting on credits and flags
+(every wait is satisfied before the launch), NVLink visibility ordering, the NCCL and NVLS transports, and
+``optimizer_state()`` / ``ema_state()`` assembled across both groups.
 """
 import gc
 import math
@@ -39,11 +57,15 @@ import torch
 from test_gpu_chain import (FP32_ULP, HEAD_RTOL, LOGIT_SPREAD, RTOL, _gather, _init_weights, _pitched, _poison,
                             dgrad_oracle, excess, fwd_oracle, head_oracle)
 from test_gpu_cross_entropy import ce_head_oracle
-from test_gpu_dp_replay import _StandInComm, _device_view
+from test_gpu_dp_replay import (_StandInComm, _device_view, dp_check, dp_peer_data, dp_prefill, dp_setup, flag_geometry,
+                                local_dp_context, ll_tiles)
 from test_gpu_gemm import grad_oracle, rtol_for, sgd_oracle
+from test_gpu_residual import check_residual_layers
 
 REF = [784, 128, 127, 126, 125, 124, 123, 10]     # the reference model; pp = 4 cuts it at the ragged 127 / 125
 WIDE = [784, 1024, 1000, 1024, 520, 1024, 130, 10]  # layer-wise GEMMs, 520-wide boundaries at pp = 2
+RES_SIZES = [784, 48, 48, 48, 48, 48, 48, 10]      # pp = 4 stage 1: two residual layers, one on each boundary
+FEATURES = dict(activation="gelu", dropout=0.3, dropout_seed=0x5EED_0F_0DD_5EED, residual=True)
 LR, MU, WD = 0.5, 0.9, 5e-4
 LR_STEPS = (0.5, 0.25, 0.375)                       # the case that changes opt.lr between steps (exact in fp32)
 STEPS = 3                                           # the epoch advances, credits come back, the staging set alternates
@@ -65,10 +87,13 @@ def _gen(*key):
 
 
 # ================================================================================================== the case grid
-def _case(sizes, pp, s, sched, mb=32, n_mu=4, env=None, precision="fp32", stateful=False, loss="mse", push=None):
-    """``push``: which push kernel the unfolded transport must reach in its outbound directions ("small" / "multi")."""
+def _case(sizes, pp, s, sched, mb=32, n_mu=4, env=None, precision="fp32", stateful=False, loss="mse", push=None, dp=1,
+          rank=0, model=None):
+    """``push``: which push kernel the unfolded transport must reach in its outbound directions ("small" / "multi").
+    ``dp`` / ``rank``: the stage is DP replica ``rank`` of ``dp`` (its peers replayed as in test_gpu_dp_replay).
+    ``model``: MLP keywords (activation, dropout, residual) of the feature cases."""
     return dict(sizes=sizes, pp=pp, s=s, sched=sched, mb=mb, n_mu=n_mu, env=env or {}, precision=precision,
-                stateful=stateful, loss=loss, push=push)
+                stateful=stateful, loss=loss, push=push, dp=dp, rank=rank, model=model or {})
 
 
 UNFOLD = {"SSB_PP_FOLD": "0"}
@@ -109,6 +134,32 @@ CASES = {
     # wide model, pp = 2: layer-wise GEMMs, 520-wide boundaries moved by the multi-CTA push in both directions
     "wide-pp2-s0-gpipe": _case(WIDE, 2, 0, "gpipe", n_mu=2, push="multi"),
     "wide-pp2-s1-gpipe": _case(WIDE, 2, 1, "gpipe", n_mu=2, push="multi"),
+    # dp x pp: the stage is replica `rank` of a dp-way group; its DP peers are replayed next to its pipeline neighbours.
+    # The deferred LL wave (folded): X is act_in on a non-first stage, dZ the masked dz_in on a non-last one
+    "ref-pp2-s0-dp2-r1-gpipe": _case(REF, 2, 0, "gpipe", dp=2, rank=1),
+    "ref-pp2-s1-dp2-r0-1f1b": _case(REF, 2, 1, "1f1b", dp=2, rank=0),
+    "ref-pp2-s1-dp2-r0-1f1b-ce": _case(REF, 2, 1, "1f1b", n_mu=2, loss="cross_entropy", dp=2, rank=0),
+    "ref-pp4-s1-dp4-r3-1f1b": _case(REF, 4, 1, "1f1b", dp=4, rank=3),
+    "ref-pp4-s2-dp8-r5-gpipe-stateful": _case(REF, 4, 2, "gpipe", stateful=True, dp=8, rank=5),
+    "ref-pp4-s2-dp2-r1-unfolded": _case(REF, 4, 2, "1f1b", env=UNFOLD, push="small", dp=2, rank=1),
+    # per-micro-batch weight gradients through memory, then one dp_reduce_sgd per layer (LL zones allocated, unused)
+    "ref-pp4-s1-dp2-r1-no-defer": _case(REF, 4, 1, "1f1b", env={"SSB_PP_DEFER_WGRAD": "0"}, dp=2, rank=1),
+    # the flag protocol on a stage
+    "ref-pp4-s1-dp4-r2-flags-two-shot-stateful": _case(REF, 4, 1, "gpipe", env={"SSB_DP_LL": "0", "SSB_DP_TWO_SHOT": "1"},
+                                                       stateful=True, dp=4, rank=2),
+    "ref-pp4-s0-dp4-r1-flags-one-shot": _case(REF, 4, 0, "1f1b", env={"SSB_DP_LL": "0"}, dp=4, rank=1),
+    "ref-pp4-s3-dp2-r1-no-chain": _case(REF, 4, 3, "1f1b", env={"SSB_NO_CHAIN": "1"}, push="small", dp=2, rank=1),
+    # a one-Linear stage, and the stage without any Linear: a DpContext with no layers
+    "ref-pp8-s3-dp2-r1-1f1b": _case(REF, 8, 3, "1f1b", dp=2, rank=1),
+    "ref-pp8-s7-dp2-r1-1f1b": _case(REF, 8, 7, "1f1b", push="small", dp=2, rank=1),
+    # layer-wise GEMMs: one-shot and two-shot layers, multi-CTA pushes
+    "wide-pp2-s0-dp2-r1-gpipe": _case(WIDE, 2, 0, "gpipe", n_mu=2, push="multi", dp=2, rank=1),
+    "wide-pp2-s1-dp4-r3-gpipe": _case(WIDE, 2, 1, "gpipe", n_mu=2, push="multi", dp=4, rank=3),
+    # residual GELU layers with dropout on both boundaries: the skip gradient is dz_in, the wgrad reads dz[L].  dp 4, so
+    # that rank 1 owns LL rows of the 48-wide layers (rows 32 .. 47; at dp 2 it would own none)
+    "res-pp4-s1-dp4-r1-gelu-drop": _case(RES_SIZES, 4, 1, "1f1b", dp=4, rank=1, model=FEATURES),
+    "res-pp4-s1-dp4-r1-gelu-drop-no-chain": _case(RES_SIZES, 4, 1, "1f1b", env={"SSB_NO_CHAIN": "1"}, push="small", dp=4,
+                                                 rank=1, model=FEATURES),
 }
 
 
@@ -246,11 +297,11 @@ def _build_stage(c, monkeypatch):
     from shallowspeed_b200.parallel import engine as E
 
     C = _C()
-    pp, s, mb, n_mu = c["pp"], c["s"], c["mb"], c["n_mu"]
-    model = MLP(c["sizes"], s, pp, mb * n_mu, loss=c["loss"]).to("cuda")
+    pp, s, mb, n_mu, dp = c["pp"], c["s"], c["mb"], c["n_mu"], c["dp"]
+    model = MLP(c["sizes"], s, pp, mb * n_mu * dp, loss=c["loss"], **c["model"]).to("cuda")
     rule = dict(momentum=MU, weight_decay=WD, nesterov=True) if c["stateful"] else {}
     opt = SGD(model.parameters(), LR, arena=model.arena, **rule)
-    ctxs = {}
+    ctxs = {"dp": []}
 
     def make_pp_context(comm, eng, n_mu, mb_rows, is_first, is_last):
         # make_pp_context with neighbours that are contexts of this process instead of CUDA IPC mappings
@@ -266,12 +317,51 @@ def _build_stage(c, monkeypatch):
 
     monkeypatch.setattr(E, "make_nccl_comm", lambda comm: None)
     monkeypatch.setattr(E, "make_pp_context", make_pp_context)
+    monkeypatch.setattr(E, "make_dp_context", local_dp_context(ctxs["dp"]))
 
     class _Shape:
         mubatch_size = mb
 
-    w = E.NativeWorker(None, _StandInComm(pp, s), model, _Shape(), opt, precision=c["precision"], pp_transport="peer")
+    w = E.NativeWorker(_StandInComm(dp, c["rank"]) if dp > 1 else None, _StandInComm(pp, s), model, _Shape(), opt,
+                       comm_mode="fused", precision=c["precision"], pp_transport="peer")
     return w, model, opt, ctxs
+
+
+def _ll_on(c, local):
+    """Whether the stage's DpContext allocates LL landing zones (dp_context.cpp)."""
+    tiles = sum(_C().dp_ll_tiles(i, o) for i, o in zip(local[:-1], local[1:]))
+    return c["dp"] > 1 and c["env"].get("SSB_DP_LL", "1") != "0" and 0 < tiles <= 128
+
+
+def _dp_protocol(c, local, deferred):
+    """"ll" when the deferred wave runs the LL kernel, else the flag protocols of the stage's layers ("one-shot",
+    "two-shot" or both, "+"-joined; "" for a stage without layers)."""
+    if deferred and c["dp"] > 1:
+        return "ll"
+    geom = flag_geometry(local, c["dp"], two_shot="SSB_DP_TWO_SHOT" in c["env"], one_shot="SSB_DP_ONE_SHOT" in c["env"])
+    return "+".join(n for n, on in (("one-shot", any(g["one_shot"] for g in geom)),
+                                    ("two-shot", any(not g["one_shot"] for g in geom))) if on)
+
+
+def _stage_grad_scale(local, relu, Ws, x, t, dz_top, n_mu, batch, loss):
+    """Per layer of a stage, the mean |weight gradient| of a plain fp64 ReLU backward pass from the stage input ``x``
+    and, on a non-last stage, the received gradient ``dz_top`` (else the loss head of the targets ``t``): the scale of
+    the injected peer partials."""
+    L, acts = len(local) - 1, [x.double()]
+    for l in range(L):
+        acts.append(fwd_oracle(acts[-1], Ws[l][:, :-1], Ws[l][:, -1], relu[l], 0.0)[0])
+    if dz_top is None:
+        mb, oracle = x.shape[0] // n_mu, ce_head_oracle if loss == "cross_entropy" else head_oracle
+        dz = torch.cat([oracle(acts[L][mu * mb:(mu + 1) * mb], t[mu * mb:(mu + 1) * mb], batch, 0.0)[1][0]
+                        for mu in range(n_mu)])
+    else:
+        dz = dz_top.double() * ((acts[L] > 0).double() if relu[-1] else 1.0)
+    out = [None] * L
+    for l in range(L, 0, -1):
+        out[l - 1] = float(torch.cat([dz.T @ acts[l - 1], dz.sum(0)[:, None]], 1).abs().mean())
+        if l > 1:
+            dz = dgrad_oracle(dz, Ws[l - 1][:, :-1], acts[l - 1] if relu[l - 2] else torch.ones_like(acts[l - 1]), 0.0)[0]
+    return out
 
 
 def _run(name, monkeypatch):
@@ -280,9 +370,11 @@ def _run(name, monkeypatch):
     c = CASES[name]
     for k, v in c["env"].items():
         monkeypatch.setenv(k, v)
-    pp, s, mb, n_mu, precision = c["pp"], c["s"], c["mb"], c["n_mu"], c["precision"]
+    pp, s, mb, n_mu, precision, dp, rank = c["pp"], c["s"], c["mb"], c["n_mu"], c["precision"], c["dp"], c["rank"]
     local = _local(c)
     L, rows = len(local) - 1, mb * n_mu
+    batch = rows * dp                                       # the global batch the loss head scales by
+    feat = bool(c["model"])                                 # gated, dropped, residual layers: check_residual_layers
     first, last, training = s == 0, s == pp - 1, c["sched"] != "inference"
     ld_in, ld_out = _lds(local)
     w, model, opt, ctxs = _build_stage(c, monkeypatch)
@@ -294,12 +386,36 @@ def _run(name, monkeypatch):
     relu = [lin.activation is not None for lin in model.linears]
 
     # ---- the path this case is meant to exercise
-    chain = "SSB_NO_CHAIN" not in c["env"] and c["sizes"] is REF and L >= 1
+    chain = "SSB_NO_CHAIN" not in c["env"] and c["sizes"] is not WIDE and L >= 1
     assert eng.uses_chain() == chain
     folded = chain and c["env"].get("SSB_PP_FOLD", "1") != "0"
-    deferred = chain and training and c["env"].get("SSB_PP_DEFER_WGRAD", "1") != "0"
+    deferred = (chain and training and c["env"].get("SSB_PP_DEFER_WGRAD", "1") != "0"
+                and (dp == 1 or _ll_on(c, local)))
     for st in (0, 1):
-        check_plan(eng.plan_text(st), n_mu, folded, deferred, first, last, training)
+        check_plan(eng.plan_text(st), n_mu, folded, deferred and dp == 1, first, last, training)
+    d = None
+    if dp > 1:
+        # the DP kernel of the plan: the deferred LL wave, or one dp_reduce_sgd per layer behind the final backward
+        C = _C()
+        protos, proto = list(eng.layer_protocols()), _dp_protocol(c, local, deferred)
+        assert ctxs["dp"][rank].ll_tiles() == (len(ll_tiles(local)) if _ll_on(c, local) else 0)
+        d = dp_setup(ctxs["dp"], rank, proto, local, c["env"], arena, protos)
+        for st in (0, 1):
+            text = eng.plan_text(st)
+            ops = [o[1] for o in _plan(text)]
+            assert ops.count("bump_epoch") == 1 and "fused_wgrad_dp" not in ops, text
+            if proto == "ll":
+                assert ops.count("dp_ll") == 1 and "dp_reduce_sgd" not in ops, text
+            else:
+                assert ops.count("dp_reduce_sgd") == L and "dp_ll" not in ops, text
+        if proto == "ll":
+            assert protos == [C.DP_PROTO_LL] * L
+        else:
+            got = ctxs["dp"][rank].layer_geometry()
+            assert len(got) == len(d["geom"]) == L
+            for g, h in zip(d["geom"], got):
+                assert all(g[key] == h[key] for key in g), (g, h)
+            assert protos == [C.DP_PROTO_ALL if g["one_shot"] else C.DP_PROTO_TWO_SHOT for g in d["geom"]]
     assert tuple(eng.boundary_lds()) == (ld_in, ld_out)
     if c["push"] is not None:
         assert not folded
@@ -325,14 +441,14 @@ def _run(name, monkeypatch):
           for _ in range(STEPS)]
     dzs = [torch.randn(rows, local[-1], generator=gen) * DZ_SCALE for _ in range(STEPS)]
     if L > 0:
-        Ws, bs = _init_weights(local, xs[0], n_mu, gen)
+        Ws, bs = _init_weights(local, xs[0], n_mu, gen, activation=model.activation)
         for i, (W, b) in enumerate(zip(Ws, bs)):
             arena.weight_view(i).copy_(W)
             arena.bias_view(i).copy_(b[None, :])
             if c["stateful"]:
                 o, k = arena.blocks[i]
                 arena.momentum_block(i)[:, : k + 1] = torch.randn(o, k + 1, generator=gen).cuda() * 1e-3
-    _poison(eng, model, local, rows, training)
+    _poison(eng, model, local, rows, training, gated=feat)
     if first and training:
         _pitched(eng.dz(0, 0), rows).fill_(NAN)            # the first stage never produces dz[0]
     lrs = LR_STEPS if c["stateful"] else (LR,) * STEPS
@@ -345,6 +461,14 @@ def _run(name, monkeypatch):
         W0 = [arena.block(i)[:, : k + 1].double().cpu() for i, (_, k) in enumerate(arena.blocks)]
         V0 = [arena.momentum_block(i)[:, : k + 1].double().cpu() for i, (_, k) in enumerate(arena.blocks)] \
             if c["stateful"] else [torch.zeros_like(W) for W in W0]
+        W0_flat = arena.weights.detach().clone()
+        model.dropout_step = step
+        if d is not None:
+            # the peers' partials at the scale of this stage's own (the stage's input and received gradient)
+            dp_epoch = int(d["me"].epoch[0].item()) + 1
+            scale = _stage_grad_scale(local, relu, W0, xs[step], ts[step], None if last else dzs[step], n_mu, batch,
+                                      c["loss"])
+            P, Wc = dp_peer_data(d, gen, arena.blocks, scale, W0, lrs[step])
         torch.cuda.synchronize()
         # ---- inbound: what the neighbours send; my flags: every poll satisfied, both credits at e - 1
         if not first:
@@ -358,6 +482,8 @@ def _run(name, monkeypatch):
             ctx.act_in.fill_(NAN)
             ctx.dz_in.fill_(NAN)
             ctx.flags.fill_(SENTINEL)
+        if d is not None:
+            dp_prefill(d, P, Wc, dp_epoch)
         torch.cuda.synchronize()
 
         opt.lr = lrs[step]
@@ -374,15 +500,15 @@ def _run(name, monkeypatch):
 
         # ---- non-vacuity
         for l in range(0 if not first else 1, L + 1):
-            if l == 0 or relu[l - 1]:
+            if not feat and (l == 0 or relu[l - 1]):
                 frac = float((act[l] > 0).double().mean())
                 assert 0.05 <= frac <= 0.95, f"step {step + 1}: {frac:.3f} of act[{l}] is positive"
         if training:
             for l in range(0 if not first else 1, L + 1):
                 assert float(dz[l].abs().max()) > 0.0, f"step {step + 1}: dz[{l}] is all zero"
 
-        # ---- 1. forward, every layer from the kernel's own input
-        for l in range(1, L + 1):
+        # ---- 1. forward, every layer from the kernel's own input (feature cases: check_residual_layers below)
+        for l in range(1, L + 1 if not feat else 1):
             W, b = W0[l - 1][:, :-1], W0[l - 1][:, -1]
             ref, bound = fwd_oracle(act[l - 1], W, b, relu[l - 1], rtol)
             res[p + f"fwd{l}"] = excess(act[l], ref, bound)
@@ -394,7 +520,7 @@ def _run(name, monkeypatch):
             oracle = ce_head_oracle if c["loss"] == "cross_entropy" else head_oracle
             for mu in range(n_mu):
                 r = slice(mu * mb, (mu + 1) * mb)
-                (pr, bp), (g, bg), (lv, bl) = oracle(act[L][r], ts[step][r], rows, HEAD_RTOL)
+                (pr, bp), (g, bg), (lv, bl) = oracle(act[L][r], ts[step][r], batch, HEAD_RTOL)
                 res[p + "probs"] = max(res.get(p + "probs", 0.0), excess(probs[r], pr, bp))
                 if training:
                     res[p + "dzL"] = max(res.get(p + "dzL", 0.0), excess(dz[L][r], g, bg))
@@ -403,18 +529,30 @@ def _run(name, monkeypatch):
                 res[p + "loss"] = abs(loss - loss_ref) / loss_bound if math.isfinite(loss) else math.inf
 
         if training:
-            # ---- 3. the received gradient, masked in place
-            if not last:
+            # ---- 3. the received gradient, masked in place (a residual last layer keeps it: dz_in stays unmodified)
+            if not last and not feat:
                 check_received_grad(dz[L].float().view(n_mu, mb, -1), act[L].float().view(n_mu, mb, -1),
                                     dzs[step].view(n_mu, mb, -1), local[-1], f"step {step + 1}: dz[{L}]")
+            elif not last:
+                assert torch.equal(me.dz_in.cpu()[..., : local[-1]], dzs[step].view(n_mu, mb, -1)), "dz_in was modified"
+            if feat:
+                # every activated, dropped, residual layer per element, with the masks of the replica's samples
+                # (mu * mb + n) * dp + rank at the stage's layer_base; the received gradient as the skip gradient g[L]
+                got = check_residual_layers(eng, model, W0_flat, xs[step], n_mu, mb, precision, lrs[step], step=step,
+                                            g_in=None if last else dzs[step].view(n_mu, mb, -1),
+                                            samples_of=lambda mu: (mu * mb + torch.arange(mb)) * dp + rank)
+                res.update({p + k: v for k, v in got.items()})
             # ---- 4. dgrad chain (layer 1 unmasked, and only on non-first stages)
             for l in range(L, 0 if not first else 1, -1):
+                if feat:
+                    break
                 mask = act[l - 1] if l >= 2 else torch.ones_like(act[0])
                 ref, bound = dgrad_oracle(dz[l], W0[l - 1][:, :-1], mask, rtol)
                 res[p + f"dgrad{l}"] = excess(dz[l - 1], ref, bound)
             if first:
                 assert bool(torch.isnan(_pitched(eng.dz(0, 0), rows)).all()), "the first stage wrote dz[0]"
-            # ---- 5. the update at this step's learning rate
+            # ---- 5. the update at this step's learning rate: local, or through the DP kernel with the peers replayed
+            own, own_b = [], []
             for i, (o, k) in enumerate(arena.blocks):
                 if deferred:
                     g, gb = grad_oracle(dz[i + 1], act[i], rtol_for(precision, rows))
@@ -422,12 +560,18 @@ def _run(name, monkeypatch):
                     g, gb = grad_oracle(dz[i + 1], act[i], rtol_for(precision, mb))
                     mag, _ = grad_oracle(dz[i + 1].abs(), act[i].abs(), 0.0)
                     gb = gb + (n_mu - 1) * FP32_ULP * mag
+                own.append(g)
+                own_b.append(gb)
+                if d is not None:
+                    continue
                 st = c["stateful"]
                 Wr, bW, Vr, bV = sgd_oracle(g, gb, W0[i], V0[i], lrs[step], MU if st else 0.0, WD if st else 0.0, st)
                 res[p + f"upd{i + 1}"] = excess(arena.block(i)[:, : k + 1].cpu(), Wr, bW)
                 if st:
                     res[p + f"mom{i + 1}"] = excess(arena.momentum_block(i)[:, : k + 1].cpu(), Vr, bV)
                 assert bool(torch.isnan(arena.block(i)[:, k + 1:]).all()), f"the padding of layer {i + 1}'s weights changed"
+            if d is not None:
+                dp_check(d, res, step, arena, own, own_b, P, Wc, W0, V0, lrs[step], c["stateful"], dp_epoch)
 
         # ---- 6. outbound tiles, read from the neighbours' memory
         if "next" in nb:
@@ -473,7 +617,7 @@ def test_grid_reaches_every_stage_and_transport_branch():
         first, last, training = s == 0, s == pp - 1, c["sched"] != "inference"
         layers = list(zip(local[:-1], local[1:]))
         eligible = L >= 1 and C.chain_eligible(layers, c["mb"], local[-1], last, c["precision"] == "fp32")
-        assert eligible == (c["sizes"] is REF and L >= 1), name
+        assert eligible == (c["sizes"] is not WIDE and L >= 1), name
         chain = eligible and "SSB_NO_CHAIN" not in c["env"]
         folded = chain and c["env"].get("SSB_PP_FOLD", "1") != "0"
         stages.add((tuple(c["sizes"]), pp, s))
@@ -496,6 +640,8 @@ def test_grid_reaches_every_stage_and_transport_branch():
         seen["loss"].add(c["loss"])
         if L == 0:
             assert last and pp == 8 and c["sizes"] is REF
+        if c["model"]:
+            assert c["sizes"] is RES_SIZES and c["dp"] > 1
     assert {(tuple(REF), pp, s) for pp in (2, 4) for s in range(pp)} <= stages
     assert {(tuple(REF), 8, 3), (tuple(REF), 8, 7), (tuple(WIDE), 2, 0), (tuple(WIDE), 2, 1)} <= stages
     assert len(_local(CASES["ref-pp8-s3-1f1b"])) == 2 and len(_local(CASES["ref-pp8-s7-1f1b"])) == 1
@@ -508,6 +654,78 @@ def test_grid_reaches_every_stage_and_transport_branch():
     assert {("fp32", True), ("fp32", False), ("tf32", True)} == seen["prec"]
     assert ("stateful", "middle") in seen["opt"]
     assert seen["loss"] == {"mse", "cross_entropy"}
+
+
+def _dp_path(c):
+    """(protocol, DP kernel, launch form) a dp > 1 case must reach, from the shape rules alone: ``_C.chain_eligible``
+    for the chain kernel, the LL zone rule and ``flag_geometry`` for the protocol."""
+    C = _C()
+    local = _local(c)
+    L, last = len(local) - 1, c["s"] == c["pp"] - 1
+    chain = (L >= 1 and "SSB_NO_CHAIN" not in c["env"]
+             and C.chain_eligible(list(zip(local[:-1], local[1:])), c["mb"], local[-1], last, c["precision"] == "fp32"))
+    deferred = chain and c["env"].get("SSB_PP_DEFER_WGRAD", "1") != "0" and _ll_on(c, local)
+    proto = _dp_protocol(c, local, deferred)
+    form = "layer-wise" if not chain else "folded" if c["env"].get("SSB_PP_FOLD", "1") != "0" else "unfolded"
+    kernel = "dp_ll" if proto == "ll" else "dp_reduce_sgd" if L else "none"
+    return proto, kernel, form
+
+
+DP_CASES = [n for n, c in CASES.items() if c["dp"] > 1]
+
+
+def test_dp_grid_reaches_every_position_protocol_and_form():
+    """The dp x pp cases reach every stage position, every DP protocol (LL, one-shot, two-shot, each through its kernel),
+    dp 2, 4 and 8, every launch form, the per-micro-batch wgrad path, the flag protocol on a stage, momentum, both
+    losses, the one-Linear and the Linear-less stage and the residual feature stage, with ranks off zero."""
+    seen = {k: set() for k in ("pos", "proto", "kernel", "dp", "form", "misc")}
+    for name in DP_CASES:
+        c = CASES[name]
+        local = _local(c)
+        L, first, last = len(local) - 1, c["s"] == 0, c["s"] == c["pp"] - 1
+        proto, kernel, form = _dp_path(c)
+        assert c["sched"] != "inference" and 0 <= c["rank"] < c["dp"], name
+        seen["pos"].add("first" if first else "last" if last else "middle")
+        seen["proto"] |= set(proto.split("+")) - {""}
+        seen["kernel"].add(kernel)
+        seen["dp"].add(c["dp"])
+        seen["form"].add(form)
+        seen["misc"] |= {f"L={L}" for L in (0, 1) if len(local) - 1 == L}
+        seen["misc"] |= {k for k, on in (("stateful", c["stateful"]), ("ce", c["loss"] == "cross_entropy"),
+                                         ("res", bool(c["model"])), ("rank>0", c["rank"] > 0),
+                                         ("no-defer", c["env"].get("SSB_PP_DEFER_WGRAD") == "0" and form != "layer-wise"),
+                                         ("flags-on-chain", proto != "ll" and form != "layer-wise" and L > 0)) if on}
+        if proto == "ll":
+            assert form != "layer-wise" and kernel == "dp_ll"
+        if c["model"]:
+            assert form in ("folded", "layer-wise") and not first and not last
+    assert seen["pos"] == {"first", "middle", "last"}
+    assert seen["proto"] == {"ll", "one-shot", "two-shot"}
+    assert seen["kernel"] == {"dp_ll", "dp_reduce_sgd", "none"}
+    assert seen["dp"] == {2, 4, 8}
+    assert seen["form"] == {"folded", "unfolded", "layer-wise"}
+    assert seen["misc"] == {"L=0", "L=1", "stateful", "ce", "res", "rank>0", "no-defer", "flags-on-chain"}
+    # every protocol at every position it can run at: LL needs the chain kernel
+    pairs = {(("first" if c["s"] == 0 else "last" if c["s"] == c["pp"] - 1 else "middle"), p)
+             for c in map(CASES.get, DP_CASES) for p in _dp_path(c)[0].split("+") if p}
+    assert {(pos, p) for pos in ("first", "middle", "last") for p in ("ll", "one-shot")} <= pairs, pairs
+    assert {("first", "two-shot"), ("middle", "two-shot"), ("last", "two-shot")} <= pairs, pairs
+
+
+@pytest.mark.parametrize("name", DP_CASES)
+def test_dp_prefill_covers_exactly_the_polled_lines_and_flags(name):
+    """For the local layers, dp and rank of every dp x pp case: the LL or flag prefill covers exactly what the replica
+    polls (test_gpu_dp_replay's checks on the stage's geometry)."""
+    from test_gpu_dp_replay import check_flag_prefill, check_ll_prefill
+
+    c = CASES[name]
+    local = _local(c)
+    proto, _kernel, _form = _dp_path(c)
+    if proto == "ll":
+        check_ll_prefill(local, c["dp"], c["rank"])
+    else:
+        check_flag_prefill(local, c["dp"], c["rank"], dict(two_shot="SSB_DP_TWO_SHOT" in c["env"],
+                                                          one_shot="SSB_DP_ONE_SHOT" in c["env"]))
 
 
 def _emulated_stage(seed=0):
@@ -584,6 +802,122 @@ def test_checks_reject_injected_faults():
         fault(t)
         with pytest.raises(AssertionError):
             _check_emulated(t)
+
+
+def _emulated_dpxpp_stage(fault=None):
+    """Replica 1 of dp = 4 of stage 1 of a pp = 4 model with residual GELU layers and dropout, one step emulated on the
+    CPU (fp64, stored in fp32) with its peer's partials, its LL update, its flags and, for the loss scale, a last stage's
+    head.  ``fault`` injects one plausible dp x pp fault; the result is what the GPU test reads back from the engine."""
+    from shallowspeed_b200.layers import MLP
+    from shallowspeed_b200.ops import functional as F
+    from test_gpu_chain import act_ref
+
+    sizes, pp, st, dp, rank, n_mu, mb, lr, step, e = [20, 48, 48, 48, 48, 48, 48, 4], 4, 1, 4, 1, 2, 3, 0.5, 4, 6
+    rows = n_mu * mb
+    model = MLP(sizes, st, pp, rows * dp, **FEATURES)
+    L = len(model.linears)
+    g = torch.Generator().manual_seed(1)
+    arena = model.arena
+    blocks = [torch.randn(o, k + 1, generator=g, dtype=torch.float64).float().double() * 0.3 for o, k in arena.blocks]
+    W0 = torch.zeros(arena.numel)
+    for i, (o, k) in enumerate(arena.blocks):
+        W0[arena.offsets[i]: arena.offsets[i] + o * arena.lds[i]].view(o, -1)[:, : k + 1] = blocks[i].float()
+    x = torch.randn(rows, 48, generator=g).clamp_min(0.0)          # act_in
+    x_stage = torch.randn(rows, 48, generator=g)                    # what the staging buffer holds
+    g_in = torch.randn(rows, 48, generator=g) * 1e-2                # dz_in
+    s = F.dropout_scale(FEATURES["dropout"])
+    src_rank = 0 if fault == "rank0-masks" else rank
+    base = 1 if fault == "layer-base" else 0
+    acts, gates = [x.double()], [None]
+    for l, lin in enumerate(model.linears, start=1):
+        z = acts[-1] @ blocks[l - 1][:, :-1].T + blocks[l - 1][:, -1]
+        keep = torch.cat([F.dropout_mask(FEATURES["dropout"], FEATURES["dropout_seed"], lin.dropout[2] + base, step,
+                                         (mu * mb + torch.arange(mb)) * dp + src_rank, lin.out_dims) for mu in range(n_mu)])
+        f, f1, _ = act_ref("gelu", z)
+        acts.append((acts[-1] + torch.where(keep, f * s, 0.0)).float().double())
+        gates.append(torch.where(keep, f1 * s, 0.0).float())           # a dropped gate is +0
+    dz = [None] * (L + 1)
+    dz[L] = g_in if fault == "dz-is-dz_in" else g_in * gates[L]      # fp32 multiply, out of place
+    gl = g_in.double()
+    for l in range(L, 0, -1):
+        pre = dz[l].double() @ blocks[l - 1][:, :-1] + gl
+        dz[l - 1] = (pre * gates[l - 1].double()).float() if l > 1 else pre.float()
+        gl = pre
+    # the update: own partial [dz.T @ act | colsum] + the peers', plain SGD on the rows this replica owns (LL: rows
+    # 32 .. 63 of every 128-row tile)
+    P = {p: [torch.randn(o, k + 1, generator=g) * 1e-2 for o, k in arena.blocks] for p in range(dp) if p != rank}
+    own, own_b, W1 = [], [], []
+    for i, (o, k) in enumerate(arena.blocks):
+        a_used = x_stage if fault == "staging-x" and i == 0 else acts[i]
+        dz_used = g_in if fault == "unmasked-dz" and i == L - 1 else dz[i + 1]
+        gr, gb = grad_oracle(dz[i + 1], acts[i], RTOL["fp32"])
+        used = torch.cat([dz_used.double().T @ a_used.double(), dz_used.double().sum(0)[:, None]], 1)
+        tot = used + sum(P[p][i].double() for p in P if not (fault == "dropped-peer" and p == 3))
+        own.append(gr)
+        own_b.append(gb)
+        W1.append((blocks[i] - lr * tot).float())
+    owned = [(torch.arange(o)[:, None] % 128 // (128 // dp) == rank).expand(o, k + 1) for o, k in arena.blocks]
+    # a last stage's loss head: dz of the logits scaled by 1 / (mb * n_mu * dp)
+    logits = torch.randn(mb, 4, generator=g, dtype=torch.float64) * 5
+    t = torch.nn.functional.one_hot(torch.randint(0, 4, (mb,), generator=g), 4).double()
+    dz_head = head_oracle(logits, t, rows * (1 if fault == "loss-scale" else dp), 0.0)[1][0].float()
+    # flags: one credit per neighbour, my arrival flags into the successor's act_arrived
+    layout = {"act_arrived": (0, 16), "dz_arrived": (16, 16), "act_credit": (32, 1), "dz_credit": (40, 1)}
+    flags = {side: neighbour_flags(layout, 48, n_mu, e, side, True) for side in ("prev", "next")}
+    if fault == "no-credit":
+        flags["prev"][layout["act_credit"][0]] = SENTINEL
+
+    class Eng:
+        def act(self, mu, l):
+            return acts[l][mu * mb:(mu + 1) * mb].float()
+
+        def dz(self, mu, l):
+            return dz[l][mu * mb:(mu + 1) * mb]
+
+        def gate(self, mu, l):
+            return gates[l][mu * mb:(mu + 1) * mb]
+
+        def g(self, mu, l):
+            assert l == L
+            return g_in[mu * mb:(mu + 1) * mb]
+
+        def uses_chain(self):
+            return True
+
+    return dict(eng=Eng(), model=model, W0=W0, x=x, g_in=g_in, n_mu=n_mu, mb=mb, dp=dp, rank=rank, step=step, lr=lr,
+                blocks=blocks, own=own, own_b=own_b, P=P, W1=W1, owned=owned, logits=logits, t=t, dz_head=dz_head,
+                batch=rows * dp, layout=layout, flags=flags, e=e)
+
+
+def _check_emulated_dpxpp(t):
+    """The GPU test's checks of a dp x pp stage, applied to an emulated one."""
+    from test_gpu_dp_replay import check_owned_update
+
+    n_mu, mb, dp, rank = t["n_mu"], t["mb"], t["dp"], t["rank"]
+    check_residual_layers(t["eng"], t["model"], t["W0"], t["x"], n_mu, mb, "fp32", t["lr"], step=t["step"],
+                          g_in=t["g_in"].view(n_mu, mb, -1), samples_of=lambda mu: (mu * mb + torch.arange(mb)) * dp + rank)
+    res = {}
+    for i, blk in enumerate(t["blocks"]):
+        assert bool(t["owned"][i].any())
+        check_owned_update(t["W1"][i], t["own"][i], t["own_b"][i], [t["P"][p][i] for p in t["P"]], blk, None, None,
+                           t["lr"], False, t["owned"][i], res, "%s" + str(i + 1))
+    (_, _), (g, bg), _ = head_oracle(t["logits"], t["t"], t["batch"], HEAD_RTOL)
+    res["dzL"] = excess(t["dz_head"], g, bg)
+    assert all(v <= 1.0 for v in res.values()), res
+    for side in ("prev", "next"):
+        check_flags(t["flags"][side], neighbour_flags(t["layout"], 48, n_mu, t["e"], side, True), side)
+
+
+def test_dpxpp_checks_reject_injected_faults():
+    """The checks of a dp x pp stage accept an emulated correct stage and reject each fault of the composition: the own
+    partial from the staging buffer instead of act_in, the LL wave reading the received gradient unmasked, dz[L] of a
+    residual last layer replaced by dz_in, a loss scale without the dp factor, rank 0's dropout masks on rank 1, the
+    stage's layer_base off by one, a peer partial dropped, and a pipeline credit not returned."""
+    _check_emulated_dpxpp(_emulated_dpxpp_stage())
+    for fault in ("staging-x", "unmasked-dz", "dz-is-dz_in", "loss-scale", "rank0-masks", "layer-base", "dropped-peer",
+                  "no-credit"):
+        with pytest.raises(AssertionError):
+            _check_emulated_dpxpp(_emulated_dpxpp_stage(fault))
 
 
 def test_plan_check_counts_pushes_and_waits_per_micro_batch():

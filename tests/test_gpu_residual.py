@@ -43,9 +43,10 @@ def _batch(rows, in_dim, classes, seed=0):
     return x.pin_memory(), y.pin_memory()
 
 
-def check_residual_layers(eng, model, W0, x, n_mu, mb, precision, lr, step=0, g_in=None):
+def check_residual_layers(eng, model, W0, x, n_mu, mb, precision, lr, step=0, g_in=None, samples_of=None):
     """Every layer of the step that just ran against fp64 from the engine's own buffers; returns {check: err / bound}.
-    ``g_in``: the gradient a non-last stage received ([n_mu, mb, out]), else None."""
+    ``g_in``: the gradient a non-last stage received ([n_mu, mb, out]), else None.  ``samples_of(mu)``: the global
+    sample index of every row of micro-batch mu, whose dropout masks the rows draw (default: mu * mb + n, one replica)."""
     from shallowspeed_b200.ops import functional as F
 
     kind, p, rtol = model.activation, model.dropout, RT[precision]
@@ -62,7 +63,7 @@ def check_residual_layers(eng, model, W0, x, n_mu, mb, precision, lr, step=0, g_
         res[k] = max(res.get(k, 0.0), v)
 
     for mu in range(n_mu):
-        samples = mu * mb + torch.arange(mb)
+        samples = samples_of(mu) if samples_of is not None else mu * mb + torch.arange(mb)
         acts = [x[mu * mb:(mu + 1) * mb].double()] + [eng.act(mu, l).double().cpu() for l in range(1, L + 1)]
         dzs = [eng.dz(mu, l).cpu() for l in range(L + 1)]
         gates = [None] * (L + 1)

@@ -82,9 +82,12 @@ static ssb::DropoutSpec drop_arg(const py::object& drop, const Tensor& like, Ten
 // y[rows, out] = act?(x @ W^T + b); prec: the products' Precision (precision.h; a bool: false TF32, true 3xTF32).  relu selects the layer's activation
 // act_kind (activation.h: ReLU by default); a smooth kind can store its gate f'(z) (* keep * s under dropout) to `gate`,
 // which the kernel addresses with y's row pitch.  drop: see drop_arg, applied after the activation.
+// res: the residual form (GemmParams::res), gated for every act_kind (a ReLU gate is 1[z > 0] * keep * s), and
+// y = skip + act(z) when `skip` ([rows, out], a row pitch of its own) is given.
 static void linear_fwd(const Tensor& x, const Tensor& W, const c10::optional<Tensor>& bias, int64_t bias_stride,
                        bool relu, Tensor& y, int64_t prec, int64_t k_splits, int64_t act_kind,
-                       const c10::optional<Tensor>& gate, const py::object& drop) {
+                       const c10::optional<Tensor>& gate, const py::object& drop, bool res,
+                       const c10::optional<Tensor>& skip) {
     check_mat(x, "x"); check_mat(W, "W"); check_mat(y, "y");
     const int rows = x.size(0), in = x.size(1), out = W.size(0);
     TORCH_CHECK(W.size(1) == in && y.size(0) == rows && y.size(1) == out, "linear_fwd: shape mismatch");
@@ -93,9 +96,14 @@ static void linear_fwd(const Tensor& x, const Tensor& W, const c10::optional<Ten
                 "linear_fwd: an activation kind, a gate or dropout needs relu (an activated layer)");
     if (gate.has_value()) {
         check_mat(*gate, "gate");
-        TORCH_CHECK(ssb::act_smooth((int)act_kind), "linear_fwd: only a smooth activation stores a gate");
+        TORCH_CHECK(res || ssb::act_smooth((int)act_kind), "linear_fwd: only a smooth activation or a residual layer stores a gate");
         TORCH_CHECK(gate->size(0) == rows && gate->size(1) == out && gate->device() == y.device(), "linear_fwd: gate shape");
         TORCH_CHECK(ld_of(*gate) == ld_of(y), "linear_fwd: the gate must have y's row pitch (the kernel writes it with y's)");
+    }
+    if (skip.has_value()) {
+        TORCH_CHECK(res, "linear_fwd: a skip needs residual");
+        check_mat(*skip, "skip");
+        TORCH_CHECK(skip->size(0) == rows && skip->size(1) == out && skip->device() == y.device(), "linear_fwd: skip shape");
     }
     c10::cuda::CUDAGuard guard(x.device());
     ssb::GemmPlan plan;
@@ -107,6 +115,11 @@ static void linear_fwd(const Tensor& x, const Tensor& W, const c10::optional<Ten
     plan.p.act_kind = (int)act_kind;
     plan.p.gate = gate.has_value() ? gate->data_ptr<float>() : nullptr;
     plan.p.drop = drop_arg(drop, x, step_dev, "linear_fwd");
+    if (res) {
+        plan.p.res = 1;
+        plan.p.skip = skip.has_value() ? skip->data_ptr<float>() : nullptr;
+        plan.p.ldskip = skip.has_value() ? ld_of(*skip) : 0;
+    }
     Tensor ws, counters;
     enable_splitk(plan, k_splits, x, ws, counters);
     cuda_ok(ssb::gemm_launch(plan, cur_stream()), "linear_fwd launch");
@@ -114,8 +127,12 @@ static void linear_fwd(const Tensor& x, const Tensor& W, const c10::optional<Ten
 
 // dx[rows, in] = (dz @ W) * (mask > 0), or * s where the mask passes under dropout (only its p is read), or * mask for a
 // smooth act_kind (the mask is then the previous layer's gate, which holds the dropout scale itself)
+// res: the residual form (GemmParams::res): x = dz @ W + skip (skip: the layer's output gradient, [rows, in]), stored to
+// gpre before the mask, then dx = x * mask (the mask is the previous layer's gate for every act_kind).  skip, gpre and
+// the mask each have a row pitch of their own.
 static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<Tensor>& mask, Tensor& dx,
-                         int64_t prec, int64_t k_splits, int64_t act_kind, const py::object& drop) {
+                         int64_t prec, int64_t k_splits, int64_t act_kind, const py::object& drop, bool res,
+                         const c10::optional<Tensor>& skip, const c10::optional<Tensor>& gpre) {
     check_mat(dz, "dz"); check_mat(W, "W"); check_mat(dx, "dx");
     const int rows = dz.size(0), out = dz.size(1), in = W.size(1);
     TORCH_CHECK(W.size(0) == out && dx.size(0) == rows && dx.size(1) == in, "linear_dgrad: shape mismatch");
@@ -125,6 +142,17 @@ static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<
                 "linear_dgrad: an activation kind or dropout needs a mask");
     TORCH_CHECK(drop.is_none() || !ssb::act_smooth((int)act_kind),
                 "linear_dgrad: a gate holds its dropout scale already; pass no dropout with a smooth act_kind");
+    TORCH_CHECK(drop.is_none() || !res, "linear_dgrad: a residual gate holds its dropout scale already; pass no dropout");
+    TORCH_CHECK(res || (!skip.has_value() && !gpre.has_value()), "linear_dgrad: skip and gpre need residual");
+    if (skip.has_value()) {
+        check_mat(*skip, "skip");
+        TORCH_CHECK(skip->size(0) == rows && skip->size(1) == in && skip->device() == dx.device(), "linear_dgrad: skip shape");
+    }
+    if (gpre.has_value()) {
+        check_mat(*gpre, "gpre");
+        TORCH_CHECK(gpre->size(0) == rows && gpre->size(1) == in && gpre->device() == dx.device(), "linear_dgrad: gpre shape");
+    }
+    if (mask.has_value()) TORCH_CHECK(mask->device() == dx.device(), "linear_dgrad: mask device");
     c10::cuda::CUDAGuard guard(dz.device());
     ssb::GemmPlan plan;
     const char* err = ssb::gemm_plan_dgrad(&plan, W.data_ptr<float>(), ld_of(W), dz.data_ptr<float>(), ld_of(dz),
@@ -135,6 +163,13 @@ static void linear_dgrad(const Tensor& dz, const Tensor& W, const c10::optional<
     Tensor step_dev;
     plan.p.act_kind = (int)act_kind;
     plan.p.drop = drop_arg(drop, dz, step_dev, "linear_dgrad");
+    if (res) {
+        plan.p.res = 1;
+        plan.p.skip = skip.has_value() ? skip->data_ptr<float>() : nullptr;
+        plan.p.ldskip = skip.has_value() ? ld_of(*skip) : 0;
+        plan.p.gpre = gpre.has_value() ? gpre->data_ptr<float>() : nullptr;
+        plan.p.ldgpre = gpre.has_value() ? ld_of(*gpre) : 0;
+    }
     Tensor ws, counters;
     enable_splitk(plan, k_splits, dz, ws, counters);
     cuda_ok(ssb::gemm_launch(plan, cur_stream()), "linear_dgrad launch");
@@ -333,10 +368,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.doc() = "shallowspeed_b200 native module: sm_90a kernels + C++ pipeline runtime";
     m.def("linear_fwd", &linear_fwd, py::arg("x"), py::arg("W"), py::arg("bias"), py::arg("bias_stride"), py::arg("relu"),
           py::arg("y"), py::arg("prec") = (int)ssb::PREC_TF32, py::arg("k_splits") = 0, py::arg("act_kind") = (int)ssb::ACT_RELU,
-          py::arg("gate") = py::none(), py::arg("drop") = py::none());
+          py::arg("gate") = py::none(), py::arg("drop") = py::none(), py::arg("res") = false, py::arg("skip") = py::none());
     m.def("linear_dgrad", &linear_dgrad, py::arg("dz"), py::arg("W"), py::arg("mask"), py::arg("dx"),
           py::arg("prec") = (int)ssb::PREC_TF32, py::arg("k_splits") = 0, py::arg("act_kind") = (int)ssb::ACT_RELU,
-          py::arg("drop") = py::none());
+          py::arg("drop") = py::none(), py::arg("res") = false, py::arg("skip") = py::none(), py::arg("gpre") = py::none());
     m.def("linear_wgrad", &linear_wgrad, py::arg("dz"), py::arg("x"), py::arg("G"), py::arg("accumulate"), py::arg("db"),
           py::arg("db_stride"), py::arg("W"), py::arg("lr"), py::arg("fuse_sgd"), py::arg("prec") = (int)ssb::PREC_TF32,
           py::arg("V") = py::none(), py::arg("momentum") = 0.0, py::arg("weight_decay") = 0.0, py::arg("nesterov") = false,

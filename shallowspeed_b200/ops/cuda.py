@@ -87,26 +87,33 @@ def _drop_arg(dropout):
 
 
 def linear_fwd(x, weight, bias=None, relu=False, out=None, precision=None, k_splits=0, activation="relu", gate=None,
-               dropout=None):
+               dropout=None, residual=False, skip=None):
     """k_splits: 0 = plain kernel, -1 = planner decides, k >= 2 = force k k-splits (experimental wide-layer variant).
     With ``relu`` the layer is activated by ``activation``; a smooth one stores f'(z) into ``gate`` (a view with ``out``'s
-    row pitch) when one is given.  ``dropout`` (see ``_drop_arg``) drops the activated output and its gate."""
+    row pitch) when one is given.  ``dropout`` (see ``_drop_arg``) drops the activated output and its gate.
+    ``residual`` runs the residual form of the layer: every activation is gated (ReLU's gate is 1[z > 0] * keep * s), and
+    ``skip`` ([rows, out], any row pitch; the layer's input in a model) is added after the activation and dropout."""
     x, weight = as_tma(x), as_tma(weight)
     rows, out_dims = x.size(0), weight.size(0)
     y = out if out is not None else empty_padded(rows, out_dims, x.device)
     b, bstride = _bias_arg(bias, out_dims)
     _C.linear_fwd(x, weight, b, bstride, bool(relu), y, _prec(precision), int(k_splits), _act_code(activation), gate,
-                  _drop_arg(dropout))
+                  _drop_arg(dropout), bool(residual), skip)
     return y
 
 
-def linear_dgrad(dz, weight, mask=None, out=None, precision=None, k_splits=0, activation="relu", dropout=None):
+def linear_dgrad(dz, weight, mask=None, out=None, precision=None, k_splits=0, activation="relu", dropout=None,
+                 residual=False, skip=None, gpre=None):
     """dX = dz @ W, masked where ``mask <= 0`` (ReLU; times the dropout scale where it passes when ``dropout`` is given), or
-    times ``mask`` for a smooth ``activation``, whose mask is the previous layer's gate."""
+    times ``mask`` for a smooth ``activation``, whose mask is the previous layer's gate.  ``residual`` runs the residual
+    form: ``skip`` (the layer's output gradient, [rows, in]) is added to dz @ W, the sum is stored to ``gpre`` before the
+    mask, and the mask is the previous layer's gate for every activation; no ``dropout`` (the gate holds its scale).  skip,
+    gpre and the mask may each have a row pitch of their own."""
     dz, weight = as_tma(dz), as_tma(weight)
     dx = out if out is not None else empty_padded(dz.size(0), weight.size(1), dz.device)
     m = None if mask is None else as_tma(mask)
-    _C.linear_dgrad(dz, weight, m, dx, _prec(precision), int(k_splits), _act_code(activation), _drop_arg(dropout))
+    _C.linear_dgrad(dz, weight, m, dx, _prec(precision), int(k_splits), _act_code(activation), _drop_arg(dropout),
+                    bool(residual), skip, gpre)
     return dx
 
 

@@ -14,6 +14,9 @@ bound); tf32 0.97 for WGRAD and 0.93 for the fused update with one row, 0.96 for
 10-term dgrad.  These come near 1 by the bound's own derivation: with one product per element (or few non-zero ones,
 behind a ReLU) nothing averages out, and two operands truncated to 10 mantissa bits reach almost 2^-9 of the product.
 
+The residual form (``tc_gemm_res_kernel``) runs through ``ops.cuda``'s ``residual=`` / ``skip=`` / ``gpre=`` at every
+tile edge and split count, in fp32, tf32 and bf16, with a nil feature where the result is the skip up to one rounding.
+
 Every input's padding columns hold NaN and every output's padding a finite sentinel, so a kernel that reads or writes
 past the end of a row fails.  The CPU tests at the end check that the grid reaches every branch of the host planner,
 and that the oracles reject a set of plausible kernel faults while they accept the exact result and an fp32 one.
@@ -804,3 +807,247 @@ def test_oracles_reject_injected_faults():
     assert excess(v_nb[:, -1], V1[:, -1], bV[:, -1]) > 1.0
     assert excess(V0d, V1, bV) > 1.0                                                # V not written back
     assert excess(W0d - SGD_LR * (gp + MU * v), W1, bW) <= 1.0
+
+
+# ================================================================================================== the residual form
+# tc_gemm_res_kernel through ops.cuda's residual=True: FWD out = skip + f(z) * keep * s (every activation gated, ReLU's
+# gate 1[z > 0] * keep * s), DGRAD gpre = dz W + skip, out = gpre * mask (the mask: the previous layer's gate).  skip,
+# gpre and the mask each have a row pitch unlike out's.  bf16 through test_gpu_bf16's operand model.  The last feature
+# of every shape is nil (FWD: zero weight row and bias, so f(0) = 0; DGRAD: zero weight column), where the result is the
+# skip itself up to one rounding: a skip rounded or truncated like an operand fails there.
+RES_PRECISIONS = ["fp32", "tf32", "bf16"]
+RES_FWD_VARIANTS = [("relu", False)] + FWD_VARIANTS
+
+
+def _res_ops(precision, k, splits=1):
+    """(operand model, rtol) of a product of K = k in this precision (test_gpu_bf16 for bf16)."""
+    if precision == "bf16":
+        from test_gpu_bf16 import bf, rtol_bf16
+
+        return bf, rtol_bf16(k, splits)
+    return (lambda t: t.double().cpu()), rtol_for(precision, k, splits)
+
+
+def _res_fwd_inputs(tag, rows, m, k):
+    x, W, b = _fwd_inputs(tag, rows, m, k)
+    W[m - 1] = 0.0                                          # the nil output feature
+    b[m - 1] = 0.0
+    _, skip = _pitched(rows, m, _gen(tag, "skip", rows, m, k), extra=12)
+    assert skip.stride(0) != _out(1, m)[1].stride(0)
+    return x, W, b, skip
+
+
+def _check_res_fwd(kind, drop, skip, y, ybuf, gbuf, x, W, b, op, rtol, res, tag):
+    rows, m = y.shape
+    keep, s = _keep(rows, m) if drop else (None, 1.0)
+    (ra, ba), gam, z = act_fwd_oracle(kind, op(x), op(W), b.cpu(), keep, s, rtol)
+    sk = skip.cpu().double() if skip is not None else torch.zeros(rows, m, dtype=torch.float64)
+    ref = sk + ra
+    res[tag + "-out"] = excess(y, ref, ba * (1.0 + U) + U * ref.abs() + ATOL)
+    res[tag + "-skip"] = excess(y[:, m - 1], sk[:, m - 1], U * sk[:, m - 1].abs() + ATOL)
+    g = gbuf[:, :m].cpu()
+    if kind == "relu":
+        e = fwd_oracle(op(x), op(W), b.cpu(), False, rtol)[1]
+        want = (z > 0).double() * s * (1.0 if keep is None else keep.double())
+        sure = z.abs() > e
+        assert torch.equal(g.double()[sure], want[sure]), f"{tag}: a ReLU gate is not 1[z > 0] * keep * s"
+        assert bool(((g == 0) | (g == s)).all()), f"{tag}: a ReLU gate is neither 0 nor s"
+    else:
+        res[tag + "-gate"] = excess(g, *gam)
+    if keep is not None:
+        want = skip.cpu()[~keep] if skip is not None else torch.zeros(int((~keep).sum()))
+        assert torch.equal(y.cpu()[~keep].view(torch.int32), want.view(torch.int32)), f"{tag}: a dropped output is not the skip"
+        assert bool((g[~keep].view(torch.int32) == 0).all()), f"{tag}: a dropped gate is not +0"
+    assert bool((ybuf[:, m:] == SENTINEL).all()), f"{tag}: FWD wrote into the output's padding"
+    assert bool((gbuf[:, m:] == SENTINEL).all()), f"{tag}: FWD wrote into the gate's padding"
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("precision", RES_PRECISIONS)
+@pytest.mark.parametrize("rows,m,k", GRID)
+def test_fwd_residual_per_element(rows, m, k, precision):
+    """Every activation with and without dropout, with a skip and without one; without one the output equals the gated
+    non-residual launch's (a smooth kind) or the plain ReLU / dropout launch's."""
+    K = _K()
+    x, W, b, skip = _res_fwd_inputs("fwd-res", rows, m, k)
+    op, rtol = _res_ops(precision, k)
+    for kind, drop in RES_FWD_VARIANTS:
+        res = {}
+        for with_skip in (True, False):
+            ybuf, y = _out(rows, m)
+            gbuf, gate = _out(rows, m)
+            K.linear_fwd(x, W, b, relu=True, out=y, precision=precision, activation=kind, gate=gate,
+                         dropout=DROP if drop else None, residual=True, skip=skip if with_skip else None)
+            torch.cuda.synchronize()
+            tag = f"{_variant(kind, drop)}-skip{int(with_skip)}"
+            _check_res_fwd(kind, drop, skip if with_skip else None, y, ybuf, gbuf, x, W, b, op, rtol, res, tag)
+        pbuf, plain = _out(rows, m)
+        K.linear_fwd(x, W, b, relu=True, out=plain, precision=precision, activation=kind, dropout=DROP if drop else None,
+                     gate=_out(rows, m)[1] if kind != "relu" else None)
+        torch.cuda.synchronize()
+        assert torch.equal(y.cpu(), plain.cpu()), f"{_variant(kind, drop)}: skip=None differs from the plain launch"
+        _note((f"fwd-res-{_variant(kind, drop)}", precision), res, f"rows={rows} m={m} k={k}")
+
+
+def _check_res_dgrad(dz, W, mask, skip, gpre, dx, dxbuf, gpbuf, op, rtol, res, tag):
+    rows, m = dx.shape
+    prod = op(dz) @ op(W)
+    sk = skip.cpu().double() if skip is not None else torch.zeros_like(prod)
+    pre = prod + sk
+    pre_b = rtol * (op(dz).abs() @ op(W).abs()) + U * (prod.abs() + sk.abs()) + ATOL
+    mk = mask.cpu().double() if mask is not None else torch.ones_like(pre)
+    res[tag + "-out"] = excess(dx, pre * mk, pre_b * mk.abs() + U * (pre * mk).abs() + ATOL)
+    res[tag + "-skip"] = excess(dx[:, m - 1], (sk * mk)[:, m - 1], 2.0 * U * (sk * mk)[:, m - 1].abs() + ATOL)
+    if gpre is not None:
+        res[tag + "-gpre"] = excess(gpre, pre, pre_b)
+        g = gpre.cpu()
+        want = (g * mask.cpu()) if mask is not None else g
+        assert torch.equal(dx.cpu().view(torch.int32), want.view(torch.int32)), f"{tag}: out is not fp32(gpre * mask)"
+        assert bool((gpbuf[:, m:] == SENTINEL).all()), f"{tag}: DGRAD wrote into gpre's padding"
+    else:
+        assert bool((gpbuf == SENTINEL).all()), f"{tag}: DGRAD wrote a gpre it was not given"
+    assert bool((dxbuf[:, m:] == SENTINEL).all()), f"{tag}: DGRAD wrote into the output's padding"
+
+
+def _res_dgrad_inputs(tag, rows, m, k):
+    dz, W, (_, gate) = _dgrad_inputs(tag, rows, m, k)
+    W[:, m - 1] = 0.0                                       # the nil input feature
+    _, skip = _pitched(rows, m, _gen(tag, "skip", rows, m, k), scale=0.5, extra=12)
+    return dz, W, gate, skip
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("precision", RES_PRECISIONS)
+@pytest.mark.parametrize("rows,m,k", GRID)
+def test_dgrad_residual_per_element(rows, m, k, precision):
+    """Every combination of skip, gpre and mask present or null."""
+    K = _K()
+    dz, W, gate, skip = _res_dgrad_inputs("dgrad-res", rows, m, k)
+    op, rtol = _res_ops(precision, k)
+    res = {}
+    for has_skip in (True, False):
+        for has_gpre in (True, False):
+            for has_mask in (True, False):
+                dxbuf, dx = _out(rows, m)
+                gpbuf, gp = _out(rows, m, extra=16)
+                assert len({dx.stride(0), gp.stride(0), gate.stride(0), skip.stride(0)}) == 4
+                K.linear_dgrad(dz, W, mask=gate if has_mask else None, out=dx, precision=precision, residual=True,
+                               skip=skip if has_skip else None, gpre=gp if has_gpre else None)
+                torch.cuda.synchronize()
+                tag = f"skip{int(has_skip)}gpre{int(has_gpre)}mask{int(has_mask)}"
+                _check_res_dgrad(dz, W, gate if has_mask else None, skip if has_skip else None, gp if has_gpre else None,
+                                 dx, dxbuf, gpbuf, op, rtol, res, tag)
+    _note(("dgrad-res", precision), res, f"rows={rows} m={m} k={k}")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("precision", RES_PRECISIONS)
+@pytest.mark.parametrize("mode", ["fwd", "dgrad"])
+@pytest.mark.parametrize("rows,m,k,forced", SPLITK_CASES, ids=[f"rows{c[0]}-m{c[1]}-k{c[2]}" for c in SPLITK_CASES])
+def test_splitk_residual_per_element_and_deterministic(rows, m, k, forced, mode, precision):
+    """The split-K instantiations of the residual form at every forced split count and the planner's, per element, two
+    launches bit-identical.  FWD: ReLU and GELU with dropout in turn; DGRAD: skip, gpre and the mask."""
+    K = _K()
+    res = {}
+    for i, ks in enumerate(tuple(forced) + (-1,)):
+        op, rtol = _res_ops(precision, k, 8)
+        tag = f"ks{ks if ks >= 0 else 'auto'}"
+        outs = []
+        for _ in range(2):
+            if mode == "fwd":
+                x, W, b, skip = _res_fwd_inputs("splitk-res", rows, m, k)
+                kind, drop = (("relu", False), ("gelu", True))[i % 2]
+                ybuf, y = _out(rows, m)
+                gbuf, gate = _out(rows, m)
+                K.linear_fwd(x, W, b, relu=True, out=y, precision=precision, k_splits=ks, activation=kind, gate=gate,
+                             dropout=DROP if drop else None, residual=True, skip=skip)
+                torch.cuda.synchronize()
+                outs.append((_bits(ybuf), _bits(gbuf)))
+            else:
+                dz, W, gate, skip = _res_dgrad_inputs("splitk-res", rows, m, k)
+                dxbuf, dx = _out(rows, m)
+                gpbuf, gp = _out(rows, m, extra=16)
+                K.linear_dgrad(dz, W, mask=gate, out=dx, precision=precision, k_splits=ks, residual=True, skip=skip, gpre=gp)
+                torch.cuda.synchronize()
+                outs.append((_bits(dxbuf), _bits(gpbuf)))
+        if mode == "fwd":
+            _check_res_fwd(kind, drop, skip, y, ybuf, gbuf, x, W, b, op, rtol, res, f"{tag}-{_variant(kind, drop)}")
+        else:
+            _check_res_dgrad(dz, W, gate, skip, gp, dx, dxbuf, gpbuf, op, rtol, res, tag)
+        assert all(torch.equal(u, v) for u, v in zip(*outs)), f"{tag} is not deterministic"
+    _note((f"splitk-{mode}-res", precision), res, f"rows={rows} m={m} k={k}")
+
+
+@pytest.mark.gpu
+def test_residual_arguments_default_to_the_plain_launch_bit_for_bit():
+    """residual=False, skip=None and gpre=None are the launches of before: the same bits as the bindings called without
+    the residual arguments, on one shape per mode; and the bindings refuse residual arguments they cannot honour."""
+    from shallowspeed_b200 import _C
+
+    K = _K()
+    x, W, b, skip = _res_fwd_inputs("res-defaults", 65, 129, 100)
+    outs = []
+    for call in range(3):
+        ybuf, y = _out(65, 129)
+        gbuf, gate = _out(65, 129)
+        if call == 0:
+            K.linear_fwd(x, W, b, relu=True, out=y, activation="gelu", gate=gate, dropout=DROP)
+        elif call == 1:
+            K.linear_fwd(x, W, b, relu=True, out=y, activation="gelu", gate=gate, dropout=DROP, residual=False, skip=None)
+        else:
+            bias, bstride = K._bias_arg(b, 129)
+            _C.linear_fwd(x, W, bias, bstride, True, y, 1, 0, 1, gate, DROP)
+        torch.cuda.synchronize()
+        outs.append((_bits(ybuf), _bits(gbuf)))
+    assert all(torch.equal(u, v) for o in outs[1:] for u, v in zip(outs[0], o))
+    dz, Wd, gate, gskip = _res_dgrad_inputs("res-defaults", 65, 129, 100)
+    outs = []
+    for call in range(3):
+        dxbuf, dx = _out(65, 129)
+        if call == 0:
+            K.linear_dgrad(dz, Wd, mask=gate, out=dx, activation="gelu")
+        elif call == 1:
+            K.linear_dgrad(dz, Wd, mask=gate, out=dx, activation="gelu", residual=False, skip=None, gpre=None)
+        else:
+            _C.linear_dgrad(dz, Wd, gate, dx, 1, 0, 1, None)
+        torch.cuda.synchronize()
+        outs.append(_bits(dxbuf))
+    assert all(torch.equal(outs[0], o) for o in outs[1:])
+    _, y = _out(65, 129)
+    _, gp = _out(65, 129)
+    with pytest.raises(RuntimeError, match="needs residual"):
+        K.linear_fwd(x, W, b, relu=True, out=y, skip=skip)
+    with pytest.raises(RuntimeError, match="need residual"):
+        K.linear_dgrad(dz, Wd, mask=gate, out=dx, skip=gskip)
+    with pytest.raises(RuntimeError, match="need residual"):
+        K.linear_dgrad(dz, Wd, mask=gate, out=dx, gpre=gp)
+    with pytest.raises(RuntimeError, match="dropout"):
+        K.linear_dgrad(dz, Wd, mask=gate, out=dx, residual=True, dropout=DROP)
+    with pytest.raises(RuntimeError, match="skip shape"):
+        K.linear_fwd(x, W, b, relu=True, out=y, residual=True, skip=skip[:, :128])
+    with pytest.raises(RuntimeError, match="gpre shape"):
+        K.linear_dgrad(dz, Wd, mask=gate, out=dx, residual=True, gpre=gp[:64])
+    with pytest.raises(RuntimeError, match="row pitch"):
+        K.linear_fwd(x, W, b, relu=True, out=y, residual=True, gate=_out(65, 129, extra=8)[1])
+    with pytest.raises(RuntimeError, match="fp32"):
+        K.linear_fwd(x, W, b, relu=True, out=y, residual=True, skip=skip.double())
+    with pytest.raises(RuntimeError, match="only a smooth activation or a residual layer"):
+        K.linear_fwd(x, W, b, relu=True, out=y, gate=_out(65, 129)[1])
+
+
+def test_residual_oracles_reject_a_rounded_skip():
+    """At a nil feature the bound is one rounding of the skip: the exact skip passes, the skip rounded to bf16 or
+    truncated to tf32 (as a product's operand would be) fails, and so does a skip gradient added after the mask."""
+    from test_gpu_bf16 import bf
+    from test_gpu_chain import tf32_trunc
+
+    g = torch.Generator().manual_seed(4)
+    skip = torch.randn(64, 8, generator=g)
+    sk = skip.double()
+    bound = U * sk.abs() + ATOL
+    assert excess(skip, sk, bound) <= 1.0
+    assert excess(bf(skip), sk, bound) > 1.0
+    assert excess(tf32_trunc(skip), sk, bound) > 1.0
+    mk = torch.rand(64, 8, generator=g).double() + 0.5
+    assert excess((skip.double() * mk).float(), sk * mk, 2.0 * U * (sk * mk).abs() + ATOL) <= 1.0
+    assert excess(sk * 0.0 + sk, sk * mk, 2.0 * U * (sk * mk).abs() + ATOL) > 1.0

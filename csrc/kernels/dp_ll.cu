@@ -375,39 +375,45 @@ void dp_ll_free(DpLLPlan* plan) {
     plan->entries_dev = nullptr;
 }
 
+using DpLLKernel = void (*)(const DpLLEntry*, DpLLParams);
+
+template <int DP>
+static DpLLKernel dp_ll_kernel_of(SgdForm form) {
+    switch (form) {
+        case SGD_PLAIN: return dp_ll_wgrad_kernel<DP>;
+        case SGD_RULE: return dp_ll_wgrad_kernel<DP, true>;
+        case SGD_EMA: return dp_ll_wgrad_kernel<DP, true, true>;
+    }
+    return nullptr;
+}
+// the instantiation of a DP width (2, 4 or 8) and update form, nullptr for another width
+static DpLLKernel dp_ll_kernel(int dp, SgdForm form) {
+    switch (dp) {
+        case 2: return dp_ll_kernel_of<2>(form);
+        case 4: return dp_ll_kernel_of<4>(form);
+        case 8: return dp_ll_kernel_of<8>(form);
+    }
+    return nullptr;
+}
+
 cudaError_t dp_ll_configure() {
-    cudaError_t err;
-    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
-    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
-    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
-    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
-    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
-    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
-    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<2, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
-    if ((err = cudaFuncSetAttribute(dp_ll_wgrad_kernel<4, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024)) != cudaSuccess) return err;
-    return cudaFuncSetAttribute(dp_ll_wgrad_kernel<8, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+    static bool configured = false;
+    if (configured) return cudaSuccess;
+    for (int dp : {2, 4, 8})
+        for (SgdForm form : {SGD_PLAIN, SGD_RULE, SGD_EMA}) {
+            const cudaError_t e = cudaFuncSetAttribute(dp_ll_kernel(dp, form), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                       220 * 1024);
+            if (e != cudaSuccess) return e;
+        }
+    configured = true;
+    return cudaSuccess;
 }
 
 cudaError_t launch_dp_ll(const DpLLPlan& plan, cudaStream_t stream) {
-    const bool stateful = plan.p.opt.has_rule(), ema = plan.p.opt.E != nullptr;
-    switch (plan.p.dp) {
-        case 2:
-            if (ema) dp_ll_wgrad_kernel<2, true, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
-            else if (stateful) dp_ll_wgrad_kernel<2, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
-            else dp_ll_wgrad_kernel<2><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
-            break;
-        case 4:
-            if (ema) dp_ll_wgrad_kernel<4, true, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
-            else if (stateful) dp_ll_wgrad_kernel<4, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
-            else dp_ll_wgrad_kernel<4><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
-            break;
-        case 8:
-            if (ema) dp_ll_wgrad_kernel<8, true, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
-            else if (stateful) dp_ll_wgrad_kernel<8, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
-            else dp_ll_wgrad_kernel<8><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
-            break;
-        default: return cudaErrorInvalidValue;
-    }
+    if (cudaError_t e = dp_ll_configure(); e != cudaSuccess) return e;
+    DpLLKernel fn = dp_ll_kernel(plan.p.dp, plan.p.opt.form());
+    if (fn == nullptr) return cudaErrorInvalidValue;
+    fn<<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev, plan.p);
     return cudaGetLastError();
 }
 

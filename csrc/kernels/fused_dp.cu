@@ -497,8 +497,6 @@ const char* fused_dp_plan(FusedDpPlan* plan, const float* dZ, int lddz, const fl
     return nullptr;
 }
 
-static bool stateful(const DpLayerParams& p) { return p.opt.has_rule(); }
-
 int dp_element_owner(int proto, int in, int out, int ld, int64_t offset, int dp, int m, int n) {
     if (dp <= 1) return -1;
     switch (proto) {
@@ -515,32 +513,48 @@ int dp_element_owner(int proto, int in, int out, int ld, int64_t offset, int dp,
     }
 }
 
-cudaError_t fused_dp_configure() {
-    cudaError_t e = cudaFuncSetAttribute(fused_wgrad_dp_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(fused_wgrad_dp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(fused_wgrad_dp_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+using FusedDpKernel = void (*)(CUtensorMap, CUtensorMap, DpLayerParams, DpPeers);
+using ReduceSgdKernel = void (*)(DpLayerParams, DpPeers);
+
+static FusedDpKernel fused_dp_kernel(SgdForm form) {
+    switch (form) {
+        case SGD_PLAIN: return fused_wgrad_dp_kernel<false>;
+        case SGD_RULE: return fused_wgrad_dp_kernel<true>;
+        case SGD_EMA: return fused_wgrad_dp_kernel<true, true>;
+    }
+    return nullptr;
+}
+static ReduceSgdKernel reduce_sgd_kernel(SgdForm form) {
+    switch (form) {
+        case SGD_PLAIN: return dp_reduce_sgd_kernel<false>;
+        case SGD_RULE: return dp_reduce_sgd_kernel<true>;
+        case SGD_EMA: return dp_reduce_sgd_kernel<true, true>;
+    }
+    return nullptr;
+}
+
+cudaError_t fused_dp_configure() {      // dp_reduce_sgd_kernel uses no dynamic shared memory
+    static bool configured = false;
+    if (configured) return cudaSuccess;
+    for (SgdForm form : {SGD_PLAIN, SGD_RULE, SGD_EMA}) {
+        const cudaError_t e = cudaFuncSetAttribute(fused_dp_kernel(form), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   220 * 1024);
+        if (e != cudaSuccess) return e;
+    }
+    configured = true;
+    return cudaSuccess;
 }
 cudaError_t launch_fused_wgrad_dp(const FusedDpPlan& plan, cudaStream_t stream) {
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = fused_dp_configure();
-        if (e != cudaSuccess) return e;
-        configured = true;
-    }
-    if (plan.p.opt.E != nullptr)
-        fused_wgrad_dp_kernel<true, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.p, plan.peers);
-    else if (stateful(plan.p))
-        fused_wgrad_dp_kernel<true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.p, plan.peers);
-    else
-        fused_wgrad_dp_kernel<false><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.p, plan.peers);
+    if (cudaError_t e = fused_dp_configure(); e != cudaSuccess) return e;
+    FusedDpKernel fn = fused_dp_kernel(plan.p.opt.form());
+    if (fn == nullptr) return cudaErrorInvalidValue;
+    fn<<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.p, plan.peers);
     return cudaGetLastError();
 }
 cudaError_t launch_dp_reduce_sgd(const FusedDpPlan& plan, cudaStream_t stream) {
-    if (plan.p.opt.E != nullptr) dp_reduce_sgd_kernel<true, true><<<plan.grid, 128, 0, stream>>>(plan.p, plan.peers);
-    else if (stateful(plan.p)) dp_reduce_sgd_kernel<true><<<plan.grid, 128, 0, stream>>>(plan.p, plan.peers);
-    else dp_reduce_sgd_kernel<false><<<plan.grid, 128, 0, stream>>>(plan.p, plan.peers);
+    ReduceSgdKernel fn = reduce_sgd_kernel(plan.p.opt.form());
+    if (fn == nullptr) return cudaErrorInvalidValue;
+    fn<<<plan.grid, 128, 0, stream>>>(plan.p, plan.peers);
     return cudaGetLastError();
 }
 cudaError_t launch_bump_epoch(uint32_t* epoch, cudaStream_t stream) {

@@ -19,6 +19,14 @@ enum GemmMode : int { GEMM_FWD = 0, GEMM_DGRAD = 1, GEMM_WGRAD = 2 };
 // the MSE loss.  CROSS_ENTROPY: softmax cross-entropy with probability targets, per-row softmax (ptx.cuh: ce_*).
 enum LossKind : int { LOSS_MSE = 0, LOSS_CROSS_ENTROPY = 1 };
 
+// The form of an SGD update, which selects the instantiation of every native update kernel: PLAIN w -= lr * g (the
+// stateless kernels), RULE with momentum or weight decay, EMA with an EMA of the weights (whatever the rule).
+enum SgdForm : int { SGD_PLAIN = 0, SGD_RULE = 1, SGD_EMA = 2 };
+inline SgdForm sgd_form(float momentum, float weight_decay, const float* E) {
+    if (E != nullptr) return SGD_EMA;
+    return momentum != 0.f || weight_decay != 0.f ? SGD_RULE : SGD_PLAIN;
+}
+
 // Hyper-parameters of the SGD update beyond lr (torch.optim.SGD, dampening 0).  The default is plain SGD, w -= lr * g,
 // which runs the stateless kernels.  V: momentum buffer laid out like the weights it belongs to (nullptr when
 // momentum == 0: weight decay alone needs no state).
@@ -32,7 +40,7 @@ struct SgdState {
     int nesterov = 0;
     float* E = nullptr;
     const float* ema_alpha = nullptr;
-    bool plain() const { return momentum == 0.f && weight_decay == 0.f && E == nullptr; }
+    SgdForm form() const { return sgd_form(momentum, weight_decay, E); }
     __host__ __device__ bool has_rule() const { return momentum != 0.f || weight_decay != 0.f; }   // the update direction is not the gradient
 };
 // nullptr if the combination is valid: 0 <= momentum < 1, weight_decay >= 0, nesterov only with momentum, a buffer
@@ -95,8 +103,9 @@ struct GemmParams {
     // DGRAD with mask reads the mask as the previous layer's gate and multiplies by it.  Last, like drop.
     int act_kind;
     float* gate;
-    // Residual form (tc_gemm_res_kernel), set by a plan with identity skips.  res: the FWD with relu / DGRAD with mask runs
-    // gated for every act_kind, ReLU included (its gate is 1[z > 0] * keep * s), and the skip fields apply (both nullable):
+    // Residual form (the GEMM's RES switch), set by a plan with identity skips.  res: the FWD with relu / DGRAD with mask
+    // runs gated for every act_kind, ReLU included (its gate is 1[z > 0] * keep * s), and the skip fields apply (both
+    // nullable):
     //   FWD:   out = skip[n * ldskip + m] + f(z)          (skip: the layer's input X)
     //   DGRAD: x = W^T dZ + skip[n * ldskip + m]          (skip: the gradient of the layer's output)
     //          gpre[n * ldgpre + m] = x, then out = x * mask   (gpre: the previous layer is residual and needs x as ITS skip)
@@ -107,7 +116,7 @@ struct GemmParams {
     float* gpre;
     int ldgpre;
     // WGRAD with fuse_sgd: the EMA of the weights (SgdState::E, pitch ldw) and its device alpha.  E set runs the STATEFUL
-    // epilogue with EMA (tc_gemm_ema_kernel), whatever the rule.  Last, like drop.
+    // epilogue with EMA (SGD_EMA), whatever the rule.  Last, like drop.
     float* E;
     const float* ema_alpha;
 };
@@ -145,7 +154,7 @@ cudaError_t gemm_launch(const GemmPlan& plan, cudaStream_t stream);
 bool gemm_drops(const GemmPlan& plan);
 // the plan runs the gated variant: a FWD with relu or a DGRAD with mask, and a smooth plan.p.act_kind (or the residual form)
 bool gemm_gated(const GemmPlan& plan);
-// the plan runs the residual form (GemmParams::res): tc_gemm_res_kernel
+// the plan runs the residual form (GemmParams::res)
 bool gemm_residual(const GemmPlan& plan);
 // the plan adds an identity skip (GemmParams::skip) or stores the pre-gate gradient (GemmParams::gpre)
 bool gemm_skips(const GemmPlan& plan);
@@ -167,13 +176,13 @@ const char* gemm_group_tiles(int out, int in, int rows, std::vector<GemmGroupTil
 struct GemmGroupPlan {
     GemmGroupEntry* entries_dev;
     int n, smem_bytes, n_gemms;
-    int stateful;                  // the plans use the stateful SGD rule (all of them or none)
-    int ema;                       // the plans update an EMA of the weights (all of them or none; implies stateful)
+    SgdForm form;                  // the form of every plan's fused update (SGD_PLAIN without fuse_sgd)
 };
 const char* gemm_group_plan(GemmGroupPlan* out, const GemmPlan* plans, int n_plans);
 cudaError_t gemm_group_launch(const GemmGroupPlan& plan, cudaStream_t stream);
 void gemm_group_free(GemmGroupPlan* plan);
-cudaError_t gemm_configure();   // opt every instantiation into > 48 KB dynamic smem (call outside graph capture)
+// opt every instantiation into > 48 KB dynamic smem; idempotent, called by the launches (call it outside graph capture)
+cudaError_t gemm_configure();
 int gemm_kernel_count();   // number of launches issued so far by this module (bench accounting)
 
 // ---- fused data-parallel path (csrc/kernels/fused_dp.cu) ---------------------------------

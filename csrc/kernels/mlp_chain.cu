@@ -1,5 +1,5 @@
-// Host side of the layer-chain kernel (mlp_chain.cuh): plans, shared-memory budgets, and the TF32 / 3xTF32 launches; the
-// BF16 launches are in mlp_chain_bf16.cu.
+// Host side of the layer-chain kernel (mlp_chain.cuh): plans, shared-memory budgets, and the launches, with the TF32 /
+// 3xTF32 instantiations; the BF16 ones are in mlp_chain_bf16.cu, the residual ones in mlp_chain_res.cu.
 #include "mlp_chain.cuh"
 
 namespace ssb {
@@ -151,25 +151,61 @@ void chain_plan_free(ChainPlan* plan) {
     plan->maps_dev = nullptr;
 }
 
-cudaError_t chain_configure() {
-    cudaError_t e;
-    if ((e = chain_configure_prec<PREC_TF32>()) != cudaSuccess) return e;
-    if ((e = chain_configure_prec<PREC_3XTF32>()) != cudaSuccess) return e;
-    return chain_configure_bf16();
+// the instantiation of a (precision, residual) pair, from the translation unit that compiles it
+static ChainKernel chain_kernel_of(int prec, bool res, ChainForm form, int ntw, bool ce, bool drop, bool gate) {
+    if (res) return chain_kernel_res(prec, form, ntw, ce, drop, gate);
+    switch (prec) {
+        case PREC_TF32: return chain_kernel<PREC_TF32, false>(form, ntw, ce, drop, gate);
+        case PREC_3XTF32: return chain_kernel<PREC_3XTF32, false>(form, ntw, ce, drop, gate);
+        case PREC_BF16: return chain_kernel_bf16(form, ntw, ce, drop, gate);
+    }
+    return nullptr;
 }
 
+cudaError_t chain_configure() {
+    static bool configured = false;
+    if (configured) return cudaSuccess;
+    for (int prec : {PREC_TF32, PREC_3XTF32, PREC_BF16})
+        for (ChainForm form : {CHAIN_PLAIN, CHAIN_FOLD, CHAIN_CLUSTER})
+            for (int ntw : {2, 4, 8})
+                for (int key = 0; key < 16; ++key)     // residual, cross-entropy, dropout, gated
+                    if (ChainKernel fn = chain_kernel_of(prec, key & 1, form, ntw, key & 2, key & 4, key & 8)) {
+                        cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+                        if (e != cudaSuccess) return e;
+                    }
+    configured = true;
+    return cudaSuccess;
+}
+
+// grid = micro-batches x plan.cluster x plan.ksplit; cluster dims (plan.cluster x plan.ksplit, 1, 1) for a cluster plan
 cudaError_t chain_launch(const ChainPlan& plan, cudaStream_t stream) {
     const ChainParams& p = plan.p;
-    const bool fold = p.in_flag != nullptr || p.out_peer != nullptr || p.x_from_global != 0;
-    const int ntw = chain_ntw(p.n_pad);
     if (p.loss_kind != LOSS_MSE && p.loss_kind != LOSS_CROSS_ENTROPY) return cudaErrorInvalidValue;
     if (!act_valid(p.act_kind)) return cudaErrorInvalidValue;
-    cudaError_t e;
-    if (p.prec == PREC_TF32) e = chain_launch_prec<PREC_TF32>(plan, ntw, fold, stream);
-    else if (p.prec == PREC_3XTF32) e = chain_launch_prec<PREC_3XTF32>(plan, ntw, fold, stream);
-    else if (p.prec == PREC_BF16) e = chain_launch_bf16(plan, ntw, fold, stream);
-    else return cudaErrorInvalidValue;
-    if (e != cudaSuccess) return e;
+    if (cudaError_t e = chain_configure(); e != cudaSuccess) return e;
+    const bool fold = p.in_flag != nullptr || p.out_peer != nullptr || p.x_from_global != 0;
+    const ChainForm form = plan.cluster > 1 ? CHAIN_CLUSTER : fold ? CHAIN_FOLD : CHAIN_PLAIN;
+    // a residual model is gated for every activation kind
+    ChainKernel fn = chain_kernel_of(p.prec, p.res != 0, form, chain_ntw(p.n_pad), p.loss_kind == LOSS_CROSS_ENTROPY,
+                                     p.drop.on(), p.res != 0 || act_smooth(p.act_kind));
+    if (fn == nullptr) return cudaErrorInvalidValue;
+    if (form == CHAIN_CLUSTER) {
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned)plan.grid);
+        cfg.blockDim = dim3(kThreads);
+        cfg.dynamicSmemBytes = (size_t)plan.smem_bytes;
+        cfg.stream = stream;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = (unsigned)(plan.cluster * plan.ksplit);
+        attr[0].val.clusterDim.y = 1;
+        attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+        if (cudaError_t e = cudaLaunchKernelEx(&cfg, fn, p); e != cudaSuccess) return e;
+    } else {
+        fn<<<plan.grid, kThreads, plan.smem_bytes, stream>>>(p);
+    }
     return cudaGetLastError();
 }
 

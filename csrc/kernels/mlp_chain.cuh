@@ -1046,92 +1046,56 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
 }
 
 
-// =========================================================================== host side: the launches of one precision
-// Every translation unit that includes this file instantiates the kernel for the precisions it dispatches:
-// mlp_chain.cu PREC_TF32 and PREC_3XTF32, mlp_chain_bf16.cu PREC_BF16, mlp_chain_res.cu the RES forms of all three, so
-// that none grows the longest compile.
+// =========================================================================== host side: the instantiations
+// Every translation unit that includes this file instantiates the kernel for the precisions it selects: mlp_chain.cu
+// PREC_TF32 and PREC_3XTF32, mlp_chain_bf16.cu PREC_BF16, mlp_chain_res.cu the RES forms of all three, so that none
+// grows the longest compile.
 
-// mlp_chain_res.cu: configuration and launch of the RES instantiations of one precision
-cudaError_t chain_configure_res(int prec);
-cudaError_t chain_launch_res(const ChainPlan& plan, int ntw, bool fold, cudaStream_t stream);
-template <int PREC, int NTW, bool CE, bool DROP, bool GATE, bool RES = false>
-static cudaError_t chain_configure_ntw() {
-    cudaError_t e;
-    const int smem = 227 * 1024;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<PREC, false, NTW, false, CE, DROP, GATE, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(mlp_chain_kernel<PREC, true, NTW, false, CE, DROP, GATE, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e;
-    return cudaFuncSetAttribute(mlp_chain_kernel<PREC, false, NTW, true, CE, DROP, GATE, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-}
-
-template <int PREC, bool DROP, bool GATE, bool RES = false>
-static cudaError_t chain_configure_kind() {
-    cudaError_t e;
-    if ((e = chain_configure_ntw<PREC, 2, false, DROP, GATE, RES>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<PREC, 4, false, DROP, GATE, RES>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<PREC, 8, false, DROP, GATE, RES>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<PREC, 2, true, DROP, GATE, RES>()) != cudaSuccess) return e;
-    if ((e = chain_configure_ntw<PREC, 4, true, DROP, GATE, RES>()) != cudaSuccess) return e;
-    return chain_configure_ntw<PREC, 8, true, DROP, GATE, RES>();
-}
-
-template <int PREC>
-static cudaError_t chain_configure_prec() {
-    cudaError_t e;
-    if ((e = chain_configure_kind<PREC, false, false>()) != cudaSuccess) return e;
-    if ((e = chain_configure_kind<PREC, true, false>()) != cudaSuccess) return e;
-    if ((e = chain_configure_kind<PREC, false, true>()) != cudaSuccess) return e;
-    if ((e = chain_configure_kind<PREC, true, true>()) != cudaSuccess) return e;
-    return chain_configure_res(PREC);
-}
-
-// grid = micro-batches x plan.cluster x plan.ksplit, cluster dims (plan.cluster x plan.ksplit, 1, 1)
-template <int PREC, int NTW, bool CE, bool DROP, bool GATE, bool RES>
-static cudaError_t chain_launch_cluster(const ChainPlan& plan, cudaStream_t stream) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)plan.grid);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = (size_t)plan.smem_bytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)(plan.cluster * plan.ksplit);
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, mlp_chain_kernel<PREC, false, NTW, true, CE, DROP, GATE, RES>, plan.p);
-}
+using ChainKernel = void (*)(ChainParams);
+// the launch form of a plan: one CTA per micro-batch, with folded pipeline boundaries (FOLD), or a cluster (CLUSTER)
+enum ChainForm : int { CHAIN_PLAIN = 0, CHAIN_FOLD = 1, CHAIN_CLUSTER = 2 };
 
 template <int PREC, int NTW, bool CE, bool DROP, bool GATE, bool RES>
-static cudaError_t chain_launch_ntw(const ChainPlan& plan, bool fold, cudaStream_t stream) {
-    if (plan.cluster > 1) return chain_launch_cluster<PREC, NTW, CE, DROP, GATE, RES>(plan, stream);
-    if (fold)
-        mlp_chain_kernel<PREC, true, NTW, false, CE, DROP, GATE, RES><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.p);
-    else
-        mlp_chain_kernel<PREC, false, NTW, false, CE, DROP, GATE, RES><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.p);
-    return cudaSuccess;
+static ChainKernel chain_kernel_form(ChainForm form) {
+    switch (form) {
+        case CHAIN_PLAIN: return mlp_chain_kernel<PREC, false, NTW, false, CE, DROP, GATE, RES>;
+        case CHAIN_FOLD: return mlp_chain_kernel<PREC, true, NTW, false, CE, DROP, GATE, RES>;
+        case CHAIN_CLUSTER: return mlp_chain_kernel<PREC, false, NTW, true, CE, DROP, GATE, RES>;
+    }
+    return nullptr;
 }
 
-template <int PREC, bool DROP, bool GATE, bool RES = false>
-static cudaError_t chain_launch_kind(const ChainPlan& plan, int ntw, bool ce, bool fold, cudaStream_t stream) {
-    if (ntw == 2) return ce ? chain_launch_ntw<PREC, 2, true, DROP, GATE, RES>(plan, fold, stream) : chain_launch_ntw<PREC, 2, false, DROP, GATE, RES>(plan, fold, stream);
-    if (ntw == 4) return ce ? chain_launch_ntw<PREC, 4, true, DROP, GATE, RES>(plan, fold, stream) : chain_launch_ntw<PREC, 4, false, DROP, GATE, RES>(plan, fold, stream);
-    return ce ? chain_launch_ntw<PREC, 8, true, DROP, GATE, RES>(plan, fold, stream) : chain_launch_ntw<PREC, 8, false, DROP, GATE, RES>(plan, fold, stream);
+template <int PREC, int NTW, bool DROP, bool GATE, bool RES>
+static ChainKernel chain_kernel_ce(ChainForm form, bool ce) {
+    return ce ? chain_kernel_form<PREC, NTW, true, DROP, GATE, RES>(form) : chain_kernel_form<PREC, NTW, false, DROP, GATE, RES>(form);
 }
 
-// the launch of a validated plan (chain_launch checks the loss and activation kinds); ntw: chain_ntw(p.n_pad)
-template <int PREC>
-static cudaError_t chain_launch_prec(const ChainPlan& plan, int ntw, bool fold, cudaStream_t stream) {
-    const ChainParams& p = plan.p;
-    const bool ce = p.loss_kind == LOSS_CROSS_ENTROPY, drop = p.drop.on();
-    if (p.res) return chain_launch_res(plan, ntw, fold, stream);   // a residual model: gated for every activation kind
-    if (!act_smooth(p.act_kind))
-        return drop ? chain_launch_kind<PREC, true, false>(plan, ntw, ce, fold, stream) : chain_launch_kind<PREC, false, false>(plan, ntw, ce, fold, stream);
-    return drop ? chain_launch_kind<PREC, true, true>(plan, ntw, ce, fold, stream) : chain_launch_kind<PREC, false, true>(plan, ntw, ce, fold, stream);
+template <int PREC, bool DROP, bool GATE, bool RES>
+static ChainKernel chain_kernel_ntw(ChainForm form, int ntw, bool ce) {
+    switch (ntw) {
+        case 2: return chain_kernel_ce<PREC, 2, DROP, GATE, RES>(form, ce);
+        case 4: return chain_kernel_ce<PREC, 4, DROP, GATE, RES>(form, ce);
+        case 8: return chain_kernel_ce<PREC, 8, DROP, GATE, RES>(form, ce);
+    }
+    return nullptr;
 }
 
-// mlp_chain_bf16.cu: chain_configure_prec / chain_launch_prec of PREC_BF16
-cudaError_t chain_configure_bf16();
-cudaError_t chain_launch_bf16(const ChainPlan& plan, int ntw, bool fold, cudaStream_t stream);
+template <int PREC, bool GATE, bool RES>
+static ChainKernel chain_kernel_drop(ChainForm form, int ntw, bool ce, bool drop) {
+    return drop ? chain_kernel_ntw<PREC, true, GATE, RES>(form, ntw, ce) : chain_kernel_ntw<PREC, false, GATE, RES>(form, ntw, ce);
+}
+
+// The instantiation of precision PREC, residual or not, that runs (form, ntw, ce, drop, gate); nullptr for a combination
+// without one (a residual model runs gated).
+template <int PREC, bool RES>
+static ChainKernel chain_kernel(ChainForm form, int ntw, bool ce, bool drop, bool gate) {
+    if constexpr (RES) return gate ? chain_kernel_drop<PREC, true, true>(form, ntw, ce, drop) : nullptr;
+    else if (gate) return chain_kernel_drop<PREC, true, false>(form, ntw, ce, drop);
+    else return chain_kernel_drop<PREC, false, false>(form, ntw, ce, drop);
+}
+
+// mlp_chain_bf16.cu: chain_kernel<PREC_BF16, false>; mlp_chain_res.cu: chain_kernel<prec, true>
+ChainKernel chain_kernel_bf16(ChainForm form, int ntw, bool ce, bool drop, bool gate);
+ChainKernel chain_kernel_res(int prec, ChainForm form, int ntw, bool ce, bool drop, bool gate);
 
 }  // namespace ssb

@@ -5,10 +5,8 @@
 
 namespace ssb {
 
-cudaError_t chain_configure_bf16() { return chain_configure_prec<PREC_BF16>(); }
-
-cudaError_t chain_launch_bf16(const ChainPlan& plan, int ntw, bool fold, cudaStream_t stream) {
-    return chain_launch_prec<PREC_BF16>(plan, ntw, fold, stream);
+ChainKernel chain_kernel_bf16(ChainForm form, int ntw, bool ce, bool drop, bool gate) {
+    return chain_kernel<PREC_BF16, false>(form, ntw, ce, drop, gate);
 }
 
 }  // namespace ssb

@@ -5,32 +5,13 @@
 
 namespace ssb {
 
-template <int PREC>
-static cudaError_t configure_res() {
-    cudaError_t e;
-    if ((e = chain_configure_kind<PREC, false, true, true>()) != cudaSuccess) return e;
-    return chain_configure_kind<PREC, true, true, true>();
-}
-
-template <int PREC>
-static cudaError_t launch_res(const ChainPlan& plan, int ntw, bool fold, cudaStream_t stream) {
-    const bool ce = plan.p.loss_kind == LOSS_CROSS_ENTROPY;
-    if (plan.p.drop.on()) return chain_launch_kind<PREC, true, true, true>(plan, ntw, ce, fold, stream);
-    return chain_launch_kind<PREC, false, true, true>(plan, ntw, ce, fold, stream);
-}
-
-cudaError_t chain_configure_res(int prec) {
-    if (prec == PREC_TF32) return configure_res<PREC_TF32>();
-    if (prec == PREC_3XTF32) return configure_res<PREC_3XTF32>();
-    if (prec == PREC_BF16) return configure_res<PREC_BF16>();
-    return cudaErrorInvalidValue;
-}
-
-cudaError_t chain_launch_res(const ChainPlan& plan, int ntw, bool fold, cudaStream_t stream) {
-    if (plan.p.prec == PREC_TF32) return launch_res<PREC_TF32>(plan, ntw, fold, stream);
-    if (plan.p.prec == PREC_3XTF32) return launch_res<PREC_3XTF32>(plan, ntw, fold, stream);
-    if (plan.p.prec == PREC_BF16) return launch_res<PREC_BF16>(plan, ntw, fold, stream);
-    return cudaErrorInvalidValue;
+ChainKernel chain_kernel_res(int prec, ChainForm form, int ntw, bool ce, bool drop, bool gate) {
+    switch (prec) {
+        case PREC_TF32: return chain_kernel<PREC_TF32, true>(form, ntw, ce, drop, gate);
+        case PREC_3XTF32: return chain_kernel<PREC_3XTF32, true>(form, ntw, ce, drop, gate);
+        case PREC_BF16: return chain_kernel<PREC_BF16, true>(form, ntw, ce, drop, gate);
+    }
+    return nullptr;
 }
 
 }  // namespace ssb

@@ -118,14 +118,21 @@ static int nvls_grid(const NvlsParams& p, int max_ctas) {
     return (int)ctas;
 }
 
+using NvlsKernel = void (*)(NvlsParams);
+
+static NvlsKernel reduce_sgd_kernel(SgdForm form) {
+    switch (form) {
+        case SGD_PLAIN: return nvls_reduce_kernel<true>;
+        case SGD_RULE: return nvls_reduce_kernel<true, true>;
+        case SGD_EMA: return nvls_reduce_kernel<true, true, true>;
+    }
+    return nullptr;
+}
+
 cudaError_t launch_nvls_reduce_sgd(const NvlsParams& p, int max_ctas, cudaStream_t stream) {
-    if (p.lr == nullptr) return cudaErrorInvalidValue;
-    if (p.opt.E != nullptr)
-        nvls_reduce_kernel<true, true, true><<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
-    else if (p.opt.has_rule())
-        nvls_reduce_kernel<true, true><<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
-    else
-        nvls_reduce_kernel<true><<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
+    NvlsKernel fn = reduce_sgd_kernel(p.opt.form());
+    if (p.lr == nullptr || fn == nullptr) return cudaErrorInvalidValue;
+    fn<<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
     return cudaGetLastError();
 }
 

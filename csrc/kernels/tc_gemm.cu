@@ -41,7 +41,7 @@ static constexpr int kGroupMinCtas = 3;                 // CTAs per SM the group
 // k-blocks; every CTA writes its raw fp32 accumulator tile to a workspace and the LAST CTA to arrive at the
 // tile's counter sums the partials in split order (deterministic) and runs the fused epilogue.  Nobody
 // waits for anybody, so the CTAs of a tile need not be co-resident.
-// The body is shared by the one-GEMM-per-launch kernels below and by the grouped weight-gradient kernel (several
+// The body is shared by the one-GEMM-per-launch kernel below and by the grouped weight-gradient kernel (several
 // layers' tiles in ONE launch, tensor maps and parameters read from a device table).
 // STATEFUL (WGRAD with fuse_sgd only): the SGD update uses momentum / weight decay (GemmParams::V, ...); the false
 // instantiations are the plain w -= lr * dW code.
@@ -525,36 +525,15 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
     }
 }
 
-template <int MODE, bool SPLITK = false, bool STATEFUL = false>
+// The per-layer kernel: one instantiation per combination of switches gemm_kernel selects.  blockIdx.z is the split
+// index, which the body reads only under SPLITK.
+template <int MODE, bool SPLITK = false, bool STATEFUL = false, bool DROP = false, bool GATE = false, bool RES = false,
+          bool EMA = false>
 __global__ void __launch_bounds__(kThreads, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
-    tc_gemm_body<MODE, SPLITK, STATEFUL>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z);
-}
-// FWD / DGRAD under dropout (a kernel of its own, so that the names and code of the dropout-free ones stay as they are)
-template <int MODE, bool SPLITK>
-__global__ void __launch_bounds__(kThreads, 1)
-tc_gemm_drop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
-    tc_gemm_body<MODE, SPLITK, false, (int)kBlockM, true>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z);
-}
-// FWD / DGRAD of a smooth activation, with or without dropout in the FWD (a kernel of its own, like tc_gemm_drop_kernel)
-template <int MODE, bool SPLITK, bool DROP>
-__global__ void __launch_bounds__(kThreads, 1)
-tc_gemm_gate_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
-    tc_gemm_body<MODE, SPLITK, false, (int)kBlockM, DROP, true>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y,
-                                                                (int)blockIdx.z);
-}
-
-// FWD / DGRAD of a residual plan (GemmParams::res), with or without dropout in the FWD (a kernel of its own, like
-// tc_gemm_gate_kernel)
-template <int MODE, bool SPLITK, bool DROP>
-__global__ void __launch_bounds__(kThreads, 1)
-tc_gemm_res_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                   const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
-    tc_gemm_body<MODE, SPLITK, false, (int)kBlockM, DROP, true, true>(tmA, tmB, tmC, p, (int)blockIdx.x, (int)blockIdx.y,
-                                                                      (int)blockIdx.z);
+    tc_gemm_body<MODE, SPLITK, STATEFUL, (int)kBlockM, DROP, GATE, RES, EMA>(tmA, tmB, tmC, p, (int)blockIdx.x,
+                                                                            (int)blockIdx.y, (int)blockIdx.z);
 }
 
 // ---- grouped weight-gradient launch: the tiles of SEVERAL layers' WGRAD GEMMs in one grid (one table entry per CTA).
@@ -562,25 +541,12 @@ tc_gemm_res_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 // step of a narrow stage is chain kernel -> grouped wgrad (+SGD) (or chain || LL kernel under DP).  The GEMMs of a narrow
 // stage have few k-blocks and at most 128 outputs, so the launch runs on narrow [32 x 32] tiles (gemm_group_tiles): several
 // small CTAs per SM, each warp with an eighth of the per-layer kernel's MMAs.
-template <bool STATEFUL = false>
+template <bool STATEFUL = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads, kGroupMinCtas) tc_wgrad_group_kernel(const GemmGroupEntry* __restrict__ entries) {
     const GemmGroupEntry& e = entries[blockIdx.x];
     const GemmParams p = e.p;                      // private copy: the body reads these fields in every loop
-    tc_gemm_body<GEMM_WGRAD, false, STATEFUL, kGroupBM>(e.tmA, e.tmB, e.tmC, p, e.bx, e.by, 0);
-}
-
-// The fused update with an EMA of the weights (GemmParams::E): the per-layer and the grouped launch, kernels of their own
-// like tc_gemm_drop_kernel
-__global__ void __launch_bounds__(kThreads, 1)
-tc_gemm_ema_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                   const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
-    tc_gemm_body<GEMM_WGRAD, false, true, (int)kBlockM, false, false, false, true>(tmA, tmB, tmC, p, (int)blockIdx.x,
-                                                                                  (int)blockIdx.y, 0);
-}
-__global__ void __launch_bounds__(kThreads, kGroupMinCtas) tc_wgrad_group_ema_kernel(const GemmGroupEntry* __restrict__ entries) {
-    const GemmGroupEntry& e = entries[blockIdx.x];
-    const GemmParams p = e.p;
-    tc_gemm_body<GEMM_WGRAD, false, true, kGroupBM, false, false, false, true>(e.tmA, e.tmB, e.tmC, p, e.bx, e.by, 0);
+    tc_gemm_body<GEMM_WGRAD, false, STATEFUL, kGroupBM, false, false, false, EMA>(e.tmA, e.tmB, e.tmC, p, e.bx, e.by,
+                                                                                0);
 }
 
 // =========================================================================== host side
@@ -631,8 +597,10 @@ const char* make_tmap_k(CUtensorMap* map, const float* base, int inner, int oute
 
 static int round_up_i(int x, int m) { return (x + m - 1) / m * m; }
 
-static bool is_stateful(const GemmParams& p) { return p.fuse_sgd && (p.momentum != 0.f || p.weight_decay != 0.f || p.E != nullptr); }
-static bool has_ema(const GemmParams& p) { return p.fuse_sgd && p.E != nullptr; }
+// the form of a plan's fused update: SGD_PLAIN without one
+static SgdForm update_form(const GemmParams& p) {
+    return p.fuse_sgd ? sgd_form(p.momentum, p.weight_decay, p.E) : SGD_PLAIN;
+}
 
 const char* sgd_state_check(const SgdState& s) {
     if (!(s.momentum >= 0.f && s.momentum < 1.f)) return "momentum must be in [0, 1)";
@@ -708,7 +676,7 @@ const char* gemm_plan_wgrad(GemmPlan* plan, const float* dZ, int lddz, const flo
     // the fused update finds the bias at db's offset from G, taken in W (and V): only the arena layout's bias column
     // (column `in` of G's block) names a slot of W
     if (fuse_sgd && db != nullptr && db != G + in) return "fuse_sgd needs db to be G's bias column (G + in)";
-    if (!opt.plain()) {
+    if (opt.form() != SGD_PLAIN) {
         if (!fuse_sgd) return "momentum / weight decay / an EMA need fuse_sgd (the update rule runs in the epilogue)";
         if (const char* e = sgd_state_check(opt)) return e;
         p.V = opt.V; p.momentum = opt.momentum; p.weight_decay = opt.weight_decay; p.nesterov = opt.nesterov;
@@ -784,13 +752,12 @@ const char* gemm_group_plan(GemmGroupPlan* out, const GemmPlan* plans, int n_pla
     if (n_plans < 1) return "gemm_group_plan: no plans";
     std::vector<GemmGroupEntry> host;
     int smem = 0;
-    const bool stateful = is_stateful(plans[0].p), ema = has_ema(plans[0].p);
+    const SgdForm form = update_form(plans[0].p);
     for (int i = 0; i < n_plans; ++i) {
         const GemmPlan& g = plans[i];
         if (g.mode != GEMM_WGRAD) return "gemm_group_plan: only weight-gradient GEMMs can be grouped";
         if (g.p.k_splits > 1) return "gemm_group_plan: split-K plans cannot be grouped";
-        if (is_stateful(g.p) != stateful) return "gemm_group_plan: plans mix the plain and the stateful SGD rule";
-        if (has_ema(g.p) != ema) return "gemm_group_plan: plans mix updates with and without an EMA";
+        if (update_form(g.p) != form) return "gemm_group_plan: plans mix update forms (plain, rule, EMA)";
         std::vector<GemmGroupTile> tiles;
         int stages = 0, bytes = 0;
         if (const char* e = gemm_group_tiles(g.p.m_total, g.p.n_total, g.p.k_total, &tiles, &stages, &bytes)) return e;
@@ -815,8 +782,7 @@ const char* gemm_group_plan(GemmGroupPlan* out, const GemmPlan* plans, int n_pla
         return "gemm_group_plan: table upload failed";
     }
     out->entries_dev = dev; out->n = (int)host.size(); out->smem_bytes = smem; out->n_gemms = n_plans;
-    out->stateful = stateful ? 1 : 0;
-    out->ema = ema ? 1 : 0;
+    out->form = form;
     return nullptr;
 }
 
@@ -828,116 +794,85 @@ void gemm_group_free(GemmGroupPlan* plan) {
 static std::atomic<int> g_launches{0};
 int gemm_kernel_count() { return g_launches.load(); }
 
-static constexpr int kMaxDynSmem = 220 * 1024;
+using GemmKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, GemmParams);
+using GroupKernel = void (*)(const GemmGroupEntry*);
+
+// The FWD / DGRAD instantiation of one mode and split-K switch: the residual form (always gated), the gated form, or the
+// ReLU form, each with or without dropout.  A DGRAD drops only in the ReLU form: a gate already holds the dropout scale.
+template <int MODE, bool SK>
+static GemmKernel epilogue_kernel(bool drop, bool gate, bool res) {
+    if constexpr (MODE == GEMM_DGRAD) {
+        if (drop) return gate || res ? nullptr : tc_gemm_kernel<MODE, SK, false, true>;
+        if (res) return tc_gemm_kernel<MODE, SK, false, false, true, true>;
+        return gate ? tc_gemm_kernel<MODE, SK, false, false, true> : tc_gemm_kernel<MODE, SK>;
+    } else {
+        if (res) return drop ? tc_gemm_kernel<MODE, SK, false, true, true, true>
+                             : tc_gemm_kernel<MODE, SK, false, false, true, true>;
+        if (gate) return drop ? tc_gemm_kernel<MODE, SK, false, true, true> : tc_gemm_kernel<MODE, SK, false, false, true>;
+        return drop ? tc_gemm_kernel<MODE, SK, false, true> : tc_gemm_kernel<MODE, SK>;
+    }
+}
+
+// The per-layer instantiation of a plan's key (gemm_launch), nullptr for a combination without one.  A WGRAD has only
+// the update forms, a FWD / DGRAD only the epilogue forms.
+static GemmKernel gemm_kernel(int mode, bool sk, bool drop, bool gate, bool res, SgdForm form) {
+    if (mode == GEMM_WGRAD) {
+        if (sk || drop || gate || res) return nullptr;
+        switch (form) {
+            case SGD_PLAIN: return tc_gemm_kernel<GEMM_WGRAD>;
+            case SGD_RULE: return tc_gemm_kernel<GEMM_WGRAD, false, true>;
+            case SGD_EMA: return tc_gemm_kernel<GEMM_WGRAD, false, true, false, false, false, true>;
+        }
+        return nullptr;
+    }
+    if (form != SGD_PLAIN) return nullptr;
+    switch (mode) {
+        case GEMM_FWD: return sk ? epilogue_kernel<GEMM_FWD, true>(drop, gate, res) : epilogue_kernel<GEMM_FWD, false>(drop, gate, res);
+        case GEMM_DGRAD: return sk ? epilogue_kernel<GEMM_DGRAD, true>(drop, gate, res)
+                                   : epilogue_kernel<GEMM_DGRAD, false>(drop, gate, res);
+    }
+    return nullptr;
+}
+
+static GroupKernel group_kernel(SgdForm form) {
+    switch (form) {
+        case SGD_PLAIN: return tc_wgrad_group_kernel<false>;
+        case SGD_RULE: return tc_wgrad_group_kernel<true>;
+        case SGD_EMA: return tc_wgrad_group_kernel<true, true>;
+    }
+    return nullptr;
+}
+
+static constexpr SgdForm kSgdForms[] = {SGD_PLAIN, SGD_RULE, SGD_EMA};
 static bool g_configured = false;
 
 cudaError_t gemm_configure() {
     if (g_configured) return cudaSuccess;
+    constexpr int kMaxDynSmem = 220 * 1024;
     cudaError_t e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_FWD>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_DGRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_WGRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_WGRAD, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    // the narrow tiles are meant to share an SM: ask for the carveout that fits the most of them
-    if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_wgrad_group_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_ema_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_wgrad_group_ema_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_wgrad_group_ema_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_FWD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_kernel<GEMM_DGRAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_drop_kernel<GEMM_FWD, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_drop_kernel<GEMM_FWD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_drop_kernel<GEMM_DGRAD, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_drop_kernel<GEMM_DGRAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_FWD, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_FWD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_FWD, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_FWD, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_DGRAD, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_gate_kernel<GEMM_DGRAD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_res_kernel<GEMM_FWD, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_res_kernel<GEMM_FWD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_res_kernel<GEMM_FWD, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_res_kernel<GEMM_FWD, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_res_kernel<GEMM_DGRAD, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(tc_gemm_res_kernel<GEMM_DGRAD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+    for (int mode : {GEMM_FWD, GEMM_DGRAD, GEMM_WGRAD})
+        for (int key = 0; key < 16; ++key)             // split-K, dropout, gated, residual
+            for (SgdForm form : kSgdForms)
+                if (GemmKernel fn = gemm_kernel(mode, key & 1, key & 2, key & 4, key & 8, form))
+                    if ((e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess)
+                        return e;
+    for (SgdForm form : kSgdForms) {
+        GroupKernel fn = group_kernel(form);
+        if ((e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+        // the narrow tiles are meant to share an SM: ask for the carveout that fits the most of them
+        e = cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        if (e != cudaSuccess) return e;
+    }
     g_configured = true;
     return cudaSuccess;
 }
 
 cudaError_t gemm_group_launch(const GemmGroupPlan& plan, cudaStream_t stream) {
-    if (!g_configured) {
-        cudaError_t e = gemm_configure();
-        if (e != cudaSuccess) return e;
-    }
-    if (plan.ema)
-        tc_wgrad_group_ema_kernel<<<plan.n, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev);
-    else if (plan.stateful)
-        tc_wgrad_group_kernel<true><<<plan.n, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev);
-    else
-        tc_wgrad_group_kernel<false><<<plan.n, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev);
+    if (cudaError_t e = gemm_configure(); e != cudaSuccess) return e;
+    GroupKernel fn = group_kernel(plan.form);
+    if (fn == nullptr) return cudaErrorInvalidValue;
+    fn<<<plan.n, kThreads, plan.smem_bytes, stream>>>(plan.entries_dev);
     g_launches.fetch_add(plan.n_gemms, std::memory_order_relaxed);
-    return cudaGetLastError();
-}
-
-template <int MODE>
-static cudaError_t launch_mode(const GemmPlan& plan, cudaStream_t stream) {
-    if (!g_configured) {
-        cudaError_t e = gemm_configure();
-        if (e != cudaSuccess) return e;
-    }
-    if constexpr (MODE != GEMM_WGRAD) {
-        if (gemm_residual(plan)) {
-            const bool drop = MODE == GEMM_FWD && plan.p.drop.on() && plan.p.relu;
-            const bool sk = plan.p.k_splits > 1;
-#define SSB_RES_LAUNCH(S, D) tc_gemm_res_kernel<MODE, S, D><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p)
-            if (sk) { if (drop) SSB_RES_LAUNCH(true, MODE == GEMM_FWD); else SSB_RES_LAUNCH(true, false); }
-            else { if (drop) SSB_RES_LAUNCH(false, MODE == GEMM_FWD); else SSB_RES_LAUNCH(false, false); }
-#undef SSB_RES_LAUNCH
-            g_launches.fetch_add(1, std::memory_order_relaxed);
-            return cudaGetLastError();
-        }
-        if (gemm_gated(plan)) {
-            // the DGRAD's gate already holds the dropout scale: only the FWD has a dropout form
-            const bool drop = MODE == GEMM_FWD && plan.p.drop.on();
-            const bool sk = plan.p.k_splits > 1;
-#define SSB_GATE_LAUNCH(S, D) tc_gemm_gate_kernel<MODE, S, D><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p)
-            if (sk) { if (drop) SSB_GATE_LAUNCH(true, MODE == GEMM_FWD); else SSB_GATE_LAUNCH(true, false); }
-            else { if (drop) SSB_GATE_LAUNCH(false, MODE == GEMM_FWD); else SSB_GATE_LAUNCH(false, false); }
-#undef SSB_GATE_LAUNCH
-            g_launches.fetch_add(1, std::memory_order_relaxed);
-            return cudaGetLastError();
-        }
-        if (gemm_drops(plan)) {
-            if (plan.p.k_splits > 1)
-                tc_gemm_drop_kernel<MODE, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
-            else
-                tc_gemm_drop_kernel<MODE, false><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
-            g_launches.fetch_add(1, std::memory_order_relaxed);
-            return cudaGetLastError();
-        }
-        if (plan.p.k_splits > 1) {
-            tc_gemm_kernel<MODE, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
-            g_launches.fetch_add(1, std::memory_order_relaxed);
-            return cudaGetLastError();
-        }
-    } else {
-        if (has_ema(plan.p)) {
-            tc_gemm_ema_kernel<<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
-            g_launches.fetch_add(1, std::memory_order_relaxed);
-            return cudaGetLastError();
-        }
-        if (is_stateful(plan.p)) {
-            tc_gemm_kernel<MODE, false, true><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
-            g_launches.fetch_add(1, std::memory_order_relaxed);
-            return cudaGetLastError();
-        }
-    }
-    tc_gemm_kernel<MODE><<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
     return cudaGetLastError();
 }
 
@@ -956,12 +891,15 @@ bool gemm_drops(const GemmPlan& plan) {
 }
 
 cudaError_t gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
-    switch (plan.mode) {
-        case GEMM_FWD: return launch_mode<GEMM_FWD>(plan, stream);
-        case GEMM_DGRAD: return launch_mode<GEMM_DGRAD>(plan, stream);
-        case GEMM_WGRAD: return launch_mode<GEMM_WGRAD>(plan, stream);
-    }
-    return cudaErrorInvalidValue;
+    if (cudaError_t e = gemm_configure(); e != cudaSuccess) return e;
+    const bool gate = gemm_gated(plan), res = gemm_residual(plan);
+    // the gated and residual forms drop only in the FWD (gemm_drops: a FWD with relu or a DGRAD with mask)
+    const bool drop = gemm_drops(plan) && (plan.mode == GEMM_FWD || !(gate || res));
+    GemmKernel fn = gemm_kernel(plan.mode, plan.p.k_splits > 1, drop, gate, res, update_form(plan.p));
+    if (fn == nullptr) return cudaErrorInvalidValue;
+    fn<<<plan.grid, kThreads, plan.smem_bytes, stream>>>(plan.tmA, plan.tmB, plan.tmC, plan.p);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return cudaGetLastError();
 }
 
 }  // namespace ssb

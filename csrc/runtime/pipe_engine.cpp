@@ -1165,7 +1165,7 @@ void PipeEngine::exec(const Op& op, int set) {
             break;
         case OP_SGD: {
             const SgdState opt = opt_for(0, set);
-            if (opt.plain()) CUDA_CHECK(launch_sgd(op.a, op.b, op.lr, op.n, st));
+            if (opt.form() == SGD_PLAIN) CUDA_CHECK(launch_sgd(op.a, op.b, op.lr, op.n, st));
             else CUDA_CHECK(launch_sgd_momentum(op.a, op.b, op.lr, opt, op.n, st));
             break;
         }

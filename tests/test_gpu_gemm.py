@@ -14,8 +14,9 @@ bound); tf32 0.97 for WGRAD and 0.93 for the fused update with one row, 0.96 for
 10-term dgrad.  These come near 1 by the bound's own derivation: with one product per element (or few non-zero ones,
 behind a ReLU) nothing averages out, and two operands truncated to 10 mantissa bits reach almost 2^-9 of the product.
 
-The residual form (``tc_gemm_res_kernel``) runs through ``ops.cuda``'s ``residual=`` / ``skip=`` / ``gpre=`` at every
-tile edge and split count, in fp32, tf32 and bf16, with a nil feature where the result is the skip up to one rounding.
+The residual form (``tc_gemm_kernel``'s ``RES``) runs through ``ops.cuda``'s ``residual=`` / ``skip=`` / ``gpre=`` at
+every tile edge and split count, in fp32, tf32 and bf16, with a nil feature where the result is the skip up to one
+rounding.
 
 Every input's padding columns hold NaN and every output's padding a finite sentinel, so a kernel that reads or writes
 past the end of a row fails.  The CPU tests at the end check that the grid reaches every branch of the host planner,
@@ -210,8 +211,8 @@ def test_dgrad_per_element(rows, m, k, precision):
 
 
 # ---------------------------------------------------------------- the activated and dropout variants
-# every forward variant gemm_configure registers: ReLU + dropout (tc_gemm_drop_kernel) and each smooth kind with and
-# without dropout (tc_gemm_gate_kernel); the launch's rows are samples (row_base + n) * dp + rank of the masks
+# every forward variant gemm_configure registers: ReLU + dropout (tc_gemm_kernel's DROP) and each smooth kind with and
+# without dropout (its GATE); the launch's rows are samples (row_base + n) * dp + rank of the masks
 FWD_VARIANTS = [("relu", True)] + [(k, d) for k in ("gelu", "silu", "tanh") for d in (False, True)]
 DROP = (0.3, 0x1234_5678_9ABC_DEF0, 6, 9, 5, 3, 2)            # p, seed, layer, step, row_base, dp, rank
 
@@ -810,7 +811,7 @@ def test_oracles_reject_injected_faults():
 
 
 # ================================================================================================== the residual form
-# tc_gemm_res_kernel through ops.cuda's residual=True: FWD out = skip + f(z) * keep * s (every activation gated, ReLU's
+# tc_gemm_kernel's RES through ops.cuda's residual=True: FWD out = skip + f(z) * keep * s (every activation gated, ReLU's
 # gate 1[z > 0] * keep * s), DGRAD gpre = dz W + skip, out = gpre * mask (the mask: the previous layer's gate).  skip,
 # gpre and the mask each have a row pitch unlike out's.  bf16 through test_gpu_bf16's operand model.  The last feature
 # of every shape is nil (FWD: zero weight row and bias, so f(0) = 0; DGRAD: zero weight column), where the result is the

@@ -804,7 +804,7 @@ def test_residual_first_layer_over_both_staging_sets(form, precision, monkeypatc
 
 @pytest.mark.gpu
 def test_splitk_residual_layers_over_two_steps(monkeypatch):
-    """The wide residual layer's split-K FWD and DGRAD (tc_gemm_res_kernel with k_splits > 1) over two steps on new
+    """The wide residual layer's split-K FWD and DGRAD (tc_gemm_kernel's RES with k_splits > 1) over two steps on new
     inputs, each step per element against its own weights: an output tile whose counter was not re-armed would keep the
     first step's value."""
     from shallowspeed_b200.parallel.engine import Trainer

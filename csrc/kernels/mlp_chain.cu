@@ -1,5 +1,6 @@
-// Host side of the layer-chain kernel (mlp_chain.cuh): plans, shared-memory budgets, and the launches, with the TF32 /
-// 3xTF32 instantiations; the BF16 ones are in mlp_chain_bf16.cu, the residual ones in mlp_chain_res.cu.
+// Host side of the layer-chain kernel (mlp_chain.cuh): plans, shared-memory budgets, and the launches, with the 3xTF32
+// instantiations; the TF32 and BF16 ones are in mlp_chain_tf32.cu and mlp_chain_bf16.cu, the residual ones in
+// mlp_chain_res.cu (3xTF32), mlp_chain_res_tf32.cu and mlp_chain_res_bf16.cu.
 #include "mlp_chain.cuh"
 
 namespace ssb {
@@ -153,11 +154,12 @@ void chain_plan_free(ChainPlan* plan) {
 
 // the instantiation of a (precision, residual) pair, from the translation unit that compiles it
 static ChainKernel chain_kernel_of(int prec, bool res, ChainForm form, int ntw, bool ce, bool drop, bool gate) {
-    if (res) return chain_kernel_res(prec, form, ntw, ce, drop, gate);
     switch (prec) {
-        case PREC_TF32: return chain_kernel<PREC_TF32, false>(form, ntw, ce, drop, gate);
-        case PREC_3XTF32: return chain_kernel<PREC_3XTF32, false>(form, ntw, ce, drop, gate);
-        case PREC_BF16: return chain_kernel_bf16(form, ntw, ce, drop, gate);
+        case PREC_TF32: return (res ? chain_kernel_res_tf32 : chain_kernel_tf32)(form, ntw, ce, drop, gate);
+        case PREC_3XTF32:
+            return res ? chain_kernel_res_3xtf32(form, ntw, ce, drop, gate)
+                       : chain_kernel<PREC_3XTF32, false>(form, ntw, ce, drop, gate);
+        case PREC_BF16: return (res ? chain_kernel_res_bf16 : chain_kernel_bf16)(form, ntw, ce, drop, gate);
     }
     return nullptr;
 }

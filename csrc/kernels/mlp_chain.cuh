@@ -154,7 +154,7 @@ __device__ __forceinline__ unsigned long long gtime() {
 #define DBG(role, idx) do { if (p.dbg != nullptr && blockIdx.x == 0 && (idx) < 256) p.dbg[(role) * 256 + (idx)] = gtime(); } while (0)
 
 // PREC (precision.h) is a compile-time switch: the single-pass TF32 instantiation carries none of the extra products, and
-// the BF16 instantiations are compiled in a translation unit of their own (mlp_chain_bf16.cu).
+// each precision's instantiations are compiled in a translation unit of their own (see chain_kernel below).
 // FOLD (pipeline boundaries inside the kernel, see ChainParams) is a compile-time switch as well: launches without a
 // folded boundary use the instantiation without its prologue and its predicated peer stores.
 // NTW: n8 tiles of a math warp's accumulator (chain_warp_cols / 8, rounded up to 2, 4 or 8) - sized at compile time
@@ -1047,9 +1047,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
 
 
 // =========================================================================== host side: the instantiations
-// Every translation unit that includes this file instantiates the kernel for the precisions it selects: mlp_chain.cu
-// PREC_TF32 and PREC_3XTF32, mlp_chain_bf16.cu PREC_BF16, mlp_chain_res.cu the RES forms of all three, so that none
-// grows the longest compile.
+// Every (precision, residual) pair is instantiated in a translation unit of its own, and the build compiles them in
+// parallel, so that no pair lengthens the longest compile: mlp_chain.cu PREC_3XTF32, mlp_chain_tf32.cu PREC_TF32,
+// mlp_chain_bf16.cu PREC_BF16, and mlp_chain_res.cu / mlp_chain_res_tf32.cu / mlp_chain_res_bf16.cu their RES forms.
 
 using ChainKernel = void (*)(ChainParams);
 // the launch form of a plan: one CTA per micro-batch, with folded pipeline boundaries (FOLD), or a cluster (CLUSTER)
@@ -1094,8 +1094,11 @@ static ChainKernel chain_kernel(ChainForm form, int ntw, bool ce, bool drop, boo
     else return chain_kernel_drop<PREC, false, false>(form, ntw, ce, drop);
 }
 
-// mlp_chain_bf16.cu: chain_kernel<PREC_BF16, false>; mlp_chain_res.cu: chain_kernel<prec, true>
+// chain_kernel<PREC, RES> of the other translation units (the 3xTF32 one without RES is mlp_chain.cu's own)
+ChainKernel chain_kernel_tf32(ChainForm form, int ntw, bool ce, bool drop, bool gate);
 ChainKernel chain_kernel_bf16(ChainForm form, int ntw, bool ce, bool drop, bool gate);
-ChainKernel chain_kernel_res(int prec, ChainForm form, int ntw, bool ce, bool drop, bool gate);
+ChainKernel chain_kernel_res_3xtf32(ChainForm form, int ntw, bool ce, bool drop, bool gate);
+ChainKernel chain_kernel_res_tf32(ChainForm form, int ntw, bool ce, bool drop, bool gate);
+ChainKernel chain_kernel_res_bf16(ChainForm form, int ntw, bool ce, bool drop, bool gate);
 
 }  // namespace ssb

@@ -1,6 +1,5 @@
-// The BF16 instantiations of the layer-chain kernel (mlp_chain.cuh), compiled apart from the TF32 / 3xTF32 ones in
-// mlp_chain.cu: the build compiles the two translation units in parallel, so a third precision does not lengthen the
-// longest compile.
+// The BF16 instantiations of the layer-chain kernel (mlp_chain.cuh), compiled apart from the other precisions: the build
+// compiles the chain's translation units in parallel, so a precision does not lengthen the longest compile.
 #include "mlp_chain.cuh"
 
 namespace ssb {

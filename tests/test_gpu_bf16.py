@@ -45,6 +45,18 @@ def bf(t):
     return t.float().cpu().bfloat16().double()
 
 
+def grad_oracle_bf16(dz, x, rtol):
+    """test_gpu_gemm.grad_oracle on the bf16-rounded operands: ``[bf(dz).T @ bf(x) | colsum(dz)]`` in fp64, the bias
+    column summed from the UNROUNDED dz in fp32 (one rounding per row).  Called with rtol 0.0 for a magnitude only."""
+    dz, x = dz.double(), x.double()
+    dzr, xr = bf(dz), bf(x)
+    g = torch.cat([dzr.T @ xr, dz.sum(0)[:, None]], dim=1)
+    mag = torch.cat([dzr.abs().T @ xr.abs(), dz.abs().sum(0)[:, None]], dim=1)
+    bound = rtol * mag + ATOL
+    bound[:, -1] += dz.shape[0] * U * mag[:, -1]
+    return g, bound
+
+
 def _note(kernel, res, what):
     v = max(res.values()) if res else 0.0
     if v > WORST.get(kernel, (-1.0, ""))[0]:

@@ -7,16 +7,13 @@ term), the bias gradient the fp32 column sum of the unrounded dZ.  So every owne
 element and every outbound tile or line is checked per element against the bf16 oracle, in the dp x pp stages as well
 (an LL and a flag-protocol stage, whose DP checks run on the partials of the swapped oracle)."""
 import pytest
-import torch
 
 import test_gpu_dp_replay as DP
 import test_gpu_pp_replay as PP
-from test_gpu_bf16 import RTOL_BF16, bf, rtol_bf16
-from test_gpu_chain import ATOL, dgrad_oracle, fwd_oracle
+from test_gpu_bf16 import RTOL_BF16, bf, grad_oracle_bf16, rtol_bf16
+from test_gpu_chain import dgrad_oracle, fwd_oracle
 
 pytestmark = pytest.mark.gpu
-
-U = 2.0**-24
 
 
 def _rtol_for(precision, k, splits=1):
@@ -24,21 +21,9 @@ def _rtol_for(precision, k, splits=1):
     return rtol_bf16(k, splits)
 
 
-def _grad_oracle(dz, x, rtol):
-    """test_gpu_gemm.grad_oracle on the bf16-rounded operands: ``[bf(dz).T @ bf(x) | colsum(dz)]`` in fp64, the bias
-    column summed from the UNROUNDED dz in fp32 (one rounding per row).  Called with rtol 0.0 for a magnitude only."""
-    dz, x = dz.double(), x.double()
-    dzr, xr = bf(dz), bf(x)
-    g = torch.cat([dzr.T @ xr, dz.sum(0)[:, None]], dim=1)
-    mag = torch.cat([dzr.abs().T @ xr.abs(), dz.abs().sum(0)[:, None]], dim=1)
-    bound = rtol * mag + ATOL
-    bound[:, -1] += dz.shape[0] * U * mag[:, -1]
-    return g, bound
-
-
 def _bf16_oracles(monkeypatch, *modules):
     for module in modules:
-        monkeypatch.setattr(module, "grad_oracle", _grad_oracle)
+        monkeypatch.setattr(module, "grad_oracle", grad_oracle_bf16)
         monkeypatch.setattr(module, "rtol_for", _rtol_for)
 
 

@@ -243,11 +243,13 @@ def check_layers(eng, model, W0, x, n_mu, mb, precision, lr, samples_of, step=0,
     fp64: act (and the gate) of every activated layer through act_fwd_oracle, with the masks of
     ``ops.functional.dropout_mask`` and dropped elements exactly 0; every dgrad through act_dgrad_oracle from the stored
     act / gate; the update through rows_update_oracle.  ``samples_of(mu)``: the global sample index of every row of
-    micro-batch mu; ``x``: the stage input of the step; ``W0``: the flat weight arena before the step.  Returns
-    {check: max err / bound}."""
+    micro-batch mu; ``x``: the stage input of the step; ``W0``: the flat weight arena before the step.  bf16 products
+    are checked from the rounded operands (test_gpu_residual.operand_model).  Returns {check: max err / bound}."""
     from shallowspeed_b200.ops import functional as F
+    from test_gpu_residual import operand_model
 
-    kind, p, rtol = model.activation, model.dropout, RTOL[precision]
+    kind, p = model.activation, model.dropout
+    op, rtol = operand_model(precision)
     s = F.dropout_scale(p) if p > 0 else 1.0
     L = len(model.linears)
     res, n_dropped, tails = {}, 0, [0, 0]
@@ -272,7 +274,7 @@ def check_layers(eng, model, W0, x, n_mu, mb, precision, lr, samples_of, step=0,
             W, b = blocks[l - 1][:, :-1], blocks[l - 1][:, -1]
             if lin.activation is not None:
                 keep = F.dropout_mask(p, model.dropout_seed, lin.dropout[2], step, samples, lin.out_dims) if p > 0 else None
-                (ra, ba), gam, z = act_fwd_oracle(kind, acts[l - 1], W, b, keep, s, rtol)
+                (ra, ba), gam, z = act_fwd_oracle(kind, op(acts[l - 1]), op(W), b, keep, s, rtol)
                 put(f"act{l}", excess(acts[l], ra, ba))
                 tails[0] += int((z.abs() > 4).sum())
                 tails[1] += int((z.abs() > 9).sum())
@@ -286,14 +288,14 @@ def check_layers(eng, model, W0, x, n_mu, mb, precision, lr, samples_of, step=0,
                     for t in dropped:
                         assert bool((t.view(torch.int32) == 0).all()), f"mu {mu} layer {l}: a dropped element is not +0"
             else:
-                ref, bound = fwd_oracle(acts[l - 1], W, b, False, rtol)
+                ref, bound = fwd_oracle(op(acts[l - 1]), op(W), b, False, rtol)
                 put(f"fwd{l}", excess(acts[l], ref, bound))
             if l >= 2:
                 prev = model.linears[l - 2]
                 if prev.activation is None:
-                    ref, bound = dgrad_oracle(dzs[l], W, torch.ones_like(acts[l - 1]), rtol)
+                    ref, bound = dgrad_oracle(op(dzs[l]), op(W), torch.ones_like(acts[l - 1]), rtol)
                 else:
-                    ref, bound = act_dgrad_oracle(dzs[l], W, kind, acts[l - 1], gates[l - 1], s, rtol)
+                    ref, bound = act_dgrad_oracle(op(dzs[l]), op(W), kind, acts[l - 1], gates[l - 1], s, rtol)
                     if kind == "relu":
                         assert bool((dzs[l - 1][acts[l - 1] == 0] == 0).all()), (mu, l)
                 put(f"dgrad{l}", excess(dzs[l - 1], ref, bound))
@@ -307,7 +309,13 @@ def check_layers(eng, model, W0, x, n_mu, mb, precision, lr, samples_of, step=0,
             o, ld = lin.out_dims, model.arena.lds[lin.block_index]
             off = model.arena.offsets[lin.block_index]
             d = (W1[off:off + o * ld] - W0[off:off + o * ld].double().cpu()).view(o, ld)[:, : lin.in_dims + 1]
-            ref, bound = rows_update_oracle(torch.cat(upd_dz[l - 1]), torch.cat(upd_a[l - 1]), blocks[l - 1], lr, rtol)
+            if precision == "bf16":
+                from test_gpu_bf16 import _update_oracle
+
+                ref, bound = _update_oracle(torch.cat(upd_dz[l - 1]), torch.cat(upd_a[l - 1]), blocks[l - 1], lr)
+            else:
+                ref, bound = rows_update_oracle(torch.cat(upd_dz[l - 1]), torch.cat(upd_a[l - 1]), blocks[l - 1], lr,
+                                                rtol)
             put(f"upd{l}", excess(d, ref, bound))
     kernel = "chain" if eng.uses_chain() else "layer-wise"
     note_worst((kernel, kind, p > 0, precision), res, f"L={L} n_mu={n_mu} mb={mb} step={step}")

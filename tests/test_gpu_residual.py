@@ -75,11 +75,12 @@ def nil_features(W, b):
 
 
 def check_residual_layers(eng, model, W0, x, n_mu, mb, precision, lr, step=0, g_in=None, samples_of=None,
-                          training=True):
+                          training=True, check_update=True):
     """Every layer of the step that just ran against fp64 from the engine's own buffers; returns {check: err / bound}.
     ``g_in``: the gradient a non-last stage received ([n_mu, mb, out]), else None.  ``samples_of(mu)``: the global
     sample index of every row of micro-batch mu, whose dropout masks the rows draw (default: mu * mb + n, one replica).
-    ``training=False``: an inference pass (no dropout, gates, dgrads or update).
+    ``training=False``: an inference pass (no dropout, gates, dgrads or update).  ``check_update=False``: the caller
+    checks the update (another rule than plain SGD at ``lr``).
 
     At the nil features of a residual layer (nil_features) the skip terms stand alone and are checked to one rounding:
     ``skip{l}``, act[l] = act[l - 1] at a nil output; ``gskip{l}``, the dgrad of layer l at a nil input is g_l alone,
@@ -204,7 +205,7 @@ def check_residual_layers(eng, model, W0, x, n_mu, mb, precision, lr, step=0, g_
                 g_val, g_bnd = pre_ref, pre_b
     W1 = model.arena.weights.detach().double().cpu()
     for l, lin in enumerate(model.linears, start=1):
-        if g_in is not None or not training:
+        if g_in is not None or not training or not check_update:
             break                                          # a replayed stage: the update is checked by its own tests
         o, ld = lin.out_dims, model.arena.lds[lin.block_index]
         off = model.arena.offsets[lin.block_index]

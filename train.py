@@ -263,7 +263,9 @@ def main(args):
         # collective over the DP group (native engine): every replica takes part, each owner contributes its entries
         ema = worker.ema_state() if engine == "native" else model.arena.ema
         n = ema_model.arena.numel
-        ema_model.arena.weights[:n].copy_(ema[:n].to(ema_model.arena.weights.device))
+        # the native ema_state() is on the host: a blocking host-to-device copy_, because the EMA worker's engine runs on
+        # non-blocking streams, which would not wait for a device-to-device copy on the current stream
+        ema_model.arena.weights[:n].copy_(ema[:n])
         return accuracy, compute_accuracy(ema_model, ema_worker, val_dataset)
 
     start_time = time.time()

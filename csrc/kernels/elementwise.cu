@@ -5,6 +5,7 @@
 #include "ptx.cuh"
 
 #include <cfloat>
+#include <climits>
 
 namespace ssb {
 
@@ -12,6 +13,11 @@ namespace ssb {
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+__device__ __forceinline__ float warp_max_nan(float v) {   // the MSE head's global max: NaN propagates (softmax_ref)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = max_nan(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
 }
 __device__ __forceinline__ float warp_sum(float v) {
@@ -22,12 +28,12 @@ __device__ __forceinline__ float warp_sum(float v) {
 template <bool IS_MAX>
 __device__ float block_reduce(float v, float* scratch) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    v = IS_MAX ? warp_max(v) : warp_sum(v);
+    v = IS_MAX ? warp_max_nan(v) : warp_sum(v);
     __syncthreads();
     if (lane == 0) scratch[warp] = v;
     __syncthreads();
     float r = IS_MAX ? -FLT_MAX : 0.f;
-    for (int i = 0; i < nw; ++i) r = IS_MAX ? fmaxf(r, scratch[i]) : r + scratch[i];   // fixed order: deterministic
+    for (int i = 0; i < nw; ++i) r = IS_MAX ? max_nan(r, scratch[i]) : r + scratch[i];   // fixed order: deterministic
     return r;
 }
 
@@ -93,7 +99,7 @@ __global__ void __launch_bounds__(256) loss_head_kernel(const float* __restrict_
     }
 
     float mx = -FLT_MAX;
-    for (int i = threadIdx.x; i < rows * cols; i += blockDim.x) mx = fmaxf(mx, logits[(size_t)(i / cols) * ldl + (i % cols)]);
+    for (int i = threadIdx.x; i < rows * cols; i += blockDim.x) mx = max_nan(mx, logits[(size_t)(i / cols) * ldl + (i % cols)]);
     const float gmax = block_reduce<true>(mx, scratch);
 
     float loss = 0.f;
@@ -203,7 +209,7 @@ DropoutSpec dropout_spec(double p, uint64_t seed) {
 }
 
 __global__ void relu_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, long n) {
-    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) y[i] = fmaxf(x[i], 0.f);
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) y[i] = relu_f(x[i]);
 }
 cudaError_t launch_relu_fwd(const float* x, float* y, long n, cudaStream_t stream) {
     int blocks = (int)((n + 255) / 256);
@@ -397,25 +403,33 @@ cudaError_t launch_sgd_momentum(float* w, const float* g, const float* lr, const
     return cudaGetLastError();
 }
 
-// one warp per row: argmax(pred) == argmax(target) (first maximum wins, like numpy.argmax)
+// does (a, ia) come before (b, ib) in argmax order?  NaN is the maximum and the lower index wins a tie, as in
+// torch.argmax / numpy.argmax; ib == INT_MAX is the empty candidate.
+__device__ __forceinline__ bool argmax_before(float a, int ia, float b, int ib) {
+    if (ia == INT_MAX) return false;
+    if (ib == INT_MAX) return true;
+    if (b != b) return a != a && ia < ib;
+    return a != a || a > b || (a == b && ia < ib);
+}
+// one warp per row: argmax(pred) == argmax(target) (first maximum wins, NaN the largest, like numpy.argmax)
 __global__ void argmax_correct_kernel(const float* __restrict__ pred, int ldp, const float* __restrict__ target, int ldt,
                                       int rows, int cols, int* correct) {
     const int lane = threadIdx.x & 31;
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (row >= rows) return;
-    float bp = -FLT_MAX, bt = -FLT_MAX;
-    int ip = cols, it = cols;
+    float bp = 0.f, bt = 0.f;
+    int ip = INT_MAX, it = INT_MAX;
     for (int c = lane; c < cols; c += 32) {
         const float a = pred[(size_t)row * ldp + c], b = target[(size_t)row * ldt + c];
-        if (a > bp) { bp = a; ip = c; }
-        if (b > bt) { bt = b; it = c; }
+        if (argmax_before(a, c, bp, ip)) { bp = a; ip = c; }
+        if (argmax_before(b, c, bt, it)) { bt = b; it = c; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         const float op = __shfl_xor_sync(0xffffffffu, bp, o); const int oip = __shfl_xor_sync(0xffffffffu, ip, o);
         const float ot = __shfl_xor_sync(0xffffffffu, bt, o); const int oit = __shfl_xor_sync(0xffffffffu, it, o);
-        if (op > bp || (op == bp && oip < ip)) { bp = op; ip = oip; }
-        if (ot > bt || (ot == bt && oit < it)) { bt = ot; it = oit; }
+        if (argmax_before(op, oip, bp, ip)) { bp = op; ip = oip; }
+        if (argmax_before(ot, oit, bt, it)) { bt = ot; it = oit; }
     }
     if (lane == 0 && ip == it) atomicAdd(correct, 1);
 }

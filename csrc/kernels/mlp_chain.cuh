@@ -133,9 +133,9 @@ __device__ __forceinline__ float warp_sum_f(float v) {
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
 }
-__device__ __forceinline__ float warp_max_f(float v) {
+__device__ __forceinline__ float warp_max_f(float v) {   // NaN-propagating: the MSE head's global max
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    for (int o = 16; o > 0; o >>= 1) v = max_nan(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
 }
 
@@ -608,7 +608,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                                     tgam[j][r] = 0.f;
                                     if (ly.relu) x = gate_fwd(x, l, t_feat(r), t_row(j, r), tgam[j][r]);
                                 } else {
-                                    if (ly.relu) x = fmaxf(x, 0.f);
+                                    if (ly.relu) x = relu_f(x);
                                     if constexpr (DROP) { if (ly.relu) x = drop_fwd(x, l, t_feat(r), t_row(j, r)); }
                                 }
                                 if constexpr (RES) { if (res_l && t_feat(r) < ly.out) x += skip_in(l, src, t_row(j, r), t_feat(r)); }
@@ -656,7 +656,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                             if constexpr (GATE) {
                                 if (ly.relu) x = gate_fwd(x, l, m, c + j, gm);
                             } else {
-                                if (ly.relu) x = fmaxf(x, 0.f);
+                                if (ly.relu) x = relu_f(x);
                                 if constexpr (DROP) { if (ly.relu) x = drop_fwd(x, l, m, c + j); }
                             }
                             if constexpr (RES) { if (res_l && m_ok) x += skip_in(l, src, c + j, m); }
@@ -721,7 +721,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_chain_kernel(const ChainParam
                         float gmax = -3.0e38f;
                         if (!ce) {
                             for (int n = lane; n < p.mb_rows; n += 32)
-                                for (int k = 0; k < C; ++k) gmax = fmaxf(gmax, scratch[n * kScratchLd + k]);
+                                for (int k = 0; k < C; ++k) gmax = max_nan(gmax, scratch[n * kScratchLd + k]);
                             gmax = warp_max_f(gmax);
                         }
                         for (int n = lane; n < N; n += 32) {

@@ -461,12 +461,19 @@ __device__ __forceinline__ void act_fwd(int kind, float z, float& a, float& g) {
         g = 1.f - t * t;
     }
 }
+// ReLU of every kernel: max(z, 0) that keeps NaN, as torch's clamp_min and numpy's maximum do (fmaxf alone returns 0
+// for a NaN, which would turn a diverged unit into a dead one).  Every other z keeps fmaxf's bits: z <= 0 (-0 included)
+// gives +0.
+__device__ __forceinline__ float relu_f(float z) { return z != z ? z : fmaxf(z, 0.f); }
+// max that propagates NaN (torch's and numpy's max); fmaxf's bits for every other pair.
+__device__ __forceinline__ float max_nan(float a, float b) { return (a != a || b != b) ? a + b : fmaxf(a, b); }
+
 // act_fwd for every ActKind, ReLU included: a = max(z, 0) and g = 1[z > 0].  The residual kernels store the gate of a
 // ReLU layer too (its output x + relu(z) is no longer its own mask); the smooth-only act_fwd stays as the gated kernels
 // compile it.
 __device__ __forceinline__ void act_fwd_any(int kind, float z, float& a, float& g) {
     if (kind == ACT_RELU) {
-        a = fmaxf(z, 0.f);
+        a = relu_f(z);
         g = z > 0.f ? 1.f : 0.f;
     } else {
         act_fwd(kind, z, a, g);

@@ -286,7 +286,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                                 x *= mk[j];
                             }
                         } else if (MODE == GEMM_FWD) {
-                            if (p.relu) x = fmaxf(x, 0.f);
+                            if (p.relu) x = relu_f(x);
                             if constexpr (DROP) x = drop_fwd(x, n);
                         } else if (mask != nullptr) {
                             x = (mk[j] > 0.f) ? (DROP ? x * p.drop.scale : x) : 0.f;
@@ -343,7 +343,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                             x *= mk[j];
                         }
                     } else if (MODE == GEMM_FWD) {
-                        if (p.relu) x = fmaxf(x, 0.f);
+                        if (p.relu) x = relu_f(x);
                         if constexpr (DROP) x = drop_fwd(x, n0 + c + j);
                     } else if (mask != nullptr) {
                         x = (mk[j] > 0.f) ? (DROP ? x * p.drop.scale : x) : 0.f;
@@ -368,8 +368,9 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
         } else {
             // WGRAD: registers -> swizzled smem panels -> ONE TMA store (overwrite) or TMA reduce-add (accumulate,
             // performed in L2) per 32-column panel.  With fuse_sgd the tile is scaled by -lr and reduce-added straight into
-            // W: dW never touches memory, zero_grad and the optimizer pass disappear.  OOB rows/columns are clipped by the
-            // tensor map, so the bias column (index n_total of the same [out, ld] block) is never touched here.
+            // W: dW never touches memory, zero_grad and the optimizer pass disappear.  OOB rows are clipped by the tensor
+            // map; columns only at 16-byte granularity, so the store may reach the bias column (index n_total of the
+            // same [out, ld] block): the columns >= n_total stage +0 (below), and the bias path writes after the store.
             // STATEFUL (fuse_sgd with momentum / weight decay): the tile holds the final dW, so each lane turns its row's
             // 16 values into the step direction d (sgd_direction) - reading and writing its V entries, and reading W
             // only with weight decay - before the same -lr scaling and reduce-add.  Columns >= n_total get d = 0 and
@@ -388,6 +389,13 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
                 if (16 * ch >= wcols) break;
                 float v[16];
                 warp_acc_row16(acc, ch, v, lane);
+                if constexpr (!STATEFUL) {
+                    // columns >= n_total stage +0, not their accumulator: that is dZ^T times the zero-filled columns of X,
+                    // NaN where dZ holds an Inf or NaN (Inf * 0), and the 16-byte store below may reach the bias slot
+                    const int nc = n0 + nw0 + 16 * ch;
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) v[j] = nc + j < p.n_total ? v[j] : 0.f;
+                }
                 if constexpr (STATEFUL) {
                     const int nc = n0 + nw0 + 16 * ch;
                     const bool has_v = p.V != nullptr, read_w = EMA || p.weight_decay != 0.f;   // weight decay and the EMA read W

@@ -49,8 +49,10 @@ def relu_ref(input: torch.Tensor) -> torch.Tensor:
 
 
 def relu_grad_ref(grad_output: torch.Tensor, bitmask: torch.Tensor) -> torch.Tensor:
+    """The mask selects, as in every kernel and torch's own ReLU backward: a masked-off gradient is +0 even when it is
+    NaN or +-Inf (a product would make NaN * 0 = NaN)."""
     assert bitmask.dtype == torch.bool
-    return grad_output * bitmask
+    return torch.where(bitmask, grad_output, 0.0)
 
 
 def linear_ref(input, weight, bias):

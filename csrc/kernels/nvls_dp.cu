@@ -14,6 +14,12 @@
 // A replica's CTAs never wait for each other (the last CTA to finish signals and is the only one that waits for
 // the peers), the peers' kernels run on other GPUs; the grid is kept <= #SMs so CTA 0 (which announces flag_in) is
 // always resident.  Spins are bounded (ptx.cuh: trap, no hang).
+//
+// Transport.  The kernel touches the team in three places only: the load-reduce of a gradient chunk, the store of a
+// result chunk and the flag add.  MULTICAST issues them to the switch (multimem.*).  REPLAY does the same through the
+// unicast views of a local team (NvlsContext::local, p.team): an fp32 sum of the members' chunks in rank order, a store
+// into every member, a release add on every member's flag word.  Everything else is one body, so a replica of a dp-way
+// group runs on one GPU against peers that are plain memory.
 #include "kernels/ptx.cuh"
 #include "runtime/nvls_context.h"
 
@@ -35,11 +41,52 @@ __device__ __forceinline__ void multimem_red_release_add(uint32_t* mc_addr, uint
     asm volatile("multimem.red.release.sys.global.add.u32 [%0], %1;" ::"l"(mc_addr), "r"(v) : "memory");
 }
 
+__device__ __forceinline__ void red_release_add(uint32_t* addr, uint32_t v) {
+    asm volatile("red.release.sys.global.add.u32 [%0], %1;" ::"l"(addr), "r"(v) : "memory");
+}
+
+enum class NvlsTransport { MULTICAST, REPLAY };
+
+// sum over the team of the gradient chunk at float offset `off`
+template <NvlsTransport T>
+__device__ __forceinline__ float4 team_ld_reduce(const NvlsParams& p, int64_t off) {
+    if constexpr (T == NvlsTransport::REPLAY) {
+        float4 s = *reinterpret_cast<const float4*>(p.team[0].G + off);
+        for (int m = 1; m < p.dp; ++m) {
+            const float4 g = *reinterpret_cast<const float4*>(p.team[m].G + off);
+            s.x += g.x; s.y += g.y; s.z += g.z; s.w += g.w;
+        }
+        return s;
+    } else {
+        return multimem_ld_reduce_f4(p.G_mc + off);
+    }
+}
+
+// the chunk at float offset `off` of every member's weights (GRADS: gradients)
+template <NvlsTransport T, bool GRADS>
+__device__ __forceinline__ void team_st(const NvlsParams& p, int64_t off, const float4& v) {
+    if constexpr (T == NvlsTransport::REPLAY) {
+        for (int m = 0; m < p.dp; ++m) *reinterpret_cast<float4*>((GRADS ? p.team[m].G : p.team[m].W) + off) = v;
+    } else {
+        multimem_st_f4((GRADS ? p.G_mc : p.W_mc) + off, v);
+    }
+}
+
+// +1 on every member's flag_in (OUT: flag_out), release
+template <NvlsTransport T, bool OUT>
+__device__ __forceinline__ void team_arrive(const NvlsParams& p) {
+    if constexpr (T == NvlsTransport::REPLAY) {
+        for (int m = 0; m < p.dp; ++m) red_release_add(OUT ? p.team[m].flag_out : p.team[m].flag_in, 1u);
+    } else {
+        multimem_red_release_add(OUT ? p.flag_out_mc : p.flag_in_mc, 1u);
+    }
+}
+
 // STATEFUL (SGD only): momentum / weight decay through sgd_direction; the owner of chunk c reads and writes its unicast
 // momentum V[c] (never multicast: no other replica touches chunk c's state).
 // EMA (with STATEFUL): the owner of chunk c also moves its unicast EMA chunk (p.opt.E) towards the new weights; with a
 // plain rule the update is the stateless one.
-template <bool SGD, bool STATEFUL = false, bool EMA = false>
+template <bool SGD, bool STATEFUL = false, bool EMA = false, NvlsTransport T = NvlsTransport::MULTICAST>
 __global__ void __launch_bounds__(256) nvls_reduce_kernel(const NvlsParams p) {
     const uint32_t epoch = *p.epoch + 1u;                     // same value on every replica (one bump per launch)
     const uint32_t target = epoch * (uint32_t)p.dp;
@@ -50,7 +97,7 @@ __global__ void __launch_bounds__(256) nvls_reduce_kernel(const NvlsParams p) {
     // ---- my gradients are final (stream order: the wgrad kernels of this step precede this launch)
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         __threadfence_system();
-        multimem_red_release_add(p.flag_in_mc, 1u);
+        team_arrive<T, false>(p);
     }
     if (threadIdx.x == 0) wait_flag_ge(p.flag_in_uc, target);  // every replica's gradients are final
     __syncthreads();
@@ -60,7 +107,7 @@ __global__ void __launch_bounds__(256) nvls_reduce_kernel(const NvlsParams p) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i * p.dp + p.rank < n4; i += stride) {
         const int64_t c = i * p.dp + p.rank;
-        const float4 g = multimem_ld_reduce_f4(p.G_mc + 4 * c);
+        const float4 g = team_ld_reduce<T>(p, 4 * c);
         if (SGD) {
             float4 w = *reinterpret_cast<const float4*>(p.W_uc + 4 * c);
             if constexpr (STATEFUL) {
@@ -87,9 +134,9 @@ __global__ void __launch_bounds__(256) nvls_reduce_kernel(const NvlsParams p) {
                 t.z = ema_lerp(t.z, w.z, alpha); t.w = ema_lerp(t.w, w.w, alpha);
                 *ep = t;
             }
-            multimem_st_f4(p.W_mc + 4 * c, w);
+            team_st<T, false>(p, 4 * c, w);
         } else {
-            multimem_st_f4(p.G_mc + 4 * c, g);
+            team_st<T, true>(p, 4 * c, g);
         }
     }
 
@@ -102,7 +149,7 @@ __global__ void __launch_bounds__(256) nvls_reduce_kernel(const NvlsParams p) {
             *p.cta_done = 0u;                                  // re-arm for the next launch (graph replay)
             *p.epoch = epoch;
             __threadfence_system();
-            multimem_red_release_add(p.flag_out_mc, 1u);
+            team_arrive<T, true>(p);
             // the kernel (= the stream) does not complete before every replica's share has landed in MY memory;
             // only this CTA waits, the others have exited, so a large grid can never starve itself
             wait_flag_ge(p.flag_out_uc, target);
@@ -120,24 +167,28 @@ static int nvls_grid(const NvlsParams& p, int max_ctas) {
 
 using NvlsKernel = void (*)(NvlsParams);
 
+template <NvlsTransport T>
 static NvlsKernel reduce_sgd_kernel(SgdForm form) {
     switch (form) {
-        case SGD_PLAIN: return nvls_reduce_kernel<true>;
-        case SGD_RULE: return nvls_reduce_kernel<true, true>;
-        case SGD_EMA: return nvls_reduce_kernel<true, true, true>;
+        case SGD_PLAIN: return nvls_reduce_kernel<true, false, false, T>;
+        case SGD_RULE: return nvls_reduce_kernel<true, true, false, T>;
+        case SGD_EMA: return nvls_reduce_kernel<true, true, true, T>;
     }
     return nullptr;
 }
 
+// a local team (p.team) runs the replay transport, a multicast object the switch's
 cudaError_t launch_nvls_reduce_sgd(const NvlsParams& p, int max_ctas, cudaStream_t stream) {
-    NvlsKernel fn = reduce_sgd_kernel(p.opt.form());
+    const SgdForm form = p.opt.form();
+    NvlsKernel fn = p.team != nullptr ? reduce_sgd_kernel<NvlsTransport::REPLAY>(form) : reduce_sgd_kernel<NvlsTransport::MULTICAST>(form);
     if (p.lr == nullptr || fn == nullptr) return cudaErrorInvalidValue;
     fn<<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
     return cudaGetLastError();
 }
 
 cudaError_t launch_nvls_allreduce(const NvlsParams& p, int max_ctas, cudaStream_t stream) {
-    nvls_reduce_kernel<false><<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
+    NvlsKernel fn = p.team != nullptr ? nvls_reduce_kernel<false, false, false, NvlsTransport::REPLAY> : nvls_reduce_kernel<false>;
+    fn<<<nvls_grid(p, max_ctas), 256, 0, stream>>>(p);
     return cudaGetLastError();
 }
 

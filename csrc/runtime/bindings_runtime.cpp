@@ -141,9 +141,40 @@ private:
 // NVLS symmetric memory (multicast object shared by the DP replicas); see runtime/nvls_context.h
 class PyNvlsContext {
 public:
-    PyNvlsContext(int dp, int rank, int64_t arena_numel, double lr)
-        : ctx_(std::make_unique<NvlsContext>(dp, rank, arena_numel, (float)lr)) {}
+    PyNvlsContext(int dp, int rank, int64_t arena_numel, double lr, int devices)
+        : ctx_(std::make_unique<NvlsContext>(dp, rank, arena_numel, (float)lr, devices)) {}
+    explicit PyNvlsContext(std::unique_ptr<NvlsContext> ctx) : ctx_(std::move(ctx)) {}
     static bool supported() { return NvlsContext::supported(); }
+    // test-facing: a member of a local team (plain device memory of this process, the kernels' replay transport)
+    static std::shared_ptr<PyNvlsContext> local(int dp, int rank, int64_t arena_numel) {
+        return std::make_shared<PyNvlsContext>(NvlsContext::local(dp, rank, arena_numel));
+    }
+    // test-facing: every member of the team, rank order, this one included
+    void open_local(const std::vector<std::shared_ptr<PyNvlsContext>>& team) {
+        std::vector<const NvlsContext*> raw;
+        for (const auto& c : team) raw.push_back(c ? c->ctx_.get() : nullptr);
+        ctx_->open_local(raw);
+    }
+    // test-facing: {name: (device pointer, bytes)} of this member's W and G (numel_pad floats each), its two flag words,
+    // the epoch and the last-CTA counter
+    py::dict buffers() {
+        const NvlsContext& c = *ctx_;
+        py::dict d;
+        auto put = [&](const char* name, const void* p, int64_t bytes) {
+            d[name] = py::make_tuple((int64_t) reinterpret_cast<uintptr_t>(p), bytes);
+        };
+        put("W", c.weights(), c.numel_pad() * 4);
+        put("G", c.grads(), c.numel_pad() * 4);
+        put("flag_in", c.flag_in(), 4);
+        put("flag_out", c.flag_out(), 4);
+        put("epoch", c.epoch_ptr(), 4);
+        put("cta_done", c.cta_done_ptr(), 4);
+        return d;
+    }
+    int64_t arena_numel() { return ctx_->arena_numel(); }
+    int64_t numel_pad() { return ctx_->numel_pad(); }
+    int dp() { return ctx_->dp(); }
+    int rank() { return ctx_->rank(); }
     int export_fd() { return ctx_->export_fd(); }
     void import_fd(int fd) { ctx_->import_fd(fd); }
     void add_device() { ctx_->add_device(); }
@@ -453,8 +484,16 @@ void bind_runtime(py::module_& m) {
         .def("rank", &PyDpContext::rank)
         .def("ll_tiles", &PyDpContext::ll_tiles);
     py::class_<PyNvlsContext, std::shared_ptr<PyNvlsContext>>(m, "NvlsContext")
-        .def(py::init<int, int, int64_t, double>())
+        .def(py::init<int, int, int64_t, double, int>(), py::arg("dp"), py::arg("rank"), py::arg("arena_numel"), py::arg("lr"),
+             py::arg("devices") = 0)
         .def_static("supported", &PyNvlsContext::supported)
+        .def_static("local", &PyNvlsContext::local, py::arg("dp"), py::arg("rank"), py::arg("arena_numel"))
+        .def("open_local", &PyNvlsContext::open_local)
+        .def("buffers", &PyNvlsContext::buffers)
+        .def("arena_numel", &PyNvlsContext::arena_numel)
+        .def("numel_pad", &PyNvlsContext::numel_pad)
+        .def("dp", &PyNvlsContext::dp)
+        .def("rank", &PyNvlsContext::rank)
         .def("export_fd", &PyNvlsContext::export_fd)
         .def("import_fd", &PyNvlsContext::import_fd)
         .def("add_device", &PyNvlsContext::add_device)

@@ -68,17 +68,33 @@ bool NvlsContext::supported() {
     return flag != 0;
 }
 
-NvlsContext::NvlsContext(int dp, int rank, int64_t arena_numel, float /*lr: unused, see nvls_context.h*/)
-    : dp_(dp), rank_(rank), arena_numel_(arena_numel) {
+namespace {
+
+void check_team(int dp, int rank, int64_t arena_numel) {
     if (dp < 2 || dp > 8) throw std::runtime_error("NvlsContext: dp must be in [2, 8]");
+    if (rank < 0 || rank >= dp) throw std::runtime_error("NvlsContext: rank must be in [0, dp)");
+    // the kernels work in float4 chunks (ParamArena keeps a multiple of 32 floats)
+    if (arena_numel <= 0 || arena_numel % 4 != 0) throw std::runtime_error("NvlsContext: arena_numel must be a positive multiple of 4");
+}
+
+int64_t pad_numel(int64_t arena_numel) { return (arena_numel + 63) / 64 * 64; }   // 256-byte multiple
+
+size_t alloc_bytes(int64_t numel_pad) { return ((size_t)2 * numel_pad + 64) * sizeof(float); }   // W | G | 2 x 32 flag words
+
+}  // namespace
+
+NvlsContext::NvlsContext(int dp, int rank, int64_t arena_numel, float /*lr: unused, see nvls_context.h*/, int devices)
+    : dp_(dp), rank_(rank), devices_(devices == 0 ? dp : devices), arena_numel_(arena_numel) {
+    check_team(dp, rank, arena_numel);
+    if (devices_ < 1 || devices_ > dp_) throw std::runtime_error("NvlsContext: devices must be in [1, dp]");
     CUDA_RT(cudaGetDevice(&dev_));
     CUDA_RT(cudaFree(nullptr));                                  // make sure the primary context exists
     if (!supported()) throw std::runtime_error("NvlsContext: this device / driver does not support NVLink multicast");
-    numel_pad_ = (arena_numel_ + 63) / 64 * 64;                  // 256-byte multiple: float4 loops never straddle the end
-    const size_t want = ((size_t)2 * numel_pad_ + 64) * sizeof(float);   // W | G | 2 x 32 flag words
+    numel_pad_ = pad_numel(arena_numel_);
+    const size_t want = alloc_bytes(numel_pad_);
     CUmulticastObjectProp mprop;
     memset(&mprop, 0, sizeof(mprop));
-    mprop.numDevices = (unsigned)dp_;
+    mprop.numDevices = (unsigned)devices_;
     mprop.size = want;
     mprop.handleTypes = CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR;
     size_t g_mc = 0, g_mem = 0;
@@ -93,8 +109,51 @@ NvlsContext::NvlsContext(int dp, int rank, int64_t arena_numel, float /*lr: unus
     CUDA_RT(cudaMemset(cta_done_, 0, 64));
 }
 
+NvlsContext::NvlsContext(int dp, int rank, int64_t arena_numel, Local)
+    : dp_(dp), rank_(rank), devices_(dp), arena_numel_(arena_numel) {
+    check_team(dp, rank, arena_numel);
+    CUDA_RT(cudaGetDevice(&dev_));
+    numel_pad_ = pad_numel(arena_numel_);
+    size_ = alloc_bytes(numel_pad_);
+    CUDA_RT(cudaMalloc(&local_mem_, size_));
+    CUDA_RT(cudaMemset(local_mem_, 0, size_));
+    uc_ptr_ = reinterpret_cast<CUdeviceptr>(local_mem_);
+    CUDA_RT(cudaMalloc(&epoch_, 64));
+    CUDA_RT(cudaMemset(epoch_, 0, 64));
+    CUDA_RT(cudaMalloc(&cta_done_, 64));
+    CUDA_RT(cudaMemset(cta_done_, 0, 64));
+    CUDA_RT(cudaDeviceSynchronize());
+}
+
+std::unique_ptr<NvlsContext> NvlsContext::local(int dp, int rank, int64_t arena_numel) {
+    return std::unique_ptr<NvlsContext>(new NvlsContext(dp, rank, arena_numel, Local{}));
+}
+
+void NvlsContext::open_local(const std::vector<const NvlsContext*>& team) {
+    if (!is_local()) throw std::runtime_error("NvlsContext::open_local: not a local team member (NvlsContext::local)");
+    if ((int)team.size() != dp_ || team[rank_] != this)
+        throw std::runtime_error("NvlsContext::open_local: the team must list dp members in rank order, this one at its rank");
+    std::vector<NvlsMember> views;
+    for (int m = 0; m < dp_; ++m) {
+        const NvlsContext* c = team[m];
+        if (c == nullptr || !c->is_local() || c->dp_ != dp_ || c->rank_ != m || c->arena_numel_ != arena_numel_ || c->dev_ != dev_)
+            throw std::runtime_error("NvlsContext::open_local: member " + std::to_string(m) +
+                                     " is not a local context of this team's size, rank, arena and device");
+        views.push_back({c->weights(), c->grads(), c->flag_in(), c->flag_out()});
+    }
+    if (team_ == nullptr) CUDA_RT(cudaMalloc(&team_, sizeof(NvlsMember) * 8));
+    CUDA_RT(cudaMemcpy(team_, views.data(), sizeof(NvlsMember) * views.size(), cudaMemcpyHostToDevice));
+}
+
 NvlsContext::~NvlsContext() {
     cudaDeviceSynchronize();
+    if (local_mem_ != nullptr) {
+        cudaFree(local_mem_);
+        cudaFree(team_);
+        cudaFree(epoch_);
+        cudaFree(cta_done_);
+        return;
+    }
     try {
         if (mc_ptr_) {
             DRV(cuMemUnmap)(mc_ptr_, size_);
@@ -117,10 +176,11 @@ NvlsContext::~NvlsContext() {
 }
 
 int NvlsContext::export_fd() {
+    if (is_local()) throw std::runtime_error("NvlsContext: a local team member has no multicast object");
     if (have_mc_) throw std::runtime_error("NvlsContext: multicast object already present");
     CUmulticastObjectProp mprop;
     memset(&mprop, 0, sizeof(mprop));
-    mprop.numDevices = (unsigned)dp_;
+    mprop.numDevices = (unsigned)devices_;
     mprop.size = size_;
     mprop.handleTypes = CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR;
     cu_check(DRV(cuMulticastCreate)(&mc_, &mprop), "cuMulticastCreate");
@@ -132,6 +192,7 @@ int NvlsContext::export_fd() {
 }
 
 void NvlsContext::import_fd(int fd) {
+    if (is_local()) throw std::runtime_error("NvlsContext: a local team member has no multicast object");
     if (have_mc_) throw std::runtime_error("NvlsContext: multicast object already present");
     cu_check(DRV(cuMemImportFromShareableHandle)(&mc_, reinterpret_cast<void*>(static_cast<uintptr_t>(fd)),
                                                  CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR),
@@ -171,19 +232,25 @@ void NvlsContext::bind_and_map() {
 }
 
 NvlsParams NvlsContext::params() const {
-    if (!mc_ptr_ || !uc_ptr_) throw std::runtime_error("NvlsContext::params before bind_and_map");
+    if (is_local() ? team_ == nullptr : (!mc_ptr_ || !uc_ptr_))
+        throw std::runtime_error(is_local() ? "NvlsContext::params before open_local" : "NvlsContext::params before bind_and_map");
     NvlsParams p{};
     float* uc = reinterpret_cast<float*>(uc_ptr_);
-    float* mc = reinterpret_cast<float*>(mc_ptr_);
     p.W_uc = uc; p.G_uc = uc + numel_pad_;
-    p.W_mc = mc; p.G_mc = mc + numel_pad_;
-    uint32_t* fuc = reinterpret_cast<uint32_t*>(uc + 2 * numel_pad_);
-    uint32_t* fmc = reinterpret_cast<uint32_t*>(mc + 2 * numel_pad_);
-    p.flag_in_uc = fuc; p.flag_in_mc = fmc;
-    p.flag_out_uc = fuc + 32; p.flag_out_mc = fmc + 32;       // separate 128-byte lines
+    p.flag_in_uc = flag_in(); p.flag_out_uc = flag_out();
+    if (is_local()) {
+        p.team = team_;                                        // W_mc / G_mc / flag_*_mc stay null: the replay transport
+    } else {
+        float* mc = reinterpret_cast<float*>(mc_ptr_);
+        p.W_mc = mc; p.G_mc = mc + numel_pad_;
+        uint32_t* fmc = reinterpret_cast<uint32_t*>(mc + 2 * numel_pad_);
+        p.flag_in_mc = fmc; p.flag_out_mc = fmc + 32;
+    }
     p.epoch = epoch_;
     p.cta_done = cta_done_;
-    p.numel = numel_pad_;
+    // the arena, not the padded allocation: the owners also read and write the caller's momentum / EMA arenas at the
+    // same offsets, and those hold arena_numel floats
+    p.numel = arena_numel_;
     p.dp = dp_; p.rank = rank_;
     p.lr = nullptr;
     return p;

@@ -14,16 +14,33 @@
 //      others:     import_fd(fd)
 //   3. every rank: add_device(); barrier; bind_and_map(); barrier
 // Layout of the allocation (floats): [ W: numel_pad ][ G: numel_pad ][ flags: 2 x 32 ]
+// The kernels reduce and update the arena's arena_numel floats only; [arena_numel, numel_pad) is never touched, and the
+// caller's momentum / EMA arenas need to cover arena_numel floats, no more.
+//
+// Local team (tests): NvlsContext::local() allocates the same layout in plain device memory of this process and
+// open_local() hands every member the unicast views of the whole team.  The kernels then run their replay transport: the
+// switch's load-reduce, store and flag add become loads, stores and atomics on the members' views (nvls_dp.cu), so one
+// replica of a dp-way group runs on one GPU against peers that are memory.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <memory>
 #include <string>
+#include <vector>
 
 #include "kernels/kernels.h"
 
 namespace ssb {
+
+// One member of a local team: unicast views of its allocation.
+struct NvlsMember {
+    float* W;
+    float* G;
+    uint32_t* flag_in;
+    uint32_t* flag_out;
+};
 
 struct NvlsParams {
     float* W_uc;            // this replica's weights (unicast mapping)
@@ -40,14 +57,20 @@ struct NvlsParams {
     int dp, rank;
     const float* lr;        // device float: learning rate of the running step (reduce_sgd only)
     SgdState opt;           // update rule; opt.V = LOCAL momentum arena (unicast), chunk c's entries live at rank c % dp
+    const NvlsMember* team; // local team: dp members in rank order, own rank included (device memory); nullptr: multicast
 };
 
 class NvlsContext {
 public:
     // lr is not used: the kernel reads the learning rate from NvlsParams::lr, a device slot the caller sets (nullptr in
     // params())
-    NvlsContext(int dp, int rank, int64_t arena_numel, float lr);
+    // devices: GPUs that join the multicast object (0: dp).  1 builds a one-device team whose kernels still run as
+    // replica `rank` of `dp`: ld_reduce then returns the local gradients alone (tests on a single GPU).
+    NvlsContext(int dp, int rank, int64_t arena_numel, float lr, int devices = 0);
     ~NvlsContext();
+    // a member of a local team (plain cudaMalloc memory, no multicast object); usable after open_local()
+    static std::unique_ptr<NvlsContext> local(int dp, int rank, int64_t arena_numel);
+    void open_local(const std::vector<const NvlsContext*>& team);   // every member, rank order, this one included
 
     static bool supported();         // CU_DEVICE_ATTRIBUTE_MULTICAST_SUPPORTED on the current device
     int export_fd();                 // leader only: creates the multicast object, returns a POSIX fd for it
@@ -62,10 +85,17 @@ public:
     size_t bytes() const { return size_; }
     int dp() const { return dp_; }
     int rank() const { return rank_; }
-    NvlsParams params() const;       // valid after bind_and_map()
+    uint32_t* flag_in() const { return reinterpret_cast<uint32_t*>(grads() + numel_pad_); }
+    uint32_t* flag_out() const { return flag_in() + 32; }           // separate 128-byte lines
+    uint32_t* epoch_ptr() const { return epoch_; }
+    unsigned int* cta_done_ptr() const { return cta_done_; }
+    bool is_local() const { return local_mem_ != nullptr; }
+    NvlsParams params() const;       // valid after bind_and_map() (open_local() for a local team)
 
 private:
-    int dp_, rank_, dev_ = 0;
+    struct Local {};
+    NvlsContext(int dp, int rank, int64_t arena_numel, Local);
+    int dp_, rank_, dev_ = 0, devices_;
     int64_t arena_numel_, numel_pad_;
     size_t size_ = 0, gran_ = 0;
     CUmemGenericAllocationHandle mc_ = 0, mem_ = 0;
@@ -73,6 +103,8 @@ private:
     CUdeviceptr uc_ptr_ = 0, mc_ptr_ = 0;
     uint32_t* epoch_ = nullptr;
     unsigned int* cta_done_ = nullptr;
+    void* local_mem_ = nullptr;      // local team: the W | G | flags allocation
+    NvlsMember* team_ = nullptr;     // local team: the members' views, device memory
 };
 
 // kernels (csrc/kernels/nvls_dp.cu)
